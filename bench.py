@@ -2,6 +2,7 @@
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
                     [--algo PPOLag|CPO|TRPOLag|FOCOPS] [--obs-dim D] [--precision bf16x3|tf32|fp32]
+                    [--dump-outputs DIR]
 
 A "step" is one epoch of a BASELINE.json workload: by default `configs[1]` = PPOLag on the synthetic Box env
 (obs 60 / act 8), 4096 HBM-resident envs per GPU, T = 128 steps per env (524 288 samples per GPU), update_iters 8,
@@ -11,14 +12,17 @@ batch_size 16384 -- i.e. the reference's `Time/FPS = steps_per_epoch / epoch_tim
 
   value   : device-timed (CUDA events, barrier + synchronize on both sides, max over ranks), everything resident in
             HBM, in-kernel Philox noise.  Arithmetic = `--precision`, default bf16x3: every layer GEMM runs on the
-            tensor cores as six kind::f16 MMAs over the three bf16 pieces of its fp32 operands with fp32
+            tensor cores as six bf16 wgmma products over the three bf16 pieces of its fp32 operands with fp32
             accumulation -- held by the tests to the bar of the exact-fp32 path (reference: fp32 Linear layers).
             The tf32 mode (5e-3) is reported as a labelled extra, never as the headline.
   e2e     : the same metric through the public `omnisafe_b200.Agent(...)` training loop with HOST buffers: every
             epoch the standard-normal action-noise stream is copied from pinned host memory (parity-mode input of
             the rollout) and the epoch's logged metrics are read back.
   --impl reference : the CPU restatement of the reference path (oracle/, torch-CPU + numpy) timed on the host cores
-            on the SAME workload size (4096 envs x T = 128 per step); /root/reference does not exist on the GPU box.
+            on the SAME workload size (4096 envs x T = 128 per step).
+  --dump-outputs DIR : after the timed epochs, what the last one computed -- the parameters after its update and a
+            fixed, seeded sample of 32768 rows of every float slab of its rollout buffer -- as DIR/<name>.npy (float32),
+            so that two builds can be compared output for output (same arguments => same inputs).
 """
 from __future__ import annotations
 
@@ -40,7 +44,7 @@ sys.path.insert(0, ROOT)
 WORKLOAD = dict(algo='PPOLag', env='SyntheticBox-v0', obs_dim=60, act_dim=8, envs_per_gpu=4096,
                 steps_per_env=128, batch_size=16384, update_iters=8, max_episode_steps=64)
 ALGOS = ('PPOLag', 'CPO', 'TRPOLag', 'FOCOPS')
-DTYPES = {'bf16x3': 'bf16x3 (fp32 operands as 3 bf16 pieces, 6 tcgen05 kind::f16 MMAs per product, fp32 accumulate: fp32-level '
+DTYPES = {'bf16x3': 'bf16x3 (fp32 operands as 3 bf16 pieces, 6 bf16 wgmma products per product, fp32 accumulate: fp32-level '
                     'results; GAE fp64 carry)',
           'tf32': 'tf32 (fp32 storage/accumulate; GAE fp64 carry)',
           'fp32': 'f32 (FMA tiles; GAE fp64 carry)'}
@@ -54,7 +58,8 @@ def _peaks():
             p = json.load(fh)
         return {'hbm_gbs': p['hbm_gbs'], 'bf16_tflops': p['bf16_tflops'],
                 'bf16_tflops_sustained': p.get('bf16_tflops_sustained', p['bf16_tflops']), 'source': 'measured'}
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0, 'source': 'fallback'}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- not measured, an upper bound
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0, 'bf16_tflops_sustained': 989.0, 'source': 'H100 SXM data sheet'}
 
 
 class ClockSampler:
@@ -135,6 +140,24 @@ def _flops_per_sample(O: int, A: int) -> int:
     return net(A) + 2 * net(1)
 
 
+def _dump_outputs(algo, out_dir: str, sample_rows: int = 32768) -> None:
+    """What the last timed epoch computed: the flat parameters after its update and a fixed, seeded sample of the
+    rows of every float slab of its rollout buffer, one float32 .npy per array (about 12 MB at the default workload)."""
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, 'theta.npy'), algo._actor_critic.theta.detach().float().cpu().numpy())
+    rows = None
+    for name, t in sorted(algo._buf.data.items()):
+        if t is None or not t.is_floating_point():
+            continue
+        flat = t.detach().reshape(-1, *t.shape[2:]) if name != 'epfin' else t.detach().reshape(t.shape[0], -1).T
+        if rows is None or rows.numel() > flat.shape[0]:
+            n = flat.shape[0]
+            idx = np.sort(np.random.default_rng(0).choice(n, size=min(sample_rows, n), replace=False))
+            rows = torch.as_tensor(idx, device=flat.device)
+        np.save(os.path.join(out_dir, f'{name}.npy'), flat.index_select(0, rows).float().cpu().numpy())
+
+
 def run_b200(args) -> dict:
     import torch.distributed as dist
 
@@ -193,6 +216,8 @@ def run_b200(args) -> dict:
     clocks = clk.summary()
     ms_per_step = ms / args.steps
     value = samples_global / (ms_per_step * 1e-3)
+    if args.dump_outputs and rank == 0:
+        _dump_outputs(algo, args.dump_outputs)
 
     # ---- end to end through the public loop with host buffers ----------------------------------
     host_eps = torch.randn(T, N, A, dtype=torch.float32).pin_memory()
@@ -235,8 +260,6 @@ def run_b200(args) -> dict:
                                          ptr(eng.gpart), ptr(eng.stats_part), ptr(eng.train_stats), 0, 0, 0, 1, 0, 0, current_stream())
         ms_k = timed(iter_launch, 10) / 10          # learning rates 0: the parameters stay put
         kname, rows_per_launch = 'minibatch_grad_x3_kernel<fused> (persistent: 1 launch = 1 update iteration)', total
-        # dram__bytes_read.sum + dram__bytes_write.sum of one launch, ncu --set full (profiles/r02_ncu_update_x3.md)
-        traffic = 218.8e6 if (O == 60 and A == 8 and total == 524288 and args.algo == 'PPOLag') else None
     else:
         fn = lib().osb_minibatch_grad_tc if args.precision == 'tf32' else lib().osb_minibatch_grad
 
@@ -248,7 +271,6 @@ def run_b200(args) -> dict:
         ms_k = timed(iter_launch, 50) / 50
         kname = 'minibatch_grad_tc_kernel' if args.precision == 'tf32' else 'minibatch_grad_kernel'
         rows_per_launch = w['batch_size']
-        traffic = 14.57e6 if (args.precision == 'tf32' and O == 60) else None     # ncu --set full, profiles/r01_ncu_minibatch_grad_tc.md
     # the GAE scan where HBM is its bound: a horizon whose 277 MB of algorithmic traffic do not fit L2 (the epoch's own
     # T = 128 launch moves 17 MB and is latency bound)
     from omnisafe_b200.common.buffer import VectorOnPolicyBuffer
@@ -267,15 +289,13 @@ def run_b200(args) -> dict:
     gae_gbs = 33.0 * total / (ms_gae * 1e-3) / 1e9
     roofline = {
         'kernel': kname, 'bound': 'tensor', 'achieved': ach_tf, 'peak': peaks['bf16_tflops_sustained'], 'unit': 'TFLOP/s',
-        'frac': ach_tf / peaks['bf16_tflops_sustained'], 'traffic': traffic,
+        'frac': ach_tf / peaks['bf16_tflops_sustained'],
         'algorithmic_flops_per_launch': float(flop_per_sample) * rows_per_launch,
         'algorithmic_bytes': row_bytes * rows_per_launch + 4.0 * eng.P * (rows_per_launch // w['batch_size']),   # sample rows read once + one gradient per minibatch step
-        'peak_source': peaks['source'] + ' (cuBLAS bf16, sustained); fp32-equivalent FLOPs are counted once although the '
-                       'bf16x3 mode executes 6 bf16 MMAs per product' if x3_path else peaks['source'] + ' (cuBLAS bf16, sustained)',
+        'peak_source': peaks['source'] + '; fp32-equivalent FLOPs are counted once although the '
+                       'bf16x3 mode executes 6 bf16 MMAs per product' if x3_path else peaks['source'],
         'us_per_launch': ms_k * 1e3, 'us_per_minibatch_step': ms_k * 1e3 / (rows_per_launch // w['batch_size']),
         'mma_executed_tflops': ach_tf * 6.0 if x3_path else None,
-        'ncu': ({'tensor_pipe_active_pct': 18.9, 'dram_bytes_per_launch': 218.8e6, 'source': 'profiles/r02_ncu_update_x3.md (ncu --set full, one launch)'}
-                if (x3_path and O == 60 and args.algo == 'PPOLag') else None),
         'gae': {'kernel': 'gae_stream_kernel<TMA>', 'bound': 'hbm', 'achieved': gae_gbs, 'peak': peaks['hbm_gbs'],
                 'unit': 'GB/s', 'frac': gae_gbs / peaks['hbm_gbs'], 'us_per_launch': ms_gae * 1e3, 'bytes_per_sample': 33,
                 'note': 'T = 128: 17 MB, latency bound (one wave of 128 CTAs, one tile each)'},
@@ -296,7 +316,7 @@ def run_b200(args) -> dict:
         'data': 'synthetic',
         'config': {'workload': _workload_name(args.algo, O), 'algo': args.algo, 'obs_dim': O, 'envs_per_gpu': N, 'steps_per_env': T,
                    'global_samples_per_step': samples_global, 'parallelism': f'dp{world}', 'matmul_precision': args.precision,
-                   'l2_policy': f'inputs larger than L2 (per-epoch slabs ~{(row_bytes + 48) * total / 1e6:.0f} MB > 126 MB)' if (row_bytes + 48) * total > 126e6
+                   'l2_policy': f'inputs larger than L2 (per-epoch slabs ~{(row_bytes + 48) * total / 1e6:.0f} MB > 50 MB)' if (row_bytes + 48) * total > 50e6
                    else 'per-epoch slabs fit L2; every epoch rewrites them (rollout) before the update reads them',
                    'noise': 'in-kernel Philox'},
         'e2e': e2e, 'gpu_launches': launches, 'clocks': clocks, 'roofline': roofline,
@@ -308,7 +328,7 @@ def run_b200(args) -> dict:
             alt.train_epoch()
         ms_alt = timed(alt.train_epoch, max(3, args.steps // 2)) / max(3, args.steps // 2)
         out['extra'] = {'tf32': {'value': samples_global / (ms_alt * 1e-3), 'unit': 'env-steps/s', 'ms_per_step': ms_alt,
-                                 'note': 'kind::tf32 tiles: 10-bit mantissa, certified only to 5e-3 -- NOT the headline'}}
+                                 'note': 'tf32 wgmma tiles: 10-bit mantissa, certified only to 5e-3 -- NOT the headline'}}
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
         out['cpu_baseline'] = cpu_baseline(args)
     if world > 1:
@@ -446,6 +466,8 @@ def main() -> None:
     ap.add_argument('--precision', default='bf16x3', choices=['bf16x3', 'tf32', 'fp32'])
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-extras', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write what the last timed epoch computed to DIR/<name>.npy (float32, < 64 MB in all)')
     args = ap.parse_args()
     # stdout carries exactly ONE JSON line: whatever libraries print while the bench runs (e.g. NCCL's version banner, written
     # by C code straight to fd 1) is sent to stderr

@@ -1,4 +1,4 @@
-/* omnisafe_b200 -- C ABI of the B200-native on-policy SafeRL hot path.
+/* omnisafe_b200 -- C ABI of the H100-native on-policy SafeRL hot path.
  *
  * The reference (PKU-Alignment/omnisafe) is pure Python: its seam for this path is the set of
  * Python methods listed below, not an FFI.  Each entry point here is what a ctypes binding of the
@@ -83,7 +83,7 @@ int osb_discount_cumsum(const void* x, int x_is_f64, int rows, int len, double d
  * (onpolicy_adapter.py:L80).  osb_rollout_step with t in [0, T) performs step t; t == T is the
  * epoch-end bootstrap launch (critics only).  eps = [N][A] standard-normal draws of this step
  * (parity mode) or NULL (in-kernel Philox keyed by noise_seed / global_step).  precision: 0 = exact
- * fp32 FMA tiles (parity), 1 = tcgen05 TF32 tiles of 128 envs (O <= 64; falls back to 0 otherwise). */
+ * fp32 FMA tiles (parity), 1 = TF32 wgmma tiles of 128 envs (O <= 64; falls back to 0 otherwise). */
 int osb_env_reset(int O, int A, int max_episode_steps, unsigned seed, unsigned term_threshold,
                   unsigned env_id_offset, float cost_threshold, int obs_normalize, int N,
                   float* s_raw, float* final_raw, int* ep_step, unsigned* episode, unsigned* gstep,
@@ -166,12 +166,12 @@ int osb_minibatch_grad(const float* theta, int O, int A, const float* obs, const
                        float entropy_coef, float focops_lam, float focops_eta,
                        const float* lagrange, const float* logstd_old, int net_mask, float* gpart,
                        float* stats_part, const int* stop_flag, void* stream);
-/* Tensor-core variant of osb_minibatch_grad: the tile GEMMs run as tcgen05.mma kind::tf32 with TMEM
+/* Tensor-core variant of osb_minibatch_grad: the tile GEMMs run as tf32 wgmma with accumulator image
  * accumulators (operands fp32 in 128B-swizzled smem tiles; transposed activations produced by
  * role-swapped MMAs).  Same arguments and outputs; O <= 64, A <= 16.  This is arithmetic mode
  * `precision = 1` of osb_ppo_update_epoch; mode 0 is the exact-fp32 FMA parity path.
- * gpart / stats_part rows: osb_tc_grid_blocks(mb_count, net_mask) -- 49 CTAs per network when
- * several networks share the launch, up to 148 when net_mask names a single network. */
+ * gpart / stats_part rows: osb_tc_grid_blocks(mb_count, net_mask) -- a third of the device's SMs per network
+ * when several networks share the launch, up to all of them (at most 148) when net_mask names a single network. */
 int osb_tc_grid_blocks(long long rows, int net_mask);
 int osb_minibatch_grad_tc(const float* theta, int O, int A, const float* obs, const float* act,
                           const float* logp, const float* adv_r, const float* adv_c,
@@ -181,7 +181,7 @@ int osb_minibatch_grad_tc(const float* theta, int O, int A, const float* obs, co
                           float entropy_coef, float focops_lam, float focops_eta,
                           const float* lagrange, const float* logstd_old, int net_mask, float* gpart,
                           float* stats_part, const int* stop_flag, void* stream);
-/* Split-bf16 ("bf16x3") parity-grade tensor-core variant (csrc/update_x3.cu): every GEMM = six kind::f16
+/* Split-bf16 ("bf16x3") parity-grade tensor-core variant (csrc/update_x3.cu): every GEMM = six bf16 wgmma
  * MMAs over the three bf16 pieces of its fp32 operands, fp32 accumulate; O <= 64, loss kinds 0 / 1 / 3. */
 int osb_minibatch_grad_x3(const float* theta, int O, int A, const float* obs, const float* act,
                           const float* logp, const float* adv_r, const float* adv_c,
@@ -200,7 +200,7 @@ int osb_actor_eval(const float* theta_actor, int O, int A, const float* obs, con
                    const float* logstd_old, const float* moments, const float* lagrange,
                    long long total, int stride, float* mu_store, double* workspace, double* out,
                    void* stream);
-/* Tensor-core (tcgen05 TF32) variant of osb_actor_eval: same arguments / outputs, O <= 64. */
+/* Tensor-core (TF32 wgmma) variant of osb_actor_eval: same arguments / outputs, O <= 64. */
 int osb_actor_eval_tc(const float* theta_actor, int O, int A, const float* obs, const float* act,
                       const float* logp, const float* adv_r, const float* adv_c, const float* mu_old,
                       const float* logstd_old, const float* moments, const float* lagrange,
@@ -338,18 +338,16 @@ int osb_nccl_allreduce(void* comm, void* buf, long long count, int is_f64, void*
 int osb_nccl_destroy(void* comm);
 
 /* ---- diagnostics ---------------------------------------------------------------------------
- * One tcgen05 (kind::tf32, TMEM accumulator) GEMM D = A * B^T on a single CTA with every operand
- * major combination; out[128][N] is the raw TMEM dump.  Pins the descriptor / swizzle conventions
- * the tensor-core MLP tiles rely on (tests/test_umma_gpu.py). */
-/* cycles for `reps` back-to-back M x N x 8 tf32 MMAs: out[0] issue->completion, out[1] issue loop. */
-int osb_umma_timing(int M, int N, int reps, long long* out, void* stream);
+ * One tf32 wgmma GEMM D = A * B^T (both operands K-major; a_mn / b_mn must be 0) on a single warpgroup;
+ * out[128][N] is the dump of the accumulator lanes.  Pins the descriptor / swizzle / lane conventions the
+ * tensor-core MLP tiles rely on (tests/test_umma_gpu.py). */
 int osb_umma_selftest(const float* A, const float* B, int M, int N, int K, int a_mn, int b_mn,
                       float* out, void* stream);
 
-/* Split-bf16 ("bf16x3", kind::f16) building blocks of the parity-grade tensor-core mode (csrc/x3.cuh):
- * one single-CTA GEMM D = A * B^T with A [M][K], B [N][K] (row-major fp32 in global memory), each operand
- * staged as three bf16 tiles (SW128 or SW32) consumed K-major or MN-major; out[128][N] = raw TMEM dump
- * (tests/test_x3_gpu.py).  The timing / epilogue probes report clock64 cycles. */
+/* Split-bf16 ("bf16x3") building blocks of the parity-grade tensor-core mode (csrc/x3.cuh):
+ * one single-warpgroup GEMM D = A * B^T with A [M][K], B [N][K] (row-major fp32 in global memory), each operand
+ * staged as three bf16 tiles (SW128 or SW32) consumed K-major or MN-major; out[128][N] = dump of the
+ * accumulator lanes (tests/test_x3_gpu.py). */
 int osb_x3_selftest(const float* A, const float* B, int M, int N, int K, int a_mn, int b_mn, int a_sw,
                     int b_sw, int b_ones, float* out, void* stream);
 int osb_x3_debug_buffer(long long* buf);
@@ -357,10 +355,6 @@ int osb_x3_debug_buffer(long long* buf);
 int osb_gae_debug_buffer(long long* buf);
 /* same for the persistent rollout kernel (tools/rollout_stage_times.py) */
 int osb_rollout_debug_buffer(long long* buf);
-int osb_x3_selftest_dbg(const float* A, const float* B, int M, int N, int K, int a_mn, int b_mn, int a_sw,
-                        int b_sw, int b_ones, int a_lbo, int a_sbo, int b_lbo, int b_sbo, float* out, void* stream);
-int osb_x3_timing(int M, int N, int reps, int style, long long* out, void* stream);
-int osb_x3_epilogue_probe(int cols, int reps, int mode, long long* out, float* sink, void* stream);
 
 #ifdef __cplusplus
 }

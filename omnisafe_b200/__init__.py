@@ -1,4 +1,4 @@
-"""omnisafe_b200: B200-native (sm_100a) on-policy SafeRL hot path behind the omnisafe surface."""
+"""omnisafe_b200: H100-native (sm_90a) on-policy SafeRL hot path behind the omnisafe surface."""
 from omnisafe_b200.algorithms import ALGORITHMS  # noqa: F401
 from omnisafe_b200.algorithms.algo_wrapper import AlgoWrapper as Agent  # noqa: F401
 

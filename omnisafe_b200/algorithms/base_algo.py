@@ -20,7 +20,7 @@ class BaseAlgo(ABC):
         dev = str(cfgs.train_cfgs.device)
         if not dev.startswith('cuda'):
             raise RuntimeError(
-                f"train_cfgs.device={dev!r}: omnisafe_b200 runs this path as sm_100a CUDA kernels only "
+                f"train_cfgs.device={dev!r}: omnisafe_b200 runs this path as sm_90a CUDA kernels only "
                 "(no CPU fallback); use the upstream omnisafe classes for CPU training")
         if not torch.cuda.is_available():
             raise RuntimeError('omnisafe_b200 needs a CUDA device (no CPU fallback)')

@@ -42,7 +42,7 @@ class UpdateEngine:
         self.cg_scalars = torch.zeros(4, **f32)
         self.scalar = torch.zeros(4, **f32)
         self._perm_seed = 0x1234567
-        self.precision = 0   # 0 = exact fp32 FMA tiles, 1 = TF32 tcgen05 tiles (5e-3), 2 = split-bf16 tcgen05 tiles (fp32-level)
+        self.precision = 0   # 0 = exact fp32 FMA tiles, 1 = TF32 wgmma tiles (5e-3), 2 = split-bf16 wgmma tiles (fp32-level)
 
     # ---- helpers ----------------------------------------------------------------------------
     def _tc(self) -> bool:

@@ -1,4 +1,4 @@
-"""On-policy algorithms on the fused sm_100a path: PolicyGradient / PPO / PPOLag / NaturalPG / RCPO /
+"""On-policy algorithms on the fused sm_90a path: PolicyGradient / PPO / PPOLag / NaturalPG / RCPO /
 TRPO / TRPOLag / CPO / PCPO / FOCOPS / CPPOPID / TRPOPID / OnCRPO / PDO / IPO / P3O.
 
 Each class mirrors the override structure of the reference

@@ -1,4 +1,4 @@
-"""Build the C-ABI CUDA library (sm_100a) in-tree: omnisafe_b200/lib/libomnisafe_b200.so.
+"""Build the C-ABI CUDA library (sm_90a) in-tree: omnisafe_b200/lib/libomnisafe_b200.so.
 
 nvcc cross-compiles without a GPU; the built .so travels to the GPU box with the repo snapshot.
 """
@@ -15,7 +15,7 @@ LIBDIR = os.path.join(HERE, 'lib')
 LIB = os.path.join(LIBDIR, 'libomnisafe_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a',
+    '-gencode', 'arch=compute_90a,code=sm_90a',
     '-O3', '-lineinfo', '-std=c++17',
     '-Xcompiler', '-fPIC',
     '--expt-relaxed-constexpr',
@@ -64,7 +64,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             sys.stderr.write(f'nvcc failed for {src}\n')
     if failed:
         raise RuntimeError('CUDA build failed')
-    subprocess.check_call([NVCC, '-shared', '-o', LIB, *objs, '-lcudart'])
+    subprocess.check_call([NVCC, *FLAGS[:2], '-shared', '-o', LIB, *objs, '-lcudart'])
     with open(stamp, 'w') as fh:
         fh.write(dig)
     return LIB

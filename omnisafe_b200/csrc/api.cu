@@ -1,5 +1,6 @@
 // C-ABI plumbing shared by all entry points: error string, version, device query.
 #include "common.cuh"
+#include <mutex>
 #include <string.h>
 
 static thread_local char g_err[1024] = "";
@@ -31,3 +32,46 @@ int osb_device_info(int device, int* sm_count, int* cc_major, int* cc_minor) {
 }
 
 }  // extern "C"
+
+namespace osb {
+
+// Device scratch for the tensor-core accumulator images (csrc/umma.cuh): one buffer per (device, slot), grown on
+// demand.  A buffer that has been handed out is never freed (growth allocates a new one and keeps the old one for the
+// life of the process), so a pointer stays valid for the launch it was fetched for and no growth synchronises the device.
+// Contract: the launches of one kernel family on one device share its buffer, so they must be ordered on one stream;
+// growth calls cudaMalloc, which CUDA-graph capture does not allow -- run a launch of the same size before capturing it.
+float* acc_scratch(int slot, size_t bytes) {
+    constexpr int MAX_DEV = 64;
+    static std::mutex mu;
+    static float* buf[MAX_DEV][ACC_SLOTS] = {};
+    static size_t cap[MAX_DEV][ACC_SLOTS] = {};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= MAX_DEV || slot < 0 || slot >= ACC_SLOTS) {
+        osb_set_error("acc_scratch: bad device or slot");
+        return nullptr;
+    }
+    std::lock_guard<std::mutex> lock(mu);
+    if (cap[dev][slot] < bytes) {
+        const size_t grown = bytes > 2 * cap[dev][slot] ? bytes : 2 * cap[dev][slot];   // geometric: few retired buffers
+        void* ptr = nullptr;
+        const cudaError_t e = cudaMalloc(&ptr, grown);
+        if (e != cudaSuccess) {
+            char msg[256];
+            snprintf(msg, sizeof(msg), "acc_scratch: cudaMalloc(%zu) -> %s", grown, cudaGetErrorString(e));
+            osb_set_error(msg);
+            return nullptr;
+        }
+        buf[dev][slot] = static_cast<float*>(ptr);
+        cap[dev][slot] = grown;
+    }
+    return buf[dev][slot];
+}
+
+int grid_sms() {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
+        return 1;
+    return n < MAX_GRID_CTAS ? n : MAX_GRID_CTAS;
+}
+
+}  // namespace osb

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the omnisafe_b200 sm_100a kernels.
+// Shared device/host helpers for the omnisafe_b200 sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -43,6 +43,18 @@ extern "C" void osb_count_launch(void);   // kernel-launch counter behind osb_la
 #define OSB_FLAG_TRUNCATED 2u
 
 namespace osb {
+
+// Scratch slots of acc_scratch(): one per kernel family, so that families running on different streams never
+// share an accumulator image.
+enum AccSlot { ACC_ROLLOUT = 0, ACC_EVAL_TC, ACC_EVAL_X3, ACC_UPDATE_TC, ACC_FVP_TC, ACC_FVP_X3, ACC_UPDATE_X3, ACC_SELFTEST, ACC_SLOTS };
+// Device buffer of at least `bytes` for the accumulator images of one launch (csrc/umma.cuh); nullptr (with the
+// error string set) when it cannot be allocated.  Launches of one slot on one device must be ordered on one stream;
+// see api.cu for the lifetime and graph-capture rules.
+float* acc_scratch(int slot, size_t bytes);
+// Persistent grids use one CTA per SM of the current device, at most MAX_GRID_CTAS (the per-CTA partial-result
+// buffers of algorithms/engine.py hold that many rows).
+constexpr int MAX_GRID_CTAS = 148;
+int grid_sms();
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -191,8 +191,8 @@ int osb_ppo_update_epoch(float* theta, float* grad, float* adam_m, float* adam_v
     OSB_CUDA(cudaMemsetAsync(kl_state, 0, 4 * sizeof(float), s));
     OSB_CUDA(cudaMemsetAsync(train_stats, 0, 3 * 8 * sizeof(float), s));
     int rc;
-    // precision 1 = TF32 tcgen05 tiles (O <= 64, loss kinds 0/1/3); otherwise the fp32 FMA parity path
-    // precision 2 = split-bf16 ("bf16x3") tcgen05 tiles: fp32-level results on the tensor cores (O <= 64,
+    // precision 1 = TF32 wgmma tiles (O <= 64, loss kinds 0/1/3); otherwise the fp32 FMA parity path
+    // precision 2 = split-bf16 ("bf16x3") wgmma tiles: fp32-level results on the tensor cores (O <= 64,
     // loss kinds 0/1/3)
     const bool use_x3 = precision == 2 && O <= 64 && (loss_kind == 0 || loss_kind == 1 || loss_kind == 2 || loss_kind == 3 || loss_kind == 5);   // FOCOPS (2), P3O (5): stepwise launches
     const bool use_x3e = precision == 2 && O <= 64;

@@ -1,7 +1,7 @@
-// Tensor-core (tcgen05, TF32) full-batch actor forward: the fast variant of actor_eval_kernel
+// Tensor-core (wgmma, TF32) full-batch actor forward: the fast variant of actor_eval_kernel
 // (csrc/update.cu).  Stores mu(theta) per row (old-policy snapshot) or reduces
 // sum KL(old||new), sum ratio*adv, sum ratio*adv_c, sum ratio, count, sum ratio*adv_r in fp64.
-// Two CTAs per SM (~100 KB smem, 128 TMEM columns each) so one CTA's epilogue overlaps the other's MMA.
+// Two CTAs per SM (~100 KB smem each) so one CTA's epilogue overlaps the other's MMA.
 #include "common.cuh"
 #include "mlp.cuh"
 #include "umma.cuh"
@@ -12,11 +12,13 @@ using namespace umma;
 
 constexpr int ET = 128;
 constexpr uint32_t EBUF = ET * 64 * 4;
+constexpr uint32_t E_COLS = 80;            // accumulator columns: Z [0, 64), OUT [64, 80)
 
 struct EvalTcArgs {
     const float* obs; const float* act; const float* logp; const float* adv_r; const float* adv_c;
     const float* mu_old; const float* logstd_old; const float* moments; const float* lagrange;
     const float* theta; float* mu_store; double* part;
+    float* acc;         // accumulator images, [gridDim.x][128][E_COLS]
     long long total; int stride, O, A;
 };
 
@@ -33,7 +35,6 @@ __global__ void __launch_bounds__(NTHREADS, 2) actor_eval_tc_kernel(EvalTcArgs p
     double* sRedD = reinterpret_cast<double*>(sLs + 64);       // [4][8]
     long long* sRow = reinterpret_cast<long long*>(sRedD + 32);  // [128]
     __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_slot;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int q = warp & 3, h = warp >> 2;
@@ -71,11 +72,8 @@ __global__ void __launch_bounds__(NTHREADS, 2) actor_eval_tc_kernel(EvalTcArgs p
         sLs[tid] = ls; sLs[16 + tid] = expf(ls); sLs[32 + tid] = lo; sLs[48 + tid] = expf(lo);
     }
     if (tid == 0) { mbar_init(&bar, 1); mbar_init_fence(); }
-    if (warp == 0) tmem_alloc(&tmem_slot, 128);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
+    const Acc tm = acc_cta(p.acc, E_COLS);
     const uint32_t lane_base = (uint32_t)(q * 32) << 16;
     constexpr uint32_t C_Z = 0, C_OUT = 64;
     uint32_t phase = 0;
@@ -116,33 +114,31 @@ __global__ void __launch_bounds__(NTHREADS, 2) actor_eval_tc_kernel(EvalTcArgs p
             }
             fence_async_smem();
             __syncthreads();
-            if (tid == 0) { tc_fence_after(); tc_gemm(tmem + C_Z, B0, ET, sW1, 64, 128, 64, 64, c > 0); mma_commit(&bar); }
+            if (warp < 4) { tc_gemm(tm, C_Z, B0, ET, sW1, 64, 128, 64, 64, c > 0); mma_commit(&bar); }
             mbar_wait(&bar, phase); phase ^= 1;
-            tc_fence_after();
         }
         {
             float v[32];
-            tmem_ld32(tmem + lane_base + C_Z + 32 * h, v);
+            acc_ld32(tm, lane_base + C_Z + 32 * h, v);
 #pragma unroll
             for (int i = 0; i < 32; ++i) v[i] = tanh_fast(v[i] + sB1[32 * h + i]);
             store_row32(B2, 32 * q + lane, 32 * h, ET, v);
         }
-        fence_async_smem(); tc_fence_before();
+        fence_async_smem();
         __syncthreads();
-        if (tid == 0) { tc_fence_after(); tc_gemm(tmem + C_Z, B2, ET, sW2, 64, 128, 64, 64, false); mma_commit(&bar); }
+        if (warp < 4) { tc_gemm(tm, C_Z, B2, ET, sW2, 64, 128, 64, 64, false); mma_commit(&bar); }
         mbar_wait(&bar, phase); phase ^= 1;
-        tc_fence_after();
         {
             float v[32];
-            tmem_ld32(tmem + lane_base + C_Z + 32 * h, v);
+            acc_ld32(tm, lane_base + C_Z + 32 * h, v);
 #pragma unroll
             for (int i = 0; i < 32; ++i) v[i] = tanh_fast(v[i] + sB2[32 * h + i]);
             store_row32(B0, 32 * q + lane, 32 * h, ET, v);
         }
-        fence_async_smem(); tc_fence_before();
+        fence_async_smem();
         __syncthreads();
-        if (tid == 0) { tc_fence_after(); tc_gemm(tmem + C_OUT, B0, ET, sW3, 16, 128, 16, 64, false); mma_commit(&bar); }
-        // prefetch per-sample scalars while the MMA runs
+        if (warp < 4) { tc_gemm(tm, C_OUT, B0, ET, sW3, 16, 128, 16, 64, false); mma_commit(&bar); }
+        // per-sample scalars: requested before the wait (warps 4-7 while warpgroup 0 computes the output layer)
         const long long row = (h == 0) ? sRow[32 * q + lane] : -1;
         float pa[16], pm[16], plogp = 0.f, padvr = 0.f, padvc = 0.f;
 #pragma unroll
@@ -154,10 +150,9 @@ __global__ void __launch_bounds__(NTHREADS, 2) actor_eval_tc_kernel(EvalTcArgs p
             plogp = __ldg(p.logp + row); padvr = __ldg(p.adv_r + row); padvc = __ldg(p.adv_c + row);
         }
         mbar_wait(&bar, phase); phase ^= 1;
-        tc_fence_after();
         if (h == 0) {
             float o16[16];
-            tmem_ld16(tmem + lane_base + C_OUT, o16);
+            acc_ld16(tm, lane_base + C_OUT, o16);
             if (row >= 0) {
                 if (p.mu_store) {
                     for (int a = 0; a < A; ++a) p.mu_store[row * A + a] = o16[a] + sB3[a];
@@ -181,7 +176,6 @@ __global__ void __launch_bounds__(NTHREADS, 2) actor_eval_tc_kernel(EvalTcArgs p
                 }
             }
         }
-        tc_fence_before();
         __syncthreads();
     }
     if (!p.mu_store) {
@@ -192,9 +186,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) actor_eval_tc_kernel(EvalTcArgs p
         __syncthreads();
         if (tid < 6) p.part[(size_t)blockIdx.x * 8 + tid] = sRedD[tid] + sRedD[8 + tid] + sRedD[16 + tid] + sRedD[24 + tid];
     }
-    tc_fence_before();
     __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, 128);
 }
 
 }  // namespace osb
@@ -231,7 +223,7 @@ int osb_actor_eval_tc(const float* theta_actor, int O, int A, const float* obs, 
                       void* stream) {
     OSB_CHECK_ARG(theta_actor && obs && total > 0 && stride > 0 && O > 0 && O <= 512 && A > 0 && A <= 16, "bad argument (O <= 512)");
     OSB_CHECK_ARG(mu_store || (act && logp && adv_r && adv_c && mu_old && logstd_old && workspace && out), "null input");
-    EvalTcArgs p{obs, act, logp, adv_r, adv_c, mu_old, logstd_old, moments, lagrange, theta_actor, mu_store, workspace, total, stride, O, A};
+    EvalTcArgs p{obs, act, logp, adv_r, adv_c, mu_old, logstd_old, moments, lagrange, theta_actor, mu_store, workspace, nullptr, total, stride, O, A};
     const size_t smem = 1024 + 2 * (size_t)EBUF + 2 * 16384 + 4096 + (64 + 64 + 16 + 64) * 4 + 32 * 8 + 128 * 8 + 64;
     static bool attr = false;
     if (!attr) {
@@ -240,7 +232,10 @@ int osb_actor_eval_tc(const float* theta_actor, int O, int A, const float* obs, 
     }
     const long long nrows = (total + stride - 1) / stride;
     const long long tiles = (nrows + ET - 1) / ET;
-    const int blocks = (int)(tiles < 296 ? tiles : 296);
+    const int cap = 2 * grid_sms();
+    const int blocks = (int)(tiles < cap ? tiles : cap);
+    p.acc = acc_scratch(ACC_EVAL_TC, (size_t)blocks * 128 * E_COLS * sizeof(float));
+    if (!p.acc) return OSB_ERR_CUDA;
     cudaStream_t s = (cudaStream_t)stream;
     actor_eval_tc_kernel<<<blocks, NTHREADS, smem, s>>>(p);
     OSB_LAUNCH_CHECK();

@@ -19,14 +19,16 @@ constexpr int EX_NT = 256;                                           // 8 warps:
 constexpr uint32_t EX_SUB = EX_T * 128, EX_ACT = 3 * EX_SUB;         // [128][64] bf16 x3
 constexpr uint32_t EX_WSUB = 64 * 128, EX_W = 3 * EX_WSUB, EX_W3SUB = 16 * 128, EX_W3 = 3 * EX_W3SUB;
 constexpr uint32_t EXO_ACT = 0, EXO_W1 = EX_ACT, EXO_W2 = EXO_W1 + EX_W, EXO_W3 = EXO_W2 + EX_W, EXO_MISC = EXO_W3 + EX_W3;
-// misc floats: b1[64] b2[64] b3[16] ls[64]; then double red[32]; long long rows[128]; barrier; tmem slot
+// misc floats: b1[64] b2[64] b3[16] ls[64]; then double red[32]; long long rows[128]; barrier
 constexpr uint32_t EXO_RED = EXO_MISC + (64 + 64 + 16 + 64) * 4, EXO_ROWS = EXO_RED + 32 * 8, EXO_BAR = EXO_ROWS + EX_T * 8,
-                   EXO_SLOT = EXO_BAR + 8, EX_SMEM = EXO_SLOT + 8;
+                   EX_SMEM = EXO_BAR + 8;
+constexpr uint32_t EX_COLS = 80;                                     // accumulator columns: Z [0, 64), OUT [64, 80)
 
 struct EvalX3Args {
     const float* obs; const float* act; const float* logp; const float* adv_r; const float* adv_c;
     const float* mu_old; const float* logstd_old; const float* moments; const float* lagrange;
     const float* theta; float* mu_store; double* part;
+    float* acc;         // accumulator images, [gridDim.x][128][EX_COLS]
     long long total; int stride, O, A;
 };
 
@@ -42,7 +44,6 @@ __global__ void __launch_bounds__(EX_NT, 2) actor_eval_x3_kernel(EvalX3Args p) {
     double* sRedD = reinterpret_cast<double*>(gbase + EXO_RED);
     long long* sRow = reinterpret_cast<long long*>(gbase + EXO_ROWS);
     const uint32_t bar = sbase + EXO_BAR;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(gbase + EXO_SLOT);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int q = warp & 3, h = warp >> 2;
@@ -88,16 +89,12 @@ __global__ void __launch_bounds__(EX_NT, 2) actor_eval_x3_kernel(EvalX3Args p) {
         asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar), "r"(1u) : "memory");
         mbar_init_fence();
     }
-    if (warp == 0) tmem_alloc(tmem_slot, 128);
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
+    const Acc tm = acc_cta(p.acc, EX_COLS);
     const uint32_t lane_base = (uint32_t)(q * 32) << 16;
     constexpr uint32_t C_Z = 0, C_OUT = 64;
     uint32_t phase = 0;
-    const bool leader = (warp == 0) && elect_one_sync();
     const uint64_t dAct = desc128(sbase + EXO_ACT), dW1 = desc128(sbase + EXO_W1), dW2 = desc128(sbase + EXO_W2), dW3 = desc128(sbase + EXO_W3);
     const uint32_t id_fwd = idesc_bf16(128, 64, 0, 0), id_out = idesc_bf16(128, 16, 0, 0);
 
@@ -148,55 +145,46 @@ __global__ void __launch_bounds__(EX_NT, 2) actor_eval_x3_kernel(EvalX3Args p) {
                 if (a < A) { pa[a] = __ldg(p.act + row * A + a); pm[a] = __ldg(p.mu_old + row * A + a); }
             plogp = __ldg(p.logp + row); padvr = __ldg(p.adv_r + row); padvc = __ldg(p.adv_c + row);
         }
-        if (warp == 0) {
-            tc_fence_after();
-            gemm_x3_warp(leader, tmem + C_Z, dAct, EX_SUB, 32u, dW1, EX_WSUB, 32u, id_fwd, 4, false);
-            if (leader) mma_commit_a(bar);
-            __syncwarp();
+        if (warp < 4) {
+            gemm_x3(tm, C_Z, dAct, EX_SUB, 32u, dW1, EX_WSUB, 32u, id_fwd, 4, false);
+            mma_commit_a(bar);
         }
         mbar_wait_a(bar, phase); phase ^= 1;
-        tc_fence_after();
 #pragma unroll
         for (int c8 = 0; c8 < 4; ++c8) {                    // H1 over X
             const int c0 = 32 * h + 8 * c8;
             float v[8];
-            tmem_ld8(tmem + lane_base + C_Z + (uint32_t)c0, v);
+            acc_ld8(tm, lane_base + C_Z + (uint32_t)c0, v);
 #pragma unroll
             for (int i = 0; i < 8; ++i) v[i] = tanh_acc(v[i] + sB1[c0 + i]);
             store8_x3(sbase + EXO_ACT, EX_SUB, s_row, c0, v);
         }
-        fence_async_smem(); tc_fence_before();
+        fence_async_smem();
         __syncthreads();
-        if (warp == 0) {
-            tc_fence_after();
-            gemm_x3_warp(leader, tmem + C_Z, dAct, EX_SUB, 32u, dW2, EX_WSUB, 32u, id_fwd, 4, false);
-            if (leader) mma_commit_a(bar);
-            __syncwarp();
+        if (warp < 4) {
+            gemm_x3(tm, C_Z, dAct, EX_SUB, 32u, dW2, EX_WSUB, 32u, id_fwd, 4, false);
+            mma_commit_a(bar);
         }
         mbar_wait_a(bar, phase); phase ^= 1;
-        tc_fence_after();
 #pragma unroll
         for (int c8 = 0; c8 < 4; ++c8) {                    // H2 over H1
             const int c0 = 32 * h + 8 * c8;
             float v[8];
-            tmem_ld8(tmem + lane_base + C_Z + (uint32_t)c0, v);
+            acc_ld8(tm, lane_base + C_Z + (uint32_t)c0, v);
 #pragma unroll
             for (int i = 0; i < 8; ++i) v[i] = tanh_acc(v[i] + sB2[c0 + i]);
             store8_x3(sbase + EXO_ACT, EX_SUB, s_row, c0, v);
         }
-        fence_async_smem(); tc_fence_before();
+        fence_async_smem();
         __syncthreads();
-        if (warp == 0) {
-            tc_fence_after();
-            gemm_x3_warp(leader, tmem + C_OUT, dAct, EX_SUB, 32u, dW3, EX_W3SUB, 32u, id_out, 4, false);
-            if (leader) mma_commit_a(bar);
-            __syncwarp();
+        if (warp < 4) {
+            gemm_x3(tm, C_OUT, dAct, EX_SUB, 32u, dW3, EX_W3SUB, 32u, id_out, 4, false);
+            mma_commit_a(bar);
         }
         mbar_wait_a(bar, phase); phase ^= 1;
-        tc_fence_after();
         if (h == 0) {
             float o16[16];
-            tmem_ld16(tmem + lane_base + C_OUT, o16);
+            acc_ld16(tm, lane_base + C_OUT, o16);
             if (row >= 0) {
                 if (p.mu_store) {
                     for (int a = 0; a < A; ++a) p.mu_store[row * A + a] = o16[a] + sB3[a];
@@ -220,7 +208,6 @@ __global__ void __launch_bounds__(EX_NT, 2) actor_eval_x3_kernel(EvalX3Args p) {
                 }
             }
         }
-        tc_fence_before();
         __syncthreads();          // the OUT MMAs (readers of the buffer) completed; every thread is done with sRow
     }
     if (!p.mu_store) {
@@ -231,9 +218,7 @@ __global__ void __launch_bounds__(EX_NT, 2) actor_eval_x3_kernel(EvalX3Args p) {
         __syncthreads();
         if (tid < 6) p.part[(size_t)blockIdx.x * 8 + tid] = sRedD[tid] + sRedD[8 + tid] + sRedD[16 + tid] + sRedD[24 + tid];
     }
-    tc_fence_before();
     __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, 128);
 }
 
 }  // namespace osb
@@ -265,7 +250,7 @@ int osb_actor_eval_x3(const float* theta_actor, int O, int A, const float* obs, 
                       void* stream) {
     OSB_CHECK_ARG(theta_actor && obs && total > 0 && stride > 0 && O > 0 && O <= 64 && A > 0 && A <= 16, "bad argument (bf16x3 evaluation needs O <= 64)");
     OSB_CHECK_ARG(mu_store || (act && logp && adv_r && adv_c && mu_old && logstd_old && workspace && out), "null input");
-    EvalX3Args p{obs, act, logp, adv_r, adv_c, mu_old, logstd_old, moments, lagrange, theta_actor, mu_store, workspace, total, stride, O, A};
+    EvalX3Args p{obs, act, logp, adv_r, adv_c, mu_old, logstd_old, moments, lagrange, theta_actor, mu_store, workspace, nullptr, total, stride, O, A};
     const size_t smem = 1024 + EX_SMEM;
     static bool attr = false;
     if (!attr) {
@@ -274,7 +259,10 @@ int osb_actor_eval_x3(const float* theta_actor, int O, int A, const float* obs, 
     }
     const long long nrows = (total + stride - 1) / stride;
     const long long tiles = (nrows + EX_T - 1) / EX_T;
-    const int blocks = (int)(tiles < 296 ? tiles : 296);
+    const int cap = 2 * grid_sms();
+    const int blocks = (int)(tiles < cap ? tiles : cap);
+    p.acc = acc_scratch(ACC_EVAL_X3, (size_t)blocks * 128 * EX_COLS * sizeof(float));
+    if (!p.acc) return OSB_ERR_CUDA;
     cudaStream_t s = (cudaStream_t)stream;
     actor_eval_x3_kernel<<<blocks, EX_NT, smem, s>>>(p);
     OSB_LAUNCH_CHECK();

@@ -7,8 +7,8 @@
 //       T1 = X V1^T + bv1,              dH1 = (1 - H1^2) T1
 //       T2 = dH1 W2^T + H1 V2^T + bv2,  dH2 = (1 - H2^2) T2
 //       dmu = dH2 W3^T + H2 V3^T + bv3
-//   next to the ordinary forward (Z1 = X W1^T + b1, H1 = tanh Z1, ...), every GEMM as six kind::f16 MMAs over the three
-//   bf16 pieces of its fp32 operands (csrc/x3.cuh) with fp32 accumulation in TMEM.  The backward half J^T diag(sigma^-2)
+//   next to the ordinary forward (Z1 = X W1^T + b1, H1 = tanh Z1, ...), every GEMM as six bf16 wgmma products over the three
+//   bf16 pieces of its fp32 operands (csrc/x3.cuh) with fp32 accumulation in the accumulator image.  The backward half J^T diag(sigma^-2)
 //   dmu / (B A) is minibatch_grad_x3_kernel with the supplied-dOUT loss kind (csrc/update_x3.cu).
 //
 // One CTA per SM, tiles of 128 samples: two activation buffers (value and tangent; X / H1 / H2 overwrite each other in
@@ -27,13 +27,15 @@ constexpr uint32_t F_SUB = FT * 128, F_ACT = 3 * F_SUB;              // [128][64
 constexpr uint32_t F_WSUB = 64 * 128, F_W = 3 * F_WSUB, F_W3SUB = 16 * 128, F_W3 = 3 * F_W3SUB;
 constexpr uint32_t FO_A0 = 0, FO_A1 = F_ACT, FO_W1 = 2 * F_ACT, FO_V1 = FO_W1 + F_W, FO_W2 = FO_V1 + F_W, FO_V2 = FO_W2 + F_W,
                    FO_W3 = FO_V2 + F_W, FO_V3 = FO_W3 + F_W3, FO_MISC = FO_V3 + F_W3;
-// misc floats: b1[64] bv1[64] b2[64] bv2[64] bv3[16]; long long rows[128]; barrier; tmem slot
-constexpr uint32_t FO_ROWS = FO_MISC + (4 * 64 + 16) * 4, FO_BAR = FO_ROWS + FT * 8, FO_SLOT = FO_BAR + 8, F_SMEM = FO_SLOT + 8;
+// misc floats: b1[64] bv1[64] b2[64] bv2[64] bv3[16]; long long rows[128]; barrier
+constexpr uint32_t FO_ROWS = FO_MISC + (4 * 64 + 16) * 4, FO_BAR = FO_ROWS + FT * 8, F_SMEM = FO_BAR + 8;
+constexpr uint32_t F_COLS = 144;                                     // accumulator columns: Z [0, 64), T [64, 128), OUT [128, 144)
 
 struct FvpX3Args {
     const float* obs; long long total; int stride;
     const float* theta; const float* vec; float* dmu;
     int O, A;
+    float* acc;         // accumulator images, [gridDim.x][128][F_COLS]
 };
 
 // [rows][64] (rows = 64 or 16, zero padded) fp32 matrix with row pitch `ld` -> bf16x3 SW128 tile
@@ -64,7 +66,6 @@ __global__ void __launch_bounds__(FNT, 1) fvp_tangent_x3_kernel(FvpX3Args p) {
     float* sBv3 = sBv2 + 64;       // [16]
     long long* sRow = reinterpret_cast<long long*>(gbase + FO_ROWS);
     const uint32_t bar = sbase + FO_BAR;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(gbase + FO_SLOT);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int q = warp & 3, h = warp >> 2;
@@ -86,16 +87,12 @@ __global__ void __launch_bounds__(FNT, 1) fvp_tangent_x3_kernel(FvpX3Args p) {
         asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar), "r"(1u) : "memory");
         mbar_init_fence();
     }
-    if (warp == 0) tmem_alloc(tmem_slot, 256);
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
+    const Acc tm = acc_cta(p.acc, F_COLS);
     const uint32_t lane_base = (uint32_t)(q * 32) << 16;
     constexpr uint32_t C_Z = 0, C_T = 64, C_OUT = 128;
     uint32_t phase = 0;
-    const bool leader = (warp == 0) && elect_one_sync();
     const uint64_t dA0 = desc128(sbase + FO_A0), dA1 = desc128(sbase + FO_A1);
     const uint64_t dW1 = desc128(sbase + FO_W1), dV1 = desc128(sbase + FO_V1), dW2 = desc128(sbase + FO_W2), dV2 = desc128(sbase + FO_V2);
     const uint64_t dW3 = desc128(sbase + FO_W3), dV3 = desc128(sbase + FO_V3);
@@ -145,21 +142,18 @@ __global__ void __launch_bounds__(FNT, 1) fvp_tangent_x3_kernel(FvpX3Args p) {
         fence_async_smem();
         __syncthreads();
         // ---- layer 1: Z1 = X W1^T, T1 = X V1^T ------------------------------------------------------------------------
-        if (warp == 0) {
-            tc_fence_after();
-            gemm_x3_warp(leader, tmem + C_Z, dA0, F_SUB, 32u, dW1, F_WSUB, 32u, id_fwd, 4, false);
-            gemm_x3_warp(leader, tmem + C_T, dA0, F_SUB, 32u, dV1, F_WSUB, 32u, id_fwd, 4, false);
-            if (leader) mma_commit_a(bar);
-            __syncwarp();
+        if (warp < 4) {
+            gemm_x3(tm, C_Z, dA0, F_SUB, 32u, dW1, F_WSUB, 32u, id_fwd, 4, false);
+            gemm_x3(tm, C_T, dA0, F_SUB, 32u, dV1, F_WSUB, 32u, id_fwd, 4, false);
+            mma_commit_a(bar);
         }
         mbar_wait_a(bar, phase); phase ^= 1;
-        tc_fence_after();
 #pragma unroll
         for (int c8 = 0; c8 < 4; ++c8) {                    // H1 over X, dH1 into the tangent buffer
             const int c0 = 32 * h + 8 * c8;
             float z[8], t[8];
-            tmem_ld8(tmem + lane_base + C_Z + (uint32_t)c0, z);
-            tmem_ld8(tmem + lane_base + C_T + (uint32_t)c0, t);
+            acc_ld8(tm, lane_base + C_Z + (uint32_t)c0, z);
+            acc_ld8(tm, lane_base + C_T + (uint32_t)c0, t);
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
                 const float hh = tanh_acc(z[i] + sB1[c0 + i]);
@@ -169,26 +163,23 @@ __global__ void __launch_bounds__(FNT, 1) fvp_tangent_x3_kernel(FvpX3Args p) {
             store8_x3(sbase + FO_A0, F_SUB, s_row, c0, z);
             store8_x3(sbase + FO_A1, F_SUB, s_row, c0, t);
         }
-        fence_async_smem(); tc_fence_before();
+        fence_async_smem();
         __syncthreads();
         // ---- layer 2: Z2 = H1 W2^T, T2 = dH1 W2^T + H1 V2^T -------------------------------------------------------------
-        if (warp == 0) {
-            tc_fence_after();
-            gemm_x3_warp(leader, tmem + C_Z, dA0, F_SUB, 32u, dW2, F_WSUB, 32u, id_fwd, 4, false);
-            gemm_x3_warp(leader, tmem + C_T, dA1, F_SUB, 32u, dW2, F_WSUB, 32u, id_fwd, 4, false);
-            gemm_x3_warp(leader, tmem + C_T, dA0, F_SUB, 32u, dV2, F_WSUB, 32u, id_fwd, 4, true);
-            if (leader) mma_commit_a(bar);
-            __syncwarp();
+        if (warp < 4) {
+            gemm_x3(tm, C_Z, dA0, F_SUB, 32u, dW2, F_WSUB, 32u, id_fwd, 4, false);
+            gemm_x3(tm, C_T, dA1, F_SUB, 32u, dW2, F_WSUB, 32u, id_fwd, 4, false);
+            gemm_x3(tm, C_T, dA0, F_SUB, 32u, dV2, F_WSUB, 32u, id_fwd, 4, true);
+            mma_commit_a(bar);
         }
         gather(tile + gridDim.x);                            // next tile's rows fly under layers 2 and 3
         mbar_wait_a(bar, phase); phase ^= 1;
-        tc_fence_after();
 #pragma unroll
         for (int c8 = 0; c8 < 4; ++c8) {                    // H2 over H1, dH2 over dH1
             const int c0 = 32 * h + 8 * c8;
             float z[8], t[8];
-            tmem_ld8(tmem + lane_base + C_Z + (uint32_t)c0, z);
-            tmem_ld8(tmem + lane_base + C_T + (uint32_t)c0, t);
+            acc_ld8(tm, lane_base + C_Z + (uint32_t)c0, z);
+            acc_ld8(tm, lane_base + C_T + (uint32_t)c0, t);
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
                 const float hh = tanh_acc(z[i] + sB2[c0 + i]);
@@ -198,31 +189,25 @@ __global__ void __launch_bounds__(FNT, 1) fvp_tangent_x3_kernel(FvpX3Args p) {
             store8_x3(sbase + FO_A0, F_SUB, s_row, c0, z);
             store8_x3(sbase + FO_A1, F_SUB, s_row, c0, t);
         }
-        fence_async_smem(); tc_fence_before();
+        fence_async_smem();
         __syncthreads();
         // ---- layer 3: dmu = dH2 W3^T + H2 V3^T + bv3 ---------------------------------------------------------------------
-        if (warp == 0) {
-            tc_fence_after();
-            gemm_x3_warp(leader, tmem + C_OUT, dA1, F_SUB, 32u, dW3, F_W3SUB, 32u, id_out, 4, false);
-            gemm_x3_warp(leader, tmem + C_OUT, dA0, F_SUB, 32u, dV3, F_W3SUB, 32u, id_out, 4, true);
-            if (leader) mma_commit_a(bar);
-            __syncwarp();
+        if (warp < 4) {
+            gemm_x3(tm, C_OUT, dA1, F_SUB, 32u, dW3, F_W3SUB, 32u, id_out, 4, false);
+            gemm_x3(tm, C_OUT, dA0, F_SUB, 32u, dV3, F_W3SUB, 32u, id_out, 4, true);
+            mma_commit_a(bar);
         }
         const long long row = (h == 0) ? sRow[s_row] : -1;
         mbar_wait_a(bar, phase); phase ^= 1;
-        tc_fence_after();
         if (h == 0) {
             float o16[16];
-            tmem_ld16(tmem + lane_base + C_OUT, o16);
+            acc_ld16(tm, lane_base + C_OUT, o16);
             if (row >= 0)
                 for (int a = 0; a < A; ++a) p.dmu[row * A + a] = o16[a] + sBv3[a];
         }
-        tc_fence_before();
         __syncthreads();          // the layer-3 MMAs (readers of both buffers) completed; every thread is done with sRow
     }
-    tc_fence_before();
     __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, 256);
 }
 
 }  // namespace osb
@@ -245,7 +230,7 @@ int osb_fvp_partials_x3(const float* theta_actor, const float* vec, int O, int A
     OSB_CHECK_ARG(O > 0 && O <= 64 && A > 0 && A <= 16, "bf16x3 path needs O <= 64, A <= 16");
     const long long nrows = (total + stride - 1) / stride;
     OSB_CHECK_ARG(nrows < (1ll << 31), "too many rows");
-    FvpX3Args t{obs, total, stride, theta_actor, vec, dmu, O, A};
+    FvpX3Args t{obs, total, stride, theta_actor, vec, dmu, O, A, nullptr};
     const size_t smem = 1024 + F_SMEM;
     static bool attr = false;
     if (!attr) {
@@ -256,6 +241,8 @@ int osb_fvp_partials_x3(const float* theta_actor, const float* vec, int O, int A
     static int n_sm = 0;
     if (!n_sm) { int dev = 0; OSB_CUDA(cudaGetDevice(&dev)); OSB_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev)); }
     const int blocks = (int)(tiles < n_sm ? tiles : n_sm);
+    t.acc = acc_scratch(ACC_FVP_X3, (size_t)blocks * 128 * F_COLS * sizeof(float));
+    if (!t.acc) return OSB_ERR_CUDA;
     fvp_tangent_x3_kernel<<<blocks, FNT, smem, (cudaStream_t)stream>>>(t);
     OSB_LAUNCH_CHECK();
     return osb_x3_fvp_backward(theta_actor, vec, O, A, obs, total, stride, dmu, gpart, stats_scratch, stream);

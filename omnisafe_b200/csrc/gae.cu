@@ -1,4 +1,4 @@
-// Dual (reward + cost) GAE as a segmented reverse inclusive scan -- sm_100a.
+// Dual (reward + cost) GAE as a segmented reverse inclusive scan -- sm_90a.
 //
 // Replaces the per-path Python recursions of the reference:
 //   omnisafe/common/buffer/onpolicy_buffer.py:L148-203 (finish_path)
@@ -302,8 +302,6 @@ __global__ void __launch_bounds__(GTHREADS, (MULTI || EST == 1 || EST == 3) ? 1 
 // onto the tile carry (<= 15 fp64 FMAs), pass 2 replays the reference's separately rounded fp64 recurrence
 // from that carry-in and stores the four output rows straight from registers (coalesced 128 B stores).
 // Path ends and the bootstrap values of cut paths (sparse) are fetched one tile ahead.
-// Measured on B200 (tools/gae_times.py): 4.1-4.2 TB/s of algorithmic traffic at T = 2048 x 4096 envs
-// (277 MB, larger than L2), 4.4-4.6 TB/s at T = 4096; the generic kernel above: 2.8 TB/s.
 constexpr int SW = 16;                                  // warps = time chunks per tile
 constexpr int SL = 8;                                   // steps per chunk
 constexpr int ST = SW * SL;                             // 128 steps per tile
@@ -314,7 +312,7 @@ constexpr uint32_t S_PLANE_V = (ST + 1) * SE * 4;       // value planes carry on
 constexpr uint32_t S_FLAGS = ST * SE;
 constexpr uint32_t S_OFF_REW = 0, S_OFF_COST = S_PLANE, S_OFF_VR = 2 * S_PLANE, S_OFF_VC = 2 * S_PLANE + S_PLANE_V,
                    S_OFF_FL = 2 * S_PLANE + 2 * S_PLANE_V, S_STAGE = S_OFF_FL + S_FLAGS;            // 69 888 B
-constexpr int NSTG = 2;                                  // stages of the input pipeline (three stages measured no faster)
+constexpr int NSTG = 2;                                  // stages of the input pipeline
 constexpr uint32_t S_OFF_MAPS = NSTG * S_STAGE;                                 // double [2][SW][4][32]: (a_r, b_r, a_c, b_c) per chunk
 constexpr uint32_t S_OFF_CARRY = S_OFF_MAPS + 2 * SW * 4 * 32 * 8;           // double [2][2][32]
 constexpr uint32_t S_OFF_RED = S_OFF_CARRY + 2 * 2 * 32 * 8;                 // double [3][SW]
@@ -364,8 +362,7 @@ __device__ __forceinline__ void s_cp_arrive(uint32_t bar) {
 // TMA = false (OSB_GAE_LDGSTS=1): every thread copies 16-byte pieces of the tile with cp.async (LDGSTS) -- ~9 copies per thread
 //   and tile, each thread's batch arriving on the stage's mbarrier.
 // TMA = true (default): one elected thread issues cp.async.bulk.tensor.2d boxes {32 envs x 128 (129) steps}.
-//   Measured on B200: boxes with 128-byte rows 4N bytes apart stream at only ~21 GB/s per SM (one row request per
-//   ~10 cycles, from DRAM and from L2 alike), capping the kernel at 2.7 TB/s with the arithmetic removed.
+//   A box of 128-byte rows 4N bytes apart costs one row request per row: the per-SM request rate, not DRAM, bounds it.
 // MODE 0: both halves by cp.async; MODE 1: both by TMA; MODE 2: the A half (reward, cost, flags) by TMA and the B half
 // (values) by cp.async -- two independent load paths working side by side.
 template <int MODE>
@@ -565,7 +562,7 @@ __global__ void __launch_bounds__(STHREADS, 1) gae_stream_kernel(const __grid_co
             const ptrdiff_t d_ac = p.adv_c - p.adv_r, d_tr = p.tv_r - p.adv_r, d_tc = p.tv_c - p.adv_r;
             // A path end restarts the recurrence (x + d * 0 == x exactly).  Each row's roundings / stores sit in their own
             // guarded block on purpose: bursts of 64-bit conversions (XU pipe) issued back to back throttle the shared
-            // memory / special-function queue (measured 6 % slower as straight-line code).  The statistics sum the fp64
+            // memory / special-function queue.  The statistics sum the fp64
             // advantages before their rounding to fp32 (|difference| <= 2^-25 relative per element, random sign).
 #pragma unroll
             for (int i = SL - 1; i >= 0; --i) {
@@ -791,8 +788,8 @@ int osb_adv_estimate(const float* rew, const float* cost, const float* val_r, co
     a.sums = sums;
     a.ticket = reinterpret_cast<unsigned int*>(workspace + (size_t)nblocks * 4 + 1);
     cudaStream_t s = (cudaStream_t)stream;
-    // the 64-register instantiation (two CTAs per SM) wins at every T measured on B200: occupancy beats
-    // the register-hungry prefetching variant, which is kept for experiments (OSB_GAE_PREFETCH=1)
+    // the 64-register instantiation (two CTAs per SM) is the default: it keeps two CTAs per SM resident, which the
+    // register-hungry prefetching variant does not; that one is kept for experiments (OSB_GAE_PREFETCH=1)
     static const bool prefetch = getenv("OSB_GAE_PREFETCH") != nullptr;
     const bool ret = disc_ret != nullptr;
     const dim3 blk(GE, GC);
@@ -841,7 +838,7 @@ int osb_adv_standardize(const float* adv_r, const float* adv_c, const float* mom
     OSB_CHECK_ARG(adv_r && adv_c && moments && out_r && out_c && n >= 0, "bad argument");
     if (n == 0) return OSB_OK;
     int blocks = (int)((n + 255) / 256);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 8 * grid_sms()) blocks = 8 * grid_sms();
     adv_standardize_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(adv_r, adv_c, moments,
                                                                     (size_t)n, out_r, out_c);
     OSB_LAUNCH_CHECK();

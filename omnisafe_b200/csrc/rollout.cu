@@ -274,10 +274,11 @@ struct StepArgs {
     uint32_t global_step; // epoch * T + t, Philox counter
     int t, T, N;
     int is_tail;          // t == T: critics only (epoch-end bootstrap)
-    int precision;        // 0 = fp32 FMA tiles of 32 envs, 1 = tcgen05 TF32 tiles of 128 envs, 2 = split-bf16 tcgen05 tiles (O <= 64)
+    int precision;        // 0 = fp32 FMA tiles of 32 envs, 1 = wgmma TF32 tiles of 128 envs, 2 = split-bf16 wgmma tiles (O <= 64)
     unsigned int* bar_ctr;    // persistent epoch kernel: grid-barrier arrival counter and release flag (zero at launch)
     unsigned int* bar_flag;
     long long* dbg;           // optional clock64 stamps (persistent kernel), normally null
+    float* acc;               // tensor-core tiles: accumulator images, one [128][R_COLS] per CTA
 };
 
 // normalise (or copy) a tile of raw observations into sX (chunk kc), zero padded.
@@ -575,19 +576,20 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
 
 // ---------------------------------------------------------------------------------------------
 // Tensor-core variant of the step kernel (train_cfgs.matmul_precision = tf32, O <= 64): tiles of 128
-// envs, the three layer GEMMs of a network as tcgen05.mma kind::tf32 with TMEM accumulators, operands
+// envs, the three layer GEMMs of a network as tf32 wgmma with accumulator images, operands
 // staged as 128B-swizzled K-major smem tiles.  Everything around the GEMMs (ObsNormalize, sampling,
 // env transition, slab append, normaliser sums, ticket) is the arithmetic of rollout_step_kernel.
 constexpr int RTC = 128;
+constexpr uint32_t R_COLS = 80;   // accumulator columns: Z [0, 64), OUT [64, 80)
 constexpr int SNW = KC + 1;   // row stride of the next-state staging tiles
 
-// X3 = false: kind::tf32 tiles (5e-3);  X3 = true: split-bf16 tiles (csrc/x3.cuh), fp32-level values / log-probs:
+// X3 = false: tf32 wgmma tiles (5e-3);  X3 = true: split-bf16 tiles (csrc/x3.cuh), fp32-level values / log-probs:
 // one bf16x3 activation buffer (X, H1, H2 overwrite each other in place), accurate tanh, warp-uniform MMA issue.
 constexpr uint32_t RX_SUB = RTC * 128, RX_WSUB = 64 * 128, RX_W3SUB = 16 * 128;
 constexpr uint32_t RTC_FOFF_TF32 = 2 * RTC * 256 + 2 * 16384 + 4096, RTC_FOFF_X3 = 3 * RX_SUB + 6 * RX_WSUB + 3 * RX_W3SUB;
 
 // PERSIST = true: ONE cooperative launch runs the whole epoch (steps 0 .. T, the last one being the critics' epoch-end
-// bootstrap): the weight tiles, biases and the TMEM allocation stay resident, every step ends in a grid barrier whose
+// bootstrap): the weight tiles, biases and the accumulator image allocation stay resident, every step ends in a grid barrier whose
 // last arriver folds the step's normaliser sums into the running statistics before it releases the others
 // (adapter/onpolicy_adapter.py:L58-136 is the loop this replaces).  Data written by other CTAs in earlier steps
 // (raw states, flags, normaliser statistics) is read with ld.global.cg.
@@ -617,7 +619,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
     float* sSd = reinterpret_cast<float*>(sGstep + RTC);                // [3][16] sigma, 2 sigma^2, log sigma per action
     float* sEarlyAcc = sSd + 48;                                        // [128] accumulated cost incl. this step (EarlyTerminated)
     __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_slot;
     __shared__ int s_last, s_anyfin;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -702,11 +703,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
         sSd[tid] = sd; sSd[16 + tid] = __fmul_rn(2.f, __fmul_rn(sd, sd)); sSd[32 + tid] = logf(sd);
     }
     if (tid == 0) { mbar_init(&bar, 1); mbar_init_fence(); s_anyfin = 0; }
-    if (warp == 0) tmem_alloc(&tmem_slot, 128);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
+    const Acc tm = acc_cta(p.acc, R_COLS);
     const uint32_t lane_base = (uint32_t)(q * 32) << 16;
     constexpr uint32_t C_Z = 0, C_OUT = 64;
     uint32_t phase = 0;
@@ -840,89 +838,76 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
         RSTAMP(2);
         if constexpr (X3) {
             // three layers on bf16x3 tiles, one activation buffer: every epilogue starts after its layer's MMAs completed
-            const bool leader = (warp == 0) && x3::elect_one_sync();
             const uint64_t dAct = x3::desc128(B0), dW1 = x3::desc128(sW1), dW2 = x3::desc128(sW2), dW3 = x3::desc128(sW3);
-            if (warp == 0) {
-                tc_fence_after();
-                x3::gemm_x3_warp(leader, tmem + C_Z, dAct, RX_SUB, 32u, dW1, RX_WSUB, 32u, x3::idesc_bf16(128, 64, 0, 0), 4, false);
-                if (leader) mma_commit(&bar);
-                __syncwarp();
+            if (warp < 4) {
+                x3::gemm_x3(tm, C_Z, dAct, RX_SUB, 32u, dW1, RX_WSUB, 32u, x3::idesc_bf16(128, 64, 0, 0), 4, false);
+                mma_commit(&bar);
             }
             mbar_wait(&bar, phase); phase ^= 1;
             RSTAMP(3);
-            tc_fence_after();
 #pragma unroll
             for (int c8 = 0; c8 < 4; ++c8) {
                 const int c0 = 32 * h + 8 * c8;
                 float v[8];
-                x3::tmem_ld8(tmem + lane_base + C_Z + (uint32_t)c0, v);
+                x3::acc_ld8(tm, lane_base + C_Z + (uint32_t)c0, v);
 #pragma unroll
                 for (int i = 0; i < 8; ++i) v[i] = x3::tanh_acc(v[i] + sB1[c0 + i]);
                 x3::store8_x3(B0, RX_SUB, 32 * q + lane, c0, v);
             }
-            fence_async_smem(); tc_fence_before();
+            fence_async_smem();
             __syncthreads();
-            if (warp == 0) {
-                tc_fence_after();
-                x3::gemm_x3_warp(leader, tmem + C_Z, dAct, RX_SUB, 32u, dW2, RX_WSUB, 32u, x3::idesc_bf16(128, 64, 0, 0), 4, false);
-                if (leader) mma_commit(&bar);
-                __syncwarp();
+            if (warp < 4) {
+                x3::gemm_x3(tm, C_Z, dAct, RX_SUB, 32u, dW2, RX_WSUB, 32u, x3::idesc_bf16(128, 64, 0, 0), 4, false);
+                mma_commit(&bar);
             }
             mbar_wait(&bar, phase); phase ^= 1;
             RSTAMP(4);
-            tc_fence_after();
 #pragma unroll
             for (int c8 = 0; c8 < 4; ++c8) {
                 const int c0 = 32 * h + 8 * c8;
                 float v[8];
-                x3::tmem_ld8(tmem + lane_base + C_Z + (uint32_t)c0, v);
+                x3::acc_ld8(tm, lane_base + C_Z + (uint32_t)c0, v);
 #pragma unroll
                 for (int i = 0; i < 8; ++i) v[i] = x3::tanh_acc(v[i] + sB2[c0 + i]);
                 x3::store8_x3(B0, RX_SUB, 32 * q + lane, c0, v);
             }
-            fence_async_smem(); tc_fence_before();
+            fence_async_smem();
             __syncthreads();
-            if (warp == 0) {
-                tc_fence_after();
-                x3::gemm_x3_warp(leader, tmem + C_OUT, dAct, RX_SUB, 32u, dW3, RX_W3SUB, 32u, x3::idesc_bf16(128, 16, 0, 0), 4, false);
-                if (leader) mma_commit(&bar);
-                __syncwarp();
+            if (warp < 4) {
+                x3::gemm_x3(tm, C_OUT, dAct, RX_SUB, 32u, dW3, RX_W3SUB, 32u, x3::idesc_bf16(128, 16, 0, 0), 4, false);
+                mma_commit(&bar);
             }
             mbar_wait(&bar, phase); phase ^= 1;
             RSTAMP(5);
-            tc_fence_after();
         } else {
-        if (tid == 0) { tc_fence_after(); tc_gemm(tmem + C_Z, B0, RTC, sW1, 64, 128, 64, 64, false); mma_commit(&bar); }
+        if (warp < 4) { tc_gemm(tm, C_Z, B0, RTC, sW1, 64, 128, 64, 64, false); mma_commit(&bar); }
         mbar_wait(&bar, phase); phase ^= 1;
-        tc_fence_after();
         {
             float v[32];
-            tmem_ld32(tmem + lane_base + C_Z + 32 * h, v);
+            acc_ld32(tm, lane_base + C_Z + 32 * h, v);
 #pragma unroll
             for (int i = 0; i < 32; ++i) v[i] = tanh_fast(v[i] + sB1[32 * h + i]);
             store_row32(B2, 32 * q + lane, 32 * h, RTC, v);
         }
-        fence_async_smem(); tc_fence_before();
+        fence_async_smem();
         __syncthreads();
-        if (tid == 0) { tc_fence_after(); tc_gemm(tmem + C_Z, B2, RTC, sW2, 64, 128, 64, 64, false); mma_commit(&bar); }
+        if (warp < 4) { tc_gemm(tm, C_Z, B2, RTC, sW2, 64, 128, 64, 64, false); mma_commit(&bar); }
         mbar_wait(&bar, phase); phase ^= 1;
-        tc_fence_after();
         {
             float v[32];
-            tmem_ld32(tmem + lane_base + C_Z + 32 * h, v);
+            acc_ld32(tm, lane_base + C_Z + 32 * h, v);
 #pragma unroll
             for (int i = 0; i < 32; ++i) v[i] = tanh_fast(v[i] + sB2[32 * h + i]);
             store_row32(B0, 32 * q + lane, 32 * h, RTC, v);
         }
-        fence_async_smem(); tc_fence_before();
+        fence_async_smem();
         __syncthreads();
-        if (tid == 0) { tc_fence_after(); tc_gemm(tmem + C_OUT, B0, RTC, sW3, 16, 128, 16, 64, false); mma_commit(&bar); }
+        if (warp < 4) { tc_gemm(tm, C_OUT, B0, RTC, sW3, 16, 128, 16, 64, false); mma_commit(&bar); }
         mbar_wait(&bar, phase); phase ^= 1;
-        tc_fence_after();
         }
         if (h == 0) {
             float o16[16];
-            tmem_ld16(tmem + lane_base + C_OUT, o16);
+            acc_ld16(tm, lane_base + C_OUT, o16);
             const int e = 32 * q + lane;
             const int env = env0 + e;
             if (net != 0) {
@@ -945,7 +930,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                 for (int a = 0; a < 16; ++a) sAct[e * OUTP + a] = o16[a] + sB3[a];   // mu
             }
         }
-        tc_fence_before();
         __syncthreads();
     }
 
@@ -1162,9 +1146,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
     }
     }   // step loop
 #undef RSTAMP
-    tc_fence_before();
     __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, 128);
 }
 
 static size_t rollout_tc_smem_bytes(bool x3) {
@@ -1320,6 +1302,8 @@ static int launch_step(StepArgs& p, cudaStream_t stream) {
             attr_tc = true;
         }
         dim3 grid_tc((p.N + RTC - 1) / RTC, p.is_tail ? 2 : 3);
+        p.acc = acc_scratch(ACC_ROLLOUT, (size_t)grid_tc.x * 3 * 128 * R_COLS * sizeof(float));
+        if (!p.acc) return OSB_ERR_CUDA;
         if (p.bar_ctr != nullptr) {
             // the whole epoch in one cooperative launch (every CTA resident: the step barrier is a software grid barrier)
             OSB_CUDA(cudaMemsetAsync(p.bar_ctr, 0, 2 * sizeof(unsigned int), stream));

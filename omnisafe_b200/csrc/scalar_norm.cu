@@ -101,7 +101,7 @@ int osb_scalar_normalize_rows(float* x, int T, int N, float clip, float* state, 
     OSB_LAUNCH_CHECK();
     const size_t total = (size_t)T * N;
     int blocks = (int)((total + SN_THREADS - 1) / SN_THREADS);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 8 * grid_sms()) blocks = 8 * grid_sms();
     row_apply_kernel<<<blocks, SN_THREADS, 0, s>>>(x, T, N, clip, row_stats);
     OSB_LAUNCH_CHECK();
     return OSB_OK;

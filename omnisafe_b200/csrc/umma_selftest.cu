@@ -1,126 +1,55 @@
-// Self-test of the tcgen05 building blocks: D[128][N] = A * B^T with every operand-major combination,
-// used by tests/test_umma_gpu.py to pin descriptor / swizzle / TMEM-lane conventions on real hardware.
+// Self-test of the tf32 wgmma building blocks: D[M][N] = A * B^T on one warpgroup, used by
+// tests/test_umma_gpu.py to pin the descriptor / swizzle / accumulator-lane conventions on real hardware.
 #include "common.cuh"
 #include "umma.cuh"
 
 namespace osb {
 
-// A given as a_mn ? A_t[K][M] : A[M][K];  B given as b_mn ? B_t[K][N] : B[N][K]   (row-major fp32)
-// out[128][N]: raw dump of TMEM lanes 0..127, columns 0..N-1.
+// A[M][K], B[N][K] (row-major fp32), both staged K-major.  out[128][N]: dump of accumulator lanes 0..127.
 __global__ void __launch_bounds__(128, 1) umma_selftest_kernel(const float* __restrict__ A,
                                                                const float* __restrict__ B, int M, int N,
-                                                               int K, int a_mn, int b_mn,
+                                                               int K, float* __restrict__ scratch,
                                                                float* __restrict__ out) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_slot;
-    // tiles: A -> rows RA x cols CA ; K-major: [M][K]; MN-major: [K][M]
-    const int RA = a_mn ? K : M, CA = a_mn ? M : K;
-    const int RB = b_mn ? K : N, CB = b_mn ? N : K;
-    const int CAp = (CA + 31) & ~31, CBp = (CB + 31) & ~31;
+    const int Kp = (K + 31) & ~31;
     uint8_t* sA = smem;
-    uint8_t* sB = smem + (size_t)(CAp / 32) * RA * 128 + 65536;   // generous gap: M=128 may read past A
-    const int tid = threadIdx.x, warp = tid >> 5;
-
-    for (int i = tid; i < 65536 / 4; i += 128) reinterpret_cast<float*>(sA + (size_t)(CAp / 32) * RA * 128)[i] = 0.f;
-    for (int i = tid; i < RA * CAp; i += 128) {
-        const int r = i / CAp, c = i % CAp;
-        *reinterpret_cast<float*>(sA + umma::sw128_offset(r, c, RA)) = (c < CA) ? A[(size_t)r * CA + c] : 0.f;
+    uint8_t* sB = smem + (size_t)(Kp / 32) * M * 128;
+    const int tid = threadIdx.x;
+    for (int i = tid; i < M * Kp; i += 128) {
+        const int r = i / Kp, c = i % Kp;
+        *reinterpret_cast<float*>(sA + umma::sw128_offset(r, c, M)) = (c < K) ? A[(size_t)r * K + c] : 0.f;
     }
-    for (int i = tid; i < RB * CBp; i += 128) {
-        const int r = i / CBp, c = i % CBp;
-        *reinterpret_cast<float*>(sB + umma::sw128_offset(r, c, RB)) = (c < CB) ? B[(size_t)r * CB + c] : 0.f;
+    for (int i = tid; i < N * Kp; i += 128) {
+        const int r = i / Kp, c = i % Kp;
+        *reinterpret_cast<float*>(sB + umma::sw128_offset(r, c, N)) = (c < K) ? B[(size_t)r * K + c] : 0.f;
     }
-    if (tid == 0) { umma::mbar_init(&bar, 1); umma::mbar_init_fence(); }
-    if (warp == 0) umma::tmem_alloc(&tmem_slot, 256);
     umma::fence_async_smem();
-    umma::tc_fence_before();
     __syncthreads();
-    umma::tc_fence_after();
-    const uint32_t tmem = tmem_slot;
-
-    if (tid == 0) {
-        // zero lanes 0..127 x N columns first (M = 128 MMA with the zeroed gap as A), then the real MMA
-        const uint32_t zA = umma::smem_u32(sA + (size_t)(CAp / 32) * RA * 128);
-        const uint32_t idz = umma::idesc_tf32(128, N, 0, b_mn);
-        umma::mma_tf32(tmem, umma::desc_kmajor(zA), b_mn ? umma::desc_mnmajor(umma::smem_u32(sB), RB * 128)
-                                                         : umma::desc_kmajor(umma::smem_u32(sB)), idz, 0u);
-        const uint32_t id = umma::idesc_tf32(M, N, a_mn, b_mn);
-        for (int k = 0; k < K; k += 8) {
-            // K-major: advance 32 B inside the 128 B row, next atom after 32 floats; MN-major: 8 rows = 1024 B
-            const uint32_t offA = a_mn ? (uint32_t)(k / 8) * 1024u : (uint32_t)((k / 32) * RA * 128 + (k % 32) * 4);
-            const uint32_t offB = b_mn ? (uint32_t)(k / 8) * 1024u : (uint32_t)((k / 32) * RB * 128 + (k % 32) * 4);
-            const uint64_t da = a_mn ? umma::desc_mnmajor(umma::smem_u32(sA) + offA, RA * 128)
-                                     : umma::desc_kmajor(umma::smem_u32(sA) + offA);
-            const uint64_t db = b_mn ? umma::desc_mnmajor(umma::smem_u32(sB) + offB, RB * 128)
-                                     : umma::desc_kmajor(umma::smem_u32(sB) + offB);
-            umma::mma_tf32(tmem, da, db, id, k > 0 ? 1u : 0u);
-        }
-        umma::mma_commit(&bar);
-    }
-    umma::mbar_wait(&bar, 0);
-    umma::tc_fence_after();
+    const umma::Acc acc = umma::acc_cta(scratch, (uint32_t)N);
+    umma::tc_gemm(acc, 0u, umma::smem_u32(sA), M, umma::smem_u32(sB), N, M, N, K, false);
+    __threadfence_block();
+    __syncthreads();
     for (int c0 = 0; c0 < N; c0 += 16) {
         float v[16];
-        umma::tmem_ld16(tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
+        umma::acc_ld16(acc, ((uint32_t)(tid & ~31) << 16) + (uint32_t)c0, v);
         for (int j = 0; j < 16; ++j) out[(size_t)tid * N + c0 + j] = v[j];
     }
-    umma::tc_fence_before();
-    __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(tmem, 256);
-}
-
-// timing probe: `reps` back-to-back MMAs of shape M x N x 8 (tf32) issued by one thread, then commit +
-// mbarrier wait; out[0] = cycles from first issue to completion, out[1] = cycles of the issue loop.
-__global__ void __launch_bounds__(128, 1) umma_timing_kernel(int M, int N, int reps, long long* out) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_slot;
-    const uint32_t pad = (1024u - (umma::smem_u32(smem_raw) & 1023u)) & 1023u;
-    const uint32_t sA = umma::smem_u32(smem_raw) + pad, sB = sA + 32768;
-    for (int i = threadIdx.x; i < 65536 / 4; i += 128) reinterpret_cast<float*>(smem_raw + pad)[i] = 1.0f;
-    if (threadIdx.x == 0) { umma::mbar_init(&bar, 1); umma::mbar_init_fence(); }
-    if (threadIdx.x < 32) umma::tmem_alloc(&tmem_slot, 256);
-    umma::fence_async_smem();
-    umma::tc_fence_before();
-    __syncthreads();
-    umma::tc_fence_after();
-    const uint32_t tmem = tmem_slot;
-    long long t0 = 0, t1 = 0, t2 = 0;
-    if (threadIdx.x == 0) {
-        const uint32_t id = umma::idesc_tf32(M, N, 0, 0);
-        t0 = clock64();
-        for (int r = 0; r < reps; ++r)
-            umma::mma_tf32(tmem, umma::desc_kmajor(sA + (uint32_t)(r & 3) * 32u), umma::desc_kmajor(sB + (uint32_t)(r & 3) * 32u), id, r > 0);
-        umma::mma_commit(&bar);
-        t1 = clock64();
-    }
-    umma::mbar_wait(&bar, 0);
-    if (threadIdx.x == 0) { t2 = clock64(); out[0] = t2 - t0; out[1] = t1 - t0; }
-    umma::tc_fence_before();
-    __syncthreads();
-    if (threadIdx.x < 32) umma::tmem_dealloc(tmem, 256);
 }
 
 }  // namespace osb
 
-extern "C" int osb_umma_timing(int M, int N, int reps, long long* out, void* stream) {
-    OSB_CHECK_ARG(out && (M == 64 || M == 128) && N % 16 == 0 && N <= 256 && reps > 0, "bad argument");
-    const size_t smem = 1024 + 65536;
-    OSB_CUDA(cudaFuncSetAttribute(osb::umma_timing_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    osb::umma_timing_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(M, N, reps, out);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
-}
-
 extern "C" int osb_umma_selftest(const float* A, const float* B, int M, int N, int K, int a_mn, int b_mn,
                                  float* out, void* stream) {
     OSB_CHECK_ARG(A && B && out, "null pointer");
-    OSB_CHECK_ARG((M == 64 || M == 128) && N % 16 == 0 && N >= 16 && N <= 256 && K % 8 == 0 && K <= 128, "bad shape");
-    const size_t smem = 1024 + 65536 + 65536 + 65536;
+    OSB_CHECK_ARG(!a_mn && !b_mn, "tf32 wgmma reads both operands K-major");
+    OSB_CHECK_ARG((M == 64 || M == 128) && (N == 16 || (N % 64 == 0 && N <= 256)) && K % 8 == 0 && K >= 8 && K <= 128,
+                  "bad shape");
+    float* scratch = osb::acc_scratch(osb::ACC_SELFTEST, (size_t)128 * N * sizeof(float));
+    if (!scratch) return OSB_ERR_CUDA;
+    const size_t smem = 1024 + (size_t)((K + 31) / 32) * (M + N) * 128;
     OSB_CUDA(cudaFuncSetAttribute(osb::umma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    osb::umma_selftest_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(A, B, M, N, K, a_mn, b_mn, out);
+    osb::umma_selftest_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(A, B, M, N, K, scratch, out);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
 }

@@ -829,10 +829,11 @@ static size_t fvp_smem_bytes() {
 
 extern "C" {
 
-// CTAs per network: the three networks of a minibatch step share the 148 SMs in one wave
+// CTAs per network: the three networks of a minibatch step share the 132 SMs in one wave
 int osb_update_grid_blocks(int mb_count) {
     int tiles = (mb_count + UT - 1) / UT;
-    return tiles < 49 ? tiles : 49;
+    const int cap = grid_sms() / 3;
+    return tiles < cap ? tiles : cap;
 }
 
 // One minibatch: fused forward + loss + backward for the networks in `net_mask`.
@@ -905,7 +906,8 @@ int osb_actor_eval(const float* theta_actor, int O, int A, const float* obs, con
     }
     const long long nrows = (total + stride - 1) / stride;
     long long tiles = (nrows + UT - 1) / UT;
-    const int blocks = (int)(tiles < 296 ? tiles : 296);
+    const int cap = 2 * grid_sms();
+    const int blocks = (int)(tiles < cap ? tiles : cap);
     cudaStream_t s = (cudaStream_t)stream;
     actor_eval_kernel<<<blocks, NTHREADS, smem, s>>>(p);
     OSB_LAUNCH_CHECK();
@@ -919,7 +921,8 @@ int osb_actor_eval(const float* theta_actor, int O, int A, const float* obs, con
 int osb_fvp_grid_blocks(long long total, int stride) {
     const long long nrows = (total + stride - 1) / stride;
     const long long tiles = (nrows + UT - 1) / UT;
-    return (int)(tiles < 148 ? tiles : 148);
+    const int cap = grid_sms();
+    return (int)(tiles < cap ? tiles : cap);
 }
 
 // gpart[blocks][P_actor] <- per-CTA partials of F v (without damping); reduce with osb_reduce_partials.

@@ -1,4 +1,4 @@
-// Tensor-core (tcgen05, kind::tf32, TMEM accumulators) variant of the fused minibatch
+// Tensor-core (wgmma, tf32 wgmma, accumulator images) variant of the fused minibatch
 // forward + loss + backward kernel -- the "fast" arithmetic mode of csrc/update.cu (which stays as
 // the exact-fp32 parity path).  Same interface, same per-CTA partial-gradient outputs.
 //
@@ -14,9 +14,9 @@
 //     MMA4  OUT   [s][o] = H2 * W3^T      -> per-sample loss, dOUT
 //     MMA5  dZ2   [s][k] = dOUT * W3      -> * (1 - H2^2)                  (B operand of dZ1^T)
 //     MMA6  dZ2^T [k][s] = W3^T * dOUT^T  -> * (1 - H2^2)                  (A operand of dW2)
-//     MMA7  dW2   [j][k] += dZ2^T * H1    (TMEM accumulator kept across tiles)
+//     MMA7  dW2   [j][k] += dZ2^T * H1    (accumulator images kept across tiles)
 //     MMA8  dZ1^T [k][s] = W2^T * dZ2^T   -> * (1 - H1^2)                  (A operand of dW1)
-//     MMA9  dW1   [j][o] += dZ1^T * X     (TMEM accumulator kept across tiles)
+//     MMA9  dW1   [j][o] += dZ1^T * X     (accumulator images kept across tiles)
 //   dW3, the bias gradients and d log_std stay on the CUDA cores (tiny).
 #include "common.cuh"
 #include "mlp.cuh"
@@ -54,6 +54,7 @@ struct TcArgs {
     float focops_lam, focops_eta;
     const float* focops_mask_mean;   // device scalar mean_i 1{KL_i <= eta} of this minibatch (pass 2) or null (pass 1)
     int forward_only;        // pass 1 of FOCOPS: statistics only, no backward
+    float* acc;              // accumulator images, one [128][TC_COLS] per CTA
 };
 
 __device__ __forceinline__ unsigned long long tc_feistel(unsigned long long k, unsigned long long n, unsigned seed) {
@@ -76,8 +77,8 @@ __device__ __forceinline__ unsigned long long tc_feistel(unsigned long long k, u
     return x;
 }
 
-// TMEM column map
-constexpr uint32_t C_Z = 0, C_ZT = 64, C_ZT2 = 192, C_OUT = 320, C_DW2 = 336, C_DW1 = 400, C_DW3 = 464, TMEM_COLS = 512;
+// accumulator column map (csrc/umma.cuh)
+constexpr uint32_t C_Z = 0, C_ZT = 64, C_ZT2 = 192, C_OUT = 320, C_DW2 = 336, C_DW1 = 400, C_DW3 = 464, TC_COLS = 480;
 constexpr int NTC = 512;   // 16 warps: lane quarter q = warp % 4, column group h = warp / 4 (0..3)
 
 // 16-column variants of the row accessors (c0 % 16 == 0)
@@ -101,7 +102,7 @@ __device__ __forceinline__ void load_row16(uint32_t base, int r, int c0, int R, 
 }
 
 // CHUNKED = obs dim > 64: layer 1 runs as a K loop over 64-column chunks of X / W1 (forward: Z1 and Z1^T
-// accumulate over chunks; backward: one dW1 chunk per MMA, flushed from TMEM into this CTA's partial gradient).
+// accumulate over chunks; backward: one dW1 chunk per MMA, flushed from accumulator image into this CTA's partial gradient).
 // EXT = the two-pass / supplied-dOUT loss kinds (FOCOPS, P3O, FVP); the plain instantiation (PPO-clip, ratio,
 // cost surrogate: the headline path) carries none of their registers or branches.
 template <bool CHUNKED, bool EXT>
@@ -133,7 +134,6 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
     float* sOld = sB3acc + 16;        // old policy: log_std[16], 1 / sigma_old^2 [16]
     long long* sRowBuf = reinterpret_cast<long long*>(sOld + 32);   // [2][128] rows of this / the next tile
     __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_slot;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int q = warp & 3, h = warp >> 2;           // h in [0, 4)
@@ -188,11 +188,8 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
     if (tid < 8) sStat[tid] = 0.f;
     if (tid < 16) sB3acc[tid] = 0.f;
     if (tid == 0) { mbar_init(&bar, 1); mbar_init_fence(); }
-    if (warp == 0) tmem_alloc(&tmem_slot, TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
+    const Acc tm = acc_cta(p.acc, TC_COLS);
     const uint32_t lane_base = (uint32_t)(q * 32) << 16;
     uint32_t phase = 0;
 
@@ -341,45 +338,39 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
                 fence_async_smem();
                 __syncthreads();
                 if (c + 1 < nchunks) load_chunk(sRow, c + 1);      // next chunk's rows fly during the MMAs
-                if (tid == 0) {
-                    tc_fence_after();
-                    tc_gemm(tmem + C_Z, B0, TT, sW1, 64, 128, 64, 64, c > 0);
-                    tc_gemm(tmem + C_ZT, sW1, 64, B0, TT, 64, 128, 64, c > 0);
+                if (warp < 4) {
+                    tc_gemm(tm, C_Z, B0, TT, sW1, 64, 128, 64, 64, c > 0);
+                    tc_gemm(tm, C_ZT, sW1, 64, B0, TT, 64, 128, 64, c > 0);
                     mma_commit(&bar);
                 }
                 mbar_wait(&bar, phase); phase ^= 1;
-                tc_fence_after();
             }
         } else {
-            if (tid == 0) {
-                tc_fence_after();
-                tc_gemm(tmem + C_Z, B0, TT, sW1, 64, 128, 64, 64, false);
-                tc_gemm(tmem + C_ZT, sW1, 64, B0, TT, 64, 128, 64, false);
+            if (warp < 4) {
+                tc_gemm(tm, C_Z, B0, TT, sW1, 64, 128, 64, 64, false);
+                tc_gemm(tm, C_ZT, sW1, 64, B0, TT, 64, 128, 64, false);
                 mma_commit(&bar);
             }
             mbar_wait(&bar, phase); phase ^= 1;
-            tc_fence_after();
         }
         {   // plain epilogue only: H1 is all that layer 2 needs
             float v[16];
-            tmem_ld16(tmem + lane_base + C_Z + c16, v);
+            acc_ld16(tm, lane_base + C_Z + c16, v);
 #pragma unroll
             for (int i = 0; i < 16; ++i) v[i] = tanh_fast(v[i] + sB1[c16 + i]);
             store_row16(B2, s_row, c16, TT, v);
         }
         fence_async_smem();
-        tc_fence_before();
         __syncthreads();
-        // ---- P2: Z2 (-> C_Z) and Z2^T (-> C_ZT2); the H1^T epilogue runs while these MMAs execute ----
-        if (tid == 0) {
-            tc_fence_after();
-            tc_gemm(tmem + C_Z, B2, TT, sW2, 64, 128, 64, 64, false);
-            tc_gemm(tmem + C_ZT2, sW2, 64, B2, TT, 64, 128, 64, false);
+        // ---- P2: Z2 (-> C_Z) and Z2^T (-> C_ZT2); warps 4-15 run the H1^T epilogue while warpgroup 0 computes them ----
+        if (warp < 4) {
+            tc_gemm(tm, C_Z, B2, TT, sW2, 64, 128, 64, 64, false);
+            tc_gemm(tm, C_ZT2, sW2, 64, B2, TT, 64, 128, 64, false);
             mma_commit(&bar);
         }
         {   // deferred: H1^T = tanh(Z1^T + b1) -> B3 (B operand of dW2, needed only in P5)
             float w[32];
-            tmem_ld32(tmem + lane_base + C_ZT + c32, w);
+            acc_ld32(tm, lane_base + C_ZT + c32, w);
             if (lane < 16) {
                 const float bb = sB1[t_row];
 #pragma unroll
@@ -388,26 +379,23 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             }
         }
         mbar_wait(&bar, phase); phase ^= 1;
-        tc_fence_after();
         {
             float v[16];
-            tmem_ld16(tmem + lane_base + C_Z + c16, v);
+            acc_ld16(tm, lane_base + C_Z + c16, v);
 #pragma unroll
             for (int i = 0; i < 16; ++i) v[i] = tanh_fast(v[i] + sB2[c16 + i]);
             store_row16(B0, s_row, c16, TT, v);                  // H2 (X is dead)
         }
         fence_async_smem();
-        tc_fence_before();
         __syncthreads();
         // ---- P3: OUT -> loss -> dOUT (B4, cols 0..31) --------------------------------------------
-        if (tid == 0) {
-            tc_fence_after();
-            tc_gemm(tmem + C_OUT, B0, TT, sW3, 16, 128, 16, 64, false);
+        if (warp < 4) {
+            tc_gemm(tm, C_OUT, B0, TT, sW3, 16, 128, 16, 64, false);
             mma_commit(&bar);
         }
         {   // deferred: H2^T = tanh(Z2^T + b2) -> B2 (H1 is dead: MMA3 / MMA3T completed)
             float w[32];
-            tmem_ld32(tmem + lane_base + C_ZT2 + c32, w);
+            acc_ld32(tm, lane_base + C_ZT2 + c32, w);
             if (lane < 16) {
                 const float bb = sB2[t_row];
 #pragma unroll
@@ -443,14 +431,13 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             }
         }
         mbar_wait(&bar, phase); phase ^= 1;
-        tc_fence_after();
         if (h == 0) {
             float st[5] = {0.f, 0.f, 0.f, 0.f, 0.f};   // loss, ratio, kl, count, focops mask
             float dls[16];
 #pragma unroll
             for (int a = 0; a < 16; ++a) dls[a] = 0.f;
             float o16[16], d32[32];
-            tmem_ld16(tmem + lane_base + C_OUT, o16);
+            acc_ld16(tm, lane_base + C_OUT, o16);
 #pragma unroll
             for (int i = 0; i < 32; ++i) d32[i] = 0.f;
             if (prow >= 0) {
@@ -553,7 +540,6 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             }
         }
         fence_async_smem();
-        tc_fence_before();
         __syncthreads();
         if (tid < 5) sStat[tid] += sRed[tid] + sRed[8 + tid] + sRed[16 + tid] + sRed[24 + tid];
         if (net == 0 && tid >= 32 && tid < 48) {
@@ -573,18 +559,16 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             continue;
         }
         // ---- P4: dZ2, dZ2^T and dW3^T += H2^T dOUT ------------------------------------------------
-        if (tid == 0) {
-            tc_fence_after();
-            tc_gemm(tmem + C_Z, B4, TT, sW3T, 64, 128, 64, 16, false);
-            tc_gemm(tmem + C_ZT, sW3T, 64, B4, TT, 64, 128, 16, false);
-            tc_gemm(tmem + C_DW3, B2, 64, B4 + 16384u, 16, 64, 16, 128, !first_tile);
+        if (warp < 4) {
+            tc_gemm(tm, C_Z, B4, TT, sW3T, 64, 128, 64, 16, false);
+            tc_gemm(tm, C_ZT, sW3T, 64, B4, TT, 64, 128, 16, false);
+            tc_gemm(tm, C_DW3, B2, 64, B4 + 16384u, 16, 64, 16, 128, !first_tile);
             mma_commit(&bar);
         }
         mbar_wait(&bar, phase); phase ^= 1;
-        tc_fence_after();
         {
             float w[32], hh[32];
-            tmem_ld32(tmem + lane_base + C_ZT + c32, w);
+            acc_ld32(tm, lane_base + C_ZT + c32, w);
             if (lane < 16) {
                 load_row32(B2, t_row, c32, 64, hh);              // H2^T
 #pragma unroll
@@ -595,22 +579,20 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
         __syncthreads();           // every read of H2^T (B2) is done before dZ2 overwrites it
         {
             float v[16], hh[16];
-            tmem_ld16(tmem + lane_base + C_Z + c16, v);
+            acc_ld16(tm, lane_base + C_Z + c16, v);
             load_row16(B0, s_row, c16, TT, hh);
 #pragma unroll
             for (int i = 0; i < 16; ++i) v[i] *= (1.f - hh[i] * hh[i]);
             store_row16(B2, s_row, c16, TT, v);                  // dZ2 [s][k]
         }
         fence_async_smem();
-        tc_fence_before();
         __syncthreads();
         // ---- P5: dW2 += dZ2^T H1 ; dZ1^T = W2^T dZ2^T --------------------------------------------
         if (CHUNKED) load_chunk(sRow, 0);             // chunk 0 of THIS tile again: P6 needs X^T chunk by chunk
         else if (vec && has_next) prefetch_x(sRowNext);    // global loads of the next tile fly during P5 / P6
-        if (tid == 0) {
-            tc_fence_after();
-            tc_gemm(tmem + C_DW2, B4, 64, B3, 64, 64, 64, 128, !first_tile);
-            tc_gemm(tmem + C_ZT, sW2T, 64, B2, TT, 64, 128, 64, false);
+        if (warp < 4) {
+            tc_gemm(tm, C_DW2, B4, 64, B3, 64, 64, 64, 128, !first_tile);
+            tc_gemm(tm, C_ZT, sW2T, 64, B2, TT, 64, 128, 64, false);
             mma_commit(&bar);
         }
         if (tid < 64) {   // db2[j] = sum_s dZ2^T[j][s]
@@ -624,10 +606,9 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             ab2 += c;
         }
         mbar_wait(&bar, phase); phase ^= 1;
-        tc_fence_after();
         {
             float w[32], hh[32];
-            tmem_ld32(tmem + lane_base + C_ZT + c32, w);
+            acc_ld32(tm, lane_base + C_ZT + c32, w);
             if (lane < 16) {
                 load_row32(B3, t_row, c32, 64, hh);
 #pragma unroll
@@ -636,19 +617,16 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             }
         }
         fence_async_smem();
-        tc_fence_before();
         __syncthreads();
         // ---- P6: dW1 += dZ1^T X --------------------------------------------------------------------
         if (CHUNKED) {
             for (int c = 0; c < nchunks; ++c) {
                 store_chunk(B1, true);               // X^T chunk [64 k][128 s]
                 fence_async_smem();
-                tc_fence_before();                   // (c > 0) every read of the previous chunk's accumulator is done
-                __syncthreads();
+                __syncthreads();                     // (c > 0) every read of the previous chunk's accumulator is done
                 if (c + 1 < nchunks) load_chunk(sRow, c + 1);
-                if (tid == 0) {
-                    tc_fence_after();
-                    tc_gemm(tmem + C_DW1, B0, 64, B1, 64, 64, 64, 128, false);
+                if (warp < 4) {
+                    tc_gemm(tm, C_DW1, B0, 64, B1, 64, 64, 64, 128, false);
                     mma_commit(&bar);
                 }
                 if (c == 0 && tid < 64) {   // db1[j] = sum_s dZ1^T[j][s]
@@ -662,10 +640,9 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
                     ab1 += cs;
                 }
                 mbar_wait(&bar, phase); phase ^= 1;
-                tc_fence_after();
                 {   // flush this chunk of dW1 into the CTA's partial gradient (each element owned by one thread)
                     float v[16];
-                    tmem_ld16(tmem + lane_base + C_DW1 + c16, v);
+                    acc_ld16(tm, lane_base + C_DW1 + c16, v);
                     if (lane < 16) {
                         float* qrow = gout + L.off_w1 + t_row * O + c * 64 + c16;
                         const int nvalid = O - (c * 64 + c16);          // columns of this 16-group inside [0, O)
@@ -684,9 +661,8 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             }
             if (has_next) load_chunk(sRowNext, 0);
         } else {
-        if (tid == 0) {
-            tc_fence_after();
-            tc_gemm(tmem + C_DW1, B0, 64, B1, 64, 64, 64, 128, !first_tile);
+        if (warp < 4) {
+            tc_gemm(tm, C_DW1, B0, 64, B1, 64, 64, 64, 128, !first_tile);
             mma_commit(&bar);
         }
         if (tid < 64) {   // db1[j] = sum_s dZ1^T[j][s]
@@ -700,7 +676,6 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             ab1 += c;
         }
         mbar_wait(&bar, phase); phase ^= 1;      // B0 / B1 are rewritten by the next tile's gather
-        tc_fence_after();
         }
         first_tile = false;
         rpar ^= 1;
@@ -713,18 +688,18 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
     } else {
         float v[16];
         float* stage = reinterpret_cast<float*>(smem_raw + pad);            // B0 region: [2][64][65]
-        tmem_ld16(tmem + lane_base + C_DW2 + c16, v);
+        acc_ld16(tm, lane_base + C_DW2 + c16, v);
         if (lane < 16)
 #pragma unroll
             for (int i = 0; i < 16; ++i) stage[t_row * 65 + c16 + i] = v[i];
         if (!CHUNKED) {
-            tmem_ld16(tmem + lane_base + C_DW1 + c16, v);
+            acc_ld16(tm, lane_base + C_DW1 + c16, v);
             if (lane < 16)
 #pragma unroll
                 for (int i = 0; i < 16; ++i) stage[64 * 65 + t_row * 65 + c16 + i] = v[i];
         }
         if (h == 0) {   // dW3^T [k][o] accumulator (M = 64 layout)
-            tmem_ld16(tmem + lane_base + C_DW3, v);
+            acc_ld16(tm, lane_base + C_DW3, v);
             if (lane < 16)
 #pragma unroll
                 for (int o = 0; o < 16; ++o) stage[2 * 64 * 65 + o * 65 + t_row] = v[o];
@@ -745,9 +720,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
         }
         if (tid < 8) p.stats_part[((size_t)blockIdx.x * 3 + net) * 8 + tid] = sStat[tid];
     }
-    tc_fence_before();
     __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, TMEM_COLS);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -762,8 +735,9 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
 struct FvpTanArgs {
     const float* obs; long long total; int stride;
     const float* theta; const float* vec; float* dmu; int O, A;
+    float* acc;              // accumulator images, one [128][F_COLS] per CTA
 };
-constexpr uint32_t F_Z1 = 0, F_Z2 = 128, F_DMU = 256;
+constexpr uint32_t F_Z1 = 0, F_Z2 = 128, F_DMU = 256, F_COLS = 272;
 
 template <bool CHUNKED>     // obs dim > 64: K loop over 64-column chunks of X / [W1;V1]
 __global__ void __launch_bounds__(NTC, 1) fvp_tangent_tc_kernel(FvpTanArgs p) {
@@ -782,7 +756,6 @@ __global__ void __launch_bounds__(NTC, 1) fvp_tangent_tc_kernel(FvpTanArgs p) {
     float* sVB3 = sVB2 + 64;           // [16]
     long long* sRowBuf = reinterpret_cast<long long*>(sVB3 + 16);   // [2][128]
     __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_slot;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int q = warp & 3, h = warp >> 2;
@@ -829,11 +802,8 @@ __global__ void __launch_bounds__(NTC, 1) fvp_tangent_tc_kernel(FvpTanArgs p) {
     }
     if (tid < 16) sVB3[tid] = (tid < A) ? __ldg(p.vec + L.off_b3 + tid) : 0.f;
     if (tid == 0) { mbar_init(&bar, 1); mbar_init_fence(); }
-    if (warp == 0) tmem_alloc(&tmem_slot, TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
+    const Acc tm = acc_cta(p.acc, F_COLS);
     const uint32_t lane_base = (uint32_t)(q * 32) << 16;
     uint32_t phase = 0;
     const int s_row = 32 * q + lane, c16 = 16 * h;
@@ -950,28 +920,24 @@ __global__ void __launch_bounds__(NTC, 1) fvp_tangent_tc_kernel(FvpTanArgs p) {
                 __syncthreads();
                 if (c + 1 < nchunks) load_chunk(sRow, c + 1);
                 else if (has_next) load_chunk(sRowNext, 0);
-                if (tid == 0) {
-                    tc_fence_after();
-                    tc_gemm(tmem + F_Z1, B0, TT, sWV1, 128, 128, 128, 64, c > 0);
+                if (warp < 4) {
+                    tc_gemm(tm, F_Z1, B0, TT, sWV1, 128, 128, 128, 64, c > 0);
                     mma_commit(&bar);
                 }
                 mbar_wait(&bar, phase); phase ^= 1;
-                tc_fence_after();
             }
         } else {
             if (vec4 && has_next) prefetch_x(sRowNext);      // next tile's rows fly during the three layers
-            if (tid == 0) {
-                tc_fence_after();
-                tc_gemm(tmem + F_Z1, B0, TT, sWV1, 128, 128, 128, 64, false);
+            if (warp < 4) {
+                tc_gemm(tm, F_Z1, B0, TT, sWV1, 128, 128, 128, 64, false);
                 mma_commit(&bar);
             }
             mbar_wait(&bar, phase); phase ^= 1;
-            tc_fence_after();
         }
         {
             float z[16], dz[16];
-            tmem_ld16(tmem + lane_base + F_Z1 + c16, z);
-            tmem_ld16(tmem + lane_base + F_Z1 + 64 + c16, dz);
+            acc_ld16(tm, lane_base + F_Z1 + c16, z);
+            acc_ld16(tm, lane_base + F_Z1 + 64 + c16, dz);
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
                 const float hh = tanh_fast(z[i] + sB1[c16 + i]);
@@ -982,21 +948,18 @@ __global__ void __launch_bounds__(NTC, 1) fvp_tangent_tc_kernel(FvpTanArgs p) {
             store_row16(B2, s_row, c16, TT, dz);     // dH1
         }
         fence_async_smem();
-        tc_fence_before();
         __syncthreads();
         // ---- layer 2: [Z2 | H1 V2^T + dH1 W2^T] ------------------------------------------------------
-        if (tid == 0) {
-            tc_fence_after();
-            tc_gemm(tmem + F_Z2, B1, TT, sWV2, 128, 128, 128, 64, false);
-            tc_gemm(tmem + F_Z2 + 64, B2, TT, sWV2, 128, 128, 64, 64, true);
+        if (warp < 4) {
+            tc_gemm(tm, F_Z2, B1, TT, sWV2, 128, 128, 128, 64, false);
+            tc_gemm(tm, F_Z2 + 64, B2, TT, sWV2, 128, 128, 64, 64, true);
             mma_commit(&bar);
         }
         mbar_wait(&bar, phase); phase ^= 1;
-        tc_fence_after();
         {
             float z[16], dz[16];
-            tmem_ld16(tmem + lane_base + F_Z2 + c16, z);
-            tmem_ld16(tmem + lane_base + F_Z2 + 64 + c16, dz);
+            acc_ld16(tm, lane_base + F_Z2 + c16, z);
+            acc_ld16(tm, lane_base + F_Z2 + 64 + c16, dz);
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
                 const float hh = tanh_fast(z[i] + sB2[c16 + i]);
@@ -1007,20 +970,17 @@ __global__ void __launch_bounds__(NTC, 1) fvp_tangent_tc_kernel(FvpTanArgs p) {
             store_row16(B1, s_row, c16, TT, dz);     // dH2 (H1 is dead: layer-2 MMAs completed)
         }
         fence_async_smem();
-        tc_fence_before();
         __syncthreads();
         // ---- output tangent: dmu = H2 V3^T + dH2 W3^T + vb3 -------------------------------------------
-        if (tid == 0) {
-            tc_fence_after();
-            tc_gemm(tmem + F_DMU, B0, TT, sWV3 + 2048u, 32, 128, 16, 64, false);
-            tc_gemm(tmem + F_DMU, B1, TT, sWV3, 32, 128, 16, 64, true);
+        if (warp < 4) {
+            tc_gemm(tm, F_DMU, B0, TT, sWV3 + 2048u, 32, 128, 16, 64, false);
+            tc_gemm(tm, F_DMU, B1, TT, sWV3, 32, 128, 16, 64, true);
             mma_commit(&bar);
         }
         mbar_wait(&bar, phase); phase ^= 1;
-        tc_fence_after();
         if (h == 0) {
             float o16[16];
-            tmem_ld16(tmem + lane_base + F_DMU, o16);
+            acc_ld16(tm, lane_base + F_DMU, o16);
             const long long row = sRow[s_row];
             if (row >= 0) {
 #pragma unroll
@@ -1028,13 +988,10 @@ __global__ void __launch_bounds__(NTC, 1) fvp_tangent_tc_kernel(FvpTanArgs p) {
                     if (a < A) p.dmu[row * A + a] = o16[a] + sVB3[a];
             }
         }
-        tc_fence_before();
         rpar ^= 1;
         __syncthreads();
     }
-    tc_fence_before();
     __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, TMEM_COLS);
 }
 
 }  // namespace osb
@@ -1048,7 +1005,7 @@ static size_t fvp_tan_smem_bytes() {
     return 1024 + 3 * (size_t)BUF + 2 * 32768 + 8192 + (4 * 64 + 16) * 4 + 2 * 128 * 8 + 64;
 }
 
-static int launch_grad_tc(const TcArgs& p, int nblocks, cudaStream_t stream) {
+static int launch_grad_tc(TcArgs& p, int nblocks, cudaStream_t stream) {
     const size_t smem = tc_smem_bytes();
     static bool attr = false;
     if (!attr) {
@@ -1060,6 +1017,8 @@ static int launch_grad_tc(const TcArgs& p, int nblocks, cudaStream_t stream) {
     }
     const bool single = (p.net_mask & (p.net_mask - 1)) == 0;     // one network: it gets every CTA
     dim3 grid(nblocks, single ? 1 : 3);
+    p.acc = acc_scratch(ACC_UPDATE_TC, (size_t)grid.x * grid.y * 128 * TC_COLS * sizeof(float));
+    if (!p.acc) return OSB_ERR_CUDA;
     const bool ext = p.kind == TC_FOCOPS || p.kind == TC_FVP || p.kind == TC_P3O;
     if (p.O > 64) {
         if (ext) minibatch_grad_tc_kernel<true, true><<<grid, NTC, smem, stream>>>(p);
@@ -1076,11 +1035,11 @@ extern "C" {
 
 int osb_update_grid_blocks(int mb_count);
 
-// CTAs along x of the tensor-core kernel: three networks share the 148 SMs (49 each); a single
+// CTAs along x of the tensor-core kernel: three networks share the SMs (a third each); a single
 // network (full-batch actor passes of the natural-gradient family) spreads over all of them.
 int osb_tc_grid_blocks(long long rows, int net_mask) {
     const long long tiles = (rows + TT - 1) / TT;
-    const int cap = ((net_mask & (net_mask - 1)) == 0) ? 148 : 49;
+    const int cap = ((net_mask & (net_mask - 1)) == 0) ? grid_sms() : grid_sms() / 3;
     return (int)(tiles < cap ? tiles : cap);
 }
 
@@ -1096,7 +1055,7 @@ __global__ void tc_mask_mean_kernel(const float* __restrict__ stats_part, int nb
     out[0] = (kind == TC_P3O) ? ((mean + jc_minus_limit > 0.f) ? kappa : 0.f) : mean;
 }
 
-// Tensor-core (TF32 tcgen05) variant of osb_minibatch_grad: same arguments, O <= 64, A <= 16.
+// Tensor-core (TF32 wgmma) variant of osb_minibatch_grad: same arguments, O <= 64, A <= 16.
 // gpart holds osb_tc_grid_blocks(mb_count, net_mask) rows of P floats.
 int osb_minibatch_grad_tc(const float* theta, int O, int A, const float* obs, const float* act,
                           const float* logp, const float* adv_r, const float* adv_c,
@@ -1151,7 +1110,9 @@ int osb_fvp_partials_tc(const float* theta_actor, const float* vec, int O, int A
     const int nb = osb_tc_grid_blocks(nrows, 1);
     cudaStream_t s = (cudaStream_t)stream;
     {
-        FvpTanArgs t{obs, total, stride, theta_actor, vec, dmu, O, A};
+        FvpTanArgs t{obs, total, stride, theta_actor, vec, dmu, O, A, nullptr};
+        t.acc = acc_scratch(ACC_FVP_TC, (size_t)nb * 128 * F_COLS * sizeof(float));
+        if (!t.acc) return OSB_ERR_CUDA;
         const size_t smem = fvp_tan_smem_bytes();
         static bool attr = false;
         if (!attr) {

@@ -1,8 +1,8 @@
 // Parity-grade tensor-core variant of the fused minibatch forward + loss + backward kernel
 // (PolicyGradient._update, algorithms/on_policy/base/policy_gradient.py:L345-524; PPO._loss_pi base/ppo.py:L35-87;
 // PPOLag._compute_adv_surrogate naive_lagrange/ppo_lag.py:L82-102): split-bf16 arithmetic (csrc/x3.cuh), i.e.
-// every GEMM is six tcgen05 kind::f16 MMAs over the three bf16 pieces of its fp32 operands with fp32
-// accumulation in TMEM -- fp32-level results on the tensor cores (the reference computes fp32 Linear layers,
+// every GEMM is six bf16 wgmma MMAs over the three bf16 pieces of its fp32 operands with fp32
+// accumulation in the accumulator image -- fp32-level results on the tensor cores (the reference computes fp32 Linear layers,
 // omnisafe/utils/model.py:L105-111).
 //
 // One CTA = one network x a strided set of 128-sample tiles (same grid / per-CTA partial-gradient contract as
@@ -77,11 +77,12 @@ struct X3Args {
     const float* fvp_vec;        // X3_FVP: direction v (its log_std block gives the log_std block of F v)
     float fvp_scale;             // X3_FVP: 1 / (rows * A)
     long long* dbg;              // optional clock64 stamps of CTA (0, 0): [0] = count, then (id, clock) pairs (tools/x3_stage_times.py)
+    float* acc;                  // accumulator images, one [128][T_COLS] per CTA
 };
 
 constexpr int XT = 128;                      // samples per tile
 constexpr int NEPI = 512;                    // 16 epilogue warps: lane quarter q = warp % 4, column group h = warp / 4
-constexpr int NTX3 = NEPI + 32;              // + the MMA-issue warp
+constexpr int NTX3 = NEPI + 128;             // + the MMA-issue warpgroup (warps 16..19)
 constexpr uint32_t ACT_SUB = XT * 128, ACT_X3 = 3 * ACT_SUB;        // [128][64] bf16 sub-tile, x3 tile
 constexpr uint32_t D_SUB = XT * 32, D_X3 = 3 * D_SUB;               // [128][16] bf16 (SW32)
 constexpr uint32_t W_SUB = 64 * 128, W_X3 = 3 * W_SUB;              // [64][64]
@@ -97,12 +98,11 @@ constexpr uint32_t OFF_ROWS = OFF_MISC + MF_END * 4;                 // long lon
 constexpr uint32_t OFF_BARS = OFF_ROWS + 2 * XT * 8;                 // uint64 [NBAR]
 enum Bar { RDY_X0 = 0, RDY_X1, RDY_H1_0, RDY_H1_1, RDY_H2_0, RDY_H2_1, RDY_D, RDY_DZ2_0, RDY_DZ2_1, RDY_DZ1,
            DONE_C1, DONE_C2, DONE_C3, DONE_C4A, DONE_C4B, DONE_C5A, DONE_C5B, DONE_C6, RDY_W, NBAR };
-constexpr uint32_t OFF_TMEMSLOT = OFF_BARS + NBAR * 8;
-constexpr uint32_t OFF_PF = OFF_TMEMSLOT + 16;                        // float [128][12]: per-sample loss inputs (AP == 8), copied asynchronously
+constexpr uint32_t OFF_PF = OFF_BARS + NBAR * 8 + 16;                       // float [128][12]: per-sample loss inputs (AP == 8), copied asynchronously
 constexpr int PF_LD = 12;
 constexpr uint32_t X3_SMEM = OFF_PF + XT * PF_LD * 4;
-// TMEM columns
-constexpr uint32_t T_ZA = 0, T_ZB = 64, T_OUT = 128, T_DW1 = 144, T_DW2 = 208, T_DW3 = 272, T_DB1 = 288, T_DB2 = 304, T_COLS = 512;
+// accumulator columns
+constexpr uint32_t T_ZA = 0, T_ZB = 64, T_OUT = 128, T_DW1 = 144, T_DW2 = 208, T_DW3 = 272, T_DB1 = 288, T_DB2 = 304, T_COLS = 320;
 
 __device__ __forceinline__ unsigned long long x3_feistel(unsigned long long k, unsigned long long n, unsigned seed) {
     int bits = 2;
@@ -204,8 +204,7 @@ constexpr int PSTR = 9472;          // FUSED: row stride of the private partial-
 //   distributed.py:L193-198), apply torch-Adam and re-stage the new weights: no relaunch, no separate
 //   optimiser kernel.
 // AP = padded action width of the loss epilogue (8 or 16).
-// (17 warps: registers are allocated per 4 warps, so a 544-thread block is sized like 640 threads: 96 registers each;
-//  __maxnreg__(120) compiles but cannot launch)
+// (20 warps = 640 threads: 96 registers each, the register file divided in units of 8 per thread)
 template <bool FUSED, int AP>
 __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
     if (p.stop_flag && *p.stop_flag) return;
@@ -219,7 +218,6 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
     float* misc = reinterpret_cast<float*>(gbase + OFF_MISC);
     long long* sRowBuf = reinterpret_cast<long long*>(gbase + OFF_ROWS);
     const uint32_t bars = sbase + OFF_BARS;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(gbase + OFF_TMEMSLOT);
     auto bar = [&](int i) { return bars + (uint32_t)i * 8u; };
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -231,7 +229,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
     // partial gradients of this CTA: FUSED -> private aligned layout, else the [CTA][P] layout optim_fused reads
     float* gout = FUSED ? p.gpart + ((size_t)((gridDim.y == 1 ? 0 : net) * G + (int)blockIdx.x)) * PSTR
                         : p.gpart + (size_t)blockIdx.x * p.P + noff;
-    const bool is_mma_warp = warp == NEPI / 32;
+    const bool is_mma_warp = warp >= NEPI / 32;        // the four warps of the MMA-issue warpgroup
     const int batch = FUSED ? p.batch_size : p.b.mb_count;
     const int n_mb = (p.b.mb_count + batch - 1) / batch;
     const bool ones_col = O < 64;          // bias of layer 1 / db1 ride in the GEMMs (see stage_weights_x3)
@@ -246,25 +244,20 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
             misc[MF_OLD + tid] = lo; misc[MF_OLD + 16 + tid] = 1.f / (so * so);
         }
     } else {
-        if (lane == 0) {
+        if (tid == NEPI) {
             for (int i = 0; i < NBAR; ++i) {
                 const uint32_t cnt = (i >= DONE_C1) ? 1u : (i == RDY_D ? 4u : 16u);      // (RDY_W: one expect_tx arrival)
                 asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar(i)), "r"(cnt) : "memory");
             }
             mbar_init_fence();
         }
-        __syncwarp();
-        tmem_alloc(tmem_slot, T_COLS);
     }
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
+    const Acc tm = acc_cta(p.acc, T_COLS);
 
     if (is_mma_warp) {
-        // ======================= MMA-issue warp: uniform control flow, one elected lane issues ==============
-        const bool leader = elect_one_sync();
+        // ======================= MMA-issue warpgroup: uniform control flow ====================================
         const uint64_t dX = desc128(sbase + OFF_X), dH1 = desc128(sbase + OFF_H1), dH2 = desc128(sbase + OFF_H2);
         const uint64_t dD = desc32(sbase + OFF_D), dW1 = desc128(sbase + OFF_W1), dW2 = desc128(sbase + OFF_W2);
         const uint64_t dW3 = desc128(sbase + OFF_W3), dOnes = desc32(sbase + OFF_ONES);
@@ -284,62 +277,48 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll 1
                 for (int ph = 0; ph < 2; ++ph) {
                     mbar_wait_a(bar(RDY_X0 + ph), par);
-                    tc_fence_after();
-                    gemm_x3_warp(leader, tmem + T_ZA, desc_add(dX, 64u * ph), ACT_SUB, 32u, desc_add(dW1, 64u * ph), W_SUB, 32u, id_fwd, 2, ph > 0);
+                    gemm_x3(tm, T_ZA, desc_add(dX, 64u * ph), ACT_SUB, 32u, desc_add(dW1, 64u * ph), W_SUB, 32u, id_fwd, 2, ph > 0);
                 }
-                if (leader) mma_commit_a(bar(DONE_C1));
-                __syncwarp();
+                mma_commit_a(bar(DONE_C1));
                 // db2 of the PREVIOUS tile (dZ2 still sits in the H2 buffer until this tile's E2): runs under E1,
                 // completes before Z2 (in-order pipe), so DONE_C2 covers it
-                if (!first && !(!FUSED && p.forward_only)) gemm_x3_warp(leader, tmem + T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, id_dw16, 8, tile != (int)blockIdx.x + G);
+                if (!first && !(!FUSED && p.forward_only)) gemm_x3(tm, T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, id_dw16, 8, tile != (int)blockIdx.x + G);
                 // Z2 = H1 W2^T
 #pragma unroll 1
                 for (int ph = 0; ph < 2; ++ph) {
                     mbar_wait_a(bar(RDY_H1_0 + ph), par);
-                    tc_fence_after();
-                    gemm_x3_warp(leader, tmem + T_ZB, desc_add(dH1, 64u * ph), ACT_SUB, 32u, desc_add(dW2, 64u * ph), W_SUB, 32u, id_fwd, 2, ph > 0);
+                    gemm_x3(tm, T_ZB, desc_add(dH1, 64u * ph), ACT_SUB, 32u, desc_add(dW2, 64u * ph), W_SUB, 32u, id_fwd, 2, ph > 0);
                 }
-                if (leader) mma_commit_a(bar(DONE_C2));
-                __syncwarp();
+                mma_commit_a(bar(DONE_C2));
                 // OUT = H2 W3^T
 #pragma unroll 1
                 for (int ph = 0; ph < 2; ++ph) {
                     mbar_wait_a(bar(RDY_H2_0 + ph), par);
-                    tc_fence_after();
-                    gemm_x3_warp(leader, tmem + T_OUT, desc_add(dH2, 64u * ph), ACT_SUB, 32u, desc_add(dW3, 64u * ph), W3_SUB, 32u, id_out, 2, ph > 0);
+                    gemm_x3(tm, T_OUT, desc_add(dH2, 64u * ph), ACT_SUB, 32u, desc_add(dW3, 64u * ph), W3_SUB, 32u, id_out, 2, ph > 0);
                 }
-                if (leader) mma_commit_a(bar(DONE_C3));
-                __syncwarp();
+                mma_commit_a(bar(DONE_C3));
                 if (!FUSED && p.forward_only) continue;              // statistics pass (FOCOPS mask mean): no backward
                 // dZ2' = dOUT W3 ; dW3^T += H2^T dOUT
                 mbar_wait_a(bar(RDY_D), par);
-                tc_fence_after();
-                gemm_x3_warp(leader, tmem + T_ZA, dD, D_SUB, 32u, dW3, W3_SUB, 2048u, id_bwd, 1, false);
-                if (leader) mma_commit_a(bar(DONE_C4A));
-                __syncwarp();
-                gemm_x3_warp(leader, tmem + T_DW3, dH2, ACT_SUB, 2048u, dD, D_SUB, 512u, id_dw16, 8, !first);
-                if (leader) mma_commit_a(bar(DONE_C4B));
-                __syncwarp();
+                gemm_x3(tm, T_ZA, dD, D_SUB, 32u, dW3, W3_SUB, 2048u, id_bwd, 1, false);
+                mma_commit_a(bar(DONE_C4A));
+                gemm_x3(tm, T_DW3, dH2, ACT_SUB, 2048u, dD, D_SUB, 512u, id_dw16, 8, !first);
+                mma_commit_a(bar(DONE_C4B));
                 // dZ1' = dZ2 W2 ; dW2 += dZ2^T H1
 #pragma unroll 1
                 for (int ph = 0; ph < 2; ++ph) {
                     mbar_wait_a(bar(RDY_DZ2_0 + ph), par);
-                    tc_fence_after();
-                    gemm_x3_warp(leader, tmem + T_ZB, desc_add(dH2, 64u * ph), ACT_SUB, 32u, desc_add(dW2, 4096u * ph), W_SUB, 2048u, id_bwd, 2, ph > 0);
+                    gemm_x3(tm, T_ZB, desc_add(dH2, 64u * ph), ACT_SUB, 32u, desc_add(dW2, 4096u * ph), W_SUB, 2048u, id_bwd, 2, ph > 0);
                 }
-                if (leader) mma_commit_a(bar(DONE_C5A));
-                __syncwarp();
-                gemm_x3_warp(leader, tmem + T_DW2, dH2, ACT_SUB, 2048u, dH1, ACT_SUB, 2048u, id_dw, 8, !first);
-                if (leader) mma_commit_a(bar(DONE_C5B));
-                __syncwarp();
+                mma_commit_a(bar(DONE_C5A));
+                gemm_x3(tm, T_DW2, dH2, ACT_SUB, 2048u, dH1, ACT_SUB, 2048u, id_dw, 8, !first);
+                mma_commit_a(bar(DONE_C5B));
                 // dW1 += dZ1^T X (column 63 = db1 with the ones column) ; last tile of the minibatch: its own db2
                 mbar_wait_a(bar(RDY_DZ1), par);
-                tc_fence_after();
-                gemm_x3_warp(leader, tmem + T_DW1, dH1, ACT_SUB, 2048u, dX, ACT_SUB, 2048u, id_dw, 8, !first);
-                if (!ones_col) gemm_x3_warp(leader, tmem + T_DB1, dH1, ACT_SUB, 2048u, dOnes, 0u, 0u, id_dw16, 8, !first);
-                if (last) gemm_x3_warp(leader, tmem + T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, id_dw16, 8, !first);
-                if (leader) mma_commit_a(bar(DONE_C6));
-                __syncwarp();
+                gemm_x3(tm, T_DW1, dH1, ACT_SUB, 2048u, dX, ACT_SUB, 2048u, id_dw, 8, !first);
+                if (!ones_col) gemm_x3(tm, T_DB1, dH1, ACT_SUB, 2048u, dOnes, 0u, 0u, id_dw16, 8, !first);
+                if (last) gemm_x3(tm, T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, id_dw16, 8, !first);
+                mma_commit_a(bar(DONE_C6));
             }
         }
     } else {
@@ -380,7 +359,6 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
         };
         auto announce = [&](int b) {        // this warp's stores of one column half are visible to the tensor core
             fence_async_smem();
-            tc_fence_before();
             __syncwarp();
             if (lane == 0) mbar_arrive(bar(b));
         };
@@ -471,7 +449,6 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 if (has_next) tile_rows(mb, tile + G, sRowNext);
                 if (it > 0 && !(!FUSED && p.forward_only)) mbar_wait_a(bar(DONE_C6), par ^ 1u);   // previous tile's dW1 / db1 read X and dZ1
                 stamp(1);
-                tc_fence_after();
 #pragma unroll
                 for (int ph = 0; ph < 2; ++ph) {
                     float v[8];
@@ -517,13 +494,12 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 }
                 // ---- E1: H1 = tanh(Z1 + b1) -------------------------------------------------------------------
                 mbar_wait_a(bar(DONE_C1), par);
-                tc_fence_after();
                 stamp(3);
 #pragma unroll
                 for (int ph = 0; ph < 2; ++ph) {
                     const int c0 = 32 * ph + 8 * h;
                     float v[8];
-                    tmem_ld8(tmem + lane_base + T_ZA + (uint32_t)c0, v);
+                    acc_ld8(tm, lane_base + T_ZA + (uint32_t)c0, v);
 #pragma unroll
                     for (int i = 0; i < 8; ++i) v[i] = tanh_acc(v[i] + sB1[c0 + i]);
                     store8_x3(sbase + OFF_H1, ACT_SUB, s_row, c0, v);
@@ -532,13 +508,12 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 // ---- E2: H2 = tanh(Z2 + b2) -------------------------------------------------------------------
                 stamp(4);
                 mbar_wait_a(bar(DONE_C2), par);
-                tc_fence_after();
                 stamp(5);
 #pragma unroll
                 for (int ph = 0; ph < 2; ++ph) {
                     const int c0 = 32 * ph + 8 * h;
                     float v[8];
-                    tmem_ld8(tmem + lane_base + T_ZB + (uint32_t)c0, v);
+                    acc_ld8(tm, lane_base + T_ZB + (uint32_t)c0, v);
 #pragma unroll
                     for (int i = 0; i < 8; ++i) v[i] = tanh_acc(v[i] + sB2[c0 + i]);
                     store8_x3(sbase + OFF_H2, ACT_SUB, s_row, c0, v);
@@ -562,19 +537,18 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                         }
                     }
                     mbar_wait_a(bar(DONE_C3), par);
-                    tc_fence_after();
                     stamp(7);
                     float o[AP], d16[16];
 #pragma unroll
                     for (int a = 0; a < 16; ++a) d16[a] = 0.f;
                     if (AP == 8) {
                         float t8[8];
-                        tmem_ld8(tmem + lane_base + T_OUT, t8);
+                        acc_ld8(tm, lane_base + T_OUT, t8);
 #pragma unroll
                         for (int a = 0; a < AP; ++a) o[a] = t8[a];
                     } else {
                         float t16[16];
-                        tmem_ld16(tmem + lane_base + T_OUT, t16);
+                        acc_ld16(tm, lane_base + T_OUT, t16);
 #pragma unroll
                         for (int a = 0; a < AP; ++a) o[a] = t16[a];
                     }
@@ -676,21 +650,20 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 stamp(9);
                 if (!FUSED && p.forward_only) {                                      // statistics pass: no backward; H2 is free once OUT is done
                     if (has_next) prefetch_x(sRowNext);
-                    if (h != 0) { mbar_wait_a(bar(DONE_C3), par); tc_fence_after(); }
+                    if (h != 0) { mbar_wait_a(bar(DONE_C3), par); }
                     rpar ^= 1;
                     continue;
                 }
                 // ---- E4: dZ2 = (dOUT W3) (1 - H2^2), stored over H2 once dW3 has read it --------------------------
                 if (has_next) prefetch_x(sRowNext);                        // next tile's rows fly during the backward half
                 mbar_wait_a(bar(DONE_C4A), par);
-                tc_fence_after();
                 stamp(10);
                 float dz[16];
 #pragma unroll
                 for (int ph = 0; ph < 2; ++ph) {
                     const int c0 = 32 * ph + 8 * h;
                     float v[8], hh[8];
-                    tmem_ld8(tmem + lane_base + T_ZA + (uint32_t)c0, v);
+                    acc_ld8(tm, lane_base + T_ZA + (uint32_t)c0, v);
                     load8_x3(sbase + OFF_H2, ACT_SUB, s_row, c0, hh);
 #pragma unroll
                     for (int i = 0; i < 8; ++i) dz[8 * ph + i] = v[i] * (1.f - hh[i] * hh[i]);
@@ -709,13 +682,12 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 // ---- E5: dZ1 = (dZ2 W2) (1 - H1^2), stored over H1 once dW2 has read it --------------------------
                 stamp(13);
                 mbar_wait_a(bar(DONE_C5A), par);
-                tc_fence_after();
                 stamp(14);
 #pragma unroll
                 for (int ph = 0; ph < 2; ++ph) {
                     const int c0 = 32 * ph + 8 * h;
                     float v[8], hh[8];
-                    tmem_ld8(tmem + lane_base + T_ZB + (uint32_t)c0, v);
+                    acc_ld8(tm, lane_base + T_ZB + (uint32_t)c0, v);
                     load8_x3(sbase + OFF_H1, ACT_SUB, s_row, c0, hh);
 #pragma unroll
                     for (int i = 0; i < 8; ++i) dz[8 * ph + i] = v[i] * (1.f - hh[i] * hh[i]);
@@ -745,7 +717,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     prefetch_x(sRowBuf + rpar * XT);
                 }
             }
-            // ---- this CTA's partial gradient of the minibatch: TMEM accumulators -> global ------------------------
+            // ---- this CTA's partial gradient of the minibatch: accumulator images -> global ------------------------
             if (have_tiles) {
                 // loss-warp sums: lanes -> warp (butterfly) -> the four loss warps (fixed order)
                 if (h == 0) {
@@ -773,12 +745,11 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     break;
                 }
                 mbar_wait_a(bar(DONE_C6), (uint32_t)((it - 1) & 1));
-                tc_fence_after();
                 stamp(21);
                 const int t_row = 16 * q + lane;       // row (lane < 16) of the M = 64 accumulators
                 const int c16 = 16 * h;
                 float v[16];
-                tmem_ld16(tmem + lane_base + T_DW2 + (uint32_t)c16, v);
+                acc_ld16(tm, lane_base + T_DW2 + (uint32_t)c16, v);
                 if (lane < 16) {
                     float* dst = gout + L.off_w2 + t_row * 64 + c16;
                     if (FUSED && (L.off_w2 & 3) == 0) {
@@ -789,7 +760,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                         for (int i = 0; i < 16; ++i) __stcg(dst + i, v[i]);
                     }
                 }
-                tmem_ld16(tmem + lane_base + T_DW1 + (uint32_t)c16, v);
+                acc_ld16(tm, lane_base + T_DW1 + (uint32_t)c16, v);
                 if (lane < 16) {
                     float* dst = gout + L.off_w1 + t_row * O + c16;
                     if (FUSED && ((L.off_w1 | O) & 3) == 0) {
@@ -804,21 +775,20 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     if (ones_col && h == 3) __stcg(gout + L.off_b1 + t_row, v[15]);        // column 63 of dW1 = db1
                 }
                 if (h == 0) {      // dW3^T [k][o]
-                    tmem_ld16(tmem + lane_base + T_DW3, v);
+                    acc_ld16(tm, lane_base + T_DW3, v);
                     if (lane < 16)
 #pragma unroll
                         for (int o = 0; o < 16; ++o)
                             if (o < L.out) __stcg(gout + L.off_w3 + o * 64 + t_row, v[o]);
                 } else if (h == 1) {
                     if (!ones_col) {
-                        tmem_ld16(tmem + lane_base + T_DB1, v);
+                        acc_ld16(tm, lane_base + T_DB1, v);
                         if (lane < 16) __stcg(gout + L.off_b1 + t_row, v[0]);
                     }
                 } else if (h == 2) {
-                    tmem_ld16(tmem + lane_base + T_DB2, v);
+                    acc_ld16(tm, lane_base + T_DB2, v);
                     if (lane < 16) __stcg(gout + L.off_b2 + t_row, v[0]);
                 }
-                tc_fence_before();
                 epi_bar_sync();                        // sRed of the four loss warps
                 if (tid < L.out) __stcg(gout + L.off_b3 + tid, (sRed[96 + tid] + sRed[112 + tid]) + (sRed[128 + tid] + sRed[144 + tid]));
                 if (net == 0 && tid >= 32 && tid < 32 + A) {
@@ -1030,9 +1000,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
         }
         if (FUSED && blockIdx.x == 0 && tid == 0) p.adam_step[net] = step_t0 + n_mb;     // every CTA read it before the first barrier
     }
-    tc_fence_before();
     __syncthreads();
-    if (is_mma_warp) tmem_dealloc(tmem, T_COLS);
 }
 
 // mean_i 1{KL_i <= eta} of a minibatch from the forward-only pass (statistic slot 4 / slot 3 of the actor rows)
@@ -1071,6 +1039,12 @@ static int x3_set_attr() {
     return OSB_OK;
 }
 
+// accumulator images for a grid of nb x (up to) 3 CTAs
+static int x3_bind_acc(X3Args& p, int nb) {
+    p.acc = acc_scratch(ACC_UPDATE_X3, (size_t)nb * 3 * 128 * T_COLS * sizeof(float));
+    return p.acc ? OSB_OK : OSB_ERR_CUDA;
+}
+
 // Split-bf16 (parity-grade tensor-core) variant of osb_minibatch_grad: same arguments, O <= 64, A <= 16,
 // loss kinds PPO-clip / ratio / cost surrogate.  gpart holds osb_tc_grid_blocks(mb_count, net_mask) rows of P floats.
 int osb_minibatch_grad_x3(const float* theta, int O, int A, const float* obs, const float* act,
@@ -1097,6 +1071,7 @@ int osb_minibatch_grad_x3(const float* theta, int O, int A, const float* obs, co
     const int nb = osb_tc_grid_blocks(mb_count, net_mask);
     int rc = x3_set_attr();
     if (rc) return rc;
+    if ((rc = x3_bind_acc(p, nb))) return rc;
     const bool single = (net_mask & (net_mask - 1)) == 0;
     if ((loss_kind == X3_FOCOPS || loss_kind == X3_P3O) && (net_mask & 1)) {
         // pass 1: actor forward only -> mean of the KL mask over the minibatch (FOCOPS: the reference's [b,1] x [b] broadcast) or
@@ -1132,6 +1107,7 @@ int osb_x3_fvp_backward(const float* theta_actor, const float* vec, int O, int A
     const int nb = osb_tc_grid_blocks(nrows, 1);
     int rc = x3_set_attr();
     if (rc) return rc;
+    if ((rc = x3_bind_acc(p, nb))) return rc;
     if (A <= 8) minibatch_grad_x3_kernel<false, 8><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(p);
     else minibatch_grad_x3_kernel<false, 16><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(p);
     OSB_LAUNCH_CHECK();
@@ -1190,6 +1166,7 @@ int osb_ppo_update_iter_x3(float* theta, float* grad, float* adam_m, float* adam
     const int nb = osb_tc_grid_blocks(first, net_mask);
     int rc = x3_set_attr();
     if (rc) return rc;
+    if ((rc = x3_bind_acc(p, nb))) return rc;
     const bool single = (net_mask & (net_mask - 1)) == 0;
     void* args[] = {&p};
     osb_count_launch();

@@ -2,9 +2,9 @@
 //
 // Every fp32 operand x is stored as three bf16 tiles x0 + x1 + x2 == x (exactly: x0 = rn_bf16(x),
 // x1 = rn_bf16(x - x0), x2 = x - x0 - x1 which has <= 8 significant bits).  A product A * B is issued as the
-// six kind::f16 MMAs  sum_{i+j<=2} A_i B_j  (the dropped terms are <= 2^-26 relative) with fp32 accumulation
-// in TMEM, small terms first.  Every bf16 x bf16 product is exact in fp32, so the result carries fp32-level
-// accuracy -- unlike kind::tf32 (10-bit mantissa), this mode meets the reference's fp32 Linear layers
+// six bf16 wgmmas  sum_{i+j<=2} A_i B_j  (the dropped terms are <= 2^-26 relative) with fp32 accumulation
+// in registers, small terms first.  Every bf16 x bf16 product is exact in fp32, so the result carries fp32-level
+// accuracy -- unlike tf32 wgmma (10-bit mantissa), this mode meets the reference's fp32 Linear layers
 // (omnisafe/utils/model.py:L105-111) at the tolerance of the exact-FMA path.
 //
 // Unlike tf32, 16-bit operands have an MN-major view under the ordinary 128-byte swizzle, so ONE stored
@@ -12,8 +12,9 @@
 // weight-gradient GEMM (MN-major, contraction over samples): no transposed copies, no role-swapped MMAs.
 //
 // Tile formats (base 1024-byte aligned):
-//   SW128: [R][64] bf16, row pitch 128 B, 16-byte chunk index XOR (row & 7)            (layout type 2)
-//   SW32 : [R][16] bf16, row pitch  32 B, 16-byte chunk index XOR ((row >> 2) & 1)     (layout type 6)
+//   SW128: [R][64] bf16, row pitch 128 B, 16-byte chunk index XOR (row & 7)            (layout code 2)
+//   SW32 : [R][16] bf16, row pitch  32 B, 16-byte chunk index XOR ((row >> 2) & 1)     (layout code 6)
+// (the layout code sits at descriptor bits [61,64); the wgmma layout field is bits [62,64): 1 = SW128, 3 = SW32)
 // An x3 tile is three such sub-tiles back to back (hi, mid, lo), `split` bytes apart.
 #pragma once
 #include "umma.cuh"
@@ -26,7 +27,7 @@ using namespace umma;
 // ---- descriptors ------------------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t desc_make(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
     return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-           ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | (1ull << 46) | ((uint64_t)layout << 61);
+           ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | ((uint64_t)layout << 61);
 }
 // SW128 tile: 8-row groups 1024 B apart, both as K-major (rows = M/N index) and MN-major (rows = K index,
 // one 64-element atom along M/N, so the leading offset is never used).
@@ -37,79 +38,95 @@ __device__ __forceinline__ uint64_t desc32(uint32_t saddr) { return desc_make(sa
 // descriptor + byte offset (start-address field only; all tiles live below 256 KB of shared memory)
 __device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t bytes) { return d + (uint64_t)(bytes >> 4); }
 
-// kind::f16 instruction descriptor, bf16 x bf16 -> fp32
+// GEMM shape word, bf16 x bf16 -> fp32: M (64 or 128), N, and which operands are read MN-major
 __device__ __forceinline__ constexpr uint32_t idesc_bf16(int M, int N, int a_mn, int b_mn) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+    return ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
-// D (+)= A * B over `nk` k-steps of 16, with the six split products (small terms first).
-//   a0 / b0: descriptors of the hi sub-tiles at k-step 0; asplit / bsplit: bytes between sub-tiles;
-//   akstep / bkstep: bytes per k-step (K-major: 32; MN-major: 16 rows * pitch).
-//   bsplit == 0 marks an exactly representable B (e.g. the ones tile): only the three A terms are issued.
-__device__ __forceinline__ void gemm_x3(uint32_t tmem_d, uint64_t a0, uint32_t asplit, uint32_t akstep,
-                                        uint64_t b0, uint32_t bsplit, uint32_t bkstep, uint32_t idesc, int nk,
-                                        bool accumulate) {
-    uint32_t acc = accumulate ? 1u : 0u;
+// One m64 x N block over nk k-steps of 16, six split products per k-step (three when B is exact).
+template <int TA, int TB, int NJ>
+__device__ __forceinline__ void x3_block(float (&d)[4 * NJ], uint64_t a0, uint32_t asplit, uint32_t akstep, uint64_t b0,
+                                         uint32_t bsplit, uint32_t bkstep, int nk) {
+    wg_fence();
+    acc_fence(d);
 #pragma unroll 1
     for (int ks = 0; ks < nk; ++ks) {
         const uint64_t a = desc_add(a0, (uint32_t)ks * akstep), b = desc_add(b0, (uint32_t)ks * bkstep);
         const uint64_t a1 = desc_add(a, asplit), a2 = desc_add(a, 2 * asplit);
-        if (bsplit == 0) {
-            mma_bf16(tmem_d, a2, b, idesc, acc);
-            mma_bf16(tmem_d, a1, b, idesc, 1u);
-            mma_bf16(tmem_d, a, b, idesc, 1u);
+        const uint32_t s = ks > 0 ? 1u : 0u;
+        if constexpr (NJ == 8) {
+            if (bsplit == 0) {
+                wgmma_bf16_n64<TA, TB>(d, a2, b, s);
+                wgmma_bf16_n64<TA, TB>(d, a1, b, 1u);
+                wgmma_bf16_n64<TA, TB>(d, a, b, 1u);
+            } else {
+                const uint64_t b1 = desc_add(b, bsplit), b2 = desc_add(b, 2 * bsplit);
+                wgmma_bf16_n64<TA, TB>(d, a2, b, s);
+                wgmma_bf16_n64<TA, TB>(d, a, b2, 1u);
+                wgmma_bf16_n64<TA, TB>(d, a1, b1, 1u);
+                wgmma_bf16_n64<TA, TB>(d, a1, b, 1u);
+                wgmma_bf16_n64<TA, TB>(d, a, b1, 1u);
+                wgmma_bf16_n64<TA, TB>(d, a, b, 1u);
+            }
         } else {
-            const uint64_t b1 = desc_add(b, bsplit), b2 = desc_add(b, 2 * bsplit);
-            mma_bf16(tmem_d, a2, b, idesc, acc);
-            mma_bf16(tmem_d, a, b2, idesc, 1u);
-            mma_bf16(tmem_d, a1, b1, idesc, 1u);
-            mma_bf16(tmem_d, a1, b, idesc, 1u);
-            mma_bf16(tmem_d, a, b1, idesc, 1u);
-            mma_bf16(tmem_d, a, b, idesc, 1u);
+            if (bsplit == 0) {
+                wgmma_bf16_n16<TA, TB>(d, a2, b, s);
+                wgmma_bf16_n16<TA, TB>(d, a1, b, 1u);
+                wgmma_bf16_n16<TA, TB>(d, a, b, 1u);
+            } else {
+                const uint64_t b1 = desc_add(b, bsplit), b2 = desc_add(b, 2 * bsplit);
+                wgmma_bf16_n16<TA, TB>(d, a2, b, s);
+                wgmma_bf16_n16<TA, TB>(d, a, b2, 1u);
+                wgmma_bf16_n16<TA, TB>(d, a1, b1, 1u);
+                wgmma_bf16_n16<TA, TB>(d, a1, b, 1u);
+                wgmma_bf16_n16<TA, TB>(d, a, b1, 1u);
+                wgmma_bf16_n16<TA, TB>(d, a, b, 1u);
+            }
         }
-        acc = 1u;
+    }
+    wg_commit_wait();
+    acc_fence(d);
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void gemm_x3_t(const Acc& acc, uint32_t d_addr, uint64_t a0, uint32_t asplit, uint32_t akstep,
+                                          uint64_t b0, uint32_t bsplit, uint32_t bkstep, int M, int N, int nk,
+                                          bool accumulate) {
+    // rows 64..127 of a K-major A: 64 rows further down the tile (row pitch 128 B for SW128, 32 B for SW32)
+    const uint32_t a_half_bytes = 64u * (((a0 >> 61) & 7u) == 2u ? 128u : 32u);
+#pragma unroll 1
+    for (int half = 0; half < M / 64; ++half) {
+        const uint64_t ah = desc_add(a0, (uint32_t)half * a_half_bytes);
+        if (N == 16) {
+            float d[8] = {};
+            x3_block<TA, TB, 2>(d, ah, asplit, akstep, b0, bsplit, bkstep, nk);
+            frag_store<2>(acc, d_addr, M, half, d, accumulate);
+        } else {
+#pragma unroll 1
+            for (int nc = 0; nc < N / 64; ++nc) {       // N > 64: K-major SW128 B, 64 rows per block
+                float d[32] = {};
+                x3_block<TA, TB, 8>(d, ah, asplit, akstep, desc_add(b0, (uint32_t)nc * 8192u), bsplit, bkstep, nk);
+                frag_store<8>(acc, d_addr + (uint32_t)(64 * nc), M, half, d, accumulate);
+            }
+        }
     }
 }
 
-
-// Warp-uniform variant for a dedicated MMA-issue warp: all 32 lanes run the descriptor arithmetic (uniform
-// datapath), only the elected lane executes the MMAs.  (Issued from divergent code, every tcgen05.mma is
-// wrapped by the compiler in a uniformisation loop that costs more than the MMA itself.)
-__device__ __forceinline__ void gemm_x3_warp(bool leader, uint32_t tmem_d, uint64_t a0, uint32_t asplit, uint32_t akstep,
-                                             uint64_t b0, uint32_t bsplit, uint32_t bkstep, uint32_t idesc, int nk,
-                                             bool accumulate) {
-    uint32_t acc = accumulate ? 1u : 0u;
-#pragma unroll 1
-    for (int ks = 0; ks < nk; ++ks) {
-        const uint64_t a = desc_add(a0, (uint32_t)ks * akstep), b = desc_add(b0, (uint32_t)ks * bkstep);
-        const uint64_t a1 = desc_add(a, asplit), a2 = desc_add(a, 2 * asplit);
-        const uint64_t b1 = desc_add(b, bsplit), b2 = desc_add(b, 2 * bsplit);
-        if (bsplit == 0) {
-            if (leader) {
-                mma_bf16(tmem_d, a2, b, idesc, acc);
-                mma_bf16(tmem_d, a1, b, idesc, 1u);
-                mma_bf16(tmem_d, a, b, idesc, 1u);
-            }
-        } else {
-            if (leader) {
-                mma_bf16(tmem_d, a2, b, idesc, acc);
-                mma_bf16(tmem_d, a, b2, idesc, 1u);
-                mma_bf16(tmem_d, a1, b1, idesc, 1u);
-                mma_bf16(tmem_d, a1, b, idesc, 1u);
-                mma_bf16(tmem_d, a, b1, idesc, 1u);
-                mma_bf16(tmem_d, a, b, idesc, 1u);
-            }
-        }
-        __syncwarp();
-        acc = 1u;
+// D[acc] (+)= A * B over `nk` k-steps of 16, with the six split products (small terms first); called by all
+// 128 threads of one warpgroup.
+//   a0 / b0: descriptors of the hi sub-tiles at k-step 0; asplit / bsplit: bytes between sub-tiles;
+//   akstep / bkstep: bytes per k-step (K-major: 32; MN-major: 16 rows * pitch); shape: idesc_bf16(M, N, a_mn, b_mn)
+//   (an MN-major A has M = 64; N is 16 or a multiple of 64, and a multiple of 64 above 64 only for a K-major B).
+//   bsplit == 0 marks an exactly representable B (e.g. the ones tile): only the three A terms are issued.
+__device__ __forceinline__ void gemm_x3(const Acc& acc, uint32_t d_addr, uint64_t a0, uint32_t asplit, uint32_t akstep,
+                                        uint64_t b0, uint32_t bsplit, uint32_t bkstep, uint32_t shape, int nk,
+                                        bool accumulate) {
+    const int M = (int)((shape >> 24) & 31u) << 4, N = (int)((shape >> 17) & 63u) << 3;
+    switch ((shape >> 15) & 3u) {
+        case 0: gemm_x3_t<0, 0>(acc, d_addr, a0, asplit, akstep, b0, bsplit, bkstep, M, N, nk, accumulate); break;
+        case 1: gemm_x3_t<1, 0>(acc, d_addr, a0, asplit, akstep, b0, bsplit, bkstep, M, N, nk, accumulate); break;
+        case 2: gemm_x3_t<0, 1>(acc, d_addr, a0, asplit, akstep, b0, bsplit, bkstep, M, N, nk, accumulate); break;
+        default: gemm_x3_t<1, 1>(acc, d_addr, a0, asplit, akstep, b0, bsplit, bkstep, M, N, nk, accumulate); break;
     }
 }
 
@@ -213,24 +230,13 @@ __device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
             : "memory");
     } while (!ok);
 }
+// mma_commit on a 32-bit shared address
 __device__ __forceinline__ void mma_commit_a(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar) : "memory");
+    __threadfence_block();
+    asm volatile("bar.sync 3, 128;\n" ::: "memory");
+    if ((threadIdx.x & 127) == 0) mbar_arrive(bar);
 }
-__device__ __forceinline__ bool elect_one_sync() {
-    uint32_t p;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}\n" : "=r"(p));
-    return p != 0;
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];\n"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
+__device__ __forceinline__ void acc_ld8(const Acc& acc, uint32_t taddr, float (&v)[8]) { acc_ld<8>(acc, taddr, v); }
 // 8 consecutive columns [c0, c0 + 8) (c0 % 8 == 0) of row r of a SW128 x3 tile
 __device__ __forceinline__ void store8_x3(uint32_t base, uint32_t split, int r, int c0, const float (&v)[8]) {
     uint32_t w0[4], w1[4], w2[4];

@@ -1,31 +1,29 @@
-// Self-test and micro-timing of the split-bf16 (kind::f16) tensor-core building blocks of csrc/x3.cuh:
-// pins on real hardware the K-major / MN-major views of one SW128 or SW32 bf16 tile, the 6-product
-// compensation and its accuracy (tests/test_x3_gpu.py), and measures how fast one thread can issue MMAs.
+// Self-test of the split-bf16 tensor-core building blocks of csrc/x3.cuh: pins on real hardware the K-major /
+// MN-major views of one SW128 or SW32 bf16 tile, the 6-product compensation and its accuracy
+// (tests/test_x3_gpu.py).
 #include "common.cuh"
 #include "x3.cuh"
 
 namespace osb {
 
-// A: row-major fp32 [M][K], B: row-major fp32 [N][K].  D[128 lanes][N] raw TMEM dump.
+// A: row-major fp32 [M][K], B: row-major fp32 [N][K].  out[128][N]: dump of accumulator lanes 0..127.
 // a_mn / b_mn: operand consumed MN-major (tile rows = K index) instead of K-major (tile rows = M/N index).
 // a_sw / b_sw: 128 (tile rows of 64 bf16) or 32 (tile rows of 16 bf16).  b_ones: B is the all-ones tile
 // (exact in bf16: three MMAs per k-step).
 __global__ void __launch_bounds__(128, 1) x3_selftest_kernel(const float* __restrict__ A, const float* __restrict__ B,
                                                              int M, int N, int K, int a_mn, int b_mn, int a_sw,
-                                                             int b_sw, int b_ones, int a_lbo, int a_sbo, int b_lbo,
-                                                             int b_sbo, float* __restrict__ out) {
+                                                             int b_sw, int b_ones, float* __restrict__ scratch,
+                                                             float* __restrict__ out) {
     using namespace x3;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_slot;
     const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
     const uint32_t sA = smem_u32(smem_raw) + pad;
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const int rowsA = a_mn ? K : M, colsA = a_mn ? M : K;
     const int rowsB = b_mn ? K : N, colsB = b_mn ? N : K;
     const uint32_t splitA = (uint32_t)((rowsA * a_sw + 1023) & ~1023), splitB = (uint32_t)((rowsB * b_sw + 1023) & ~1023);
-    const uint32_t sB = sA + 3 * splitA + 16384;   // gap: an M = 128 MMA over a 64-row tile reads past it
-    for (uint32_t i = tid; i < (3 * splitA + 16384 + 3 * splitB + 16384) / 4; i += 128)
+    const uint32_t sB = sA + 3 * splitA;
+    for (uint32_t i = tid; i < (3 * splitA + 3 * splitB) / 4; i += 128)
         reinterpret_cast<uint32_t*>(smem_raw + pad)[i] = 0u;
     __syncthreads();
     for (int i = tid; i < rowsA * colsA; i += 128) {
@@ -38,174 +36,35 @@ __global__ void __launch_bounds__(128, 1) x3_selftest_kernel(const float* __rest
         const float v = b_ones ? 1.0f : (b_mn ? B[(size_t)c * K + r] : B[(size_t)r * K + c]);
         store1_x3(sB, splitB, b_sw == 128 ? off128(r, c) : off32(r, c), v);
     }
-    if (tid == 0) { mbar_init(&bar, 1); mbar_init_fence(); }
-    if (warp == 0) tmem_alloc(&tmem_slot, 256);
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
-    if (tid == 0) {
-        // clear all 128 lanes first: M = 128 product with the zeroed gap after A as the A operand
-        const uint64_t a0 = desc_make(sA, (uint32_t)a_lbo, (uint32_t)a_sbo, a_sw == 128 ? 2u : 6u);
-        const uint64_t b0 = desc_make(sB, (uint32_t)b_lbo, (uint32_t)b_sbo, b_sw == 128 ? 2u : 6u);
-        mma_bf16(tmem, desc128(sA + 3 * splitA), b0, idesc_bf16(128, N, 0, b_mn), 0u);
-        gemm_x3(tmem, a0, splitA, a_mn ? 16u * (uint32_t)a_sw : 32u, b0, b_ones ? 0u : splitB,
-                b_mn ? 16u * (uint32_t)b_sw : 32u, idesc_bf16(M, N, a_mn, b_mn), K / 16, true);
-        mma_commit(&bar);
+    const Acc acc = acc_cta(scratch, (uint32_t)N);
+    const uint64_t a0 = a_sw == 128 ? desc128(sA) : desc32(sA), b0 = b_sw == 128 ? desc128(sB) : desc32(sB);
+    gemm_x3(acc, 0u, a0, splitA, a_mn ? 16u * (uint32_t)a_sw : 32u, b0, b_ones ? 0u : splitB,
+            b_mn ? 16u * (uint32_t)b_sw : 32u, idesc_bf16(M, N, a_mn, b_mn), K / 16, false);
+    __threadfence_block();
+    __syncthreads();
+    for (int c0 = 0; c0 < N; c0 += 8) {
+        float v[8];
+        acc_ld8(acc, ((uint32_t)(tid & ~31) << 16) + (uint32_t)c0, v);
+        for (int j = 0; j < 8; ++j) out[(size_t)tid * N + c0 + j] = v[j];
     }
-    mbar_wait(&bar, 0);
-    tc_fence_after();
-    for (int c0 = 0; c0 < N; c0 += 16) {
-        float v[16];
-        tmem_ld16(tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
-        for (int j = 0; j < 16; ++j) out[(size_t)tid * N + c0 + j] = v[j];
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, 256);
-}
-
-__device__ __forceinline__ bool elect_one() {
-    uint32_t p;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}\n" : "=r"(p));
-    return p != 0;
-}
-
-// MMA issue-rate probe.  style 0: `if (tid == 0)` loop (per-thread descriptor arithmetic);
-// style 1: a whole warp runs the loop (uniform descriptor arithmetic), one elected lane issues.
-// out[0] = cycles first issue -> completion, out[1] = cycles of the issue loop.
-__global__ void __launch_bounds__(128, 1) x3_timing_kernel(int M, int N, int reps, int style, long long* out) {
-    using namespace x3;
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_slot;
-    const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
-    const uint32_t sA = smem_u32(smem_raw) + pad, sB = sA + 65536;
-    for (int i = threadIdx.x; i < (65536 + 65536) / 4; i += 128) reinterpret_cast<uint32_t*>(smem_raw + pad)[i] = 0x3F803F80u;
-    if (threadIdx.x == 0) { mbar_init(&bar, 1); mbar_init_fence(); }
-    if (threadIdx.x < 32) tmem_alloc(&tmem_slot, 256);
-    fence_async_smem();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
-    const uint32_t id = idesc_bf16(M, N, 0, 0);
-    long long t0 = 0, t1 = 0, t2 = 0;
-    if (style == 0) {
-        if (threadIdx.x == 0) {
-            t0 = clock64();
-            gemm_x3(tmem, desc128(sA), 16384u, 32u, desc128(sB), 16384u, 32u, id, reps / 6, false);
-            mma_commit(&bar);
-            t1 = clock64();
-        }
-    } else if (threadIdx.x < 32) {
-        const uint64_t a0 = desc128(sA), b0 = desc128(sB);
-        const uint32_t alt = (style == 2) ? 128u : 0u;       // style 2: two accumulators, alternating per MMA
-        const bool leader = elect_one();
-        t0 = clock64();
-#pragma unroll 1
-        for (int r = 0; r < reps; r += 6) {
-            const uint64_t a = desc_add(a0, (uint32_t)((r / 6) & 3) * 32u), b = desc_add(b0, (uint32_t)((r / 6) & 3) * 32u);
-            if (leader) {
-                mma_bf16(tmem, desc_add(a, 32768u), b, id, r > 0);
-                mma_bf16(tmem + alt, a, desc_add(b, 32768u), id, r > 0);
-                mma_bf16(tmem, desc_add(a, 16384u), desc_add(b, 16384u), id, 1u);
-                mma_bf16(tmem + alt, desc_add(a, 16384u), b, id, 1u);
-                mma_bf16(tmem, a, desc_add(b, 16384u), id, 1u);
-                mma_bf16(tmem + alt, a, b, id, 1u);
-            }
-            __syncwarp();
-        }
-        if (leader) mma_commit(&bar);
-        t1 = clock64();
-    }
-    mbar_wait(&bar, 0);
-    if (threadIdx.x == 0) { t2 = clock64(); out[0] = t2 - t0; out[1] = t1 - t0; }
-    tc_fence_before();
-    __syncthreads();
-    if (threadIdx.x < 32) tmem_dealloc(tmem, 256);
-}
-
-// epilogue probe: 16 warps, each reads `cols` columns of its lane quarter `reps` times (tcgen05.ld x16),
-// optionally followed by the accurate tanh + 3-way split + swizzled stores of one activation tile.
-// out[warp] = cycles.
-__global__ void __launch_bounds__(512, 1) x3_epilogue_probe_kernel(int cols, int reps, int mode, long long* out, float* sink) {
-    using namespace x3;
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ uint32_t tmem_slot;
-    const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
-    const uint32_t tile = smem_u32(smem_raw) + pad;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, q = warp & 3, h = warp >> 2;
-    if (warp == 0) tmem_alloc(&tmem_slot, 256);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot + ((uint32_t)(q * 32) << 16);
-    float acc = 0.f;
-    __syncthreads();
-    const long long t0 = clock64();
-    for (int r = 0; r < reps; ++r) {
-        for (int c0 = 16 * h; c0 < cols; c0 += 64) {
-            float v[16];
-            tmem_ld16(tmem + (uint32_t)c0, v);
-            if (mode >= 1) {
-#pragma unroll
-                for (int i = 0; i < 16; ++i) v[i] = tanh_acc(v[i] + 0.125f * (float)i);
-            }
-            if (mode >= 2) store16_x3(tile, 16384u, 32 * q + lane, c0 & 63, v);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) acc += v[i];
-        }
-        if (mode >= 2) { fence_async_smem(); __syncthreads(); }
-    }
-    const long long t1 = clock64();
-    if (lane == 0) out[warp] = t1 - t0;
-    if (acc == 123.456f) sink[tid] = acc;
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_slot, 256);
 }
 
 }  // namespace osb
 
-extern "C" int osb_x3_selftest_dbg(const float* A, const float* B, int M, int N, int K, int a_mn, int b_mn, int a_sw,
-                                   int b_sw, int b_ones, int a_lbo, int a_sbo, int b_lbo, int b_sbo, float* out,
-                                   void* stream) {
-    OSB_CHECK_ARG(A && B && out, "null pointer");
-    OSB_CHECK_ARG((M == 64 || M == 128) && N % 8 == 0 && N >= 8 && N <= 256 && K % 16 == 0 && K >= 16 && K <= 128, "bad shape");
-    OSB_CHECK_ARG((a_sw == 128 || a_sw == 32) && (b_sw == 128 || b_sw == 32), "swizzle must be 128 or 32");
-    OSB_CHECK_ARG((a_mn ? M : K) <= (a_sw == 128 ? 64 : 16) && (b_mn ? N : K) <= (b_sw == 128 ? 64 : 16), "tile wider than one swizzle atom");
-    OSB_CHECK_ARG(M == 128 || a_mn || true, "");
-    const size_t smem = 1024 + 3 * 16384 + 16384 + 3 * 16384 + 16384;
-    OSB_CUDA(cudaFuncSetAttribute(osb::x3_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    osb::x3_selftest_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(A, B, M, N, K, a_mn, b_mn, a_sw, b_sw, b_ones, a_lbo, a_sbo,
-                                                                    b_lbo, b_sbo, out);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
-}
-
-// the production descriptor conventions of csrc/x3.cuh
 extern "C" int osb_x3_selftest(const float* A, const float* B, int M, int N, int K, int a_mn, int b_mn, int a_sw,
                                int b_sw, int b_ones, float* out, void* stream) {
-    return osb_x3_selftest_dbg(A, B, M, N, K, a_mn, b_mn, a_sw, b_sw, b_ones, osb::x3::LBO_DEFAULT, a_sw == 128 ? 1024 : 256,
-                               osb::x3::LBO_DEFAULT, b_sw == 128 ? 1024 : 256, out, stream);
-}
-
-extern "C" int osb_x3_timing(int M, int N, int reps, int style, long long* out, void* stream) {
-    OSB_CHECK_ARG(out && (M == 64 || M == 128) && N % 16 == 0 && N <= 256 && reps > 0 && reps % 6 == 0, "bad argument");
-    const size_t smem = 1024 + 65536 + 65536;
-    OSB_CUDA(cudaFuncSetAttribute(osb::x3_timing_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    osb::x3_timing_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(M, N, reps, style, out);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
-}
-
-extern "C" int osb_x3_epilogue_probe(int cols, int reps, int mode, long long* out, float* sink, void* stream) {
-    OSB_CHECK_ARG(out && sink && cols % 64 == 0 && cols >= 64 && cols <= 256 && reps > 0, "bad argument");
-    const size_t smem = 1024 + 3 * 16384;
-    OSB_CUDA(cudaFuncSetAttribute(osb::x3_epilogue_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    osb::x3_epilogue_probe_kernel<<<1, 512, smem, (cudaStream_t)stream>>>(cols, reps, mode, out, sink);
+    OSB_CHECK_ARG(A && B && out, "null pointer");
+    OSB_CHECK_ARG((M == 64 || M == 128) && (N == 16 || N == 64) && K % 16 == 0 && K >= 16 && K <= 128, "bad shape");
+    OSB_CHECK_ARG((a_sw == 128 || a_sw == 32) && (b_sw == 128 || b_sw == 32), "swizzle must be 128 or 32");
+    OSB_CHECK_ARG((a_mn ? M : K) <= (a_sw == 128 ? 64 : 16) && (b_mn ? N : K) <= (b_sw == 128 ? 64 : 16), "tile wider than one swizzle atom");
+    OSB_CHECK_ARG(!(a_mn && M == 128), "an MN-major A has 64 rows");
+    float* scratch = osb::acc_scratch(osb::ACC_SELFTEST, (size_t)128 * N * sizeof(float));
+    if (!scratch) return OSB_ERR_CUDA;
+    const size_t smem = 1024 + 3 * 16384 + 3 * 16384;
+    OSB_CUDA(cudaFuncSetAttribute(osb::x3_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    osb::x3_selftest_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(A, B, M, N, K, a_mn, b_mn, a_sw, b_sw, b_ones, scratch, out);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
 }

@@ -48,7 +48,7 @@ class ConstraintActorCritic:
         hs_a = list(model_cfgs.actor.hidden_sizes)
         hs_c = list(model_cfgs.critic.hidden_sizes)
         assert hs_a == [HID, HID] and hs_c == [HID, HID], (
-            'the fused sm_100a kernels are specialised for hidden_sizes [64, 64]')
+            'the fused sm_90a kernels are specialised for hidden_sizes [64, 64]')
         assert model_cfgs.actor.activation == 'tanh' and model_cfgs.critic.activation == 'tanh', (
             'the fused kernels implement tanh activations')
         assert model_cfgs.actor_type == 'gaussian_learning'

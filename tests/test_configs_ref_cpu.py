@@ -1,14 +1,14 @@
-"""CPU, build container only: every shipped YAML `defaults` block equals the upstream block of the same
-algorithm key for key (plus the `matmul_precision` extension and the env_cfgs placeholder).  Skipped where
-/root/reference does not exist (GPU box)."""
+"""CPU: every shipped YAML `defaults` block equals the upstream block of the same algorithm key for key (plus the
+`matmul_precision` extension and the env_cfgs placeholder).  The upstream blocks (omnisafe/configs/on-policy/*.yaml,
+flattened to dotted keys) are stored in tests/golden/upstream_config_defaults.json."""
+import json
 import os
 
-import pytest
 import yaml
 
-REF = '/root/reference/omnisafe/configs/on-policy'
-MINE = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'omnisafe_b200', 'configs', 'on-policy')
-pytestmark = pytest.mark.skipif(not os.path.isdir(REF), reason='reference tree not present')
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+UPSTREAM = os.path.join(ROOT, 'tests', 'golden', 'upstream_config_defaults.json')
+MINE = os.path.join(ROOT, 'omnisafe_b200', 'configs', 'on-policy')
 
 
 def _flat(d, pre=''):
@@ -24,14 +24,16 @@ def _flat(d, pre=''):
 def test_yaml_defaults_equal_upstream():
     from omnisafe_b200.algorithms import ALGORITHMS
 
+    with open(UPSTREAM) as fh:
+        upstream = json.load(fh)
     names = sorted(f[:-5] for f in os.listdir(MINE) if f.endswith('.yaml'))
     assert set(names) == set(ALGORITHMS['on-policy'])          # one YAML per registered class
+    assert set(names) == set(upstream)
     for name in names:
-        with open(os.path.join(REF, name + '.yaml')) as fh:
-            ref = _flat(yaml.safe_load(fh)['defaults'])
+        ref = upstream[name]
         with open(os.path.join(MINE, name + '.yaml')) as fh:
             doc = yaml.safe_load(fh)
         mine = _flat(doc['defaults'])
         assert mine.pop('train_cfgs.matmul_precision') == 'fp32', name        # parity arithmetic by default
         assert mine == ref, (name, {k: (ref.get(k), mine.get(k)) for k in set(ref) | set(mine) if ref.get(k) != mine.get(k)})
-        assert 'SyntheticBox-v0' in doc                                           # the B200 workload block
+        assert 'SyntheticBox-v0' in doc                                           # the synthetic workload block

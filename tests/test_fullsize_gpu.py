@@ -67,7 +67,7 @@ def test_update_gradient_is_linear_in_the_batch(cuda, fn_name):
 
 @pytest.mark.timeout(300)
 def test_update_tensor_core_vs_fp32_and_sampled_autograd(cuda):
-    """Full-size minibatch (16 384 rows through the Feistel window): tcgen05 tiles vs fp32 tiles, and the fp32
+    """Full-size minibatch (16 384 rows through the Feistel window): wgmma tiles vs fp32 tiles, and the fp32
     tiles vs autograd of the oracle loss on the same rows."""
     agent, buf, eng = _device_batch(cuda, seed=3)
     B = T * N

@@ -206,7 +206,7 @@ def test_rollout_philox_fast_mode(cuda):
 @pytest.mark.timeout(180)
 @pytest.mark.parametrize('N,T,tmax,term_prob', [(256, 24, 8, 0.0), (200, 20, 6, 0.05)])
 def test_rollout_tensor_core_mode(cuda, N, T, tmax, term_prob):
-    """matmul_precision = tf32 (tcgen05 tiles of 128 envs): same trajectory as the oracle up to the
+    """matmul_precision = tf32 (wgmma tiles of 128 envs): same trajectory as the oracle up to the
     TF32 rounding of the three layer GEMMs (tolerance 5e-3 on values / actions, stated here); the
     env / normaliser / bookkeeping arithmetic is unchanged."""
     from omnisafe_b200.adapter.onpolicy_adapter import OnPolicyAdapter
@@ -245,7 +245,7 @@ def test_rollout_tensor_core_mode(cuda, N, T, tmax, term_prob):
 @pytest.mark.parametrize('N,T,tmax,term_prob,precision', [(256, 24, 8, 0.0, 2), (200, 20, 6, 0.05, 2), (100, 33, 7, 0.02, 2),
                                                           (4096, 128, 64, 0.0, 0), (4096, 128, 64, 0.0, 2)])
 def test_rollout_vs_oracle_bf16x3_and_headline(cuda, N, T, tmax, term_prob, precision):
-    """matmul_precision = bf16x3 (tcgen05 kind::f16, three bf16 pieces per fp32 operand) is held to the bar of the exact
+    """matmul_precision = bf16x3 (bf16 wgmma, three bf16 pieces per fp32 operand) is held to the bar of the exact
     fp32 tiles -- 2e-5 on every slab vs the oracle (the tf32 tiles get 5e-3) -- and both modes are checked at the headline
     size of the bench workload (4096 envs x 128 steps, obs 60 / act 8)."""
     O, A = 60, 8

@@ -1,5 +1,5 @@
-"""Pins the tcgen05 conventions (smem descriptors, 128B swizzle, K-/MN-major views of one tile,
-TMEM lane mapping) with a single-CTA GEMM against numpy."""
+"""Pins the wgmma conventions (smem descriptors, 128B swizzle, K-/MN-major views of one tile,
+accumulator lane mapping) with a single-CTA GEMM against numpy."""
 import numpy as np
 import pytest
 import torch
@@ -12,7 +12,7 @@ def _tf32(x):
     return u.view(np.float32)
 
 
-# K-major operands only: for kind::tf32 an MN-major operand needs the SWIZZLE_128B_BASE32B layout
+# K-major operands only: for tf32 wgmma an MN-major operand needs the SWIZZLE_128B_BASE32B layout
 # (32-byte swizzle base), i.e. it cannot share a physical tile with the K-major view -- which is why
 # the kernels produce transposed activations with role-swapped MMAs instead (csrc/update_tc.cu).
 @pytest.mark.parametrize('M,N,K,a_mn,b_mn', [
@@ -35,6 +35,6 @@ def test_umma_gemm(cuda, M, N, K, a_mn, b_mn):
     if M == 128:
         np.testing.assert_allclose(got, want, rtol=2e-3, atol=2e-3)
     else:
-        # M = 64: report where the 64 rows land in TMEM (lane mapping), then check values
-        rows = [32 * (r // 16) + r % 16 for r in range(64)]   # M = 64: row r -> TMEM lane 32*(r/16) + r%16
+        # M = 64: report where the 64 rows land in the accumulator image (lane mapping), then check values
+        rows = [32 * (r // 16) + r % 16 for r in range(64)]   # M = 64: row r -> accumulator lane 32*(r/16) + r%16
         np.testing.assert_allclose(got[rows], want, rtol=2e-3, atol=2e-3)

@@ -267,7 +267,7 @@ def test_p3o_update_epoch_golden(cuda, golden_dir, precision):
 @pytest.mark.parametrize('tc', [0, 1])
 def test_p3o_gate_vs_autograd(cuda, jc_minus_limit, tc):
     """Both states of the relu gate (inactive: plain PPO-clip gradient; active: + kappa d mean(ratio adv_c)),
-    fp32 tiles and tcgen05 tiles, against autograd of the oracle loss."""
+    fp32 tiles and wgmma tiles, against autograd of the oracle loss."""
     from omnisafe_b200._lib import current_stream, lib, ptr
 
     N, T, O, A = 40, 25, 60, 8

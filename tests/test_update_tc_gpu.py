@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 (TF32) variant of the fused minibatch kernel vs autograd and vs the exact-fp32
+"""GPU: the wgmma (TF32) variant of the fused minibatch kernel vs autograd and vs the exact-fp32
 path.  Tolerance: TF32 keeps 10 mantissa bits, so gradients agree to ~1e-2 of their scale (stated
 here; the fp32 FMA path is the 1e-5 parity path)."""
 import numpy as np
@@ -156,8 +156,8 @@ def test_tc_fvp_vs_fp32_fvp(cuda, O, A, N, T, stride):
 @pytest.mark.timeout(120)
 @pytest.mark.parametrize('loss_kind', [1, 3])
 def test_tc_full_batch_actor_grad(cuda, loss_kind):
-    """actor_loss_grad (natural_pg.py:L150-157) in tensor-core mode -- a single network spread over up to
-    148 CTAs -- vs the exact-fp32 kernel."""
+    """actor_loss_grad (natural_pg.py:L150-157) in tensor-core mode -- a single network spread over one
+    CTA per SM -- vs the exact-fp32 kernel."""
     rng = np.random.default_rng(21)
     N, T, O, A = 300, 70, 60, 8          # 165 tiles of 128 rows: more tiles than CTAs, ragged tail
     theta = oac.init_theta(O, A, seed=4)

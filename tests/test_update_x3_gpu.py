@@ -1,4 +1,4 @@
-"""GPU: the split-bf16 ("bf16x3", tcgen05 kind::f16, six MMAs per product) variant of the fused minibatch
+"""GPU: the split-bf16 ("bf16x3", bf16 wgmma, six MMAs per product) variant of the fused minibatch
 kernel.  It is held to the SAME bars as the exact-fp32 FMA path (tests/test_update_gpu.py): gradients vs
 oracle autograd at rtol 2e-4 / atol 2e-5 of the scale (and <= 1e-4 l2-relative per parameter block), and a whole
 PPOLag._update against the golden fixture of the unmodified reference at the fp32-mode tolerance."""

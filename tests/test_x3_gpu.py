@@ -1,4 +1,4 @@
-"""Pins the split-bf16 ("bf16x3", tcgen05 kind::f16) building blocks of csrc/x3.cuh on real hardware:
+"""Pins the split-bf16 ("bf16x3", bf16 wgmma) building blocks of csrc/x3.cuh on real hardware:
 the K-major and MN-major views of one physical SW128 / SW32 bf16 tile, the six-product compensation,
 and its fp32-level accuracy (the parity-grade tensor-core mode rests on these conventions)."""
 import numpy as np

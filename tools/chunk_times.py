@@ -1,4 +1,4 @@
-"""CUDA-event timing of the update-side kernels at a given obs dim (default 376), fp32 FMA tiles vs tcgen05
+"""CUDA-event timing of the update-side kernels at a given obs dim (default 376), fp32 FMA tiles vs wgmma
 tiles: minibatch gradient (16384 rows, 3 networks), Fisher-vector product, full-batch evaluation."""
 import json
 import sys

@@ -1,5 +1,5 @@
 """CUDA-event timing of the Fisher-vector product and full-batch actor gradient, fp32 FMA tiles vs
-tcgen05 tiles (headline batch 4096 x 128, O = 60, A = 8)."""
+wgmma tiles (headline batch 4096 x 128, O = 60, A = 8)."""
 import json
 import sys
 
