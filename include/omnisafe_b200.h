@@ -134,6 +134,40 @@ int osb_rollout_set_early_termination(float* cost_acc, float cost_limit);
  * across epochs; window_sums[4] <- {sum EpRet, sum EpCost, sum EpLen, count} (fp64). */
 int osb_episode_window(const unsigned char* flags, const float* epfin, int T, int N, int W,
                        float* ring, int* meta, double* window_sums, void* stream);
+/* ---- rollout on an external env (a user CMDP stepped in PyTorch) ----------------------------
+ * The fused step split at the env boundary.  Per epoch: env.reset() -> osb_ext_reset_ingest; for t in [0, T):
+ * osb_ext_act(t) -> env.step(act_env) -> osb_ext_observe(t); then osb_ext_act(T) (epoch-end bootstrap, critics only)
+ * and osb_episode_window.  State arrays as for osb_rollout_step: s_raw[2][N][O] and final_raw[2][N][O] by step parity,
+ * ep_ret / ep_cost / ep_len [N], the normaliser state (acc_all / acc_fin / fin_count are not used: the observation
+ * statistics are combined from fp64 per-tile moments in fixed tile order, so they are exact to fp64 rounding for any
+ * observation range and the same on every run).  workspace: osb_ext_workspace_doubles(O, N) doubles.
+ * nonfinite (device int) is set to 1 when an observation (next or final) is not finite; it is never cleared here.
+ * osb_ext_act = the network half of osb_rollout_step (same arithmetic in every precision mode, O > 64 under 1 / 2
+ * falls back to the fp32 tiles): obs / act / logp / value slabs, bootstrap values of paths truncated at t - 1 (from
+ * final_raw with mean1 / std1) and at t == T the epoch-end bootstrap; act_env[N][A] <- ActionScale(act) onto
+ * [act_lo, act_hi] (wrapper.py:L510-512, fp32 lo + (hi - lo) * (a + 1) / 2, no clipping); the act slab keeps the
+ * unscaled action.  osb_ext_observe: rew / cost / flags / epfin of step t, episode bookkeeping, next obs -> s_raw,
+ * rows of final_obs selected by final_mask -> final_raw (both may be NULL: no final observation), ObsNormalize push
+ * of the final rows (-> mean1 / std1) then of all rows (wrapper.py:L231-241).  terminated / truncated / final_mask
+ * are one byte per env (0 / non-zero). */
+int osb_ext_workspace_doubles(int O, int N);
+int osb_ext_reset_ingest(int O, int N, int obs_normalize, const float* obs, float* s_raw, float* ep_ret, float* ep_cost,
+                         int* ep_len, float* norm_mean, float* norm_sumsq, float* norm_std, float* norm_mean1,
+                         float* norm_std1, long long* norm_count, int* had_fin, unsigned* ticket, double* workspace,
+                         int* nonfinite, void* stream);
+int osb_ext_act(int O, int A, int obs_normalize, int N, int T, int t, unsigned env_id_offset, float* s_raw,
+                float* final_raw, float* norm_mean, float* norm_std, float* norm_mean1, float* norm_std1,
+                long long* norm_count, float* obs, float* act, float* logp, float* val_r, float* val_c, float* boot_r,
+                float* boot_c, unsigned char* flags, const float* theta, const float* eps, unsigned noise_seed,
+                unsigned global_step, const float* act_lo, const float* act_hi, float* act_env, int precision,
+                void* stream);
+int osb_ext_observe(int O, int N, int T, int t, int obs_normalize, const float* next_obs, const float* rew,
+                    const float* cost, const unsigned char* terminated, const unsigned char* truncated,
+                    const float* final_obs, const unsigned char* final_mask, float* s_raw, float* final_raw,
+                    float* ep_ret, float* ep_cost, int* ep_len, float* norm_mean, float* norm_sumsq, float* norm_std,
+                    float* norm_mean1, float* norm_std1, long long* norm_count, int* had_fin, unsigned* ticket,
+                    float* rew_slab, float* cost_slab, unsigned char* flags, float* epfin, double* workspace,
+                    int* nonfinite, void* stream);
 /* RewardNormalize / CostNormalize (envs/wrapper.py:L280-423; Normalizer(shape=(), clip=5),
  * common/normalizer.py:L88-139) applied to one epoch's slab x[T][N] in place, after the rollout: row t
  * is pushed into the running statistics (batch of N) and normalised with the statistics valid right

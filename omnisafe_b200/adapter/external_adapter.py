@@ -1,0 +1,161 @@
+"""On-policy adapter for user-registered CMDPs: the env steps in PyTorch, everything else stays on the kernels.
+
+Same constructor, `rollout(steps_per_epoch, agent, buffer, logger, eps=None)`, `save()` and `obs_dim / act_dim /
+num_envs` as `OnPolicyAdapter` (omnisafe/adapter/onpolicy_adapter.py:L30-175).  One epoch:
+
+    env.reset() -> osb_ext_reset_ingest
+    for t in 0 .. T-1:  osb_ext_act(t) -> env.step(action) -> osb_ext_observe(t)
+    osb_ext_act(T) (epoch-end bootstrap) -> osb_episode_window -> Reward / CostNormalize slab post-pass
+
+osb_ext_act runs ObsNormalize, the three MLP forwards, sampling / log-prob and ActionScale, appends the obs / act /
+logp / value slabs and writes the bootstrap values; osb_ext_observe appends reward / cost / flags, keeps the episode
+statistics and feeds the observation normaliser.  Nothing in the loop synchronises the host except the env's own code
+(and, for an env on the CPU, the copy of the action to it).  A non-finite observation raises `OsbError` at the end of
+the epoch.
+"""
+from __future__ import annotations
+
+import torch
+
+from omnisafe_b200._lib import OsbError, current_stream, lib, ptr
+from omnisafe_b200.common.normalizer import Normalizer, ScalarNormalizer
+from omnisafe_b200.envs.core import check_env, make
+
+
+class ExternalEnvAdapter:
+    def __init__(self, env_id: str, num_envs: int, seed: int, cfgs, device='cuda',
+                 env_id_offset: int = 0) -> None:
+        self._cfgs = cfgs
+        self._device = torch.device(device)
+        env_cfgs = getattr(cfgs, 'env_cfgs', None) or {}
+        env_cfgs = dict(env_cfgs.todict() if hasattr(env_cfgs, 'todict') else env_cfgs)
+        env_cfgs.pop('env_id_offset', None)
+        self._env = make(env_id, num_envs=num_envs, device=self._device, **env_cfgs)
+        self._obs_dim, self._act_dim, lo, hi = check_env(self._env)
+        self._num_envs = int(num_envs)
+        self._env.set_seed(seed)                      # per-rank seed, as OnlineAdapter does (online_adapter.py:L81)
+        self._env_id_offset = int(env_id_offset)
+        algo = cfgs.algo_cfgs
+        self._reward_normalizer = ScalarNormalizer(5.0, self._device) if getattr(algo, 'reward_normalize', False) else None
+        self._cost_normalizer = ScalarNormalizer(5.0, self._device) if getattr(algo, 'cost_normalize', False) else None
+        self._obs_normalize = bool(getattr(algo, 'obs_normalize', True))
+        self._obs_normalizer = Normalizer((self._obs_dim,), clip=5.0, device=self._device)
+        W = int(getattr(cfgs.logger_cfgs, 'window_lens', 100))
+        self.window_lens = W
+        self.ep_ring = torch.zeros(3, W, dtype=torch.float32, device=self._device)
+        self.ep_meta = torch.zeros(2, dtype=torch.int32, device=self._device)
+        self.window_sums = torch.zeros(4, dtype=torch.float64, device=self._device)
+        self._epoch_index = 0
+        prec = str(getattr(cfgs.train_cfgs, 'matmul_precision', 'bf16x3') if hasattr(cfgs, 'train_cfgs') else 'fp32')
+        self.precision = {'fp32': 0, 'tf32': 1, 'bf16x3': 2}[prec]
+        self.noise_seed = (int(seed) * 2654435761 + 12345) & 0xFFFFFFFF
+        N, O, A, dev = self._num_envs, self._obs_dim, self._act_dim, self._device
+        f32 = dict(dtype=torch.float32, device=dev)
+        self.s_raw = torch.zeros(2, N, O, **f32)
+        self.final_raw = torch.zeros(2, N, O, **f32)
+        self.ep_ret = torch.zeros(N, **f32)
+        self.ep_cost = torch.zeros(N, **f32)
+        self.ep_len = torch.zeros(N, dtype=torch.int32, device=dev)
+        self.act_lo = torch.as_tensor(lo).to(dev)
+        self.act_hi = torch.as_tensor(hi).to(dev)
+        self.act_env = torch.zeros(N, A, **f32)
+        self._ws = torch.zeros(lib().osb_ext_workspace_doubles(O, N), dtype=torch.float64, device=dev)
+        self.nonfinite = torch.zeros(1, dtype=torch.int32, device=dev)
+
+    @property
+    def env(self):
+        return self._env
+
+    @property
+    def obs_dim(self) -> int:
+        return self._obs_dim
+
+    @property
+    def act_dim(self) -> int:
+        return self._act_dim
+
+    @property
+    def num_envs(self) -> int:
+        return self._num_envs
+
+    def save(self) -> dict:
+        """What OnlineAdapter.save() exposes for checkpoints (online_adapter.py:L222-231)."""
+        saved = {'obs_normalizer': self._obs_normalizer} if self._obs_normalize else {}
+        if self._reward_normalizer is not None:
+            saved['reward_normalizer'] = self._reward_normalizer
+        if self._cost_normalizer is not None:
+            saved['cost_normalizer'] = self._cost_normalizer
+        return saved
+
+    # ---- env output -> contiguous device tensors ---------------------------------------------------
+    def _rows(self, x, width: int | None = None, dtype=torch.float32) -> torch.Tensor:
+        x = torch.as_tensor(x)
+        shape = (self._num_envs,) if width is None else (self._num_envs, width)
+        return x.to(device=self._device, dtype=dtype).reshape(shape).contiguous()
+
+    def _norm_ptrs(self) -> list:
+        n = self._obs_normalizer
+        return [ptr(n.mean), ptr(n.sumsq), ptr(n.std), ptr(n.mean1), ptr(n.std1), ptr(n.count), ptr(n.had_fin),
+                ptr(n.ticket)]
+
+    def rollout(self, steps_per_epoch: int, agent, buffer, logger=None, eps=None) -> None:
+        """Roll the envs for `steps_per_epoch` steps each and fill `buffer` (see the module docstring).
+
+        `eps` (optional, [T, N, A]) supplies the standard-normal stream (parity mode); by default the kernel draws
+        Philox noise."""
+        T, N, O, A = int(steps_per_epoch), self._num_envs, self._obs_dim, self._act_dim
+        assert T == buffer.T and N == buffer.N
+        if eps is not None:
+            assert eps.shape == (T, N, A) and eps.dtype == torch.float32
+        L, d, s = lib(), buffer.data, current_stream()
+        on = int(self._obs_normalize)
+        nz = self._obs_normalizer
+        obs, _ = self._env.reset()
+        env_dev = torch.as_tensor(obs).device
+        obs = self._rows(obs, O)
+        L.osb_ext_reset_ingest(O, N, on, ptr(obs), ptr(self.s_raw), ptr(self.ep_ret), ptr(self.ep_cost),
+                               ptr(self.ep_len), *self._norm_ptrs(), ptr(self._ws), ptr(self.nonfinite), s)
+
+        def act(t: int) -> None:
+            L.osb_ext_act(O, A, on, N, T, t, self._env_id_offset & 0xFFFFFFFF, ptr(self.s_raw), ptr(self.final_raw),
+                          ptr(nz.mean), ptr(nz.std), ptr(nz.mean1), ptr(nz.std1), ptr(nz.count),
+                          ptr(d['obs']), ptr(d['act']), ptr(d['logp']), ptr(d['value_r']), ptr(d['value_c']),
+                          ptr(d['boot_r']), ptr(d['boot_c']), ptr(d['flags']), ptr(agent.theta),
+                          ptr(eps[t]) if (eps is not None and t < T) else 0, self.noise_seed,
+                          (self._epoch_index * T + t) & 0xFFFFFFFF, ptr(self.act_lo), ptr(self.act_hi),
+                          ptr(self.act_env), int(self.precision), s)
+
+        for t in range(T):
+            act(t)
+            # a fresh tensor every step, as the reference hands the env: the buffer is rewritten by the next act step
+            action = self.act_env.to(env_dev, copy=True)
+            if N == 1:
+                action = action[0]                  # a single env takes an unbatched action (reference Unsqueeze)
+            nobs, rew, cost, term, trunc, info = self._env.step(action)
+            nobs = self._rows(nobs, O)
+            rew, cost = self._rows(rew), self._rows(cost)
+            term, trunc = self._rows(term, dtype=torch.uint8), self._rows(trunc, dtype=torch.uint8)
+            final = mask = None
+            if 'final_observation' in info:
+                final = self._rows(info['final_observation'], O)
+                mask = info.get('_final_observation')
+                mask = (term | trunc) if mask is None else self._rows(mask, dtype=torch.uint8)
+            L.osb_ext_observe(O, N, T, t, on, ptr(nobs), ptr(rew), ptr(cost), ptr(term), ptr(trunc), ptr(final),
+                              ptr(mask), ptr(self.s_raw), ptr(self.final_raw), ptr(self.ep_ret), ptr(self.ep_cost),
+                              ptr(self.ep_len), *self._norm_ptrs(), ptr(d['reward']), ptr(d['cost']),
+                              ptr(d['flags']), ptr(d['epfin']), ptr(self._ws), ptr(self.nonfinite), s)
+        act(T)
+        L.osb_episode_window(ptr(d['flags']), ptr(d['epfin']), T, N, self.window_lens, ptr(self.ep_ring),
+                             ptr(self.ep_meta), ptr(self.window_sums), s)
+        # the per-step reward / cost normalisation of the reference commutes with the rollout (OnPolicyAdapter.rollout)
+        if self._reward_normalizer is not None:
+            self._reward_normalizer.normalize_rows_(d['reward'])
+        if self._cost_normalizer is not None:
+            self._cost_normalizer.normalize_rows_(d['cost'])
+        self._epoch_index += 1
+        if int(self.nonfinite.item()):
+            self.nonfinite.zero_()
+            raise OsbError(f'{type(self._env).__name__} returned a non-finite observation during the last epoch')
+
+    def close(self) -> None:
+        self._env.close()

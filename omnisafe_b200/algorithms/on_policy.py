@@ -16,6 +16,7 @@ import torch
 
 from omnisafe_b200.adapter.onpolicy_adapter import OnPolicyAdapter
 from omnisafe_b200.adapter.early_terminated_adapter import EarlyTerminatedAdapter
+from omnisafe_b200.adapter.external_adapter import ExternalEnvAdapter
 from omnisafe_b200.adapter.saute_adapter import SauteAdapter
 from omnisafe_b200.adapter.simmer_adapter import SimmerAdapter
 from omnisafe_b200.algorithms import registry
@@ -26,8 +27,20 @@ from omnisafe_b200.common.buffer import VectorOnPolicyBuffer
 from omnisafe_b200.common.lagrange import Lagrange
 from omnisafe_b200.common.logger import Logger
 from omnisafe_b200.common.pid_lagrange import PIDLagrangian
+from omnisafe_b200.envs.synthetic import support_envs as synthetic_envs
 from omnisafe_b200.models.actor_critic import ConstraintActorCritic
 from omnisafe_b200.utils import distributed
+
+
+def _plain_adapter(env_id: str):
+    """The synthetic env runs inside the fused rollout kernel; a registered CMDP is stepped in PyTorch around the
+    act / observe kernels."""
+    return OnPolicyAdapter if env_id in synthetic_envs() else ExternalEnvAdapter
+
+
+def _require_synthetic(env_id: str, what: str) -> None:
+    if env_id not in synthetic_envs():
+        raise NotImplementedError(f'{what} runs on the synthetic env only; {env_id} is a registered external env')
 
 
 @registry.register
@@ -40,8 +53,8 @@ class PolicyGradient(BaseAlgo):
     def _init_env(self) -> None:
         t, a = self._cfgs.train_cfgs, self._cfgs.algo_cfgs
         rank = distributed.get_rank()
-        self._env = OnPolicyAdapter(self._env_id, t.vector_env_nums, self._seed, self._cfgs,
-                                    device=self._device, env_id_offset=rank * t.vector_env_nums)
+        self._env = _plain_adapter(self._env_id)(self._env_id, t.vector_env_nums, self._seed, self._cfgs,
+                                                 device=self._device, env_id_offset=rank * t.vector_env_nums)
         self._steps_per_epoch = distributed.local_steps(a.steps_per_epoch, t.vector_env_nums)
 
     def _init_model(self) -> None:
@@ -606,6 +619,7 @@ class _SauteMixin:
     _adapter_cls = SauteAdapter
 
     def _init_env(self) -> None:
+        _require_synthetic(self._env_id, type(self).__name__)
         t, a = self._cfgs.train_cfgs, self._cfgs.algo_cfgs
         rank = distributed.get_rank()
         self._env = self._adapter_cls(self._env_id, t.vector_env_nums, self._seed, self._cfgs, device=self._device,
@@ -656,6 +670,7 @@ class _EarlyTerminatedMixin:
     """early_terminated/ppo_early_terminated.py:L43-66, early_terminated/trpo_early_terminated.py."""
 
     def _init_env(self) -> None:
+        _require_synthetic(self._env_id, type(self).__name__)
         t, a = self._cfgs.train_cfgs, self._cfgs.algo_cfgs
         rank = distributed.get_rank()
         self._env = EarlyTerminatedAdapter(self._env_id, t.vector_env_nums, self._seed, self._cfgs, device=self._device,

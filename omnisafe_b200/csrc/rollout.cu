@@ -106,13 +106,9 @@ __device__ __forceinline__ float env_next_value(float s, float a, float b) {
 }
 
 // Chan / Golub / LeVeque batched update as Normalizer._push writes it (normalizer.py:L102-120),
-// fp32 state, batch moments derived from the fixed-point sums.
-__device__ void norm_push(float& mean, float& sumsq, long long count_old, long long n,
-                          long long sx_fix, long long sxx_fix) {
-    const double sx = (double)sx_fix / FIX_SCALE, sxx = (double)sxx_fix / FIX_SCALE;
-    const double mraw = sx / (double)n;
-    double m2 = sxx - (double)n * mraw * mraw;
-    if (m2 < 0.0) m2 = 0.0;
+// fp32 state, from the batch mean and sum of squared deviations (fp64).
+__device__ __forceinline__ void norm_push_moments(float& mean, float& sumsq, long long count_old, long long n,
+                                                  double mraw, double m2) {
     const float mean_raw = (float)mraw, sumq_raw = (float)m2;
     const long long count = count_old + n;
     const float delta = __fadd_rn(mean_raw, -mean);
@@ -120,6 +116,15 @@ __device__ void norm_push(float& mean, float& sumsq, long long count_old, long l
     const float d2 = __fmul_rn(delta, delta);
     const float corr = __fdiv_rn(__fmul_rn(__fmul_rn(d2, (float)count_old), (float)n), (float)count);
     sumsq = __fadd_rn(sumsq, __fadd_rn(sumq_raw, corr));
+}
+// the same update with the batch moments derived from the fixed-point sums
+__device__ void norm_push(float& mean, float& sumsq, long long count_old, long long n,
+                          long long sx_fix, long long sxx_fix) {
+    const double sx = (double)sx_fix / FIX_SCALE, sxx = (double)sxx_fix / FIX_SCALE;
+    const double mraw = sx / (double)n;
+    double m2 = sxx - (double)n * mraw * mraw;
+    if (m2 < 0.0) m2 = 0.0;
+    norm_push_moments(mean, sumsq, count_old, n, mraw, m2);
 }
 __device__ __forceinline__ float norm_std(float sumsq, long long count) {
     const float var = __fdiv_rn(sumsq, (float)(count - 1));
@@ -279,7 +284,17 @@ struct StepArgs {
     unsigned int* bar_flag;
     long long* dbg;           // optional clock64 stamps (persistent kernel), normally null
     float* acc;               // tensor-core tiles: accumulator images, one [128][R_COLS] per CTA
+    // external-env act step (EXT instantiations only): the sampled action after ActionScale onto [act_lo, act_hi]
+    const float* act_lo;      // [A]
+    const float* act_hi;      // [A]
+    float* act_env;           // [N][A]
 };
+
+// ActionScale (wrapper.py:L510-512) from [-1, 1] onto [lo, hi] in the reference's fp32 order:
+// lo + (hi - lo) * (a - (-1)) / (1 - (-1)).  No clipping: the env receives what the wrapper would hand it.
+__device__ __forceinline__ float action_scale(float a, float lo, float hi) {
+    return __fadd_rn(lo, __fdiv_rn(__fmul_rn(__fadd_rn(hi, -lo), __fadd_rn(a, 1.f)), 2.f));
+}
 
 // normalise (or copy) a tile of raw observations into sX (chunk kc), zero padded.
 // z = per-env safety state (Saute) appended as column O of the network input (rows are On = O + 1 wide then), or null;
@@ -327,6 +342,10 @@ __device__ __forceinline__ float saute_step(const SauteSpec& sa, int t, int N, i
     return out;
 }
 
+// EXT = true: the act half of a step on a user env (csrc: osb_ext_act).  The network part is the same; the actor CTAs
+// hand the scaled action to the env through p.act_env instead of running the synthetic transition, and the normaliser is
+// fed by the observe kernel after env.step.
+template <bool EXT>
 __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
     extern __shared__ __align__(16) float smem[];
     NetSmem W;
@@ -451,12 +470,16 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
             lp += term;
             sAct[e * OUTP + a] = act;
             if (ok) p.sl.act[((size_t)t * N + env) * A + a] = act;
+            if constexpr (EXT) {
+                if (ok) p.act_env[(size_t)env * A + a] = action_scale(act, __ldg(p.act_lo + a), __ldg(p.act_hi + a));
+            }
         }
         lp += __shfl_xor_sync(0xffffffffu, lp, 1);
         lp += __shfl_xor_sync(0xffffffffu, lp, 2);
         lp += __shfl_xor_sync(0xffffffffu, lp, 4);
         if (ok && q == 0) p.sl.logp[(size_t)t * N + env] = lp;
     }
+    if constexpr (EXT) return;
     __syncthreads();
 
     // ---- env transition ----------------------------------------------------------------------
@@ -593,8 +616,11 @@ constexpr uint32_t RTC_FOFF_TF32 = 2 * RTC * 256 + 2 * 16384 + 4096, RTC_FOFF_X3
 // last arriver folds the step's normaliser sums into the running statistics before it releases the others
 // (adapter/onpolicy_adapter.py:L58-136 is the loop this replaces).  Data written by other CTAs in earlier steps
 // (raw states, flags, normaliser statistics) is read with ld.global.cg.
-template <bool X3, bool PERSIST>
+// EXT = true: the act half of a step on a user env, as in rollout_step_kernel<true> (never persistent: Python runs
+// env.step between the launches).
+template <bool X3, bool PERSIST, bool EXT = false>
 __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p) {
+    static_assert(!(EXT && PERSIST), "the external-env act step is one launch per step");
     using namespace umma;
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
@@ -725,7 +751,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
     float* s_nxt = p.st.s_raw + (size_t)((t + 1) & 1) * N * O;
     if (PERSIST) { if (tid == 0) s_anyfin = 0; __syncthreads(); }
     // which envs of this tile finish in this step (time limit / hash-driven termination): known before the forward
-    if (net == 0 && tid < RTC) {
+    if (!EXT && net == 0 && tid < RTC) {
         const int env = env0 + tid;
         int fl = 0, ep_step = 0; uint32_t epi = 0, gstep = 0;
         if (env < N) {
@@ -964,6 +990,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                         lp += term;
                         sAct[e * OUTP + a] = act;
                         if (ok) p.sl.act[((size_t)t * N + env) * A + a] = act;
+                        if constexpr (EXT) {
+                            if (ok) p.act_env[(size_t)env * A + a] = action_scale(act, __ldg(p.act_lo + a), __ldg(p.act_hi + a));
+                        }
                     }
                 }
                 lp += __shfl_xor_sync(0xffffffffu, lp, 1);
@@ -992,6 +1021,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                     lp += term;
                     sAct[e * OUTP + a] = act;
                     if (ok) p.sl.act[((size_t)t * N + env) * A + a] = act;
+                    if constexpr (EXT) {
+                        if (ok) p.act_env[(size_t)env * A + a] = action_scale(act, __ldg(p.act_lo + a), __ldg(p.act_hi + a));
+                    }
                 }
                 lp += __shfl_xor_sync(0xffffffffu, lp, 1);
                 lp += __shfl_xor_sync(0xffffffffu, lp, 2);
@@ -999,6 +1031,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                 if (ok && qq == 0) p.sl.logp[(size_t)t * N + env] = lp;
             }
         }
+        if constexpr (EXT) return;
         __syncthreads();
         if (p.et.cost_acc) {      // EarlyTerminated: the step's cost is known from state dim 0 -> finish flags before the transition
             if (tid < RTC && env0 + tid < N) {
@@ -1137,7 +1170,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
             __syncthreads();
             RSTAMP(10);
         }
-    } else if (p.es.obs_normalize && !is_tail) {
+    } else if (!EXT && p.es.obs_normalize && !is_tail) {
         __threadfence();
         __syncthreads();
         if (tid == 0) s_last = (atomicAdd(p.ns.ticket, 1u) == gridDim.x * gridDim.y - 1) ? 1 : 0;
@@ -1153,6 +1186,169 @@ static size_t rollout_tc_smem_bytes(bool x3) {
     return 1024 + (x3 ? RTC_FOFF_X3 : RTC_FOFF_TF32) +
            (64 + 64 + 16 + 64 + 64 + RTC * OUTP + 2 * RTC * SNW) * sizeof(float) + 4 * 4 * 64 * sizeof(long long) +
            5 * RTC * sizeof(int) + 48 * sizeof(float) + 64;
+}
+
+// ---------------------------------------------------------------------------------------------
+// External envs (a user CMDP stepped in PyTorch): the observe half of a step, after env.step, and the ingest of the
+// reset observations at epoch start (onpolicy_adapter.py:L80).  Elementwise over tiles of XT envs: slab append, episode
+// bookkeeping (onpolicy_adapter.py:L138-175), next / final observations into the parity buffers the act kernels read,
+// and ObsNormalize (wrapper.py:L231-241: final rows first -> mean1 / std1, then all rows).
+//
+// The observations of a user env have no bound, so the fixed-point sums of the synthetic path do not apply: each tile
+// writes fp64 (mean, M2) per column for all rows and for the final rows, and the last CTA (ticket) combines them in tile
+// order (Chan et al.) -- no floating-point atomics, the same result on every run.
+constexpr int XT = 32;
+
+struct ExtObs {
+    const float* next_obs;      // [N][O] raw observation after the step (rows that finished are already reset)
+    const float* rew;           // [N]
+    const float* cost;          // [N]
+    const uint8_t* term;        // [N]
+    const uint8_t* trunc;       // [N]
+    const float* final_obs;     // [N][O] or null
+    const uint8_t* final_mask;  // [N] rows of final_obs that hold a final observation, or null
+    double* part;               // [tiles][4][O] (mean, M2) of all rows and of the final rows, then [tiles] final-row counts
+    int* nonfinite;             // [1] set to 1 when an observation is not finite
+};
+
+__device__ __forceinline__ void chan_combine(double& n, double& m, double& q, double nk, double mk, double qk) {
+    if (nk == 0.0) return;
+    if (n == 0.0) { n = nk; m = mk; q = qk; return; }
+    const double nn = n + nk, d = mk - m;
+    m += d * nk / nn;
+    q += qk + d * d * n * nk / nn;
+    n = nn;
+}
+
+__global__ void __launch_bounds__(NTHREADS) ext_observe_kernel(ExtObs x, EnvState st, NormState ns, Slabs sl, int O, int N,
+                                                               int T, int t, int obs_normalize, int is_reset) {
+    __shared__ int sFin[XT];
+    __shared__ int s_bad, s_last, s_nfin;
+    const int tid = threadIdx.x, tile = blockIdx.x, ntiles = gridDim.x;
+    const int env0 = tile * XT, rows = min(XT, N - env0);
+    if (tid == 0) s_bad = 0;
+    if (tid < XT) {
+        const int env = env0 + tid;
+        int fin = 0;
+        if (tid < rows) {
+            if (is_reset) {
+                st.ep_ret[env] = 0.f; st.ep_cost[env] = 0.f; st.ep_len[env] = 0;
+            } else {
+                fin = (x.final_obs && x.final_mask && x.final_mask[env]) ? 1 : 0;
+                const float r = x.rew[env], c = x.cost[env];
+                const bool te = x.term[env] != 0, tr = x.trunc[env] != 0;
+                const size_t idx = (size_t)t * N + env;
+                sl.rew[idx] = r;
+                sl.cost[idx] = c;
+                sl.flags[idx] = (uint8_t)((te ? OSB_FLAG_TERMINATED : 0u) | (tr ? OSB_FLAG_TRUNCATED : 0u));
+                const float er = __fadd_rn(st.ep_ret[env], r), ec = __fadd_rn(st.ep_cost[env], c);
+                const int el = st.ep_len[env] + 1;
+                if (te || tr) {
+                    const size_t TN = (size_t)T * N;
+                    sl.epfin[idx] = er; sl.epfin[TN + idx] = ec; sl.epfin[2 * TN + idx] = (float)el;
+                    st.ep_ret[env] = 0.f; st.ep_cost[env] = 0.f; st.ep_len[env] = 0;
+                } else {
+                    st.ep_ret[env] = er; st.ep_cost[env] = ec; st.ep_len[env] = el;
+                }
+            }
+        }
+        sFin[tid] = fin;
+    }
+    __syncthreads();
+
+    // step t reads parity t & 1, so the reset observation goes to buffer 0 and the next one of step t to (t + 1) & 1
+    float* s_nxt = st.s_raw + (size_t)(is_reset ? 0 : ((t + 1) & 1)) * N * O;
+    float* fin_out = st.final_raw + (size_t)(t & 1) * N * O;
+    bool bad = false;
+    for (int i = tid; i < rows * O; i += NTHREADS) {
+        const int r = i / O;
+        const size_t g = (size_t)env0 * O + i;
+        const float v = x.next_obs[g];
+        bad |= !isfinite(v);
+        s_nxt[g] = v;
+        if (sFin[r]) {
+            const float f = x.final_obs[g];
+            bad |= !isfinite(f);
+            fin_out[g] = f;
+        }
+    }
+    if (bad) s_bad = 1;
+    if (!obs_normalize) {
+        __syncthreads();
+        if (tid == 0 && s_bad) *x.nonfinite = 1;
+        return;
+    }
+
+    // per-tile moments (two passes over the tile's rows, fp64)
+    int nf = 0;
+    for (int r = 0; r < rows; ++r) nf += sFin[r];
+    double* P = x.part + (size_t)tile * 4 * O;
+    for (int j = tid; j < O; j += NTHREADS) {
+        double s = 0.0, sf = 0.0;
+        for (int r = 0; r < rows; ++r) {
+            const size_t g = (size_t)(env0 + r) * O + j;
+            s += (double)x.next_obs[g];
+            if (sFin[r]) sf += (double)x.final_obs[g];
+        }
+        const double m = s / rows, mf = nf ? sf / nf : 0.0;
+        double q = 0.0, qf = 0.0;
+        for (int r = 0; r < rows; ++r) {
+            const size_t g = (size_t)(env0 + r) * O + j;
+            const double d = (double)x.next_obs[g] - m;
+            q += d * d;
+            if (sFin[r]) { const double df = (double)x.final_obs[g] - mf; qf += df * df; }
+        }
+        P[j] = m; P[O + j] = q; P[2 * O + j] = mf; P[3 * O + j] = qf;
+    }
+    if (tid == 0) x.part[(size_t)ntiles * 4 * O + tile] = (double)nf;
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) {
+        if (s_bad) *x.nonfinite = 1;
+        s_last = (atomicAdd(ns.ticket, 1u) == (unsigned)ntiles - 1u) ? 1 : 0;
+    }
+    __syncthreads();
+    if (!s_last) return;
+
+    // last CTA: combine the tiles in order and push final rows, then all rows (norm_finalize's sequence)
+    __threadfence();
+    const double* cnt = x.part + (size_t)ntiles * 4 * O;
+    if (tid == 0) {
+        int total = 0;
+        for (int k = 0; k < ntiles; ++k) total += (int)__ldcg(cnt + k);
+        s_nfin = total;
+    }
+    __syncthreads();
+    const int nfin = s_nfin;
+    const long long count = __ldcg(ns.count);
+    for (int j = tid; j < O; j += NTHREADS) {
+        double n = 0.0, m = 0.0, q = 0.0, nF = 0.0, mF = 0.0, qF = 0.0;
+        for (int k = 0; k < ntiles; ++k) {
+            const double* Pk = x.part + (size_t)k * 4 * O;
+            chan_combine(n, m, q, (double)min(XT, N - k * XT), __ldcg(Pk + j), __ldcg(Pk + O + j));
+            chan_combine(nF, mF, qF, __ldcg(cnt + k), __ldcg(Pk + 2 * O + j), __ldcg(Pk + 3 * O + j));
+        }
+        float mean = __ldcg(ns.mean + j), sumsq = __ldcg(ns.sumsq + j);
+        long long c = count;
+        if (nfin > 0) {
+            norm_push_moments(mean, sumsq, c, nfin, mF, qF);
+            c += nfin;
+            ns.mean1[j] = mean;
+            ns.std1[j] = norm_std(sumsq, c);
+        }
+        norm_push_moments(mean, sumsq, c, N, m, q);
+        c += N;
+        ns.mean[j] = mean;
+        ns.sumsq[j] = sumsq;
+        ns.std[j] = norm_std(sumsq, c);
+    }
+    __syncthreads();
+    if (tid == 0) {
+        ns.count[1] = count + nfin;
+        ns.count[0] = count + nfin + N;
+        *ns.had_fin = nfin > 0 ? 1 : 0;
+        *ns.ticket = 0u;
+    }
 }
 
 // Window of the last <= W finished episodes in (step, env) append order: Logger deque semantics
@@ -1288,6 +1484,10 @@ int osb_env_reset(int O, int A, int max_episode_steps, unsigned seed, unsigned t
 
 static long long* g_rollout_dbg = nullptr;
 
+}  // extern "C"
+
+// EXT = true: the act step of the external-env path (never the persistent kernel)
+template <bool EXT>
 static int launch_step(StepArgs& p, cudaStream_t stream) {
     const int On = p.es.O + (p.sa.safety ? 1 : 0);
     if ((p.precision == 1 || p.precision == 2) && On <= 64) {
@@ -1295,15 +1495,26 @@ static int launch_step(StepArgs& p, cudaStream_t stream) {
         const size_t smem_tc = rollout_tc_smem_bytes(x3);
         static bool attr_tc = false;
         if (!attr_tc) {
-            OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(false)));
-            OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(true)));
-            OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(false)));
-            OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(true)));
+            if constexpr (EXT) {
+                OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(false)));
+                OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(true)));
+            } else {
+                OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(false)));
+                OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(true)));
+                OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(false)));
+                OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(true)));
+            }
             attr_tc = true;
         }
         dim3 grid_tc((p.N + RTC - 1) / RTC, p.is_tail ? 2 : 3);
         p.acc = acc_scratch(ACC_ROLLOUT, (size_t)grid_tc.x * 3 * 128 * R_COLS * sizeof(float));
         if (!p.acc) return OSB_ERR_CUDA;
+        if (EXT) {
+            if (x3) rollout_step_tc_kernel<true, false, true><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
+            else rollout_step_tc_kernel<false, false, true><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
+            OSB_LAUNCH_CHECK();
+            return OSB_OK;
+        }
         if (p.bar_ctr != nullptr) {
             // the whole epoch in one cooperative launch (every CTA resident: the step barrier is a software grid barrier)
             OSB_CUDA(cudaMemsetAsync(p.bar_ctr, 0, 2 * sizeof(unsigned int), stream));
@@ -1321,14 +1532,16 @@ static int launch_step(StepArgs& p, cudaStream_t stream) {
     const size_t smem = rollout_smem_bytes(On);
     static size_t attr = 0;
     if (smem > attr) {
-        OSB_CUDA(cudaFuncSetAttribute(rollout_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        OSB_CUDA(cudaFuncSetAttribute(rollout_step_kernel<EXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = smem;
     }
     dim3 grid((p.N + RT - 1) / RT, p.is_tail ? 2 : 3);
-    rollout_step_kernel<<<grid, NTHREADS, smem, stream>>>(p);
+    rollout_step_kernel<EXT><<<grid, NTHREADS, smem, stream>>>(p);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
 }
+
+extern "C" {
 
 // Saute / Simmer mode of the following osb_env_reset / osb_rollout_* calls (process-wide until changed): safety = [2][N]
 // device floats (the safety state z by step parity), or NULL for the plain OnPolicyAdapter semantics.  The networks then
@@ -1372,7 +1585,7 @@ int osb_rollout_step(int O, int A, int max_episode_steps, unsigned seed, unsigne
     p.theta = theta; p.eps = eps; p.noise_seed = noise_seed; p.global_step = global_step;
     p.t = t; p.T = T; p.N = N; p.is_tail = (t == T) ? 1 : 0; p.precision = precision;
     p.bar_ctr = nullptr; p.bar_flag = nullptr; p.dbg = nullptr;
-    return launch_step(p, (cudaStream_t)stream);
+    return launch_step<false>(p, (cudaStream_t)stream);
 }
 
 int osb_rollout_epoch(int O, int A, int max_episode_steps, unsigned seed, unsigned term_threshold,
@@ -1413,7 +1626,7 @@ int osb_rollout_epoch(int O, int A, int max_episode_steps, unsigned seed, unsign
         if (!d_bar) OSB_CUDA(cudaMalloc(&d_bar, 64));
         p.bar_ctr = d_bar; p.bar_flag = d_bar + 1;
         p.t = 0; p.is_tail = 0; p.eps = eps_all; p.global_step = epoch_index * (unsigned)T;
-        rc = launch_step(p, s);
+        rc = launch_step<false>(p, s);
         if (rc) return rc;
         return osb_episode_window(flags, epfin, T, N, W, ring, meta, window_sums, stream);
     }
@@ -1421,7 +1634,7 @@ int osb_rollout_epoch(int O, int A, int max_episode_steps, unsigned seed, unsign
         p.t = t; p.is_tail = (t == T) ? 1 : 0;
         p.eps = (eps_all && t < T) ? eps_all + (size_t)t * N * A : nullptr;
         p.global_step = epoch_index * (unsigned)T + (unsigned)t;
-        rc = launch_step(p, s);
+        rc = launch_step<false>(p, s);
         if (rc) return rc;
     }
     return osb_episode_window(flags, epfin, T, N, W, ring, meta, window_sums, stream);
@@ -1436,6 +1649,69 @@ int osb_episode_window(const unsigned char* flags, const float* epfin, int T, in
     window_sums_kernel<<<1, 32, 0, s>>>(ring, meta, W, window_sums);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
+}
+
+// ---- external envs ---------------------------------------------------------------------------
+int osb_ext_workspace_doubles(int O, int N) { return ((N + XT - 1) / XT) * (4 * O + 1); }
+
+static int launch_observe(const ExtObs& x, EnvState st, NormState ns, Slabs sl, int O, int N, int T, int t,
+                          int obs_normalize, int is_reset, void* stream) {
+    ext_observe_kernel<<<(N + XT - 1) / XT, NTHREADS, 0, (cudaStream_t)stream>>>(x, st, ns, sl, O, N, T, t, obs_normalize,
+                                                                                 is_reset);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}
+
+int osb_ext_reset_ingest(int O, int N, int obs_normalize, const float* obs, float* s_raw, float* ep_ret, float* ep_cost,
+                         int* ep_len, float* norm_mean, float* norm_sumsq, float* norm_std, float* norm_mean1,
+                         float* norm_std1, long long* norm_count, int* had_fin, unsigned* ticket, double* workspace,
+                         int* nonfinite, void* stream) {
+    OSB_CHECK_ARG(O > 0 && N > 0 && obs && s_raw && ep_ret && ep_cost && ep_len && workspace && nonfinite, "bad argument");
+    ExtObs x{obs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, workspace, nonfinite};
+    EnvState st{s_raw, nullptr, nullptr, nullptr, nullptr, ep_ret, ep_cost, ep_len, nullptr};
+    NormState ns{norm_mean, norm_sumsq, norm_std, norm_mean1, norm_std1, norm_count, nullptr, nullptr, nullptr, had_fin, ticket};
+    Slabs sl{};
+    return launch_observe(x, st, ns, sl, O, N, 1, 0, obs_normalize, 1, stream);
+}
+
+int osb_ext_observe(int O, int N, int T, int t, int obs_normalize, const float* next_obs, const float* rew,
+                    const float* cost, const unsigned char* terminated, const unsigned char* truncated,
+                    const float* final_obs, const unsigned char* final_mask, float* s_raw, float* final_raw,
+                    float* ep_ret, float* ep_cost, int* ep_len, float* norm_mean, float* norm_sumsq, float* norm_std,
+                    float* norm_mean1, float* norm_std1, long long* norm_count, int* had_fin, unsigned* ticket,
+                    float* rew_slab, float* cost_slab, unsigned char* flags, float* epfin, double* workspace,
+                    int* nonfinite, void* stream) {
+    OSB_CHECK_ARG(O > 0 && N > 0 && T > 0 && t >= 0 && t < T, "bad dims / step index");
+    OSB_CHECK_ARG(next_obs && rew && cost && terminated && truncated && s_raw && final_raw && rew_slab && cost_slab &&
+                  flags && epfin && workspace && nonfinite, "bad argument");
+    ExtObs x{next_obs, rew, cost, terminated, truncated, final_obs, final_mask, workspace, nonfinite};
+    EnvState st{s_raw, final_raw, nullptr, nullptr, nullptr, ep_ret, ep_cost, ep_len, nullptr};
+    NormState ns{norm_mean, norm_sumsq, norm_std, norm_mean1, norm_std1, norm_count, nullptr, nullptr, nullptr, had_fin, ticket};
+    Slabs sl{nullptr, nullptr, nullptr, rew_slab, cost_slab, nullptr, nullptr, nullptr, nullptr, flags, epfin};
+    return launch_observe(x, st, ns, sl, O, N, T, t, obs_normalize, 0, stream);
+}
+
+int osb_ext_act(int O, int A, int obs_normalize, int N, int T, int t, unsigned env_id_offset, float* s_raw,
+                float* final_raw, float* norm_mean, float* norm_std, float* norm_mean1, float* norm_std1,
+                long long* norm_count, float* obs, float* act, float* logp, float* val_r, float* val_c, float* boot_r,
+                float* boot_c, unsigned char* flags, const float* theta, const float* eps, unsigned noise_seed,
+                unsigned global_step, const float* act_lo, const float* act_hi, float* act_env, int precision,
+                void* stream) {
+    OSB_CHECK_ARG(O > 0 && A > 0 && A <= OUTP && N > 0 && T > 0, "bad dims (need 0 < A <= 16)");
+    OSB_CHECK_ARG(t >= 0 && t <= T, "step index out of range");
+    OSB_CHECK_ARG(t == T || (act_lo && act_hi && act_env), "act_lo / act_hi / act_env are required for t < T");
+    StepArgs p{};
+    p.es = EnvSpec{O, A, 0, 0u, 0u, env_id_offset, 0.f, obs_normalize};
+    p.st = EnvState{s_raw, final_raw, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    p.ns = NormState{norm_mean, nullptr, norm_std, norm_mean1, norm_std1, norm_count, nullptr, nullptr, nullptr, nullptr, nullptr};
+    p.sl = Slabs{obs, act, logp, nullptr, nullptr, val_r, val_c, boot_r, boot_c, flags, nullptr};
+    p.sa = SauteSpec{nullptr, 1.f, 1.f, 0.f, 1.f};
+    p.et = EarlySpec{nullptr, 0.f};
+    p.theta = theta; p.eps = eps; p.noise_seed = noise_seed; p.global_step = global_step;
+    p.t = t; p.T = T; p.N = N; p.is_tail = (t == T) ? 1 : 0; p.precision = precision;
+    p.bar_ctr = nullptr; p.bar_flag = nullptr; p.dbg = nullptr;
+    p.act_lo = act_lo; p.act_hi = act_hi; p.act_env = act_env;
+    return launch_step<true>(p, (cudaStream_t)stream);
 }
 
 }  // extern "C"
