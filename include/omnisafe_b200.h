@@ -202,7 +202,7 @@ int osb_minibatch_grad(const float* theta, int O, int A, const float* obs, const
                        float* stats_part, const int* stop_flag, void* stream);
 /* Tensor-core variant of osb_minibatch_grad: the tile GEMMs run as tf32 wgmma with accumulator image
  * accumulators (operands fp32 in 128B-swizzled smem tiles; transposed activations produced by
- * role-swapped MMAs).  Same arguments and outputs; O <= 64, A <= 16.  This is arithmetic mode
+ * role-swapped MMAs).  Same arguments and outputs; O <= 512, A <= 16.  This is arithmetic mode
  * `precision = 1` of osb_ppo_update_epoch; mode 0 is the exact-fp32 FMA parity path.
  * gpart / stats_part rows: osb_tc_grid_blocks(mb_count, net_mask) -- a third of the device's SMs per network
  * when several networks share the launch, up to all of them (at most 148) when net_mask names a single network. */
@@ -216,7 +216,7 @@ int osb_minibatch_grad_tc(const float* theta, int O, int A, const float* obs, co
                           const float* lagrange, const float* logstd_old, int net_mask, float* gpart,
                           float* stats_part, const int* stop_flag, void* stream);
 /* Split-bf16 ("bf16x3") parity-grade tensor-core variant (csrc/update_x3.cu): every GEMM = six bf16 wgmma
- * MMAs over the three bf16 pieces of its fp32 operands, fp32 accumulate; O <= 64, loss kinds 0 / 1 / 3. */
+ * MMAs over the three bf16 pieces of its fp32 operands, fp32 accumulate; O <= 64, A <= 16, every loss kind. */
 int osb_minibatch_grad_x3(const float* theta, int O, int A, const float* obs, const float* act,
                           const float* logp, const float* adv_r, const float* adv_c,
                           const float* tv_r, const float* tv_c, const float* mu_old,
@@ -234,7 +234,7 @@ int osb_actor_eval(const float* theta_actor, int O, int A, const float* obs, con
                    const float* logstd_old, const float* moments, const float* lagrange,
                    long long total, int stride, float* mu_store, double* workspace, double* out,
                    void* stream);
-/* Tensor-core (TF32 wgmma) variant of osb_actor_eval: same arguments / outputs, O <= 64. */
+/* Tensor-core (TF32 wgmma) variant of osb_actor_eval: same arguments / outputs, O <= 512. */
 int osb_actor_eval_tc(const float* theta_actor, int O, int A, const float* obs, const float* act,
                       const float* logp, const float* adv_r, const float* adv_c, const float* mu_old,
                       const float* logstd_old, const float* moments, const float* lagrange,
@@ -265,7 +265,7 @@ int osb_actor_eval_x3(const float* theta_actor, int O, int A, const float* obs, 
 int osb_fvp_grid_blocks(long long total, int stride);
 int osb_fvp_partials(const float* theta_actor, const float* vec, int O, int A, const float* obs,
                      long long total, int stride, float* gpart, void* stream);
-/* Tensor-core Fisher-vector product (O <= 64): forward-mode tangent pass with stacked [W;V] weight
+/* Tensor-core Fisher-vector product (O <= 512): forward-mode tangent pass with stacked [W;V] weight
  * tiles (dmu scratch [total][A]) + the actor backward of the tensor-core gradient kernel.
  * gpart: osb_tc_grid_blocks(rows, 1) rows of P_actor floats, rows = ceil(total / stride);
  * stats_scratch: that many * 24 floats.  Reduce with osb_reduce_partials. */

@@ -2,6 +2,7 @@
 // C-ABI call so that no Python sits between the ~800 kernel launches, plus a thin dlopen binding of
 // NCCL for the per-step flat gradient all-reduce (utils/distributed.py:L142-228 avg_grads/dist_avg).
 #include "common.cuh"
+#include "loss.cuh"
 #include "mlp.cuh"
 #include <dlfcn.h>
 #include <stdlib.h>
@@ -191,16 +192,14 @@ int osb_ppo_update_epoch(float* theta, float* grad, float* adam_m, float* adam_v
     OSB_CUDA(cudaMemsetAsync(kl_state, 0, 4 * sizeof(float), s));
     OSB_CUDA(cudaMemsetAsync(train_stats, 0, 3 * 8 * sizeof(float), s));
     int rc;
-    // precision 1 = TF32 wgmma tiles (O <= 64, loss kinds 0/1/3); otherwise the fp32 FMA parity path
-    // precision 2 = split-bf16 ("bf16x3") wgmma tiles: fp32-level results on the tensor cores (O <= 64,
-    // loss kinds 0/1/3)
-    const bool use_x3 = precision == 2 && O <= 64 && (loss_kind == 0 || loss_kind == 1 || loss_kind == 2 || loss_kind == 3 || loss_kind == 5);   // FOCOPS (2), P3O (5): stepwise launches
-    const bool use_x3e = precision == 2 && O <= 64;
+    // precision 1 = TF32 wgmma tiles (O <= 512); precision 2 = split-bf16 ("bf16x3") wgmma tiles: fp32-level results
+    // on the tensor cores (O <= 64); otherwise the fp32 FMA parity path.  Every mode takes loss kinds 0-3 and 5.
+    const bool use_x3 = precision == 2 && O <= 64;
     const bool use_tc = precision == 1 && O <= 512;
     const bool train_actor = (net_mask & 1) != 0;
     if (train_actor) {
         OSB_CHECK_ARG(mu_old && logstd_old && eval_ws && eval_out, "actor update needs mu_old/logstd_old/eval buffers");
-        rc = (use_x3e ? osb_actor_eval_x3 : use_tc ? osb_actor_eval_tc : osb_actor_eval)(theta, O, A, obs, nullptr, nullptr, nullptr, nullptr,
+        rc = (use_x3 ? osb_actor_eval_x3 : use_tc ? osb_actor_eval_tc : osb_actor_eval)(theta, O, A, obs, nullptr, nullptr, nullptr, nullptr,
                                                           nullptr, nullptr, nullptr, nullptr, total, 1, mu_old,
                                                           nullptr, nullptr, stream);
         if (rc) return rc;
@@ -209,7 +208,7 @@ int osb_ppo_update_epoch(float* theta, float* grad, float* adam_m, float* adam_v
     const float gscale = 1.0f / (float)world_size;
     // bf16x3 + (one rank | NVLink peer exchange): the whole iteration is one persistent kernel with the optimiser inside
     const bool p2p_ok = world_size > 1 && peer_buf && peer_flag && p2p_error;
-    const bool fuse_x3 = use_x3 && loss_kind != 2 && loss_kind != 5 && (world_size == 1 || p2p_ok) && !getenv("OSB_X3_NO_FUSE");
+    const bool fuse_x3 = use_x3 && !osb::loss_two_pass(loss_kind) && (world_size == 1 || p2p_ok) && !getenv("OSB_X3_NO_FUSE");
     for (int it = 0; it < update_iters; ++it) {
         const int* perm_it = perm ? perm + (size_t)it * total : nullptr;
         if (fuse_x3) {
@@ -258,7 +257,7 @@ int osb_ppo_update_epoch(float* theta, float* grad, float* adam_m, float* adam_v
             if (rc) return rc;
         }
         if (train_actor) {
-            rc = (use_x3e ? osb_actor_eval_x3 : use_tc ? osb_actor_eval_tc : osb_actor_eval)(theta, O, A, obs, act, logp, adv_r, adv_c, mu_old,
+            rc = (use_x3 ? osb_actor_eval_x3 : use_tc ? osb_actor_eval_tc : osb_actor_eval)(theta, O, A, obs, act, logp, adv_r, adv_c, mu_old,
                                                               logstd_old, moments, lagrange, total, 1, nullptr,
                                                               eval_ws, eval_out, stream);
             if (rc) return rc;

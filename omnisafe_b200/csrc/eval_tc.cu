@@ -3,6 +3,7 @@
 // sum KL(old||new), sum ratio*adv, sum ratio*adv_c, sum ratio, count, sum ratio*adv_r in fp64.
 // Two CTAs per SM (~100 KB smem each) so one CTA's epilogue overlaps the other's MMA.
 #include "common.cuh"
+#include "loss.cuh"
 #include "mlp.cuh"
 #include "umma.cuh"
 
@@ -31,7 +32,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) actor_eval_tc_kernel(EvalTcArgs p
     float* sB1 = reinterpret_cast<float*>(smem_raw + pad + 2 * EBUF + 2 * 16384 + 4096);
     float* sB2 = sB1 + 64;
     float* sB3 = sB2 + 64;      // [16]
-    float* sLs = sB3 + 16;      // logstd_new[16], sigma_new[16], logstd_old[16], sigma_old[16]
+    float* sLs = sB3 + 16;      // [64] evaluation policy constants of csrc/loss.cuh
     double* sRedD = reinterpret_cast<double*>(sLs + 64);       // [4][8]
     long long* sRow = reinterpret_cast<long long*>(sRedD + 32);  // [128]
     __shared__ uint64_t bar;
@@ -67,9 +68,8 @@ __global__ void __launch_bounds__(NTHREADS, 2) actor_eval_tc_kernel(EvalTcArgs p
     if (tid < 64) { sB1[tid] = __ldg(theta + L.off_b1 + tid); sB2[tid] = __ldg(theta + L.off_b2 + tid); }
     if (tid < 16) {
         sB3[tid] = (tid < A) ? __ldg(theta + L.off_b3 + tid) : 0.f;
-        const float ls = (tid < A) ? __ldg(theta + L.off_logstd + tid) : 0.f;
-        const float lo = (tid < A && p.logstd_old) ? __ldg(p.logstd_old + tid) : 0.f;
-        sLs[tid] = ls; sLs[16 + tid] = expf(ls); sLs[32 + tid] = lo; sLs[48 + tid] = expf(lo);
+        stage_eval_policy(sLs, tid, (tid < A) ? __ldg(theta + L.off_logstd + tid) : 0.f,
+                          (tid < A && p.logstd_old) ? __ldg(p.logstd_old + tid) : 0.f);
     }
     if (tid == 0) { mbar_init(&bar, 1); mbar_init_fence(); }
     __syncthreads();
@@ -81,9 +81,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) actor_eval_tc_kernel(EvalTcArgs p
     const int nchunks = (O + 63) >> 6;
     const long long nrows = (p.total + p.stride - 1) / p.stride;
     const long long ntiles = (nrows + ET - 1) / ET;
-    const float lam = p.lagrange ? __ldg(p.lagrange) : 0.f;
-    float m_r = 0.f, s_r = 1.f, m_c = 0.f;
-    if (p.moments) { m_r = __ldg(p.moments); s_r = __ldg(p.moments + 1); m_c = __ldg(p.moments + 2); }
+    const AdvNorm an = adv_norm(p.moments, p.lagrange);
     double acc[6] = {0, 0, 0, 0, 0, 0};
 
     for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -157,22 +155,10 @@ __global__ void __launch_bounds__(NTHREADS, 2) actor_eval_tc_kernel(EvalTcArgs p
                 if (p.mu_store) {
                     for (int a = 0; a < A; ++a) p.mu_store[row * A + a] = o16[a] + sB3[a];
                 } else {
-                    float logp_new = 0.f, kl = 0.f;
+                    float mu[16];
 #pragma unroll
-                    for (int a = 0; a < 16; ++a)
-                        if (a < A) {
-                            const float mu = o16[a] + sB3[a], sd = sLs[16 + a], so = sLs[48 + a];
-                            const float d = pa[a] - mu;
-                            logp_new += -(d * d) / (2.f * sd * sd) - sLs[a] - 0.9189385332046727f;
-                            const float vr = (so / sd) * (so / sd);
-                            const float t1 = (pm[a] - mu) / sd;
-                            kl += 0.5f * (vr + t1 * t1 - 1.f - logf(vr));
-                        }
-                    const float ratio = expf(logp_new - plogp);
-                    const float adv_r = (padvr - m_r) / s_r, adv_c = padvc - m_c;
-                    const float adv = (adv_r - lam * adv_c) / (1.f + lam);
-                    acc[0] += (double)kl; acc[1] += (double)(ratio * adv); acc[2] += (double)(ratio * adv_c);
-                    acc[3] += (double)ratio; acc[4] += 1.0; acc[5] += (double)(ratio * adv_r);
+                    for (int a = 0; a < 16; ++a) mu[a] = o16[a] + sB3[a];
+                    eval_sample<16>(an, A, mu, pa, pm, plogp, padvr, padvc, sLs, acc);
                 }
             }
         }
@@ -200,26 +186,6 @@ int osb_actor_eval_tc(const float* theta_actor, int O, int A, const float* obs, 
                       const float* logp, const float* adv_r, const float* adv_c, const float* mu_old,
                       const float* logstd_old, const float* moments, const float* lagrange,
                       long long total, int stride, float* mu_store, double* workspace, double* out,
-                      void* stream);
-__global__ void eval_tc_reduce_kernel(const double* __restrict__ part, int nblocks, double* __restrict__ out) {
-    // 32 groups x 8 statistics: group g sums CTAs g, g+32, ... ; the 32 group sums fold in a fixed order
-    __shared__ double sh[32][8];
-    const int q = threadIdx.x & 7, g = threadIdx.x >> 3;
-    double s = 0.0;
-    for (int b = g; b < nblocks; b += 32) s += part[(size_t)b * 8 + q];
-    sh[g][q] = s;
-    __syncthreads();
-    if (threadIdx.x < 8) {
-        double t = 0.0;
-        for (int i = 0; i < 32; ++i) t += sh[i][threadIdx.x];
-        out[threadIdx.x] = (threadIdx.x < 6) ? t : 0.0;
-    }
-}
-
-int osb_actor_eval_tc(const float* theta_actor, int O, int A, const float* obs, const float* act,
-                      const float* logp, const float* adv_r, const float* adv_c, const float* mu_old,
-                      const float* logstd_old, const float* moments, const float* lagrange,
-                      long long total, int stride, float* mu_store, double* workspace, double* out,
                       void* stream) {
     OSB_CHECK_ARG(theta_actor && obs && total > 0 && stride > 0 && O > 0 && O <= 512 && A > 0 && A <= 16, "bad argument (O <= 512)");
     OSB_CHECK_ARG(mu_store || (act && logp && adv_r && adv_c && mu_old && logstd_old && workspace && out), "null input");
@@ -239,11 +205,7 @@ int osb_actor_eval_tc(const float* theta_actor, int O, int A, const float* obs, 
     cudaStream_t s = (cudaStream_t)stream;
     actor_eval_tc_kernel<<<blocks, NTHREADS, smem, s>>>(p);
     OSB_LAUNCH_CHECK();
-    if (!mu_store) {
-        eval_tc_reduce_kernel<<<1, 256, 0, s>>>(workspace, blocks, out);
-        OSB_LAUNCH_CHECK();
-    }
-    return OSB_OK;
+    return mu_store ? OSB_OK : eval_reduce(workspace, blocks, out, s);
 }
 
 }  // extern "C"

@@ -7,6 +7,7 @@
 // that layer's MMAs have completed), so a CTA needs 48 KB + 54 KB of weights and TWO CTAs share an SM: one
 // CTA's epilogue runs under the other's MMAs.
 #include "common.cuh"
+#include "loss.cuh"
 #include "mlp.cuh"
 #include "x3.cuh"
 
@@ -40,7 +41,7 @@ __global__ void __launch_bounds__(EX_NT, 2) actor_eval_x3_kernel(EvalX3Args p) {
     float* sB1 = reinterpret_cast<float*>(gbase + EXO_MISC);
     float* sB2 = sB1 + 64;
     float* sB3 = sB2 + 64;      // [16]
-    float* sLs = sB3 + 16;      // logstd_new[16], sigma_new[16], logstd_old[16], sigma_old[16]
+    float* sLs = sB3 + 16;      // [64] evaluation policy constants of csrc/loss.cuh
     double* sRedD = reinterpret_cast<double*>(gbase + EXO_RED);
     long long* sRow = reinterpret_cast<long long*>(gbase + EXO_ROWS);
     const uint32_t bar = sbase + EXO_BAR;
@@ -81,9 +82,8 @@ __global__ void __launch_bounds__(EX_NT, 2) actor_eval_x3_kernel(EvalX3Args p) {
     if (tid < 64) { sB1[tid] = __ldg(theta + L.off_b1 + tid); sB2[tid] = __ldg(theta + L.off_b2 + tid); }
     if (tid < 16) {
         sB3[tid] = (tid < A) ? __ldg(theta + L.off_b3 + tid) : 0.f;
-        const float ls = (tid < A) ? __ldg(theta + L.off_logstd + tid) : 0.f;
-        const float lo = (tid < A && p.logstd_old) ? __ldg(p.logstd_old + tid) : 0.f;
-        sLs[tid] = ls; sLs[16 + tid] = expf(ls); sLs[32 + tid] = lo; sLs[48 + tid] = expf(lo);
+        stage_eval_policy(sLs, tid, (tid < A) ? __ldg(theta + L.off_logstd + tid) : 0.f,
+                          (tid < A && p.logstd_old) ? __ldg(p.logstd_old + tid) : 0.f);
     }
     if (tid == 0) {
         asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar), "r"(1u) : "memory");
@@ -100,9 +100,7 @@ __global__ void __launch_bounds__(EX_NT, 2) actor_eval_x3_kernel(EvalX3Args p) {
 
     const long long nrows = (p.total + p.stride - 1) / p.stride;
     const long long ntiles = (nrows + EX_T - 1) / EX_T;
-    const float lam = p.lagrange ? __ldg(p.lagrange) : 0.f;
-    float m_r = 0.f, s_r = 1.f, m_c = 0.f;
-    if (p.moments) { m_r = __ldg(p.moments); s_r = __ldg(p.moments + 1); m_c = __ldg(p.moments + 2); }
+    const AdvNorm an = adv_norm(p.moments, p.lagrange);
     double acc[6] = {0, 0, 0, 0, 0, 0};
     const int xm = tid >> 1, xh = (tid & 1) << 5;          // X gather: row, 32-column half
     const bool vec = (O & 3) == 0;
@@ -189,22 +187,10 @@ __global__ void __launch_bounds__(EX_NT, 2) actor_eval_x3_kernel(EvalX3Args p) {
                 if (p.mu_store) {
                     for (int a = 0; a < A; ++a) p.mu_store[row * A + a] = o16[a] + sB3[a];
                 } else {
-                    float logp_new = 0.f, kl = 0.f;
+                    float mu[16];
 #pragma unroll
-                    for (int a = 0; a < 16; ++a)
-                        if (a < A) {
-                            const float mu = o16[a] + sB3[a], sd = sLs[16 + a], so = sLs[48 + a];
-                            const float d = pa[a] - mu;
-                            logp_new += -(d * d) / (2.f * sd * sd) - sLs[a] - 0.9189385332046727f;
-                            const float vr = (so / sd) * (so / sd);
-                            const float t1 = (pm[a] - mu) / sd;
-                            kl += 0.5f * (vr + t1 * t1 - 1.f - logf(vr));
-                        }
-                    const float ratio = expf(logp_new - plogp);
-                    const float adv_r = (padvr - m_r) / s_r, adv_c = padvc - m_c;
-                    const float adv = (adv_r - lam * adv_c) / (1.f + lam);
-                    acc[0] += (double)kl; acc[1] += (double)(ratio * adv); acc[2] += (double)(ratio * adv_c);
-                    acc[3] += (double)ratio; acc[4] += 1.0; acc[5] += (double)(ratio * adv_r);
+                    for (int a = 0; a < 16; ++a) mu[a] = o16[a] + sB3[a];
+                    eval_sample<16>(an, A, mu, pa, pm, plogp, padvr, padvc, sLs, acc);
                 }
             }
         }
@@ -226,21 +212,6 @@ __global__ void __launch_bounds__(EX_NT, 2) actor_eval_x3_kernel(EvalX3Args p) {
 using namespace osb;
 
 extern "C" {
-
-// 32 groups x 8 statistics: group g sums CTAs g, g+32, ... ; the 32 group sums fold in a fixed order
-__global__ void eval_x3_reduce_kernel(const double* __restrict__ part, int nblocks, double* __restrict__ out) {
-    __shared__ double sh[32][8];
-    const int q = threadIdx.x & 7, g = threadIdx.x >> 3;
-    double s = 0.0;
-    for (int b = g; b < nblocks; b += 32) s += part[(size_t)b * 8 + q];
-    sh[g][q] = s;
-    __syncthreads();
-    if (threadIdx.x < 8) {
-        double t = 0.0;
-        for (int i = 0; i < 32; ++i) t += sh[i][threadIdx.x];
-        out[threadIdx.x] = (threadIdx.x < 6) ? t : 0.0;
-    }
-}
 
 // Split-bf16 variant of osb_actor_eval (O <= 64): same arguments and outputs, fp32-level accuracy.
 int osb_actor_eval_x3(const float* theta_actor, int O, int A, const float* obs, const float* act,
@@ -266,11 +237,7 @@ int osb_actor_eval_x3(const float* theta_actor, int O, int A, const float* obs, 
     cudaStream_t s = (cudaStream_t)stream;
     actor_eval_x3_kernel<<<blocks, EX_NT, smem, s>>>(p);
     OSB_LAUNCH_CHECK();
-    if (!mu_store) {
-        eval_x3_reduce_kernel<<<1, 256, 0, s>>>(workspace, blocks, out);
-        OSB_LAUNCH_CHECK();
-    }
-    return OSB_OK;
+    return mu_store ? OSB_OK : eval_reduce(workspace, blocks, out, s);
 }
 
 }  // extern "C"

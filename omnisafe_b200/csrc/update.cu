@@ -5,94 +5,35 @@
 // Replaces the reference's
 //   PolicyGradient._update minibatch body   algorithms/on_policy/base/policy_gradient.py:L369-381
 //   _update_reward_critic / _update_cost_critic / _update_actor            :L407-524
-//   PPO._loss_pi                            algorithms/on_policy/base/ppo.py:L35-87
-//   PPOLag._compute_adv_surrogate           naive_lagrange/ppo_lag.py:L82-102
-//   PolicyGradient._loss_pi (plain ratio)   base/policy_gradient.py:L551-588
-//   CPO._loss_pi_cost                       second_order/cpo.py:L182-212
-//   FOCOPS._loss_pi                         first_order/focops.py:L62-108
-//   KL early-stop evaluation                base/policy_gradient.py:L383-397
 //   NaturalPG._fvp                          base/natural_pg.py:L74-119  (analytic Gauss-Newton form)
+// with the per-sample losses and evaluation statistics of csrc/loss.cuh.
 //
 // One CTA = one network x a strided set of 128-sample tiles.  Samples are addressed by slab row
-// (t*N + i); a minibatch is a window [mb_start, mb_start + mb_count) of a permutation that is either
-// supplied (parity mode: the reference's DataLoader order) or generated in-kernel by a keyed
-// Feistel bijection (fast mode) -- no gather buffers are materialised.
+// (t*N + i); a minibatch is a window of the sample order of csrc/loss.cuh (supplied permutation or
+// keyed Feistel bijection) -- no gather buffers are materialised.
 #include "common.cuh"
+#include "loss.cuh"
 #include "mlp.cuh"
 
 namespace osb {
 
 constexpr int UT = 128;  // samples per tile
-
-enum LossKind { LOSS_PPO_CLIP = 0, LOSS_RATIO = 1, LOSS_FOCOPS = 2, LOSS_COST = 3, LOSS_P3O = 5 };   // 4 = FVP (tensor-core kernel)
-
-struct Batch {
-    const float* obs;     // [rows][O]
-    const float* act;     // [rows][A]
-    const float* logp;    // [rows]
-    const float* adv_r;   // [rows] raw advantages (standardised on the fly with `moments`)
-    const float* adv_c;   // [rows]
-    const float* tv_r;    // [rows]
-    const float* tv_c;    // [rows]
-    const float* mu_old;  // [rows][A] (FOCOPS / KL), may be null
-    const float* moments; // [4] mean_r, std_r + 1e-8, mean_c, 1
-    const int* perm;      // [total] slab rows in minibatch order, or null (Feistel)
-    long long total;      // number of samples the permutation ranges over
-    unsigned perm_seed;   // Feistel key (fast mode)
-    long long mb_start;   // window of the permutation processed by this launch
-    int mb_count;
-};
-
-// Keyed bijection on [0, n): 4-round Feistel on the enclosing power-of-four domain + cycle walking.
-__device__ __forceinline__ unsigned long long feistel_perm(unsigned long long k, unsigned long long n,
-                                                           unsigned seed) {
-    int bits = 2;
-    while ((1ull << bits) < n) bits += 2;
-    const int half = bits >> 1;
-    const unsigned mask = (1u << half) - 1u;
-    unsigned long long x = k;
-    do {
-        unsigned l = (unsigned)(x >> half) & mask, r = (unsigned)x & mask;
-#pragma unroll
-        for (int round = 0; round < 4; ++round) {
-            const unsigned f = mix32(r ^ (seed + 0x9E3779B9u * (unsigned)(round + 1))) & mask;
-            const unsigned nl = r;
-            r = l ^ f;
-            l = nl;
-        }
-        x = ((unsigned long long)l << half) | r;
-    } while (x >= n);
-    return x;
-}
-
-struct LossCfg {
-    int kind;             // LossKind for the actor
-    float clip;           // PPO clip
-    float entropy_coef;
-    float focops_lam, focops_eta;
-    const float* lagrange;   // device scalar lambda or null (-> 0): adv = (adv_r - l*adv_c)/(1+l)
-    const float* logstd_old; // [A] (FOCOPS), may be null
-    const float* focops_mask_mean;  // device scalar mean_i 1{KL_i <= eta} of this minibatch (FOCOPS pass 2)
-};
+static_assert(OUTP == 16, "policy constants of csrc/loss.cuh are laid out 16 per field");
 
 // stats slots (per launch, summed over CTAs in fixed order)
-enum { ST_LOSS_PI = 0, ST_RATIO = 1, ST_LOSS_VR = 2, ST_LOSS_VC = 3, ST_KL = 4, ST_COUNT = 5, ST_N = 8 };
+enum { ST_N = 8 };
 
 struct GradArgs {
     Batch b;
-    LossCfg lc;
+    LossParams lc;
     const float* theta;
     float* gpart;          // [gridDim.x][P] partial gradients (each CTA writes its network's segment)
     float* stats_part;     // [gridDim.x][3][ST_N]
     const int* stop_flag;  // device flag: non-zero -> kernel is a no-op (KL early stop)
     int O, A, P;
     int net_mask;          // bit n set -> process network n
-    int forward_only;      // FOCOPS pass 1: actor forward + statistics only (no gradients written)
+    int forward_only;      // pass 1 of FOCOPS / P3O: actor forward + statistics only (no gradients written)
 };
-
-__device__ __forceinline__ long long sample_row(const Batch& b, long long k) {
-    return b.perm ? (long long)b.perm[k] : (long long)feistel_perm((unsigned long long)k, (unsigned long long)b.total, b.perm_seed);
-}
 
 // gather chunk kc of the observation rows of a tile into sX (zero padded)
 __device__ __forceinline__ void gather_obs(const float* __restrict__ obs, const long long* sRow, int O,
@@ -138,7 +79,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p)
     float* sD = base;  base += UT * LD;
     float* sO = base;  base += UT * LDO;
     float* sRed = base; base += 4 * 2 * OUTP;
-    float* sLs = base;  base += 3 * OUTP;   // logstd, sigma, accumulated dlogstd
+    float* sPol = base; base += 3 * OUTP;   // policy constants of csrc/loss.cuh
+    float* sOld = base; base += 2 * OUTP;
+    float* sDls = base; base += OUTP;       // accumulated d log_std
     float* sStat = base; base += ST_N;
     long long* sRow = reinterpret_cast<long long*>(base);  // [UT] (8-byte aligned: offsets are even)
 
@@ -154,10 +97,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p)
     load_net_rest<true>(theta, L, W);
     load_w1_chunk(theta, L, 0, W);
     if (threadIdx.x < OUTP) {
-        const float ls = (net == 0 && threadIdx.x < A) ? __ldg(theta + L.off_logstd + threadIdx.x) : 0.f;
-        sLs[threadIdx.x] = ls;
-        sLs[OUTP + threadIdx.x] = expf(ls);
-        sLs[2 * OUTP + threadIdx.x] = 0.f;
+        const bool act = net == 0 && threadIdx.x < A;
+        stage_policy(sPol, threadIdx.x, act ? __ldg(theta + L.off_logstd + threadIdx.x) : 0.f);
+        stage_policy_old(sOld, threadIdx.x, (act && p.lc.logstd_old) ? __ldg(p.lc.logstd_old + threadIdx.x) : 0.f);
+        sDls[threadIdx.x] = 0.f;
     }
     if (threadIdx.x < ST_N) sStat[threadIdx.x] = 0.f;
 
@@ -169,8 +112,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p)
 #pragma unroll
         for (int b = 0; b < 4; ++b) { aw1[a][b] = 0.f; aw2[a][b] = 0.f; }
     }
-    const float lam = (p.lc.lagrange != nullptr) ? __ldg(p.lc.lagrange) : 0.f;
-    const float m_r = __ldg(p.b.moments + 0), s_r = __ldg(p.b.moments + 1), m_c = __ldg(p.b.moments + 2);
+    const AdvNorm an = adv_norm(p.b.moments, p.lc.lagrange);
     bool first_tile = true;
 
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -207,85 +149,26 @@ __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p)
                     sO[m * LDO] = 2.f * d * inv_b;                       // d mse / d v
                     for (int o = 1; o < OUTP; ++o) sO[m * LDO + o] = 0.f;
                 } else {
-                    float logp_new = 0.f, kl = 0.f;
-                    float diff[OUTP];
+                    float mu[OUTP], act[OUTP];
 #pragma unroll
                     for (int a = 0; a < OUTP; ++a) {
-                        diff[a] = 0.f;
+                        mu[a] = 0.f; act[a] = 0.f;
                         if (a < A) {
-                            const float mu = sO[m * LDO + a];
-                            const float sd = sLs[OUTP + a];
-                            const float d = __ldg(p.b.act + row * A + a) - mu;
-                            diff[a] = d;
-                            logp_new += -(d * d) / (2.f * sd * sd) - sLs[a] - 0.9189385332046727f;
+                            mu[a] = sO[m * LDO + a];
+                            act[a] = __ldg(p.b.act + row * A + a);
                         }
                     }
-                    const float ratio = expf(logp_new - __ldg(p.b.logp + row));
-                    const float adv_r = (__ldg(p.b.adv_r + row) - m_r) / s_r;
-                    const float adv_c = __ldg(p.b.adv_c + row) - m_c;
-                    float adv = (adv_r - lam * adv_c) / (1.f + lam);
-                    float dlogp = 0.f, loss = 0.f, dmask = 0.f;
-                    if (p.lc.kind == LOSS_PPO_CLIP || p.lc.kind == LOSS_P3O) {
-                        const float rc = fminf(fmaxf(ratio, 1.f - p.lc.clip), 1.f + p.lc.clip);
-                        const float s1 = ratio * adv, s2 = rc * adv;
-                        loss = -fminf(s1, s2);
-                        dlogp = (s1 <= s2) ? -adv * ratio * inv_b : 0.f;
-                        if (p.lc.kind == LOSS_P3O) {
-                            // P3O (penalty_function/p3o.py:L48-91): + kappa * relu(mean_j(ratio_j adv_c_j) + Jc - limit).
-                            // gate = kappa when the minibatch mean (forward-only pass 1) makes the relu active.
-                            // Statistic slot 2: pass 1 -> ratio * adv_c; pass 2 -> the penalty term (Loss/Loss_pi_cost),
-                            // slot 0 stays the PPO part as the reference logs Loss/Loss_pi (ppo.py:L80-86).
-                            const bool pass2 = p.lc.focops_mask_mean != nullptr;
-                            const float gate = pass2 ? __ldg(p.lc.focops_mask_mean) : 0.f;
-                            dlogp += gate * adv_c * ratio * inv_b;
-                            kl = pass2 ? gate * (ratio * adv_c + p.lc.focops_eta) : ratio * adv_c;
-                        }
-                    } else if (p.lc.kind == LOSS_RATIO) {
-                        loss = -ratio * adv;
-                        dlogp = -adv * ratio * inv_b;
-                    } else if (p.lc.kind == LOSS_COST) {
-                        loss = ratio * adv_c;
-                        dlogp = adv_c * ratio * inv_b;
-                    } else {
-                        // FOCOPS.  The reference forms (kl[b,1] - ratio[b]*adv[b]/lam) * mask[b,1] and takes
-                        // the mean of the resulting [b,b] matrix (first_order/focops.py:L85-89), i.e.
-                        //   loss = mean_i(mask_i kl_i) - mean_i(mask_i) * mean_j(ratio_j adv_j) / lam ;
-                        // mean_i(mask_i) of this minibatch comes from the forward-only pass 1.
-                        for (int a = 0; a < A; ++a) {
-                            const float so = expf(__ldg(p.lc.logstd_old + a)), sn = sLs[OUTP + a];
-                            const float dm = sO[m * LDO + a] - __ldg(p.b.mu_old + row * A + a);
-                            kl += (__ldg(p.lc.logstd_old + a) - sLs[a]) + (sn * sn + dm * dm) / (2.f * so * so) - 0.5f;
-                        }
-                        dmask = (kl <= p.lc.focops_eta) ? 1.f : 0.f;
-                        const float mbar = p.lc.focops_mask_mean ? __ldg(p.lc.focops_mask_mean) : dmask;
-                        loss = kl * dmask - mbar * ratio * adv / p.lc.focops_lam;
-                        dlogp = -mbar * adv * ratio / p.lc.focops_lam * inv_b;
-                        st[4] = dmask;
-                    }
-                    st[0] = loss; st[1] = ratio; st[2] = kl; st[3] = 1.f;
-#pragma unroll
-                    for (int a = 0; a < OUTP; ++a) {
-                        float dmu = 0.f;
-                        if (a < A) {
-                            const float sd = sLs[OUTP + a];
-                            const float iv = 1.f / (sd * sd);
-                            dmu = dlogp * diff[a] * iv;                    // d logp / d mu
-                            dls[a] = dlogp * (diff[a] * diff[a] * iv - 1.f);   // d logp / d log_std
-                            if (p.lc.kind == LOSS_FOCOPS) {
-                                const float so = expf(__ldg(p.lc.logstd_old + a));
-                                const float dm = sO[m * LDO + a] - __ldg(p.b.mu_old + row * A + a);
-                                dmu += dmask * inv_b * dm / (so * so);
-                                dls[a] += dmask * inv_b * (sd * sd / (so * so) - 1.f);
-                            }
-                        }
-                        diff[a] = dmu;
-                    }
-#pragma unroll
-                    for (int a = 0; a < OUTP; ++a) sO[m * LDO + a] = diff[a];
+                    // dOUT overwrites OUT: columns >= A are zero
+                    for (int a = A; a < OUTP; ++a) sO[m * LDO + a] = 0.f;
+                    actor_sample_loss<true, OUTP>(p.lc, an, A, inv_b, mu, act,
+                                                                       [&](int a) { return __ldg(p.lc.mu_old + row * A + a); },
+                                                                       __ldg(p.b.logp + row),
+                                                                       __ldg(p.b.adv_r + row), __ldg(p.b.adv_c + row), sPol, sOld, st,
+                                                                       [&](int a, float dm, float dl) { sO[m * LDO + a] = dm; dls[a] = dl; });
                 }
             }
             block_reduce_store<5>(st, sRed, sStat, true);
-            if (net == 0) block_reduce_store<OUTP>(dls, sRed, sLs + 2 * OUTP, true);
+            if (net == 0) block_reduce_store<OUTP>(dls, sRed, sDls, true);
         }
         __syncthreads();
         if (p.forward_only) { first_tile = false; continue; }
@@ -414,11 +297,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p)
         if (threadIdx.x < L.out) gout[L.off_b3 + threadIdx.x] = ab3;
         __syncthreads();
         if (net == 0 && threadIdx.x < A) {
-            float g = sLs[2 * OUTP + threadIdx.x];
+            float g = sDls[threadIdx.x];
             // entropy bonus: loss -= coef * mean(entropy); d entropy / d log_std_a = 1 (mean over A)
-            // (only PPO._loss_pi / FOCOPS._loss_pi carry the entropy term)
-            if (blockIdx.x == 0 && (p.lc.kind == LOSS_PPO_CLIP || p.lc.kind == LOSS_FOCOPS || p.lc.kind == LOSS_P3O))
-                g -= p.lc.entropy_coef / (float)A;
+            if (blockIdx.x == 0 && loss_has_entropy(p.lc.kind)) g -= p.lc.entropy_coef / (float)A;
             gout[L.off_logstd + threadIdx.x] = g;
         }
         if (threadIdx.x < ST_N)
@@ -431,6 +312,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p)
 // or reduce  sum KL(old||new), sum ratio*adv, sum ratio*adv_c, sum ratio  (fp64 partials).
 struct EvalArgs {
     Batch b;                 // perm unused: rows [0, total)
+    const float* mu_old;     // [rows][A]
     const float* theta;      // actor parameters (first segment of flat theta, or a trial vector)
     const float* logstd_old; // [A]
     const float* lagrange;   // lambda or null
@@ -448,7 +330,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) actor_eval_kernel(EvalArgs p) {
     float* sH1 = base; base += UT * LD;
     float* sH2 = base; base += UT * LD;
     float* sO = base;  base += UT * LDO;
-    float* sLs = base; base += 2 * OUTP;
+    float* sPol = base; base += 4 * OUTP;   // evaluation policy constants of csrc/loss.cuh
     double* sRedD = reinterpret_cast<double*>(base); base += 2 * 4 * 8;
     long long* sRow = reinterpret_cast<long long*>(base);
 
@@ -458,15 +340,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) actor_eval_kernel(EvalArgs p) {
     load_net_rest<false>(p.theta, L, W);
     load_w1_chunk(p.theta, L, 0, W);
     if (threadIdx.x < OUTP) {
-        const float ls = threadIdx.x < A ? __ldg(p.theta + L.off_logstd + threadIdx.x) : 0.f;
-        sLs[threadIdx.x] = ls;
-        sLs[OUTP + threadIdx.x] = expf(ls);
+        const bool act = threadIdx.x < A;
+        stage_eval_policy(sPol, threadIdx.x, act ? __ldg(p.theta + L.off_logstd + threadIdx.x) : 0.f,
+                          (act && p.logstd_old) ? __ldg(p.logstd_old + threadIdx.x) : 0.f);
     }
     const long long nrows = (p.b.total + p.stride - 1) / p.stride;
     const long long ntiles = (nrows + UT - 1) / UT;
-    const float lam = p.lagrange ? __ldg(p.lagrange) : 0.f;
-    float m_r = 0.f, s_r = 1.f, m_c = 0.f;
-    if (p.b.moments) { m_r = __ldg(p.b.moments); s_r = __ldg(p.b.moments + 1); m_c = __ldg(p.b.moments + 2); }
+    const AdvNorm an = adv_norm(p.b.moments, p.lagrange);
     double acc[6] = {0, 0, 0, 0, 0, 0};  // kl, ratio*adv, ratio*adv_c, ratio, count, ratio*adv_r(std)
 
     for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -488,24 +368,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) actor_eval_kernel(EvalArgs p) {
                 if (p.mu_store) {
                     for (int a = 0; a < A; ++a) p.mu_store[row * A + a] = sO[threadIdx.x * LDO + a];
                 } else {
-                    float logp_new = 0.f, kl = 0.f;
-                    for (int a = 0; a < A; ++a) {
-                        const float mu = sO[threadIdx.x * LDO + a], sd = sLs[OUTP + a];
-                        const float d = __ldg(p.b.act + row * A + a) - mu;
-                        logp_new += -(d * d) / (2.f * sd * sd) - sLs[a] - 0.9189385332046727f;
-                        // KL(old || new) per dim (torch.distributions.kl._kl_normal_normal)
-                        const float lso = __ldg(p.logstd_old + a);
-                        const float so = expf(lso);
-                        const float vr = (so / sd) * (so / sd);
-                        const float t1 = (__ldg(p.b.mu_old + row * A + a) - mu) / sd;
-                        kl += 0.5f * (vr + t1 * t1 - 1.f - logf(vr));
+                    float mu[OUTP], act[OUTP], mo[OUTP];
+#pragma unroll
+                    for (int a = 0; a < OUTP; ++a) {
+                        mu[a] = 0.f; act[a] = 0.f; mo[a] = 0.f;
+                        if (a < A) {
+                            mu[a] = sO[threadIdx.x * LDO + a];
+                            act[a] = __ldg(p.b.act + row * A + a);
+                            mo[a] = __ldg(p.mu_old + row * A + a);
+                        }
                     }
-                    const float ratio = expf(logp_new - __ldg(p.b.logp + row));
-                    const float adv_r = (__ldg(p.b.adv_r + row) - m_r) / s_r;
-                    const float adv_c = __ldg(p.b.adv_c + row) - m_c;
-                    const float adv = (adv_r - lam * adv_c) / (1.f + lam);
-                    acc[0] += (double)kl; acc[1] += (double)(ratio * adv); acc[2] += (double)(ratio * adv_c);
-                    acc[3] += (double)ratio; acc[4] += 1.0; acc[5] += (double)(ratio * adv_r);
+                    eval_sample<OUTP>(an, A, mu, act, mo, __ldg(p.b.logp + row), __ldg(p.b.adv_r + row),
+                                      __ldg(p.b.adv_c + row), sPol, acc);
                 }
             }
         }
@@ -523,21 +397,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) actor_eval_kernel(EvalArgs p) {
             for (int ww = 0; ww < NTHREADS / 32; ++ww) s += sRedD[ww * 8 + threadIdx.x];
             p.part[(size_t)blockIdx.x * 8 + threadIdx.x] = s;
         }
-    }
-}
-
-__global__ void eval_reduce_kernel(const double* __restrict__ part, int nblocks, double* __restrict__ out) {
-    // 32 groups x 8 statistics: group g sums CTAs g, g+32, ... ; the 32 group sums fold in a fixed order
-    __shared__ double sh[32][8];
-    const int q = threadIdx.x & 7, g = threadIdx.x >> 3;
-    double s = 0.0;
-    for (int b = g; b < nblocks; b += 32) s += part[(size_t)b * 8 + q];
-    sh[g][q] = s;
-    __syncthreads();
-    if (threadIdx.x < 8) {
-        double t = 0.0;
-        for (int i = 0; i < 32; ++i) t += sh[i][threadIdx.x];
-        out[threadIdx.x] = t;
     }
 }
 
@@ -797,29 +656,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) fvp_kernel(FvpArgs p) {
     }
 }
 
-// Pass 1 of the two-pass losses, fixed order over the actor's per-CTA statistics:
-//   FOCOPS: out = mean_i mask_i                      (slot 4 / slot 3)
-//   P3O:    out = kappa if mean_i(ratio_i adv_c_i) + (Jc - limit) > 0 else 0   (slot 2 / slot 3; F.relu gate)
-__global__ void focops_mask_mean_kernel(const float* __restrict__ stats_part, int nblocks, float* __restrict__ out,
-                                        const int* __restrict__ stop_flag, int kind, float kappa, float jc_minus_limit) {
-    if (threadIdx.x != 0 || (stop_flag && *stop_flag)) return;
-    const int slot = (kind == LOSS_P3O) ? 2 : 4;
-    float m = 0.f, n = 0.f;
-    for (int b = 0; b < nblocks; ++b) { m += stats_part[((size_t)b * 3) * ST_N + slot]; n += stats_part[((size_t)b * 3) * ST_N + 3]; }
-    const float mean = n > 0.f ? m / n : 0.f;
-    out[0] = (kind == LOSS_P3O) ? ((mean + jc_minus_limit > 0.f) ? kappa : 0.f) : mean;
-}
-
 }  // namespace osb
 
 using namespace osb;
 
 static size_t grad_smem_bytes() {
-    size_t f = NETSMEM_FLOATS_BWD + 4 * UT * LD + UT * LDO + 4 * 2 * OUTP + 3 * OUTP + ST_N;
+    size_t f = NETSMEM_FLOATS_BWD + 4 * UT * LD + UT * LDO + 4 * 2 * OUTP + 6 * OUTP + ST_N;
     return f * sizeof(float) + UT * sizeof(long long) + 16;
 }
 static size_t eval_smem_bytes() {
-    size_t f = NETSMEM_FLOATS_FWD + 3 * UT * LD + UT * LDO + 2 * OUTP + 2 * 2 * 4 * 8;
+    size_t f = NETSMEM_FLOATS_FWD + 3 * UT * LD + UT * LDO + 4 * OUTP + 2 * 2 * 4 * 8;
     return f * sizeof(float) + UT * sizeof(long long) + 16;
 }
 static size_t fvp_smem_bytes() {
@@ -846,14 +692,13 @@ int osb_minibatch_grad(const float* theta, int O, int A, const float* obs, const
                        float entropy_coef, float focops_lam, float focops_eta,
                        const float* lagrange, const float* logstd_old, int net_mask, float* gpart,
                        float* stats_part, const int* stop_flag, void* stream) {
-    static float* d_mask_mean = nullptr;   // FOCOPS scratch scalar
     OSB_CHECK_ARG(theta && obs && act && logp && adv_r && adv_c && tv_r && tv_c && moments, "null input");
     OSB_CHECK_ARG(O > 0 && A > 0 && A <= OUTP && mb_count > 0 && total > 0, "bad dims");
     OSB_CHECK_ARG(mb_start >= 0 && mb_start + mb_count <= total, "minibatch window out of range");
     OSB_CHECK_ARG(loss_kind != LOSS_FOCOPS || (mu_old && logstd_old), "FOCOPS needs mu_old/logstd_old");
     GradArgs p;
-    p.b = Batch{obs, act, logp, adv_r, adv_c, tv_r, tv_c, mu_old, moments, perm, total, perm_seed, mb_start, mb_count};
-    p.lc = LossCfg{loss_kind, clip, entropy_coef, focops_lam, focops_eta, lagrange, logstd_old, nullptr};
+    p.b = Batch{obs, act, logp, adv_r, adv_c, tv_r, tv_c, moments, perm, total, perm_seed, mb_start, mb_count, 0};
+    p.lc = LossParams{loss_kind, clip, entropy_coef, focops_lam, focops_eta, lagrange, mu_old, logstd_old, nullptr};
     p.forward_only = 0;
     p.theta = theta; p.gpart = gpart; p.stats_part = stats_part; p.stop_flag = stop_flag;
     p.O = O; p.A = A;
@@ -866,18 +711,13 @@ int osb_minibatch_grad(const float* theta, int O, int A, const float* obs, const
         attr = true;
     }
     dim3 grid(osb_update_grid_blocks(mb_count), 3);
-    if ((loss_kind == LOSS_FOCOPS || loss_kind == LOSS_P3O) && (net_mask & 1)) {
-        // pass 1: actor forward only -> mean mask of the minibatch (FOCOPS: the reference's [b,1] x [b]
-        // broadcast) or the relu gate of the minibatch-mean cost surrogate (P3O)
-        if (!d_mask_mean) OSB_CUDA(cudaMalloc(&d_mask_mean, sizeof(float)));
+    if (loss_two_pass(loss_kind) && (net_mask & 1)) {   // pass 1: actor forward only
         GradArgs q = p;
         q.forward_only = 1; q.net_mask = 1;
         minibatch_grad_kernel<<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(q);
         OSB_LAUNCH_CHECK();
-        focops_mask_mean_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(stats_part, (int)grid.x, d_mask_mean, stop_flag,
-                                                                    loss_kind, focops_lam, focops_eta);
-        OSB_LAUNCH_CHECK();
-        p.lc.focops_mask_mean = d_mask_mean;
+        const int rc = pass1_gate(stats_part, (int)grid.x, stop_flag, p.lc, (cudaStream_t)stream);
+        if (rc) return rc;
     }
     minibatch_grad_kernel<<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(p);
     OSB_LAUNCH_CHECK();
@@ -895,8 +735,8 @@ int osb_actor_eval(const float* theta_actor, int O, int A, const float* obs, con
     OSB_CHECK_ARG(theta_actor && obs && total > 0 && stride > 0, "bad argument");
     OSB_CHECK_ARG(mu_store || (act && logp && adv_r && adv_c && mu_old && logstd_old && workspace && out), "null input");
     EvalArgs p;
-    p.b = Batch{obs, act, logp, adv_r, adv_c, nullptr, nullptr, mu_old, moments, nullptr, total, 0u, 0, 0};
-    p.theta = theta_actor; p.logstd_old = logstd_old; p.lagrange = lagrange; p.mu_store = mu_store;
+    p.b = Batch{obs, act, logp, adv_r, adv_c, nullptr, nullptr, moments, nullptr, total, 0u, 0, 0, 0};
+    p.mu_old = mu_old; p.theta = theta_actor; p.logstd_old = logstd_old; p.lagrange = lagrange; p.mu_store = mu_store;
     p.part = workspace; p.O = O; p.A = A; p.stride = stride;
     const size_t smem = eval_smem_bytes();
     static bool attr = false;
@@ -911,11 +751,7 @@ int osb_actor_eval(const float* theta_actor, int O, int A, const float* obs, con
     cudaStream_t s = (cudaStream_t)stream;
     actor_eval_kernel<<<blocks, NTHREADS, smem, s>>>(p);
     OSB_LAUNCH_CHECK();
-    if (!mu_store) {
-        eval_reduce_kernel<<<1, 256, 0, s>>>(workspace, blocks, out);
-        OSB_LAUNCH_CHECK();
-    }
-    return OSB_OK;
+    return mu_store ? OSB_OK : eval_reduce(workspace, blocks, out, s);
 }
 
 int osb_fvp_grid_blocks(long long total, int stride) {

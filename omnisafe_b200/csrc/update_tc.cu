@@ -7,7 +7,7 @@
 // needed with the sample index as the contraction dimension (weight gradients) is produced a second
 // time in transposed form by a role-swapped MMA (D^T = W * X^T) instead of a transposed copy:
 //
-//   per 128-sample tile and network (O <= 64):
+//   per 128-sample tile and network (O <= 64; for 64 < O <= 512, MMA1 / MMA2 and MMA9 loop over 64-column chunks of X):
 //     MMA1  Z1    [s][n] = X  * W1^T      -> H1    = tanh(.+b1)            (A operand of layer 2)
 //     MMA2  Z1^T  [n][s] = W1 * X^T       -> H1^T                          (B operand of dW2)
 //     MMA3  Z2    [s][n] = H1 * W2^T      -> H2
@@ -19,6 +19,7 @@
 //     MMA9  dW1   [j][o] += dZ1^T * X     (accumulator images kept across tiles)
 //   dW3, the bias gradients and d log_std stay on the CUDA cores (tiny).
 #include "common.cuh"
+#include "loss.cuh"
 #include "mlp.cuh"
 #include "umma.cuh"
 
@@ -29,53 +30,20 @@ using namespace umma;
 constexpr int TT = 128;                 // samples per tile
 constexpr uint32_t BUF = TT * 64 * 4;   // 32 KB activation buffer ([128][64] or [64][128] fp32)
 
-enum TcLoss { TC_PPO_CLIP = 0, TC_RATIO = 1, TC_FOCOPS = 2, TC_COST = 3, TC_FVP = 4, TC_P3O = 5 };   // TC_FVP: dOUT supplied (Fisher-vector product)
-
-struct TcBatch {
-    const float* obs; const float* act; const float* logp; const float* adv_r; const float* adv_c;
-    const float* tv_r; const float* tv_c; const float* moments; const int* perm;
-    long long total; unsigned perm_seed; long long mb_start; int mb_count;
-    int identity_stride;     // > 0: row = (mb_start + local) * identity_stride (full-batch passes, fvp_sample_freq)
-};
 struct TcArgs {
-    TcBatch b;
-    int kind; float clip, entropy_coef;
-    const float* lagrange;
+    Batch b;
+    LossParams lc;
     const float* theta;
     float* gpart;
     float* stats_part;
     const int* stop_flag;
     int O, A, P, net_mask;
-    const float* fvp_dmu;    // TC_FVP: tangent of mu per row [total][A] (fvp_tangent_tc_kernel)
-    const float* fvp_vec;    // TC_FVP: direction v (log_std block of F v)
-    float fvp_scale;         // TC_FVP: 1 / (rows * A)
-    const float* mu_old;     // TC_FOCOPS: old-policy mean per row, log_std of the old policy,
-    const float* logstd_old;
-    float focops_lam, focops_eta;
-    const float* focops_mask_mean;   // device scalar mean_i 1{KL_i <= eta} of this minibatch (pass 2) or null (pass 1)
-    int forward_only;        // pass 1 of FOCOPS: statistics only, no backward
+    const float* fvp_dmu;    // LOSS_FVP: tangent of mu per row [total][A] (fvp_tangent_tc_kernel)
+    const float* fvp_vec;    // LOSS_FVP: direction v (log_std block of F v)
+    float fvp_scale;         // LOSS_FVP: 1 / (rows * A)
+    int forward_only;        // pass 1 of FOCOPS / P3O: statistics only, no backward
     float* acc;              // accumulator images, one [128][TC_COLS] per CTA
 };
-
-__device__ __forceinline__ unsigned long long tc_feistel(unsigned long long k, unsigned long long n, unsigned seed) {
-    int bits = 2;
-    while ((1ull << bits) < n) bits += 2;
-    const int half = bits >> 1;
-    const unsigned mask = (1u << half) - 1u;
-    unsigned long long x = k;
-    do {
-        unsigned l = (unsigned)(x >> half) & mask, r = (unsigned)x & mask;
-#pragma unroll
-        for (int round = 0; round < 4; ++round) {
-            const unsigned f = mix32(r ^ (seed + 0x9E3779B9u * (unsigned)(round + 1))) & mask;
-            const unsigned nl = r;
-            r = l ^ f;
-            l = nl;
-        }
-        x = ((unsigned long long)l << half) | r;
-    } while (x >= n);
-    return x;
-}
 
 // accumulator column map (csrc/umma.cuh)
 constexpr uint32_t C_Z = 0, C_ZT = 64, C_ZT2 = 192, C_OUT = 320, C_DW2 = 336, C_DW1 = 400, C_DW3 = 464, TC_COLS = 480;
@@ -127,12 +95,13 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
     float* sB1 = reinterpret_cast<float*>(smem_raw + pad + 5 * BUF + 3 * 16384 + 4096 + 8192);
     float* sB2 = sB1 + 64;
     float* sB3 = sB2 + 64;            // [16]
-    float* sLs = sB3 + 16;            // logstd[16], sigma[16], dlogstd acc[16]
-    float* sStat = sLs + 48;          // [8]
+    float* sPol = sB3 + 16;           // [48] policy constants of csrc/loss.cuh
+    float* sStat = sPol + 48;         // [8]
     float* sRed = sStat + 8;          // [4 * 8 + 4 * 16 + 4 * 16]
     float* sB3acc = sRed + 160;       // [16]
-    float* sOld = sB3acc + 16;        // old policy: log_std[16], 1 / sigma_old^2 [16]
-    long long* sRowBuf = reinterpret_cast<long long*>(sOld + 32);   // [2][128] rows of this / the next tile
+    float* sOld = sB3acc + 16;        // [32] old-policy constants of csrc/loss.cuh
+    float* sDls = sOld + 32;          // [16] accumulated d log_std
+    long long* sRowBuf = reinterpret_cast<long long*>(sDls + 16);   // [2][128] rows of this / the next tile
     __shared__ uint64_t bar;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -180,10 +149,10 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
     if (tid < 64) { sB1[tid] = __ldg(theta + L.off_b1 + tid); sB2[tid] = __ldg(theta + L.off_b2 + tid); }
     if (tid < 16) {
         sB3[tid] = (tid < L.out) ? __ldg(theta + L.off_b3 + tid) : 0.f;
-        const float ls = (net == 0 && tid < A) ? __ldg(theta + L.off_logstd + tid) : 0.f;
-        sLs[tid] = ls; sLs[16 + tid] = expf(ls); sLs[32 + tid] = 0.f;
-        const float lso = (net == 0 && tid < A && p.logstd_old) ? __ldg(p.logstd_old + tid) : 0.f;
-        sOld[tid] = lso; sOld[16 + tid] = expf(-2.f * lso);
+        const bool act = net == 0 && tid < A;
+        stage_policy(sPol, tid, act ? __ldg(theta + L.off_logstd + tid) : 0.f);
+        stage_policy_old(sOld, tid, (act && p.lc.logstd_old) ? __ldg(p.lc.logstd_old + tid) : 0.f);
+        sDls[tid] = 0.f;
     }
     if (tid < 8) sStat[tid] = 0.f;
     if (tid < 16) sB3acc[tid] = 0.f;
@@ -193,10 +162,8 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
     const uint32_t lane_base = (uint32_t)(q * 32) << 16;
     uint32_t phase = 0;
 
-    const float lam = (p.lagrange != nullptr) ? __ldg(p.lagrange) : 0.f;
-    float m_r = 0.f, s_r = 1.f, m_c = 0.f;
-    if (p.b.moments) { m_r = __ldg(p.b.moments + 0); s_r = __ldg(p.b.moments + 1); m_c = __ldg(p.b.moments + 2); }
-    const bool is_fvp = EXT && p.kind == TC_FVP, is_focops = EXT && p.kind == TC_FOCOPS, is_p3o = EXT && p.kind == TC_P3O;
+    const AdvNorm an = adv_norm(p.b.moments, p.lc.lagrange);
+    const bool is_fvp = EXT && p.lc.kind == LOSS_FVP, is_focops = EXT && p.lc.kind == LOSS_FOCOPS;
     float ab1 = 0.f, ab2 = 0.f;
     bool first_tile = true;
     const int s_row = 32 * q + lane;       // sample row of this thread in [s][.] accumulators
@@ -208,13 +175,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
     auto tile_rows = [&](int tile, long long* dst) {
         if (tid < TT) {
             const int local = tile * TT + tid;
-            long long row = -1;
-            if (local < p.b.mb_count) {
-                const long long k = p.b.mb_start + local;
-                if (p.b.identity_stride > 0) row = k * p.b.identity_stride;
-                else row = p.b.perm ? (long long)p.b.perm[k] : (long long)tc_feistel((unsigned long long)k, (unsigned long long)p.b.total, p.b.perm_seed);
-            }
-            dst[tid] = row;
+            dst[tid] = (local < p.b.mb_count) ? sample_row(p.b, p.b.mb_start + local) : -1;
         }
     };
     float4 xpre[4];
@@ -404,22 +365,17 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             }
         }
         // per-sample scalars: issue the global loads before blocking on the MMA
-        float pf_act[16], pf_mu[16], pf_logp = 0.f, pf_advr = 0.f, pf_advc = 0.f, pf_tv = 0.f;
+        float pf_act[16], pf_logp = 0.f, pf_advr = 0.f, pf_advc = 0.f, pf_tv = 0.f;
         const long long prow = (h == 0) ? sRow[s_row] : -1;
         {
 #pragma unroll
-            for (int a = 0; a < 16; ++a) { pf_act[a] = 0.f; pf_mu[a] = 0.f; }
+            for (int a = 0; a < 16; ++a) pf_act[a] = 0.f;
             if (prow >= 0) {
                 if (net == 0) {
                     const float* src = is_fvp ? p.fvp_dmu : p.b.act;
 #pragma unroll
                     for (int a = 0; a < 16; ++a)
                         if (a < A) pf_act[a] = __ldg(src + prow * A + a);
-                    if (is_focops) {
-#pragma unroll
-                        for (int a = 0; a < 16; ++a)
-                            if (a < A) pf_mu[a] = __ldg(p.mu_old + prow * A + a);
-                    }
                     if (!is_fvp) {
                         pf_logp = __ldg(p.b.logp + prow);
                         pf_advr = __ldg(p.b.adv_r + prow);
@@ -450,73 +406,18 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
 #pragma unroll
                     for (int a = 0; a < 16; ++a)
                         if (a < A) {
-                            const float sd = sLs[16 + a];
+                            const float sd = sPol[16 + a];
                             d32[a] = pf_act[a] / (sd * sd) * p.fvp_scale;
                         }
                     st[3] = 1.f;
                 } else {
-                    float logp_new = 0.f, diff[16];
+                    float mu[16];
 #pragma unroll
-                    for (int a = 0; a < 16; ++a) {
-                        diff[a] = 0.f;
-                        if (a < A) {
-                            const float sd = sLs[16 + a];
-                            const float d = pf_act[a] - (o16[a] + sB3[a]);
-                            diff[a] = d;
-                            logp_new += -(d * d) / (2.f * sd * sd) - sLs[a] - 0.9189385332046727f;
-                        }
-                    }
-                    const float ratio = expf(logp_new - pf_logp);
-                    const float adv_r = (pf_advr - m_r) / s_r;
-                    const float adv_c = pf_advc - m_c;
-                    const float adv = (adv_r - lam * adv_c) / (1.f + lam);
-                    float dlogp, loss, dmask = 0.f;
-                    if (is_focops) {
-                        // first_order/focops.py:L62-108 incl. the reference's [b,1] x [b] broadcast:
-                        //   loss = mean_i(mask_i kl_i) - mean_i(mask_i) * mean_j(ratio_j adv_j) / lam
-                        float kl = 0.f;
-#pragma unroll
-                        for (int a = 0; a < 16; ++a)
-                            if (a < A) {
-                                const float sn = sLs[16 + a];
-                                const float dm = (o16[a] + sB3[a]) - pf_mu[a];
-                                kl += (sOld[a] - sLs[a]) + (sn * sn + dm * dm) * 0.5f * sOld[16 + a] - 0.5f;
-                            }
-                        dmask = (kl <= p.focops_eta) ? 1.f : 0.f;
-                        const float mbar = p.focops_mask_mean ? __ldg(p.focops_mask_mean) : dmask;
-                        loss = kl * dmask - mbar * ratio * adv / p.focops_lam;
-                        dlogp = -mbar * adv * ratio / p.focops_lam * inv_b;
-                        st[2] = kl; st[4] = dmask;
-                    } else if (p.kind == TC_PPO_CLIP || is_p3o) {
-                        const float rc = fminf(fmaxf(ratio, 1.f - p.clip), 1.f + p.clip);
-                        const float s1 = ratio * adv, s2 = rc * adv;
-                        loss = -fminf(s1, s2);
-                        dlogp = (s1 <= s2) ? -adv * ratio * inv_b : 0.f;
-                        if (is_p3o) {   // + kappa * relu(mean(ratio adv_c) + Jc - limit), gate from pass 1
-                            const bool pass2 = p.focops_mask_mean != nullptr;
-                            const float gate = pass2 ? __ldg(p.focops_mask_mean) : 0.f;
-                            dlogp += gate * adv_c * ratio * inv_b;
-                            st[2] = pass2 ? gate * (ratio * adv_c + p.focops_eta) : ratio * adv_c;   // Loss/Loss_pi_cost
-                        }
-                    } else if (p.kind == TC_RATIO) {
-                        loss = -ratio * adv; dlogp = -adv * ratio * inv_b;
-                    } else {
-                        loss = ratio * adv_c; dlogp = adv_c * ratio * inv_b;
-                    }
-                    st[0] = loss; st[1] = ratio; st[3] = 1.f;
-#pragma unroll
-                    for (int a = 0; a < 16; ++a)
-                        if (a < A) {
-                            const float sd = sLs[16 + a];
-                            const float iv = 1.f / (sd * sd);
-                            d32[a] = dlogp * diff[a] * iv;
-                            dls[a] = dlogp * (diff[a] * diff[a] * iv - 1.f);
-                            if (is_focops) {
-                                const float dm = (o16[a] + sB3[a]) - pf_mu[a];
-                                d32[a] += dmask * inv_b * dm * sOld[16 + a];
-                                dls[a] += dmask * inv_b * (sd * sd * sOld[16 + a] - 1.f);
-                            }
-                        }
+                    for (int a = 0; a < 16; ++a) mu[a] = o16[a] + sB3[a];
+                    actor_sample_loss<EXT, 16>(p.lc, an, A, inv_b, mu, pf_act,
+                                                                    [&](int a) { return __ldg(p.lc.mu_old + prow * A + a); }, pf_logp, pf_advr,
+                                                                    pf_advc, sPol, sOld, st,
+                                                                    [&](int a, float dm, float dl) { d32[a] = dm; dls[a] = dl; });
                 }
             }
             store_row32(B4, s_row, 0, TT, d32);
@@ -544,13 +445,13 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
         if (tid < 5) sStat[tid] += sRed[tid] + sRed[8 + tid] + sRed[16 + tid] + sRed[24 + tid];
         if (net == 0 && tid >= 32 && tid < 48) {
             const int a = tid - 32;
-            sLs[32 + a] += sRed[32 + a] + sRed[48 + a] + sRed[64 + a] + sRed[80 + a];
+            sDls[a] += sRed[32 + a] + sRed[48 + a] + sRed[64 + a] + sRed[80 + a];
         }
         if (tid >= 64 && tid < 64 + L.out) {
             const int a = tid - 64;
             sB3acc[a] += sRed[96 + a] + sRed[112 + a] + sRed[128 + a] + sRed[144 + a];
         }
-        if (EXT && p.forward_only) {   // FOCOPS / P3O pass 1: statistics only
+        if (EXT && p.forward_only) {   // pass 1: statistics only
             if (CHUNKED) { if (has_next) load_chunk(sRowNext, 0); }
             else if (vec && has_next) prefetch_x(sRowNext);
             first_tile = false;
@@ -712,8 +613,8 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
         if (tid < 64) { gout[L.off_b1 + tid] = ab1; gout[L.off_b2 + tid] = ab2; }
         if (tid < L.out) gout[L.off_b3 + tid] = sB3acc[tid];
         if (net == 0 && tid < A) {
-            float g = sLs[32 + tid];
-            if (blockIdx.x == 0 && (p.kind == TC_PPO_CLIP || is_p3o || is_focops)) g -= p.entropy_coef / (float)A;
+            float g = sDls[tid];
+            if (blockIdx.x == 0 && loss_has_entropy<EXT>(p.lc.kind)) g -= p.lc.entropy_coef / (float)A;
             // log_std block of the Fisher matrix: (2/A) v, counted once (natural_pg.py:L74-119, analytic form)
             if (is_fvp) g = (blockIdx.x == 0) ? 2.f / (float)A * __ldg(p.fvp_vec + L.off_logstd + tid) : 0.f;
             gout[L.off_logstd + tid] = g;
@@ -731,7 +632,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
 //     [Z1 | X V1^T]            = X   [W1;V1]^T
 //     [Z2 | H1 V2^T + dH1 W2^T] = H1 [W2;V2]^T  (+)  dH1 W2^T   (accumulated into the right half)
 //     dmu                       = H2 V3^T + dH2 W3^T + vb3
-// The backward half (J^T diag(sigma^-2) dmu) is minibatch_grad_tc_kernel with kind TC_FVP.
+// The backward half (J^T diag(sigma^-2) dmu) is minibatch_grad_tc_kernel with kind LOSS_FVP.
 struct FvpTanArgs {
     const float* obs; long long total; int stride;
     const float* theta; const float* vec; float* dmu; int O, A;
@@ -999,7 +900,7 @@ __global__ void __launch_bounds__(NTC, 1) fvp_tangent_tc_kernel(FvpTanArgs p) {
 using namespace osb;
 
 static size_t tc_smem_bytes() {
-    return 1024 + 5 * (size_t)BUF + 3 * 16384 + 4096 + 8192 + (64 + 64 + 16 + 48 + 8 + 160 + 16 + 32) * 4 + 2 * 128 * 8 + 64;
+    return 1024 + 5 * (size_t)BUF + 3 * 16384 + 4096 + 8192 + (64 + 64 + 16 + 48 + 8 + 160 + 16 + 32 + 16) * 4 + 2 * 128 * 8 + 64;
 }
 static size_t fvp_tan_smem_bytes() {
     return 1024 + 3 * (size_t)BUF + 2 * 32768 + 8192 + (4 * 64 + 16) * 4 + 2 * 128 * 8 + 64;
@@ -1019,7 +920,7 @@ static int launch_grad_tc(TcArgs& p, int nblocks, cudaStream_t stream) {
     dim3 grid(nblocks, single ? 1 : 3);
     p.acc = acc_scratch(ACC_UPDATE_TC, (size_t)grid.x * grid.y * 128 * TC_COLS * sizeof(float));
     if (!p.acc) return OSB_ERR_CUDA;
-    const bool ext = p.kind == TC_FOCOPS || p.kind == TC_FVP || p.kind == TC_P3O;
+    const bool ext = loss_two_pass(p.lc.kind) || p.lc.kind == LOSS_FVP;
     if (p.O > 64) {
         if (ext) minibatch_grad_tc_kernel<true, true><<<grid, NTC, smem, stream>>>(p);
         else minibatch_grad_tc_kernel<true, false><<<grid, NTC, smem, stream>>>(p);
@@ -1043,19 +944,7 @@ int osb_tc_grid_blocks(long long rows, int net_mask) {
     return (int)(tiles < cap ? tiles : cap);
 }
 
-// FOCOPS pass 1 -> mean_i mask_i of the minibatch (stats slot 4 / slot 3 of the actor), fixed order.
-//   P3O:    out = kappa if mean_i(ratio_i adv_c_i) + (Jc - limit) > 0 else 0   (slot 2 / slot 3)
-__global__ void tc_mask_mean_kernel(const float* __restrict__ stats_part, int nblocks, float* __restrict__ out,
-                                    const int* __restrict__ stop_flag, int kind, float kappa, float jc_minus_limit) {
-    if (threadIdx.x != 0 || (stop_flag && *stop_flag)) return;
-    const int slot = (kind == TC_P3O) ? 2 : 4;
-    float m = 0.f, n = 0.f;
-    for (int b = 0; b < nblocks; ++b) { m += stats_part[((size_t)b * 3) * 8 + slot]; n += stats_part[((size_t)b * 3) * 8 + 3]; }
-    const float mean = n > 0.f ? m / n : 0.f;
-    out[0] = (kind == TC_P3O) ? ((mean + jc_minus_limit > 0.f) ? kappa : 0.f) : mean;
-}
-
-// Tensor-core (TF32 wgmma) variant of osb_minibatch_grad: same arguments, O <= 64, A <= 16.
+// Tensor-core (TF32 wgmma) variant of osb_minibatch_grad: same arguments, O <= 512, A <= 16.
 // gpart holds osb_tc_grid_blocks(mb_count, net_mask) rows of P floats.
 int osb_minibatch_grad_tc(const float* theta, int O, int A, const float* obs, const float* act,
                           const float* logp, const float* adv_r, const float* adv_c,
@@ -1065,39 +954,32 @@ int osb_minibatch_grad_tc(const float* theta, int O, int A, const float* obs, co
                           float entropy_coef, float focops_lam, float focops_eta,
                           const float* lagrange, const float* logstd_old, int net_mask, float* gpart,
                           float* stats_part, const int* stop_flag, void* stream) {
-    static float* d_mask_mean = nullptr;   // FOCOPS scratch scalar
     OSB_CHECK_ARG(theta && obs && act && logp && adv_r && adv_c && tv_r && tv_c && moments, "null input");
     OSB_CHECK_ARG(O > 0 && O <= 512 && A > 0 && A <= 16 && mb_count > 0 && total > 0, "tensor-core path needs O <= 512, A <= 16");
     OSB_CHECK_ARG(mb_start >= 0 && mb_start + mb_count <= total, "minibatch window out of range");
-    OSB_CHECK_ARG((loss_kind >= 0 && loss_kind <= 3) || loss_kind == TC_P3O, "loss kind");
-    OSB_CHECK_ARG(loss_kind != TC_FOCOPS || (mu_old && logstd_old), "FOCOPS needs mu_old/logstd_old");
+    OSB_CHECK_ARG((loss_kind >= 0 && loss_kind <= 3) || loss_kind == LOSS_P3O, "loss kind");
+    OSB_CHECK_ARG(loss_kind != LOSS_FOCOPS || (mu_old && logstd_old), "FOCOPS needs mu_old/logstd_old");
     OSB_CHECK_ARG(net_mask > 0 && net_mask < 8, "net_mask");
     TcArgs p;
-    p.b = TcBatch{obs, act, logp, adv_r, adv_c, tv_r, tv_c, moments, perm, total, perm_seed, mb_start, mb_count, 0};
-    p.kind = loss_kind; p.clip = clip; p.entropy_coef = entropy_coef; p.lagrange = lagrange;
+    p.b = Batch{obs, act, logp, adv_r, adv_c, tv_r, tv_c, moments, perm, total, perm_seed, mb_start, mb_count, 0};
+    p.lc = LossParams{loss_kind, clip, entropy_coef, focops_lam, focops_eta, lagrange, mu_old, logstd_old, nullptr};
     p.theta = theta; p.gpart = gpart; p.stats_part = stats_part; p.stop_flag = stop_flag;
     p.O = O; p.A = A; p.P = actor_layout(O, A).size + 2 * critic_layout(O, A).size; p.net_mask = net_mask;
     p.fvp_dmu = nullptr; p.fvp_vec = nullptr; p.fvp_scale = 0.f;
-    p.mu_old = mu_old; p.logstd_old = logstd_old; p.focops_lam = focops_lam; p.focops_eta = focops_eta;
-    p.focops_mask_mean = nullptr; p.forward_only = 0;
+    p.forward_only = 0;
     const int nb = osb_tc_grid_blocks(mb_count, net_mask);
-    if ((loss_kind == TC_FOCOPS || loss_kind == TC_P3O) && (net_mask & 1)) {
-        // pass 1: actor forward only -> mean mask of the minibatch (the reference's [b,1] x [b] broadcast)
-        if (!d_mask_mean) OSB_CUDA(cudaMalloc(&d_mask_mean, sizeof(float)));
+    if (loss_two_pass(loss_kind) && (net_mask & 1)) {   // pass 1: actor forward only
         TcArgs q = p;
         q.forward_only = 1; q.net_mask = 1;
         const int nb1 = osb_tc_grid_blocks(mb_count, 1);
         int rc = launch_grad_tc(q, nb1, (cudaStream_t)stream);
         if (rc) return rc;
-        tc_mask_mean_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(stats_part, nb1, d_mask_mean, stop_flag, loss_kind,
-                                                                focops_lam, focops_eta);
-        OSB_LAUNCH_CHECK();
-        p.focops_mask_mean = d_mask_mean;
+        if ((rc = pass1_gate(stats_part, nb1, stop_flag, p.lc, (cudaStream_t)stream))) return rc;
     }
     return launch_grad_tc(p, nb, (cudaStream_t)stream);
 }
 
-// Tensor-core Fisher-vector product partials (O <= 64): tangent forward (dmu scratch [total][A]) then
+// Tensor-core Fisher-vector product partials (O <= 512): tangent forward (dmu scratch [total][A]) then
 // the actor backward of minibatch_grad_tc_kernel.  gpart: osb_tc_grid_blocks(rows, 1) rows of
 // P_actor floats; stats_scratch: that many * 24 floats.  Reduce with osb_reduce_partials.
 int osb_fvp_partials_tc(const float* theta_actor, const float* vec, int O, int A, const float* obs,
@@ -1125,13 +1007,12 @@ int osb_fvp_partials_tc(const float* theta_actor, const float* vec, int O, int A
         OSB_LAUNCH_CHECK();
     }
     TcArgs p;
-    p.b = TcBatch{obs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, total, 0u, 0, (int)nrows, stride};
-    p.kind = TC_FVP; p.clip = 0.f; p.entropy_coef = 0.f; p.lagrange = nullptr;
+    p.b = Batch{obs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, total, 0u, 0, (int)nrows, stride};
+    p.lc = LossParams{LOSS_FVP, 0.f, 0.f, 1.f, 0.f, nullptr, nullptr, nullptr, nullptr};
     p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch; p.stop_flag = nullptr;
     p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
     p.fvp_dmu = dmu; p.fvp_vec = vec; p.fvp_scale = 1.0f / ((float)nrows * (float)A);
-    p.mu_old = nullptr; p.logstd_old = nullptr; p.focops_lam = 1.f; p.focops_eta = 0.f;
-    p.focops_mask_mean = nullptr; p.forward_only = 0;
+    p.forward_only = 0;
     return launch_grad_tc(p, nb, s);
 }
 

@@ -28,6 +28,7 @@
 // Adam owners.  Loss kinds: PPO-clip, ratio, cost surrogate (fused or stepwise), FOCOPS and P3O (stepwise, with a
 // forward-only statistics pass), supplied dOUT (Fisher-vector product backward).
 #include "common.cuh"
+#include "loss.cuh"
 #include "mlp.cuh"
 #include "x3.cuh"
 
@@ -38,18 +39,9 @@ using namespace x3;
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 512;\n" ::: "memory"); }      // epilogue warps only
 __device__ __forceinline__ void loss_bar_sync() { asm volatile("bar.sync 2, 128;\n" ::: "memory"); }     // loss warps (h == 0)
 
-enum X3Loss { X3_PPO_CLIP = 0, X3_RATIO = 1, X3_FOCOPS = 2, X3_COST = 3, X3_FVP = 4, X3_P3O = 5 };   // X3_FVP: dOUT supplied (Fisher-vector product)
-
-struct X3Batch {
-    const float* obs; const float* act; const float* logp; const float* adv_r; const float* adv_c;
-    const float* tv_r; const float* tv_c; const float* moments; const int* perm;
-    long long total; unsigned perm_seed; long long mb_start; int mb_count;
-    int identity_stride;     // > 0: row = (mb_start + local) * identity_stride (full-batch passes)
-};
 struct X3Args {
-    X3Batch b;
-    int kind; float clip, entropy_coef;
-    const float* lagrange;
+    Batch b;
+    LossParams lc;
     const float* theta;
     float* gpart;            // [gridDim.x][P]
     float* stats_part;       // [gridDim.x][3][8]
@@ -70,12 +62,10 @@ struct X3Args {
     int* error_flag;
     uint8_t* wimg;               // FUSED: [3 nets][W_IMG] bf16x3 images of the weight tiles (W1 | W2 | W3), written by the Adam owners,
                                  // pulled into shared memory with one bulk copy (TMA) after every optimiser step
-    // X3_FOCOPS (first_order/focops.py:L62-108; stepwise launches only): old policy per sample, the minibatch mean of the
-    // KL mask from the forward-only pass 1 (null in pass 1), forward_only = statistics only
-    const float* mu_old; const float* logstd_old; const float* focops_mask_mean; float focops_lam, focops_eta; int forward_only;
-    const float* fvp_dmu;        // X3_FVP: tangent of mu per slab row [total][A] (fvp_tangent_x3_kernel)
-    const float* fvp_vec;        // X3_FVP: direction v (its log_std block gives the log_std block of F v)
-    float fvp_scale;             // X3_FVP: 1 / (rows * A)
+    int forward_only;            // pass 1 of FOCOPS / P3O (stepwise launches only): statistics only
+    const float* fvp_dmu;        // LOSS_FVP: tangent of mu per slab row [total][A] (fvp_tangent_x3_kernel)
+    const float* fvp_vec;        // LOSS_FVP: direction v (its log_std block gives the log_std block of F v)
+    float fvp_scale;             // LOSS_FVP: 1 / (rows * A)
     long long* dbg;              // optional clock64 stamps of CTA (0, 0): [0] = count, then (id, clock) pairs (tools/x3_stage_times.py)
     float* acc;                  // accumulator images, one [128][T_COLS] per CTA
 };
@@ -103,26 +93,6 @@ constexpr int PF_LD = 12;
 constexpr uint32_t X3_SMEM = OFF_PF + XT * PF_LD * 4;
 // accumulator columns
 constexpr uint32_t T_ZA = 0, T_ZB = 64, T_OUT = 128, T_DW1 = 144, T_DW2 = 208, T_DW3 = 272, T_DB1 = 288, T_DB2 = 304, T_COLS = 320;
-
-__device__ __forceinline__ unsigned long long x3_feistel(unsigned long long k, unsigned long long n, unsigned seed) {
-    int bits = 2;
-    while ((1ull << bits) < n) bits += 2;
-    const int half = bits >> 1;
-    const unsigned mask = (1u << half) - 1u;
-    unsigned long long x = k;
-    do {
-        unsigned l = (unsigned)(x >> half) & mask, r = (unsigned)x & mask;
-#pragma unroll
-        for (int round = 0; round < 4; ++round) {
-            const unsigned f = mix32(r ^ (seed + 0x9E3779B9u * (unsigned)(round + 1))) & mask;
-            const unsigned nl = r;
-            r = l ^ f;
-            l = nl;
-        }
-        x = ((unsigned long long)l << half) | r;
-    } while (x >= n);
-    return x;
-}
 
 // fp32 parameters of one network -> bf16x3 weight tiles + fp32 biases in shared memory (all NEPI epilogue threads).
 // All global loads are issued before the first store (one L2 round trip instead of one per loop iteration).
@@ -175,8 +145,7 @@ __device__ __forceinline__ void stage_weights_x3(uint32_t sbase, float* misc, co
     if (tid < 64) { misc[MF_B1 + tid] = bb1; misc[MF_B2 + tid] = bb2; }
     if (tid < 16) {
         misc[MF_B3 + tid] = bb3;
-        const float sd = expf(ls);
-        misc[MF_LS + tid] = ls; misc[MF_LS + 16 + tid] = sd; misc[MF_LS + 32 + tid] = 1.f / (sd * sd);   // log sigma, sigma, 1 / sigma^2
+        stage_policy(misc + MF_LS, tid, ls);
     }
 }
 
@@ -238,11 +207,8 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
     if (!is_mma_warp) {
         stage_weights_x3(sbase, misc, theta, L, net, O, A, tid);
         if (tid < 128) reinterpret_cast<uint32_t*>(gbase + OFF_ONES)[tid] = 0x3F803F80u;       // bf16 1.0 x 256
-        if (tid < 16 && (!FUSED && p.kind == X3_FOCOPS)) {
-            const float lo = (tid < A) ? __ldg(p.logstd_old + tid) : 0.f;
-            const float so = expf(lo);
-            misc[MF_OLD + tid] = lo; misc[MF_OLD + 16 + tid] = 1.f / (so * so);
-        }
+        if (tid < 16 && (!FUSED && p.lc.kind == LOSS_FOCOPS))
+            stage_policy_old(misc + MF_OLD, tid, (tid < A) ? __ldg(p.lc.logstd_old + tid) : 0.f);
     } else {
         if (tid == NEPI) {
             for (int i = 0; i < NBAR; ++i) {
@@ -326,10 +292,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
         const int q = warp & 3, h = warp >> 2;
         const uint32_t lane_base = (uint32_t)(q * 32) << 16;
         const int s_row = 32 * q + lane;                 // sample row of this thread in the [s][.] accumulators
-        const float lam = (p.lagrange != nullptr) ? __ldg(p.lagrange) : 0.f;
-        float m_r = 0.f, s_r = 1.f, m_c = 0.f;
-        if (p.b.moments) { m_r = __ldg(p.b.moments + 0); s_r = __ldg(p.b.moments + 1); m_c = __ldg(p.b.moments + 2); }
-        const float inv_sr = 1.f / s_r, inv_1lam = 1.f / (1.f + lam);
+        const AdvNorm an = adv_norm(p.b.moments, p.lc.lagrange);
         float* sB1 = misc + MF_B1; float* sB2 = misc + MF_B2; float* sB3 = misc + MF_B3; float* sLs = misc + MF_LS;
         float* sRed = misc + MF_RED; float* sPart = misc + MF_PART; float* sScal = misc + MF_SCAL;
 
@@ -390,13 +353,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 long long start; int count;
                 mb_geom(mb, start, count);
                 const int local = tile * XT + tid;
-                long long row = -1;
-                if (local < count) {
-                    const long long k = start + local;
-                    if (p.b.identity_stride > 0) row = k * p.b.identity_stride;
-                    else row = p.b.perm ? (long long)p.b.perm[k] : (long long)x3_feistel((unsigned long long)k, (unsigned long long)p.b.total, p.b.perm_seed);
-                }
-                dst[tid] = row;
+                dst[tid] = (local < count) ? sample_row(p.b, start + local) : -1;
             }
         };
         int step_t0 = 0;
@@ -468,7 +425,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll
                     for (int a = 0; a < AP; ++a) pf_act[a] = 0.f;
                     if (prow >= 0) {
-                        const float* asrc = (p.kind == X3_FVP) ? p.fvp_dmu : p.b.act;
+                        const float* asrc = (p.lc.kind == LOSS_FVP) ? p.fvp_dmu : p.b.act;
                         if (AP == 8) {
                             const uint32_t dst = sbase + OFF_PF + (uint32_t)(s_row * PF_LD) * 4u;
                             auto cp4 = [&](uint32_t d, const float* src) {
@@ -478,7 +435,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll
                                 for (int a = 0; a < AP; ++a)
                                     if (a < A) cp4(dst + 4u * a, asrc + prow * A + a);
-                                if (p.kind != X3_FVP) { cp4(dst + 32u, p.b.logp + prow); cp4(dst + 36u, p.b.adv_r + prow); cp4(dst + 40u, p.b.adv_c + prow); }
+                                if (p.lc.kind != LOSS_FVP) { cp4(dst + 32u, p.b.logp + prow); cp4(dst + 36u, p.b.adv_r + prow); cp4(dst + 40u, p.b.adv_c + prow); }
                             } else {
                                 cp4(dst + 32u, (net == 1 ? p.b.tv_r : p.b.tv_c) + prow);
                             }
@@ -486,7 +443,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll
                             for (int a = 0; a < AP; ++a)
                                 if (a < A) pf_act[a] = __ldg(asrc + prow * A + a);
-                            if (p.kind != X3_FVP) { pf_logp = __ldg(p.b.logp + prow); pf_advr = __ldg(p.b.adv_r + prow); pf_advc = __ldg(p.b.adv_c + prow); }
+                            if (p.lc.kind != LOSS_FVP) { pf_logp = __ldg(p.b.logp + prow); pf_advr = __ldg(p.b.adv_r + prow); pf_advc = __ldg(p.b.adv_c + prow); }
                         } else {
                             pf_tv = __ldg((net == 1 ? p.b.tv_r : p.b.tv_c) + prow);
                         }
@@ -558,7 +515,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                             acc_st[0] += d * d; acc_st[3] += 1.f;
                             d16[0] = 2.f * d * inv_b;
                             acc_db[0] += d16[0];
-                        } else if (p.kind == X3_FVP) {
+                        } else if (p.lc.kind == LOSS_FVP) {
                             // J^T diag(sigma^-2) dmu / (B A): the supplied tangent is the output gradient
                             acc_st[3] += 1.f;
 #pragma unroll
@@ -569,78 +526,15 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                                     acc_db[a] += dm;
                                 }
                         } else {
-                            float logp_new = 0.f, diff[AP];
+                            float mu[AP];
 #pragma unroll
-                            for (int a = 0; a < AP; ++a) {
-                                diff[a] = 0.f;
-                                if (a < A) {
-                                    const float d = pf_act[a] - (o[a] + sB3[a]);
-                                    diff[a] = d;
-                                    logp_new += -(d * d) * (0.5f * sLs[32 + a]) - sLs[a] - 0.9189385332046727f;
-                                }
-                            }
-                            const float ratio = expf(logp_new - pf_logp);
-                            const float adv_r = (pf_advr - m_r) * inv_sr;
-                            const float adv_c = pf_advc - m_c;
-                            const float adv = (adv_r - lam * adv_c) * inv_1lam;
-                            float dlogp, loss;
-                            if (p.kind == X3_PPO_CLIP || (!FUSED && p.kind == X3_P3O)) {
-                                const float rc = fminf(fmaxf(ratio, 1.f - p.clip), 1.f + p.clip);
-                                const float s1 = ratio * adv, s2 = rc * adv;
-                                loss = -fminf(s1, s2);
-                                dlogp = (s1 <= s2) ? -adv * ratio * inv_b : 0.f;
-                                if (!FUSED && p.kind == X3_P3O) {
-                                    // P3O (penalty_function/p3o.py:L48-91): + kappa * relu(mean_j(ratio_j adv_c_j) + Jc - limit); the gate
-                                    // (kappa when the minibatch mean makes the relu active) comes from the forward-only pass 1.
-                                    // Statistic slot 2: pass 1 -> ratio * adv_c; pass 2 -> the penalty term (Loss/Loss_pi_cost).
-                                    const bool pass2 = p.focops_mask_mean != nullptr;
-                                    const float gate = pass2 ? __ldg(p.focops_mask_mean) : 0.f;
-                                    dlogp += gate * adv_c * ratio * inv_b;
-                                    acc_st[2] += pass2 ? gate * (ratio * adv_c + p.focops_eta) : ratio * adv_c;
-                                }
-                            } else if (p.kind == X3_RATIO) {
-                                loss = -ratio * adv; dlogp = -adv * ratio * inv_b;
-                            } else if (p.kind == X3_COST) {
-                                loss = ratio * adv_c; dlogp = adv_c * ratio * inv_b;
-                            }
-                            float dmask = 0.f, dmo[AP];
-#pragma unroll
-                            for (int a = 0; a < AP; ++a) dmo[a] = 0.f;
-                            if ((!FUSED && p.kind == X3_FOCOPS)) {
-                                // The reference forms (kl[b,1] - ratio[b] adv[b] / lam) * mask[b,1] and takes the mean of the
-                                // [b,b] matrix (first_order/focops.py:L85-89):  loss = mean_i(mask_i kl_i) - mean_i(mask_i)
-                                // mean_j(ratio_j adv_j) / lam;  mean_i(mask_i) of this minibatch comes from the forward-only pass 1.
-                                const float* sOld = misc + MF_OLD;
-                                float kl = 0.f;
-#pragma unroll
-                                for (int a = 0; a < AP; ++a)
-                                    if (a < A) {
-                                        const float sn = sLs[16 + a];
-                                        dmo[a] = (o[a] + sB3[a]) - __ldg(p.mu_old + prow * A + a);
-                                        kl += (sOld[a] - sLs[a]) + (sn * sn + dmo[a] * dmo[a]) * (0.5f * sOld[16 + a]) - 0.5f;
-                                    }
-                                dmask = (kl <= p.focops_eta) ? 1.f : 0.f;
-                                const float mbar = p.focops_mask_mean ? __ldg(p.focops_mask_mean) : dmask;
-                                loss = kl * dmask - mbar * ratio * adv / p.focops_lam;
-                                dlogp = -mbar * adv * ratio / p.focops_lam * inv_b;
-                                acc_st[2] += kl; acc_st[4] += dmask;
-                            }
-                            acc_st[0] += loss; acc_st[1] += ratio; acc_st[3] += 1.f;
-#pragma unroll
-                            for (int a = 0; a < AP; ++a)
-                                if (a < A) {
-                                    const float iv = sLs[32 + a];
-                                    float dm = dlogp * diff[a] * iv;
-                                    float dl = dlogp * (diff[a] * diff[a] * iv - 1.f);
-                                    if ((!FUSED && p.kind == X3_FOCOPS)) {
-                                        const float sn = sLs[16 + a];
-                                        dm += dmask * inv_b * dmo[a] * (misc + MF_OLD)[16 + a];
-                                        dl += dmask * inv_b * (sn * sn * (misc + MF_OLD)[16 + a] - 1.f);
-                                    }
-                                    d16[a] = dm;
-                                    acc_db[a] += dm;
-                                    acc_dls[a] += dl;
-                                }
+                            for (int a = 0; a < AP; ++a) mu[a] = o[a] + sB3[a];
+                            actor_sample_loss<!FUSED, AP>(p.lc, an, A, inv_b, mu, pf_act,
+                                                                               [&](int a) { return __ldg(p.lc.mu_old + prow * A + a); },
+                                                                               pf_logp, pf_advr, pf_advc, sLs, misc + MF_OLD, acc_st,
+                                                                               [&](int a, float dm, float dl) {
+                                                                                   d16[a] = dm; acc_db[a] += dm; acc_dls[a] += dl;
+                                                                               });
                         }
                     }
                     store16_x3_sw32(sbase + OFF_D, D_SUB, s_row, d16);
@@ -794,8 +688,8 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 if (net == 0 && tid >= 32 && tid < 32 + A) {
                     const int a = tid - 32;
                     float g = (sRed[32 + a] + sRed[48 + a]) + (sRed[64 + a] + sRed[80 + a]);
-                    if (blockIdx.x == 0 && (p.kind == X3_PPO_CLIP || (!FUSED && (p.kind == X3_FOCOPS || p.kind == X3_P3O)))) g -= p.entropy_coef / (float)A;
-                    if (p.kind == X3_FVP) g = (blockIdx.x == 0) ? 2.f / (float)A * __ldg(p.fvp_vec + L.off_logstd + a) : 0.f;
+                    if (blockIdx.x == 0 && loss_has_entropy<!FUSED>(p.lc.kind)) g -= p.lc.entropy_coef / (float)A;
+                    if (p.lc.kind == LOSS_FVP) g = (blockIdx.x == 0) ? 2.f / (float)A * __ldg(p.fvp_vec + L.off_logstd + a) : 0.f;
                     __stcg(gout + L.off_logstd + a, g);
                 }
                 if (tid >= 64 && tid < 72) {
@@ -987,9 +881,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 if (tid >= 128 && tid < 144) {
                     const int i = tid - 128;
                     misc[MF_B3 + i] = (i < L.out) ? __ldcg(theta + L.off_b3 + i) : 0.f;
-                    const float ls = (net == 0 && i < A) ? __ldcg(theta + L.off_logstd + i) : 0.f;
-                    const float sd = expf(ls);
-                    misc[MF_LS + i] = ls; misc[MF_LS + 16 + i] = sd; misc[MF_LS + 32 + i] = 1.f / (sd * sd);
+                    stage_policy(misc + MF_LS, i, (net == 0 && i < A) ? __ldcg(theta + L.off_logstd + i) : 0.f);
                 }
                 mbar_wait_a(bar(RDY_W), (uint32_t)(mb & 1));
             } else {
@@ -1001,17 +893,6 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
         if (FUSED && blockIdx.x == 0 && tid == 0) p.adam_step[net] = step_t0 + n_mb;     // every CTA read it before the first barrier
     }
     __syncthreads();
-}
-
-// mean_i 1{KL_i <= eta} of a minibatch from the forward-only pass (statistic slot 4 / slot 3 of the actor rows)
-__global__ void x3_mask_mean_kernel(const float* __restrict__ stats_part, int nblocks, float* __restrict__ out,
-                                    const int* __restrict__ stop_flag, int kind, float kappa, float jc_minus_limit) {
-    if (threadIdx.x != 0 || (stop_flag && *stop_flag)) return;
-    const int slot = (kind == X3_P3O) ? 2 : 4;
-    float m = 0.f, n = 0.f;
-    for (int b = 0; b < nblocks; ++b) { m += stats_part[((size_t)b * 3) * 8 + slot]; n += stats_part[((size_t)b * 3) * 8 + 3]; }
-    const float mean = n > 0.f ? m / n : 0.f;
-    out[0] = (kind == X3_P3O) ? ((mean + jc_minus_limit > 0.f) ? kappa : 0.f) : mean;
 }
 
 }  // namespace osb
@@ -1046,7 +927,7 @@ static int x3_bind_acc(X3Args& p, int nb) {
 }
 
 // Split-bf16 (parity-grade tensor-core) variant of osb_minibatch_grad: same arguments, O <= 64, A <= 16,
-// loss kinds PPO-clip / ratio / cost surrogate.  gpart holds osb_tc_grid_blocks(mb_count, net_mask) rows of P floats.
+// loss kinds PPO-clip / ratio / FOCOPS / cost surrogate / P3O.  gpart holds osb_tc_grid_blocks(mb_count, net_mask) rows of P floats.
 int osb_minibatch_grad_x3(const float* theta, int O, int A, const float* obs, const float* act,
                           const float* logp, const float* adv_r, const float* adv_c,
                           const float* tv_r, const float* tv_c, const float* mu_old,
@@ -1058,13 +939,12 @@ int osb_minibatch_grad_x3(const float* theta, int O, int A, const float* obs, co
     OSB_CHECK_ARG(theta && obs && act && logp && adv_r && adv_c && tv_r && tv_c && moments, "null input");
     OSB_CHECK_ARG(O > 0 && O <= 64 && A > 0 && A <= 16 && mb_count > 0 && total > 0, "bf16x3 path needs O <= 64, A <= 16");
     OSB_CHECK_ARG(mb_start >= 0 && mb_start + mb_count <= total, "minibatch window out of range");
-    OSB_CHECK_ARG(loss_kind == X3_PPO_CLIP || loss_kind == X3_RATIO || loss_kind == X3_COST || loss_kind == X3_FOCOPS || loss_kind == X3_P3O, "loss kind not on the bf16x3 path");
-    OSB_CHECK_ARG(loss_kind != X3_FOCOPS || (mu_old && logstd_old), "FOCOPS needs mu_old / logstd_old");
+    OSB_CHECK_ARG((loss_kind >= 0 && loss_kind <= 3) || loss_kind == LOSS_P3O, "loss kind not on the bf16x3 path");
+    OSB_CHECK_ARG(loss_kind != LOSS_FOCOPS || (mu_old && logstd_old), "FOCOPS needs mu_old / logstd_old");
     OSB_CHECK_ARG(net_mask > 0 && net_mask < 8, "net_mask");
     X3Args p = {};
-    p.b = X3Batch{obs, act, logp, adv_r, adv_c, tv_r, tv_c, moments, perm, total, perm_seed, mb_start, mb_count, 0};
-    p.mu_old = mu_old; p.logstd_old = logstd_old; p.focops_lam = focops_lam; p.focops_eta = focops_eta;
-    p.kind = loss_kind; p.clip = clip; p.entropy_coef = entropy_coef; p.lagrange = lagrange;
+    p.b = Batch{obs, act, logp, adv_r, adv_c, tv_r, tv_c, moments, perm, total, perm_seed, mb_start, mb_count, 0};
+    p.lc = LossParams{loss_kind, clip, entropy_coef, focops_lam, focops_eta, lagrange, mu_old, logstd_old, nullptr};
     p.theta = theta; p.gpart = gpart; p.stats_part = stats_part; p.stop_flag = stop_flag;
     p.O = O; p.A = A; p.P = actor_layout(O, A).size + 2 * critic_layout(O, A).size; p.net_mask = net_mask;
     p.batch_size = mb_count; p.world = 1; p.dbg = g_x3_dbg;
@@ -1073,20 +953,14 @@ int osb_minibatch_grad_x3(const float* theta, int O, int A, const float* obs, co
     if (rc) return rc;
     if ((rc = x3_bind_acc(p, nb))) return rc;
     const bool single = (net_mask & (net_mask - 1)) == 0;
-    if ((loss_kind == X3_FOCOPS || loss_kind == X3_P3O) && (net_mask & 1)) {
-        // pass 1: actor forward only -> mean of the KL mask over the minibatch (FOCOPS: the reference's [b,1] x [b] broadcast) or
-        // the relu gate of the minibatch-mean cost surrogate (P3O: focops_lam carries kappa, focops_eta carries Jc - limit)
-        static float* d_mask_mean = nullptr;
-        if (!d_mask_mean) OSB_CUDA(cudaMalloc(&d_mask_mean, sizeof(float)));
+    if (loss_two_pass(loss_kind) && (net_mask & 1)) {   // pass 1: actor forward only
         X3Args q = p;
         q.forward_only = 1; q.net_mask = 1;
         const int nb1 = osb_tc_grid_blocks(mb_count, 1);
         if (A <= 8) minibatch_grad_x3_kernel<false, 8><<<dim3(nb1, 1), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(q);
         else minibatch_grad_x3_kernel<false, 16><<<dim3(nb1, 1), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(q);
         OSB_LAUNCH_CHECK();
-        x3_mask_mean_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(stats_part, nb1, d_mask_mean, stop_flag, loss_kind, focops_lam, focops_eta);
-        OSB_LAUNCH_CHECK();
-        p.focops_mask_mean = d_mask_mean;
+        if ((rc = pass1_gate(stats_part, nb1, stop_flag, p.lc, (cudaStream_t)stream))) return rc;
     }
     if (A <= 8) minibatch_grad_x3_kernel<false, 8><<<dim3(nb, single ? 1 : 3), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(p);
     else minibatch_grad_x3_kernel<false, 16><<<dim3(nb, single ? 1 : 3), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(p);
@@ -1099,8 +973,8 @@ int osb_x3_fvp_backward(const float* theta_actor, const float* vec, int O, int A
                         const float* dmu, float* gpart, float* stats_scratch, void* stream) {
     const long long nrows = (total + stride - 1) / stride;
     X3Args p = {};
-    p.b = X3Batch{obs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, total, 0u, 0, (int)nrows, stride};
-    p.kind = X3_FVP; p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch;
+    p.b = Batch{obs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, total, 0u, 0, (int)nrows, stride};
+    p.lc.kind = LOSS_FVP; p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch;
     p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
     p.batch_size = (int)nrows; p.world = 1; p.dbg = nullptr;
     p.fvp_dmu = dmu; p.fvp_vec = vec; p.fvp_scale = 1.0f / ((float)nrows * (float)A);
@@ -1133,7 +1007,7 @@ int osb_ppo_update_iter_x3(float* theta, float* grad, float* adam_m, float* adam
                            int* p2p_error, void* stream) {
     OSB_CHECK_ARG(theta && grad && adam_m && adam_v && adam_step && obs && act && logp && adv_r && adv_c && tv_r && tv_c && moments, "null input");
     OSB_CHECK_ARG(O > 0 && O <= 64 && A > 0 && A <= 16 && batch_size > 0 && total > 0 && total < (1ll << 31), "bf16x3 path needs O <= 64, A <= 16");
-    OSB_CHECK_ARG(loss_kind == X3_PPO_CLIP || loss_kind == X3_RATIO || loss_kind == X3_COST, "loss kind not on the bf16x3 path");
+    OSB_CHECK_ARG(loss_kind == LOSS_PPO_CLIP || loss_kind == LOSS_RATIO || loss_kind == LOSS_COST, "loss kind not on the fused bf16x3 path");
     OSB_CHECK_ARG(net_mask > 0 && net_mask < 8 && gpart && stats_part && train_stats, "bad argument");
     OSB_CHECK_ARG(world >= 1 && (world == 1 || (peer_buf && peer_flag && p2p_error && rank >= 0 && rank < world && world <= 64)), "bad p2p argument");
     static float* d_ws = nullptr;            // [0, 4): barrier counters (u32); [64, 64 + 6 * 148): slice norms
@@ -1142,8 +1016,8 @@ int osb_ppo_update_iter_x3(float* theta, float* grad, float* adam_m, float* adam
     if (!d_ws) OSB_CUDA(cudaMalloc(&d_ws, (64 + 6 * 148) * sizeof(float)));
     OSB_CUDA(cudaMemsetAsync(d_ws, 0, 4 * sizeof(unsigned int), s));
     X3Args p = {};
-    p.b = X3Batch{obs, act, logp, adv_r, adv_c, tv_r, tv_c, moments, perm, total, perm_seed, 0, (int)total, 0};
-    p.kind = loss_kind; p.clip = clip; p.entropy_coef = entropy_coef; p.lagrange = lagrange;
+    p.b = Batch{obs, act, logp, adv_r, adv_c, tv_r, tv_c, moments, perm, total, perm_seed, 0, (int)total, 0};
+    p.lc.kind = loss_kind; p.lc.clip = clip; p.lc.entropy_coef = entropy_coef; p.lc.lagrange = lagrange;
     p.theta = theta; p.gpart = gpart; p.stats_part = stats_part; p.stop_flag = stop_flag;
     p.O = O; p.A = A; p.P = actor_layout(O, A).size + 2 * critic_layout(O, A).size; p.net_mask = net_mask;
     p.batch_size = batch_size; p.theta_rw = theta; p.grad = grad; p.adam_m = adam_m; p.adam_v = adam_v; p.adam_step = adam_step;
