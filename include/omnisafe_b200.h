@@ -168,6 +168,22 @@ int osb_ext_observe(int O, int N, int T, int t, int obs_normalize, const float* 
                     float* norm_mean1, float* norm_std1, long long* norm_count, int* had_fin, unsigned* ticket,
                     float* rew_slab, float* cost_slab, unsigned char* flags, float* epfin, double* workspace,
                     int* nonfinite, void* stream);
+/* CUDA-graph capture of the external-env epoch (for envs whose step is itself capturable).
+ * osb_ext_prepare performs every one-time host action of osb_ext_act / osb_ext_act_graph for these dimensions
+ * (kernel attributes, the tensor-core accumulator image at its final size); call it before capturing.  An act launch on
+ * a capturing stream that would still need one of them fails with OSB_ERR_UNSUPPORTED instead of breaking the capture.
+ * osb_ext_act_graph = osb_ext_act with the Philox counter read on the device: *epoch_dev * T + t (unsigned wrap-around,
+ * the same value osb_ext_act gets from global_step = epoch * T + t), so a replayed act draws the noise of the epoch the
+ * counter holds.  osb_ext_epoch_advance adds 1 to *epoch_dev on the stream (one thread; captured last in an epoch).
+ * osb_ext_reset_ingest and osb_ext_observe need no preparation. */
+int osb_ext_prepare(int O, int A, int N, int precision);
+int osb_ext_act_graph(int O, int A, int obs_normalize, int N, int T, int t, unsigned env_id_offset, float* s_raw,
+                      float* final_raw, float* norm_mean, float* norm_std, float* norm_mean1, float* norm_std1,
+                      long long* norm_count, float* obs, float* act, float* logp, float* val_r, float* val_c,
+                      float* boot_r, float* boot_c, unsigned char* flags, const float* theta, const float* eps,
+                      unsigned noise_seed, const unsigned* epoch_dev, const float* act_lo, const float* act_hi,
+                      float* act_env, int precision, void* stream);
+int osb_ext_epoch_advance(unsigned* epoch_dev, void* stream);
 /* RewardNormalize / CostNormalize (envs/wrapper.py:L280-423; Normalizer(shape=(), clip=5),
  * common/normalizer.py:L88-139) applied to one epoch's slab x[T][N] in place, after the rollout: row t
  * is pushed into the running statistics (batch of N) and normalised with the statistics valid right

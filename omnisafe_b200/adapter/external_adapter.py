@@ -12,8 +12,16 @@ logp / value slabs and writes the bootstrap values; osb_ext_observe appends rewa
 statistics and feeds the observation normaliser.  Nothing in the loop synchronises the host except the env's own code
 (and, for an env on the CPU, the copy of the action to it).  A non-finite observation raises `OsbError` at the end of
 the epoch.
+
+For an env that declares `graph_safe` (envs/core.py) the loop from osb_ext_act(0) to osb_ext_act(T) is captured into
+one CUDA graph in the second epoch and replayed from then on (the first epoch runs eagerly and warms everything up); the
+captured act launches read the Philox epoch from a device counter that the graph's last kernel advances.  The reset and
+everything after the epoch-end act run outside the graph, with the same code as the eager loop.  OSB_NO_GRAPH=1 keeps
+every epoch eager.
 """
 from __future__ import annotations
+
+import os
 
 import torch
 
@@ -61,6 +69,15 @@ class ExternalEnvAdapter:
         self.act_env = torch.zeros(N, A, **f32)
         self._ws = torch.zeros(lib().osb_ext_workspace_doubles(O, N), dtype=torch.float64, device=dev)
         self.nonfinite = torch.zeros(1, dtype=torch.int32, device=dev)
+        # CUDA-graph replay of the epoch for envs that declare graph_safe (envs/core.py); OSB_NO_GRAPH=1 turns it off
+        self._use_graph = bool(getattr(self._env, 'graph_safe', False)) and not os.getenv('OSB_NO_GRAPH')
+        self._mode_logged = False
+        self._graph = None
+        self._graph_key_baked = None
+        self.captures = 0                               # graphs captured so far (a recapture follows a pointer change)
+        self._epoch_dev = torch.zeros(1, dtype=torch.int32, device=dev)    # u32 Philox epoch counter of the replays
+        self._obs0 = torch.zeros(N, O, **f32)           # static copy of env.reset()'s observation (graph mode)
+        self._eps_buf = None                            # static [T, N, A] copy of the parity-mode noise (graph mode)
 
     @property
     def env(self):
@@ -98,35 +115,30 @@ class ExternalEnvAdapter:
         return [ptr(n.mean), ptr(n.sumsq), ptr(n.std), ptr(n.mean1), ptr(n.std1), ptr(n.count), ptr(n.had_fin),
                 ptr(n.ticket)]
 
-    def rollout(self, steps_per_epoch: int, agent, buffer, logger=None, eps=None) -> None:
-        """Roll the envs for `steps_per_epoch` steps each and fill `buffer` (see the module docstring).
+    @property
+    def graph_mode(self) -> str:
+        """'graph' when the epoch's steps are replayed from a CUDA graph (from the second epoch on), else 'eager'."""
+        return 'graph' if self._use_graph else 'eager'
 
-        `eps` (optional, [T, N, A]) supplies the standard-normal stream (parity mode); by default the kernel draws
-        Philox noise."""
-        T, N, O, A = int(steps_per_epoch), self._num_envs, self._obs_dim, self._act_dim
-        assert T == buffer.T and N == buffer.N
-        if eps is not None:
-            assert eps.shape == (T, N, A) and eps.dtype == torch.float32
-        L, d, s = lib(), buffer.data, current_stream()
+    def _act(self, agent, d, T: int, t: int, eps_t, s: int, epoch_dev=None) -> None:
+        """One act launch: eager with the host Philox counter, or (epoch_dev) the capturable form reading it on the GPU."""
+        nz, O, A, N = self._obs_normalizer, self._obs_dim, self._act_dim, self._num_envs
+        head = (O, A, int(self._obs_normalize), N, T, t, self._env_id_offset & 0xFFFFFFFF, ptr(self.s_raw),
+                ptr(self.final_raw), ptr(nz.mean), ptr(nz.std), ptr(nz.mean1), ptr(nz.std1), ptr(nz.count),
+                ptr(d['obs']), ptr(d['act']), ptr(d['logp']), ptr(d['value_r']), ptr(d['value_c']), ptr(d['boot_r']),
+                ptr(d['boot_c']), ptr(d['flags']), ptr(agent.theta), ptr(eps_t), self.noise_seed)
+        tail = (ptr(self.act_lo), ptr(self.act_hi), ptr(self.act_env), int(self.precision), s)
+        if epoch_dev is None:
+            lib().osb_ext_act(*head, (self._epoch_index * T + t) & 0xFFFFFFFF, *tail)
+        else:
+            lib().osb_ext_act_graph(*head, ptr(epoch_dev), *tail)
+
+    def _steps(self, T: int, agent, d, eps, s: int, env_dev, epoch_dev=None, capture: bool = False) -> None:
+        """Steps 0 .. T-1 (act, env.step, observe) and the epoch-end act, eagerly or into the graph being captured."""
+        L, N, O = lib(), self._num_envs, self._obs_dim
         on = int(self._obs_normalize)
-        nz = self._obs_normalizer
-        obs, _ = self._env.reset()
-        env_dev = torch.as_tensor(obs).device
-        obs = self._rows(obs, O)
-        L.osb_ext_reset_ingest(O, N, on, ptr(obs), ptr(self.s_raw), ptr(self.ep_ret), ptr(self.ep_cost),
-                               ptr(self.ep_len), *self._norm_ptrs(), ptr(self._ws), ptr(self.nonfinite), s)
-
-        def act(t: int) -> None:
-            L.osb_ext_act(O, A, on, N, T, t, self._env_id_offset & 0xFFFFFFFF, ptr(self.s_raw), ptr(self.final_raw),
-                          ptr(nz.mean), ptr(nz.std), ptr(nz.mean1), ptr(nz.std1), ptr(nz.count),
-                          ptr(d['obs']), ptr(d['act']), ptr(d['logp']), ptr(d['value_r']), ptr(d['value_c']),
-                          ptr(d['boot_r']), ptr(d['boot_c']), ptr(d['flags']), ptr(agent.theta),
-                          ptr(eps[t]) if (eps is not None and t < T) else 0, self.noise_seed,
-                          (self._epoch_index * T + t) & 0xFFFFFFFF, ptr(self.act_lo), ptr(self.act_hi),
-                          ptr(self.act_env), int(self.precision), s)
-
         for t in range(T):
-            act(t)
+            self._act(agent, d, T, t, None if eps is None else eps[t], s, epoch_dev)
             # a fresh tensor every step, as the reference hands the env: the buffer is rewritten by the next act step
             action = self.act_env.to(env_dev, copy=True)
             if N == 1:
@@ -136,6 +148,9 @@ class ExternalEnvAdapter:
             rew, cost = self._rows(rew), self._rows(cost)
             term, trunc = self._rows(term, dtype=torch.uint8), self._rows(trunc, dtype=torch.uint8)
             final = mask = None
+            if capture and ('final_observation' not in info or '_final_observation' not in info):
+                raise OsbError(f'{type(self._env).__name__} is graph_safe but its step info lacks final_observation / '
+                               '_final_observation: a captured step must report them on every step')
             if 'final_observation' in info:
                 final = self._rows(info['final_observation'], O)
                 mask = info.get('_final_observation')
@@ -144,9 +159,74 @@ class ExternalEnvAdapter:
                               ptr(mask), ptr(self.s_raw), ptr(self.final_raw), ptr(self.ep_ret), ptr(self.ep_cost),
                               ptr(self.ep_len), *self._norm_ptrs(), ptr(d['reward']), ptr(d['cost']),
                               ptr(d['flags']), ptr(d['epfin']), ptr(self._ws), ptr(self.nonfinite), s)
-        act(T)
-        L.osb_episode_window(ptr(d['flags']), ptr(d['epfin']), T, N, self.window_lens, ptr(self.ep_ring),
-                             ptr(self.ep_meta), ptr(self.window_sums), s)
+        self._act(agent, d, T, T, None, s, epoch_dev)
+
+    def _graph_key(self, T: int, agent, d, eps, reset_obs) -> tuple:
+        """The device pointers (and shape) a captured epoch bakes in; a change of any of them forces a recapture."""
+        return (T, ptr(agent.theta), tuple(ptr(v) for v in d.values() if v is not None), ptr(eps),
+                tuple(self._norm_ptrs()), torch.as_tensor(reset_obs).untyped_storage().data_ptr())
+
+    def _capture(self, T: int, agent, d, eps, env_dev) -> None:
+        """Capture the T steps, the epoch-end act and the Philox epoch advance into one CUDA graph."""
+        N, O, A = self._num_envs, self._obs_dim, self._act_dim
+        self._graph = None                          # release the old graph (and its pool) before capturing anew
+        lib().osb_ext_prepare(O, A, N, int(self.precision))
+        e = self._epoch_index & 0xFFFFFFFF
+        self._epoch_dev.fill_(e - (1 << 32) if e >= (1 << 31) else e)     # the u32 counter, stored as int32 bits
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, pool=torch.cuda.graph_pool_handle()):
+            s = current_stream()
+            self._steps(T, agent, d, eps, s, env_dev, self._epoch_dev, capture=True)
+            lib().osb_ext_epoch_advance(ptr(self._epoch_dev), s)
+        self._graph = graph
+        self.captures += 1
+
+    def rollout(self, steps_per_epoch: int, agent, buffer, logger=None, eps=None) -> None:
+        """Roll the envs for `steps_per_epoch` steps each and fill `buffer` (see the module docstring).
+
+        `eps` (optional, [T, N, A]) supplies the standard-normal stream (parity mode); by default the kernel draws
+        Philox noise."""
+        T, N, O, A = int(steps_per_epoch), self._num_envs, self._obs_dim, self._act_dim
+        assert T == buffer.T and N == buffer.N
+        if eps is not None:
+            assert eps.shape == (T, N, A) and eps.dtype == torch.float32
+        if logger is not None and not self._mode_logged:
+            logger.log(f'{type(self._env).__name__}: external-env rollout in {self.graph_mode} mode')
+            self._mode_logged = True
+        L, d, s = lib(), buffer.data, current_stream()
+        obs, _ = self._env.reset()
+        env_dev = torch.as_tensor(obs).device
+        if self._use_graph and env_dev.type != 'cuda':
+            raise ValueError(f'{type(self._env).__name__} declares graph_safe but reset() returned observations on {env_dev}')
+        replay = self._use_graph and self._epoch_index > 0
+        reset_obs = obs
+        if replay:
+            obs = self._obs0.copy_(torch.as_tensor(reset_obs).reshape(N, O))
+        else:
+            obs = self._rows(obs, O)
+        L.osb_ext_reset_ingest(O, N, int(self._obs_normalize), ptr(obs), ptr(self.s_raw), ptr(self.ep_ret),
+                               ptr(self.ep_cost), ptr(self.ep_len), *self._norm_ptrs(), ptr(self._ws),
+                               ptr(self.nonfinite), s)
+        if replay:
+            if eps is not None:
+                if self._eps_buf is None or self._eps_buf.shape != (T, N, A):
+                    self._eps_buf = torch.empty(T, N, A, dtype=torch.float32, device=self._device)
+                self._eps_buf.copy_(eps)
+            eps_g = None if eps is None else self._eps_buf
+            key = self._graph_key(T, agent, d, eps_g, reset_obs)
+            if self._graph is None or key != self._graph_key_baked:
+                self._capture(T, agent, d, eps_g, env_dev)
+                self._graph_key_baked = key
+            self._graph.replay()
+        else:
+            self._steps(T, agent, d, eps, s, env_dev)
+        self._end_epoch(T, d, s)
+
+    def _end_epoch(self, T: int, d, s: int) -> None:
+        """Episode window, Reward / CostNormalize post-pass and the non-finite check (eager and graph epochs alike)."""
+        N = self._num_envs
+        lib().osb_episode_window(ptr(d['flags']), ptr(d['epfin']), T, N, self.window_lens, ptr(self.ep_ring),
+                                 ptr(self.ep_meta), ptr(self.window_sums), s)
         # the per-step reward / cost normalisation of the reference commutes with the rollout (OnPolicyAdapter.rollout)
         if self._reward_normalizer is not None:
             self._reward_normalizer.normalize_rows_(d['reward'])

@@ -39,12 +39,14 @@ namespace osb {
 // demand.  A buffer that has been handed out is never freed (growth allocates a new one and keeps the old one for the
 // life of the process), so a pointer stays valid for the launch it was fetched for and no growth synchronises the device.
 // Contract: the launches of one kernel family on one device share its buffer, so they must be ordered on one stream;
-// growth calls cudaMalloc, which CUDA-graph capture does not allow -- run a launch of the same size before capturing it.
+// growth calls cudaMalloc, which CUDA-graph capture does not allow -- run a launch of the same size before capturing it
+// (acc_scratch_capacity tells whether a launch would grow the buffer).
+static constexpr int MAX_DEV = 64;
+static std::mutex mu;
+static float* buf[MAX_DEV][ACC_SLOTS] = {};
+static size_t cap[MAX_DEV][ACC_SLOTS] = {};
+
 float* acc_scratch(int slot, size_t bytes) {
-    constexpr int MAX_DEV = 64;
-    static std::mutex mu;
-    static float* buf[MAX_DEV][ACC_SLOTS] = {};
-    static size_t cap[MAX_DEV][ACC_SLOTS] = {};
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= MAX_DEV || slot < 0 || slot >= ACC_SLOTS) {
         osb_set_error("acc_scratch: bad device or slot");
@@ -65,6 +67,13 @@ float* acc_scratch(int slot, size_t bytes) {
         cap[dev][slot] = grown;
     }
     return buf[dev][slot];
+}
+
+size_t acc_scratch_capacity(int slot) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= MAX_DEV || slot < 0 || slot >= ACC_SLOTS) return 0;
+    std::lock_guard<std::mutex> lock(mu);
+    return cap[dev][slot];
 }
 
 int grid_sms() {

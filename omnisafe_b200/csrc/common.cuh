@@ -51,6 +51,8 @@ enum AccSlot { ACC_ROLLOUT = 0, ACC_EVAL_TC, ACC_EVAL_X3, ACC_UPDATE_TC, ACC_FVP
 // error string set) when it cannot be allocated.  Launches of one slot on one device must be ordered on one stream;
 // see api.cu for the lifetime and graph-capture rules.
 float* acc_scratch(int slot, size_t bytes);
+// Bytes acc_scratch(slot, bytes) can hand out on the current device without allocating (0 before the first call).
+size_t acc_scratch_capacity(int slot);
 // Persistent grids use one CTA per SM of the current device, at most MAX_GRID_CTAS (the per-CTA partial-result
 // buffers of algorithms/engine.py hold that many rows).
 constexpr int MAX_GRID_CTAS = 148;

@@ -288,7 +288,15 @@ struct StepArgs {
     const float* act_lo;      // [A]
     const float* act_hi;      // [A]
     float* act_env;           // [N][A]
+    // external-env act step replayed from a CUDA graph: the Philox counter is *epoch_dev * T + t (u32 wrap-around, as
+    // the host computes global_step) instead of global_step.  Null: global_step is used.
+    const unsigned* epoch_dev;
 };
+
+// Philox counter of an act step: a graph replay reads the epoch from the device, an eager launch passes it
+__device__ __forceinline__ uint32_t act_global_step(const StepArgs& p) {
+    return p.epoch_dev ? __ldg(p.epoch_dev) * (uint32_t)p.T + (uint32_t)p.t : p.global_step;
+}
 
 // ActionScale (wrapper.py:L510-512) from [-1, 1] onto [lo, hi] in the reference's fp32 order:
 // lo + (hi - lo) * (a - (-1)) / (1 - (-1)).  No clipping: the env receives what the wrapper would hand it.
@@ -453,6 +461,8 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
         const int e = threadIdx.x >> 3, q = threadIdx.x & 7;
         const int env = env0 + e;
         const bool ok = env < N;
+        uint32_t gstep = p.global_step;
+        if constexpr (EXT) gstep = act_global_step(p);
         float lp = 0.f;
         for (int a = q; a < A; a += 8) {
             const float mu = sO[e * LDO + a];
@@ -460,7 +470,7 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
             float eps = 0.f;
             if (ok)
                 eps = p.eps ? p.eps[(size_t)env * A + a]
-                            : philox_normal(p.noise_seed, p.es.env_id_offset + env, p.global_step, a);
+                            : philox_normal(p.noise_seed, p.es.env_id_offset + env, gstep, a);
             const float act = __fadd_rn(mu, __fmul_rn(sd, eps));   // Normal.rsample: loc + eps*scale
             // Normal.log_prob: -((x-loc)^2)/(2 var) - log(scale) - log(sqrt(2 pi))
             const float d = __fadd_rn(act, -mu);
@@ -974,7 +984,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                 float n0 = 0.f, n1 = 0.f;
                 if (ok && a0 < A) {
                     if (eps_t) { n0 = eps_t[(size_t)env * A + a0]; n1 = (a1 < A) ? eps_t[(size_t)env * A + a1] : 0.f; }
-                    else philox_normal2(p.noise_seed, p.es.env_id_offset + env, gstep_t, pr, n0, n1);
+                    else philox_normal2(p.noise_seed, p.es.env_id_offset + env, EXT ? act_global_step(p) : gstep_t, pr, n0, n1);
                 }
                 float lp = 0.f;
 #pragma unroll
@@ -1013,7 +1023,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                     float eps = 0.f;
                     if (ok)
                         eps = eps_t ? eps_t[(size_t)env * A + a]
-                                    : philox_normal(p.noise_seed, p.es.env_id_offset + env, gstep_t, a);
+                                    : philox_normal(p.noise_seed, p.es.env_id_offset + env, EXT ? act_global_step(p) : gstep_t, a);
                     const float act = __fadd_rn(mu, __fmul_rn(sd, eps));
                     const float d = __fadd_rn(act, -mu);
                     float term = __fdiv_rn(-__fmul_rn(d, d), sSd[16 + a]);
@@ -1486,9 +1496,25 @@ static long long* g_rollout_dbg = nullptr;
 
 }  // extern "C"
 
-// EXT = true: the act step of the external-env path (never the persistent kernel)
+// The one-time host actions of an act launch on an external env -- kernel attributes and the accumulator image -- call
+// cudaFuncSetAttribute / cudaMalloc, which CUDA-graph capture does not allow.  osb_ext_prepare performs them before a
+// capture; a launch on a capturing stream that would still need one fails here instead of breaking the capture.
+static int ext_refuse_if_capturing(cudaStream_t stream, const char* what) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    OSB_CUDA(cudaStreamIsCapturing(stream, &cs));
+    if (cs == cudaStreamCaptureStatusNone) return OSB_OK;
+    char msg[256];
+    snprintf(msg, sizeof(msg), "osb_ext_act on a capturing stream needs %s: call osb_ext_prepare before the capture", what);
+    osb_set_error(msg);
+    return OSB_ERR_UNSUPPORTED;
+}
+
+static size_t rollout_tc_acc_bytes(int N) { return (size_t)((N + RTC - 1) / RTC) * 3 * 128 * R_COLS * sizeof(float); }
+
+// EXT = true: the act step of the external-env path (never the persistent kernel).  prepare_only: perform the host
+// actions (attributes, accumulator image) and launch nothing (osb_ext_prepare).
 template <bool EXT>
-static int launch_step(StepArgs& p, cudaStream_t stream) {
+static int launch_step(StepArgs& p, cudaStream_t stream, bool prepare_only = false) {
     const int On = p.es.O + (p.sa.safety ? 1 : 0);
     if ((p.precision == 1 || p.precision == 2) && On <= 64) {
         const bool x3 = p.precision == 2;
@@ -1496,6 +1522,7 @@ static int launch_step(StepArgs& p, cudaStream_t stream) {
         static bool attr_tc = false;
         if (!attr_tc) {
             if constexpr (EXT) {
+                if (int rc = ext_refuse_if_capturing(stream, "the tensor-core kernel attributes")) return rc;
                 OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(false)));
                 OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(true)));
             } else {
@@ -1507,8 +1534,13 @@ static int launch_step(StepArgs& p, cudaStream_t stream) {
             attr_tc = true;
         }
         dim3 grid_tc((p.N + RTC - 1) / RTC, p.is_tail ? 2 : 3);
-        p.acc = acc_scratch(ACC_ROLLOUT, (size_t)grid_tc.x * 3 * 128 * R_COLS * sizeof(float));
+        if constexpr (EXT) {
+            if (acc_scratch_capacity(ACC_ROLLOUT) < rollout_tc_acc_bytes(p.N))
+                if (int rc = ext_refuse_if_capturing(stream, "a larger accumulator image")) return rc;
+        }
+        p.acc = acc_scratch(ACC_ROLLOUT, rollout_tc_acc_bytes(p.N));
         if (!p.acc) return OSB_ERR_CUDA;
+        if (prepare_only) return OSB_OK;
         if (EXT) {
             if (x3) rollout_step_tc_kernel<true, false, true><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
             else rollout_step_tc_kernel<false, false, true><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
@@ -1532,9 +1564,13 @@ static int launch_step(StepArgs& p, cudaStream_t stream) {
     const size_t smem = rollout_smem_bytes(On);
     static size_t attr = 0;
     if (smem > attr) {
+        if constexpr (EXT) {
+            if (int rc = ext_refuse_if_capturing(stream, "a larger shared-memory attribute")) return rc;
+        }
         OSB_CUDA(cudaFuncSetAttribute(rollout_step_kernel<EXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = smem;
     }
+    if (prepare_only) return OSB_OK;
     dim3 grid((p.N + RT - 1) / RT, p.is_tail ? 2 : 3);
     rollout_step_kernel<EXT><<<grid, NTHREADS, smem, stream>>>(p);
     OSB_LAUNCH_CHECK();
@@ -1691,12 +1727,15 @@ int osb_ext_observe(int O, int N, int T, int t, int obs_normalize, const float* 
     return launch_observe(x, st, ns, sl, O, N, T, t, obs_normalize, 0, stream);
 }
 
-int osb_ext_act(int O, int A, int obs_normalize, int N, int T, int t, unsigned env_id_offset, float* s_raw,
-                float* final_raw, float* norm_mean, float* norm_std, float* norm_mean1, float* norm_std1,
-                long long* norm_count, float* obs, float* act, float* logp, float* val_r, float* val_c, float* boot_r,
-                float* boot_c, unsigned char* flags, const float* theta, const float* eps, unsigned noise_seed,
-                unsigned global_step, const float* act_lo, const float* act_hi, float* act_env, int precision,
-                void* stream) {
+}  // extern "C"
+
+// one act launch of the external-env path; epoch_dev non-null: the Philox counter is read on the device
+static int ext_act(int O, int A, int obs_normalize, int N, int T, int t, unsigned env_id_offset, float* s_raw,
+                   float* final_raw, float* norm_mean, float* norm_std, float* norm_mean1, float* norm_std1,
+                   long long* norm_count, float* obs, float* act, float* logp, float* val_r, float* val_c,
+                   float* boot_r, float* boot_c, unsigned char* flags, const float* theta, const float* eps,
+                   unsigned noise_seed, unsigned global_step, const unsigned* epoch_dev, const float* act_lo,
+                   const float* act_hi, float* act_env, int precision, void* stream) {
     OSB_CHECK_ARG(O > 0 && A > 0 && A <= OUTP && N > 0 && T > 0, "bad dims (need 0 < A <= 16)");
     OSB_CHECK_ARG(t >= 0 && t <= T, "step index out of range");
     OSB_CHECK_ARG(t == T || (act_lo && act_hi && act_env), "act_lo / act_hi / act_env are required for t < T");
@@ -1711,7 +1750,51 @@ int osb_ext_act(int O, int A, int obs_normalize, int N, int T, int t, unsigned e
     p.t = t; p.T = T; p.N = N; p.is_tail = (t == T) ? 1 : 0; p.precision = precision;
     p.bar_ctr = nullptr; p.bar_flag = nullptr; p.dbg = nullptr;
     p.act_lo = act_lo; p.act_hi = act_hi; p.act_env = act_env;
+    p.epoch_dev = epoch_dev;
     return launch_step<true>(p, (cudaStream_t)stream);
+}
+
+static __global__ void ext_epoch_advance_kernel(unsigned* epoch_dev) { *epoch_dev += 1u; }
+
+extern "C" {
+
+int osb_ext_act(int O, int A, int obs_normalize, int N, int T, int t, unsigned env_id_offset, float* s_raw,
+                float* final_raw, float* norm_mean, float* norm_std, float* norm_mean1, float* norm_std1,
+                long long* norm_count, float* obs, float* act, float* logp, float* val_r, float* val_c, float* boot_r,
+                float* boot_c, unsigned char* flags, const float* theta, const float* eps, unsigned noise_seed,
+                unsigned global_step, const float* act_lo, const float* act_hi, float* act_env, int precision,
+                void* stream) {
+    return ext_act(O, A, obs_normalize, N, T, t, env_id_offset, s_raw, final_raw, norm_mean, norm_std, norm_mean1,
+                   norm_std1, norm_count, obs, act, logp, val_r, val_c, boot_r, boot_c, flags, theta, eps, noise_seed,
+                   global_step, nullptr, act_lo, act_hi, act_env, precision, stream);
+}
+
+int osb_ext_act_graph(int O, int A, int obs_normalize, int N, int T, int t, unsigned env_id_offset, float* s_raw,
+                      float* final_raw, float* norm_mean, float* norm_std, float* norm_mean1, float* norm_std1,
+                      long long* norm_count, float* obs, float* act, float* logp, float* val_r, float* val_c,
+                      float* boot_r, float* boot_c, unsigned char* flags, const float* theta, const float* eps,
+                      unsigned noise_seed, const unsigned* epoch_dev, const float* act_lo, const float* act_hi,
+                      float* act_env, int precision, void* stream) {
+    OSB_CHECK_ARG(epoch_dev, "epoch_dev is required");
+    return ext_act(O, A, obs_normalize, N, T, t, env_id_offset, s_raw, final_raw, norm_mean, norm_std, norm_mean1,
+                   norm_std1, norm_count, obs, act, logp, val_r, val_c, boot_r, boot_c, flags, theta, eps, noise_seed,
+                   0u, epoch_dev, act_lo, act_hi, act_env, precision, stream);
+}
+
+int osb_ext_epoch_advance(unsigned* epoch_dev, void* stream) {
+    OSB_CHECK_ARG(epoch_dev, "epoch_dev is required");
+    ext_epoch_advance_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(epoch_dev);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}
+
+int osb_ext_prepare(int O, int A, int N, int precision) {
+    OSB_CHECK_ARG(O > 0 && A > 0 && A <= OUTP && N > 0, "bad dims (need 0 < A <= 16)");
+    StepArgs p{};
+    p.es = EnvSpec{O, A, 0, 0u, 0u, 0u, 0.f, 0};
+    p.sa = SauteSpec{nullptr, 1.f, 1.f, 0.f, 1.f};
+    p.N = N; p.precision = precision;
+    return launch_step<true>(p, nullptr, true);
 }
 
 }  // extern "C"

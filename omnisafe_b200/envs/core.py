@@ -9,6 +9,19 @@ The env keeps the reference's multi-env contract (online_adapter.py:L52-140): `r
 itself and reports their last observation in `info['final_observation']` (rows selected by the boolean
 `info['_final_observation']`; when that mask is absent every finished row is taken).  With `num_envs == 1` unbatched
 tensors are accepted, as the reference's `Unsqueeze` wrapper does.  Tensors may live on the CPU or on any CUDA device.
+
+An env may set `graph_safe = True` (an omnisafe_b200 extension, like the `need_*` flags).  The adapter then captures
+the epoch's steps -- the act kernels, `env.step` and the observe kernels -- into one CUDA graph and replays it every
+epoch, which removes the host's per-launch cost.  Such an env promises:
+- it lives on the training CUDA device and says so in `device` (or `_device`), a CUDA `torch.device`;
+- `step` and `reset` keep their state in the same storage from call to call, writing it in place (`copy_`, `out=`)
+  instead of rebinding attributes: a replay reads the state the previous replay wrote.  `reset` returns the same
+  storage every epoch (its state, or a fixed buffer); a new one makes the adapter capture the graph again;
+- `step` does not synchronise with the host, has no data-dependent Python control flow and keeps no host-side state
+  (RNG, counters) that must advance from step to step: it runs once per step at capture, never at replay;
+- `info` holds `final_observation` and `_final_observation` on every step (the mask all false when nothing finished),
+  so its structure is the same on every step;
+- the tensors `step` returns may be fresh each call: the adapter copies them inside the graph.
 """
 from __future__ import annotations
 
@@ -50,6 +63,7 @@ class CMDP(ABC):
     need_time_limit_wrapper: bool = False
     need_auto_reset_wrapper: bool = False
     need_evaluation: bool = True
+    graph_safe: bool = False        # omnisafe_b200: the step may be captured into a CUDA graph (module docstring)
 
     _support_envs: ClassVar[list[str]]
 
@@ -190,4 +204,9 @@ def check_env(env) -> tuple[int, int, np.ndarray, np.ndarray]:
     hi = np.broadcast_to(np.asarray(act.high, np.float32), (A,)).copy()
     if not (np.isfinite(lo).all() and np.isfinite(hi).all()):
         raise ValueError(f'{name}: the action bounds must be finite (ActionScale maps [-1, 1] onto them), got {lo} .. {hi}')
+    if getattr(env, 'graph_safe', False):
+        dev = getattr(env, 'device', None) or getattr(env, '_device', None)
+        if dev is None or getattr(dev, 'type', str(dev).split(':')[0]) != 'cuda':
+            raise ValueError(f'{name} declares graph_safe but its observations are not on a CUDA device (device = {dev}): '
+                             'a graph-safe env lives on the training GPU and exposes it as `device`')
     return O, A, lo, hi

@@ -1,12 +1,14 @@
 """Throughput of the external-env path: the bench.py headline workload (PPOLag, 4096 envs x T = 128, obs 60 / act 8,
 batch 16384, update_iters 8) on a PyTorch-on-GPU port of the synthetic dynamics registered as a user CMDP.
 
-    python tools/external_env_bench.py [--steps K] [--warmup W] [--precision bf16x3|tf32|fp32]
+    python tools/external_env_bench.py [--steps K] [--warmup W] [--precision bf16x3|tf32|fp32] [--graph]
 
 Every env step is one act launch, the env's own PyTorch kernels and one observe launch.  Prints ONE JSON line:
 env-steps/s over full epochs (rollout + GAE + update, CUDA events), and one rollout split into the device time spent
 inside env.step (CUDA events at its entry and exit) and the rest (act / observe kernels, episode window, launch gaps).
-Logs go to a temporary directory; nothing is written to the tree.
+--graph runs the graph-safe TorchBox (same arithmetic, state written in place, no events inside step), whose epoch the
+adapter replays from a CUDA graph; it reports env-steps/s and the rollout time per epoch only.  With OSB_NO_GRAPH=1 the
+same env runs eagerly.  Logs go to a temporary directory; nothing is written to the tree.
 """
 from __future__ import annotations
 
@@ -22,6 +24,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 ENV_ID = 'TorchBox-v0'
+GRAPH_ENV_ID = 'TorchBoxGraph-v0'
 N, T, O, A, TMAX = 4096, 128, 60, 8, 64
 
 
@@ -97,7 +100,35 @@ def register_torch_box() -> None:
         def close(self):
             pass
 
+    class TorchBoxGraph(TorchBox):
+        """TorchBox for CUDA-graph capture: the same arithmetic with the state updated in place."""
+        _support_envs = [GRAPH_ENV_ID]  # noqa: RUF012
+        graph_safe = True
+
+        def __init__(self, env_id, num_envs=1, device='cuda', **kw):
+            super().__init__(env_id, num_envs=num_envs, device=device, **kw)
+            self._device = torch.device(device)
+
+        def reset(self, seed=None, options=None):
+            self.episode += 1
+            self.ep_step.zero_()
+            self.s.copy_(self._reset_values(self.episode))
+            return self.s, {}
+
+        def step(self, action):
+            a = action.clamp(-1.0, 1.0)
+            sn = (0.95 * self.s + 0.1 * a[:, self.idx] + self.bias).clamp(-10.0, 10.0)
+            reward = 1.0 - (sn * sn).mean(1)
+            cost = (sn[:, 0] > 0.0).to(torch.float32)
+            trunc = (self.ep_step + 1) >= self.tmax
+            term = torch.zeros_like(trunc)
+            self.episode.copy_(torch.where(trunc, self.episode + 1, self.episode))
+            self.s.copy_(torch.where(trunc[:, None], self._reset_values(self.episode), sn))
+            self.ep_step.copy_(torch.where(trunc, torch.zeros_like(self.ep_step), self.ep_step + 1))
+            return self.s, reward, cost, term, trunc, {'final_observation': sn, '_final_observation': trunc}
+
     env_register(TorchBox)
+    env_register(TorchBoxGraph)
 
 
 def timed(fn, k: int) -> float:
@@ -127,10 +158,12 @@ def main() -> None:
     ap.add_argument('--steps', type=int, default=5)
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--precision', default='bf16x3', choices=['bf16x3', 'tf32', 'fp32'])
+    ap.add_argument('--graph', action='store_true', help='graph-safe TorchBox: the epoch is replayed from a CUDA graph')
     args = ap.parse_args()
     import omnisafe_b200
 
     register_torch_box()
+    env_id = GRAPH_ENV_ID if args.graph else ENV_ID
     spe = N * T
     cfg = {'seed': 0,
            'train_cfgs': {'device': 'cuda', 'vector_env_nums': N, 'parallel': 1,
@@ -139,18 +172,22 @@ def main() -> None:
            'logger_cfgs': {'log_dir': tempfile.mkdtemp(prefix='osb_extbench_'), 'use_tensorboard': False,
                            'save_model_freq': 10 ** 9},
            'env_cfgs': {'obs_dim': O, 'act_dim': A, 'max_episode_steps': TMAX}}
-    algo = omnisafe_b200.Agent('PPOLag', ENV_ID, custom_cfgs=cfg).agent
+    algo = omnisafe_b200.Agent('PPOLag', env_id, custom_cfgs=cfg).agent
     for _ in range(max(args.warmup, 1)):
         algo.train_epoch()
     ms = timed(algo.train_epoch, args.steps) / args.steps
     env, k = algo._env.env, 3
-    env.timing = []
+    if not args.graph:
+        env.timing = []
     ms_roll = timed(lambda: algo._env.rollout(algo._steps_per_epoch, algo._actor_critic, algo._buf, algo._logger), k) / k
-    ms_env = sum(a.elapsed_time(b) for a, b in env.timing) / k
+    split = {}
+    if not args.graph:
+        ms_env = sum(a.elapsed_time(b) for a, b in env.timing) / k
+        split = {'env_step_ms': ms_env, 'kernel_ms': ms_roll - ms_env}
     print(json.dumps({
-        'metric': f'env-steps/sec (rollout+GAE+update) PPO-Lag, {ENV_ID} through the external-env path',
+        'metric': f'env-steps/sec (rollout+GAE+update) PPO-Lag, {env_id} through the external-env path',
         'value': spe / (ms * 1e-3), 'unit': 'env-steps/s', 'ms_per_step': ms, 'steps': args.steps,
-        'rollout_ms': ms_roll, 'env_step_ms': ms_env, 'kernel_ms': ms_roll - ms_env,
+        'rollout_ms': ms_roll, **split, 'graph_mode': algo._env.graph_mode,
         'config': {'envs': N, 'steps_per_env': T, 'obs_dim': O, 'act_dim': A, 'batch_size': 16384, 'update_iters': 8,
                    'matmul_precision': args.precision, 'noise': 'in-kernel Philox'},
         **gpu_info()}), flush=True)
