@@ -14,7 +14,6 @@
 // ObsNormalize reduction is done with order-independent fixed-point atomics and finalised by the
 // last actor CTA of the launch; the next launch (= kernel boundary = grid sync) consumes it.
 #include "common.cuh"
-#include <stdlib.h>
 #include "mlp.cuh"
 #include "umma.cuh"
 #include "x3.cuh"
@@ -167,13 +166,40 @@ __device__ void norm_finalize(const NormState& ns, int O, long long n_all) {
 // spec), so one fp32 -> int64 conversion gives the same integer as the fp64 product did.
 __device__ __forceinline__ long long to_fix(float x) { return __float2ll_rn(x * 68719476736.0f); }
 
+// adds a tile's fixed-point sums of column j to the launch's accumulators: x and x^2 over all next-obs rows, and over the
+// final-observation rows when there are any
+__device__ __forceinline__ void push_fix_sums(const NormState& ns, int O, int j, long long sx, long long sxx, long long fx,
+                                              long long fxx) {
+    atomicAdd((unsigned long long*)(ns.acc_all + j), (unsigned long long)sx);
+    atomicAdd((unsigned long long*)(ns.acc_all + O + j), (unsigned long long)sxx);
+    if (fx != 0 || fxx != 0) {
+        atomicAdd((unsigned long long*)(ns.acc_fin + j), (unsigned long long)fx);
+        atomicAdd((unsigned long long*)(ns.acc_fin + O + j), (unsigned long long)fxx);
+    }
+}
+
+// Called by every thread of every CTA of the launch: true in the CTA that arrives last at the ticket, after every CTA's
+// global writes are visible to it.
+__device__ __forceinline__ bool last_cta(unsigned int* ticket) {
+    __shared__ int s_last;
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) s_last = (atomicAdd(ticket, 1u) == gridDim.x * gridDim.y - 1) ? 1 : 0;
+    __syncthreads();
+    return s_last;
+}
+
+// ObsNormalize of one value (Normalizer.normalize, normalizer.py:L122-139): clip((x - mean) / std, -5, 5)
+__device__ __forceinline__ float norm_clip(float v, float mean, float std) {
+    return fminf(fmaxf(__fdiv_rn(__fadd_rn(v, -mean), std), -5.f), 5.f);
+}
+
 // ---------------------------------------------------------------------------------------------
 // reset of all envs (OnPolicyAdapter.rollout resets every epoch: onpolicy_adapter.py:L80) and the
 // normaliser push of the reset observations (ObsNormalize.reset, wrapper.py:L243-261).
 __global__ void __launch_bounds__(NTHREADS) env_reset_kernel(EnvSpec es, EnvState st, NormState ns, SauteSpec sa,
                                                              int N) {
     __shared__ float sNew[RT][KC + 1];
-    __shared__ int s_last;
     const int env0 = blockIdx.x * RT;
     const int O = es.O;
     const int e = threadIdx.x >> 3, q = threadIdx.x & 7;
@@ -201,8 +227,7 @@ __global__ void __launch_bounds__(NTHREADS) env_reset_kernel(EnvSpec es, EnvStat
                         sx += to_fix(v);
                         sxx += to_fix(__fmul_rn(v, v));
                     }
-                atomicAdd((unsigned long long*)(ns.acc_all + j), (unsigned long long)sx);
-                atomicAdd((unsigned long long*)(ns.acc_all + O + j), (unsigned long long)sxx);
+                push_fix_sums(ns, O, j, sx, sxx, 0, 0);
             }
         }
         __syncthreads();
@@ -215,13 +240,7 @@ __global__ void __launch_bounds__(NTHREADS) env_reset_kernel(EnvSpec es, EnvStat
         st.ep_len[env] = 0;
         if (sa.safety) sa.safety[env] = sa.init;   // buffer 0: step 0 reads parity 0
     }
-    if (es.obs_normalize) {
-        __threadfence();
-        __syncthreads();
-        if (threadIdx.x == 0) s_last = (atomicAdd(ns.ticket, 1u) == gridDim.x - 1) ? 1 : 0;
-        __syncthreads();
-        if (s_last) norm_finalize(ns, O, (long long)N);
-    }
+    if (es.obs_normalize && last_cta(ns.ticket)) norm_finalize(ns, O, (long long)N);
 }
 
 // Philox4x32-10 (fast-mode noise); counter = (env gid, global step, lane block, 0).
@@ -231,25 +250,9 @@ __device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint
     const uint32_t n0 = hi1 ^ c[1] ^ k0, n2 = hi0 ^ c[3] ^ k1;
     c[0] = n0; c[1] = lo1; c[2] = n2; c[3] = lo0;
 }
-__device__ float philox_normal(uint32_t seed, uint32_t gid, uint32_t step, int a) {
-    uint32_t c[4] = {gid, step, (uint32_t)(a >> 2), 0x0B200u};
-    uint32_t k0 = seed, k1 = 0xCAFEF00Du;
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        philox_round(c, k0, k1);
-        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-    }
-    const int pair = (a & 3) >> 1;
-    const float u0 = ((float)(c[2 * pair] >> 8) + 0.5f) * (1.0f / 16777216.0f);
-    const float u1 = ((float)(c[2 * pair + 1] >> 8) + 0.5f) * (1.0f / 16777216.0f);
-    const float r = sqrtf(-2.0f * logf(u0));
-    float sn, cs;
-    sincosf(6.283185307179586f * u1, &sn, &cs);
-    return (a & 1) ? r * sn : r * cs;
-}
-
-// both normals of action pair pr (actions 2 pr, 2 pr + 1): same values as philox_normal(seed, gid, step, 2 pr [+ 1])
-__device__ void philox_normal2(uint32_t seed, uint32_t gid, uint32_t step, int pr, float& n0, float& n1) {
+// both normals of action pair pr (actions 2 pr, 2 pr + 1): one Philox block serves two pairs, Box-Muller gives the pair's
+// (cos, sin) values
+__device__ float2 philox_normal2(uint32_t seed, uint32_t gid, uint32_t step, int pr) {
     uint32_t c[4] = {gid, step, (uint32_t)(pr >> 1), 0x0B200u};
     uint32_t k0 = seed, k1 = 0xCAFEF00Du;
 #pragma unroll
@@ -263,7 +266,12 @@ __device__ void philox_normal2(uint32_t seed, uint32_t gid, uint32_t step, int p
     const float r = sqrtf(-2.0f * logf(u0));
     float sn, cs;
     sincosf(6.283185307179586f * u1, &sn, &cs);
-    n0 = r * cs; n1 = r * sn;
+    return make_float2(r * cs, r * sn);
+}
+// the normal of action a alone
+__device__ float philox_normal(uint32_t seed, uint32_t gid, uint32_t step, int a) {
+    const float2 n = philox_normal2(seed, gid, step, a >> 1);
+    return (a & 1) ? n.y : n.x;
 }
 
 struct StepArgs {
@@ -304,6 +312,42 @@ __device__ __forceinline__ float action_scale(float a, float lo, float hi) {
     return __fadd_rn(lo, __fdiv_rn(__fmul_rn(__fadd_rn(hi, -lo), __fadd_rn(a, 1.f)), 2.f));
 }
 
+// One action component of Normal(mu, sigma): the action rsample gives (loc + eps * scale) and, in `term`, its log_prob
+// term -((x - loc)^2) / (2 var) - log(scale) - log(sqrt(2 pi)).  two_var = 2 sigma^2, log_sd = log sigma.
+__device__ __forceinline__ float sample_action(float mu, float sd, float two_var, float log_sd, float eps, float& term) {
+    const float act = __fadd_rn(mu, __fmul_rn(sd, eps));
+    const float d = __fadd_rn(act, -mu);
+    term = __fdiv_rn(-__fmul_rn(d, d), two_var);
+    term = __fadd_rn(__fadd_rn(term, -log_sd), -0.9189385332046727f);
+    return act;
+}
+
+// the sampled action a of env at step t into the act slab; EXT: also scaled onto the user env's box for env.step
+template <bool EXT>
+__device__ __forceinline__ void store_action(const StepArgs& p, int t, int env, int a, float act) {
+    p.sl.act[((size_t)t * p.N + env) * p.es.A + a] = act;
+    if constexpr (EXT) p.act_env[(size_t)env * p.es.A + a] = action_scale(act, __ldg(p.act_lo + a), __ldg(p.act_hi + a));
+}
+
+// A path cut at a step without termination (time limit): its critics bootstrap from the final observation.
+__device__ __forceinline__ bool cut_path(unsigned f) { return (f & OSB_FLAG_TRUNCATED) && !(f & OSB_FLAG_TERMINATED); }
+
+// Critic output v of env (net 1: reward critic, 2: cost critic).  boot_cut: v is V(final observation of step t - 1),
+// stored where that path was cut; tail (t == T): v is the epoch-end bootstrap, stored unless the path ended at T - 1;
+// otherwise v is the value at step t.
+__device__ __forceinline__ void store_critic(const Slabs& sl, int net, int N, int t, int env, bool boot_cut, bool tail,
+                                             float v) {
+    if (boot_cut) {
+        const size_t idx = (size_t)(t - 1) * N + env;
+        if (cut_path(__ldcg(sl.flags + idx))) (net == 1 ? sl.boot_r : sl.boot_c)[idx] = v;
+    } else if (tail) {
+        const size_t idx = (size_t)(t - 1) * N + env;
+        if (__ldcg(sl.flags + idx) == 0) (net == 1 ? sl.boot_r : sl.boot_c)[idx] = v;
+    } else {
+        (net == 1 ? sl.val_r : sl.val_c)[(size_t)t * N + env] = v;
+    }
+}
+
 // normalise (or copy) a tile of raw observations into sX (chunk kc), zero padded.
 // z = per-env safety state (Saute) appended as column O of the network input (rows are On = O + 1 wide then), or null;
 // z_one: the final observations of finished episodes carry z = 1 (the state was reset before the augmentation).
@@ -319,10 +363,7 @@ __device__ __forceinline__ void load_obs_tile(const float* __restrict__ raw, int
         float v = 0.f;
         if (env < N && j < O) {
             v = raw[(size_t)env * O + j];
-            if (normalize) {
-                v = __fdiv_rn(__fadd_rn(v, -sMean[j]), sStd[j]);
-                v = fminf(fmaxf(v, -5.f), 5.f);
-            }
+            if (normalize) v = norm_clip(v, sMean[j], sStd[j]);
             if (obs_out) obs_out[(size_t)env * On + j] = v;
         } else if (env < N && j == O && z) {
             v = z_one ? 1.f : __ldcg(z + env);
@@ -350,6 +391,67 @@ __device__ __forceinline__ float saute_step(const SauteSpec& sa, int t, int N, i
     return out;
 }
 
+// Episode-end word of a synthetic env's step.  EP_EARLY: EarlyTerminated's cost limit ends the episode as a termination;
+// EP_BOTH: it does so in the step the env's own episode ends, so the env auto-resets and then the adapter resets it.
+enum : int { EP_FIN = 1, EP_TERM = 2, EP_TRUNC = 4, EP_EARLY = 8, EP_BOTH = 16 };
+
+// the env's own episode end: time limit and hash-driven termination
+__device__ __forceinline__ int episode_end(const EnvSpec& es, uint32_t gid, int ep_step, uint32_t gstep) {
+    const bool trunc = ep_step + 1 >= es.max_episode_steps;
+    const bool term = es.term_threshold != 0u && hash4(es.seed ^ 0xA5A5A5A5u, gid, gstep, 0xFFFFu) < es.term_threshold;
+    return ((term || trunc) ? EP_FIN : 0) | (term ? EP_TERM : 0) | (trunc ? EP_TRUNC : 0);
+}
+// the word after the accumulated cost exceeded the limit
+__device__ __forceinline__ int early_end(int fl) { return fl | ((fl & EP_FIN) ? EP_BOTH : 0) | EP_FIN | EP_TERM | EP_EARLY; }
+// episode counter after an episode end (the reset observation's hash input)
+__device__ __forceinline__ uint32_t next_episode(uint32_t epi, int fl) { return epi + ((fl & EP_BOTH) ? 2u : 1u); }
+
+// Step t of one env into the reward / cost / flags slabs, and the episode statistics (_log_value, _log_metrics,
+// _reset_log: onpolicy_adapter.py:L138-175): an episode that ends here leaves (EpRet, EpCost, EpLen) in epfin.
+// rew_store goes to the slab, rew_acc into the episode return (Saute stores its own reward; the return keeps the env's).
+__device__ __forceinline__ void record_step(const Slabs& sl, const EnvState& st, int T, int N, int t, int env,
+                                            float rew_store, float rew_acc, float cst, bool term, bool trunc) {
+    const size_t idx = (size_t)t * N + env;
+    sl.rew[idx] = rew_store;
+    sl.cost[idx] = cst;
+    sl.flags[idx] = (uint8_t)((term ? OSB_FLAG_TERMINATED : 0u) | (trunc ? OSB_FLAG_TRUNCATED : 0u));
+    const float er = __fadd_rn(st.ep_ret[env], rew_acc);
+    const float ec = __fadd_rn(st.ep_cost[env], cst);
+    const int el = st.ep_len[env] + 1;
+    if (term || trunc) {
+        const size_t TN = (size_t)T * N;
+        sl.epfin[idx] = er;
+        sl.epfin[TN + idx] = ec;
+        sl.epfin[2 * TN + idx] = (float)el;
+        st.ep_ret[env] = 0.f; st.ep_cost[env] = 0.f; st.ep_len[env] = 0;
+    } else {
+        st.ep_ret[env] = er; st.ep_cost[env] = ec; st.ep_len[env] = el;
+    }
+}
+
+// The end of a synthetic env's step t: reward 1 - mean_j s'_j^2 (sumsq = sum_j s'_j^2 in the spec's summation tree; 0 on
+// an EarlyTerminated end), cost = [s'_0 > cost_threshold], the Saute state, the step record and the env's counters.
+// ep_step / epi / gstep are the values before the step, acc_cost the EarlyTerminated accumulator including this step.  They
+// are references so that the tensor-core kernel's shared-memory copies are read where they are used, not held in registers
+// across the divisions.
+__device__ __forceinline__ void synthetic_step_end(const StepArgs& p, int N, int T, int O, int t, int env, int fl,
+                                                   float sumsq, float s0n, const int& ep_step, const uint32_t& epi,
+                                                   const uint32_t& gstep, const float& acc_cost) {
+    const bool fin = fl & EP_FIN, early = fl & EP_EARLY;
+    const float rew = early ? 0.f : __fadd_rn(1.f, -__fdiv_rn(sumsq, (float)O));
+    const float cst = (s0n > p.es.cost_threshold) ? 1.f : 0.f;
+    record_step(p.sl, p.st, T, N, t, env, saute_step(p.sa, t, N, env, rew, cst, fin), rew, cst, fl & EP_TERM,
+                fl & EP_TRUNC);
+    if (p.et.cost_acc) p.et.cost_acc[env] = early ? 0.f : acc_cost;
+    if (fin) {
+        p.st.episode[env] = next_episode(epi, fl);
+        p.st.ep_step[env] = 0;
+    } else {
+        p.st.ep_step[env] = ep_step + 1;
+    }
+    p.st.gstep[env] = gstep + 1u;
+}
+
 // EXT = true: the act half of a step on a user env (csrc: osb_ext_act).  The network part is the same; the actor CTAs
 // hand the scaled action to the env through p.act_env instead of running the synthetic transition, and the normaliser is
 // fed by the observe kernel after env.step.
@@ -370,11 +472,11 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
     float* sRew = base;  base += RT;
     float* sCost = base; base += RT;
     int* sFlag = reinterpret_cast<int*>(base); base += RT;
-    __shared__ int s_last, s_anyfin;
+    __shared__ int s_anyfin;
 
     const int net = p.is_tail ? (int)blockIdx.y + 1 : (int)blockIdx.y;
     const int env0 = blockIdx.x * RT;
-    const int O = p.es.O, A = p.es.A, N = p.N, T = p.T, t = p.t;
+    const int O = p.es.O, A = p.es.A, N = p.N, t = p.t;
     const int On = O + (p.sa.safety ? 1 : 0);            // network input width (Saute: [obs | z])
     const float* z_cur = p.sa.safety ? p.sa.safety + (size_t)(t & 1) * N : nullptr;
     const int nchunks = (On + KC - 1) / KC;
@@ -396,10 +498,8 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
     if (net != 0 && t > 0) {
         if (threadIdx.x == 0) s_anyfin = 0;
         __syncthreads();
-        if (threadIdx.x < RT && env0 + threadIdx.x < N) {
-            const unsigned f = p.sl.flags[(size_t)(t - 1) * N + env0 + threadIdx.x];
-            if ((f & OSB_FLAG_TRUNCATED) && !(f & OSB_FLAG_TERMINATED)) s_anyfin = 1;
-        }
+        if (threadIdx.x < RT && env0 + threadIdx.x < N && cut_path(p.sl.flags[(size_t)(t - 1) * N + env0 + threadIdx.x]))
+            s_anyfin = 1;
         __syncthreads();
         if (s_anyfin) {
             const bool norm1 = p.es.obs_normalize && p.ns.count[1] > 1;
@@ -415,12 +515,8 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
             __syncthreads();
             mlp_hidden<RT>(sX, sH1, sH2, W, nchunks, load_chunk_fin);
             mlp_out<RT>(sH2, sO, W, 1);
-            if (threadIdx.x < RT && env0 + threadIdx.x < N) {
-                const size_t idx = (size_t)(t - 1) * N + env0 + threadIdx.x;
-                const unsigned f = p.sl.flags[idx];
-                if ((f & OSB_FLAG_TRUNCATED) && !(f & OSB_FLAG_TERMINATED))
-                    (net == 1 ? p.sl.boot_r : p.sl.boot_c)[idx] = sO[threadIdx.x * LDO];
-            }
+            if (threadIdx.x < RT && env0 + threadIdx.x < N)
+                store_critic(p.sl, net, N, t, env0 + threadIdx.x, true, false, sO[threadIdx.x * LDO]);
             __syncthreads();
             if (nchunks > 1) { load_w1_chunk(theta, L, 0, W); }
         }
@@ -442,18 +538,8 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
     mlp_hidden<RT>(sX, sH1, sH2, W, nchunks, load_chunk_cur);
     mlp_out<RT>(sH2, sO, W, L.out);
 
-    if (net != 0) {
-        if (threadIdx.x < RT && env0 + threadIdx.x < N) {
-            const float v = sO[threadIdx.x * LDO];
-            if (!p.is_tail) {
-                (net == 1 ? p.sl.val_r : p.sl.val_c)[(size_t)t * N + env0 + threadIdx.x] = v;
-            } else {
-                // epoch end: bootstrap with V(next obs) unless the path already ended at T-1
-                const size_t idx = (size_t)(T - 1) * N + env0 + threadIdx.x;
-                if (p.sl.flags[idx] == 0) (net == 1 ? p.sl.boot_r : p.sl.boot_c)[idx] = v;
-            }
-        }
-    }
+    if (net != 0 && threadIdx.x < RT && env0 + threadIdx.x < N)
+        store_critic(p.sl, net, N, t, env0 + threadIdx.x, false, p.is_tail, sO[threadIdx.x * LDO]);
 
     // ---- actor CTA: sample, log-prob ---------------------------------------------------------
     if (net == 0) {
@@ -471,18 +557,11 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
             if (ok)
                 eps = p.eps ? p.eps[(size_t)env * A + a]
                             : philox_normal(p.noise_seed, p.es.env_id_offset + env, gstep, a);
-            const float act = __fadd_rn(mu, __fmul_rn(sd, eps));   // Normal.rsample: loc + eps*scale
-            // Normal.log_prob: -((x-loc)^2)/(2 var) - log(scale) - log(sqrt(2 pi))
-            const float d = __fadd_rn(act, -mu);
-            const float var = __fmul_rn(sd, sd);
-            float term = __fdiv_rn(-__fmul_rn(d, d), __fmul_rn(2.f, var));
-            term = __fadd_rn(__fadd_rn(term, -logf(sd)), -0.9189385332046727f);
+            float term;
+            const float act = sample_action(mu, sd, __fmul_rn(2.f, __fmul_rn(sd, sd)), logf(sd), eps, term);
             lp += term;
             sAct[e * OUTP + a] = act;
-            if (ok) p.sl.act[((size_t)t * N + env) * A + a] = act;
-            if constexpr (EXT) {
-                if (ok) p.act_env[(size_t)env * A + a] = action_scale(act, __ldg(p.act_lo + a), __ldg(p.act_hi + a));
-            }
+            if (ok) store_action<EXT>(p, t, env, a, act);
         }
         lp += __shfl_xor_sync(0xffffffffu, lp, 1);
         lp += __shfl_xor_sync(0xffffffffu, lp, 2);
@@ -498,20 +577,17 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
         const int env = env0 + e;
         const bool ok = env < N;
         const uint32_t gid = p.es.env_id_offset + env;
-        int ep_step = 0; uint32_t epi = 0, gstep = 0;
-        if (ok) { ep_step = p.st.ep_step[env]; epi = p.st.episode[env]; gstep = p.st.gstep[env]; }
-        const bool trunc = ok && (ep_step + 1 >= p.es.max_episode_steps);
-        const bool term = ok && p.es.term_threshold != 0u &&
-                          hash4(p.es.seed ^ 0xA5A5A5A5u, gid, gstep, 0xFFFFu) < p.es.term_threshold;
-        const bool fin_env = term || trunc;               // the env's own episode end
-        bool early = false;                               // EarlyTerminated: accumulated cost over the limit
+        int ep_step = 0, fl = 0; uint32_t epi = 0, gstep = 0;
         float acc_cost = 0.f;
-        if (ok && p.et.cost_acc) {
-            acc_cost = __fadd_rn(p.et.cost_acc[env], env_step_cost(p.es, s_cur[(size_t)env * O], sAct[e * OUTP], __ldg(p.st.bias)));
-            early = acc_cost > p.et.cost_limit;
+        if (ok) {
+            ep_step = p.st.ep_step[env]; epi = p.st.episode[env]; gstep = p.st.gstep[env];
+            fl = episode_end(p.es, gid, ep_step, gstep);
+            if (p.et.cost_acc) {
+                acc_cost = __fadd_rn(p.et.cost_acc[env], env_step_cost(p.es, s_cur[(size_t)env * O], sAct[e * OUTP], __ldg(p.st.bias)));
+                if (acc_cost > p.et.cost_limit) fl = early_end(fl);
+            }
         }
-        const bool fin = fin_env || early;
-        const uint32_t epi_inc = (fin_env && early) ? 2u : 1u;   // the env's auto-reset and then the adapter's reset
+        const bool fin = fl & EP_FIN;
         float part = 0.f, s0n = 0.f;
         float* finrow = p.st.final_raw + ((size_t)(t & 1) * N + (ok ? env : 0)) * O;
         for (int c0 = 0; c0 < O; c0 += KC) {
@@ -527,7 +603,7 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
                     part = __fadd_rn(part, __fmul_rn(sn, sn));
                     if (j == 0) s0n = sn;
                     fv = sn;
-                    nv = fin ? env_reset_value(p.es, gid, epi + epi_inc, j) : sn;
+                    nv = fin ? env_reset_value(p.es, gid, next_episode(epi, fl), j) : sn;
                     s_nxt[(size_t)env * O + j] = nv;
                     if (fin) finrow[j] = sn;
                 }
@@ -549,46 +625,16 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
                                 fx += to_fix(w); fxx += to_fix(__fmul_rn(w, w));
                             }
                         }
-                    atomicAdd((unsigned long long*)(p.ns.acc_all + j), (unsigned long long)sx);
-                    atomicAdd((unsigned long long*)(p.ns.acc_all + O + j), (unsigned long long)sxx);
-                    if (fx != 0 || fxx != 0) {
-                        atomicAdd((unsigned long long*)(p.ns.acc_fin + j), (unsigned long long)fx);
-                        atomicAdd((unsigned long long*)(p.ns.acc_fin + O + j), (unsigned long long)fxx);
-                    }
+                    push_fix_sums(p.ns, O, j, sx, sxx, fx, fxx);
                 }
             }
             __syncthreads();
         }
-        // reward = 1 - mean_j s'_j^2 with the fixed summation tree shared with the oracle
+        // sum_j s'_j^2 in the fixed summation tree shared with the oracle
         part = __fadd_rn(part, __shfl_xor_sync(0xffffffffu, part, 1));
         part = __fadd_rn(part, __shfl_xor_sync(0xffffffffu, part, 2));
         part = __fadd_rn(part, __shfl_xor_sync(0xffffffffu, part, 4));
-        if (ok && q == 0) {
-            const float rew = early ? 0.f : __fadd_rn(1.f, -__fdiv_rn(part, (float)O));
-            const float cst = (s0n > p.es.cost_threshold) ? 1.f : 0.f;
-            const size_t idx = (size_t)t * N + env;
-            p.sl.rew[idx] = saute_step(p.sa, t, N, env, rew, cst, fin);
-            p.sl.cost[idx] = cst;
-            p.sl.flags[idx] = (uint8_t)(((term || early) ? OSB_FLAG_TERMINATED : 0u) | (trunc ? OSB_FLAG_TRUNCATED : 0u));
-            if (p.et.cost_acc) p.et.cost_acc[env] = early ? 0.f : acc_cost;
-            // adapter bookkeeping: _log_value, _log_metrics, _reset_log (onpolicy_adapter.py:L138-175)
-            const float er = __fadd_rn(p.st.ep_ret[env], rew);
-            const float ec = __fadd_rn(p.st.ep_cost[env], cst);
-            const int el = p.st.ep_len[env] + 1;
-            if (fin) {
-                const size_t TN = (size_t)T * N;
-                p.sl.epfin[idx] = er;
-                p.sl.epfin[TN + idx] = ec;
-                p.sl.epfin[2 * TN + idx] = (float)el;
-                p.st.ep_ret[env] = 0.f; p.st.ep_cost[env] = 0.f; p.st.ep_len[env] = 0;
-                p.st.episode[env] = epi + epi_inc;
-                p.st.ep_step[env] = 0;
-            } else {
-                p.st.ep_ret[env] = er; p.st.ep_cost[env] = ec; p.st.ep_len[env] = el;
-                p.st.ep_step[env] = ep_step + 1;
-            }
-            p.st.gstep[env] = gstep + 1u;
-        }
+        if (ok && q == 0) synthetic_step_end(p, N, p.T, O, t, env, fl, part, s0n, ep_step, epi, gstep, acc_cost);
         if (p.es.obs_normalize && threadIdx.x == 0) {
             int nf = 0;
             for (int r = 0; r < RT; ++r) nf += (env0 + r < N) ? sFlag[r] : 0;
@@ -597,14 +643,7 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
     }
     // every CTA (actor and critic) has now consumed the normaliser state of this step; the last
     // one to arrive folds the step's sums into it for the next launch.
-    if (p.es.obs_normalize && !p.is_tail) {
-        __threadfence();
-        __syncthreads();
-        if (threadIdx.x == 0)
-            s_last = (atomicAdd(p.ns.ticket, 1u) == gridDim.x * gridDim.y - 1) ? 1 : 0;
-        __syncthreads();
-        if (s_last) norm_finalize(p.ns, O, (long long)N);
-    }
+    if (p.es.obs_normalize && !p.is_tail && last_cta(p.ns.ticket)) norm_finalize(p.ns, O, (long long)N);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -620,6 +659,24 @@ constexpr int SNW = KC + 1;   // row stride of the next-state staging tiles
 // one bf16x3 activation buffer (X, H1, H2 overwrite each other in place), accurate tanh, warp-uniform MMA issue.
 constexpr uint32_t RX_SUB = RTC * 128, RX_WSUB = 64 * 128, RX_W3SUB = 16 * 128;
 constexpr uint32_t RTC_FOFF_TF32 = 2 * RTC * 256 + 2 * 16384 + 4096, RTC_FOFF_X3 = 3 * RX_SUB + 6 * RX_WSUB + 3 * RX_W3SUB;
+// the 4-byte-word region after the operand tiles (all offsets in words)
+constexpr int TF_B1 = 0;                          // [64] layer biases
+constexpr int TF_B2 = TF_B1 + 64;                 // [64]
+constexpr int TF_B3 = TF_B2 + 64;                 // [16]
+constexpr int TF_MEAN = TF_B3 + 16;               // [64] ObsNormalize mean
+constexpr int TF_STD = TF_MEAN + 64;              // [64] ObsNormalize std
+constexpr int TF_ACT = TF_STD + 64;               // [128][16] mu, then the sampled action
+constexpr int TF_RAW = TF_ACT + RTC * OUTP;       // [128][65] raw current state of the tile (actor CTAs; kept by the obs staging)
+constexpr int TF_SN = TF_RAW + RTC * SNW;         // [128][65] state after the transition, before any reset
+constexpr int TF_ACC = TF_SN + RTC * SNW;         // long long [4][4][64] partial fixed-point sums
+constexpr int TF_FLAG = TF_ACC + 2 * 4 * 4 * 64;  // [128] episode-end word (EP_*)
+constexpr int TF_EPI = TF_FLAG + RTC;             // [128] episode counter
+constexpr int TF_STEP = TF_EPI + RTC;             // [128] step inside the episode
+constexpr int TF_GSTEP = TF_STEP + RTC;           // [128] total steps of the env (termination hash counter)
+constexpr int TF_SD = TF_GSTEP + RTC;             // [3][16] sigma, 2 sigma^2, log sigma per action
+constexpr int TF_EARLY = TF_SD + 48;              // [128] accumulated cost incl. this step (EarlyTerminated)
+constexpr int TF_WORDS = TF_EARLY + RTC;
+static_assert(TF_ACC % 2 == 0, "the fixed-point sums need 8-byte alignment");
 
 // PERSIST = true: ONE cooperative launch runs the whole epoch (steps 0 .. T, the last one being the critics' epoch-end
 // bootstrap): the weight tiles, biases and the accumulator image allocation stay resident, every step ends in a grid barrier whose
@@ -639,21 +696,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
     const uint32_t sW1 = X3 ? B0 + 3 * RX_SUB : B2 + RTC * 256;
     const uint32_t sW2 = sW1 + (X3 ? 3 * RX_WSUB : 16384u), sW3 = sW2 + (X3 ? 3 * RX_WSUB : 16384u);
     float* fbase = reinterpret_cast<float*>(smem_raw + pad + (X3 ? RTC_FOFF_X3 : RTC_FOFF_TF32));
-    float* sB1 = fbase;            // [64]
-    float* sB2 = sB1 + 64;         // [64]
-    float* sB3 = sB2 + 64;         // [16]
-    float* sMean = sB3 + 16;       // [64]
-    float* sRstd = sMean + 64;     // [64]  1 / std
-    float* sAct = sRstd + 64;      // [128][16]
-    float* sRaw = sAct + RTC * OUTP;           // [128][65] raw current state of the tile (actor CTAs; kept by the obs staging)
-    float* sSn = sRaw + RTC * SNW;             // [128][65] state after the transition, before any reset
-    long long* sAcc = reinterpret_cast<long long*>(sSn + RTC * SNW);    // [4][4][64] partial fixed-point sums
-    int* sFlag = reinterpret_cast<int*>(sAcc + 4 * 4 * 64);             // [128] bit 0 finished, bit 1 terminated, bit 2 truncated
-    uint32_t* sEpi = reinterpret_cast<uint32_t*>(sFlag + RTC);          // [128] episode counter
-    int* sStep = reinterpret_cast<int*>(sEpi + RTC);                    // [128] step inside the episode
-    uint32_t* sGstep = reinterpret_cast<uint32_t*>(sStep + RTC);        // [128] total steps of the env (termination hash counter)
-    float* sSd = reinterpret_cast<float*>(sGstep + RTC);                // [3][16] sigma, 2 sigma^2, log sigma per action
-    float* sEarlyAcc = sSd + 48;                                        // [128] accumulated cost incl. this step (EarlyTerminated)
+    float* sB1 = fbase + TF_B1;
+    float* sB2 = fbase + TF_B2;
+    float* sB3 = fbase + TF_B3;
+    float* sMean = fbase + TF_MEAN;
+    float* sStd = fbase + TF_STD;
+    float* sAct = fbase + TF_ACT;
+    float* sRaw = fbase + TF_RAW;
+    float* sSn = fbase + TF_SN;
+    long long* sAcc = reinterpret_cast<long long*>(fbase + TF_ACC);
+    int* sFlag = reinterpret_cast<int*>(fbase + TF_FLAG);
+    uint32_t* sEpi = reinterpret_cast<uint32_t*>(fbase + TF_EPI);
+    int* sStep = reinterpret_cast<int*>(fbase + TF_STEP);
+    uint32_t* sGstep = reinterpret_cast<uint32_t*>(fbase + TF_GSTEP);
+    float* sSd = fbase + TF_SD;
+    float* sEarlyAcc = fbase + TF_EARLY;
     __shared__ uint64_t bar;
     __shared__ int s_last, s_anyfin;
 
@@ -766,20 +823,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
         int fl = 0, ep_step = 0; uint32_t epi = 0, gstep = 0;
         if (env < N) {
             ep_step = p.st.ep_step[env]; epi = p.st.episode[env]; gstep = p.st.gstep[env];
-            const bool trunc = ep_step + 1 >= p.es.max_episode_steps;
-            const bool term = p.es.term_threshold != 0u &&
-                              hash4(p.es.seed ^ 0xA5A5A5A5u, p.es.env_id_offset + env, gstep, 0xFFFFu) < p.es.term_threshold;
-            fl = ((term || trunc) ? 1 : 0) | (term ? 2 : 0) | (trunc ? 4 : 0);
+            fl = episode_end(p.es, p.es.env_id_offset + env, ep_step, gstep);
         }
         sFlag[tid] = fl; sEpi[tid] = epi; sStep[tid] = ep_step; sGstep[tid] = gstep;
     }
     RSTAMP(1);
 
     // does this critic tile need bootstrap values for paths cut in the previous step?
-    if (net != 0 && t > 0 && tid < RTC && env0 + tid < N) {
-        const unsigned f = __ldcg(p.sl.flags + (size_t)(t - 1) * N + env0 + tid);
-        if ((f & OSB_FLAG_TRUNCATED) && !(f & OSB_FLAG_TERMINATED)) s_anyfin = 1;
-    }
+    if (net != 0 && t > 0 && tid < RTC && env0 + tid < N && cut_path(__ldcg(p.sl.flags + (size_t)(t - 1) * N + env0 + tid)))
+        s_anyfin = 1;
     __syncthreads();
     const int first_pass = (net != 0 && t > 0 && s_anyfin) ? 0 : 1;
 
@@ -792,7 +844,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
         const bool norm_on = pass ? normalize : (p.es.obs_normalize && __ldcg(p.ns.count + 1) > 1);
         float* obs_out = (pass && net == 0) ? p.sl.obs + (size_t)t * N * On : nullptr;
         const bool own_state = PERSIST && pass && net == 0 && t > t_first;
-        if (tid < 64) { sMean[tid] = (tid < O) ? __ldcg(gmean + tid) : 0.f; sRstd[tid] = (tid < O) ? __ldcg(gstd + tid) : 1.f; }
+        if (tid < 64) { sMean[tid] = (tid < O) ? __ldcg(gmean + tid) : 0.f; sStd[tid] = (tid < O) ? __ldcg(gstd + tid) : 1.f; }
         __syncthreads();
         if ((O & 3) == 0 && On == O) {   // 128-bit row loads, all 8 in flight per thread
             const int kq = tid & 15, k4 = kq << 2;
@@ -808,7 +860,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                                             : make_float4(0.f, 0.f, 0.f, 0.f);
             }
             const float m0 = sMean[k4], m1 = sMean[k4 + 1], m2 = sMean[k4 + 2], m3 = sMean[k4 + 3];
-            const float r0 = sRstd[k4], r1 = sRstd[k4 + 1], r2 = sRstd[k4 + 2], r3 = sRstd[k4 + 3];
+            const float s0 = sStd[k4], s1 = sStd[k4 + 1], s2 = sStd[k4 + 2], s3 = sStd[k4 + 3];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 const int e = (tid >> 4) + 16 * j;
@@ -817,10 +869,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                 if (pass && net == 0 && k4 < O) { float* r = sRaw + e * SNW + k4; r[0] = v.x; r[1] = v.y; r[2] = v.z; r[3] = v.w; }
                 if (env < N && k4 < O) {
                     if (norm_on) {
-                        v.x = fminf(fmaxf(__fdiv_rn(__fadd_rn(v.x, -m0), r0), -5.f), 5.f);
-                        v.y = fminf(fmaxf(__fdiv_rn(__fadd_rn(v.y, -m1), r1), -5.f), 5.f);
-                        v.z = fminf(fmaxf(__fdiv_rn(__fadd_rn(v.z, -m2), r2), -5.f), 5.f);
-                        v.w = fminf(fmaxf(__fdiv_rn(__fadd_rn(v.w, -m3), r3), -5.f), 5.f);
+                        v.x = norm_clip(v.x, m0, s0);
+                        v.y = norm_clip(v.y, m1, s1);
+                        v.z = norm_clip(v.z, m2, s2);
+                        v.w = norm_clip(v.w, m3, s3);
                     }
                     if (obs_out) *reinterpret_cast<float4*>(obs_out + (size_t)env * O + k4) = v;
                 }
@@ -840,7 +892,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
             }
         } else {
             const int k = tid & 63;
-            const float mk = sMean[k], sk = sRstd[k];
+            const float mk = sMean[k], sk = sStd[k];
 #pragma unroll 8
             for (int j = 0; j < 32; ++j) {
                 const int e = (tid >> 6) + 4 * j;
@@ -849,7 +901,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                 if (env < N && k < O) {
                     v = own_state ? sRaw[e * SNW + k] : __ldcg(raw + (size_t)env * O + k);
                     if (pass && net == 0) sRaw[e * SNW + k] = v;
-                    if (norm_on) v = fminf(fmaxf(__fdiv_rn(__fadd_rn(v, -mk), sk), -5.f), 5.f);
+                    if (norm_on) v = norm_clip(v, mk, sk);
                     if (obs_out) obs_out[(size_t)env * On + k] = v;
                 }
                 if constexpr (X3) x3::store1_x3(B0, RX_SUB, x3::off128(e, k), v);
@@ -947,20 +999,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
             const int e = 32 * q + lane;
             const int env = env0 + e;
             if (net != 0) {
-                if (env < N) {
-                    const float v = o16[0] + sB3[0];
-                    if (pass == 0) {
-                        const size_t idx = (size_t)(t - 1) * N + env;
-                        const unsigned f = __ldcg(p.sl.flags + idx);
-                        if ((f & OSB_FLAG_TRUNCATED) && !(f & OSB_FLAG_TERMINATED))
-                            (net == 1 ? p.sl.boot_r : p.sl.boot_c)[idx] = v;
-                    } else if (!is_tail) {
-                        (net == 1 ? p.sl.val_r : p.sl.val_c)[(size_t)t * N + env] = v;
-                    } else {
-                        const size_t idx = (size_t)(T - 1) * N + env;
-                        if (__ldcg(p.sl.flags + idx) == 0) (net == 1 ? p.sl.boot_r : p.sl.boot_c)[idx] = v;
-                    }
-                }
+                if (env < N) store_critic(p.sl, net, N, t, env, pass == 0, is_tail, o16[0] + sB3[0]);
             } else {
 #pragma unroll
                 for (int a = 0; a < 16; ++a) sAct[e * OUTP + a] = o16[a] + sB3[a];   // mu
@@ -981,28 +1020,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                 const int e = 64 * g + (tid >> 2);
                 const int env = env0 + e;
                 const bool ok = env < N;
-                float n0 = 0.f, n1 = 0.f;
+                float2 n = make_float2(0.f, 0.f);
                 if (ok && a0 < A) {
-                    if (eps_t) { n0 = eps_t[(size_t)env * A + a0]; n1 = (a1 < A) ? eps_t[(size_t)env * A + a1] : 0.f; }
-                    else philox_normal2(p.noise_seed, p.es.env_id_offset + env, EXT ? act_global_step(p) : gstep_t, pr, n0, n1);
+                    if (eps_t) { n.x = eps_t[(size_t)env * A + a0]; n.y = (a1 < A) ? eps_t[(size_t)env * A + a1] : 0.f; }
+                    else n = philox_normal2(p.noise_seed, p.es.env_id_offset + env, EXT ? act_global_step(p) : gstep_t, pr);
                 }
                 float lp = 0.f;
 #pragma unroll
                 for (int u = 0; u < 2; ++u) {
                     const int a = a0 + u;
                     if (a < A) {
-                        const float mu = sAct[e * OUTP + a];
-                        const float sd = sSd[a];
-                        const float act = __fadd_rn(mu, __fmul_rn(sd, u ? n1 : n0));      // Normal.rsample: loc + eps * scale
-                        const float d = __fadd_rn(act, -mu);
-                        float term = __fdiv_rn(-__fmul_rn(d, d), sSd[16 + a]);               // / (2 var)
-                        term = __fadd_rn(__fadd_rn(term, -sSd[32 + a]), -0.9189385332046727f);
+                        float term;
+                        const float act = sample_action(sAct[e * OUTP + a], sSd[a], sSd[16 + a], sSd[32 + a], u ? n.y : n.x, term);
                         lp += term;
                         sAct[e * OUTP + a] = act;
-                        if (ok) p.sl.act[((size_t)t * N + env) * A + a] = act;
-                        if constexpr (EXT) {
-                            if (ok) p.act_env[(size_t)env * A + a] = action_scale(act, __ldg(p.act_lo + a), __ldg(p.act_hi + a));
-                        }
+                        if (ok) store_action<EXT>(p, t, env, a, act);
                     }
                 }
                 lp += __shfl_xor_sync(0xffffffffu, lp, 1);
@@ -1018,22 +1050,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                 const bool ok = env < N;
                 float lp = 0.f;
                 for (int a = qq; a < A; a += 8) {
-                    const float mu = sAct[e * OUTP + a];
-                    const float sd = sSd[a];
                     float eps = 0.f;
                     if (ok)
                         eps = eps_t ? eps_t[(size_t)env * A + a]
                                     : philox_normal(p.noise_seed, p.es.env_id_offset + env, EXT ? act_global_step(p) : gstep_t, a);
-                    const float act = __fadd_rn(mu, __fmul_rn(sd, eps));
-                    const float d = __fadd_rn(act, -mu);
-                    float term = __fdiv_rn(-__fmul_rn(d, d), sSd[16 + a]);
-                    term = __fadd_rn(__fadd_rn(term, -sSd[32 + a]), -0.9189385332046727f);
+                    float term;
+                    const float act = sample_action(sAct[e * OUTP + a], sSd[a], sSd[16 + a], sSd[32 + a], eps, term);
                     lp += term;
                     sAct[e * OUTP + a] = act;
-                    if (ok) p.sl.act[((size_t)t * N + env) * A + a] = act;
-                    if constexpr (EXT) {
-                        if (ok) p.act_env[(size_t)env * A + a] = action_scale(act, __ldg(p.act_lo + a), __ldg(p.act_hi + a));
-                    }
+                    if (ok) store_action<EXT>(p, t, env, a, act);
                 }
                 lp += __shfl_xor_sync(0xffffffffu, lp, 1);
                 lp += __shfl_xor_sync(0xffffffffu, lp, 2);
@@ -1047,7 +1072,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
             if (tid < RTC && env0 + tid < N) {
                 const int env = env0 + tid;
                 const float acc = __fadd_rn(p.et.cost_acc[env], env_step_cost(p.es, sRaw[tid * SNW], sAct[tid * OUTP], __ldg(p.st.bias)));
-                if (acc > p.et.cost_limit) sFlag[tid] |= ((sFlag[tid] & 1) ? 16 : 0) | 1 | 2 | 8;   // bit 3 early, bit 4 both ends at once
+                if (acc > p.et.cost_limit) sFlag[tid] = early_end(sFlag[tid]);
                 sEarlyAcc[tid] = acc;
             }
             __syncthreads();
@@ -1073,8 +1098,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                         const float sn = env_next_value(sRaw[e * SNW + j], a, bj);
                         const int fl = sFlag[e];
                         float nv = sn;
-                        if (fl & 1) {
-                            nv = env_reset_value(p.es, p.es.env_id_offset + env, sEpi[e] + ((fl & 16) ? 2u : 1u), j);
+                        if (fl & EP_FIN) {
+                            nv = env_reset_value(p.es, p.es.env_id_offset + env, next_episode(sEpi[e], fl), j);
                             p.st.final_raw[((size_t)(t & 1) * N + env) * O + j] = sn;
                             fx += to_fix(sn); fxx += to_fix(__fmul_rn(sn, sn));
                         }
@@ -1109,35 +1134,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
             }
             float tot = __fadd_rn(__fadd_rn(part[0], part[1]), __fadd_rn(part[2], part[3]));
             tot = __fadd_rn(tot, __shfl_xor_sync(0xffffffffu, tot, 1));
-            if (ok && e_half == 0) {
-                const int fl = sFlag[e_env];
-                const bool fin = fl & 1, term = fl & 2, trunc = fl & 4;
-                const uint32_t epi = sEpi[e_env];
-                const bool early = fl & 8;
-                const float rew = early ? 0.f : __fadd_rn(1.f, -__fdiv_rn(tot, (float)O));
-                const float cst = (sSn[e_env * SNW] > p.es.cost_threshold) ? 1.f : 0.f;
-                if (p.et.cost_acc) p.et.cost_acc[env] = early ? 0.f : sEarlyAcc[e_env];
-                const size_t idx = (size_t)t * N + env;
-                p.sl.rew[idx] = saute_step(p.sa, t, N, env, rew, cst, fin);
-                p.sl.cost[idx] = cst;
-                p.sl.flags[idx] = (uint8_t)((term ? OSB_FLAG_TERMINATED : 0u) | (trunc ? OSB_FLAG_TRUNCATED : 0u));
-                const float erv = __fadd_rn(p.st.ep_ret[env], rew);
-                const float ecv = __fadd_rn(p.st.ep_cost[env], cst);
-                const int el = p.st.ep_len[env] + 1;
-                if (fin) {
-                    const size_t TN = (size_t)T * N;
-                    p.sl.epfin[idx] = erv;
-                    p.sl.epfin[TN + idx] = ecv;
-                    p.sl.epfin[2 * TN + idx] = (float)el;
-                    p.st.ep_ret[env] = 0.f; p.st.ep_cost[env] = 0.f; p.st.ep_len[env] = 0;
-                    p.st.episode[env] = epi + ((fl & 16) ? 2u : 1u);
-                    p.st.ep_step[env] = 0;
-                } else {
-                    p.st.ep_ret[env] = erv; p.st.ep_cost[env] = ecv; p.st.ep_len[env] = el;
-                    p.st.ep_step[env] = sStep[e_env] + 1;
-                }
-                p.st.gstep[env] = sGstep[e_env] + 1u;
-            }
+            if (ok && e_half == 0)
+                synthetic_step_end(p, N, T, O, t, env, sFlag[e_env], tot, sSn[e_env * SNW], sStep[e_env], sEpi[e_env], sGstep[e_env],
+                                   sEarlyAcc[e_env]);
         }
         if (p.es.obs_normalize) {
             if (tid < O) {
@@ -1146,16 +1145,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                     a0 += sAcc[(gg * 4 + 0) * 64 + tid]; a1 += sAcc[(gg * 4 + 1) * 64 + tid];
                     a2 += sAcc[(gg * 4 + 2) * 64 + tid]; a3 += sAcc[(gg * 4 + 3) * 64 + tid];
                 }
-                atomicAdd((unsigned long long*)(p.ns.acc_all + tid), (unsigned long long)a0);
-                atomicAdd((unsigned long long*)(p.ns.acc_all + O + tid), (unsigned long long)a1);
-                if (a2 != 0 || a3 != 0) {
-                    atomicAdd((unsigned long long*)(p.ns.acc_fin + tid), (unsigned long long)a2);
-                    atomicAdd((unsigned long long*)(p.ns.acc_fin + O + tid), (unsigned long long)a3);
-                }
+                push_fix_sums(p.ns, O, tid, a0, a1, a2, a3);
             }
             if (tid == 64) {
                 int nfin = 0;
-                for (int r = 0; r < RTC; ++r) nfin += (env0 + r < N) ? (sFlag[r] & 1) : 0;
+                for (int r = 0; r < RTC; ++r) nfin += (env0 + r < N) ? (sFlag[r] & EP_FIN) : 0;
                 if (nfin) atomicAdd(p.ns.fin_count, nfin);
             }
         }
@@ -1180,22 +1174,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
             __syncthreads();
             RSTAMP(10);
         }
-    } else if (!EXT && p.es.obs_normalize && !is_tail) {
-        __threadfence();
-        __syncthreads();
-        if (tid == 0) s_last = (atomicAdd(p.ns.ticket, 1u) == gridDim.x * gridDim.y - 1) ? 1 : 0;
-        __syncthreads();
-        if (s_last) norm_finalize(p.ns, O, (long long)N);
+    } else if (!EXT && p.es.obs_normalize && !is_tail && last_cta(p.ns.ticket)) {
+        norm_finalize(p.ns, O, (long long)N);
     }
     }   // step loop
 #undef RSTAMP
     __syncthreads();
 }
 
+// 1024: the alignment pad in front of the operand tiles
 static size_t rollout_tc_smem_bytes(bool x3) {
-    return 1024 + (x3 ? RTC_FOFF_X3 : RTC_FOFF_TF32) +
-           (64 + 64 + 16 + 64 + 64 + RTC * OUTP + 2 * RTC * SNW) * sizeof(float) + 4 * 4 * 64 * sizeof(long long) +
-           5 * RTC * sizeof(int) + 48 * sizeof(float) + 64;
+    return 1024 + (x3 ? RTC_FOFF_X3 : RTC_FOFF_TF32) + TF_WORDS * sizeof(float) + 64;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1233,7 +1222,7 @@ __device__ __forceinline__ void chan_combine(double& n, double& m, double& q, do
 __global__ void __launch_bounds__(NTHREADS) ext_observe_kernel(ExtObs x, EnvState st, NormState ns, Slabs sl, int O, int N,
                                                                int T, int t, int obs_normalize, int is_reset) {
     __shared__ int sFin[XT];
-    __shared__ int s_bad, s_last, s_nfin;
+    __shared__ int s_bad, s_nfin;
     const int tid = threadIdx.x, tile = blockIdx.x, ntiles = gridDim.x;
     const int env0 = tile * XT, rows = min(XT, N - env0);
     if (tid == 0) s_bad = 0;
@@ -1245,21 +1234,8 @@ __global__ void __launch_bounds__(NTHREADS) ext_observe_kernel(ExtObs x, EnvStat
                 st.ep_ret[env] = 0.f; st.ep_cost[env] = 0.f; st.ep_len[env] = 0;
             } else {
                 fin = (x.final_obs && x.final_mask && x.final_mask[env]) ? 1 : 0;
-                const float r = x.rew[env], c = x.cost[env];
-                const bool te = x.term[env] != 0, tr = x.trunc[env] != 0;
-                const size_t idx = (size_t)t * N + env;
-                sl.rew[idx] = r;
-                sl.cost[idx] = c;
-                sl.flags[idx] = (uint8_t)((te ? OSB_FLAG_TERMINATED : 0u) | (tr ? OSB_FLAG_TRUNCATED : 0u));
-                const float er = __fadd_rn(st.ep_ret[env], r), ec = __fadd_rn(st.ep_cost[env], c);
-                const int el = st.ep_len[env] + 1;
-                if (te || tr) {
-                    const size_t TN = (size_t)T * N;
-                    sl.epfin[idx] = er; sl.epfin[TN + idx] = ec; sl.epfin[2 * TN + idx] = (float)el;
-                    st.ep_ret[env] = 0.f; st.ep_cost[env] = 0.f; st.ep_len[env] = 0;
-                } else {
-                    st.ep_ret[env] = er; st.ep_cost[env] = ec; st.ep_len[env] = el;
-                }
+                const float r = x.rew[env];
+                record_step(sl, st, T, N, t, env, r, r, x.cost[env], x.term[env] != 0, x.trunc[env] != 0);
             }
         }
         sFin[tid] = fin;
@@ -1311,14 +1287,9 @@ __global__ void __launch_bounds__(NTHREADS) ext_observe_kernel(ExtObs x, EnvStat
         P[j] = m; P[O + j] = q; P[2 * O + j] = mf; P[3 * O + j] = qf;
     }
     if (tid == 0) x.part[(size_t)ntiles * 4 * O + tile] = (double)nf;
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) {
-        if (s_bad) *x.nonfinite = 1;
-        s_last = (atomicAdd(ns.ticket, 1u) == (unsigned)ntiles - 1u) ? 1 : 0;
-    }
-    __syncthreads();
-    if (!s_last) return;
+    const bool last = last_cta(ns.ticket);
+    if (tid == 0 && s_bad) *x.nonfinite = 1;
+    if (!last) return;
 
     // last CTA: combine the tiles in order and push final rows, then all rows (norm_finalize's sequence)
     __threadfence();
@@ -1469,6 +1440,12 @@ static size_t rollout_smem_bytes(int O) {   // O = network input width
     return f * sizeof(float);
 }
 
+static int launch_env_reset(const EnvSpec& es, const EnvState& st, const NormState& ns, int N, cudaStream_t stream) {
+    env_reset_kernel<<<(N + RT - 1) / RT, NTHREADS, 0, stream>>>(es, st, ns, g_saute, N);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}
+
 extern "C" {
 
 int osb_episode_window(const unsigned char* flags, const float* epfin, int T, int N, int W,
@@ -1487,14 +1464,34 @@ int osb_env_reset(int O, int A, int max_episode_steps, unsigned seed, unsigned t
     EnvState st{s_raw, final_raw, ep_step, episode, gstep, ep_ret, ep_cost, ep_len, bias};
     NormState ns{norm_mean, norm_sumsq, norm_std, norm_mean1, norm_std1, norm_count, acc_all,
                  acc_fin, fin_count, had_fin, ticket};
-    env_reset_kernel<<<(N + RT - 1) / RT, NTHREADS, 0, (cudaStream_t)stream>>>(es, st, ns, g_saute, N);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    return launch_env_reset(es, st, ns, N, (cudaStream_t)stream);
 }
 
 static long long* g_rollout_dbg = nullptr;
 
 }  // extern "C"
+
+// StepArgs of the synthetic env's step and epoch entries, which share this argument list
+static StepArgs synthetic_step_args(int O, int A, int max_episode_steps, unsigned seed, unsigned term_threshold,
+                                    unsigned env_id_offset, float cost_threshold, int obs_normalize, int N, int T,
+                                    float* s_raw, float* final_raw, int* ep_step, unsigned* episode, unsigned* gstep,
+                                    float* ep_ret, float* ep_cost, int* ep_len, const float* bias, float* norm_mean,
+                                    float* norm_sumsq, float* norm_std, float* norm_mean1, float* norm_std1,
+                                    long long* norm_count, long long* acc_all, long long* acc_fin, int* fin_count,
+                                    int* had_fin, unsigned* ticket, float* obs, float* act, float* logp, float* rew,
+                                    float* cost, float* val_r, float* val_c, float* boot_r, float* boot_c,
+                                    unsigned char* flags, float* epfin, const float* theta, unsigned noise_seed,
+                                    int precision) {
+    StepArgs p{};
+    p.es = EnvSpec{O, A, max_episode_steps, seed, term_threshold, env_id_offset, cost_threshold, obs_normalize};
+    p.st = EnvState{s_raw, final_raw, ep_step, episode, gstep, ep_ret, ep_cost, ep_len, bias};
+    p.ns = NormState{norm_mean, norm_sumsq, norm_std, norm_mean1, norm_std1, norm_count, acc_all,
+                     acc_fin, fin_count, had_fin, ticket};
+    p.sl = Slabs{obs, act, logp, rew, cost, val_r, val_c, boot_r, boot_c, flags, epfin};
+    p.sa = g_saute; p.et = g_early;
+    p.theta = theta; p.noise_seed = noise_seed; p.T = T; p.N = N; p.precision = precision;
+    return p;
+}
 
 // The one-time host actions of an act launch on an external env -- kernel attributes and the accumulator image -- call
 // cudaFuncSetAttribute / cudaMalloc, which CUDA-graph capture does not allow.  osb_ext_prepare performs them before a
@@ -1523,14 +1520,15 @@ static int launch_step(StepArgs& p, cudaStream_t stream, bool prepare_only = fal
         if (!attr_tc) {
             if constexpr (EXT) {
                 if (int rc = ext_refuse_if_capturing(stream, "the tensor-core kernel attributes")) return rc;
-                OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(false)));
-                OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(true)));
-            } else {
-                OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(false)));
-                OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(true)));
-                OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(false)));
-                OSB_CUDA(cudaFuncSetAttribute(rollout_step_tc_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollout_tc_smem_bytes(true)));
             }
+            // {tf32, bf16x3} x {one step, the persistent epoch}; EXT launches only the one-step pair
+            const void* kernels[] = {(const void*)rollout_step_tc_kernel<false, false, EXT>,
+                                     (const void*)rollout_step_tc_kernel<true, false, EXT>,
+                                     (const void*)rollout_step_tc_kernel<false, true>,
+                                     (const void*)rollout_step_tc_kernel<true, true>};
+            for (int i = 0; i < (EXT ? 2 : 4); ++i)
+                OSB_CUDA(cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (int)rollout_tc_smem_bytes(i & 1)));
             attr_tc = true;
         }
         dim3 grid_tc((p.N + RTC - 1) / RTC, p.is_tail ? 2 : 3);
@@ -1541,12 +1539,6 @@ static int launch_step(StepArgs& p, cudaStream_t stream, bool prepare_only = fal
         p.acc = acc_scratch(ACC_ROLLOUT, rollout_tc_acc_bytes(p.N));
         if (!p.acc) return OSB_ERR_CUDA;
         if (prepare_only) return OSB_OK;
-        if (EXT) {
-            if (x3) rollout_step_tc_kernel<true, false, true><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
-            else rollout_step_tc_kernel<false, false, true><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
-            OSB_LAUNCH_CHECK();
-            return OSB_OK;
-        }
         if (p.bar_ctr != nullptr) {
             // the whole epoch in one cooperative launch (every CTA resident: the step barrier is a software grid barrier)
             OSB_CUDA(cudaMemsetAsync(p.bar_ctr, 0, 2 * sizeof(unsigned int), stream));
@@ -1556,8 +1548,8 @@ static int launch_step(StepArgs& p, cudaStream_t stream, bool prepare_only = fal
                                                  dim3((p.N + RTC - 1) / RTC, 3), dim3(NTHREADS), args, smem_tc, stream));
             return OSB_OK;
         }
-        if (x3) rollout_step_tc_kernel<true, false><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
-        else rollout_step_tc_kernel<false, false><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
+        if (x3) rollout_step_tc_kernel<true, false, EXT><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
+        else rollout_step_tc_kernel<false, false, EXT><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
         OSB_LAUNCH_CHECK();
         return OSB_OK;
     }
@@ -1611,16 +1603,13 @@ int osb_rollout_step(int O, int A, int max_episode_steps, unsigned seed, unsigne
                      unsigned global_step, int precision, void* stream) {
     OSB_CHECK_ARG(O > 0 && A > 0 && A <= OUTP && N > 0 && T > 0, "bad dims (need 0 < A <= 16)");
     OSB_CHECK_ARG(t >= 0 && t <= T, "step index out of range");
-    StepArgs p;
-    p.es = EnvSpec{O, A, max_episode_steps, seed, term_threshold, env_id_offset, cost_threshold, obs_normalize};
-    p.st = EnvState{s_raw, final_raw, ep_step, episode, gstep, ep_ret, ep_cost, ep_len, bias};
-    p.ns = NormState{norm_mean, norm_sumsq, norm_std, norm_mean1, norm_std1, norm_count, acc_all,
-                     acc_fin, fin_count, had_fin, ticket};
-    p.sl = Slabs{obs, act, logp, rew, cost, val_r, val_c, boot_r, boot_c, flags, epfin};
-    p.sa = g_saute; p.et = g_early;
-    p.theta = theta; p.eps = eps; p.noise_seed = noise_seed; p.global_step = global_step;
-    p.t = t; p.T = T; p.N = N; p.is_tail = (t == T) ? 1 : 0; p.precision = precision;
-    p.bar_ctr = nullptr; p.bar_flag = nullptr; p.dbg = nullptr;
+    StepArgs p = synthetic_step_args(O, A, max_episode_steps, seed, term_threshold, env_id_offset, cost_threshold,
+                                     obs_normalize, N, T, s_raw, final_raw, ep_step, episode, gstep, ep_ret, ep_cost,
+                                     ep_len, bias, norm_mean, norm_sumsq, norm_std, norm_mean1, norm_std1, norm_count,
+                                     acc_all, acc_fin, fin_count, had_fin, ticket, obs, act, logp, rew, cost, val_r,
+                                     val_c, boot_r, boot_c, flags, epfin, theta, noise_seed, precision);
+    p.eps = eps; p.global_step = global_step;
+    p.t = t; p.is_tail = (t == T) ? 1 : 0;
     return launch_step<false>(p, (cudaStream_t)stream);
 }
 
@@ -1638,26 +1627,18 @@ int osb_rollout_epoch(int O, int A, int max_episode_steps, unsigned seed, unsign
                       int precision, void* stream) {
     OSB_CHECK_ARG(O > 0 && A > 0 && A <= OUTP && N > 0 && T > 0, "bad dims (need 0 < A <= 16)");
     cudaStream_t s = (cudaStream_t)stream;
-    int rc = osb_env_reset(O, A, max_episode_steps, seed, term_threshold, env_id_offset,
-                           cost_threshold, obs_normalize, N, s_raw, final_raw, ep_step, episode,
-                           gstep, ep_ret, ep_cost, ep_len, bias, norm_mean, norm_sumsq, norm_std,
-                           norm_mean1, norm_std1, norm_count, acc_all, acc_fin, fin_count, had_fin,
-                           ticket, stream);
+    StepArgs p = synthetic_step_args(O, A, max_episode_steps, seed, term_threshold, env_id_offset, cost_threshold,
+                                     obs_normalize, N, T, s_raw, final_raw, ep_step, episode, gstep, ep_ret, ep_cost,
+                                     ep_len, bias, norm_mean, norm_sumsq, norm_std, norm_mean1, norm_std1, norm_count,
+                                     acc_all, acc_fin, fin_count, had_fin, ticket, obs, act, logp, rew, cost, val_r,
+                                     val_c, boot_r, boot_c, flags, epfin, theta, noise_seed, precision);
+    int rc = launch_env_reset(p.es, p.st, p.ns, N, s);
     if (rc) return rc;
-    StepArgs p;
-    p.es = EnvSpec{O, A, max_episode_steps, seed, term_threshold, env_id_offset, cost_threshold, obs_normalize};
-    p.st = EnvState{s_raw, final_raw, ep_step, episode, gstep, ep_ret, ep_cost, ep_len, bias};
-    p.ns = NormState{norm_mean, norm_sumsq, norm_std, norm_mean1, norm_std1, norm_count, acc_all,
-                     acc_fin, fin_count, had_fin, ticket};
-    p.sl = Slabs{obs, act, logp, rew, cost, val_r, val_c, boot_r, boot_c, flags, epfin};
-    p.sa = g_saute; p.et = g_early;
-    p.theta = theta; p.noise_seed = noise_seed; p.T = T; p.N = N; p.precision = precision;
-    p.bar_ctr = nullptr; p.bar_flag = nullptr; p.dbg = g_rollout_dbg;
+    p.dbg = g_rollout_dbg;
     // tensor-core modes with every CTA resident (grid = env tiles x 3 networks <= SMs): one persistent launch per epoch
-    static const bool stepwise = getenv("OSB_ROLLOUT_STEPWISE") != nullptr;
     static int n_sm = 0;
     if (!n_sm) { int dev = 0; OSB_CUDA(cudaGetDevice(&dev)); OSB_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev)); }
-    if (!stepwise && (precision == 1 || precision == 2) && O + (g_saute.safety ? 1 : 0) <= 64 && ((N + RTC - 1) / RTC) * 3 <= n_sm) {
+    if ((precision == 1 || precision == 2) && O + (g_saute.safety ? 1 : 0) <= 64 && ((N + RTC - 1) / RTC) * 3 <= n_sm) {
         static unsigned int* d_bar = nullptr;
         if (!d_bar) OSB_CUDA(cudaMalloc(&d_bar, 64));
         p.bar_ctr = d_bar; p.bar_flag = d_bar + 1;
@@ -1729,6 +1710,16 @@ int osb_ext_observe(int O, int N, int T, int t, int obs_normalize, const float* 
 
 }  // extern "C"
 
+// StepArgs of the external-env act step: a user env, so no synthetic env, Saute or EarlyTerminated state
+static StepArgs ext_step_args(int O, int A, int obs_normalize, int N, int precision) {
+    StepArgs p{};
+    p.es = EnvSpec{O, A, 0, 0u, 0u, 0u, 0.f, obs_normalize};
+    p.sa = SauteSpec{nullptr, 1.f, 1.f, 0.f, 1.f};
+    p.et = EarlySpec{nullptr, 0.f};
+    p.N = N; p.precision = precision;
+    return p;
+}
+
 // one act launch of the external-env path; epoch_dev non-null: the Philox counter is read on the device
 static int ext_act(int O, int A, int obs_normalize, int N, int T, int t, unsigned env_id_offset, float* s_raw,
                    float* final_raw, float* norm_mean, float* norm_std, float* norm_mean1, float* norm_std1,
@@ -1739,16 +1730,13 @@ static int ext_act(int O, int A, int obs_normalize, int N, int T, int t, unsigne
     OSB_CHECK_ARG(O > 0 && A > 0 && A <= OUTP && N > 0 && T > 0, "bad dims (need 0 < A <= 16)");
     OSB_CHECK_ARG(t >= 0 && t <= T, "step index out of range");
     OSB_CHECK_ARG(t == T || (act_lo && act_hi && act_env), "act_lo / act_hi / act_env are required for t < T");
-    StepArgs p{};
-    p.es = EnvSpec{O, A, 0, 0u, 0u, env_id_offset, 0.f, obs_normalize};
-    p.st = EnvState{s_raw, final_raw, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    p.ns = NormState{norm_mean, nullptr, norm_std, norm_mean1, norm_std1, norm_count, nullptr, nullptr, nullptr, nullptr, nullptr};
+    StepArgs p = ext_step_args(O, A, obs_normalize, N, precision);
+    p.es.env_id_offset = env_id_offset;
+    p.st.s_raw = s_raw; p.st.final_raw = final_raw;
+    p.ns.mean = norm_mean; p.ns.std = norm_std; p.ns.mean1 = norm_mean1; p.ns.std1 = norm_std1; p.ns.count = norm_count;
     p.sl = Slabs{obs, act, logp, nullptr, nullptr, val_r, val_c, boot_r, boot_c, flags, nullptr};
-    p.sa = SauteSpec{nullptr, 1.f, 1.f, 0.f, 1.f};
-    p.et = EarlySpec{nullptr, 0.f};
     p.theta = theta; p.eps = eps; p.noise_seed = noise_seed; p.global_step = global_step;
-    p.t = t; p.T = T; p.N = N; p.is_tail = (t == T) ? 1 : 0; p.precision = precision;
-    p.bar_ctr = nullptr; p.bar_flag = nullptr; p.dbg = nullptr;
+    p.t = t; p.T = T; p.is_tail = (t == T) ? 1 : 0;
     p.act_lo = act_lo; p.act_hi = act_hi; p.act_env = act_env;
     p.epoch_dev = epoch_dev;
     return launch_step<true>(p, (cudaStream_t)stream);
@@ -1790,10 +1778,7 @@ int osb_ext_epoch_advance(unsigned* epoch_dev, void* stream) {
 
 int osb_ext_prepare(int O, int A, int N, int precision) {
     OSB_CHECK_ARG(O > 0 && A > 0 && A <= OUTP && N > 0, "bad dims (need 0 < A <= 16)");
-    StepArgs p{};
-    p.es = EnvSpec{O, A, 0, 0u, 0u, 0u, 0.f, 0};
-    p.sa = SauteSpec{nullptr, 1.f, 1.f, 0.f, 1.f};
-    p.N = N; p.precision = precision;
+    StepArgs p = ext_step_args(O, A, 0, N, precision);
     return launch_step<true>(p, nullptr, true);
 }
 
