@@ -192,6 +192,27 @@ int osb_ext_epoch_advance(unsigned* epoch_dev, void* stream);
 int osb_scalar_normalize_rows(float* x, int T, int N, float clip, float* state, long long* count,
                               float* workspace, void* stream);
 
+/* ---- policy step on a trained model (no env, no slabs) ------------------------------------------
+ * replaces ConstraintActorCritic.step          models/actor_critic/constraint_actor_critic.py:L84-109
+ *          GaussianLearningActor.predict / forward / log_prob   models/actor/gaussian_learning_actor.py:L64-139
+ *          VCritic.forward                       models/critic/v_critic.py:L75-92
+ * B >= 1 rows of already normalised observations obs[B][O] (what the model sees behind ObsNormalize); theta as above
+ * with 1 <= A <= 16 and hidden sizes [64, 64].  net_mask bit0 actor, bit1 reward critic, bit2 cost critic (at least
+ * one).  Actor: mean[B][A]; act[B][A] = mean + exp(log_std) * eps with eps[B][A] caller-supplied standard-normal draws
+ * (Normal.rsample), or act = mean when eps is NULL (deterministic); logp[B] = sum_a Normal(mean, std).log_prob of act,
+ * or of act_in[B][A] when act_in is given (act must then be NULL; eps and act_in are exclusive).  mean, act and logp
+ * may each be NULL (not written).  Critics: value_r[B] / value_c[B], required when their bit is set.  The arithmetic of
+ * osb_rollout_step in each precision: 0 = fp32 FMA tiles (any O), 1 = tf32 wgmma tiles (O <= 512), 2 = bf16x3 wgmma
+ * tiles (O <= 64); a tensor-core mode outside its bound runs on the fp32 tiles.  Writes nothing else: no RNG, normaliser
+ * or slab state.  Launches of this entry share one accumulator image per device: order them on one stream.
+ * osb_policy_prepare performs the one-time host actions (kernel attributes, the accumulator image sized for any B);
+ * the first osb_policy_step does them too, and a call on a capturing stream that would still need them fails with
+ * OSB_ERR_UNSUPPORTED instead of breaking the capture. */
+int osb_policy_prepare(void);
+int osb_policy_step(const float* theta, int O, int A, long long B, const float* obs, const float* eps,
+                    const float* act_in, int net_mask, int precision, float* mean, float* act, float* logp,
+                    float* value_r, float* value_c, void* stream);
+
 /* ---- learner: fused minibatch forward + loss + backward ------------------------------------
  * replaces PolicyGradient._update minibatch body  algorithms/on_policy/base/policy_gradient.py:L369-381
  *          _update_reward_critic/_update_cost_critic/_update_actor                       :L407-524

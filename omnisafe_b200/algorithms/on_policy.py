@@ -73,6 +73,7 @@ class PolicyGradient(BaseAlgo):
         prec = str(getattr(self._cfgs.train_cfgs, 'matmul_precision', 'bf16x3'))   # upstream YAMLs have no such key: parity-grade tensor-core tiles
         assert prec in ('fp32', 'tf32', 'bf16x3'), "train_cfgs.matmul_precision must be 'fp32', 'tf32' or 'bf16x3'"
         self._engine.precision = {'fp32': 0, 'tf32': 1, 'bf16x3': 2}[prec]
+        self._actor_critic.precision = self._engine.precision   # step / predict / critics use the training arithmetic
         self._stats8 = torch.zeros(8, dtype=torch.float64, device=self._device)
 
     def _init_log(self) -> None:

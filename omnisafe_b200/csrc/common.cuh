@@ -46,7 +46,7 @@ namespace osb {
 
 // Scratch slots of acc_scratch(): one per kernel family, so that families running on different streams never
 // share an accumulator image.
-enum AccSlot { ACC_ROLLOUT = 0, ACC_EVAL_TC, ACC_EVAL_X3, ACC_UPDATE_TC, ACC_FVP_TC, ACC_FVP_X3, ACC_UPDATE_X3, ACC_SELFTEST, ACC_SLOTS };
+enum AccSlot { ACC_ROLLOUT = 0, ACC_EVAL_TC, ACC_EVAL_X3, ACC_UPDATE_TC, ACC_FVP_TC, ACC_FVP_X3, ACC_UPDATE_X3, ACC_SELFTEST, ACC_POLICY, ACC_SLOTS };
 // Device buffer of at least `bytes` for the accumulator images of one launch (csrc/umma.cuh); nullptr (with the
 // error string set) when it cannot be allocated.  Launches of one slot on one device must be ordered on one stream;
 // see api.cu for the lifetime and graph-capture rules.

@@ -14,6 +14,7 @@
 // ObsNormalize reduction is done with order-independent fixed-point atomics and finalised by the
 // last actor CTA of the launch; the next launch (= kernel boundary = grid sync) consumes it.
 #include "common.cuh"
+#include "gaussian.cuh"
 #include "mlp.cuh"
 #include "umma.cuh"
 #include "x3.cuh"
@@ -310,16 +311,6 @@ __device__ __forceinline__ uint32_t act_global_step(const StepArgs& p) {
 // lo + (hi - lo) * (a - (-1)) / (1 - (-1)).  No clipping: the env receives what the wrapper would hand it.
 __device__ __forceinline__ float action_scale(float a, float lo, float hi) {
     return __fadd_rn(lo, __fdiv_rn(__fmul_rn(__fadd_rn(hi, -lo), __fadd_rn(a, 1.f)), 2.f));
-}
-
-// One action component of Normal(mu, sigma): the action rsample gives (loc + eps * scale) and, in `term`, its log_prob
-// term -((x - loc)^2) / (2 var) - log(scale) - log(sqrt(2 pi)).  two_var = 2 sigma^2, log_sd = log sigma.
-__device__ __forceinline__ float sample_action(float mu, float sd, float two_var, float log_sd, float eps, float& term) {
-    const float act = __fadd_rn(mu, __fmul_rn(sd, eps));
-    const float d = __fadd_rn(act, -mu);
-    term = __fdiv_rn(-__fmul_rn(d, d), two_var);
-    term = __fadd_rn(__fadd_rn(term, -log_sd), -0.9189385332046727f);
-    return act;
 }
 
 // the sampled action a of env at step t into the act slab; EXT: also scaled onto the user env's box for env.step

@@ -10,6 +10,13 @@ decay of the actor learning rate.  All parameters live in ONE flat fp32 device v
 kernels share it.  `actor_state_dict()` re-exports the actor under the reference's key names so
 `{'pi': ..., 'obs_normalizer': ...}` checkpoints stay loadable by the reference Evaluator
 (omnisafe/evaluator.py:L153-178, algorithms/on_policy/base/policy_gradient.py:L183-189).
+
+The reference's model API on a trained policy -- `step` / `forward`, `actor.predict / forward / log_prob / std` and
+`reward_critic(obs)` / `cost_critic(obs)` -- runs on one batched launch of the policy-step kernel (csrc/policy.cu,
+osb_policy_step) in the model's `precision` (0 fp32, 1 tf32, 2 bf16x3; the algorithms set it from
+train_cfgs.matmul_precision).  Observations are the normalised ones the networks see, `[O]` or `[..., O]`.  These calls
+read `theta` and nothing else: the rollout's Philox counters, slabs and normalisers and the optimiser state are not
+touched.  A stochastic action draws its noise from torch's global generator exactly as Normal.rsample does.
 """
 from __future__ import annotations
 
@@ -17,8 +24,13 @@ import math
 
 import numpy as np
 import torch
+from torch.distributions import Normal
+from torch.distributions.utils import _standard_normal
+
+from omnisafe_b200._lib import lib, ptr
 
 HID = 64
+NET_ACTOR, NET_REWARD, NET_COST = 1, 2, 4   # net_mask bits of osb_policy_step
 
 
 def param_layout(obs_dim: int, act_dim: int, hid: int = HID) -> dict:
@@ -68,6 +80,10 @@ class ConstraintActorCritic:
         self.epochs = max(int(epochs), 1)
         self._sched_epoch = 0
         self._init_parameters(generator)
+        self.precision = 2   # arithmetic of step / actor / critics: 0 fp32, 1 tf32, 2 bf16x3
+        self.actor = GaussianLearningActor(self)
+        self.reward_critic = VCritic(self, NET_REWARD)
+        self.cost_critic = VCritic(self, NET_COST)
 
     # -- initialisation (utils/model.py:L25-44: kaiming_uniform_(a=sqrt(5)); torch default bias)
     def _init_parameters(self, generator) -> None:
@@ -112,3 +128,129 @@ class ConstraintActorCritic:
 
     def actor_scheduler_step(self) -> None:
         self._sched_epoch += 1
+
+    # -- acting (constraint_actor_critic.py:L84-109) ----------------------------------------------
+    def step(self, obs, deterministic: bool = False) -> tuple[torch.Tensor, ...]:
+        """(action, value_r, value_c, log_prob) of `obs` in one launch: the action is the mean when `deterministic`,
+        otherwise mean + std * eps with eps drawn as Normal.rsample draws it."""
+        obs, lead = self._flat_obs(obs)
+        eps = None if deterministic else self._draw_eps(lead)
+        out = self._launch(obs, NET_ACTOR | NET_REWARD | NET_COST, eps=eps, act=True, logp=True)
+        self.actor._after_inference = False   # predict + log_prob, as the reference's step leaves the actor
+        return (out['act'].view(*lead, self.act_dim), out['value_r'].view(lead), out['value_c'].view(lead),
+                out['logp'].view(lead))
+
+    def forward(self, obs, deterministic: bool = False) -> tuple[torch.Tensor, ...]:
+        return self.step(obs, deterministic=deterministic)
+
+    __call__ = forward
+
+    def _flat_obs(self, obs) -> tuple[torch.Tensor, torch.Size]:
+        obs = torch.as_tensor(obs).to(device=self.device, dtype=torch.float32)
+        assert obs.dim() >= 1 and obs.shape[-1] == self.obs_dim, (
+            f'observations must be [{self.obs_dim}] or [..., {self.obs_dim}], got {tuple(obs.shape)}')
+        return obs.reshape(-1, self.obs_dim).contiguous(), obs.shape[:-1]
+
+    def _draw_eps(self, lead: torch.Size) -> torch.Tensor:
+        # the draw Normal(mean, std).rsample() makes for a [..., A] batch (torch/distributions/normal.py)
+        return _standard_normal((*lead, self.act_dim), dtype=torch.float32, device=self.device).reshape(-1, self.act_dim)
+
+    def _launch(self, obs: torch.Tensor, net_mask: int, eps=None, act_in=None, mean=False, act=False,
+                logp=False) -> dict[str, torch.Tensor]:
+        """One osb_policy_step launch on rows obs[B][O]; returns the requested outputs, flat ([B][A] / [B])."""
+        B, A = obs.shape[0], self.act_dim
+        new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=self.device)   # noqa: E731
+        out = {}
+        if net_mask & NET_ACTOR:
+            if mean:
+                out['mean'] = new(B, A)
+            if act:
+                out['act'] = new(B, A)
+            if logp:
+                out['logp'] = new(B)
+        if net_mask & NET_REWARD:
+            out['value_r'] = new(B)
+        if net_mask & NET_COST:
+            out['value_c'] = new(B)
+        if B == 0:
+            return out
+        with torch.cuda.device(self.device):
+            lib().osb_policy_step(
+                ptr(self.theta), self.obs_dim, A, B, ptr(obs), ptr(eps), ptr(act_in), net_mask, int(self.precision),
+                ptr(out.get('mean')), ptr(out.get('act')), ptr(out.get('logp')), ptr(out.get('value_r')),
+                ptr(out.get('value_c')), torch.cuda.current_stream(self.device).cuda_stream)
+        return out
+
+
+class GaussianLearningActor:
+    """models/actor/gaussian_learning_actor.py:L64-139 on the policy-step kernel: the mean network and the
+    state-independent `log_std` are the actor's slice of the model's `theta`."""
+
+    def __init__(self, model: ConstraintActorCritic) -> None:
+        self._model = model
+        self._after_inference = False
+        self._current_obs: torch.Tensor | None = None
+        self._current_lead: torch.Size | None = None
+
+    def _log_std(self) -> torch.Tensor:
+        m = self._model
+        off, shape = m.layout['actor']['entries']['log_std']
+        return m.theta[off:off + shape[0]]
+
+    def _remember(self, obs: torch.Tensor, lead: torch.Size) -> None:
+        self._current_obs, self._current_lead = obs, lead
+        self._after_inference = True
+
+    def predict(self, obs, deterministic: bool = False) -> torch.Tensor:
+        """The mean if `deterministic`, else a sample of Normal(mean, std) (rsample's noise draw)."""
+        m = self._model
+        obs, lead = m._flat_obs(obs)
+        eps = None if deterministic else m._draw_eps(lead)
+        act = m._launch(obs, NET_ACTOR, eps=eps, act=True)['act']
+        self._remember(obs, lead)
+        return act.view(*lead, m.act_dim)
+
+    def forward(self, obs) -> Normal:
+        """Normal(mean(obs), exp(log_std))."""
+        m = self._model
+        obs, lead = m._flat_obs(obs)
+        mean = m._launch(obs, NET_ACTOR, mean=True)['mean']
+        self._remember(obs, lead)
+        return Normal(mean.view(*lead, m.act_dim), torch.exp(self._log_std()))
+
+    __call__ = forward
+
+    def log_prob(self, act) -> torch.Tensor:
+        """Summed log-probability of `act` under the distribution of the last predict / forward."""
+        assert self._after_inference, 'log_prob() should be called after predict() or forward()'
+        self._after_inference = False
+        m = self._model
+        act = torch.as_tensor(act).to(device=m.device, dtype=torch.float32)
+        assert act.shape == (*self._current_lead, m.act_dim), (
+            f'act must be {(*self._current_lead, m.act_dim)} like the last predict / forward, got {tuple(act.shape)}')
+        act_in = act.reshape(-1, m.act_dim).contiguous()
+        return m._launch(self._current_obs, NET_ACTOR, act_in=act_in, logp=True)['logp'].view(self._current_lead)
+
+    @property
+    def std(self) -> float:
+        return torch.exp(self._log_std()).mean().item()
+
+    @std.setter
+    def std(self, std: float) -> None:
+        self._log_std().fill_(torch.log(torch.tensor(std, device=self._model.device)))
+
+
+class VCritic:
+    """models/critic/v_critic.py:L75-92 (one critic): `critic(obs)` returns the list [value], value = [...]."""
+
+    def __init__(self, model: ConstraintActorCritic, net_bit: int) -> None:
+        self._model = model
+        self._bit = net_bit
+
+    def forward(self, obs) -> list[torch.Tensor]:
+        m = self._model
+        obs, lead = m._flat_obs(obs)
+        out = m._launch(obs, self._bit)
+        return [out['value_r' if self._bit == NET_REWARD else 'value_c'].view(lead)]
+
+    __call__ = forward
