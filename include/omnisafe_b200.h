@@ -291,7 +291,7 @@ int osb_ppo_update_iter_x3(float* theta, float* grad, float* adam_m, float* adam
                            float lr_critic_c, float* gpart, float* stats_part, float* train_stats,
                            const int* stop_flag, void* peer_buf, void* peer_flag, int world, int rank,
                            int* p2p_error, void* stream);
-/* Split-bf16 (parity-grade tensor-core) variant, O <= 64 (csrc/eval_x3.cu). */
+/* Split-bf16 (parity-grade tensor-core) variant, O <= 64 (csrc/eval_tc.cu). */
 int osb_actor_eval_x3(const float* theta_actor, int O, int A, const float* obs, const float* act,
                       const float* logp, const float* adv_r, const float* adv_c, const float* mu_old,
                       const float* logstd_old, const float* moments, const float* lagrange,

@@ -1,5 +1,5 @@
 // Per-sample arithmetic of the learner, shared by the fp32 (update.cu), tf32 (update_tc.cu, eval_tc.cu) and
-// bf16x3 (update_x3.cu, eval_x3.cu) kernels: the loss kinds, the minibatch sample order, the actor loss of the
+// bf16x3 (update_x3.cu, eval_tc.cu) kernels: the loss kinds, the minibatch sample order, the actor loss of the
 // update with its gradients, and the statistics of the full-batch evaluation.  The kernels differ in how they
 // stage a sample's inputs and how they reduce the results; what they compute per sample is defined here once.
 //

@@ -5,9 +5,10 @@
 //           standard-normal eps; eps == null: act = mean, predict(obs, deterministic=True)), logp[B] of act or of a
 //           caller-supplied act_in (GaussianLearningActor.log_prob, gaussian_learning_actor.py:L64-139);
 //   critic: value[B] (VCritic.forward, models/critic/v_critic.py:L75-92).
-// The arithmetic is the rollout's (csrc/rollout.cu) in every precision mode: the same tiles, the same staging of the
-// operands, the same Gaussian helpers (csrc/gaussian.cuh) and the same log-prob summation tree, so a slab row of the
-// rollout fed back through this kernel gives the action, log-prob and values the rollout stored.
+// The arithmetic is the rollout's (csrc/rollout.cu) in every precision mode: the tensor-core modes run the forward of
+// csrc/tc_forward.cuh that the rollout and the evaluation kernels run, the fp32 mode the mlp.cuh tiles, and the actor
+// head uses the same Gaussian helpers (csrc/gaussian.cuh) and log-prob summation tree, so a slab row of the rollout
+// fed back through this kernel gives the action, log-prob and values the rollout stored.
 //   precision 0: fp32 FMA tiles of 32 rows (csrc/mlp.cuh), any O;
 //   precision 1: tf32 wgmma tiles of 128 rows (csrc/umma.cuh), layer 1 K-chunked for 64 < O <= 512;
 //   precision 2: bf16x3 wgmma tiles of 128 rows (csrc/x3.cuh), O <= 64.
@@ -15,8 +16,7 @@
 #include "common.cuh"
 #include "gaussian.cuh"
 #include "mlp.cuh"
-#include "umma.cuh"
-#include "x3.cuh"
+#include "tc_forward.cuh"
 
 namespace osb {
 
@@ -30,7 +30,7 @@ struct PolicyArgs {
     float* logp;           // [B] or null
     float* value_r;        // [B] or null
     float* value_c;        // [B] or null
-    float* acc;            // tensor-core tiles: accumulator images, one [128][P_COLS] per CTA
+    float* acc;            // tensor-core tiles: accumulator images, one [128][TC_COLS] per CTA
     long long B;
     int O, A;
     int nets;              // network of grid row y: (nets >> 2y) & 3
@@ -38,21 +38,17 @@ struct PolicyArgs {
 };
 
 constexpr int PT = 32;            // rows per fp32 tile (the rollout's RT)
-constexpr int PTC = 128;          // rows per tensor-core tile (the rollout's RTC)
-constexpr uint32_t P_COLS = 80;   // accumulator columns: Z [0, 64), OUT [64, 80)
-// operand tiles (bytes after the 1024-byte alignment pad): tf32 X / H2 [128][64], H1 [128][64], W1, W2 [64][64], W3 [16][64];
-// bf16x3: one activation buffer (X, H1, H2 in place) and the weights, three bf16 pieces each
-constexpr uint32_t PX_SUB = PTC * 128, PX_WSUB = 64 * 128, PX_W3SUB = 16 * 128;
-constexpr uint32_t P_FOFF_TF32 = 2 * PTC * 256 + 2 * 16384 + 4096, P_FOFF_X3 = 3 * PX_SUB + 6 * PX_WSUB + 3 * PX_W3SUB;
-// the 4-byte-word region after the operand tiles (offsets in words)
+// the 4-byte-word region after the tensor-core operand tiles (offsets in words)
 constexpr int PW_B1 = 0;                  // [64] layer biases
 constexpr int PW_B2 = PW_B1 + 64;         // [64]
 constexpr int PW_B3 = PW_B2 + 64;         // [16]
 constexpr int PW_SD = PW_B3 + 16;         // [3][16] sigma, 2 sigma^2, log sigma per action
 constexpr int PW_MU = PW_SD + 48;         // [128][16] mean of the tile's rows (actor CTAs)
-constexpr int PW_WORDS = PW_MU + PTC * OUTP;
+constexpr int PW_WORDS = PW_MU + TC_ROWS * OUTP;
 
-static size_t policy_tc_smem_bytes(bool x3) { return 1024 + (x3 ? P_FOFF_X3 : P_FOFF_TF32) + PW_WORDS * sizeof(float); }
+static size_t policy_tc_smem_bytes(bool x3) {
+    return 1024 + (x3 ? TcTiles<true>::FLOATS : TcTiles<false>::FLOATS) + PW_WORDS * sizeof(float);
+}
 static size_t policy_fma_smem_bytes() { return (NETSMEM_FLOATS_FWD + 3 * PT * LD + PT * LDO + 48) * sizeof(float); }
 
 __device__ __forceinline__ int policy_net(const PolicyArgs& p) { return (p.nets >> (2 * blockIdx.y)) & 3; }
@@ -136,18 +132,15 @@ __global__ void __launch_bounds__(NTHREADS) policy_fma_kernel(PolicyArgs p) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// Tensor-core tiles: grid (CTAs per network, networks), each CTA loops over tiles of 128 rows.  The three layer GEMMs,
-// the operand staging and the epilogues are those of rollout_step_tc_kernel (X3 = true: bf16x3, X3 = false: tf32).
+// Tensor-core tiles: grid (CTAs per network, networks), each CTA loops over tiles of 128 rows through the forward of
+// rollout_step_tc_kernel (csrc/tc_forward.cuh; X3 = true: bf16x3, X3 = false: tf32).
 template <bool X3>
 __global__ void __launch_bounds__(NTHREADS, 2) policy_tc_kernel(PolicyArgs p) {
     using namespace umma;
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
-    const uint32_t B0 = smem_u32(smem_raw) + pad;       // X -> H2   (X3: X -> H1 -> H2, bf16x3)
-    const uint32_t B2 = B0 + PTC * 256;                 // H1        (X3: unused)
-    const uint32_t sW1 = X3 ? B0 + 3 * PX_SUB : B2 + PTC * 256;
-    const uint32_t sW2 = sW1 + (X3 ? 3 * PX_WSUB : 16384u), sW3 = sW2 + (X3 ? 3 * PX_WSUB : 16384u);
-    float* fbase = reinterpret_cast<float*>(smem_raw + pad + (X3 ? P_FOFF_X3 : P_FOFF_TF32));
+    const uint32_t B0 = smem_u32(smem_raw) + pad;
+    float* fbase = reinterpret_cast<float*>(smem_raw + pad + TcTiles<X3>::FLOATS);
     float* sB1 = fbase + PW_B1;
     float* sB2 = fbase + PW_B2;
     float* sB3 = fbase + PW_B3;
@@ -163,177 +156,25 @@ __global__ void __launch_bounds__(NTHREADS, 2) policy_tc_kernel(PolicyArgs p) {
     const float* theta = p.theta + net_offset(net, O, p.A);
     const int nchunks = X3 ? 1 : (O + 63) >> 6;
 
-    if constexpr (X3) {   // weights -> bf16x3 tiles
-        for (int i = tid; i < 64 * 32; i += NTHREADS) {
-            const int n = i >> 5, k = (i & 31) << 1;
-            const float a1 = (k < O) ? __ldg(theta + L.off_w1 + n * O + k) : 0.f;
-            const float b1 = (k + 1 < O) ? __ldg(theta + L.off_w1 + n * O + k + 1) : 0.f;
-            const float a2 = __ldg(theta + L.off_w2 + n * 64 + k), b2 = __ldg(theta + L.off_w2 + n * 64 + k + 1);
-            const uint32_t off = x3::off128(n, k);
-            uint32_t w0, w1, w2;
-            x3::split2(a1, b1, w0, w1, w2);
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW1 + off), "r"(w0) : "memory");
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW1 + PX_WSUB + off), "r"(w1) : "memory");
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW1 + 2 * PX_WSUB + off), "r"(w2) : "memory");
-            x3::split2(a2, b2, w0, w1, w2);
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW2 + off), "r"(w0) : "memory");
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW2 + PX_WSUB + off), "r"(w1) : "memory");
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW2 + 2 * PX_WSUB + off), "r"(w2) : "memory");
-        }
-        for (int i = tid; i < 16 * 32; i += NTHREADS) {
-            const int o = i >> 5, k = (i & 31) << 1;
-            const float a = (o < L.out) ? __ldg(theta + L.off_w3 + o * 64 + k) : 0.f;
-            const float b = (o < L.out) ? __ldg(theta + L.off_w3 + o * 64 + k + 1) : 0.f;
-            const uint32_t off = x3::off128(o, k);
-            uint32_t w0, w1, w2;
-            x3::split2(a, b, w0, w1, w2);
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW3 + off), "r"(w0) : "memory");
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW3 + PX_W3SUB + off), "r"(w1) : "memory");
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW3 + 2 * PX_W3SUB + off), "r"(w2) : "memory");
-        }
-    } else {   // tf32 weights; W1 here only when it is one chunk, otherwise with each X chunk below
-        const int k = tid & 63;
-        for (int j = 0; j < 16; ++j) {
-            const int n = (tid >> 6) + 4 * j;
-            if (nchunks == 1) sts(tile_addr(sW1, n, k, 64), tf32r((k < O) ? __ldg(theta + L.off_w1 + n * O + k) : 0.f));
-            sts(tile_addr(sW2, n, k, 64), tf32r(__ldg(theta + L.off_w2 + n * 64 + k)));
-        }
-        for (int j = 0; j < 4; ++j) {
-            const int o = (tid >> 6) + 4 * j;
-            sts(tile_addr(sW3, o, k, 16), tf32r((o < L.out) ? __ldg(theta + L.off_w3 + o * 64 + k) : 0.f));
-        }
-    }
-    if (tid < 64) { sB1[tid] = __ldg(theta + L.off_b1 + tid); sB2[tid] = __ldg(theta + L.off_b2 + tid); }
-    if (tid < 16) sB3[tid] = (tid < L.out) ? __ldg(theta + L.off_b3 + tid) : 0.f;
+    tc_stage_weights<X3>(B0, theta, L, O, sB1, sB2, sB3);
     if (net == 0) stage_sigma(p, sSd);
     if (tid == 0) { mbar_init(&bar, 1); mbar_init_fence(); }
     fence_async_smem();
     __syncthreads();
-    const Acc tm = acc_cta(p.acc, P_COLS);
+    const Acc tm = acc_cta(p.acc, TC_COLS);
     const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    constexpr uint32_t C_Z = 0, C_OUT = 64;
     uint32_t phase = 0;
-    const long long ntiles = (p.B + PTC - 1) / PTC;
+    const long long ntiles = (p.B + TC_ROWS - 1) / TC_ROWS;
 
 #pragma unroll 1
     for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const long long r0 = tile * PTC;
-        if constexpr (X3) {
-            // X tile: thread -> row tid / 2, 32-column half; the previous tile's MMAs have completed, the buffer is free
-            const int xm = tid >> 1, xh = (tid & 1) << 5;
-            const long long row = r0 + xm;
-            const bool in = row < p.B;
-#pragma unroll
-            for (int c8 = 0; c8 < 4; ++c8) {
-                const int c0 = xh + 8 * c8;
-                float v[8];
-                if (p.vec) {
-#pragma unroll
-                    for (int v4 = 0; v4 < 2; ++v4) {
-                        const int c = c0 + 4 * v4;
-                        const float4 x = (in && c < O) ? __ldg(reinterpret_cast<const float4*>(p.obs + row * O + c))
-                                                       : make_float4(0.f, 0.f, 0.f, 0.f);
-                        v[4 * v4] = x.x; v[4 * v4 + 1] = x.y; v[4 * v4 + 2] = x.z; v[4 * v4 + 3] = x.w;
-                    }
-                } else {
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) v[i] = (in && c0 + i < O) ? __ldg(p.obs + row * O + c0 + i) : 0.f;
-                }
-                x3::store8_x3(B0, PX_SUB, xm, c0, v);
-            }
-            fence_async_smem();
-            __syncthreads();
-            const uint64_t dAct = x3::desc128(B0), dW1 = x3::desc128(sW1), dW2 = x3::desc128(sW2), dW3 = x3::desc128(sW3);
-            if (warp < 4) {
-                x3::gemm_x3(tm, C_Z, dAct, PX_SUB, 32u, dW1, PX_WSUB, 32u, x3::idesc_bf16(128, 64, 0, 0), 4, false);
-                mma_commit(&bar);
-            }
-            mbar_wait(&bar, phase); phase ^= 1;
-#pragma unroll
-            for (int c8 = 0; c8 < 4; ++c8) {
-                const int c0 = 32 * h + 8 * c8;
-                float v[8];
-                x3::acc_ld8(tm, lane_base + C_Z + (uint32_t)c0, v);
-#pragma unroll
-                for (int i = 0; i < 8; ++i) v[i] = x3::tanh_acc(v[i] + sB1[c0 + i]);
-                x3::store8_x3(B0, PX_SUB, 32 * q + lane, c0, v);
-            }
-            fence_async_smem();
-            __syncthreads();
-            if (warp < 4) {
-                x3::gemm_x3(tm, C_Z, dAct, PX_SUB, 32u, dW2, PX_WSUB, 32u, x3::idesc_bf16(128, 64, 0, 0), 4, false);
-                mma_commit(&bar);
-            }
-            mbar_wait(&bar, phase); phase ^= 1;
-#pragma unroll
-            for (int c8 = 0; c8 < 4; ++c8) {
-                const int c0 = 32 * h + 8 * c8;
-                float v[8];
-                x3::acc_ld8(tm, lane_base + C_Z + (uint32_t)c0, v);
-#pragma unroll
-                for (int i = 0; i < 8; ++i) v[i] = x3::tanh_acc(v[i] + sB2[c0 + i]);
-                x3::store8_x3(B0, PX_SUB, 32 * q + lane, c0, v);
-            }
-            fence_async_smem();
-            __syncthreads();
-            if (warp < 4) {
-                x3::gemm_x3(tm, C_OUT, dAct, PX_SUB, 32u, dW3, PX_W3SUB, 32u, x3::idesc_bf16(128, 16, 0, 0), 4, false);
-                mma_commit(&bar);
-            }
-            mbar_wait(&bar, phase); phase ^= 1;
-        } else {
-#pragma unroll 1
-            for (int c = 0; c < nchunks; ++c) {   // layer 1 as a K loop over 64-column chunks of X / W1
-                const int k = tid & 63, col = c * 64 + k;
-                if (nchunks > 1) {
-                    float w1c[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) w1c[j] = (col < O) ? __ldg(theta + L.off_w1 + ((tid >> 6) + 4 * j) * O + col) : 0.f;
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) sts(tile_addr(sW1, (tid >> 6) + 4 * j, k, 64), tf32r(w1c[j]));
-                }
-#pragma unroll
-                for (int half = 0; half < 2; ++half) {
-                    float xv[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const long long row = r0 + (tid >> 6) + 4 * (16 * half + j);
-                        xv[j] = (row < p.B && col < O) ? __ldg(p.obs + row * O + col) : 0.f;
-                    }
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) sts(tile_addr(B0, (tid >> 6) + 4 * (16 * half + j), k, PTC), tf32r(xv[j]));
-                }
-                fence_async_smem();
-                __syncthreads();
-                if (warp < 4) { tc_gemm(tm, C_Z, B0, PTC, sW1, 64, 128, 64, 64, c > 0); mma_commit(&bar); }
-                mbar_wait(&bar, phase); phase ^= 1;
-            }
-            {
-                float v[32];
-                acc_ld32(tm, lane_base + C_Z + 32 * h, v);
-#pragma unroll
-                for (int i = 0; i < 32; ++i) v[i] = tanh_fast(v[i] + sB1[32 * h + i]);
-                store_row32(B2, 32 * q + lane, 32 * h, PTC, v);
-            }
-            fence_async_smem();
-            __syncthreads();
-            if (warp < 4) { tc_gemm(tm, C_Z, B2, PTC, sW2, 64, 128, 64, 64, false); mma_commit(&bar); }
-            mbar_wait(&bar, phase); phase ^= 1;
-            {
-                float v[32];
-                acc_ld32(tm, lane_base + C_Z + 32 * h, v);
-#pragma unroll
-                for (int i = 0; i < 32; ++i) v[i] = tanh_fast(v[i] + sB2[32 * h + i]);
-                store_row32(B0, 32 * q + lane, 32 * h, PTC, v);
-            }
-            fence_async_smem();
-            __syncthreads();
-            if (warp < 4) { tc_gemm(tm, C_OUT, B0, PTC, sW3, 16, 128, 16, 64, false); mma_commit(&bar); }
-            mbar_wait(&bar, phase); phase ^= 1;
-        }
+        const long long r0 = tile * TC_ROWS;
+        auto row_of = [&](int m) -> long long { return r0 + m < p.B ? r0 + m : -1; };
+        tc_forward<X3>(B0, tm, &bar, phase, sB1, sB2, nchunks,
+                       [&](int c) { tc_stage_rows<X3>(B0, p.obs, O, p.vec, c, theta, L, row_of); });
         if (h == 0) {
             float o16[16];
-            acc_ld16(tm, lane_base + C_OUT, o16);
+            acc_ld16(tm, lane_base + TC_C_OUT, o16);
             const int e = 32 * q + lane;
             if (net != 0) {
                 if (r0 + e < p.B) (net == 1 ? p.value_r : p.value_c)[r0 + e] = o16[0] + sB3[0];
@@ -344,7 +185,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) policy_tc_kernel(PolicyArgs p) {
         }
         __syncthreads();
         if (net == 0) {
-            policy_head(p, sMu, OUTP, sSd, r0, PTC);
+            policy_head(p, sMu, OUTP, sSd, r0, TC_ROWS);
             __syncthreads();
         }
     }
@@ -355,12 +196,12 @@ static bool use_tf32(int precision, int O) { return precision == 1 && O <= 512; 
 
 // CTAs per network of a tensor-core launch: about two per SM over the whole grid, never more than there are tiles
 static int policy_tc_blocks(long long B, int nnets) {
-    const long long tiles = (B + PTC - 1) / PTC;
+    const long long tiles = (B + TC_ROWS - 1) / TC_ROWS;
     const int cap = (2 * grid_sms() + nnets - 1) / nnets;
     return (int)(tiles < cap ? tiles : cap);
 }
 // accumulator images for the largest tensor-core grid on this device (any B, any net_mask)
-static size_t policy_acc_bytes() { return (size_t)(2 * grid_sms() + 2) * 128 * P_COLS * sizeof(float); }
+static size_t policy_acc_bytes() { return (size_t)(2 * grid_sms() + 2) * 128 * TC_COLS * sizeof(float); }
 
 // One-time host actions: the kernels' shared-memory attributes and the accumulator images.  Never called on a
 // capturing stream (see osb_policy_step).

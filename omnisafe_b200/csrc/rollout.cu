@@ -16,8 +16,7 @@
 #include "common.cuh"
 #include "gaussian.cuh"
 #include "mlp.cuh"
-#include "umma.cuh"
-#include "x3.cuh"
+#include "tc_forward.cuh"
 
 namespace osb {
 
@@ -292,7 +291,7 @@ struct StepArgs {
     unsigned int* bar_ctr;    // persistent epoch kernel: grid-barrier arrival counter and release flag (zero at launch)
     unsigned int* bar_flag;
     long long* dbg;           // optional clock64 stamps (persistent kernel), normally null
-    float* acc;               // tensor-core tiles: accumulator images, one [128][R_COLS] per CTA
+    float* acc;               // tensor-core tiles: accumulator images, one [128][TC_COLS] per CTA
     // external-env act step (EXT instantiations only): the sampled action after ActionScale onto [act_lo, act_hi]
     const float* act_lo;      // [A]
     const float* act_hi;      // [A]
@@ -639,17 +638,12 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
 
 // ---------------------------------------------------------------------------------------------
 // Tensor-core variant of the step kernel (train_cfgs.matmul_precision = tf32, O <= 64): tiles of 128
-// envs, the three layer GEMMs of a network as tf32 wgmma with accumulator images, operands
-// staged as 128B-swizzled K-major smem tiles.  Everything around the GEMMs (ObsNormalize, sampling,
-// env transition, slab append, normaliser sums, ticket) is the arithmetic of rollout_step_kernel.
-constexpr int RTC = 128;
-constexpr uint32_t R_COLS = 80;   // accumulator columns: Z [0, 64), OUT [64, 80)
+// envs, the forward of a network on the tensor-core tiles of csrc/tc_forward.cuh (X3 = false: tf32 (5e-3); X3 = true:
+// split-bf16, fp32-level values / log-probs).  Everything around the forward (ObsNormalize, sampling, env transition,
+// slab append, normaliser sums, ticket) is the arithmetic of rollout_step_kernel.
+constexpr int RTC = TC_ROWS;
 constexpr int SNW = KC + 1;   // row stride of the next-state staging tiles
 
-// X3 = false: tf32 wgmma tiles (5e-3);  X3 = true: split-bf16 tiles (csrc/x3.cuh), fp32-level values / log-probs:
-// one bf16x3 activation buffer (X, H1, H2 overwrite each other in place), accurate tanh, warp-uniform MMA issue.
-constexpr uint32_t RX_SUB = RTC * 128, RX_WSUB = 64 * 128, RX_W3SUB = 16 * 128;
-constexpr uint32_t RTC_FOFF_TF32 = 2 * RTC * 256 + 2 * 16384 + 4096, RTC_FOFF_X3 = 3 * RX_SUB + 6 * RX_WSUB + 3 * RX_W3SUB;
 // the 4-byte-word region after the operand tiles (all offsets in words)
 constexpr int TF_B1 = 0;                          // [64] layer biases
 constexpr int TF_B2 = TF_B1 + 64;                 // [64]
@@ -682,11 +676,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
     using namespace umma;
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
-    const uint32_t B0 = smem_u32(smem_raw) + pad;       // X -> H2   (X3: X -> H1 -> H2, bf16x3)
-    const uint32_t B2 = B0 + RTC * 256;                 // H1        (X3: unused)
-    const uint32_t sW1 = X3 ? B0 + 3 * RX_SUB : B2 + RTC * 256;
-    const uint32_t sW2 = sW1 + (X3 ? 3 * RX_WSUB : 16384u), sW3 = sW2 + (X3 ? 3 * RX_WSUB : 16384u);
-    float* fbase = reinterpret_cast<float*>(smem_raw + pad + (X3 ? RTC_FOFF_X3 : RTC_FOFF_TF32));
+    const uint32_t B0 = smem_u32(smem_raw) + pad;       // the X tile comes first (TcTiles::X == 0)
+    float* fbase = reinterpret_cast<float*>(smem_raw + pad + TcTiles<X3>::FLOATS);
     float* sB1 = fbase + TF_B1;
     float* sB2 = fbase + TF_B2;
     float* sB3 = fbase + TF_B3;
@@ -717,80 +708,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
     const int my_env = env0 + e_env;
     const bool my_ok = (net == 0) && my_env < N;
 
-    if constexpr (X3) {   // weights -> bf16x3 tiles (all loads first)
-        float a1[8], b1[8], a2[8], b2[8], a3[2], b3[2];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int i = tid + j * NTHREADS, n = i >> 5, k = (i & 31) << 1;
-            a1[j] = (k < On) ? __ldg(theta + L.off_w1 + n * On + k) : 0.f;
-            b1[j] = (k + 1 < On) ? __ldg(theta + L.off_w1 + n * On + k + 1) : 0.f;
-            a2[j] = __ldg(theta + L.off_w2 + n * 64 + k); b2[j] = __ldg(theta + L.off_w2 + n * 64 + k + 1);
-        }
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-            const int i = tid + j * NTHREADS, o = i >> 5, k = (i & 31) << 1;
-            a3[j] = (o < L.out) ? __ldg(theta + L.off_w3 + o * 64 + k) : 0.f;
-            b3[j] = (o < L.out) ? __ldg(theta + L.off_w3 + o * 64 + k + 1) : 0.f;
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int i = tid + j * NTHREADS, n = i >> 5, k = (i & 31) << 1;
-            uint32_t w0, w1, w2;
-            const uint32_t off = x3::off128(n, k);
-            x3::split2(a1[j], b1[j], w0, w1, w2);
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW1 + off), "r"(w0) : "memory");
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW1 + RX_WSUB + off), "r"(w1) : "memory");
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW1 + 2 * RX_WSUB + off), "r"(w2) : "memory");
-            x3::split2(a2[j], b2[j], w0, w1, w2);
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW2 + off), "r"(w0) : "memory");
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW2 + RX_WSUB + off), "r"(w1) : "memory");
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW2 + 2 * RX_WSUB + off), "r"(w2) : "memory");
-        }
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-            const int i = tid + j * NTHREADS, o = i >> 5, k = (i & 31) << 1;
-            uint32_t w0, w1, w2;
-            const uint32_t off = x3::off128(o, k);
-            x3::split2(a3[j], b3[j], w0, w1, w2);
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW3 + off), "r"(w0) : "memory");
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW3 + RX_W3SUB + off), "r"(w1) : "memory");
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sW3 + 2 * RX_W3SUB + off), "r"(w2) : "memory");
-        }
-    } else
-    {   // weights (batched loads)
-        float w1v[16], w2v[16], w3v[4];
-        const int k = tid & 63;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-            const int n = (tid >> 6) + 4 * j;
-            w1v[j] = (k < On) ? __ldg(theta + L.off_w1 + n * On + k) : 0.f;
-            w2v[j] = __ldg(theta + L.off_w2 + n * 64 + k);
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int o = (tid >> 6) + 4 * j;
-            w3v[j] = (o < L.out) ? __ldg(theta + L.off_w3 + o * 64 + k) : 0.f;
-        }
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-            const int n = (tid >> 6) + 4 * j;
-            sts(tile_addr(sW1, n, k, 64), tf32r(w1v[j]));
-            sts(tile_addr(sW2, n, k, 64), tf32r(w2v[j]));
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) sts(tile_addr(sW3, (tid >> 6) + 4 * j, k, 16), tf32r(w3v[j]));
-    }
-    if (tid < 64) { sB1[tid] = __ldg(theta + L.off_b1 + tid); sB2[tid] = __ldg(theta + L.off_b2 + tid); }
-    if (tid < 16) sB3[tid] = (tid < L.out) ? __ldg(theta + L.off_b3 + tid) : 0.f;
+    tc_stage_weights<X3>(B0, theta, L, On, sB1, sB2, sB3);
     if (net == 0 && tid < 16) {          // Normal(mu, sigma): sigma = exp(log_std) is state independent
         const float sd = (tid < A) ? expf(__ldg(theta + L.off_logstd + tid)) : 1.f;
         sSd[tid] = sd; sSd[16 + tid] = __fmul_rn(2.f, __fmul_rn(sd, sd)); sSd[32 + tid] = logf(sd);
     }
     if (tid == 0) { mbar_init(&bar, 1); mbar_init_fence(); s_anyfin = 0; }
     __syncthreads();
-    const Acc tm = acc_cta(p.acc, R_COLS);
+    const Acc tm = acc_cta(p.acc, TC_COLS);
     const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    constexpr uint32_t C_Z = 0, C_OUT = 64;
     uint32_t phase = 0;
 
     // development aid (tools/rollout_stage_times.py): clock64 stamps of thread 0 of the first actor and reward-critic CTA
@@ -873,8 +799,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                     x3::split2(v.z, v.w, w0[1], w1[1], w2[1]);
                     const uint32_t o = B0 + x3::off128(e, k4);
                     asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(o), "r"(w0[0]), "r"(w0[1]) : "memory");
-                    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(o + RX_SUB), "r"(w1[0]), "r"(w1[1]) : "memory");
-                    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(o + 2 * RX_SUB), "r"(w2[0]), "r"(w2[1]) : "memory");
+                    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(o + TcTiles<true>::SUB), "r"(w1[0]), "r"(w1[1]) : "memory");
+                    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(o + 2 * TcTiles<true>::SUB), "r"(w2[0]), "r"(w2[1]) : "memory");
                 } else {
                 asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(tile_addr(B0, e, k4, RTC)),
                              "f"(tf32r(v.x)), "f"(tf32r(v.y)), "f"(tf32r(v.z)), "f"(tf32r(v.w))
@@ -895,7 +821,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                     if (norm_on) v = norm_clip(v, mk, sk);
                     if (obs_out) obs_out[(size_t)env * On + k] = v;
                 }
-                if constexpr (X3) x3::store1_x3(B0, RX_SUB, x3::off128(e, k), v);
+                if constexpr (X3) x3::store1_x3(B0, TcTiles<true>::SUB, x3::off128(e, k), v);
                 else sts(tile_addr(B0, e, k, RTC), tf32r(v));
             }
         }
@@ -908,85 +834,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                     z = pass ? __ldcg(p.sa.safety + (size_t)(t & 1) * N + env) : 1.f;
                     if (obs_out) obs_out[(size_t)env * On + O] = z;
                 }
-                if constexpr (X3) x3::store1_x3(B0, RX_SUB, x3::off128(tid, O), z);
+                if constexpr (X3) x3::store1_x3(B0, TcTiles<true>::SUB, x3::off128(tid, O), z);
                 else sts(tile_addr(B0, tid, O, RTC), tf32r(z));
             }
         }
         fence_async_smem();
         __syncthreads();
         RSTAMP(2);
-        if constexpr (X3) {
-            // three layers on bf16x3 tiles, one activation buffer: every epilogue starts after its layer's MMAs completed
-            const uint64_t dAct = x3::desc128(B0), dW1 = x3::desc128(sW1), dW2 = x3::desc128(sW2), dW3 = x3::desc128(sW3);
-            if (warp < 4) {
-                x3::gemm_x3(tm, C_Z, dAct, RX_SUB, 32u, dW1, RX_WSUB, 32u, x3::idesc_bf16(128, 64, 0, 0), 4, false);
-                mma_commit(&bar);
-            }
-            mbar_wait(&bar, phase); phase ^= 1;
-            RSTAMP(3);
-#pragma unroll
-            for (int c8 = 0; c8 < 4; ++c8) {
-                const int c0 = 32 * h + 8 * c8;
-                float v[8];
-                x3::acc_ld8(tm, lane_base + C_Z + (uint32_t)c0, v);
-#pragma unroll
-                for (int i = 0; i < 8; ++i) v[i] = x3::tanh_acc(v[i] + sB1[c0 + i]);
-                x3::store8_x3(B0, RX_SUB, 32 * q + lane, c0, v);
-            }
-            fence_async_smem();
-            __syncthreads();
-            if (warp < 4) {
-                x3::gemm_x3(tm, C_Z, dAct, RX_SUB, 32u, dW2, RX_WSUB, 32u, x3::idesc_bf16(128, 64, 0, 0), 4, false);
-                mma_commit(&bar);
-            }
-            mbar_wait(&bar, phase); phase ^= 1;
-            RSTAMP(4);
-#pragma unroll
-            for (int c8 = 0; c8 < 4; ++c8) {
-                const int c0 = 32 * h + 8 * c8;
-                float v[8];
-                x3::acc_ld8(tm, lane_base + C_Z + (uint32_t)c0, v);
-#pragma unroll
-                for (int i = 0; i < 8; ++i) v[i] = x3::tanh_acc(v[i] + sB2[c0 + i]);
-                x3::store8_x3(B0, RX_SUB, 32 * q + lane, c0, v);
-            }
-            fence_async_smem();
-            __syncthreads();
-            if (warp < 4) {
-                x3::gemm_x3(tm, C_OUT, dAct, RX_SUB, 32u, dW3, RX_W3SUB, 32u, x3::idesc_bf16(128, 16, 0, 0), 4, false);
-                mma_commit(&bar);
-            }
-            mbar_wait(&bar, phase); phase ^= 1;
-            RSTAMP(5);
-        } else {
-        if (warp < 4) { tc_gemm(tm, C_Z, B0, RTC, sW1, 64, 128, 64, 64, false); mma_commit(&bar); }
-        mbar_wait(&bar, phase); phase ^= 1;
-        {
-            float v[32];
-            acc_ld32(tm, lane_base + C_Z + 32 * h, v);
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = tanh_fast(v[i] + sB1[32 * h + i]);
-            store_row32(B2, 32 * q + lane, 32 * h, RTC, v);
-        }
-        fence_async_smem();
-        __syncthreads();
-        if (warp < 4) { tc_gemm(tm, C_Z, B2, RTC, sW2, 64, 128, 64, 64, false); mma_commit(&bar); }
-        mbar_wait(&bar, phase); phase ^= 1;
-        {
-            float v[32];
-            acc_ld32(tm, lane_base + C_Z + 32 * h, v);
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = tanh_fast(v[i] + sB2[32 * h + i]);
-            store_row32(B0, 32 * q + lane, 32 * h, RTC, v);
-        }
-        fence_async_smem();
-        __syncthreads();
-        if (warp < 4) { tc_gemm(tm, C_OUT, B0, RTC, sW3, 16, 128, 16, 64, false); mma_commit(&bar); }
-        mbar_wait(&bar, phase); phase ^= 1;
-        }
+        tc_forward<X3>(B0, tm, &bar, phase, sB1, sB2, 1, TcNop{}, [&](int l) {   // bf16x3: stamps 3-5, one per layer
+            if (X3) RSTAMP(2 + l);
+        });
         if (h == 0) {
             float o16[16];
-            acc_ld16(tm, lane_base + C_OUT, o16);
+            acc_ld16(tm, lane_base + TC_C_OUT, o16);
             const int e = 32 * q + lane;
             const int env = env0 + e;
             if (net != 0) {
@@ -1175,7 +1035,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
 
 // 1024: the alignment pad in front of the operand tiles
 static size_t rollout_tc_smem_bytes(bool x3) {
-    return 1024 + (x3 ? RTC_FOFF_X3 : RTC_FOFF_TF32) + TF_WORDS * sizeof(float) + 64;
+    return 1024 + (x3 ? TcTiles<true>::FLOATS : TcTiles<false>::FLOATS) + TF_WORDS * sizeof(float) + 64;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1497,7 +1357,7 @@ static int ext_refuse_if_capturing(cudaStream_t stream, const char* what) {
     return OSB_ERR_UNSUPPORTED;
 }
 
-static size_t rollout_tc_acc_bytes(int N) { return (size_t)((N + RTC - 1) / RTC) * 3 * 128 * R_COLS * sizeof(float); }
+static size_t rollout_tc_acc_bytes(int N) { return (size_t)((N + RTC - 1) / RTC) * 3 * 128 * TC_COLS * sizeof(float); }
 
 // EXT = true: the act step of the external-env path (never the persistent kernel).  prepare_only: perform the host
 // actions (attributes, accumulator image) and launch nothing (osb_ext_prepare).

@@ -156,7 +156,7 @@ def _external_epoch(dev, N, T, O, A, precision, eps):
     return agent, buf
 
 
-@pytest.mark.parametrize('precision', [0, 2])
+@pytest.mark.parametrize('precision', [0, 1, 2])
 @pytest.mark.parametrize('env', ['synthetic', 'widebox'])
 def test_agrees_with_rollout(cuda, precision, env):
     N, T = 300, 8
@@ -172,6 +172,26 @@ def test_agrees_with_rollout(cuda, precision, env):
             _close(out[k], d[slab][t], 2e-5, f'{env} precision {precision} t {t} {k}')
             bitwise &= torch.equal(out[k], d[slab][t])
     print(f'{env} precision {precision}: policy step vs rollout slabs bit for bit: {bitwise}')
+    if precision != 0:      # the tensor-core modes run one forward (csrc/tc_forward.cuh) in both kernels
+        assert bitwise
+
+
+@pytest.mark.parametrize('precision,O', [(1, 60), (1, 111), (1, 376), (2, 17), (2, 60), (2, 64)])
+def test_eval_snapshot_is_the_policy_mean(cuda, precision, O):
+    """The evaluation kernel's old-policy snapshot (mu_store) and the policy step's mean are one function, bit for bit."""
+    from omnisafe_b200._lib import lib, ptr
+
+    A, B = 6, 1000
+    m = _model(cuda, O, A, precision)
+    obs = torch.randn(B, O, device=cuda).clamp_(-5, 5)
+    mean = m._launch(obs, 1, mean=True)['mean']
+    mu = torch.full((B, A), float('nan'), device=cuda)
+    fn = lib().osb_actor_eval_x3 if precision == 2 else lib().osb_actor_eval_tc
+    rc = fn(ptr(m.theta), O, A, ptr(obs), 0, 0, 0, 0, 0, 0, 0, 0, B, 1, ptr(mu), 0, 0,
+            torch.cuda.current_stream().cuda_stream)
+    assert rc == 0
+    torch.cuda.synchronize()
+    assert torch.equal(mu, mean)
 
 
 @pytest.mark.parametrize('precision', [0, 1, 2])
