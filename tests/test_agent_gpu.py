@@ -7,6 +7,8 @@ import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
+# the class goldens run on the exact fp32 tiles and on the split-bf16 tiles (the SyntheticBox-v0 default), same bars
+PRECISIONS = ['fp32', 'bf16x3']
 
 
 def _custom(tmp, N=64, T=32, epochs=3, **algo):
@@ -59,21 +61,23 @@ def test_ppolag_learning_signal(cuda, tmp_path):
 
 
 @pytest.mark.parametrize('name,fname', [('CPO', 'update_cpo.npz'), ('PCPO', 'update_pcpo.npz')])
-def test_cpo_update_golden(cuda, tmp_path, golden_dir, name, fname):
+@pytest.mark.parametrize('prec', PRECISIONS)
+def test_cpo_update_golden(cuda, tmp_path, golden_dir, name, fname, prec):
     """CPO._update / PCPO._update of the unmodified reference vs ours on identical data: same case
-    analysis, same step, same parameters afterwards."""
+    analysis, same step, same parameters afterwards, on the fp32 and the split-bf16 tiles."""
     import omnisafe_b200
 
     g = np.load(os.path.join(golden_dir, fname))
     N, T, O, A = int(g['N']), int(g['T']), int(g['O']), int(g['A'])
     cfg = {
         'seed': int(g['seed']) if 'seed' in g.files else 7,
-        'train_cfgs': {'device': 'cuda', 'vector_env_nums': N, 'total_steps': N * T * 2},
+        'train_cfgs': {'device': 'cuda', 'vector_env_nums': N, 'total_steps': N * T * 2, 'matmul_precision': prec},
         'algo_cfgs': {'steps_per_epoch': N * T, 'batch_size': 32, 'update_iters': 2, 'cost_limit': float(g['cost_limit'])},
         'logger_cfgs': {'log_dir': str(tmp_path), 'window_lens': 10, 'use_tensorboard': False},
         'env_cfgs': {'obs_dim': O, 'act_dim': A, 'max_episode_steps': 8, 'term_prob': 0.05},
     }
     algo = omnisafe_b200.Agent(name, 'SyntheticBox-v0', custom_cfgs=cfg).agent
+    assert algo._engine.precision == {'fp32': 0, 'bf16x3': 2}[prec]
     algo._actor_critic.load_flat(g['theta0'])
     data = {k[5:]: g[k] for k in g.files if k.startswith('data_')}
 
@@ -130,7 +134,8 @@ def test_pid_lagrange_kernel_golden(cuda, golden_dir):
 
 
 @pytest.mark.parametrize('fname', ['update_trpolag.npz', 'update_oncrpo.npz', 'update_rcpo.npz'])
-def test_trpo_family_update_golden(cuda, tmp_path, golden_dir, fname):
+@pytest.mark.parametrize('prec', PRECISIONS)
+def test_trpo_family_update_golden(cuda, tmp_path, golden_dir, fname, prec):
     """TRPOLag._update / OnCRPO._update (cost-surrogate branch) / RCPO._update (plain natural step) of the
     unmodified reference vs ours on identical data: same natural direction, same accepted line-search step,
     same parameters afterwards."""
@@ -142,7 +147,7 @@ def test_trpo_family_update_golden(cuda, tmp_path, golden_dir, fname):
     extra = {k[6:]: float(g[k]) for k in g.files if k.startswith('extra_')}
     cfg = {
         'seed': int(g['seed']),
-        'train_cfgs': {'device': 'cuda', 'vector_env_nums': N, 'total_steps': N * T * 2},
+        'train_cfgs': {'device': 'cuda', 'vector_env_nums': N, 'total_steps': N * T * 2, 'matmul_precision': prec},
         'algo_cfgs': {'steps_per_epoch': N * T, 'batch_size': 32, 'update_iters': 2, **extra},
         'logger_cfgs': {'log_dir': str(tmp_path), 'window_lens': 10, 'use_tensorboard': False},
         'env_cfgs': {'obs_dim': O, 'act_dim': A, 'max_episode_steps': 8, 'term_prob': 0.05},
@@ -151,6 +156,7 @@ def test_trpo_family_update_golden(cuda, tmp_path, golden_dir, fname):
     if lag:
         cfg['lagrange_cfgs'] = lag
     algo = omnisafe_b200.Agent(name, 'SyntheticBox-v0', custom_cfgs=cfg).agent
+    assert algo._engine.precision == {'fp32': 0, 'bf16x3': 2}[prec]
     algo._actor_critic.load_flat(g['theta0'])
     data = {k[5:]: g[k] for k in g.files if k.startswith('data_')}
 
@@ -180,7 +186,8 @@ def test_trpo_family_update_golden(cuda, tmp_path, golden_dir, fname):
 
 
 @pytest.mark.parametrize('fname', ['update_ipo.npz', 'update_cppopid.npz', 'update_pdo.npz'])
-def test_first_order_family_update_golden(cuda, tmp_path, golden_dir, fname):
+@pytest.mark.parametrize('prec', PRECISIONS)
+def test_first_order_family_update_golden(cuda, tmp_path, golden_dir, fname, prec):
     """IPO._update / CPPOPID._update / PDO._update of the unmodified reference vs ours on identical data:
     the class derives the same penalty / multiplier from Jc and the fused update lands on the same parameters."""
     import omnisafe_b200
@@ -190,7 +197,7 @@ def test_first_order_family_update_golden(cuda, tmp_path, golden_dir, fname):
     N, T, O, A = int(g['N']), int(g['T']), int(g['O']), int(g['A'])
     cfg = {
         'seed': int(g['seed']),
-        'train_cfgs': {'device': 'cuda', 'vector_env_nums': N, 'total_steps': N * T * 2},
+        'train_cfgs': {'device': 'cuda', 'vector_env_nums': N, 'total_steps': N * T * 2, 'matmul_precision': prec},
         'algo_cfgs': {'steps_per_epoch': N * T, 'batch_size': 32, 'update_iters': 2,
                       **{k[6:]: float(g[k]) for k in g.files if k.startswith('extra_')}},
         'logger_cfgs': {'log_dir': str(tmp_path), 'window_lens': 10, 'use_tensorboard': False},
@@ -200,6 +207,7 @@ def test_first_order_family_update_golden(cuda, tmp_path, golden_dir, fname):
     if lag:
         cfg['lagrange_cfgs'] = lag
     algo = omnisafe_b200.Agent(name, 'SyntheticBox-v0', custom_cfgs=cfg).agent
+    assert algo._engine.precision == {'fp32': 0, 'bf16x3': 2}[prec]
     algo._actor_critic.load_flat(g['theta0'])
     data = {k[5:]: g[k] for k in g.files if k.startswith('data_')}
 

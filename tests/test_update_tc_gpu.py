@@ -126,8 +126,9 @@ def test_tc_actor_eval_matches_fp32_eval(cuda, O):
 @pytest.mark.parametrize('O,A,N,T,stride', [(60, 8, 64, 40, 1), (17, 6, 9, 31, 1), (64, 16, 100, 50, 3), (60, 8, 512, 80, 1),
                                              (111, 8, 40, 30, 1), (376, 8, 64, 40, 2)])
 def test_tc_fvp_vs_fp32_fvp(cuda, O, A, N, T, stride):
-    """Tensor-core Fisher-vector product (tangent kernel + TC backward) vs the exact-fp32 FVP kernel
-    (itself checked against double-backward autograd in test_update_gpu).  Tolerance 5e-3 l2-relative."""
+    """Tensor-core Fisher-vector product (tangent kernel + TC backward) vs the exact-fp32 FVP kernel.  Both are
+    checked against the float64 double-backward FVP at these and more shapes in
+    test_natural_gradient_gpu::test_fvp_vs_fp64.  Tolerance 5e-3 l2-relative."""
     from omnisafe_b200._lib import current_stream, lib, ptr
 
     rng = np.random.default_rng(O * 7 + N)
