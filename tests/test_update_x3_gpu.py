@@ -140,7 +140,8 @@ def test_x3_epoch_matches_fp32_epoch(cuda):
 @pytest.mark.parametrize('N,T,batch,iters', [(64, 32, 512, 3), (50, 26, 512, 2), (13, 100, 640, 2), (256, 80, 16384, 1)])
 def test_x3_fused_iteration_equals_stepwise(cuda, N, T, batch, iters):
     """The persistent kernel (optimiser inside, software grid barriers, short last minibatch, CTAs without a tile)
-    and the launch-per-minibatch path (bf16x3 gradient kernel + optim_fused) produce the same parameters."""
+    and the launch-per-minibatch path (bf16x3 gradient kernel + optim_fused) produce the same parameters.  Both
+    paths share the clip formula, so this does not check the clip itself: test_optimizer_gpu does, against float64."""
     rng = np.random.default_rng(N + T)
     O, A = 60, 8
     theta = oac.init_theta(O, A, seed=2)
