@@ -111,27 +111,115 @@ def step64(state, grads, *, max_grad_norm, lrs, critic_norm_coef, O, net_mask: i
     return state, rec
 
 
+def actor_loss64(d, old, act, logp, adv, adv_r, adv_c, *, loss_kind, clip=0.2, entropy_coef=0.0, focops_lam=1.0,
+                 focops_eta=0.0):
+    """Actor loss of one minibatch for every loss kind of the update kernels, in float64.  d: the policy being
+    trained on the minibatch rows; old: the old policy on the same rows (FOCOPS only); adv: the Lagrangian mix;
+    adv_r / adv_c: the standardised advantages.  The kernels' parameter names: FOCOPS temperature focops_lam and
+    trust region focops_eta; P3O kappa = focops_lam and Jc - cost_limit = focops_eta.
+      0 PPO clip on adv (+ entropy bonus)                                    base/ppo.py:L35-87
+      1 -mean(ratio adv), 3 mean(ratio adv_c)                                policy_gradient.py:L551-588, cpo.py:L182-212
+      2 FOCOPS: mean_i(m_i kl_i) - mean_i(m_i) mean_j(ratio_j adv_j) / lam (+ entropy bonus), kl_i = KL(new || old)
+        summed over the action dims, m_i = 1{kl_i <= eta} on detached values.  This is the mean of the reference's
+        [b, b] broadcast (first_order/focops.py:L85-89, Learner.loss_pi_focops) without forming it.
+      5 P3O: PPO clip on adv_r (+ entropy bonus) + kappa relu(mean(ratio adv_c) + Jc - limit)   p3o.py:L48-91
+    Returns (loss to differentiate, info): info['stats'] = [slot 0, slot 1, slot 2, slot 4] of the kernels' logged
+    actor statistics (slot 0: the loss without the entropy bonus and without the P3O penalty; slot 1: mean ratio;
+    slot 2: FOCOPS mean KL, P3O penalty term; slot 4: FOCOPS mask mean); info['pass1']: what the forward-only pass
+    reduces (FOCOPS mask mean, P3O mean(ratio adv_c)); info['gate']: P3O kappa or 0; info['margin']: distance of
+    the pass-1 decisions from their boundary (FOCOPS min_i |kl_i - eta|, P3O |mean + Jc - limit|); info['entropy']: the
+    mean entropy over rows and action dims (what the bonus multiplies)."""
+    ratio = torch.exp(d.log_prob(act).sum(-1) - logp)
+    slot2 = slot4 = 0.0
+    info = {'pass1': None, 'gate': None, 'margin': None}
+    if loss_kind in (0, 5):
+        a = adv_r if loss_kind == 5 else adv
+        loss = -torch.min(ratio * a, torch.clamp(ratio, 1 - clip, 1 + clip) * a).mean()
+    elif loss_kind == 1:
+        loss = -(ratio * adv).mean()
+    elif loss_kind == 3:
+        loss = (ratio * adv_c).mean()
+    else:
+        assert loss_kind == 2
+        kl = kl_divergence(d, old).sum(-1)
+        m = (kl.detach() <= focops_eta).to(F64)
+        loss = (m * kl).mean() - m.mean() * (ratio * adv).mean() / focops_lam
+        slot2, slot4 = float(kl.detach().mean()), float(m.mean())
+        info['pass1'] = slot4
+        info['margin'] = float((kl.detach() - focops_eta).abs().min())
+    slot0 = float(loss.detach())
+    if loss_kind == 5:
+        z = (ratio * adv_c).mean() + focops_eta
+        penalty = focops_lam * torch.relu(z)
+        loss = loss + penalty
+        slot2 = float(penalty.detach())
+        info['pass1'] = float(z.detach()) - focops_eta
+        info['gate'] = focops_lam if float(z.detach()) > 0 else 0.0
+        info['margin'] = abs(float(z.detach()))
+    if loss_kind in (0, 2, 5) and entropy_coef:
+        loss = loss - entropy_coef * d.entropy().mean()
+    info['stats'] = [slot0, float(ratio.detach().mean()), slot2, slot4]
+    info['entropy'] = float(d.entropy().detach().mean())
+    return loss, info
+
+
+def minibatch64(theta, data, moments, idx, lam, *, loss_kind, old_mu=None, old_logstd=None, critic_norm_coef=0.0,
+                net_mask=7, **loss_kw):
+    """The data gradient of every network on the minibatch rows `idx` (env-major) at `theta`, as one launch of a
+    minibatch gradient kernel + osb_grad_reduce leaves it: critics mse + critic_norm_coef sum theta^2, the actor
+    loss of actor_loss64 with the old policy Normal(old_mu[idx], exp(old_logstd)).  Returns (flat gradient, actor
+    info of actor_loss64)."""
+    theta = np.asarray(theta, np.float32).astype(np.float64)
+    O = np.asarray(data['obs']).shape[1]
+    lay = _dims(theta.size, O)
+    idx = torch.as_tensor(np.asarray(idx, np.int64))
+    o = f64._t64(data['obs'])[idx]
+    adv_r, adv_c, adv = (x[idx] for x in f64._std_adv(data, moments, lam))
+    grad, info = np.zeros_like(theta), None
+    for k, net in enumerate(NETS):
+        if not (net_mask >> k) & 1:
+            continue
+        p = _leaves(theta, lay, net, grad=True)
+        if net == 'actor':
+            old = None
+            if old_mu is not None:
+                old = Normal(f64._t64(old_mu)[idx], torch.exp(f64._t64(old_logstd)).expand(len(idx), -1))
+            loss, info = actor_loss64(ac.actor_dist(p, o), old, f64._t64(data['act'])[idx], f64._t64(data['logp'])[idx],
+                                      adv, adv_r, adv_c, loss_kind=loss_kind, **loss_kw)
+        else:
+            tgt = f64._t64(data['target_value_r' if net == 'reward_critic' else 'target_value_c'])[idx]
+            loss = torch.nn.functional.mse_loss(ac.critic_value(p, o), tgt)
+            for t in p.values():
+                loss = loss + t.pow(2).sum() * critic_norm_coef
+        loss.backward()
+        s = lay[net]['start']
+        grad[s:s + lay[net]['size']] = _flat([t.grad for t in p.values()])
+    return grad, info
+
+
 def ppo_epoch64(theta, data, moments, perms, lam, *, net_mask, loss_kind, batch_size, update_iters, clip=0.2,
-                entropy_coef=0.0, critic_norm_coef=0.001, max_grad_norm=40.0, lrs=(3e-4, 3e-4, 3e-4),
-                target_kl=0.02, kl_early_stop=False, state=None):
-    """PolicyGradient._update (policy_gradient.py:L345-405) in float64 for the loss kinds of the fused kernels:
-    0 PPO clip (+ entropy bonus), 1 plain ratio surrogate, 3 cost surrogate (CPO / PCPO cost pass).  `data` is
-    env-major with RAW advantages; `perms[i]` is the env-major sample order of pass i.  The minibatch gradients of
-    all networks are taken at the same theta (the networks do not share parameters, so the order of the three
-    steps does not matter).  A pass that trains the actor ends with the full-batch KL against the policy the epoch
-    started from and the early stop; without the actor every pass runs.
+                entropy_coef=0.0, focops_lam=1.0, focops_eta=0.0, critic_norm_coef=0.001, max_grad_norm=40.0,
+                lrs=(3e-4, 3e-4, 3e-4), target_kl=0.02, kl_early_stop=False, state=None):
+    """PolicyGradient._update (policy_gradient.py:L345-405) / FOCOPS._update in float64 for every loss kind of the
+    update kernels (actor_loss64): 0 PPO clip (+ entropy bonus), 1 plain ratio surrogate, 2 FOCOPS, 3 cost surrogate
+    (CPO / PCPO cost pass), 5 P3O (no Lagrangian mix: P3O trains on adv_r).  `data` is env-major with RAW
+    advantages; `perms[i]` is the env-major sample order of pass i.  The minibatch gradients of all networks are
+    taken at the same theta (the networks do not share parameters, so the order of the three steps does not
+    matter).  FOCOPS's old policy is the one the epoch started from.  A pass that trains the actor ends with the
+    full-batch KL against that policy and the early stop; without the actor every pass runs.
 
     Returns (state, record, passes): record is one dict per minibatch step with norm [3], coef [3], grad (clipped,
-    flat), loss [3] (logged values: critic mse + coef * sum theta^2; actor surrogate without the entropy bonus),
-    ratio (mean ratio of the actor), plus 'kl' [passes]."""
-    assert loss_kind in (0, 1, 3)
+    flat), loss [3] (logged values: critic mse + coef * sum theta^2; actor: slot 0 of actor_loss64), ratio (mean
+    ratio of the actor), and for the actor 'stats' / 'pass1' / 'gate' / 'margin' / 'entropy' of actor_loss64; plus 'kl'
+    [passes]."""
+    assert loss_kind in (0, 1, 2, 3, 5)
     state = init_state(theta) if state is None else _copy(state)
     P = state['theta'].size
     O = np.asarray(data['obs']).shape[1]
     lay = _dims(P, O)
     obs, act, logp = f64._t64(data['obs']), f64._t64(data['act']), f64._t64(data['logp'])
     tgt = {'reward_critic': f64._t64(data['target_value_r']), 'cost_critic': f64._t64(data['target_value_c'])}
-    _, adv_c, adv = f64._std_adv(data, moments, lam)
+    adv_r, adv_c, adv = f64._std_adv(data, moments, lam)
     train_actor = bool(net_mask & 1)
     if train_actor:
         with torch.no_grad():
@@ -151,18 +239,11 @@ def ppo_epoch64(theta, data, moments, perms, lam, *, net_mask, loss_kind, batch_
                     surr = {}
 
                     def loss_fn(p, surr=surr):
-                        d = ac.actor_dist(p, o)
-                        ratio = torch.exp(d.log_prob(act[idx]).sum(-1) - logp[idx])
-                        if loss_kind == 0:
-                            a = adv[idx]
-                            loss = -torch.min(ratio * a, torch.clamp(ratio, 1 - clip, 1 + clip) * a).mean()
-                        elif loss_kind == 1:
-                            loss = -(ratio * adv[idx]).mean()
-                        else:
-                            loss = (ratio * adv_c[idx]).mean()
-                        surr['loss'], surr['ratio'] = float(loss.detach()), float(ratio.detach().mean())
-                        if loss_kind == 0 and entropy_coef:
-                            loss = loss - entropy_coef * d.entropy().mean()
+                        loss, info = actor_loss64(
+                            ac.actor_dist(p, o), Normal(old.loc[idx], old.scale[idx]), act[idx], logp[idx], adv[idx],
+                            adv_r[idx], adv_c[idx], loss_kind=loss_kind, clip=clip, entropy_coef=entropy_coef,
+                            focops_lam=focops_lam, focops_eta=focops_eta)
+                        surr.update(info)
                         return loss
                 else:
                     def loss_fn(p, net=net):
@@ -171,9 +252,10 @@ def ppo_epoch64(theta, data, moments, perms, lam, *, net_mask, loss_kind, batch_
                                                      critic_norm_coef=critic_norm_coef)
                 sl = slice(lay[net]['start'], lay[net]['start'] + lay[net]['size'])
                 rec['norm'][k], rec['coef'][k], rec['grad'][sl] = norm, coef, grad
-                rec['loss'][k] = surr['loss'] if net == 'actor' else logged
+                rec['loss'][k] = surr['stats'][0] if net == 'actor' else logged
                 if net == 'actor':
-                    rec['ratio'] = surr['ratio']
+                    rec['ratio'] = surr['stats'][1]
+                    rec.update({key: surr[key] for key in ('stats', 'pass1', 'gate', 'margin', 'entropy')})
             record.append(rec)
         passes += 1
         if train_actor:
