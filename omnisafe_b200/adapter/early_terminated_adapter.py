@@ -9,6 +9,7 @@ import torch
 
 from omnisafe_b200._lib import lib, ptr
 from omnisafe_b200.adapter.onpolicy_adapter import OnPolicyAdapter
+from omnisafe_b200.utils.train_state import restore, snapshot
 
 
 class EarlyTerminatedAdapter(OnPolicyAdapter):
@@ -23,3 +24,10 @@ class EarlyTerminatedAdapter(OnPolicyAdapter):
             super().rollout(steps_per_epoch, agent, buffer, logger, eps=eps)
         finally:
             lib().osb_rollout_set_early_termination(0, 0.0)
+
+    def train_state(self) -> dict:
+        return {**super().train_state(), 'cost_logger': snapshot(self._cost_logger)[0]}
+
+    def load_train_state(self, state: dict) -> None:
+        super().load_train_state(state)
+        restore(self._cost_logger, state['cost_logger'], 'early-termination cost accumulator')

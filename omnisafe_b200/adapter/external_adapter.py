@@ -14,7 +14,8 @@ statistics and feeds the observation normaliser.  Nothing in the loop synchronis
 the epoch.
 
 For an env that declares `graph_safe` (envs/core.py) the loop from osb_ext_act(0) to osb_ext_act(T) is captured into
-one CUDA graph in the second epoch and replayed from then on (the first epoch runs eagerly and warms everything up); the
+one CUDA graph in the second epoch and replayed from then on (the first epoch the adapter runs -- also the first one
+after `load_train_state` in a resumed process -- is eager and warms everything up); the
 captured act launches read the Philox epoch from a device counter that the graph's last kernel advances.  The reset and
 everything after the epoch-end act run outside the graph, with the same code as the eager loop.  OSB_NO_GRAPH=1 keeps
 every epoch eager.
@@ -26,8 +27,10 @@ import os
 import torch
 
 from omnisafe_b200._lib import OsbError, current_stream, lib, ptr
+from omnisafe_b200.adapter.onpolicy_adapter import episode_state, load_episode_state
 from omnisafe_b200.common.normalizer import Normalizer, ScalarNormalizer
 from omnisafe_b200.envs.core import check_env, make
+from omnisafe_b200.utils.train_state import restore, snapshot
 
 
 class ExternalEnvAdapter:
@@ -72,6 +75,7 @@ class ExternalEnvAdapter:
         # CUDA-graph replay of the epoch for envs that declare graph_safe (envs/core.py); OSB_NO_GRAPH=1 turns it off
         self._use_graph = bool(getattr(self._env, 'graph_safe', False)) and not os.getenv('OSB_NO_GRAPH')
         self._mode_logged = False
+        self._warm = False                              # an epoch ran in this process: the next one may replay
         self._graph = None
         self._graph_key_baked = None
         self.captures = 0                               # graphs captured so far (a recapture follows a pointer change)
@@ -198,7 +202,7 @@ class ExternalEnvAdapter:
         env_dev = torch.as_tensor(obs).device
         if self._use_graph and env_dev.type != 'cuda':
             raise ValueError(f'{type(self._env).__name__} declares graph_safe but reset() returned observations on {env_dev}')
-        replay = self._use_graph and self._epoch_index > 0
+        replay = self._use_graph and self._warm
         reset_obs = obs
         if replay:
             obs = self._obs0.copy_(torch.as_tensor(reset_obs).reshape(N, O))
@@ -233,9 +237,31 @@ class ExternalEnvAdapter:
         if self._cost_normalizer is not None:
             self._cost_normalizer.normalize_rows_(d['cost'])
         self._epoch_index += 1
+        self._warm = True
         if int(self.nonfinite.item()):
             self.nonfinite.zero_()
             raise OsbError(f'{type(self._env).__name__} returned a non-finite observation during the last epoch')
+
+    def train_state(self) -> dict:
+        """The adapter's own per-env state, the episode window, the normalisers and -- when the env has the optional
+        `state_dict()` / `load_state_dict(sd)` hooks (envs/core.py) -- the env's state."""
+        s_raw, final_raw, ep_ret, ep_cost, ep_len = snapshot(self.s_raw, self.final_raw, self.ep_ret, self.ep_cost,
+                                                             self.ep_len)
+        state = {**episode_state(self), 's_raw': s_raw, 'final_raw': final_raw, 'ep_ret': ep_ret, 'ep_cost': ep_cost,
+                 'ep_len': ep_len}
+        hook = getattr(self._env, 'state_dict', None)
+        if callable(hook):
+            state['env'] = hook()
+        return state
+
+    def load_train_state(self, state: dict) -> None:
+        """Restores in place; the first epoch after it runs eagerly (graph-safe envs capture in the one after)."""
+        load_episode_state(self, state)
+        for k in ('s_raw', 'final_raw', 'ep_ret', 'ep_cost', 'ep_len'):
+            restore(getattr(self, k), state[k], f'external-env adapter {k}')
+        hook = getattr(self._env, 'load_state_dict', None)
+        if 'env' in state and callable(hook):
+            hook(state['env'])
 
     def close(self) -> None:
         self._env.close()

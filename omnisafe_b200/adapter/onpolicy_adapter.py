@@ -12,6 +12,7 @@ import torch
 from omnisafe_b200._lib import current_stream, lib, ptr
 from omnisafe_b200.common.normalizer import Normalizer, ScalarNormalizer
 from omnisafe_b200.envs.synthetic import SyntheticBoxEnv
+from omnisafe_b200.utils.train_state import restore, snapshot
 
 
 class OnPolicyAdapter:
@@ -90,5 +91,40 @@ class OnPolicyAdapter:
             self._cost_normalizer.normalize_rows_(buffer.data['cost'])
         self._epoch_index += 1
 
+    def train_state(self) -> dict:
+        return {**episode_state(self), 'env': self._env.train_state()}
+
+    def load_train_state(self, state: dict) -> None:
+        load_episode_state(self, state)
+        self._env.load_train_state(state['env'])
+
     def close(self) -> None:
         self._env.close()
+
+
+def episode_state(ad) -> dict:
+    """The state an adapter (OnPolicyAdapter, ExternalEnvAdapter) carries from one epoch to the next besides its env's:
+    the Philox epoch counter, the episode window and every normaliser."""
+    ring, meta, sums = snapshot(ad.ep_ring, ad.ep_meta, ad.window_sums)
+    state = {'epoch_index': ad._epoch_index, 'ep_ring': ring, 'ep_meta': meta, 'window_sums': sums,
+             'obs_normalizer': ad._obs_normalizer.train_state()}
+    for key in ('reward_normalizer', 'cost_normalizer'):
+        nz = getattr(ad, f'_{key}')
+        if nz is not None:
+            state[key] = nz.train_state()
+    return state
+
+
+def load_episode_state(ad, state: dict) -> None:
+    ad._epoch_index = int(state['epoch_index'])
+    restore(ad.ep_ring, state['ep_ring'], 'episode ring')
+    restore(ad.ep_meta, state['ep_meta'], 'episode ring counters')
+    restore(ad.window_sums, state['window_sums'], 'episode window sums')
+    ad._obs_normalizer.load_train_state(state['obs_normalizer'])
+    for key in ('reward_normalizer', 'cost_normalizer'):
+        nz = getattr(ad, f'_{key}')
+        if (nz is not None) != (key in state):
+            raise RuntimeError(f'training state: {key} is {"absent" if nz is None else "present"} in this run, '
+                               f'{"present" if key in state else "absent"} in the saved one')
+        if nz is not None:
+            nz.load_train_state(state[key])

@@ -13,6 +13,7 @@ import torch
 
 from omnisafe_b200._lib import lib, ptr
 from omnisafe_b200.adapter.onpolicy_adapter import OnPolicyAdapter
+from omnisafe_b200.utils.train_state import restore, snapshot
 
 
 def per_step_budget(budget: float, saute_gamma: float, max_ep_len: float) -> float:
@@ -48,6 +49,13 @@ class SauteAdapter(OnPolicyAdapter):
         finally:
             lib().osb_rollout_set_saute(0, 1.0, 1.0, 0.0, 1.0)
         self._last_buffer = buffer
+
+    def train_state(self) -> dict:
+        return {**super().train_state(), 'safety': snapshot(self.safety)[0]}
+
+    def load_train_state(self, state: dict) -> None:
+        super().load_train_state(state)
+        restore(self.safety, state['safety'], 'Saute safety state')
 
     def ep_budget_mean(self) -> float:
         """Metrics/EpBudget (saute_adapter.py:L218-260): per finished episode the sum of the safety state after each of

@@ -29,3 +29,16 @@ class SimmerAdapter(SauteAdapter):
         self._budget_t = self._controller.act(safety_budget=self._budget_t, observation=obs)
         self._rel_t = self._budget_t / self._upper_t
         self._safety_budget = float(self._budget_t[0, 0])
+
+    def train_state(self) -> dict:
+        return {**super().train_state(), 'budget': self._budget_t.clone(), 'rel': self._rel_t.clone(),
+                'safety_budget': self._safety_budget, 'controller': self._controller.train_state()}
+
+    def load_train_state(self, state: dict) -> None:
+        super().load_train_state(state)
+        if tuple(state['budget'].shape) != tuple(self._budget_t.shape):
+            raise RuntimeError(f'training state: Simmer budget is {tuple(state["budget"].shape)}, this run has '
+                               f'{tuple(self._budget_t.shape)}')
+        self._budget_t, self._rel_t = state['budget'].clone(), state['rel'].clone()
+        self._safety_budget = float(state['safety_budget'])
+        self._controller.load_train_state(state['controller'])

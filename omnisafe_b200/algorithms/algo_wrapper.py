@@ -1,13 +1,16 @@
 """`omnisafe_b200.Agent` -- the `omnisafe.Agent(algo, env_id, train_terminal_cfgs, custom_cfgs)`
 entry point (mirrors omnisafe/algorithms/algo_wrapper.py:L36-269: config merge, checks,
-`distributed.fork`, `registry.get(algo)(env_id, cfgs)`, `learn()`)."""
+`distributed.fork`, `registry.get(algo)(env_id, cfgs)`, `learn()`), plus saving the training state and resuming a
+stopped run from it (`save_state`, `learn(save_state_freq=...)`, `resume`; upstream has no resume)."""
 from __future__ import annotations
 
+import json
+import os
 import sys
 
 from omnisafe_b200.algorithms import ALGORITHM2TYPE, registry
 from omnisafe_b200.envs import support_envs
-from omnisafe_b200.utils import distributed
+from omnisafe_b200.utils import distributed, train_state
 from omnisafe_b200.utils.config import (Config, check_all_configs, get_default_kwargs_yaml,
                                         recursive_check_config)
 
@@ -45,14 +48,52 @@ class AlgoWrapper:
             f"{self.env_id} doesn't exist. omnisafe_b200 accelerates {support_envs()}; "
             'use upstream omnisafe for simulator-backed environments.')
 
-    def _init_algo(self) -> None:
+    def _init_algo(self, run_dir: str | None = None) -> None:
         check_all_configs(self.cfgs)
         if distributed.fork(self.cfgs.train_cfgs.parallel, device=self.cfgs.train_cfgs.device):
             sys.exit()
-        self.agent = registry.get(self.algo)(env_id=self.env_id, cfgs=self.cfgs)
+        if run_dir is None:
+            self.agent = registry.get(self.algo)(env_id=self.env_id, cfgs=self.cfgs)
+        else:
+            self.agent = registry.get(self.algo).continuing(run_dir, env_id=self.env_id, cfgs=self.cfgs)
 
-    def learn(self) -> tuple[float, float, float]:
-        return self.agent.learn()
+    @classmethod
+    def resume(cls, state_dir: str) -> AlgoWrapper:
+        """Continue a run from a training state `save_state` / `learn(save_state_freq=...)` wrote.
+
+        The run is rebuilt from its config.json (the configuration cannot change on resume) through the same checks and
+        `distributed.fork` as a new run -- so a script calling `Agent.resume(d).learn()` under `parallel: 2` works --
+        then every rank loads its state in place.  `learn()` trains the remaining epochs into the original run directory:
+        progress.csv is appended to, torch_save/epoch-k.pt keeps its numbering, config.json stays as it is."""
+        state_dir = os.path.abspath(state_dir)
+        meta = train_state.read_meta(state_dir)
+        run_dir = train_state.run_dir(state_dir)
+        path = os.path.join(run_dir, 'config.json')
+        if not os.path.exists(path):
+            raise RuntimeError(f'{path} is missing: {state_dir} is not inside a run directory')
+        with open(path, encoding='utf-8') as fh:
+            cfgs = Config.dict2config(json.load(fh))
+        self = cls.__new__(cls)
+        self.algo, self.env_id = cfgs.algo, cfgs.env_id
+        self.train_terminal_cfgs = self.custom_cfgs = None
+        self._evaluator = None
+        assert self.algo in ALGORITHM2TYPE, f'{self.algo} doesn\'t exist. Please choose from {list(ALGORITHM2TYPE)}.'
+        self.algo_type = ALGORITHM2TYPE[self.algo]
+        self.cfgs = cfgs
+        self._init_checks()
+        train_state.check_meta(meta, train_state.config_meta(cfgs, int(cfgs.train_cfgs.parallel)), state_dir)
+        self._init_algo(run_dir=run_dir)
+        self.agent.load_train_state(state_dir)
+        return self
+
+    def learn(self, save_state_freq: int = 0) -> tuple[float, float, float]:
+        """Train (the remaining epochs, after `resume`).  `save_state_freq` > 0: also write the training state after every
+        `save_state_freq`-th epoch and after the last one, to <log_dir>/train_state/epoch-{k}/."""
+        return self.agent.learn(save_state_freq=save_state_freq)
+
+    def save_state(self) -> str:
+        """Write the training state now (between epochs; every rank calls it) and return its directory."""
+        return self.agent.save_train_state()
 
     def evaluate(self, *_, **__):
         raise NotImplementedError('evaluation / rendering stay with the upstream Evaluator, which loads '

@@ -11,6 +11,17 @@ from omnisafe_b200.utils.config import Config
 
 
 class BaseAlgo(ABC):
+    _run_dir: str | None = None     # the directory of a run being resumed (`continuing`): the logger continues it
+
+    @classmethod
+    def continuing(cls, run_dir: str, env_id: str, cfgs: Config) -> BaseAlgo:
+        """Construct the algorithm of an existing run directory (for `load_train_state`), keeping the upstream
+        constructor signature `(env_id, cfgs)`."""
+        obj = cls.__new__(cls)
+        obj._run_dir = run_dir
+        obj.__init__(env_id, cfgs)
+        return obj
+
     def __init__(self, env_id: str, cfgs: Config) -> None:
         self._env_id = env_id
         self._cfgs = cfgs

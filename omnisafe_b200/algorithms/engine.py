@@ -8,6 +8,7 @@ import torch
 
 from omnisafe_b200._lib import current_stream, lib, ptr
 from omnisafe_b200.utils import distributed
+from omnisafe_b200.utils.train_state import restore, snapshot
 
 LOSS_PPO_CLIP, LOSS_RATIO, LOSS_FOCOPS, LOSS_COST, LOSS_P3O = 0, 1, 2, 3, 5
 NET_ACTOR, NET_CRITIC_R, NET_CRITIC_C = 1, 2, 4
@@ -64,6 +65,15 @@ class UpdateEngine:
     def next_perm_seed(self) -> int:
         self._perm_seed = (self._perm_seed * 1664525 + 1013904223) & 0xFFFFFFFF
         return self._perm_seed
+
+    def train_state(self) -> dict:
+        """The minibatch-permutation LCG and kl_state: NaturalPG / RCPO log the KL an epoch leaves in kl_state[0] as the
+        next epoch's final KL (NaturalPG._update).  Everything else here is rewritten before it is read in an epoch."""
+        return {'perm_seed': self._perm_seed, 'kl_state': snapshot(self.kl_state)[0]}
+
+    def load_train_state(self, state: dict) -> None:
+        self._perm_seed = int(state['perm_seed'])
+        restore(self.kl_state, state['kl_state'], 'update kl_state')
 
     # ---- PolicyGradient._update loop (one C call) -----------------------------------------
     def ppo_epoch(self, *, loss_kind, lagrange, net_mask, batch_size, update_iters, clip=0.2,

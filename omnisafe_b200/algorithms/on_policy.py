@@ -29,7 +29,7 @@ from omnisafe_b200.common.logger import Logger
 from omnisafe_b200.common.pid_lagrange import PIDLagrangian
 from omnisafe_b200.envs.synthetic import support_envs as synthetic_envs
 from omnisafe_b200.models.actor_critic import ConstraintActorCritic
-from omnisafe_b200.utils import distributed
+from omnisafe_b200.utils import distributed, train_state
 
 
 def _plain_adapter(env_id: str):
@@ -75,11 +75,13 @@ class PolicyGradient(BaseAlgo):
         self._engine.precision = {'fp32': 0, 'tf32': 1, 'bf16x3': 2}[prec]
         self._actor_critic.precision = self._engine.precision   # step / predict / critics use the training arithmetic
         self._stats8 = torch.zeros(8, dtype=torch.float64, device=self._device)
+        self._epochs_done = 0       # epochs trained so far (a resumed run starts at the saved count)
+        self._first_epoch = 0       # where learn() starts
 
     def _init_log(self) -> None:
         lc = self._cfgs.logger_cfgs
         self._logger = Logger(lc.log_dir, self._cfgs.exp_name, seed=self._cfgs.seed, config=self._cfgs,
-                              verbose=bool(getattr(lc, 'verbose', False)))
+                              verbose=bool(getattr(lc, 'verbose', False)), run_dir=self._run_dir)
         what = {'pi': self._actor_critic.actor_state_dict}
         what.update(self._env.save())
         self._logger.setup_torch_saver(what)
@@ -90,13 +92,17 @@ class PolicyGradient(BaseAlgo):
             self._logger.register_key(key)
 
     # ---- training loop (policy_gradient.py:L238-306) -------------------------------------------
-    def learn(self) -> tuple[float, float, float]:
+    def learn(self, save_state_freq: int = 0) -> tuple[float, float, float]:
+        """Train epochs `_first_epoch` (0, or k after `load_train_state`) .. epochs-1.  `save_state_freq` > 0: write the
+        training state after every `save_state_freq`-th epoch and after the last one."""
         self._start_time = time.time()
         t = self._cfgs.train_cfgs
-        for epoch in range(t.epochs):
+        for epoch in range(self._first_epoch, t.epochs):
             self.train_epoch(log=True, epoch=epoch)
             if (epoch + 1) % self._cfgs.logger_cfgs.save_model_freq == 0 or (epoch + 1) == t.epochs:
                 self._logger.torch_save()
+            if save_state_freq > 0 and ((epoch + 1) % save_state_freq == 0 or (epoch + 1) == t.epochs):
+                self.save_train_state()
         ep = self._window_means()
         self._logger.close()
         self._env.close()
@@ -113,6 +119,7 @@ class PolicyGradient(BaseAlgo):
         roll = time.time()
         self._update()
         self._actor_critic.actor_scheduler_step()
+        self._epochs_done += 1
         if not log:
             self._epochs_unchecked = getattr(self, '_epochs_unchecked', 0) + 1
             if distributed.world_size() > 1 and self._epochs_unchecked >= 16:     # the NVLink exchange reports time-outs through a flag
@@ -168,6 +175,50 @@ class PolicyGradient(BaseAlgo):
     def _log_extra(self) -> None:
         pass
 
+    # ---- training state: save at an epoch boundary, resume bit for bit ---------------------------------------------------
+    def _state_meta(self) -> dict:
+        return {**train_state.config_meta(self._cfgs, distributed.world_size()), 'obs_dim': self._env.obs_dim,
+                'act_dim': self._env.act_dim}
+
+    def _train_state(self) -> dict:
+        """This rank's state, composed from the owners' train_state() (subclasses add their own entries).  The global
+        RNGs are part of it: the policy step's sampling and user envs draw from them."""
+        return {'epochs_done': self._epochs_done, 'model': self._actor_critic.train_state(),
+                'engine': self._engine.train_state(), 'env': self._env.train_state(),
+                'logger': self._logger.train_state(),
+                'rng': {'cpu': torch.get_rng_state(), 'cuda': torch.cuda.get_rng_state(self._device)}}
+
+    def _load_train_state(self, state: dict) -> None:
+        self._actor_critic.load_train_state(state['model'])
+        self._engine.load_train_state(state['engine'])
+        self._env.load_train_state(state['env'])
+        self._logger.load_train_state(state['logger'])
+        torch.set_rng_state(state['rng']['cpu'])
+        torch.cuda.set_rng_state(state['rng']['cuda'], self._device)
+        self._epochs_done = self._first_epoch = int(state['epochs_done'])
+
+    def save_train_state(self) -> str:
+        """Write every rank's training state to <log_dir>/train_state/epoch-{k}/ (k = epochs trained) and return the
+        directory.  Call it between epochs; every rank must call it."""
+        k = self._epochs_done
+        rank = distributed.get_rank()
+        sdir = distributed.broadcast_object(train_state.state_dir(self._logger.log_dir, k))
+        if rank == 0:
+            train_state.begin(sdir)
+        distributed.barrier()
+        train_state.write_rank(sdir, rank, k, self._train_state())
+        distributed.barrier()
+        if rank == 0:
+            train_state.write_meta(sdir, {**self._state_meta(), 'epoch': k})
+        distributed.barrier()
+        return sdir
+
+    def load_train_state(self, sdir: str) -> None:
+        """Load this rank's state from a directory `save_train_state` wrote, into the tensors this object allocated."""
+        meta = train_state.read_meta(sdir)
+        train_state.check_meta(meta, self._state_meta(), sdir)
+        self._load_train_state(train_state.load_rank(sdir, distributed.get_rank(), int(meta['epoch'])))
+
     # ---- update (policy_gradient.py:L308-405) -----------------------------------------------------
     def _lagrange_ptr(self):
         return None
@@ -209,6 +260,13 @@ class _LagrangeMixin:
     def _lagrange_ptr(self):
         return self._lagrange.state
 
+    def _train_state(self) -> dict:
+        return {**super()._train_state(), 'lagrange': self._lagrange.train_state()}
+
+    def _load_train_state(self, state: dict) -> None:
+        super()._load_train_state(state)
+        self._lagrange.load_train_state(state['lagrange'])
+
     def _update(self, *args, **kwargs) -> None:
         # Jc = windowed mean EpCost (already all-reduced); first update lambda, then the networks
         self._lagrange.update_lagrange_multiplier(self._env.window_sums)
@@ -247,6 +305,14 @@ class IPO(PPO):
 
     def _lagrange_ptr(self):
         return self._penalty_state
+
+    def _train_state(self) -> dict:
+        return {**super()._train_state(), 'penalty_state': self._penalty_state.cpu().clone(), 'penalty': self._penalty}
+
+    def _load_train_state(self, state: dict) -> None:
+        super()._load_train_state(state)
+        train_state.restore(self._penalty_state, state['penalty_state'], 'IPO penalty state')
+        self._penalty = float(state['penalty'])
 
     def _update(self, *args, **kwargs) -> None:
         a = self._cfgs.algo_cfgs
@@ -599,6 +665,13 @@ class OnCRPO(TRPO):
 
     def _adv_lagrange(self):
         return None
+
+    def _train_state(self) -> dict:
+        return {**super()._train_state(), 'rew_update': self._rew_update, 'cost_update': self._cost_update}
+
+    def _load_train_state(self, state: dict) -> None:
+        super()._load_train_state(state)
+        self._rew_update, self._cost_update = int(state['rew_update']), int(state['cost_update'])
 
     def _surrogate_kind(self) -> int:
         a = self._cfgs.algo_cfgs

@@ -9,6 +9,7 @@ from __future__ import annotations
 import torch
 
 from omnisafe_b200._lib import current_stream, lib, ptr
+from omnisafe_b200.utils.train_state import restore, snapshot
 
 
 class Lagrange:
@@ -29,6 +30,13 @@ class Lagrange:
     @property
     def lagrangian_multiplier(self) -> torch.Tensor:
         return self.state[0]
+
+    def train_state(self) -> dict:
+        """lambda and its Adam moments / step count."""
+        return {'state': snapshot(self.state)[0]}
+
+    def load_train_state(self, state: dict) -> None:
+        restore(self.state, state['state'], 'Lagrange state')
 
     def update_lagrange_multiplier(self, Jc) -> None:   # noqa: N803  (the reference's argument name)
         """Reference signature `update_lagrange_multiplier(Jc: float)` (common/lagrange.py:L114-136): Adam step on

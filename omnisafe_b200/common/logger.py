@@ -19,9 +19,12 @@ from omnisafe_b200.utils import distributed
 
 
 class Logger:
-    def __init__(self, output_dir: str, exp_name: str, seed: int = 0, config=None, verbose: bool = False) -> None:
+    def __init__(self, output_dir: str, exp_name: str, seed: int = 0, config=None, verbose: bool = False,
+                 run_dir: str | None = None) -> None:
+        """`run_dir`: continue an existing run's directory (a resumed run): config.json stays as it is and
+        progress.csv is opened by `load_train_state`."""
         hms = time.strftime('%Y-%m-%d-%H-%M-%S')
-        self._log_dir = os.path.join(output_dir, exp_name, f'seed-{str(seed).zfill(3)}-{hms}')
+        self._log_dir = run_dir or os.path.join(output_dir, exp_name, f'seed-{str(seed).zfill(3)}-{hms}')
         self._master = distributed.is_master()
         self._verbose = verbose
         self._epoch = 0
@@ -30,7 +33,8 @@ class Logger:
         self._first = True
         self._what_to_save = None
         self._csv = None
-        if self._master:
+        self._file = None
+        if self._master and run_dir is None:
             os.makedirs(os.path.join(self._log_dir, 'torch_save'), exist_ok=True)
             self._file = open(os.path.join(self._log_dir, 'progress.csv'), 'w', encoding='utf-8', newline='')
             if config is not None:
@@ -85,6 +89,37 @@ class Logger:
             if self._verbose:
                 print(' | '.join(f'{k}={self._row[k]:.4g}' for k in self._keys if 'Metrics' in k or 'FPS' in k), flush=True)
         self._epoch += 1
+
+    def train_state(self) -> dict:
+        return {'epoch': self._epoch}
+
+    def load_train_state(self, state: dict) -> None:
+        """Continue at epoch `state['epoch']`: progress.csv keeps its header and the rows of the epochs before it -- rows
+        a stopped run wrote after its last saved state belong to epochs that run again -- and is appended to."""
+        self._epoch = int(state['epoch'])
+        if not self._master:
+            return
+        path = os.path.join(self._log_dir, 'progress.csv')
+        lines = []
+        if os.path.exists(path):
+            with open(path, encoding='utf-8', newline='') as fh:
+                lines = fh.read().splitlines(keepends=True)
+        if self._epoch > 0:
+            if len(lines) < 1 + self._epoch:
+                raise RuntimeError(f'{path} has {max(len(lines) - 1, 0)} epoch rows, the training state is at epoch '
+                                   f'{self._epoch}')
+            header = next(csv.reader(lines[:1]))
+            if header != self._keys:
+                raise RuntimeError(f'{path}: the header differs from the keys this run logs')
+        lines = lines[:1 + self._epoch] if self._epoch > 0 else []
+        tmp = f'{path}.tmp-{os.getpid()}'
+        with open(tmp, 'w', encoding='utf-8', newline='') as fh:
+            fh.writelines(lines)
+        os.replace(tmp, path)
+        self._file = open(path, 'a', encoding='utf-8', newline='')
+        if lines:
+            self._csv = csv.writer(self._file)
+            self._first = False
 
     def close(self) -> None:
         if self._master and self._file:

@@ -9,6 +9,8 @@ from __future__ import annotations
 
 import torch
 
+from omnisafe_b200.utils.train_state import restore, snapshot
+
 
 class Normalizer:
     def __init__(self, shape: tuple[int, ...], clip: float = 5.0, device='cuda') -> None:
@@ -53,6 +55,16 @@ class Normalizer:
         self.mean.copy_(sd['_mean']); self.sumsq.copy_(sd['_sumsq']); self.std.copy_(sd['_std'])
         self.count[0] = int(sd['_count'])
 
+    _STATE = ('mean', 'sumsq', 'std', 'mean1', 'std1', 'count', 'acc_all', 'acc_fin', 'fin_count', 'had_fin', 'ticket')
+
+    def train_state(self) -> dict[str, torch.Tensor]:
+        """Every tensor the rollout kernels carry from step to step (state_dict() keeps the reference's subset)."""
+        return dict(zip(self._STATE, snapshot(*(getattr(self, k) for k in self._STATE))))
+
+    def load_train_state(self, state: dict) -> None:
+        for k in self._STATE:
+            restore(getattr(self, k), state[k], f'obs normaliser {k}')
+
 
 class ScalarNormalizer:
     """`Normalizer(shape=(), clip=5)` of RewardNormalize / CostNormalize (envs/wrapper.py:L280-423) with its
@@ -94,3 +106,11 @@ class ScalarNormalizer:
     def load_state_dict(self, sd: dict[str, torch.Tensor]) -> None:
         self.state[0] = float(sd['_mean']); self.state[1] = float(sd['_sumsq']); self.state[2] = float(sd['_std'])
         self.count[0] = int(sd['_count'])
+
+    def train_state(self) -> dict[str, torch.Tensor]:
+        state, count = snapshot(self.state, self.count)
+        return {'state': state, 'count': count}
+
+    def load_train_state(self, state: dict) -> None:
+        restore(self.state, state['state'], 'scalar normaliser state')
+        restore(self.count, state['count'], 'scalar normaliser count')

@@ -9,6 +9,7 @@ from __future__ import annotations
 import torch
 
 from omnisafe_b200._lib import current_stream, lib, ptr
+from omnisafe_b200.utils.train_state import restore, snapshot
 
 
 class PIDLagrangian:
@@ -32,6 +33,15 @@ class PIDLagrangian:
     @property
     def lagrangian_multiplier(self) -> torch.Tensor:
         return self.state[0]
+
+    def train_state(self) -> dict:
+        """The fp64 controller terms (integral, EMAs, the derivative delay line) and the fp32 multiplier."""
+        pid_state, state = snapshot(self.pid_state, self.state)
+        return {'pid_state': pid_state, 'state': state}
+
+    def load_train_state(self, state: dict) -> None:
+        restore(self.pid_state, state['pid_state'], 'PID-Lagrangian controller state')
+        restore(self.state, state['state'], 'PID-Lagrangian multiplier')
 
     def pid_update(self, window_sums: torch.Tensor) -> None:
         """`window_sums` = device fp64 {sum EpRet, sum EpCost, sum EpLen, count} of the episode window

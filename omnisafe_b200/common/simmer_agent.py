@@ -33,3 +33,13 @@ class SimmerPIDAgent:
         new_budget = torch.clamp(safety_budget + step, _TINY_BUDGET * torch.ones_like(safety_budget), self._bound)
         self._last_action, self._last_raw, self._last_err = new_budget - safety_budget, raw, err
         return new_budget
+
+    def train_state(self) -> dict:
+        return {'last_action': self._last_action.clone(), 'last_raw': self._last_raw.clone(),
+                'last_err': self._last_err.clone(), 'window': [e.clone() for e in self._window]}
+
+    def load_train_state(self, state: dict) -> None:
+        self._last_action = state['last_action'].clone()
+        self._last_raw = state['last_raw'].clone()
+        self._last_err = state['last_err'].clone()
+        self._window = deque((e.clone() for e in state['window']), maxlen=self._window.maxlen)

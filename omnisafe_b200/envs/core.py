@@ -22,6 +22,13 @@ epoch, which removes the host's per-launch cost.  Such an env promises:
 - `info` holds `final_observation` and `_final_observation` on every step (the mask all false when nothing finished),
   so its structure is the same on every step;
 - the tensors `step` returns may be fresh each call: the adapter copies them inside the graph.
+
+An env may also define `state_dict() -> dict` and `load_state_dict(sd)` (optional, an omnisafe_b200 extension).  When it
+does, a saved training state (`AlgoWrapper.save_state`, `learn(save_state_freq=...)`) holds what `state_dict()` returns and
+`Agent.resume` hands it back to `load_state_dict` right after `set_seed`, before the first epoch; a run that resumes then
+continues to the same bits as one that never stopped.  `sd` holds CPU tensors (the file is loaded onto the CPU).  A
+graph-safe env writes them into its existing state in place (`copy_`), since the storage is captured.  Without the hooks
+the env starts the resumed run in its freshly seeded state, and only the library's own state is restored.
 """
 from __future__ import annotations
 

@@ -12,6 +12,8 @@ from __future__ import annotations
 import numpy as np
 import torch
 
+from omnisafe_b200.utils.train_state import restore
+
 _SUPPORT = ['SyntheticBox-v0']
 
 
@@ -79,6 +81,16 @@ class SyntheticBoxEnv:
     def state_ptrs(self) -> list:
         return [t.data_ptr() for t in (self.s_raw, self.final_raw, self.ep_step, self.episode,
                                        self.gstep, self.ep_ret, self.ep_cost, self.ep_len, self.bias)]
+
+    _STATE = ('s_raw', 'final_raw', 'ep_step', 'episode', 'gstep', 'ep_ret', 'ep_cost', 'ep_len')
+
+    def train_state(self) -> dict:
+        """The per-env state the rollout kernel carries across epochs (`bias` is a function of obs_dim)."""
+        return {k: getattr(self, k).detach().cpu().clone() for k in self._STATE}
+
+    def load_train_state(self, state: dict) -> None:
+        for k in self._STATE:
+            restore(getattr(self, k), state[k], f'synthetic env {k}')
 
     def close(self) -> None:
         pass

@@ -28,6 +28,7 @@ from torch.distributions import Normal
 from torch.distributions.utils import _standard_normal
 
 from omnisafe_b200._lib import lib, ptr
+from omnisafe_b200.utils.train_state import restore, snapshot
 
 HID = 64
 NET_ACTOR, NET_REWARD, NET_COST = 1, 2, 4   # net_mask bits of osb_policy_step
@@ -128,6 +129,17 @@ class ConstraintActorCritic:
 
     def actor_scheduler_step(self) -> None:
         self._sched_epoch += 1
+
+    # -- training state (the reference-format actor_state_dict() stays what epoch-k.pt holds) -----
+    def train_state(self) -> dict:
+        """Parameters, Adam moments, per-network Adam step counts and the LinearLR epoch."""
+        theta, m, v, step = snapshot(self.theta, self.adam_m, self.adam_v, self.adam_step)
+        return {'theta': theta, 'adam_m': m, 'adam_v': v, 'adam_step': step, 'sched_epoch': self._sched_epoch}
+
+    def load_train_state(self, state: dict) -> None:
+        for k in ('theta', 'adam_m', 'adam_v', 'adam_step'):
+            restore(getattr(self, k), state[k], f'model {k}')
+        self._sched_epoch = int(state['sched_epoch'])
 
     # -- acting (constraint_actor_critic.py:L84-109) ----------------------------------------------
     def step(self, obs, deterministic: bool = False) -> tuple[torch.Tensor, ...]:

@@ -133,6 +133,20 @@ def all_reduce_(t: torch.Tensor) -> torch.Tensor:
     return t
 
 
+def barrier() -> None:
+    if world_size() > 1:
+        dist.barrier()
+
+
+def broadcast_object(obj):
+    """Rank 0's `obj` on every rank (a picklable host object)."""
+    if world_size() == 1:
+        return obj
+    box = [obj]
+    dist.broadcast_object_list(box, src=0)
+    return box[0]
+
+
 def dist_avg(value: torch.Tensor | float) -> torch.Tensor:
     """Average over ranks (omnisafe/utils/distributed.py:L231-260)."""
     t = torch.as_tensor(value, dtype=torch.float32).clone()
