@@ -134,6 +134,55 @@ int osb_rollout_set_early_termination(float* cost_acc, float cost_limit);
  * across epochs; window_sums[4] <- {sum EpRet, sum EpCost, sum EpLen, count} (fp64). */
 int osb_episode_window(const unsigned char* flags, const float* epfin, int T, int N, int W,
                        float* ring, int* meta, double* window_sums, void* stream);
+/* ---- evaluation of a saved policy on the synthetic env (Evaluator.evaluate, omnisafe/evaluator.py:L399-490) ---------
+ * N envs (seed, env id offset 0), env e runs episodes e, e + N, ... of num_episodes (N <= num_episodes) with the
+ * deterministic action (the mean, the bits osb_policy_step gives without eps) and ActionScale.  Per step, as
+ * ObsNormalize pushes them: the final observations of envs whose env episode ended, the next observations of every env
+ * still running (an env that ended hands back its auto-reset observation), then the observations of the envs reset after
+ * the step.  N == 1 resets the env after every episode (the reference calls env.reset()); N > 1 only resets an env whose
+ * episode was cut by the cost rule.  Episode sums in fp64: return += reward, cost += cost_criteria^length * cost; early:
+ * the episode also ends once that cost >= cost_limit (PPOEarlyTerminated).  safety = [2][N] device floats or NULL:
+ * Saute / Simmer, z (column O of the network input) starts every episode at 1, z <- (z - cost / safety_budget) /
+ * saute_gamma after every step, the reward is never replaced.  The env and normaliser arrays are those of
+ * osb_rollout_step (the normaliser holds the loaded statistics; on return it holds the drifted ones).  Workspace,
+ * zeroed by the caller except left[e] = episodes of env e and ctr[0] = N: left, done_eps, len [N] ints, ret, cost [N]
+ * doubles, acc_rst [2][O] long longs, ctr [3] ints.  Results: out_ret / out_cost [num_episodes] doubles, out_len ints, in
+ * episode order.  act_out = [N][A] floats or NULL: the deterministic action of each env in the last step it ran.
+ * Precision 1 / 2 with O (+ 1 with safety) <= 64 run the tensor-core tiles, everything else the fp32 tiles.  On the
+ * tensor-core tiles, when the ceil(N / 128) CTAs fit on the SMs and per_step == 0, ONE cooperative launch runs every step
+ * with a grid barrier per step and ends when every env has finished; otherwise one launch per step, and the host reads
+ * the 4-byte done word ctr[0] (envs still running) every 16 steps -- its only synchronisation.  Both give the same bits. */
+int osb_eval_synthetic(int O, int A, int max_episode_steps, unsigned seed, unsigned term_threshold, float cost_threshold,
+                       int obs_normalize, int N, int num_episodes, float* s_raw, float* final_raw, int* ep_step,
+                       unsigned* episode, unsigned* gstep, float* ep_ret, float* ep_cost, int* ep_len, const float* bias,
+                       float* norm_mean, float* norm_sumsq, float* norm_std, float* norm_mean1, float* norm_std1,
+                       long long* norm_count, long long* acc_all, long long* acc_fin, int* fin_count, int* had_fin,
+                       unsigned* ticket, float* safety, float safety_budget, float saute_gamma, int early,
+                       double cost_limit, double cost_criteria, int* left, int* done_eps, double* ret, double* cost,
+                       int* len, long long* acc_rst, int* ctr, double* out_ret, double* out_cost, int* out_len,
+                       float* act_out, const float* theta, int precision, int per_step, void* stream);
+/* Evaluation on a registered env (a user CMDP stepped in PyTorch), same semantics and workspace (acc_rst unused).
+ * Per episode schedule: env.reset() -> osb_eval_ext_observe(is_reset = 1, t = -1); for t = 0, 1, ...:
+ * osb_eval_ext_act(t) -> env.step(act_env) -> osb_eval_ext_observe(t); then read ctr: ctr[0] == 0 ends the evaluation,
+ * ctr[2] > 0 (N == 1: the episode ended and another follows) asks for env.reset() -> osb_eval_ext_observe(is_reset = 1, t).
+ * N > 1 relies on the envs resetting themselves.  osb_eval_ext_act: ObsNormalize, the deterministic forward, act_env[N][A]
+ * <- ActionScale onto [act_lo, act_hi] (as osb_ext_act), act_out as above; no slabs.  osb_eval_ext_observe: the fp64
+ * sums, Saute z, the cost rule and the episode ends of the running envs; next_obs -> s_raw (the buffer step t + 1
+ * reads); ObsNormalize pushes the final rows of running envs (final_obs / final_mask may be NULL), then the next rows
+ * of running envs (reset: the rows of envs with episodes left) from fp64 per-tile moments combined in tile order.
+ * workspace: osb_eval_ext_workspace_doubles(O, N) doubles; nonfinite as for osb_ext_observe. */
+int osb_eval_ext_workspace_doubles(int O, int N);
+int osb_eval_ext_act(int O, int A, int obs_normalize, int N, int t, const float* s_raw, const float* norm_mean,
+                     const float* norm_std, const long long* norm_count, const float* safety, const float* theta,
+                     const float* act_lo, const float* act_hi, float* act_env, const int* left, const int* ctr,
+                     float* act_out, int precision, void* stream);
+int osb_eval_ext_observe(int O, int N, int t, int obs_normalize, int is_reset, const float* next_obs, const float* rew,
+                         const float* cost, const unsigned char* terminated, const unsigned char* truncated,
+                         const float* final_obs, const unsigned char* final_mask, float* s_raw, float* norm_mean,
+                         float* norm_sumsq, float* norm_std, long long* norm_count, unsigned* ticket, float* safety,
+                         float safety_budget, float saute_gamma, int early, double cost_limit, double cost_criteria,
+                         int* left, int* done_eps, double* ret, double* cost_acc, int* len, int* ctr, double* out_ret,
+                         double* out_cost, int* out_len, double* workspace, int* nonfinite, void* stream);
 /* ---- rollout on an external env (a user CMDP stepped in PyTorch) ----------------------------
  * The fused step split at the env boundary.  Per epoch: env.reset() -> osb_ext_reset_ingest; for t in [0, T):
  * osb_ext_act(t) -> env.step(act_env) -> osb_ext_observe(t); then osb_ext_act(T) (epoch-end bootstrap, critics only)

@@ -1,6 +1,6 @@
 """`omnisafe_b200.Agent` -- the `omnisafe.Agent(algo, env_id, train_terminal_cfgs, custom_cfgs)`
 entry point (mirrors omnisafe/algorithms/algo_wrapper.py:L36-269: config merge, checks,
-`distributed.fork`, `registry.get(algo)(env_id, cfgs)`, `learn()`), plus saving the training state and resuming a
+`distributed.fork`, `registry.get(algo)(env_id, cfgs)`, `learn()`, `evaluate()`), plus saving the training state and resuming a
 stopped run from it (`save_state`, `learn(save_state_freq=...)`, `resume`; upstream has no resume)."""
 from __future__ import annotations
 
@@ -10,6 +10,7 @@ import sys
 
 from omnisafe_b200.algorithms import ALGORITHM2TYPE, registry
 from omnisafe_b200.envs import support_envs
+from omnisafe_b200.evaluator import Evaluator
 from omnisafe_b200.utils import distributed, train_state
 from omnisafe_b200.utils.config import (Config, check_all_configs, get_default_kwargs_yaml,
                                         recursive_check_config)
@@ -95,6 +96,18 @@ class AlgoWrapper:
         """Write the training state now (between epochs; every rank calls it) and return its directory."""
         return self.agent.save_train_state()
 
-    def evaluate(self, *_, **__):
-        raise NotImplementedError('evaluation / rendering stay with the upstream Evaluator, which loads '
-                                  "this run's torch_save/epoch-k.pt (omnisafe/evaluator.py:L113-178)")
+    def evaluate(self, num_episodes: int = 10, cost_criteria: float = 1.0, num_envs: int = 1) -> None:
+        """Evaluate every torch_save/*.pt of this run with `Evaluator` (algo_wrapper.py:L215-231), in sorted file order
+        (upstream takes the directory's scandir order).  `num_envs`: see `Evaluator.evaluate`."""
+        log_dir = self.agent.logger.log_dir
+        save_dir = os.path.join(log_dir, 'torch_save')
+        assert os.path.isdir(save_dir), 'Please run learn() first!'
+        if self._evaluator is None:
+            self._evaluator = Evaluator()
+        for name in sorted(os.listdir(save_dir)):
+            if os.path.isfile(os.path.join(save_dir, name)) and name.split('.')[-1] == 'pt':
+                self._evaluator.load_saved(save_dir=log_dir, model_name=name)
+                self._evaluator.evaluate(num_episodes=num_episodes, cost_criteria=cost_criteria, num_envs=num_envs)
+
+    def render(self, *_, **__):
+        raise NotImplementedError('rendering is not supported')

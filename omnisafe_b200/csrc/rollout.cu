@@ -274,6 +274,29 @@ __device__ float philox_normal(uint32_t seed, uint32_t gid, uint32_t step, int a
     return (a & 1) ? n.y : n.x;
 }
 
+// Evaluation of a saved policy (Evaluator.evaluate, evaluator.py:L399-490) on N synthetic envs: env e runs episodes
+// e, e + N, ... of num_episodes with the deterministic action, and accumulates each in fp64 like the reference's
+// Python floats.  Results land in episode order.
+struct EvalSpec {
+    int* left;            // [N] episodes the env still has to run, the current one included (0: the env is idle)
+    int* done_eps;        // [N] episodes it has finished
+    double* ret;          // [N] return of the current episode
+    double* cost;         // [N] its cost, discounted by crit^length
+    int* len;             // [N] its length
+    double* out_ret;      // [num_episodes] results in episode order
+    double* out_cost;
+    int* out_len;
+    long long* acc_rst;   // [2][O] fixed-point sums of the reset rows of a step
+    int* ctr;             // [3]: [0] envs running at the start of this step (0: evaluation done -- the done word),
+                          //      [1] the same for the next step, [2] reset rows of this step
+    double crit;          // cost_criteria
+    double cost_limit;    // EarlyTerminated: an episode also ends once its discounted cost >= cost_limit
+    int early;
+    int explicit_reset;   // N == 1: the env is reset after every episode, as the reference calls env.reset();
+                          // N > 1: the envs reset themselves, only an episode cut by the cost rule resets the env
+    float* act_out;       // [N][A] the action of each running env in the last step it ran, or null
+};
+
 struct StepArgs {
     EnvSpec es;
     EnvState st;
@@ -299,6 +322,7 @@ struct StepArgs {
     // external-env act step replayed from a CUDA graph: the Philox counter is *epoch_dev * T + t (u32 wrap-around, as
     // the host computes global_step) instead of global_step.  Null: global_step is used.
     const unsigned* epoch_dev;
+    EvalSpec ev;              // EVAL instantiations only
 };
 
 // Philox counter of an act step: a graph replay reads the epoch from the device, an eager launch passes it
@@ -363,11 +387,18 @@ __device__ __forceinline__ void load_obs_tile(const float* __restrict__ raw, int
     }
 }
 
+// ActionScale (wrapper.py:L510-512) from [-1,1] onto the synthetic env's [-1,1] box, then the env's own clip
+__device__ __forceinline__ float env_action(float a) {
+    a = __fadd_rn(__fadd_rn(a, 1.f), -1.f);
+    return fminf(fmaxf(a, -1.f), 1.f);
+}
+// reward 1 - mean_j s'_j^2 from sumsq = sum_j s'_j^2 (in the spec's summation tree), and the cost [s'_0 > threshold]
+__device__ __forceinline__ float env_reward(float sumsq, int O) { return __fadd_rn(1.f, -__fdiv_rn(sumsq, (float)O)); }
+__device__ __forceinline__ float env_cost(const EnvSpec& es, float s0n) { return (s0n > es.cost_threshold) ? 1.f : 0.f; }
+
 // cost of this step (indicator on the next value of state dim 0) from the current raw state and the sampled action
 __device__ __forceinline__ float env_step_cost(const EnvSpec& es, float s0, float act0, float bias0) {
-    float a = __fadd_rn(__fadd_rn(act0, 1.f), -1.f);
-    a = fminf(fmaxf(a, -1.f), 1.f);
-    return (env_next_value(s0, a, bias0) > es.cost_threshold) ? 1.f : 0.f;
+    return env_cost(es, env_next_value(s0, env_action(act0), bias0));
 }
 
 // SauteAdapter.step (saute_adapter.py:L172-217) for one env: z <- (z - cost / budget) / gamma, reward override once
@@ -428,8 +459,8 @@ __device__ __forceinline__ void synthetic_step_end(const StepArgs& p, int N, int
                                                    float sumsq, float s0n, const int& ep_step, const uint32_t& epi,
                                                    const uint32_t& gstep, const float& acc_cost) {
     const bool fin = fl & EP_FIN, early = fl & EP_EARLY;
-    const float rew = early ? 0.f : __fadd_rn(1.f, -__fdiv_rn(sumsq, (float)O));
-    const float cst = (s0n > p.es.cost_threshold) ? 1.f : 0.f;
+    const float rew = early ? 0.f : env_reward(sumsq, O);
+    const float cst = env_cost(p.es, s0n);
     record_step(p.sl, p.st, T, N, t, env, saute_step(p.sa, t, N, env, rew, cst, fin), rew, cst, fl & EP_TERM,
                 fl & EP_TRUNC);
     if (p.et.cost_acc) p.et.cost_acc[env] = early ? 0.f : acc_cost;
@@ -442,11 +473,204 @@ __device__ __forceinline__ void synthetic_step_end(const StepArgs& p, int N, int
     p.st.gstep[env] = gstep + 1u;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Evaluation of a saved policy (EVAL instantiations of the step kernels), after the actor forward of a tile of R envs;
+// sMu[e * ld + a] holds the mean of env env0 + e.
+//
+// eval_action: the deterministic action in place (sample_action with eps = 0: the bits osb_policy_step gives without
+// eps), into act_out for running envs and, EXT, scaled onto [act_lo, act_hi] into act_env for env.step.
+template <int R, bool EXT>
+__device__ void eval_action(const StepArgs& p, int env0, float* sMu, int ld, const float* log_std) {
+    const int A = p.es.A, N = p.N;
+    for (int i = threadIdx.x; i < R * A; i += NTHREADS) {
+        const int e = i / A, a = i % A, env = env0 + e;
+        const float sd = expf(__ldg(log_std + a));
+        float term;
+        const float act = sample_action(sMu[e * ld + a], sd, __fmul_rn(2.f, __fmul_rn(sd, sd)), logf(sd), 0.f, term);
+        sMu[e * ld + a] = act;
+        if (env < N) {
+            if (p.ev.act_out && __ldcg(p.ev.left + env) > 0) p.ev.act_out[(size_t)env * A + a] = act;
+            if constexpr (EXT) p.act_env[(size_t)env * A + a] = action_scale(act, __ldg(p.act_lo + a), __ldg(p.act_hi + a));
+        }
+    }
+}
+
+// The synthetic env's evaluation step t of the tile.  Per running env (one thread each): ActionScale, the transition
+// into final_raw (scratch of this step), reward / cost, the fp64 episode sums, the Saute state, the EarlyTerminated rule
+// and the episode end.  Then the normaliser sums of the rows the reference pushes in this step, in its order: the final
+// observations of envs that ended, the next observations of every running env (an env that ended hands back its
+// auto-reset observation), and the observations of the envs reset after the step.  sF / sE1 / sE2: R ints of shared
+// scratch each.  eval_finalize (one CTA, after every CTA's step) folds the sums into the statistics.
+template <int R>
+__device__ void eval_step(const StepArgs& p, int t, int env0, float* sMu, int ld, const float* log_std, int* sF,
+                          uint32_t* sE1, uint32_t* sE2) {
+    const EvalSpec& ev = p.ev;
+    const int O = p.es.O, A = p.es.A, N = p.N, tid = threadIdx.x;
+    eval_action<R, false>(p, env0, sMu, ld, log_std);
+    __syncthreads();
+    const float* s_cur = p.st.s_raw + (size_t)(t & 1) * N * O;
+    float* s_nxt = p.st.s_raw + (size_t)((t + 1) & 1) * N * O;
+    float* sn_all = p.st.final_raw + (size_t)(t & 1) * N * O;
+    if (tid < R) {
+        const int env = env0 + tid;
+        int f = 0;
+        if (env < N && ev.left[env] > 0) {
+            const uint32_t gid = p.es.env_id_offset + env;
+            const int ep_step = p.st.ep_step[env];
+            const uint32_t epi = p.st.episode[env], gstep = p.st.gstep[env];
+            const bool envfin = episode_end(p.es, gid, ep_step, gstep) & EP_FIN;
+            const float* s = s_cur + (size_t)env * O;
+            float* sn = sn_all + (size_t)env * O;
+            // p_q = sum of s'_j^2 over j = q (mod 8), ascending; combined in the spec's tree
+            float part[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+            for (int j = 0; j < O; ++j) {
+                const float v = env_next_value(s[j], env_action(sMu[tid * ld + (j % A)]), __ldg(p.st.bias + j));
+                part[j & 7] = __fadd_rn(part[j & 7], __fmul_rn(v, v));
+                sn[j] = v;
+            }
+            const float tot = __fadd_rn(__fadd_rn(__fadd_rn(part[0], part[1]), __fadd_rn(part[2], part[3])),
+                                        __fadd_rn(__fadd_rn(part[4], part[5]), __fadd_rn(part[6], part[7])));
+            const float rew = env_reward(tot, O);
+            const float cst = env_cost(p.es, sn[0]);
+            const int len = ev.len[env];
+            const double r64 = ev.ret[env] + (double)rew;
+            const double c64 = ev.cost[env] + pow(ev.crit, (double)len) * (double)cst;
+            const bool done = envfin || (ev.early && c64 >= ev.cost_limit);
+            saute_step(p.sa, t, N, env, rew, cst, done);      // z returns to 1 when the episode ends
+            const int left = ev.left[env];
+            const bool rst = done && left > 1 && (ev.explicit_reset || !envfin);
+            uint32_t epi_n = envfin ? epi + 1u : epi;      // the env's own reset on its episode end
+            const uint32_t epi_auto = epi_n;
+            if (rst) ++epi_n;
+            p.st.episode[env] = epi_n;
+            p.st.ep_step[env] = (envfin || rst) ? 0 : ep_step + 1;
+            p.st.gstep[env] = gstep + 1u;
+            if (done) {
+                const int k = ev.done_eps[env];
+                const size_t out = (size_t)env + (size_t)k * N;
+                ev.out_ret[out] = r64; ev.out_cost[out] = c64; ev.out_len[out] = len + 1;
+                ev.done_eps[env] = k + 1;
+                ev.left[env] = left - 1;
+                ev.ret[env] = 0.0; ev.cost[env] = 0.0; ev.len[env] = 0;
+            } else {
+                ev.ret[env] = r64; ev.cost[env] = c64; ev.len[env] = len + 1;
+            }
+            for (int j = 0; j < O; ++j)
+                s_nxt[(size_t)env * O + j] = rst ? env_reset_value(p.es, gid, epi_n, j)
+                                                 : envfin ? env_reset_value(p.es, gid, epi_auto, j) : sn[j];
+            f = 1 | (envfin ? 2 : 0) | (rst ? 4 : 0) | ((!done || left > 1) ? 8 : 0);
+            sE1[tid] = epi_auto; sE2[tid] = epi_n;
+        }
+        sF[tid] = f;
+    }
+    __syncthreads();
+    if (p.es.obs_normalize) {
+        for (int j = tid; j < O; j += NTHREADS) {
+            long long sx = 0, sxx = 0, fx = 0, fxx = 0, rx = 0, rxx = 0;
+            for (int r = 0; r < R; ++r) {
+                const int f = sF[r];
+                if (!(f & 1)) continue;
+                const uint32_t gid = p.es.env_id_offset + env0 + r;
+                const float w = sn_all[(size_t)(env0 + r) * O + j];
+                const float v = (f & 2) ? env_reset_value(p.es, gid, sE1[r], j) : w;
+                sx += to_fix(v); sxx += to_fix(__fmul_rn(v, v));
+                if (f & 2) { fx += to_fix(w); fxx += to_fix(__fmul_rn(w, w)); }
+                if (f & 4) {
+                    const float u = env_reset_value(p.es, gid, sE2[r], j);
+                    rx += to_fix(u); rxx += to_fix(__fmul_rn(u, u));
+                }
+            }
+            push_fix_sums(p.ns, O, j, sx, sxx, fx, fxx);
+            if (rx != 0 || rxx != 0) {
+                atomicAdd((unsigned long long*)(ev.acc_rst + j), (unsigned long long)rx);
+                atomicAdd((unsigned long long*)(ev.acc_rst + O + j), (unsigned long long)rxx);
+            }
+        }
+    }
+    if (tid == 0) {
+        int nfin = 0, nrst = 0, nnext = 0;
+        for (int r = 0; r < R; ++r) {
+            nfin += (sF[r] >> 1) & 1; nrst += (sF[r] >> 2) & 1; nnext += (sF[r] >> 3) & 1;
+        }
+        if (nfin) atomicAdd(p.ns.fin_count, nfin);
+        if (nrst) atomicAdd(ev.ctr + 2, nrst);
+        if (nnext) atomicAdd(ev.ctr + 1, nnext);
+    }
+}
+
+// One CTA, after every CTA's eval_step of the step: pushes the step's rows into the statistics (final rows, next rows,
+// reset rows: three pushes, as Normalizer.normalize is called three times) and advances the done word.
+__device__ void eval_finalize(const StepArgs& p) {
+    const EvalSpec& ev = p.ev;
+    const int O = p.es.O, tid = threadIdx.x;
+    __threadfence();
+    const int nfin = *((volatile int*)p.ns.fin_count), nall = *((volatile int*)ev.ctr),
+              nrst = *((volatile int*)(ev.ctr + 2));
+    const long long count = __ldcg(p.ns.count);
+    if (p.es.obs_normalize) {
+        for (int j = tid; j < O; j += NTHREADS) {
+            float mean = __ldcg(p.ns.mean + j), sumsq = __ldcg(p.ns.sumsq + j);
+            long long c = count;
+            if (nfin > 0) {
+                norm_push(mean, sumsq, c, nfin, __ldcg(p.ns.acc_fin + j), __ldcg(p.ns.acc_fin + O + j));
+                c += nfin;
+            }
+            norm_push(mean, sumsq, c, nall, __ldcg(p.ns.acc_all + j), __ldcg(p.ns.acc_all + O + j));
+            c += nall;
+            if (nrst > 0) {
+                norm_push(mean, sumsq, c, nrst, __ldcg(ev.acc_rst + j), __ldcg(ev.acc_rst + O + j));
+                c += nrst;
+            }
+            p.ns.mean[j] = mean;
+            p.ns.sumsq[j] = sumsq;
+            p.ns.std[j] = norm_std(sumsq, c);
+            p.ns.acc_all[j] = 0; p.ns.acc_all[O + j] = 0;
+            p.ns.acc_fin[j] = 0; p.ns.acc_fin[O + j] = 0;
+            ev.acc_rst[j] = 0; ev.acc_rst[O + j] = 0;
+        }
+    }
+    __syncthreads();
+    if (tid == 0) {
+        p.ns.count[0] = count + nfin + nall + nrst;
+        *p.ns.fin_count = 0;
+        ev.ctr[0] = __ldcg(ev.ctr + 1);
+        ev.ctr[1] = 0;
+        ev.ctr[2] = 0;
+        *p.ns.ticket = 0u;
+    }
+}
+
+// Software grid barrier at the end of step t of a persistent (cooperative) launch: every CTA arrives, the last one runs
+// on_last() (the step's fold into the running state) before it releases the others.  bar_ctr / bar_flag are zero at launch.
+template <class F>
+__device__ __forceinline__ void grid_step_barrier(const StepArgs& p, int t, int& s_last, F on_last) {
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) s_last = (atomicAdd(p.bar_ctr, 1u) == gridDim.x * gridDim.y * (unsigned)(t + 1) - 1u) ? 1 : 0;
+    __syncthreads();
+    if (s_last) {
+        on_last();
+        __threadfence();
+        __syncthreads();
+        if (threadIdx.x == 0) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p.bar_flag), "r"((unsigned)(t + 1)) : "memory");
+    } else if (threadIdx.x == 0) {
+        unsigned v;
+        do { asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p.bar_flag) : "memory"); } while (v < (unsigned)(t + 1));
+    }
+    __syncthreads();
+}
+
 // EXT = true: the act half of a step on a user env (csrc: osb_ext_act).  The network part is the same; the actor CTAs
 // hand the scaled action to the env through p.act_env instead of running the synthetic transition, and the normaliser is
 // fed by the observe kernel after env.step.
-template <bool EXT>
+// EVAL = true: a step of the evaluation of a saved policy (actor CTAs only, no slabs): eval_step on the synthetic env;
+// EXT, the deterministic action into act_env for env.step (the observe half is ext_eval_observe_kernel).  A launch after
+// every env has finished its episodes returns at once.
+template <bool EXT, bool EVAL = false>
 __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
+    if constexpr (EVAL) {
+        if (__ldcg(p.ev.ctr) == 0) return;
+    }
     extern __shared__ __align__(16) float smem[];
     NetSmem W;
     float* base = carve_net_smem<false>(smem, W);
@@ -485,7 +709,7 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
     };
 
     // ---- bootstrap values of paths that ended in the previous step (critic CTAs only) --------
-    if (net != 0 && t > 0) {
+    if (!EVAL && net != 0 && t > 0) {
         if (threadIdx.x == 0) s_anyfin = 0;
         __syncthreads();
         if (threadIdx.x < RT && env0 + threadIdx.x < N && cut_path(p.sl.flags[(size_t)(t - 1) * N + env0 + threadIdx.x]))
@@ -515,7 +739,7 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
     // ---- forward on the current observation ------------------------------------------------
     for (int j = threadIdx.x; j < O; j += NTHREADS) { sMean[j] = p.ns.mean[j]; sStd[j] = p.ns.std[j]; }
     __syncthreads();
-    if (net == 0 && nchunks > 1) {
+    if (!EVAL && net == 0 && nchunks > 1) {
         // write the whole normalised observation row once (chunks > 0 are not revisited below)
         for (int kc = 1; kc < nchunks; ++kc)
             load_obs_tile(s_cur, env0, N, O, kc, sMean, sStd, normalize, sX,
@@ -523,10 +747,21 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
         __syncthreads();
     }
     load_obs_tile(s_cur, env0, N, O, 0, sMean, sStd, normalize, sX,
-                  (net == 0) ? p.sl.obs + (size_t)t * N * On : nullptr, z_cur);
+                  (!EVAL && net == 0) ? p.sl.obs + (size_t)t * N * On : nullptr, z_cur);
     __syncthreads();
     mlp_hidden<RT>(sX, sH1, sH2, W, nchunks, load_chunk_cur);
     mlp_out<RT>(sH2, sO, W, L.out);
+    if constexpr (EVAL) {
+        __syncthreads();
+        if constexpr (EXT) {
+            eval_action<RT, true>(p, env0, sO, LDO, theta + L.off_logstd);
+        } else {
+            eval_step<RT>(p, t, env0, sO, LDO, theta + L.off_logstd, sFlag, reinterpret_cast<uint32_t*>(sNew),
+                          reinterpret_cast<uint32_t*>(sFin));
+            if (last_cta(p.ns.ticket)) eval_finalize(p);
+        }
+        return;
+    }
 
     if (net != 0 && threadIdx.x < RT && env0 + threadIdx.x < N)
         store_critic(p.sl, net, N, t, env0 + threadIdx.x, false, p.is_tail, sO[threadIdx.x * LDO]);
@@ -584,10 +819,7 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
             for (int j = c0 + q; j < min(O, c0 + KC); j += 8) {
                 float nv = 0.f, fv = 0.f;
                 if (ok) {
-                    // ActionScale (wrapper.py:L510-512) from [-1,1] onto the env's [-1,1] box
-                    float a = sAct[e * OUTP + (j % A)];
-                    a = __fadd_rn(__fadd_rn(a, 1.f), -1.f);
-                    a = fminf(fmaxf(a, -1.f), 1.f);
+                    const float a = env_action(sAct[e * OUTP + (j % A)]);
                     const float s = s_cur[(size_t)env * O + j];
                     const float sn = env_next_value(s, a, __ldg(p.st.bias + j));
                     part = __fadd_rn(part, __fmul_rn(sn, sn));
@@ -670,9 +902,16 @@ static_assert(TF_ACC % 2 == 0, "the fixed-point sums need 8-byte alignment");
 // (raw states, flags, normaliser statistics) is read with ld.global.cg.
 // EXT = true: the act half of a step on a user env, as in rollout_step_kernel<true> (never persistent: Python runs
 // env.step between the launches).
-template <bool X3, bool PERSIST, bool EXT = false>
+// EVAL = true: the evaluation of a saved policy, as in rollout_step_kernel<EXT, true>; PERSIST (synthetic env only): ONE
+// cooperative launch runs every step until all envs have finished, the last CTA at each step's grid barrier running
+// eval_finalize.
+template <bool X3, bool PERSIST, bool EXT = false, bool EVAL = false>
 __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p) {
     static_assert(!(EXT && PERSIST), "the external-env act step is one launch per step");
+    static_assert(!(EXT && PERSIST), "the external-env steps are one launch per step");
+    if constexpr (EVAL) {
+        if (__ldcg(p.ev.ctr) == 0) return;
+    }
     using namespace umma;
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
@@ -728,6 +967,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
     for (int t = t_first; t <= t_last; ++t) {
     const bool is_tail = t == T;
     if (PERSIST && is_tail && net == 0) break;          // the tail step is the critics' (no barrier follows it)
+    if (EVAL && PERSIST && t > 0 && __ldcg(p.ev.ctr) == 0) break;   // every env has finished (uniform after the barrier)
     const float* eps_t = PERSIST ? (p.eps ? p.eps + (size_t)t * N * A : nullptr) : p.eps;
     const uint32_t gstep_t = PERSIST ? p.global_step + (uint32_t)t : p.global_step;
     const bool normalize = p.es.obs_normalize && __ldcg(p.ns.count) > 1;
@@ -735,7 +975,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
     float* s_nxt = p.st.s_raw + (size_t)((t + 1) & 1) * N * O;
     if (PERSIST) { if (tid == 0) s_anyfin = 0; __syncthreads(); }
     // which envs of this tile finish in this step (time limit / hash-driven termination): known before the forward
-    if (!EXT && net == 0 && tid < RTC) {
+    if (!EXT && !EVAL && net == 0 && tid < RTC) {
         const int env = env0 + tid;
         int fl = 0, ep_step = 0; uint32_t epi = 0, gstep = 0;
         if (env < N) {
@@ -759,8 +999,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
         const float* gmean = pass ? p.ns.mean : p.ns.mean1;
         const float* gstd = pass ? p.ns.std : p.ns.std1;
         const bool norm_on = pass ? normalize : (p.es.obs_normalize && __ldcg(p.ns.count + 1) > 1);
-        float* obs_out = (pass && net == 0) ? p.sl.obs + (size_t)t * N * On : nullptr;
-        const bool own_state = PERSIST && pass && net == 0 && t > t_first;
+        float* obs_out = (!EVAL && pass && net == 0) ? p.sl.obs + (size_t)t * N * On : nullptr;
+        const bool own_state = !EVAL && PERSIST && pass && net == 0 && t > t_first;
         if (tid < 64) { sMean[tid] = (tid < O) ? __ldcg(gmean + tid) : 0.f; sStd[tid] = (tid < O) ? __ldcg(gstd + tid) : 1.f; }
         __syncthreads();
         if ((O & 3) == 0 && On == O) {   // 128-bit row loads, all 8 in flight per thread
@@ -858,6 +1098,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
         }
         __syncthreads();
     }
+    if constexpr (EVAL) {
+        if constexpr (EXT) {
+            eval_action<RTC, true>(p, env0, sAct, OUTP, theta + L.off_logstd);
+            return;
+        } else {
+            eval_step<RTC>(p, t, env0, sAct, OUTP, theta + L.off_logstd, sFlag, sEpi, reinterpret_cast<uint32_t*>(sStep));
+            if constexpr (PERSIST) {
+                grid_step_barrier(p, t, s_last, [&] { eval_finalize(p); });
+                continue;
+            } else {
+                if (last_cta(p.ns.ticket)) eval_finalize(p);
+                return;
+            }
+        }
+    }
 
     RSTAMP(6);
     if (net == 0) {
@@ -942,10 +1197,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                 for (int e = 32 * g; e < 32 * g + 32; ++e) {
                     const int env = env0 + e;
                     if (env < N) {
-                        // ActionScale (wrapper.py:L510-512) from [-1,1] onto the env's [-1,1] box
-                        float a = sAct[e * OUTP + ja];
-                        a = __fadd_rn(__fadd_rn(a, 1.f), -1.f);
-                        a = fminf(fmaxf(a, -1.f), 1.f);
+                        const float a = env_action(sAct[e * OUTP + ja]);
                         const float sn = env_next_value(sRaw[e * SNW + j], a, bj);
                         const int fl = sFlag[e];
                         float nv = sn;
@@ -1179,6 +1431,141 @@ __global__ void __launch_bounds__(NTHREADS) ext_observe_kernel(ExtObs x, EnvStat
         ns.count[1] = count + nfin;
         ns.count[0] = count + nfin + N;
         *ns.had_fin = nfin > 0 ? 1 : 0;
+        *ns.ticket = 0u;
+    }
+}
+
+// Evaluation of a saved policy on a user env (Evaluator.evaluate with a registered env), the observe half of step t after
+// env.step; is_reset: the ingest of env.reset()'s observations (before step t + 1; t = -1 for the first reset).  Per env
+// still running (left > 0), one thread each: the fp64 episode sums, the EarlyTerminated rule, the Saute state, the
+// episode end and the results, as eval_step does for the synthetic env.  The next observations go to the state buffer
+// step t + 1 reads.  ObsNormalize pushes the final observations of the running envs that report one, then the next
+// observations of every running env (reset: the observations of every env with episodes left), as fp64 per-tile
+// moments combined in tile order by the last CTA (ext_observe_kernel's scheme), with per-tile row counts.  The last CTA
+// also advances the done word ctr[0]; ctr[2] counts the envs to reset now (N == 1: every episode end with episodes left),
+// and a reset ingest clears it.
+__global__ void __launch_bounds__(NTHREADS) ext_eval_observe_kernel(ExtObs x, EnvState st, NormState ns, SauteSpec sa,
+                                                                    EvalSpec ev, int O, int N, int t, int obs_normalize,
+                                                                    int is_reset) {
+    __shared__ int sRun[XT], sFin[XT];
+    __shared__ int s_bad, s_nrun, s_nfin;
+    const int tid = threadIdx.x, tile = blockIdx.x, ntiles = gridDim.x;
+    const int env0 = tile * XT, rows = min(XT, N - env0);
+    if (tid == 0) s_bad = 0;
+    if (tid < XT) {
+        const int env = env0 + tid;
+        int run = 0, fin = 0, nxt = 0, rst = 0;
+        if (tid < rows && ev.left[env] > 0) {
+            run = 1;
+            if (!is_reset) {
+                fin = (x.final_obs && x.final_mask && x.final_mask[env]) ? 1 : 0;
+                const float rew = x.rew[env], cst = x.cost[env];
+                const int len = ev.len[env];
+                const double r64 = ev.ret[env] + (double)rew;
+                const double c64 = ev.cost[env] + pow(ev.crit, (double)len) * (double)cst;
+                const bool done = x.term[env] != 0 || x.trunc[env] != 0 || (ev.early && c64 >= ev.cost_limit);
+                if (sa.safety) saute_step(sa, t, N, env, rew, cst, done);
+                const int left = ev.left[env];
+                if (done) {
+                    const int k = ev.done_eps[env];
+                    const size_t out = (size_t)env + (size_t)k * N;
+                    ev.out_ret[out] = r64; ev.out_cost[out] = c64; ev.out_len[out] = len + 1;
+                    ev.done_eps[env] = k + 1;
+                    ev.left[env] = left - 1;
+                    ev.ret[env] = 0.0; ev.cost[env] = 0.0; ev.len[env] = 0;
+                } else {
+                    ev.ret[env] = r64; ev.cost[env] = c64; ev.len[env] = len + 1;
+                }
+                nxt = (!done || left > 1) ? 1 : 0;
+                rst = (done && left > 1 && ev.explicit_reset) ? 1 : 0;
+            }
+        }
+        sRun[tid] = run; sFin[tid] = fin;
+        if (!is_reset) {
+            if (nxt) atomicAdd(ev.ctr + 1, 1);
+            if (rst) atomicAdd(ev.ctr + 2, 1);
+        }
+    }
+    __syncthreads();
+    float* s_nxt = st.s_raw + (size_t)((t + 1) & 1) * N * O;
+    bool bad = false;
+    for (int i = tid; i < rows * O; i += NTHREADS) {
+        const size_t g = (size_t)env0 * O + i;
+        const float v = x.next_obs[g];
+        bad |= sRun[i / O] && !isfinite(v);
+        s_nxt[g] = v;
+        if (sFin[i / O]) bad |= !isfinite(x.final_obs[g]);
+    }
+    if (bad) s_bad = 1;
+    int nr = 0, nf = 0;
+    for (int r = 0; r < rows; ++r) { nr += sRun[r]; nf += sFin[r]; }
+    double* P = x.part + (size_t)tile * 4 * O;
+    if (obs_normalize) {
+        for (int j = tid; j < O; j += NTHREADS) {
+            double sm = 0.0, sf = 0.0;
+            for (int r = 0; r < rows; ++r) {
+                const size_t g = (size_t)(env0 + r) * O + j;
+                if (sRun[r]) sm += (double)x.next_obs[g];
+                if (sFin[r]) sf += (double)x.final_obs[g];
+            }
+            const double m = nr ? sm / nr : 0.0, mf = nf ? sf / nf : 0.0;
+            double q = 0.0, qf = 0.0;
+            for (int r = 0; r < rows; ++r) {
+                const size_t g = (size_t)(env0 + r) * O + j;
+                if (sRun[r]) { const double d = (double)x.next_obs[g] - m; q += d * d; }
+                if (sFin[r]) { const double df = (double)x.final_obs[g] - mf; qf += df * df; }
+            }
+            P[j] = m; P[O + j] = q; P[2 * O + j] = mf; P[3 * O + j] = qf;
+        }
+    }
+    double* cnt = x.part + (size_t)ntiles * 4 * O;
+    if (tid == 0) { cnt[2 * tile] = (double)nr; cnt[2 * tile + 1] = (double)nf; }
+    const bool last = last_cta(ns.ticket);
+    if (tid == 0 && s_bad) *x.nonfinite = 1;
+    if (!last) return;
+
+    // last CTA: combine the tiles in order, push the final rows, then the running rows
+    __threadfence();
+    if (tid == 0) {
+        int a = 0, b = 0;
+        for (int k = 0; k < ntiles; ++k) { a += (int)__ldcg(cnt + 2 * k); b += (int)__ldcg(cnt + 2 * k + 1); }
+        s_nrun = a; s_nfin = b;
+    }
+    __syncthreads();
+    const int nrun = s_nrun, nfin = s_nfin;
+    const long long count = __ldcg(ns.count);
+    if (obs_normalize) {
+        for (int j = tid; j < O; j += NTHREADS) {
+            double n = 0.0, m = 0.0, q = 0.0, nF = 0.0, mF = 0.0, qF = 0.0;
+            for (int k = 0; k < ntiles; ++k) {
+                const double* Pk = x.part + (size_t)k * 4 * O;
+                chan_combine(n, m, q, __ldcg(cnt + 2 * k), __ldcg(Pk + j), __ldcg(Pk + O + j));
+                chan_combine(nF, mF, qF, __ldcg(cnt + 2 * k + 1), __ldcg(Pk + 2 * O + j), __ldcg(Pk + 3 * O + j));
+            }
+            float mean = __ldcg(ns.mean + j), sumsq = __ldcg(ns.sumsq + j);
+            long long c = count;
+            if (nfin > 0) {
+                norm_push_moments(mean, sumsq, c, nfin, mF, qF);
+                c += nfin;
+            }
+            if (nrun > 0) {
+                norm_push_moments(mean, sumsq, c, nrun, m, q);
+                c += nrun;
+            }
+            ns.mean[j] = mean;
+            ns.sumsq[j] = sumsq;
+            ns.std[j] = norm_std(sumsq, c);
+        }
+    }
+    __syncthreads();
+    if (tid == 0) {
+        ns.count[0] = count + nfin + nrun;
+        if (is_reset) {
+            ev.ctr[2] = 0;
+        } else {
+            ev.ctr[0] = __ldcg(ev.ctr + 1);
+            ev.ctr[1] = 0;
+        }
         *ns.ticket = 0u;
     }
 }
@@ -1515,6 +1902,169 @@ int osb_episode_window(const unsigned char* flags, const float* epfin, int T, in
     episode_window_kernel<<<1, 1024, 0, s>>>(flags, epfin, T, N, W, ring, meta);
     OSB_LAUNCH_CHECK();
     window_sums_kernel<<<1, 32, 0, s>>>(ring, meta, W, window_sums);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}
+
+}  // extern "C"
+
+// Evaluation launches: the tensor-core tiles for tf32 / bf16x3 with a network input of <= 64 columns (the rollout's
+// rule), else the fp32 tiles; grid = env tiles x the actor.  persistent (synthetic env, tensor-core tiles, every CTA
+// resident): ONE cooperative launch runs all steps (p.T = their bound); otherwise one launch is one step.
+static StepArgs ext_step_args(int O, int A, int obs_normalize, int N, int precision);
+
+template <bool EXT>
+static int launch_eval(StepArgs& p, cudaStream_t stream, bool persistent) {
+    const int On = p.es.O + (p.sa.safety ? 1 : 0);
+    if ((p.precision == 1 || p.precision == 2) && On <= 64) {
+        const bool x3 = p.precision == 2;
+        static bool attr_tc = false;
+        if (!attr_tc) {
+            const void* kernels[] = {(const void*)rollout_step_tc_kernel<false, false, EXT, true>,
+                                     (const void*)rollout_step_tc_kernel<true, false, EXT, true>,
+                                     (const void*)rollout_step_tc_kernel<false, true, false, true>,
+                                     (const void*)rollout_step_tc_kernel<true, true, false, true>};
+            for (int i = 0; i < (EXT ? 2 : 4); ++i)
+                OSB_CUDA(cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (int)rollout_tc_smem_bytes(i & 1)));
+            attr_tc = true;
+        }
+        p.acc = acc_scratch(ACC_ROLLOUT, rollout_tc_acc_bytes(p.N));
+        if (!p.acc) return OSB_ERR_CUDA;
+        const dim3 grid((p.N + RTC - 1) / RTC, 1);
+        const size_t smem = rollout_tc_smem_bytes(x3);
+        if constexpr (!EXT) {
+            if (persistent) {
+                OSB_CUDA(cudaMemsetAsync(p.bar_ctr, 0, 2 * sizeof(unsigned int), stream));
+                void* args[] = {&p};
+                osb_count_launch();
+                OSB_CUDA(cudaLaunchCooperativeKernel(x3 ? (void*)rollout_step_tc_kernel<true, true, false, true>
+                                                        : (void*)rollout_step_tc_kernel<false, true, false, true>,
+                                                     grid, dim3(NTHREADS), args, smem, stream));
+                return OSB_OK;
+            }
+        }
+        if (x3) rollout_step_tc_kernel<true, false, EXT, true><<<grid, NTHREADS, smem, stream>>>(p);
+        else rollout_step_tc_kernel<false, false, EXT, true><<<grid, NTHREADS, smem, stream>>>(p);
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    }
+    const size_t smem = rollout_smem_bytes(On);
+    static size_t attr = 0;
+    if (smem > attr) {
+        OSB_CUDA(cudaFuncSetAttribute(rollout_step_kernel<EXT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attr = smem;
+    }
+    rollout_step_kernel<EXT, true><<<dim3((p.N + RT - 1) / RT, 1), NTHREADS, smem, stream>>>(p);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}
+
+static int sm_count() {
+    static int n_sm = 0;
+    if (!n_sm) { int dev = 0; OSB_CUDA(cudaGetDevice(&dev)); OSB_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev)); }
+    return n_sm;
+}
+
+extern "C" {
+
+int osb_eval_synthetic(int O, int A, int max_episode_steps, unsigned seed, unsigned term_threshold, float cost_threshold,
+                       int obs_normalize, int N, int num_episodes, float* s_raw, float* final_raw, int* ep_step,
+                       unsigned* episode, unsigned* gstep, float* ep_ret, float* ep_cost, int* ep_len, const float* bias,
+                       float* norm_mean, float* norm_sumsq, float* norm_std, float* norm_mean1, float* norm_std1,
+                       long long* norm_count, long long* acc_all, long long* acc_fin, int* fin_count, int* had_fin,
+                       unsigned* ticket, float* safety, float safety_budget, float saute_gamma, int early,
+                       double cost_limit, double cost_criteria, int* left, int* done_eps, double* ret, double* cost,
+                       int* len, long long* acc_rst, int* ctr, double* out_ret, double* out_cost, int* out_len,
+                       float* act_out, const float* theta, int precision, int per_step, void* stream) {
+    OSB_CHECK_ARG(O > 0 && A > 0 && A <= OUTP && N > 0 && num_episodes >= N && max_episode_steps > 0,
+                  "bad dims (need 0 < A <= 16, 0 < N <= num_episodes, max_episode_steps > 0)");
+    OSB_CHECK_ARG(precision >= 0 && precision <= 2, "precision must be 0, 1 or 2");
+    OSB_CHECK_ARG(safety == nullptr || (safety_budget > 0.f && saute_gamma > 0.f), "safety_budget and saute_gamma must be positive");
+    OSB_CHECK_ARG(left && done_eps && ret && cost && len && acc_rst && ctr && out_ret && out_cost && out_len && theta,
+                  "bad argument");
+    cudaStream_t s = (cudaStream_t)stream;
+    // every episode ends by its time limit, so no env runs more than this many steps
+    const long long steps = (long long)((num_episodes + N - 1) / N) * max_episode_steps;
+    OSB_CHECK_ARG(steps < (1ll << 30), "too many steps per env");
+    StepArgs p = synthetic_step_args(O, A, max_episode_steps, seed, term_threshold, 0u, cost_threshold, obs_normalize,
+                                     N, (int)steps, s_raw, final_raw, ep_step, episode, gstep, ep_ret, ep_cost, ep_len,
+                                     bias, norm_mean, norm_sumsq, norm_std, norm_mean1, norm_std1, norm_count, acc_all,
+                                     acc_fin, fin_count, had_fin, ticket, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                     nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, theta, 0u, precision);
+    // the safety state z starts every episode at 1, Saute and Simmer alike; the reward is never replaced
+    p.sa = SauteSpec{safety, safety ? safety_budget : 1.f, safety ? saute_gamma : 1.f, 0.f, 1.f};
+    p.et = EarlySpec{nullptr, 0.f};
+    p.ev = EvalSpec{left, done_eps, ret, cost, len, out_ret, out_cost, out_len, acc_rst, ctr, cost_criteria, cost_limit,
+                    early, N == 1 ? 1 : 0, act_out};
+    // every env's first episode starts from a reset, its observations pushed as one batch (a vector env's reset)
+    env_reset_kernel<<<(N + RT - 1) / RT, NTHREADS, 0, s>>>(p.es, p.st, p.ns, p.sa, N);
+    OSB_LAUNCH_CHECK();
+    const int On = O + (safety ? 1 : 0);
+    if (!per_step && (precision == 1 || precision == 2) && On <= 64 && (N + RTC - 1) / RTC <= sm_count()) {
+        static unsigned int* d_bar = nullptr;
+        if (!d_bar) OSB_CUDA(cudaMalloc(&d_bar, 64));
+        p.bar_ctr = d_bar; p.bar_flag = d_bar + 1;
+        p.t = 0;
+        return launch_eval<false>(p, s, true);
+    }
+    static int* h_done = nullptr;
+    if (!h_done) OSB_CUDA(cudaMallocHost(&h_done, sizeof(int)));
+    constexpr int CHECK_EVERY = 16;     // the done word is read after every 16 launches; later launches return at once
+    for (long long t = 0; t < steps; ++t) {
+        p.t = (int)(t & 1);     // the parity of the state buffers (T = the step bound keeps every launch a full step)
+        if (int rc = launch_eval<false>(p, s, false)) return rc;
+        if ((t + 1) % CHECK_EVERY == 0 && t + 1 < steps) {
+            OSB_CUDA(cudaMemcpyAsync(h_done, ctr, sizeof(int), cudaMemcpyDeviceToHost, s));
+            OSB_CUDA(cudaStreamSynchronize(s));
+            if (*h_done == 0) break;
+        }
+    }
+    return OSB_OK;
+}
+
+int osb_eval_ext_workspace_doubles(int O, int N) { return ((N + XT - 1) / XT) * (4 * O + 2); }
+
+int osb_eval_ext_act(int O, int A, int obs_normalize, int N, int t, const float* s_raw, const float* norm_mean,
+                     const float* norm_std, const long long* norm_count, const float* safety, const float* theta,
+                     const float* act_lo, const float* act_hi, float* act_env, const int* left, const int* ctr,
+                     float* act_out, int precision, void* stream) {
+    OSB_CHECK_ARG(O > 0 && A > 0 && A <= OUTP && N > 0 && t >= 0, "bad dims (need 0 < A <= 16) / step index");
+    OSB_CHECK_ARG(precision >= 0 && precision <= 2, "precision must be 0, 1 or 2");
+    OSB_CHECK_ARG(s_raw && norm_mean && norm_std && norm_count && theta && act_lo && act_hi && act_env && left && ctr,
+                  "bad argument");
+    StepArgs p = ext_step_args(O, A, obs_normalize, N, precision);
+    p.st.s_raw = const_cast<float*>(s_raw);
+    p.ns.mean = const_cast<float*>(norm_mean); p.ns.std = const_cast<float*>(norm_std);
+    p.ns.count = const_cast<long long*>(norm_count);
+    p.sa.safety = const_cast<float*>(safety);
+    p.theta = theta; p.t = t & 1; p.T = 2;
+    p.act_lo = act_lo; p.act_hi = act_hi; p.act_env = act_env;
+    p.ev.left = const_cast<int*>(left); p.ev.ctr = const_cast<int*>(ctr); p.ev.act_out = act_out;
+    return launch_eval<true>(p, (cudaStream_t)stream, false);
+}
+
+int osb_eval_ext_observe(int O, int N, int t, int obs_normalize, int is_reset, const float* next_obs, const float* rew,
+                         const float* cost, const unsigned char* terminated, const unsigned char* truncated,
+                         const float* final_obs, const unsigned char* final_mask, float* s_raw, float* norm_mean,
+                         float* norm_sumsq, float* norm_std, long long* norm_count, unsigned* ticket, float* safety,
+                         float safety_budget, float saute_gamma, int early, double cost_limit, double cost_criteria,
+                         int* left, int* done_eps, double* ret, double* cost_acc, int* len, int* ctr, double* out_ret,
+                         double* out_cost, int* out_len, double* workspace, int* nonfinite, void* stream) {
+    OSB_CHECK_ARG(O > 0 && N > 0 && t >= -1, "bad dims / step index");
+    OSB_CHECK_ARG(next_obs && s_raw && norm_mean && norm_sumsq && norm_std && norm_count && ticket && left && ctr &&
+                  workspace && nonfinite, "bad argument");
+    OSB_CHECK_ARG(is_reset || (rew && cost && terminated && truncated && done_eps && ret && cost_acc && len && out_ret &&
+                               out_cost && out_len), "bad argument");
+    OSB_CHECK_ARG(safety == nullptr || (safety_budget > 0.f && saute_gamma > 0.f), "safety_budget and saute_gamma must be positive");
+    ExtObs x{next_obs, rew, cost, terminated, truncated, final_obs, final_mask, workspace, nonfinite};
+    EnvState st{s_raw, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    NormState ns{norm_mean, norm_sumsq, norm_std, nullptr, nullptr, norm_count, nullptr, nullptr, nullptr, nullptr, ticket};
+    SauteSpec sa{safety, safety ? safety_budget : 1.f, safety ? saute_gamma : 1.f, 0.f, 1.f};
+    EvalSpec ev{left, done_eps, ret, cost_acc, len, out_ret, out_cost, out_len, nullptr, ctr, cost_criteria, cost_limit,
+                early, N == 1 ? 1 : 0, nullptr};
+    ext_eval_observe_kernel<<<(N + XT - 1) / XT, NTHREADS, 0, (cudaStream_t)stream>>>(x, st, ns, sa, ev, O, N, t,
+                                                                                     obs_normalize, is_reset);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
 }
