@@ -217,6 +217,28 @@ int osb_ext_observe(int O, int N, int T, int t, int obs_normalize, const float* 
                     float* norm_mean1, float* norm_std1, long long* norm_count, int* had_fin, unsigned* ticket,
                     float* rew_slab, float* cost_slab, unsigned char* flags, float* epfin, double* workspace,
                     int* nonfinite, void* stream);
+/* EarlyTerminated on an external env (early_terminated_adapter.py:L77-87, per env).  osb_ext_observe_early =
+ * osb_ext_observe plus the cost-limit rule: cost_acc[N] (device floats, carried across episodes and epochs) += the
+ * env's cost; where it exceeds cost_limit the step stores reward 0 (slab and episode return), terminated = 1 and the
+ * env's truncated, the accumulator is cleared and trig[N] (one byte per env, written every step) is 1.  An ordinary
+ * episode end does not clear the accumulator.  trig_total (device int, or NULL) is zeroed on the stream and receives the
+ * number of triggered envs.  The observation rows and their ObsNormalize pushes are those of osb_ext_observe.
+ * The caller then resets the triggered envs and hands their observations to osb_ext_reset_rows (same t): rows of
+ * obs[N][O] with mask set go to the state buffer step t + 1 reads and are pushed into the observation statistics after
+ * the step's pushes (one batch, device-side row count; no masked row leaves the statistics untouched).  mean1 / std1 /
+ * had_fin are not changed.  workspace: osb_ext_workspace_doubles(O, N) doubles, as for osb_ext_observe.  Both calls
+ * are capturable into a CUDA graph. */
+int osb_ext_observe_early(int O, int N, int T, int t, int obs_normalize, const float* next_obs, const float* rew,
+                          const float* cost, const unsigned char* terminated, const unsigned char* truncated,
+                          const float* final_obs, const unsigned char* final_mask, float* s_raw, float* final_raw,
+                          float* ep_ret, float* ep_cost, int* ep_len, float* norm_mean, float* norm_sumsq,
+                          float* norm_std, float* norm_mean1, float* norm_std1, long long* norm_count, int* had_fin,
+                          unsigned* ticket, float* rew_slab, float* cost_slab, unsigned char* flags, float* epfin,
+                          double* workspace, int* nonfinite, float* cost_acc, float cost_limit, unsigned char* trig,
+                          int* trig_total, void* stream);
+int osb_ext_reset_rows(int O, int N, int t, int obs_normalize, const unsigned char* mask, const float* obs, float* s_raw,
+                       float* norm_mean, float* norm_sumsq, float* norm_std, long long* norm_count, unsigned* ticket,
+                       double* workspace, int* nonfinite, void* stream);
 /* CUDA-graph capture of the external-env epoch (for envs whose step is itself capturable).
  * osb_ext_prepare performs every one-time host action of osb_ext_act / osb_ext_act_graph for these dimensions
  * (kernel attributes, the tensor-core accumulator image at its final size); call it before capturing.  An act launch on

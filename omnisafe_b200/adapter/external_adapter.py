@@ -139,8 +139,7 @@ class ExternalEnvAdapter:
 
     def _steps(self, T: int, agent, d, eps, s: int, env_dev, epoch_dev=None, capture: bool = False) -> None:
         """Steps 0 .. T-1 (act, env.step, observe) and the epoch-end act, eagerly or into the graph being captured."""
-        L, N, O = lib(), self._num_envs, self._obs_dim
-        on = int(self._obs_normalize)
+        N, O = self._num_envs, self._obs_dim
         for t in range(T):
             self._act(agent, d, T, t, None if eps is None else eps[t], s, epoch_dev)
             # a fresh tensor every step, as the reference hands the env: the buffer is rewritten by the next act step
@@ -159,11 +158,19 @@ class ExternalEnvAdapter:
                 final = self._rows(info['final_observation'], O)
                 mask = info.get('_final_observation')
                 mask = (term | trunc) if mask is None else self._rows(mask, dtype=torch.uint8)
-            L.osb_ext_observe(O, N, T, t, on, ptr(nobs), ptr(rew), ptr(cost), ptr(term), ptr(trunc), ptr(final),
-                              ptr(mask), ptr(self.s_raw), ptr(self.final_raw), ptr(self.ep_ret), ptr(self.ep_cost),
-                              ptr(self.ep_len), *self._norm_ptrs(), ptr(d['reward']), ptr(d['cost']),
-                              ptr(d['flags']), ptr(d['epfin']), ptr(self._ws), ptr(self.nonfinite), s)
+            self._observe(T, t, d, (ptr(nobs), ptr(rew), ptr(cost), ptr(term), ptr(trunc), ptr(final), ptr(mask)), s,
+                          env_dev)
         self._act(agent, d, T, T, None, s, epoch_dev)
+
+    def _observe(self, T: int, t: int, d, step_ptrs: tuple, s: int, env_dev) -> None:
+        """The observe launch of step t; step_ptrs = (next obs, reward, cost, terminated, truncated, final obs, final
+        mask) as device pointers."""
+        lib().osb_ext_observe(*self._observe_args(T, t, d, step_ptrs), s)
+
+    def _observe_args(self, T: int, t: int, d, step_ptrs: tuple) -> tuple:
+        return (self._obs_dim, self._num_envs, T, t, int(self._obs_normalize), *step_ptrs, ptr(self.s_raw),
+                ptr(self.final_raw), ptr(self.ep_ret), ptr(self.ep_cost), ptr(self.ep_len), *self._norm_ptrs(),
+                ptr(d['reward']), ptr(d['cost']), ptr(d['flags']), ptr(d['epfin']), ptr(self._ws), ptr(self.nonfinite))
 
     def _graph_key(self, T: int, agent, d, eps, reset_obs) -> tuple:
         """The device pointers (and shape) a captured epoch bakes in; a change of any of them forces a recapture."""

@@ -15,7 +15,7 @@ import time
 import torch
 
 from omnisafe_b200.adapter.onpolicy_adapter import OnPolicyAdapter
-from omnisafe_b200.adapter.early_terminated_adapter import EarlyTerminatedAdapter
+from omnisafe_b200.adapter.early_terminated_adapter import EarlyTerminatedAdapter, ExternalEarlyTerminatedAdapter
 from omnisafe_b200.adapter.external_adapter import ExternalEnvAdapter
 from omnisafe_b200.adapter.saute_adapter import SauteAdapter
 from omnisafe_b200.adapter.simmer_adapter import SimmerAdapter
@@ -741,14 +741,15 @@ class TRPOSimmerPID(_SimmerMixin, TRPO):
 
 
 class _EarlyTerminatedMixin:
-    """early_terminated/ppo_early_terminated.py:L43-66, early_terminated/trpo_early_terminated.py."""
+    """early_terminated/ppo_early_terminated.py:L43-66, early_terminated/trpo_early_terminated.py.  The cost-limit rule
+    runs in the fused rollout on the synthetic env and in the observe kernel on a registered one."""
 
     def _init_env(self) -> None:
-        _require_synthetic(self._env_id, type(self).__name__)
         t, a = self._cfgs.train_cfgs, self._cfgs.algo_cfgs
         rank = distributed.get_rank()
-        self._env = EarlyTerminatedAdapter(self._env_id, t.vector_env_nums, self._seed, self._cfgs, device=self._device,
-                                           env_id_offset=rank * t.vector_env_nums)
+        cls = EarlyTerminatedAdapter if self._env_id in synthetic_envs() else ExternalEarlyTerminatedAdapter
+        self._env = cls(self._env_id, t.vector_env_nums, self._seed, self._cfgs, device=self._device,
+                        env_id_offset=rank * t.vector_env_nums)
         self._steps_per_epoch = distributed.local_steps(a.steps_per_epoch, t.vector_env_nums)
 
 

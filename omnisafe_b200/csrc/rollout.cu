@@ -1322,8 +1322,17 @@ __device__ __forceinline__ void chan_combine(double& n, double& m, double& q, do
     n = nn;
 }
 
-__global__ void __launch_bounds__(NTHREADS) ext_observe_kernel(ExtObs x, EnvState st, NormState ns, Slabs sl, int O, int N,
-                                                               int T, int t, int obs_normalize, int is_reset) {
+// EARLY: EarlyTerminatedAdapter.step on top of the step (early_terminated_adapter.py:L77-87), one thread per env.  The
+// env's raw cost goes into the accumulator; once it exceeds cost_limit the step stores reward 0 (in the slab and in the
+// episode return), terminated = 1 and truncated as the env reported it, the accumulator is cleared, and trig[env] = 1
+// asks the host to reset the env (ext_reset_rows_kernel then ingests the reset observation).  An ordinary episode end
+// leaves the accumulator alone.  trig_total, when not null, receives the number of triggered envs (zeroed by the host
+// before the launch).  The observation rows are those env.step returned, so ObsNormalize pushes the env's own final rows
+// and then every next row, a triggered env that did not end contributing its pre-reset state.
+template <bool EARLY>
+__device__ __forceinline__ void ext_observe_step(ExtObs x, EnvState st, NormState ns, Slabs sl, int O, int N, int T, int t,
+                                                 int obs_normalize, int is_reset, EarlySpec et, uint8_t* trig,
+                                                 int* trig_total) {
     __shared__ int sFin[XT];
     __shared__ int s_bad, s_nfin;
     const int tid = threadIdx.x, tile = blockIdx.x, ntiles = gridDim.x;
@@ -1337,8 +1346,18 @@ __global__ void __launch_bounds__(NTHREADS) ext_observe_kernel(ExtObs x, EnvStat
                 st.ep_ret[env] = 0.f; st.ep_cost[env] = 0.f; st.ep_len[env] = 0;
             } else {
                 fin = (x.final_obs && x.final_mask && x.final_mask[env]) ? 1 : 0;
-                const float r = x.rew[env];
-                record_step(sl, st, T, N, t, env, r, r, x.cost[env], x.term[env] != 0, x.trunc[env] != 0);
+                if constexpr (EARLY) {
+                    const float acc = __fadd_rn(et.cost_acc[env], x.cost[env]);
+                    const bool hit = acc > et.cost_limit;
+                    et.cost_acc[env] = hit ? 0.f : acc;
+                    trig[env] = hit ? 1 : 0;
+                    if (hit && trig_total) atomicAdd(trig_total, 1);
+                    const float r = hit ? 0.f : x.rew[env];
+                    record_step(sl, st, T, N, t, env, r, r, x.cost[env], hit || x.term[env] != 0, x.trunc[env] != 0);
+                } else {
+                    const float r = x.rew[env];
+                    record_step(sl, st, T, N, t, env, r, r, x.cost[env], x.term[env] != 0, x.trunc[env] != 0);
+                }
             }
         }
         sFin[tid] = fin;
@@ -1431,6 +1450,97 @@ __global__ void __launch_bounds__(NTHREADS) ext_observe_kernel(ExtObs x, EnvStat
         ns.count[1] = count + nfin;
         ns.count[0] = count + nfin + N;
         *ns.had_fin = nfin > 0 ? 1 : 0;
+        *ns.ticket = 0u;
+    }
+}
+
+__global__ void __launch_bounds__(NTHREADS) ext_observe_kernel(ExtObs x, EnvState st, NormState ns, Slabs sl, int O, int N,
+                                                               int T, int t, int obs_normalize, int is_reset) {
+    ext_observe_step<false>(x, st, ns, sl, O, N, T, t, obs_normalize, is_reset, EarlySpec{nullptr, 0.f}, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(NTHREADS) ext_observe_early_kernel(ExtObs x, EnvState st, NormState ns, Slabs sl,
+                                                                     int O, int N, int T, int t, int obs_normalize,
+                                                                     EarlySpec et, uint8_t* trig, int* trig_total) {
+    ext_observe_step<true>(x, st, ns, sl, O, N, T, t, obs_normalize, 0, et, trig, trig_total);
+}
+
+// The reset observations of the envs the cost rule cut at step t (rows of obs where mask is set; the others are ignored)
+// into the state buffer step t + 1 reads, and their ObsNormalize push (ObsNormalize.reset, wrapper.py:L243-261) after the
+// step's own pushes: fp64 per-tile moments of the masked rows combined in tile order by the last CTA, with per-tile row
+// counts, so the row count stays on the device.  No masked row: the statistics are untouched.  mean1 / std1 / had_fin
+// keep the values of the step's final-row push, which the next act launch's truncation bootstraps read.
+__global__ void __launch_bounds__(NTHREADS, 1) ext_reset_rows_kernel(const float* __restrict__ obs,
+                                                                  const uint8_t* __restrict__ mask, float* s_nxt,
+                                                                  NormState ns, double* part, int* nonfinite, int O,
+                                                                  int N, int obs_normalize) {
+    __shared__ int sM[XT];
+    __shared__ int s_bad, s_n;
+    const int tid = threadIdx.x, tile = blockIdx.x, ntiles = gridDim.x;
+    const int env0 = tile * XT, rows = min(XT, N - env0);
+    if (tid == 0) s_bad = 0;
+    if (tid < XT) sM[tid] = (tid < rows && mask[env0 + tid] != 0) ? 1 : 0;
+    __syncthreads();
+    bool bad = false;
+    for (int i = tid; i < rows * O; i += NTHREADS) {
+        if (sM[i / O]) {
+            const size_t g = (size_t)env0 * O + i;
+            const float v = obs[g];
+            bad |= !isfinite(v);
+            s_nxt[g] = v;
+        }
+    }
+    if (bad) s_bad = 1;
+    if (!obs_normalize) {
+        __syncthreads();
+        if (tid == 0 && s_bad) *nonfinite = 1;
+        return;
+    }
+    int nr = 0;
+    for (int r = 0; r < rows; ++r) nr += sM[r];
+    double* P = part + (size_t)tile * 2 * O;
+    for (int j = tid; j < O; j += NTHREADS) {
+        double s = 0.0;
+        for (int r = 0; r < rows; ++r)
+            if (sM[r]) s += (double)obs[(size_t)(env0 + r) * O + j];
+        const double m = nr ? s / nr : 0.0;
+        double q = 0.0;
+        for (int r = 0; r < rows; ++r)
+            if (sM[r]) { const double d = (double)obs[(size_t)(env0 + r) * O + j] - m; q += d * d; }
+        P[j] = m; P[O + j] = q;
+    }
+    double* cnt = part + (size_t)ntiles * 2 * O;
+    if (tid == 0) cnt[tile] = (double)nr;
+    const bool last = last_cta(ns.ticket);
+    if (tid == 0 && s_bad) *nonfinite = 1;
+    if (!last) return;
+
+    __threadfence();
+    if (tid == 0) {
+        int total = 0;
+        for (int k = 0; k < ntiles; ++k) total += (int)__ldcg(cnt + k);
+        s_n = total;
+    }
+    __syncthreads();
+    const int n = s_n;
+    const long long count = __ldcg(ns.count);
+    if (n > 0) {
+        for (int j = tid; j < O; j += NTHREADS) {
+            double nn = 0.0, m = 0.0, q = 0.0;
+            for (int k = 0; k < ntiles; ++k) {
+                const double* Pk = part + (size_t)k * 2 * O;
+                chan_combine(nn, m, q, __ldcg(cnt + k), __ldcg(Pk + j), __ldcg(Pk + O + j));
+            }
+            float mean = __ldcg(ns.mean + j), sumsq = __ldcg(ns.sumsq + j);
+            norm_push_moments(mean, sumsq, count, n, m, q);
+            ns.mean[j] = mean;
+            ns.sumsq[j] = sumsq;
+            ns.std[j] = norm_std(sumsq, count + n);
+        }
+    }
+    __syncthreads();
+    if (tid == 0) {
+        ns.count[0] = count + n;
         *ns.ticket = 0u;
     }
 }
@@ -2107,6 +2217,42 @@ int osb_ext_observe(int O, int N, int T, int t, int obs_normalize, const float* 
     NormState ns{norm_mean, norm_sumsq, norm_std, norm_mean1, norm_std1, norm_count, nullptr, nullptr, nullptr, had_fin, ticket};
     Slabs sl{nullptr, nullptr, nullptr, rew_slab, cost_slab, nullptr, nullptr, nullptr, nullptr, flags, epfin};
     return launch_observe(x, st, ns, sl, O, N, T, t, obs_normalize, 0, stream);
+}
+
+int osb_ext_observe_early(int O, int N, int T, int t, int obs_normalize, const float* next_obs, const float* rew,
+                          const float* cost, const unsigned char* terminated, const unsigned char* truncated,
+                          const float* final_obs, const unsigned char* final_mask, float* s_raw, float* final_raw,
+                          float* ep_ret, float* ep_cost, int* ep_len, float* norm_mean, float* norm_sumsq,
+                          float* norm_std, float* norm_mean1, float* norm_std1, long long* norm_count, int* had_fin,
+                          unsigned* ticket, float* rew_slab, float* cost_slab, unsigned char* flags, float* epfin,
+                          double* workspace, int* nonfinite, float* cost_acc, float cost_limit, unsigned char* trig,
+                          int* trig_total, void* stream) {
+    OSB_CHECK_ARG(O > 0 && N > 0 && T > 0 && t >= 0 && t < T, "bad dims / step index");
+    OSB_CHECK_ARG(next_obs && rew && cost && terminated && truncated && s_raw && final_raw && rew_slab && cost_slab &&
+                  flags && epfin && workspace && nonfinite && cost_acc && trig, "bad argument");
+    cudaStream_t s = (cudaStream_t)stream;
+    if (trig_total) OSB_CUDA(cudaMemsetAsync(trig_total, 0, sizeof(int), s));
+    ExtObs x{next_obs, rew, cost, terminated, truncated, final_obs, final_mask, workspace, nonfinite};
+    EnvState st{s_raw, final_raw, nullptr, nullptr, nullptr, ep_ret, ep_cost, ep_len, nullptr};
+    NormState ns{norm_mean, norm_sumsq, norm_std, norm_mean1, norm_std1, norm_count, nullptr, nullptr, nullptr, had_fin, ticket};
+    Slabs sl{nullptr, nullptr, nullptr, rew_slab, cost_slab, nullptr, nullptr, nullptr, nullptr, flags, epfin};
+    ext_observe_early_kernel<<<(N + XT - 1) / XT, NTHREADS, 0, s>>>(x, st, ns, sl, O, N, T, t, obs_normalize,
+                                                                    EarlySpec{cost_acc, cost_limit}, trig, trig_total);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}
+
+int osb_ext_reset_rows(int O, int N, int t, int obs_normalize, const unsigned char* mask, const float* obs, float* s_raw,
+                       float* norm_mean, float* norm_sumsq, float* norm_std, long long* norm_count, unsigned* ticket,
+                       double* workspace, int* nonfinite, void* stream) {
+    OSB_CHECK_ARG(O > 0 && N > 0 && t >= 0, "bad dims / step index");
+    OSB_CHECK_ARG(mask && obs && s_raw && norm_mean && norm_sumsq && norm_std && norm_count && ticket && workspace &&
+                  nonfinite, "bad argument");
+    NormState ns{norm_mean, norm_sumsq, norm_std, nullptr, nullptr, norm_count, nullptr, nullptr, nullptr, nullptr, ticket};
+    ext_reset_rows_kernel<<<(N + XT - 1) / XT, NTHREADS, 0, (cudaStream_t)stream>>>(
+        obs, mask, s_raw + (size_t)((t + 1) & 1) * N * O, ns, workspace, nonfinite, O, N, obs_normalize);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
 }
 
 }  // extern "C"

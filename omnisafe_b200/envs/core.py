@@ -23,6 +23,14 @@ epoch, which removes the host's per-launch cost.  Such an env promises:
   so its structure is the same on every step;
 - the tensors `step` returns may be fresh each call: the adapter copies them inside the graph.
 
+An env may define `reset_envs(mask) -> obs` (optional, an omnisafe_b200 extension): a reset of some envs only.  `mask` is
+an [N] bool tensor on the env's device; the masked envs start fresh episodes and the masked rows of the returned [N, O]
+hold their first observations (the other rows are ignored).  An all-false mask leaves the env's state untouched; at
+N = 1, `reset_envs(tensor([True]))` is equivalent to `reset()`.  For a `graph_safe` env the call must be capturable, as
+`step` is: no host synchronisation, and the same output storage on every call.  The EarlyTerminated algorithms use it to
+reset the envs the cost limit cuts: with it they run any number of envs (a graph-safe env keeps its epoch in the CUDA
+graph); without it they run a single env only, as upstream does, resetting it through `reset()` and eagerly.
+
 An env may also define `state_dict() -> dict` and `load_state_dict(sd)` (optional, an omnisafe_b200 extension).  When it
 does, a saved training state (`AlgoWrapper.save_state`, `learn(save_state_freq=...)`) holds what `state_dict()` returns and
 `Agent.resume` hands it back to `load_state_dict` right after `set_seed`, before the first epoch; a run that resumes then

@@ -1,14 +1,16 @@
 """Throughput of the external-env path: the bench.py headline workload (PPOLag, 4096 envs x T = 128, obs 60 / act 8,
 batch 16384, update_iters 8) on a PyTorch-on-GPU port of the synthetic dynamics registered as a user CMDP.
 
-    python tools/external_env_bench.py [--steps K] [--warmup W] [--precision bf16x3|tf32|fp32] [--graph]
+    python tools/external_env_bench.py [--steps K] [--warmup W] [--precision bf16x3|tf32|fp32] [--graph] [--algo NAME]
 
 Every env step is one act launch, the env's own PyTorch kernels and one observe launch.  Prints ONE JSON line:
 env-steps/s over full epochs (rollout + GAE + update, CUDA events), and one rollout split into the device time spent
 inside env.step (CUDA events at its entry and exit) and the rest (act / observe kernels, episode window, launch gaps).
 --graph runs the graph-safe TorchBox (same arithmetic, state written in place, no events inside step), whose epoch the
 adapter replays from a CUDA graph; it reports env-steps/s and the rollout time per epoch only.  With OSB_NO_GRAPH=1 the
-same env runs eagerly.  Logs go to a temporary directory; nothing is written to the tree.
+same env runs eagerly.  --algo picks the algorithm (default PPOLag); TorchBox has the optional reset_envs(mask) hook, so
+PPOEarlyTerminated runs the cost-limit rule on all 4096 envs (graph-safe TorchBox: inside the replayed graph).  Logs go to
+a temporary directory; nothing is written to the tree.
 """
 from __future__ import annotations
 
@@ -97,6 +99,12 @@ def register_torch_box() -> None:
                 self.timing.append(ev)
             return self.s, reward, cost, term, trunc, info
 
+        def reset_envs(self, mask):
+            self.episode = torch.where(mask, self.episode + 1, self.episode)
+            self.ep_step = torch.where(mask, torch.zeros_like(self.ep_step), self.ep_step)
+            self.s = torch.where(mask[:, None], self._reset_values(self.episode), self.s)
+            return self.s
+
         def close(self):
             pass
 
@@ -126,6 +134,12 @@ def register_torch_box() -> None:
             self.s.copy_(torch.where(trunc[:, None], self._reset_values(self.episode), sn))
             self.ep_step.copy_(torch.where(trunc, torch.zeros_like(self.ep_step), self.ep_step + 1))
             return self.s, reward, cost, term, trunc, {'final_observation': sn, '_final_observation': trunc}
+
+        def reset_envs(self, mask):
+            self.episode.copy_(torch.where(mask, self.episode + 1, self.episode))
+            self.ep_step.copy_(torch.where(mask, torch.zeros_like(self.ep_step), self.ep_step))
+            self.s.copy_(torch.where(mask[:, None], self._reset_values(self.episode), self.s))
+            return self.s
 
     env_register(TorchBox)
     env_register(TorchBoxGraph)
@@ -159,6 +173,7 @@ def main() -> None:
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--precision', default='bf16x3', choices=['bf16x3', 'tf32', 'fp32'])
     ap.add_argument('--graph', action='store_true', help='graph-safe TorchBox: the epoch is replayed from a CUDA graph')
+    ap.add_argument('--algo', default='PPOLag', help='algorithm, e.g. PPOLag or PPOEarlyTerminated')
     args = ap.parse_args()
     import omnisafe_b200
 
@@ -172,7 +187,7 @@ def main() -> None:
            'logger_cfgs': {'log_dir': tempfile.mkdtemp(prefix='osb_extbench_'), 'use_tensorboard': False,
                            'save_model_freq': 10 ** 9},
            'env_cfgs': {'obs_dim': O, 'act_dim': A, 'max_episode_steps': TMAX}}
-    algo = omnisafe_b200.Agent('PPOLag', env_id, custom_cfgs=cfg).agent
+    algo = omnisafe_b200.Agent(args.algo, env_id, custom_cfgs=cfg).agent
     for _ in range(max(args.warmup, 1)):
         algo.train_epoch()
     ms = timed(algo.train_epoch, args.steps) / args.steps
@@ -185,7 +200,7 @@ def main() -> None:
         ms_env = sum(a.elapsed_time(b) for a, b in env.timing) / k
         split = {'env_step_ms': ms_env, 'kernel_ms': ms_roll - ms_env}
     print(json.dumps({
-        'metric': f'env-steps/sec (rollout+GAE+update) PPO-Lag, {env_id} through the external-env path',
+        'metric': f'env-steps/sec (rollout+GAE+update) {args.algo}, {env_id} through the external-env path',
         'value': spe / (ms * 1e-3), 'unit': 'env-steps/s', 'ms_per_step': ms, 'steps': args.steps,
         'rollout_ms': ms_roll, **split, 'graph_mode': algo._env.graph_mode,
         'config': {'envs': N, 'steps_per_env': T, 'obs_dim': O, 'act_dim': A, 'batch_size': 16384, 'update_iters': 8,
