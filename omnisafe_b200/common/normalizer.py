@@ -3,7 +3,8 @@
 Mirrors omnisafe/common/normalizer.py:L25-158: `_mean`, `_sumsq`, `_var`, `_std`, `_count`, `_clip`
 are exposed through state_dict() with the reference's key names so checkpoints stay loadable by
 the reference Evaluator (omnisafe/evaluator.py:L153-178).  The update itself (Normalizer._push) is
-fused into the rollout kernel (csrc/rollout.cu: norm_push / norm_finalize).
+fused into the rollout kernels (csrc/rollout.cu: norm_fold on the synthetic env, the observe kernels on a registered
+env; the fp32 update itself in csrc/normalizer.cuh).
 """
 from __future__ import annotations
 

@@ -11,11 +11,12 @@
 // Grid = (ceil(N/32) env tiles) x (3 networks).  Actor CTAs sample the action, run the env
 // transition, append the step to the time-major slabs and feed the running-normaliser sums; critic
 // CTAs write V_r / V_c and the bootstrap values of paths cut in the previous step.  The grid-wide
-// ObsNormalize reduction is done with order-independent fixed-point atomics and finalised by the
-// last actor CTA of the launch; the next launch (= kernel boundary = grid sync) consumes it.
+// ObsNormalize reduction is done with order-independent fixed-point atomics and folded into the statistics by the
+// last CTA of the launch (norm_fold); the next launch (= kernel boundary = grid sync) consumes it.
 #include "common.cuh"
 #include "gaussian.cuh"
 #include "mlp.cuh"
+#include "normalizer.cuh"
 #include "tc_forward.cuh"
 
 namespace osb {
@@ -104,19 +105,7 @@ __device__ __forceinline__ float env_next_value(float s, float a, float b) {
     return fminf(fmaxf(v, -10.f), 10.f);
 }
 
-// Chan / Golub / LeVeque batched update as Normalizer._push writes it (normalizer.py:L102-120),
-// fp32 state, from the batch mean and sum of squared deviations (fp64).
-__device__ __forceinline__ void norm_push_moments(float& mean, float& sumsq, long long count_old, long long n,
-                                                  double mraw, double m2) {
-    const float mean_raw = (float)mraw, sumq_raw = (float)m2;
-    const long long count = count_old + n;
-    const float delta = __fadd_rn(mean_raw, -mean);
-    mean = __fadd_rn(mean, __fdiv_rn(__fmul_rn(delta, (float)n), (float)count));
-    const float d2 = __fmul_rn(delta, delta);
-    const float corr = __fdiv_rn(__fmul_rn(__fmul_rn(d2, (float)count_old), (float)n), (float)count);
-    sumsq = __fadd_rn(sumsq, __fadd_rn(sumq_raw, corr));
-}
-// the same update with the batch moments derived from the fixed-point sums
+// Normalizer._push of a batch of n rows given by its fixed-point sums x, x^2
 __device__ void norm_push(float& mean, float& sumsq, long long count_old, long long n,
                           long long sx_fix, long long sxx_fix) {
     const double sx = (double)sx_fix / FIX_SCALE, sxx = (double)sxx_fix / FIX_SCALE;
@@ -125,38 +114,46 @@ __device__ void norm_push(float& mean, float& sumsq, long long count_old, long l
     if (m2 < 0.0) m2 = 0.0;
     norm_push_moments(mean, sumsq, count_old, n, mraw, m2);
 }
-__device__ __forceinline__ float norm_std(float sumsq, long long count) {
-    const float var = __fdiv_rn(sumsq, (float)(count - 1));
-    return fmaxf(sqrtf(var), 1e-2f);
-}
 
-// Executed by the last-arriving actor CTA: fold the launch's sums into the running statistics.
-__device__ void norm_finalize(const NormState& ns, int O, long long n_all) {
+// Executed by the last-arriving CTA of a launch: folds the launch's fixed-point sums into the running statistics in
+// ObsNormalize's push order -- the final-observation rows (acc_fin, *fin_count rows; none: skipped), the next
+// observations (acc_all, n_all > 0 rows), then the reset rows (acc_rst, n_rst rows; none or null: skipped) -- and clears
+// the sums and fin_count.  stats1: mean1 / std1 / count[1] / had_fin take the state after the final rows, which the
+// bootstrap values of the next step's truncated paths are computed from.  push = false: only count[0] advances.
+__device__ void norm_fold(const NormState& ns, int O, long long n_all, bool stats1, bool push = true,
+                          long long* acc_rst = nullptr, long long n_rst = 0) {
     __threadfence();
     const int nfin = *((volatile int*)ns.fin_count);
     long long count = __ldcg(ns.count);          // (.cg: in the persistent kernel another SM may have written these last step)
-    for (int j = threadIdx.x; j < O; j += blockDim.x) {
+    for (int j = threadIdx.x; push && j < O; j += blockDim.x) {
         float mean = __ldcg(ns.mean + j), sumsq = __ldcg(ns.sumsq + j);
         long long c = count;
         if (nfin > 0) {
             norm_push(mean, sumsq, c, nfin, __ldcg(ns.acc_fin + j), __ldcg(ns.acc_fin + O + j));
             c += nfin;
-            ns.mean1[j] = mean;
-            ns.std1[j] = norm_std(sumsq, c);
+            if (stats1) {
+                ns.mean1[j] = mean;
+                ns.std1[j] = norm_std(sumsq, c);
+            }
         }
         norm_push(mean, sumsq, c, n_all, __ldcg(ns.acc_all + j), __ldcg(ns.acc_all + O + j));
         c += n_all;
+        if (n_rst > 0) {
+            norm_push(mean, sumsq, c, n_rst, __ldcg(acc_rst + j), __ldcg(acc_rst + O + j));
+            c += n_rst;
+        }
         ns.mean[j] = mean;
         ns.sumsq[j] = sumsq;
         ns.std[j] = norm_std(sumsq, c);
         ns.acc_all[j] = 0; ns.acc_all[O + j] = 0;
         ns.acc_fin[j] = 0; ns.acc_fin[O + j] = 0;
+        if (acc_rst) { acc_rst[j] = 0; acc_rst[O + j] = 0; }
     }
     __syncthreads();
     if (threadIdx.x == 0) {
-        ns.count[1] = count + nfin;
-        ns.count[0] = count + nfin + n_all;
-        *ns.had_fin = nfin > 0 ? 1 : 0;
+        if (stats1) ns.count[1] = count + nfin;
+        ns.count[0] = count + nfin + n_all + n_rst;
+        if (stats1) *ns.had_fin = nfin > 0 ? 1 : 0;
         *ns.fin_count = 0;
         *ns.ticket = 0u;
     }
@@ -240,7 +237,7 @@ __global__ void __launch_bounds__(NTHREADS) env_reset_kernel(EnvSpec es, EnvStat
         st.ep_len[env] = 0;
         if (sa.safety) sa.safety[env] = sa.init;   // buffer 0: step 0 reads parity 0
     }
-    if (es.obs_normalize && last_cta(ns.ticket)) norm_finalize(ns, O, (long long)N);
+    if (es.obs_normalize && last_cta(ns.ticket)) norm_fold(ns, O, N, true);
 }
 
 // Philox4x32-10 (fast-mode noise); counter = (env gid, global step, lane block, 0).
@@ -500,7 +497,7 @@ __device__ void eval_action(const StepArgs& p, int env0, float* sMu, int ld, con
 // and the episode end.  Then the normaliser sums of the rows the reference pushes in this step, in its order: the final
 // observations of envs that ended, the next observations of every running env (an env that ended hands back its
 // auto-reset observation), and the observations of the envs reset after the step.  sF / sE1 / sE2: R ints of shared
-// scratch each.  eval_finalize (one CTA, after every CTA's step) folds the sums into the statistics.
+// scratch each.  eval_fold (one CTA, after every CTA's step) folds the sums into the statistics.
 template <int R>
 __device__ void eval_step(const StepArgs& p, int t, int env0, float* sMu, int ld, const float* log_std, int* sF,
                           uint32_t* sE1, uint32_t* sE2) {
@@ -600,50 +597,22 @@ __device__ void eval_step(const StepArgs& p, int t, int env0, float* sMu, int ld
 
 // One CTA, after every CTA's eval_step of the step: pushes the step's rows into the statistics (final rows, next rows,
 // reset rows: three pushes, as Normalizer.normalize is called three times) and advances the done word.
-__device__ void eval_finalize(const StepArgs& p) {
+__device__ void eval_fold(const StepArgs& p) {
     const EvalSpec& ev = p.ev;
-    const int O = p.es.O, tid = threadIdx.x;
     __threadfence();
-    const int nfin = *((volatile int*)p.ns.fin_count), nall = *((volatile int*)ev.ctr),
-              nrst = *((volatile int*)(ev.ctr + 2));
-    const long long count = __ldcg(p.ns.count);
-    if (p.es.obs_normalize) {
-        for (int j = tid; j < O; j += NTHREADS) {
-            float mean = __ldcg(p.ns.mean + j), sumsq = __ldcg(p.ns.sumsq + j);
-            long long c = count;
-            if (nfin > 0) {
-                norm_push(mean, sumsq, c, nfin, __ldcg(p.ns.acc_fin + j), __ldcg(p.ns.acc_fin + O + j));
-                c += nfin;
-            }
-            norm_push(mean, sumsq, c, nall, __ldcg(p.ns.acc_all + j), __ldcg(p.ns.acc_all + O + j));
-            c += nall;
-            if (nrst > 0) {
-                norm_push(mean, sumsq, c, nrst, __ldcg(ev.acc_rst + j), __ldcg(ev.acc_rst + O + j));
-                c += nrst;
-            }
-            p.ns.mean[j] = mean;
-            p.ns.sumsq[j] = sumsq;
-            p.ns.std[j] = norm_std(sumsq, c);
-            p.ns.acc_all[j] = 0; p.ns.acc_all[O + j] = 0;
-            p.ns.acc_fin[j] = 0; p.ns.acc_fin[O + j] = 0;
-            ev.acc_rst[j] = 0; ev.acc_rst[O + j] = 0;
-        }
-    }
-    __syncthreads();
-    if (tid == 0) {
-        p.ns.count[0] = count + nfin + nall + nrst;
-        *p.ns.fin_count = 0;
+    const int nall = *((volatile int*)ev.ctr), nrst = *((volatile int*)(ev.ctr + 2));
+    norm_fold(p.ns, p.es.O, nall, false, p.es.obs_normalize, ev.acc_rst, nrst);
+    if (threadIdx.x == 0) {
         ev.ctr[0] = __ldcg(ev.ctr + 1);
         ev.ctr[1] = 0;
         ev.ctr[2] = 0;
-        *p.ns.ticket = 0u;
     }
 }
 
 // Software grid barrier at the end of step t of a persistent (cooperative) launch: every CTA arrives, the last one runs
 // on_last() (the step's fold into the running state) before it releases the others.  bar_ctr / bar_flag are zero at launch.
 template <class F>
-__device__ __forceinline__ void grid_step_barrier(const StepArgs& p, int t, int& s_last, F on_last) {
+__device__ __forceinline__ void grid_step_barrier(const StepArgs& p, int t, int& s_last, F&& on_last) {
     __threadfence();
     __syncthreads();
     if (threadIdx.x == 0) s_last = (atomicAdd(p.bar_ctr, 1u) == gridDim.x * gridDim.y * (unsigned)(t + 1) - 1u) ? 1 : 0;
@@ -758,7 +727,7 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
         } else {
             eval_step<RT>(p, t, env0, sO, LDO, theta + L.off_logstd, sFlag, reinterpret_cast<uint32_t*>(sNew),
                           reinterpret_cast<uint32_t*>(sFin));
-            if (last_cta(p.ns.ticket)) eval_finalize(p);
+            if (last_cta(p.ns.ticket)) eval_fold(p);
         }
         return;
     }
@@ -865,7 +834,7 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
     }
     // every CTA (actor and critic) has now consumed the normaliser state of this step; the last
     // one to arrive folds the step's sums into it for the next launch.
-    if (p.es.obs_normalize && !p.is_tail && last_cta(p.ns.ticket)) norm_finalize(p.ns, O, (long long)N);
+    if (p.es.obs_normalize && !p.is_tail && last_cta(p.ns.ticket)) norm_fold(p.ns, O, N, true);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -904,10 +873,9 @@ static_assert(TF_ACC % 2 == 0, "the fixed-point sums need 8-byte alignment");
 // env.step between the launches).
 // EVAL = true: the evaluation of a saved policy, as in rollout_step_kernel<EXT, true>; PERSIST (synthetic env only): ONE
 // cooperative launch runs every step until all envs have finished, the last CTA at each step's grid barrier running
-// eval_finalize.
+// eval_fold.
 template <bool X3, bool PERSIST, bool EXT = false, bool EVAL = false>
 __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p) {
-    static_assert(!(EXT && PERSIST), "the external-env act step is one launch per step");
     static_assert(!(EXT && PERSIST), "the external-env steps are one launch per step");
     if constexpr (EVAL) {
         if (__ldcg(p.ev.ctr) == 0) return;
@@ -1105,10 +1073,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
         } else {
             eval_step<RTC>(p, t, env0, sAct, OUTP, theta + L.off_logstd, sFlag, sEpi, reinterpret_cast<uint32_t*>(sStep));
             if constexpr (PERSIST) {
-                grid_step_barrier(p, t, s_last, [&] { eval_finalize(p); });
+                grid_step_barrier(p, t, s_last, [&] { eval_fold(p); });
                 continue;
             } else {
-                if (last_cta(p.ns.ticket)) eval_finalize(p);
+                if (last_cta(p.ns.ticket)) eval_fold(p);
                 return;
             }
         }
@@ -1260,25 +1228,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
     RSTAMP(9);
     if (PERSIST) {
         if (!is_tail) {
-            // grid barrier; the last CTA to arrive folds the step's sums into the running statistics, then releases
-            __threadfence();
-            __syncthreads();
-            if (tid == 0) s_last = (atomicAdd(p.bar_ctr, 1u) == gridDim.x * gridDim.y * (unsigned)(t + 1) - 1u) ? 1 : 0;
-            __syncthreads();
-            if (s_last) {
-                if (p.es.obs_normalize) norm_finalize(p.ns, O, (long long)N);
-                __threadfence();
-                __syncthreads();
-                if (tid == 0) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p.bar_flag), "r"((unsigned)(t + 1)) : "memory");
-            } else if (tid == 0) {
-                unsigned v;
-                do { asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p.bar_flag) : "memory"); } while (v < (unsigned)(t + 1));
-            }
-            __syncthreads();
+            grid_step_barrier(p, t, s_last, [&] { if (p.es.obs_normalize) norm_fold(p.ns, O, N, true); });
             RSTAMP(10);
         }
     } else if (!EXT && p.es.obs_normalize && !is_tail && last_cta(p.ns.ticket)) {
-        norm_finalize(p.ns, O, (long long)N);
+        norm_fold(p.ns, O, N, true);
     }
     }   // step loop
 #undef RSTAMP
@@ -1413,7 +1367,7 @@ __device__ __forceinline__ void ext_observe_step(ExtObs x, EnvState st, NormStat
     if (tid == 0 && s_bad) *x.nonfinite = 1;
     if (!last) return;
 
-    // last CTA: combine the tiles in order and push final rows, then all rows (norm_finalize's sequence)
+    // last CTA: combine the tiles in order and push final rows, then all rows (norm_fold's sequence)
     __threadfence();
     const double* cnt = x.part + (size_t)ntiles * 4 * O;
     if (tid == 0) {
@@ -1856,12 +1810,29 @@ static int ext_refuse_if_capturing(cudaStream_t stream, const char* what) {
 
 static size_t rollout_tc_acc_bytes(int N) { return (size_t)((N + RTC - 1) / RTC) * 3 * 128 * TC_COLS * sizeof(float); }
 
-// EXT = true: the act step of the external-env path (never the persistent kernel).  prepare_only: perform the host
-// actions (attributes, accumulator image) and launch nothing (osb_ext_prepare).
-template <bool EXT>
-static int launch_step(StepArgs& p, cudaStream_t stream, bool prepare_only = false) {
-    const int On = p.es.O + (p.sa.safety ? 1 : 0);
-    if ((p.precision == 1 || p.precision == 2) && On <= 64) {
+static int sm_count() {
+    static int n_sm = 0;
+    if (!n_sm) { int dev = 0; OSB_CUDA(cudaGetDevice(&dev)); OSB_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev)); }
+    return n_sm;
+}
+
+// tf32 / bf16x3 with a network input of <= 64 columns run on the tensor-core tiles, everything else on the fp32 tiles
+static bool tc_tiles(const StepArgs& p) {
+    return (p.precision == 1 || p.precision == 2) && p.es.O + (p.sa.safety ? 1 : 0) <= 64;
+}
+// the persistent kernel needs every CTA (env tiles x networks) resident
+static bool persistent_fits(const StepArgs& p, int nets) { return tc_tiles(p) && (p.N + RTC - 1) / RTC * nets <= sm_count(); }
+
+static unsigned int* g_grid_bar = nullptr;   // grid-barrier arrival counter and release flag of the persistent kernels
+
+// One launch of the step kernels: a training step (EVAL = false: grid = env tiles x the actor and both critics, the
+// epoch-end tail only the critics) or an evaluation step (grid = env tiles x the actor); on the synthetic env or, EXT,
+// the act half of a step on a user env.  persistent (synthetic env, persistent_fits): ONE cooperative launch runs every
+// step.  prepare_only: perform the host actions (attributes, accumulator image) and launch nothing (osb_ext_prepare).
+template <bool EXT, bool EVAL>
+static int launch_rollout(StepArgs& p, cudaStream_t stream, bool persistent = false, bool prepare_only = false) {
+    const int nets = EVAL ? 1 : (p.is_tail ? 2 : 3);
+    if (tc_tiles(p)) {
         const bool x3 = p.precision == 2;
         const size_t smem_tc = rollout_tc_smem_bytes(x3);
         static bool attr_tc = false;
@@ -1869,17 +1840,16 @@ static int launch_step(StepArgs& p, cudaStream_t stream, bool prepare_only = fal
             if constexpr (EXT) {
                 if (int rc = ext_refuse_if_capturing(stream, "the tensor-core kernel attributes")) return rc;
             }
-            // {tf32, bf16x3} x {one step, the persistent epoch}; EXT launches only the one-step pair
-            const void* kernels[] = {(const void*)rollout_step_tc_kernel<false, false, EXT>,
-                                     (const void*)rollout_step_tc_kernel<true, false, EXT>,
-                                     (const void*)rollout_step_tc_kernel<false, true>,
-                                     (const void*)rollout_step_tc_kernel<true, true>};
+            // {tf32, bf16x3} x {one step, persistent}; EXT launches only the one-step pair
+            const void* kernels[] = {(const void*)rollout_step_tc_kernel<false, false, EXT, EVAL>,
+                                     (const void*)rollout_step_tc_kernel<true, false, EXT, EVAL>,
+                                     (const void*)rollout_step_tc_kernel<false, true, false, EVAL>,
+                                     (const void*)rollout_step_tc_kernel<true, true, false, EVAL>};
             for (int i = 0; i < (EXT ? 2 : 4); ++i)
                 OSB_CUDA(cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize,
                                               (int)rollout_tc_smem_bytes(i & 1)));
             attr_tc = true;
         }
-        dim3 grid_tc((p.N + RTC - 1) / RTC, p.is_tail ? 2 : 3);
         if constexpr (EXT) {
             if (acc_scratch_capacity(ACC_ROLLOUT) < rollout_tc_acc_bytes(p.N))
                 if (int rc = ext_refuse_if_capturing(stream, "a larger accumulator image")) return rc;
@@ -1887,32 +1857,36 @@ static int launch_step(StepArgs& p, cudaStream_t stream, bool prepare_only = fal
         p.acc = acc_scratch(ACC_ROLLOUT, rollout_tc_acc_bytes(p.N));
         if (!p.acc) return OSB_ERR_CUDA;
         if (prepare_only) return OSB_OK;
-        if (p.bar_ctr != nullptr) {
-            // the whole epoch in one cooperative launch (every CTA resident: the step barrier is a software grid barrier)
+        const dim3 grid_tc((p.N + RTC - 1) / RTC, nets);
+        if (persistent) {
+            // every CTA resident: the step barrier is a software grid barrier
+            if (!g_grid_bar) OSB_CUDA(cudaMalloc(&g_grid_bar, 64));
+            p.bar_ctr = g_grid_bar; p.bar_flag = g_grid_bar + 1;
             OSB_CUDA(cudaMemsetAsync(p.bar_ctr, 0, 2 * sizeof(unsigned int), stream));
             void* args[] = {&p};
             osb_count_launch();
-            OSB_CUDA(cudaLaunchCooperativeKernel(x3 ? (void*)rollout_step_tc_kernel<true, true> : (void*)rollout_step_tc_kernel<false, true>,
-                                                 dim3((p.N + RTC - 1) / RTC, 3), dim3(NTHREADS), args, smem_tc, stream));
+            OSB_CUDA(cudaLaunchCooperativeKernel(x3 ? (void*)rollout_step_tc_kernel<true, true, false, EVAL>
+                                                    : (void*)rollout_step_tc_kernel<false, true, false, EVAL>,
+                                                 grid_tc, dim3(NTHREADS), args, smem_tc, stream));
             return OSB_OK;
         }
-        if (x3) rollout_step_tc_kernel<true, false, EXT><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
-        else rollout_step_tc_kernel<false, false, EXT><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
+        if (x3) rollout_step_tc_kernel<true, false, EXT, EVAL><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
+        else rollout_step_tc_kernel<false, false, EXT, EVAL><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
         OSB_LAUNCH_CHECK();
         return OSB_OK;
     }
+    const int On = p.es.O + (p.sa.safety ? 1 : 0);
     const size_t smem = rollout_smem_bytes(On);
     static size_t attr = 0;
     if (smem > attr) {
         if constexpr (EXT) {
             if (int rc = ext_refuse_if_capturing(stream, "a larger shared-memory attribute")) return rc;
         }
-        OSB_CUDA(cudaFuncSetAttribute(rollout_step_kernel<EXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        OSB_CUDA(cudaFuncSetAttribute(rollout_step_kernel<EXT, EVAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = smem;
     }
     if (prepare_only) return OSB_OK;
-    dim3 grid((p.N + RT - 1) / RT, p.is_tail ? 2 : 3);
-    rollout_step_kernel<EXT><<<grid, NTHREADS, smem, stream>>>(p);
+    rollout_step_kernel<EXT, EVAL><<<dim3((p.N + RT - 1) / RT, nets), NTHREADS, smem, stream>>>(p);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
 }
@@ -1958,7 +1932,7 @@ int osb_rollout_step(int O, int A, int max_episode_steps, unsigned seed, unsigne
                                      val_c, boot_r, boot_c, flags, epfin, theta, noise_seed, precision);
     p.eps = eps; p.global_step = global_step;
     p.t = t; p.is_tail = (t == T) ? 1 : 0;
-    return launch_step<false>(p, (cudaStream_t)stream);
+    return launch_rollout<false, false>(p, (cudaStream_t)stream);
 }
 
 int osb_rollout_epoch(int O, int A, int max_episode_steps, unsigned seed, unsigned term_threshold,
@@ -1983,15 +1957,10 @@ int osb_rollout_epoch(int O, int A, int max_episode_steps, unsigned seed, unsign
     int rc = launch_env_reset(p.es, p.st, p.ns, N, s);
     if (rc) return rc;
     p.dbg = g_rollout_dbg;
-    // tensor-core modes with every CTA resident (grid = env tiles x 3 networks <= SMs): one persistent launch per epoch
-    static int n_sm = 0;
-    if (!n_sm) { int dev = 0; OSB_CUDA(cudaGetDevice(&dev)); OSB_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev)); }
-    if ((precision == 1 || precision == 2) && O + (g_saute.safety ? 1 : 0) <= 64 && ((N + RTC - 1) / RTC) * 3 <= n_sm) {
-        static unsigned int* d_bar = nullptr;
-        if (!d_bar) OSB_CUDA(cudaMalloc(&d_bar, 64));
-        p.bar_ctr = d_bar; p.bar_flag = d_bar + 1;
+    // tensor-core modes with every CTA resident: one persistent launch per epoch
+    if (persistent_fits(p, 3)) {
         p.t = 0; p.is_tail = 0; p.eps = eps_all; p.global_step = epoch_index * (unsigned)T;
-        rc = launch_step<false>(p, s);
+        rc = launch_rollout<false, false>(p, s, true);
         if (rc) return rc;
         return osb_episode_window(flags, epfin, T, N, W, ring, meta, window_sums, stream);
     }
@@ -1999,7 +1968,7 @@ int osb_rollout_epoch(int O, int A, int max_episode_steps, unsigned seed, unsign
         p.t = t; p.is_tail = (t == T) ? 1 : 0;
         p.eps = (eps_all && t < T) ? eps_all + (size_t)t * N * A : nullptr;
         p.global_step = epoch_index * (unsigned)T + (unsigned)t;
-        rc = launch_step<false>(p, s);
+        rc = launch_rollout<false, false>(p, s);
         if (rc) return rc;
     }
     return osb_episode_window(flags, epfin, T, N, W, ring, meta, window_sums, stream);
@@ -2018,63 +1987,7 @@ int osb_episode_window(const unsigned char* flags, const float* epfin, int T, in
 
 }  // extern "C"
 
-// Evaluation launches: the tensor-core tiles for tf32 / bf16x3 with a network input of <= 64 columns (the rollout's
-// rule), else the fp32 tiles; grid = env tiles x the actor.  persistent (synthetic env, tensor-core tiles, every CTA
-// resident): ONE cooperative launch runs all steps (p.T = their bound); otherwise one launch is one step.
 static StepArgs ext_step_args(int O, int A, int obs_normalize, int N, int precision);
-
-template <bool EXT>
-static int launch_eval(StepArgs& p, cudaStream_t stream, bool persistent) {
-    const int On = p.es.O + (p.sa.safety ? 1 : 0);
-    if ((p.precision == 1 || p.precision == 2) && On <= 64) {
-        const bool x3 = p.precision == 2;
-        static bool attr_tc = false;
-        if (!attr_tc) {
-            const void* kernels[] = {(const void*)rollout_step_tc_kernel<false, false, EXT, true>,
-                                     (const void*)rollout_step_tc_kernel<true, false, EXT, true>,
-                                     (const void*)rollout_step_tc_kernel<false, true, false, true>,
-                                     (const void*)rollout_step_tc_kernel<true, true, false, true>};
-            for (int i = 0; i < (EXT ? 2 : 4); ++i)
-                OSB_CUDA(cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (int)rollout_tc_smem_bytes(i & 1)));
-            attr_tc = true;
-        }
-        p.acc = acc_scratch(ACC_ROLLOUT, rollout_tc_acc_bytes(p.N));
-        if (!p.acc) return OSB_ERR_CUDA;
-        const dim3 grid((p.N + RTC - 1) / RTC, 1);
-        const size_t smem = rollout_tc_smem_bytes(x3);
-        if constexpr (!EXT) {
-            if (persistent) {
-                OSB_CUDA(cudaMemsetAsync(p.bar_ctr, 0, 2 * sizeof(unsigned int), stream));
-                void* args[] = {&p};
-                osb_count_launch();
-                OSB_CUDA(cudaLaunchCooperativeKernel(x3 ? (void*)rollout_step_tc_kernel<true, true, false, true>
-                                                        : (void*)rollout_step_tc_kernel<false, true, false, true>,
-                                                     grid, dim3(NTHREADS), args, smem, stream));
-                return OSB_OK;
-            }
-        }
-        if (x3) rollout_step_tc_kernel<true, false, EXT, true><<<grid, NTHREADS, smem, stream>>>(p);
-        else rollout_step_tc_kernel<false, false, EXT, true><<<grid, NTHREADS, smem, stream>>>(p);
-        OSB_LAUNCH_CHECK();
-        return OSB_OK;
-    }
-    const size_t smem = rollout_smem_bytes(On);
-    static size_t attr = 0;
-    if (smem > attr) {
-        OSB_CUDA(cudaFuncSetAttribute(rollout_step_kernel<EXT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = smem;
-    }
-    rollout_step_kernel<EXT, true><<<dim3((p.N + RT - 1) / RT, 1), NTHREADS, smem, stream>>>(p);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
-}
-
-static int sm_count() {
-    static int n_sm = 0;
-    if (!n_sm) { int dev = 0; OSB_CUDA(cudaGetDevice(&dev)); OSB_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev)); }
-    return n_sm;
-}
 
 extern "C" {
 
@@ -2110,20 +2023,16 @@ int osb_eval_synthetic(int O, int A, int max_episode_steps, unsigned seed, unsig
     // every env's first episode starts from a reset, its observations pushed as one batch (a vector env's reset)
     env_reset_kernel<<<(N + RT - 1) / RT, NTHREADS, 0, s>>>(p.es, p.st, p.ns, p.sa, N);
     OSB_LAUNCH_CHECK();
-    const int On = O + (safety ? 1 : 0);
-    if (!per_step && (precision == 1 || precision == 2) && On <= 64 && (N + RTC - 1) / RTC <= sm_count()) {
-        static unsigned int* d_bar = nullptr;
-        if (!d_bar) OSB_CUDA(cudaMalloc(&d_bar, 64));
-        p.bar_ctr = d_bar; p.bar_flag = d_bar + 1;
+    if (!per_step && persistent_fits(p, 1)) {   // p.T bounds the persistent kernel's steps
         p.t = 0;
-        return launch_eval<false>(p, s, true);
+        return launch_rollout<false, true>(p, s, true);
     }
     static int* h_done = nullptr;
     if (!h_done) OSB_CUDA(cudaMallocHost(&h_done, sizeof(int)));
     constexpr int CHECK_EVERY = 16;     // the done word is read after every 16 launches; later launches return at once
     for (long long t = 0; t < steps; ++t) {
         p.t = (int)(t & 1);     // the parity of the state buffers (T = the step bound keeps every launch a full step)
-        if (int rc = launch_eval<false>(p, s, false)) return rc;
+        if (int rc = launch_rollout<false, true>(p, s)) return rc;
         if ((t + 1) % CHECK_EVERY == 0 && t + 1 < steps) {
             OSB_CUDA(cudaMemcpyAsync(h_done, ctr, sizeof(int), cudaMemcpyDeviceToHost, s));
             OSB_CUDA(cudaStreamSynchronize(s));
@@ -2151,7 +2060,7 @@ int osb_eval_ext_act(int O, int A, int obs_normalize, int N, int t, const float*
     p.theta = theta; p.t = t & 1; p.T = 2;
     p.act_lo = act_lo; p.act_hi = act_hi; p.act_env = act_env;
     p.ev.left = const_cast<int*>(left); p.ev.ctr = const_cast<int*>(ctr); p.ev.act_out = act_out;
-    return launch_eval<true>(p, (cudaStream_t)stream, false);
+    return launch_rollout<true, true>(p, (cudaStream_t)stream);
 }
 
 int osb_eval_ext_observe(int O, int N, int t, int obs_normalize, int is_reset, const float* next_obs, const float* rew,
@@ -2286,7 +2195,7 @@ static int ext_act(int O, int A, int obs_normalize, int N, int T, int t, unsigne
     p.t = t; p.T = T; p.is_tail = (t == T) ? 1 : 0;
     p.act_lo = act_lo; p.act_hi = act_hi; p.act_env = act_env;
     p.epoch_dev = epoch_dev;
-    return launch_step<true>(p, (cudaStream_t)stream);
+    return launch_rollout<true, false>(p, (cudaStream_t)stream);
 }
 
 static __global__ void ext_epoch_advance_kernel(unsigned* epoch_dev) { *epoch_dev += 1u; }
@@ -2326,7 +2235,7 @@ int osb_ext_epoch_advance(unsigned* epoch_dev, void* stream) {
 int osb_ext_prepare(int O, int A, int N, int precision) {
     OSB_CHECK_ARG(O > 0 && A > 0 && A <= OUTP && N > 0, "bad dims (need 0 < A <= 16)");
     StepArgs p = ext_step_args(O, A, 0, N, precision);
-    return launch_step<true>(p, nullptr, true);
+    return launch_rollout<true, false>(p, nullptr, false, true);
 }
 
 }  // extern "C"

@@ -11,6 +11,7 @@
 //   3. row_apply_kernel   : x <- clamp((x - mean_t) / std_t, -clip, clip) with the statistics valid
 //                           right after step t's push (count <= 1: passthrough, normalizer.py:L104).
 #include "common.cuh"
+#include "normalizer.cuh"
 
 namespace osb {
 
@@ -55,15 +56,11 @@ __global__ void row_chan_kernel(const float* __restrict__ moments, int T, int N,
         const float mean_raw = moments[2 * t], sumq_raw = moments[2 * t + 1];
         if (c == 0) {                     // Normalizer._first (normalizer.py:L117-125)
             mean = mean_raw; sumsq = sumq_raw; c = N;
-        } else {                          // normalizer.py:L126-135
-            const long long cn = c + N;
-            const float delta = __fadd_rn(mean_raw, -mean);
-            mean = __fadd_rn(mean, __fdiv_rn(__fmul_rn(delta, (float)N), (float)cn));
-            const float corr = __fdiv_rn(__fmul_rn(__fmul_rn(__fmul_rn(delta, delta), (float)c), (float)N), (float)cn);
-            sumsq = __fadd_rn(sumsq, __fadd_rn(sumq_raw, corr));
-            c = cn;
+        } else {
+            norm_push_moments(mean, sumsq, c, N, mean_raw, sumq_raw);   // fp32 -> fp64 -> fp32 is exact
+            c += N;
         }
-        stdv = fmaxf(sqrtf(__fdiv_rn(sumsq, (float)(c - 1))), 1e-2f);   // L136-138 (c == 1: inf/nan -> unused)
+        stdv = norm_std(sumsq, c);        // c == 1: inf/nan -> unused
         row_stats[2 * t] = mean;
         row_stats[2 * t + 1] = (c <= 1) ? -1.f : stdv;
     }
