@@ -489,7 +489,8 @@ int osb_umma_selftest(const float* A, const float* B, int M, int N, int K, int a
 /* Split-bf16 ("bf16x3") building blocks of the parity-grade tensor-core mode (csrc/x3.cuh):
  * one single-warpgroup GEMM D = A * B^T with A [M][K], B [N][K] (row-major fp32 in global memory), each operand
  * staged as three bf16 tiles (SW128 or SW32) consumed K-major or MN-major; out[128][N] = dump of the
- * accumulator lanes (tests/test_x3_gpu.py). */
+ * accumulator lanes (tests/test_x3_gpu.py).  (M, N, K, a_mn, b_mn, b_ones) must be one of the GEMM shapes the
+ * kernels issue (csrc/x3_selftest.cu); any other shape is refused. */
 int osb_x3_selftest(const float* A, const float* B, int M, int N, int K, int a_mn, int b_mn, int a_sw,
                     int b_sw, int b_ones, float* out, void* stream);
 int osb_x3_debug_buffer(long long* buf);

@@ -96,7 +96,6 @@ __global__ void __launch_bounds__(FNT, 1) fvp_tangent_x3_kernel(FvpX3Args p) {
     const uint64_t dA0 = desc128(sbase + FO_A0), dA1 = desc128(sbase + FO_A1);
     const uint64_t dW1 = desc128(sbase + FO_W1), dV1 = desc128(sbase + FO_V1), dW2 = desc128(sbase + FO_W2), dV2 = desc128(sbase + FO_V2);
     const uint64_t dW3 = desc128(sbase + FO_W3), dV3 = desc128(sbase + FO_V3);
-    const uint32_t id_fwd = idesc_bf16(128, 64, 0, 0), id_out = idesc_bf16(128, 16, 0, 0);
 
     const long long nrows = (p.total + p.stride - 1) / p.stride;
     const long long ntiles = (nrows + FT - 1) / FT;
@@ -142,9 +141,9 @@ __global__ void __launch_bounds__(FNT, 1) fvp_tangent_x3_kernel(FvpX3Args p) {
         fence_async_smem();
         __syncthreads();
         // ---- layer 1: Z1 = X W1^T, T1 = X V1^T ------------------------------------------------------------------------
-        if (warp < 4) {
-            gemm_x3(tm, C_Z, dA0, F_SUB, 32u, dW1, F_WSUB, 32u, id_fwd, 4, false);
-            gemm_x3(tm, C_T, dA0, F_SUB, 32u, dV1, F_WSUB, 32u, id_fwd, 4, false);
+        if (warpgroup_index() == 0) {
+            gemm_x3<128, 64, 4, 0, 0>(tm, C_Z, dA0, F_SUB, 32u, dW1, F_WSUB, 32u, false);
+            gemm_x3<128, 64, 4, 0, 0>(tm, C_T, dA0, F_SUB, 32u, dV1, F_WSUB, 32u, false);
             mma_commit_a(bar);
         }
         mbar_wait_a(bar, phase); phase ^= 1;
@@ -166,10 +165,10 @@ __global__ void __launch_bounds__(FNT, 1) fvp_tangent_x3_kernel(FvpX3Args p) {
         fence_async_smem();
         __syncthreads();
         // ---- layer 2: Z2 = H1 W2^T, T2 = dH1 W2^T + H1 V2^T -------------------------------------------------------------
-        if (warp < 4) {
-            gemm_x3(tm, C_Z, dA0, F_SUB, 32u, dW2, F_WSUB, 32u, id_fwd, 4, false);
-            gemm_x3(tm, C_T, dA1, F_SUB, 32u, dW2, F_WSUB, 32u, id_fwd, 4, false);
-            gemm_x3(tm, C_T, dA0, F_SUB, 32u, dV2, F_WSUB, 32u, id_fwd, 4, true);
+        if (warpgroup_index() == 0) {
+            gemm_x3<128, 64, 4, 0, 0>(tm, C_Z, dA0, F_SUB, 32u, dW2, F_WSUB, 32u, false);
+            gemm_x3<128, 64, 4, 0, 0>(tm, C_T, dA1, F_SUB, 32u, dW2, F_WSUB, 32u, false);
+            gemm_x3<128, 64, 4, 0, 0>(tm, C_T, dA0, F_SUB, 32u, dV2, F_WSUB, 32u, true);
             mma_commit_a(bar);
         }
         gather(tile + gridDim.x);                            // next tile's rows fly under layers 2 and 3
@@ -192,9 +191,9 @@ __global__ void __launch_bounds__(FNT, 1) fvp_tangent_x3_kernel(FvpX3Args p) {
         fence_async_smem();
         __syncthreads();
         // ---- layer 3: dmu = dH2 W3^T + H2 V3^T + bv3 ---------------------------------------------------------------------
-        if (warp < 4) {
-            gemm_x3(tm, C_OUT, dA1, F_SUB, 32u, dW3, F_W3SUB, 32u, id_out, 4, false);
-            gemm_x3(tm, C_OUT, dA0, F_SUB, 32u, dV3, F_W3SUB, 32u, id_out, 4, true);
+        if (warpgroup_index() == 0) {
+            gemm_x3<128, 16, 4, 0, 0>(tm, C_OUT, dA1, F_SUB, 32u, dW3, F_W3SUB, 32u, false);
+            gemm_x3<128, 16, 4, 0, 0>(tm, C_OUT, dA0, F_SUB, 32u, dV3, F_W3SUB, 32u, true);
             mma_commit_a(bar);
         }
         const long long row = (h == 0) ? sRow[s_row] : -1;

@@ -197,6 +197,7 @@ __device__ __forceinline__ void tc_forward(uint32_t base, const umma::Acc& tm, u
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q = warp & 3, h = warp >> 2;
     const uint32_t lane_base = (uint32_t)(q * 32) << 16;
+    const bool mma_wg = warpgroup_index() == 0;         // warpgroup 0 issues the MMAs
     if constexpr (X3) {
         const uint64_t dAct = x3::desc128(base + T::X), dW1 = x3::desc128(base + T::W1), dW2 = x3::desc128(base + T::W2),
                        dW3 = x3::desc128(base + T::W3);
@@ -214,22 +215,22 @@ __device__ __forceinline__ void tc_forward(uint32_t base, const umma::Acc& tm, u
             __syncthreads();
         };
         stage_chunk(0);
-        if (warp < 4) {
-            x3::gemm_x3(tm, TC_C_Z, dAct, T::SUB, 32u, dW1, T::WSUB, 32u, x3::idesc_bf16(128, 64, 0, 0), 4, false);
+        if (mma_wg) {
+            x3::gemm_x3<128, 64, 4, 0, 0>(tm, TC_C_Z, dAct, T::SUB, 32u, dW1, T::WSUB, 32u, false);
             mma_commit(bar);
         }
         mbar_wait(bar, phase); phase ^= 1;
         after(1);
         hidden(sB1);
-        if (warp < 4) {
-            x3::gemm_x3(tm, TC_C_Z, dAct, T::SUB, 32u, dW2, T::WSUB, 32u, x3::idesc_bf16(128, 64, 0, 0), 4, false);
+        if (mma_wg) {
+            x3::gemm_x3<128, 64, 4, 0, 0>(tm, TC_C_Z, dAct, T::SUB, 32u, dW2, T::WSUB, 32u, false);
             mma_commit(bar);
         }
         mbar_wait(bar, phase); phase ^= 1;
         after(2);
         hidden(sB2);
-        if (warp < 4) {
-            x3::gemm_x3(tm, TC_C_OUT, dAct, T::SUB, 32u, dW3, T::W3SUB, 32u, x3::idesc_bf16(128, 16, 0, 0), 4, false);
+        if (mma_wg) {
+            x3::gemm_x3<128, 16, 4, 0, 0>(tm, TC_C_OUT, dAct, T::SUB, 32u, dW3, T::W3SUB, 32u, false);
             mma_commit(bar);
         }
         mbar_wait(bar, phase); phase ^= 1;
@@ -248,16 +249,16 @@ __device__ __forceinline__ void tc_forward(uint32_t base, const umma::Acc& tm, u
 #pragma unroll 1
         for (int c = 0; c < nchunks; ++c) {
             stage_chunk(c);
-            if (warp < 4) { tc_gemm(tm, TC_C_Z, sX, TC_ROWS, base + T::W1, 64, 128, 64, 64, c > 0); mma_commit(bar); }
+            if (mma_wg) { tc_gemm(tm, TC_C_Z, sX, TC_ROWS, base + T::W1, 64, 128, 64, 64, c > 0); mma_commit(bar); }
             mbar_wait(bar, phase); phase ^= 1;
         }
         after(1);
         hidden(sB1, sH1);
-        if (warp < 4) { tc_gemm(tm, TC_C_Z, sH1, TC_ROWS, base + T::W2, 64, 128, 64, 64, false); mma_commit(bar); }
+        if (mma_wg) { tc_gemm(tm, TC_C_Z, sH1, TC_ROWS, base + T::W2, 64, 128, 64, 64, false); mma_commit(bar); }
         mbar_wait(bar, phase); phase ^= 1;
         after(2);
         hidden(sB2, sX);
-        if (warp < 4) { tc_gemm(tm, TC_C_OUT, sX, TC_ROWS, base + T::W3, 16, 128, 16, 64, false); mma_commit(bar); }
+        if (mma_wg) { tc_gemm(tm, TC_C_OUT, sX, TC_ROWS, base + T::W3, 16, 128, 16, 64, false); mma_commit(bar); }
         mbar_wait(bar, phase); phase ^= 1;
         after(3);
     }

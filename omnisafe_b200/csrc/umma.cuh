@@ -104,10 +104,19 @@ __device__ __forceinline__ void wgmma_bf16_n16(float (&d)[8], uint64_t a, uint64
         : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB) : "memory");
 }
 
+// Warpgroup of the calling thread, taken from lane 0 so that ptxas can prove a branch on it uniform over the warp.
+// A wgmma-issuing branch must test this value: on a test of threadIdx.x itself ptxas assumes a divergent path and
+// waits on every wgmma before issuing the next (C7520).
+__device__ __forceinline__ int warpgroup_index() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0); }
+
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+// wait until at most N committed groups of this warpgroup are pending
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void wg_commit_wait() {
-    asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory");
-    asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory");
+    wg_commit();
+    wg_wait<0>();
 }
 template <int R>
 __device__ __forceinline__ void acc_fence(float (&d)[R]) {
@@ -126,18 +135,37 @@ __device__ __forceinline__ Acc acc_cta(float* scratch, uint32_t pitch) {
     return Acc{scratch + cta * 128 * pitch, pitch};
 }
 
-// Writes (or adds) the m64 x (8 NJ) fragment d of this warpgroup thread, rows 64 half .. 64 half + 63 of an
-// M-row product, columns from the accumulator address taddr.
+// Where row rr (0 or 1) of the m64 fragment of this warpgroup thread starts in the image: rows 64 half .. 64 half + 63
+// of an M-row product, columns from the accumulator address taddr.  Element (rr, j, e) lies at [8 j + e].
+__device__ __forceinline__ float* frag_row(const Acc& acc, uint32_t taddr, int M, int half, int rr) {
+    const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+    const int m = 64 * half + 16 * w + (l >> 2) + 8 * rr;
+    const uint32_t lane = (taddr >> 16) + (uint32_t)(M == 128 ? m : 32 * (m >> 4) + (m & 15));
+    return acc.p + (size_t)lane * acc.pitch + (taddr & 0xFFFFu) + 2u * (uint32_t)(l & 3);
+}
+
+// Reads the image values under the m64 x (8 NJ) fragment, in the fragment's register order.
+template <int NJ>
+__device__ __forceinline__ void frag_load(const Acc& acc, uint32_t taddr, int M, int half, float (&o)[4 * NJ]) {
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+        const float* row = frag_row(acc, taddr, M, half, rr);
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+            const float2 v = *reinterpret_cast<const float2*>(row + 8 * j);
+            o[4 * j + 2 * rr] = v.x;
+            o[4 * j + 2 * rr + 1] = v.y;
+        }
+    }
+}
+
+// Writes (or adds) the m64 x (8 NJ) fragment d of this warpgroup thread (see frag_row).
 template <int NJ>
 __device__ __forceinline__ void frag_store(const Acc& acc, uint32_t taddr, int M, int half, const float (&d)[4 * NJ],
                                            bool accumulate) {
-    const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
-    const uint32_t col = (taddr & 0xFFFFu) + 2u * (uint32_t)(l & 3);
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
-        const int m = 64 * half + 16 * w + (l >> 2) + 8 * rr;
-        const uint32_t lane = (taddr >> 16) + (uint32_t)(M == 128 ? m : 32 * (m >> 4) + (m & 15));
-        float* row = acc.p + (size_t)lane * acc.pitch + col;
+        float* row = frag_row(acc, taddr, M, half, rr);
 #pragma unroll
         for (int j = 0; j < NJ; ++j) {
             float2 v = make_float2(d[4 * j + 2 * rr], d[4 * j + 2 * rr + 1]);

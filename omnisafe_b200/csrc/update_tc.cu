@@ -299,7 +299,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
                 fence_async_smem();
                 __syncthreads();
                 if (c + 1 < nchunks) load_chunk(sRow, c + 1);      // next chunk's rows fly during the MMAs
-                if (warp < 4) {
+                if (warpgroup_index() == 0) {
                     tc_gemm(tm, C_Z, B0, TT, sW1, 64, 128, 64, 64, c > 0);
                     tc_gemm(tm, C_ZT, sW1, 64, B0, TT, 64, 128, 64, c > 0);
                     mma_commit(&bar);
@@ -307,7 +307,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
                 mbar_wait(&bar, phase); phase ^= 1;
             }
         } else {
-            if (warp < 4) {
+            if (warpgroup_index() == 0) {
                 tc_gemm(tm, C_Z, B0, TT, sW1, 64, 128, 64, 64, false);
                 tc_gemm(tm, C_ZT, sW1, 64, B0, TT, 64, 128, 64, false);
                 mma_commit(&bar);
@@ -324,7 +324,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
         fence_async_smem();
         __syncthreads();
         // ---- P2: Z2 (-> C_Z) and Z2^T (-> C_ZT2); warps 4-15 run the H1^T epilogue while warpgroup 0 computes them ----
-        if (warp < 4) {
+        if (warpgroup_index() == 0) {
             tc_gemm(tm, C_Z, B2, TT, sW2, 64, 128, 64, 64, false);
             tc_gemm(tm, C_ZT2, sW2, 64, B2, TT, 64, 128, 64, false);
             mma_commit(&bar);
@@ -350,7 +350,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
         fence_async_smem();
         __syncthreads();
         // ---- P3: OUT -> loss -> dOUT (B4, cols 0..31) --------------------------------------------
-        if (warp < 4) {
+        if (warpgroup_index() == 0) {
             tc_gemm(tm, C_OUT, B0, TT, sW3, 16, 128, 16, 64, false);
             mma_commit(&bar);
         }
@@ -460,7 +460,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             continue;
         }
         // ---- P4: dZ2, dZ2^T and dW3^T += H2^T dOUT ------------------------------------------------
-        if (warp < 4) {
+        if (warpgroup_index() == 0) {
             tc_gemm(tm, C_Z, B4, TT, sW3T, 64, 128, 64, 16, false);
             tc_gemm(tm, C_ZT, sW3T, 64, B4, TT, 64, 128, 16, false);
             tc_gemm(tm, C_DW3, B2, 64, B4 + 16384u, 16, 64, 16, 128, !first_tile);
@@ -491,7 +491,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
         // ---- P5: dW2 += dZ2^T H1 ; dZ1^T = W2^T dZ2^T --------------------------------------------
         if (CHUNKED) load_chunk(sRow, 0);             // chunk 0 of THIS tile again: P6 needs X^T chunk by chunk
         else if (vec && has_next) prefetch_x(sRowNext);    // global loads of the next tile fly during P5 / P6
-        if (warp < 4) {
+        if (warpgroup_index() == 0) {
             tc_gemm(tm, C_DW2, B4, 64, B3, 64, 64, 64, 128, !first_tile);
             tc_gemm(tm, C_ZT, sW2T, 64, B2, TT, 64, 128, 64, false);
             mma_commit(&bar);
@@ -526,7 +526,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
                 fence_async_smem();
                 __syncthreads();                     // (c > 0) every read of the previous chunk's accumulator is done
                 if (c + 1 < nchunks) load_chunk(sRow, c + 1);
-                if (warp < 4) {
+                if (warpgroup_index() == 0) {
                     tc_gemm(tm, C_DW1, B0, 64, B1, 64, 64, 64, 128, false);
                     mma_commit(&bar);
                 }
@@ -562,7 +562,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             }
             if (has_next) load_chunk(sRowNext, 0);
         } else {
-        if (warp < 4) {
+        if (warpgroup_index() == 0) {
             tc_gemm(tm, C_DW1, B0, 64, B1, 64, 64, 64, 128, !first_tile);
             mma_commit(&bar);
         }
@@ -821,7 +821,7 @@ __global__ void __launch_bounds__(NTC, 1) fvp_tangent_tc_kernel(FvpTanArgs p) {
                 __syncthreads();
                 if (c + 1 < nchunks) load_chunk(sRow, c + 1);
                 else if (has_next) load_chunk(sRowNext, 0);
-                if (warp < 4) {
+                if (warpgroup_index() == 0) {
                     tc_gemm(tm, F_Z1, B0, TT, sWV1, 128, 128, 128, 64, c > 0);
                     mma_commit(&bar);
                 }
@@ -829,7 +829,7 @@ __global__ void __launch_bounds__(NTC, 1) fvp_tangent_tc_kernel(FvpTanArgs p) {
             }
         } else {
             if (vec4 && has_next) prefetch_x(sRowNext);      // next tile's rows fly during the three layers
-            if (warp < 4) {
+            if (warpgroup_index() == 0) {
                 tc_gemm(tm, F_Z1, B0, TT, sWV1, 128, 128, 128, 64, false);
                 mma_commit(&bar);
             }
@@ -851,7 +851,7 @@ __global__ void __launch_bounds__(NTC, 1) fvp_tangent_tc_kernel(FvpTanArgs p) {
         fence_async_smem();
         __syncthreads();
         // ---- layer 2: [Z2 | H1 V2^T + dH1 W2^T] ------------------------------------------------------
-        if (warp < 4) {
+        if (warpgroup_index() == 0) {
             tc_gemm(tm, F_Z2, B1, TT, sWV2, 128, 128, 128, 64, false);
             tc_gemm(tm, F_Z2 + 64, B2, TT, sWV2, 128, 128, 64, 64, true);
             mma_commit(&bar);
@@ -873,7 +873,7 @@ __global__ void __launch_bounds__(NTC, 1) fvp_tangent_tc_kernel(FvpTanArgs p) {
         fence_async_smem();
         __syncthreads();
         // ---- output tangent: dmu = H2 V3^T + dH2 W3^T + vb3 -------------------------------------------
-        if (warp < 4) {
+        if (warpgroup_index() == 0) {
             tc_gemm(tm, F_DMU, B0, TT, sWV3 + 2048u, 32, 128, 16, 64, false);
             tc_gemm(tm, F_DMU, B1, TT, sWV3, 32, 128, 16, 64, true);
             mma_commit(&bar);

@@ -198,7 +198,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
     // partial gradients of this CTA: FUSED -> private aligned layout, else the [CTA][P] layout optim_fused reads
     float* gout = FUSED ? p.gpart + ((size_t)((gridDim.y == 1 ? 0 : net) * G + (int)blockIdx.x)) * PSTR
                         : p.gpart + (size_t)blockIdx.x * p.P + noff;
-    const bool is_mma_warp = warp >= NEPI / 32;        // the four warps of the MMA-issue warpgroup
+    const bool is_mma_warp = warpgroup_index() == NEPI / 128;     // the four warps of the MMA-issue warpgroup
     const int batch = FUSED ? p.batch_size : p.b.mb_count;
     const int n_mb = (p.b.mb_count + batch - 1) / batch;
     const bool ones_col = O < 64;          // bias of layer 1 / db1 ride in the GEMMs (see stage_weights_x3)
@@ -227,8 +227,6 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
         const uint64_t dX = desc128(sbase + OFF_X), dH1 = desc128(sbase + OFF_H1), dH2 = desc128(sbase + OFF_H2);
         const uint64_t dD = desc32(sbase + OFF_D), dW1 = desc128(sbase + OFF_W1), dW2 = desc128(sbase + OFF_W2);
         const uint64_t dW3 = desc128(sbase + OFF_W3), dOnes = desc32(sbase + OFF_ONES);
-        const uint32_t id_fwd = idesc_bf16(128, 64, 0, 0), id_out = idesc_bf16(128, 16, 0, 0), id_bwd = idesc_bf16(128, 64, 0, 1);
-        const uint32_t id_dw = idesc_bf16(64, 64, 1, 1), id_dw16 = idesc_bf16(64, 16, 1, 1);
         int it = 0;
 #pragma unroll 1
         for (int mb = 0; mb < n_mb; ++mb) {
@@ -243,47 +241,47 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll 1
                 for (int ph = 0; ph < 2; ++ph) {
                     mbar_wait_a(bar(RDY_X0 + ph), par);
-                    gemm_x3(tm, T_ZA, desc_add(dX, 64u * ph), ACT_SUB, 32u, desc_add(dW1, 64u * ph), W_SUB, 32u, id_fwd, 2, ph > 0);
+                    gemm_x3<128, 64, 2, 0, 0>(tm, T_ZA, desc_add(dX, 64u * ph), ACT_SUB, 32u, desc_add(dW1, 64u * ph), W_SUB, 32u, ph > 0);
                 }
                 mma_commit_a(bar(DONE_C1));
                 // db2 of the PREVIOUS tile (dZ2 still sits in the H2 buffer until this tile's E2): runs under E1,
                 // completes before Z2 (in-order pipe), so DONE_C2 covers it
-                if (!first && !(!FUSED && p.forward_only)) gemm_x3(tm, T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, id_dw16, 8, tile != (int)blockIdx.x + G);
+                if (!first && !(!FUSED && p.forward_only)) gemm_x3<64, 16, 8, 1, 1, true>(tm, T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, tile != (int)blockIdx.x + G);
                 // Z2 = H1 W2^T
 #pragma unroll 1
                 for (int ph = 0; ph < 2; ++ph) {
                     mbar_wait_a(bar(RDY_H1_0 + ph), par);
-                    gemm_x3(tm, T_ZB, desc_add(dH1, 64u * ph), ACT_SUB, 32u, desc_add(dW2, 64u * ph), W_SUB, 32u, id_fwd, 2, ph > 0);
+                    gemm_x3<128, 64, 2, 0, 0>(tm, T_ZB, desc_add(dH1, 64u * ph), ACT_SUB, 32u, desc_add(dW2, 64u * ph), W_SUB, 32u, ph > 0);
                 }
                 mma_commit_a(bar(DONE_C2));
                 // OUT = H2 W3^T
 #pragma unroll 1
                 for (int ph = 0; ph < 2; ++ph) {
                     mbar_wait_a(bar(RDY_H2_0 + ph), par);
-                    gemm_x3(tm, T_OUT, desc_add(dH2, 64u * ph), ACT_SUB, 32u, desc_add(dW3, 64u * ph), W3_SUB, 32u, id_out, 2, ph > 0);
+                    gemm_x3<128, 16, 2, 0, 0>(tm, T_OUT, desc_add(dH2, 64u * ph), ACT_SUB, 32u, desc_add(dW3, 64u * ph), W3_SUB, 32u, ph > 0);
                 }
                 mma_commit_a(bar(DONE_C3));
                 if (!FUSED && p.forward_only) continue;              // statistics pass (FOCOPS mask mean): no backward
                 // dZ2' = dOUT W3 ; dW3^T += H2^T dOUT
                 mbar_wait_a(bar(RDY_D), par);
-                gemm_x3(tm, T_ZA, dD, D_SUB, 32u, dW3, W3_SUB, 2048u, id_bwd, 1, false);
+                gemm_x3<128, 64, 1, 0, 1>(tm, T_ZA, dD, D_SUB, 32u, dW3, W3_SUB, 2048u, false);
                 mma_commit_a(bar(DONE_C4A));
-                gemm_x3(tm, T_DW3, dH2, ACT_SUB, 2048u, dD, D_SUB, 512u, id_dw16, 8, !first);
+                gemm_x3<64, 16, 8, 1, 1>(tm, T_DW3, dH2, ACT_SUB, 2048u, dD, D_SUB, 512u, !first);
                 mma_commit_a(bar(DONE_C4B));
                 // dZ1' = dZ2 W2 ; dW2 += dZ2^T H1
 #pragma unroll 1
                 for (int ph = 0; ph < 2; ++ph) {
                     mbar_wait_a(bar(RDY_DZ2_0 + ph), par);
-                    gemm_x3(tm, T_ZB, desc_add(dH2, 64u * ph), ACT_SUB, 32u, desc_add(dW2, 4096u * ph), W_SUB, 2048u, id_bwd, 2, ph > 0);
+                    gemm_x3<128, 64, 2, 0, 1>(tm, T_ZB, desc_add(dH2, 64u * ph), ACT_SUB, 32u, desc_add(dW2, 4096u * ph), W_SUB, 2048u, ph > 0);
                 }
                 mma_commit_a(bar(DONE_C5A));
-                gemm_x3(tm, T_DW2, dH2, ACT_SUB, 2048u, dH1, ACT_SUB, 2048u, id_dw, 8, !first);
+                gemm_x3<64, 64, 8, 1, 1>(tm, T_DW2, dH2, ACT_SUB, 2048u, dH1, ACT_SUB, 2048u, !first);
                 mma_commit_a(bar(DONE_C5B));
                 // dW1 += dZ1^T X (column 63 = db1 with the ones column) ; last tile of the minibatch: its own db2
                 mbar_wait_a(bar(RDY_DZ1), par);
-                gemm_x3(tm, T_DW1, dH1, ACT_SUB, 2048u, dX, ACT_SUB, 2048u, id_dw, 8, !first);
-                if (!ones_col) gemm_x3(tm, T_DB1, dH1, ACT_SUB, 2048u, dOnes, 0u, 0u, id_dw16, 8, !first);
-                if (last) gemm_x3(tm, T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, id_dw16, 8, !first);
+                gemm_x3<64, 64, 8, 1, 1>(tm, T_DW1, dH1, ACT_SUB, 2048u, dX, ACT_SUB, 2048u, !first);
+                if (!ones_col) gemm_x3<64, 16, 8, 1, 1, true>(tm, T_DB1, dH1, ACT_SUB, 2048u, dOnes, 0u, 0u, !first);
+                if (last) gemm_x3<64, 16, 8, 1, 1, true>(tm, T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, !first);
                 mma_commit_a(bar(DONE_C6));
             }
         }

@@ -38,95 +38,85 @@ __device__ __forceinline__ uint64_t desc32(uint32_t saddr) { return desc_make(sa
 // descriptor + byte offset (start-address field only; all tiles live below 256 KB of shared memory)
 __device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t bytes) { return d + (uint64_t)(bytes >> 4); }
 
-// GEMM shape word, bf16 x bf16 -> fp32: M (64 or 128), N, and which operands are read MN-major
-__device__ __forceinline__ constexpr uint32_t idesc_bf16(int M, int N, int a_mn, int b_mn) {
-    return ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// d, hidden from loop-invariant code motion (see gemm_x3)
+__device__ __forceinline__ uint64_t desc_fresh(uint64_t d) {
+    asm volatile("" : "+l"(d));
+    return d;
 }
 
-// One m64 x N block over nk k-steps of 16, six split products per k-step (three when B is exact).
-template <int TA, int TB, int NJ>
+// One m64 x (8 NJ) block over NK k-steps of 16, six split products per k-step (three when B is exact), small terms
+// first: one fence, an unbroken run of wgmmas and one commit.  The caller waits on the group.
+template <int TA, int TB, int NJ, int NK, bool B_EXACT>
 __device__ __forceinline__ void x3_block(float (&d)[4 * NJ], uint64_t a0, uint32_t asplit, uint32_t akstep, uint64_t b0,
-                                         uint32_t bsplit, uint32_t bkstep, int nk) {
+                                         uint32_t bsplit, uint32_t bkstep) {
+    auto mma = [&](uint64_t a, uint64_t b, uint32_t s) {
+        if constexpr (NJ == 8) wgmma_bf16_n64<TA, TB>(d, a, b, s);
+        else wgmma_bf16_n16<TA, TB>(d, a, b, s);
+    };
     wg_fence();
     acc_fence(d);
-#pragma unroll 1
-    for (int ks = 0; ks < nk; ++ks) {
+#pragma unroll
+    for (int ks = 0; ks < NK; ++ks) {
         const uint64_t a = desc_add(a0, (uint32_t)ks * akstep), b = desc_add(b0, (uint32_t)ks * bkstep);
         const uint64_t a1 = desc_add(a, asplit), a2 = desc_add(a, 2 * asplit);
         const uint32_t s = ks > 0 ? 1u : 0u;
-        if constexpr (NJ == 8) {
-            if (bsplit == 0) {
-                wgmma_bf16_n64<TA, TB>(d, a2, b, s);
-                wgmma_bf16_n64<TA, TB>(d, a1, b, 1u);
-                wgmma_bf16_n64<TA, TB>(d, a, b, 1u);
-            } else {
-                const uint64_t b1 = desc_add(b, bsplit), b2 = desc_add(b, 2 * bsplit);
-                wgmma_bf16_n64<TA, TB>(d, a2, b, s);
-                wgmma_bf16_n64<TA, TB>(d, a, b2, 1u);
-                wgmma_bf16_n64<TA, TB>(d, a1, b1, 1u);
-                wgmma_bf16_n64<TA, TB>(d, a1, b, 1u);
-                wgmma_bf16_n64<TA, TB>(d, a, b1, 1u);
-                wgmma_bf16_n64<TA, TB>(d, a, b, 1u);
-            }
+        if constexpr (B_EXACT) {
+            mma(a2, b, s);
+            mma(a1, b, 1u);
+            mma(a, b, 1u);
         } else {
-            if (bsplit == 0) {
-                wgmma_bf16_n16<TA, TB>(d, a2, b, s);
-                wgmma_bf16_n16<TA, TB>(d, a1, b, 1u);
-                wgmma_bf16_n16<TA, TB>(d, a, b, 1u);
-            } else {
-                const uint64_t b1 = desc_add(b, bsplit), b2 = desc_add(b, 2 * bsplit);
-                wgmma_bf16_n16<TA, TB>(d, a2, b, s);
-                wgmma_bf16_n16<TA, TB>(d, a, b2, 1u);
-                wgmma_bf16_n16<TA, TB>(d, a1, b1, 1u);
-                wgmma_bf16_n16<TA, TB>(d, a1, b, 1u);
-                wgmma_bf16_n16<TA, TB>(d, a, b1, 1u);
-                wgmma_bf16_n16<TA, TB>(d, a, b, 1u);
-            }
+            const uint64_t b1 = desc_add(b, bsplit), b2 = desc_add(b, 2 * bsplit);
+            mma(a2, b, s);
+            mma(a, b2, 1u);
+            mma(a1, b1, 1u);
+            mma(a1, b, 1u);
+            mma(a, b1, 1u);
+            mma(a, b, 1u);
         }
     }
-    wg_commit_wait();
-    acc_fence(d);
+    wg_commit();
 }
 
-template <int TA, int TB>
-__device__ __forceinline__ void gemm_x3_t(const Acc& acc, uint32_t d_addr, uint64_t a0, uint32_t asplit, uint32_t akstep,
-                                          uint64_t b0, uint32_t bsplit, uint32_t bkstep, int M, int N, int nk,
-                                          bool accumulate) {
+// D[acc] (+)= A * B over NK k-steps of 16, with the six split products (small terms first); called by all 128 threads
+// of one warpgroup.
+//   M = 64 or 128, N = 16 or 64; TA / TB: A / B read MN-major (an MN-major A has M = 64); B_EXACT: B is exactly
+//   representable in bf16 (e.g. the ones tile), only the three A terms are issued and bsplit is not read.
+//   a0 / b0: descriptors of the hi sub-tiles at k-step 0; asplit / bsplit: bytes between sub-tiles;
+//   akstep / bkstep: bytes per k-step (K-major: 32; MN-major: 16 rows * pitch).
+// M = 128 issues both m64 halves before draining the first: half 0 is stored while half 1 runs.  M = 64 reads the
+// image values it adds to before waiting on its MMAs.  Either way the stored value is d, or d + old, as one fp32 add.
+template <int M, int N, int NK, int TA, int TB, bool B_EXACT = false>
+__device__ __forceinline__ void gemm_x3(const Acc& acc, uint32_t d_addr, uint64_t a0, uint32_t asplit, uint32_t akstep,
+                                        uint64_t b0, uint32_t bsplit, uint32_t bkstep, bool accumulate) {
+    static_assert((M == 64 || (M == 128 && TA == 0)) && (N == 16 || N == 64), "unsupported bf16x3 GEMM shape");
+    constexpr int NJ = N / 8;
+    // Every descriptor of the unrolled k-steps is invariant in the callers' tile loops; computed once there and held
+    // across them, they would not fit in registers next to the accumulators.  Derive them afresh at every call.
+    a0 = desc_fresh(a0);
+    b0 = desc_fresh(b0);
     // rows 64..127 of a K-major A: 64 rows further down the tile (row pitch 128 B for SW128, 32 B for SW32)
     const uint32_t a_half_bytes = 64u * (((a0 >> 61) & 7u) == 2u ? 128u : 32u);
-#pragma unroll 1
-    for (int half = 0; half < M / 64; ++half) {
-        const uint64_t ah = desc_add(a0, (uint32_t)half * a_half_bytes);
-        if (N == 16) {
-            float d[8] = {};
-            x3_block<TA, TB, 2>(d, ah, asplit, akstep, b0, bsplit, bkstep, nk);
-            frag_store<2>(acc, d_addr, M, half, d, accumulate);
-        } else {
-#pragma unroll 1
-            for (int nc = 0; nc < N / 64; ++nc) {       // N > 64: K-major SW128 B, 64 rows per block
-                float d[32] = {};
-                x3_block<TA, TB, 8>(d, ah, asplit, akstep, desc_add(b0, (uint32_t)nc * 8192u), bsplit, bkstep, nk);
-                frag_store<8>(acc, d_addr + (uint32_t)(64 * nc), M, half, d, accumulate);
-            }
+    if constexpr (M == 128) {
+        float d0[4 * NJ] = {}, d1[4 * NJ] = {};
+        x3_block<TA, TB, NJ, NK, B_EXACT>(d0, a0, asplit, akstep, b0, bsplit, bkstep);
+        x3_block<TA, TB, NJ, NK, B_EXACT>(d1, desc_add(a0, a_half_bytes), asplit, akstep, b0, bsplit, bkstep);
+        wg_wait<1>();
+        acc_fence(d0);
+        frag_store<NJ>(acc, d_addr, M, 0, d0, accumulate);
+        wg_wait<0>();
+        acc_fence(d1);
+        frag_store<NJ>(acc, d_addr, M, 1, d1, accumulate);
+    } else {
+        float d[4 * NJ] = {}, old[4 * NJ];
+        x3_block<TA, TB, NJ, NK, B_EXACT>(d, a0, asplit, akstep, b0, bsplit, bkstep);
+        frag_load<NJ>(acc, d_addr, M, 0, old);
+        wg_wait<0>();
+        acc_fence(d);
+        if (accumulate) {
+#pragma unroll
+            for (int i = 0; i < 4 * NJ; ++i) d[i] = d[i] + old[i];
         }
-    }
-}
-
-// D[acc] (+)= A * B over `nk` k-steps of 16, with the six split products (small terms first); called by all
-// 128 threads of one warpgroup.
-//   a0 / b0: descriptors of the hi sub-tiles at k-step 0; asplit / bsplit: bytes between sub-tiles;
-//   akstep / bkstep: bytes per k-step (K-major: 32; MN-major: 16 rows * pitch); shape: idesc_bf16(M, N, a_mn, b_mn)
-//   (an MN-major A has M = 64; N is 16 or a multiple of 64, and a multiple of 64 above 64 only for a K-major B).
-//   bsplit == 0 marks an exactly representable B (e.g. the ones tile): only the three A terms are issued.
-__device__ __forceinline__ void gemm_x3(const Acc& acc, uint32_t d_addr, uint64_t a0, uint32_t asplit, uint32_t akstep,
-                                        uint64_t b0, uint32_t bsplit, uint32_t bkstep, uint32_t shape, int nk,
-                                        bool accumulate) {
-    const int M = (int)((shape >> 24) & 31u) << 4, N = (int)((shape >> 17) & 63u) << 3;
-    switch ((shape >> 15) & 3u) {
-        case 0: gemm_x3_t<0, 0>(acc, d_addr, a0, asplit, akstep, b0, bsplit, bkstep, M, N, nk, accumulate); break;
-        case 1: gemm_x3_t<1, 0>(acc, d_addr, a0, asplit, akstep, b0, bsplit, bkstep, M, N, nk, accumulate); break;
-        case 2: gemm_x3_t<0, 1>(acc, d_addr, a0, asplit, akstep, b0, bsplit, bkstep, M, N, nk, accumulate); break;
-        default: gemm_x3_t<1, 1>(acc, d_addr, a0, asplit, akstep, b0, bsplit, bkstep, M, N, nk, accumulate); break;
+        frag_store<NJ>(acc, d_addr, M, 0, d, false);
     }
 }
 

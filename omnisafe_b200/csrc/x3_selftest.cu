@@ -6,15 +6,25 @@
 
 namespace osb {
 
+// The GEMM shapes the kernels issue (gemm_x3 takes its shape as template arguments).
+struct X3TestShape { int M, N, K, a_mn, b_mn, b_ones; };
+constexpr X3TestShape X3_TEST_SHAPES[] = {
+    {128, 64, 64, 0, 0, 0}, {128, 16, 64, 0, 0, 0}, {128, 64, 16, 0, 1, 0}, {128, 64, 64, 0, 1, 0},
+    {64, 64, 128, 1, 1, 0}, {64, 16, 128, 1, 1, 0}, {64, 16, 128, 1, 1, 1}, {64, 64, 64, 0, 0, 0},
+};
+constexpr int X3_NSHAPES = sizeof(X3_TEST_SHAPES) / sizeof(X3_TEST_SHAPES[0]);
+
 // A: row-major fp32 [M][K], B: row-major fp32 [N][K].  out[128][N]: dump of accumulator lanes 0..127.
 // a_mn / b_mn: operand consumed MN-major (tile rows = K index) instead of K-major (tile rows = M/N index).
 // a_sw / b_sw: 128 (tile rows of 64 bf16) or 32 (tile rows of 16 bf16).  b_ones: B is the all-ones tile
 // (exact in bf16: three MMAs per k-step).
+template <int S>
 __global__ void __launch_bounds__(128, 1) x3_selftest_kernel(const float* __restrict__ A, const float* __restrict__ B,
-                                                             int M, int N, int K, int a_mn, int b_mn, int a_sw,
-                                                             int b_sw, int b_ones, float* __restrict__ scratch,
+                                                             int a_sw, int b_sw, float* __restrict__ scratch,
                                                              float* __restrict__ out) {
     using namespace x3;
+    constexpr X3TestShape sh = X3_TEST_SHAPES[S];
+    constexpr int M = sh.M, N = sh.N, K = sh.K, a_mn = sh.a_mn, b_mn = sh.b_mn, b_ones = sh.b_ones;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
     const uint32_t sA = smem_u32(smem_raw) + pad;
@@ -40,8 +50,8 @@ __global__ void __launch_bounds__(128, 1) x3_selftest_kernel(const float* __rest
     __syncthreads();
     const Acc acc = acc_cta(scratch, (uint32_t)N);
     const uint64_t a0 = a_sw == 128 ? desc128(sA) : desc32(sA), b0 = b_sw == 128 ? desc128(sB) : desc32(sB);
-    gemm_x3(acc, 0u, a0, splitA, a_mn ? 16u * (uint32_t)a_sw : 32u, b0, b_ones ? 0u : splitB,
-            b_mn ? 16u * (uint32_t)b_sw : 32u, idesc_bf16(M, N, a_mn, b_mn), K / 16, false);
+    gemm_x3<M, N, K / 16, a_mn, b_mn, b_ones != 0>(acc, 0u, a0, splitA, a_mn ? 16u * (uint32_t)a_sw : 32u, b0, splitB,
+                                                   b_mn ? 16u * (uint32_t)b_sw : 32u, false);
     __threadfence_block();
     __syncthreads();
     for (int c0 = 0; c0 < N; c0 += 8) {
@@ -56,15 +66,23 @@ __global__ void __launch_bounds__(128, 1) x3_selftest_kernel(const float* __rest
 extern "C" int osb_x3_selftest(const float* A, const float* B, int M, int N, int K, int a_mn, int b_mn, int a_sw,
                                int b_sw, int b_ones, float* out, void* stream) {
     OSB_CHECK_ARG(A && B && out, "null pointer");
-    OSB_CHECK_ARG((M == 64 || M == 128) && (N == 16 || N == 64) && K % 16 == 0 && K >= 16 && K <= 128, "bad shape");
+    int shape = -1;
+    for (int i = 0; i < osb::X3_NSHAPES; ++i) {
+        const osb::X3TestShape& t = osb::X3_TEST_SHAPES[i];
+        if (t.M == M && t.N == N && t.K == K && t.a_mn == a_mn && t.b_mn == b_mn && t.b_ones == b_ones) shape = i;
+    }
+    OSB_CHECK_ARG(shape >= 0, "not a GEMM shape of the kernels");
     OSB_CHECK_ARG((a_sw == 128 || a_sw == 32) && (b_sw == 128 || b_sw == 32), "swizzle must be 128 or 32");
     OSB_CHECK_ARG((a_mn ? M : K) <= (a_sw == 128 ? 64 : 16) && (b_mn ? N : K) <= (b_sw == 128 ? 64 : 16), "tile wider than one swizzle atom");
-    OSB_CHECK_ARG(!(a_mn && M == 128), "an MN-major A has 64 rows");
+    using Kernel = void (*)(const float*, const float*, int, int, float*, float*);
+    const Kernel kernels[osb::X3_NSHAPES] = {osb::x3_selftest_kernel<0>, osb::x3_selftest_kernel<1>, osb::x3_selftest_kernel<2>,
+                                             osb::x3_selftest_kernel<3>, osb::x3_selftest_kernel<4>, osb::x3_selftest_kernel<5>,
+                                             osb::x3_selftest_kernel<6>, osb::x3_selftest_kernel<7>};
     float* scratch = osb::acc_scratch(osb::ACC_SELFTEST, (size_t)128 * N * sizeof(float));
     if (!scratch) return OSB_ERR_CUDA;
     const size_t smem = 1024 + 3 * 16384 + 3 * 16384;
-    OSB_CUDA(cudaFuncSetAttribute(osb::x3_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    osb::x3_selftest_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(A, B, M, N, K, a_mn, b_mn, a_sw, b_sw, b_ones, scratch, out);
+    OSB_CUDA(cudaFuncSetAttribute(kernels[shape], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernels[shape]<<<1, 128, smem, (cudaStream_t)stream>>>(A, B, a_sw, b_sw, scratch, out);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
 }

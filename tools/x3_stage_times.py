@@ -35,3 +35,13 @@ for which, off in (('thread 0 (loss warp)', 0), ('thread 256', 1024)):
         if id_ == 28:
             cnt28 += 1
             if cnt28 == 2: break
+# the first minibatch above is one sample of each hop: the median over every stamped tile of thread 0 is steadier
+import statistics
+d = dbg[0:1024].cpu().tolist()
+rows = [(d[1 + 2 * i], d[2 + 2 * i]) for i in range(d[0])]
+hops = {}
+for (_, c0), (id1, c1) in zip(rows, rows[1:]):
+    hops.setdefault(id1, []).append(c1 - c0)
+print('== thread 0: median cycles from the previous stamp, over all stamps of the launch')
+for id_ in sorted(hops):
+    print(f'  {NAMES.get(id_, id_):16s} {statistics.median(hops[id_]):8.0f} cyc  (n = {len(hops[id_])})')
