@@ -114,10 +114,6 @@ __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.s
 // wait until at most N committed groups of this warpgroup are pending
 template <int N>
 __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
-__device__ __forceinline__ void wg_commit_wait() {
-    wg_commit();
-    wg_wait<0>();
-}
 template <int R>
 __device__ __forceinline__ void acc_fence(float (&d)[R]) {
 #pragma unroll
@@ -144,40 +140,46 @@ __device__ __forceinline__ float* frag_row(const Acc& acc, uint32_t taddr, int M
     return acc.p + (size_t)lane * acc.pitch + (taddr & 0xFFFFu) + 2u * (uint32_t)(l & 3);
 }
 
-// Reads the image values under the m64 x (8 NJ) fragment, in the fragment's register order.
-template <int NJ>
-__device__ __forceinline__ void frag_load(const Acc& acc, uint32_t taddr, int M, int half, float (&o)[4 * NJ]) {
+// One row of the fragment (rr = 0 or 1, see frag_row), NB float2 of it from column pair j0 on: the image values under
+// them, read as independent loads that are all in flight together; the fragment registers d written there; and d + o
+// written there, one fp32 add per element.  A product that adds to the image reads a batch before it adds and stores:
+// a load, add, store chain per element would put one image round trip after another.
+template <int NB>
+__device__ __forceinline__ void row_load(const float* row, int j0, float2 (&o)[NB]) {
 #pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-        const float* row = frag_row(acc, taddr, M, half, rr);
+    for (int j = 0; j < NB; ++j) o[j] = *reinterpret_cast<const float2*>(row + 8 * (j0 + j));
+}
+template <int ND, int NB>
+__device__ __forceinline__ void row_add_store(float* row, int rr, const float (&d)[ND], int j0, const float2 (&o)[NB]) {
 #pragma unroll
-        for (int j = 0; j < NJ; ++j) {
-            const float2 v = *reinterpret_cast<const float2*>(row + 8 * j);
-            o[4 * j + 2 * rr] = v.x;
-            o[4 * j + 2 * rr + 1] = v.y;
-        }
+    for (int j = 0; j < NB; ++j) {
+        const int i = 4 * (j0 + j) + 2 * rr;
+        *reinterpret_cast<float2*>(row + 8 * (j0 + j)) = make_float2(d[i] + o[j].x, d[i + 1] + o[j].y);
     }
 }
 
-// Writes (or adds) the m64 x (8 NJ) fragment d of this warpgroup thread (see frag_row).
+// The m64 x (8 NJ) fragment of this warpgroup thread: the image values under it (both rows in flight), the fragment
+// written, and the fragment written as d + o.
 template <int NJ>
-__device__ __forceinline__ void frag_store(const Acc& acc, uint32_t taddr, int M, int half, const float (&d)[4 * NJ],
-                                           bool accumulate) {
+__device__ __forceinline__ void frag_load(const Acc& acc, uint32_t taddr, int M, int half, float2 (&o)[2][NJ]) {
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) row_load(frag_row(acc, taddr, M, half, rr), 0, o[rr]);
+}
+template <int NJ>
+__device__ __forceinline__ void frag_store(const Acc& acc, uint32_t taddr, int M, int half, const float (&d)[4 * NJ]) {
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
         float* row = frag_row(acc, taddr, M, half, rr);
 #pragma unroll
-        for (int j = 0; j < NJ; ++j) {
-            float2 v = make_float2(d[4 * j + 2 * rr], d[4 * j + 2 * rr + 1]);
-            float2* q = reinterpret_cast<float2*>(row + 8 * j);
-            if (accumulate) {
-                const float2 o = *q;
-                v.x += o.x;
-                v.y += o.y;
-            }
-            *q = v;
-        }
+        for (int j = 0; j < NJ; ++j)
+            *reinterpret_cast<float2*>(row + 8 * j) = make_float2(d[4 * j + 2 * rr], d[4 * j + 2 * rr + 1]);
     }
+}
+template <int NJ>
+__device__ __forceinline__ void frag_add_store(const Acc& acc, uint32_t taddr, int M, int half, const float (&d)[4 * NJ],
+                                               const float2 (&o)[2][NJ]) {
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) row_add_store(frag_row(acc, taddr, M, half, rr), rr, d, 0, o[rr]);
 }
 
 // The issuing warpgroup's image writes -> visible to the CTA, then one arrival on the mbarrier (count 1).
@@ -205,7 +207,8 @@ __device__ __forceinline__ void acc_ld32(const Acc& acc, uint32_t taddr, float (
 __device__ __forceinline__ void acc_ld16(const Acc& acc, uint32_t taddr, float (&v)[16]) { acc_ld<16>(acc, taddr, v); }
 
 // D[acc] (+)= A * B^T, both K-major SW128 tf32 tiles with RA / RB rows (M = 64 or 128, N = 16 or a multiple
-// of 64, K % 8 == 0); called by all 128 threads of one warpgroup.
+// of 64, K % 8 == 0); called by all 128 threads of one warpgroup.  With accumulate, the image values under a
+// fragment are read while its MMAs run.
 __device__ __forceinline__ void tc_gemm(const Acc& acc, uint32_t d_addr, uint32_t a_base, int RA, uint32_t b_base,
                                         int RB, int M, int N, int K, bool accumulate) {
 #pragma unroll 1
@@ -213,6 +216,7 @@ __device__ __forceinline__ void tc_gemm(const Acc& acc, uint32_t d_addr, uint32_
         const uint32_t a_half = a_base + (uint32_t)half * 64u * 128u;
         if (N == 16) {
             float d[8] = {};
+            float2 old[2][2];
             wg_fence();
             acc_fence(d);
 #pragma unroll 1
@@ -221,13 +225,17 @@ __device__ __forceinline__ void tc_gemm(const Acc& acc, uint32_t d_addr, uint32_
                 const uint32_t offB = (uint32_t)((ks >> 2) * RB * 128 + (ks & 3) * 32);
                 wgmma_tf32_n16(d, desc_kmajor(a_half + offA), desc_kmajor(b_base + offB), ks > 0 ? 1u : 0u);
             }
-            wg_commit_wait();
+            wg_commit();
+            if (accumulate) frag_load<2>(acc, d_addr, M, half, old);
+            wg_wait<0>();
             acc_fence(d);
-            frag_store<2>(acc, d_addr, M, half, d, accumulate);
+            if (accumulate) frag_add_store<2>(acc, d_addr, M, half, d, old);
+            else frag_store<2>(acc, d_addr, M, half, d);
         } else {
 #pragma unroll 1
             for (int nc = 0; nc < N / 64; ++nc) {
                 float d[32] = {};
+                float2 old[2][8];
                 wg_fence();
                 acc_fence(d);
 #pragma unroll 1
@@ -236,9 +244,12 @@ __device__ __forceinline__ void tc_gemm(const Acc& acc, uint32_t d_addr, uint32_
                     const uint32_t offB = (uint32_t)((ks >> 2) * RB * 128 + (ks & 3) * 32 + nc * 64 * 128);
                     wgmma_tf32_n64(d, desc_kmajor(a_half + offA), desc_kmajor(b_base + offB), ks > 0 ? 1u : 0u);
                 }
-                wg_commit_wait();
+                wg_commit();
+                if (accumulate) frag_load<8>(acc, d_addr + (uint32_t)(64 * nc), M, half, old);
+                wg_wait<0>();
                 acc_fence(d);
-                frag_store<8>(acc, d_addr + (uint32_t)(64 * nc), M, half, d, accumulate);
+                if (accumulate) frag_add_store<8>(acc, d_addr + (uint32_t)(64 * nc), M, half, d, old);
+                else frag_store<8>(acc, d_addr + (uint32_t)(64 * nc), M, half, d);
             }
         }
     }

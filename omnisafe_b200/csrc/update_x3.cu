@@ -227,6 +227,17 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
         const uint64_t dX = desc128(sbase + OFF_X), dH1 = desc128(sbase + OFF_H1), dH2 = desc128(sbase + OFF_H2);
         const uint64_t dD = desc32(sbase + OFF_D), dW1 = desc128(sbase + OFF_W1), dW2 = desc128(sbase + OFF_W2);
         const uint64_t dW3 = desc128(sbase + OFF_W3), dOnes = desc32(sbase + OFF_ONES);
+        // stage-time stamps of this warpgroup (third region of p.dbg).  Ids: 100 + 20 k for product k of Z1, Z2, OUT, dZ2',
+        // dZ1', plus 4 ph + {0: operands ready, 1 / 2: MMAs of rows 0-63 / 64-127 complete, 3: image stored} for column-half
+        // phase ph, plus 8 once the product is committed; 200 / 201 / 202: dW3, dW2 and the last gradient product committed.
+        const bool mdbg_on = p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && tid == NEPI;
+        int mdbg_n = 0;
+        auto mstamp = [&](int id) {
+            if (mdbg_on && mdbg_n < 400) {
+                long long* d = p.dbg + 2048;
+                d[1 + 2 * mdbg_n] = id; d[2 + 2 * mdbg_n] = clock64(); ++mdbg_n; d[0] = mdbg_n;
+            }
+        };
         int it = 0;
 #pragma unroll 1
         for (int mb = 0; mb < n_mb; ++mb) {
@@ -241,9 +252,12 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll 1
                 for (int ph = 0; ph < 2; ++ph) {
                     mbar_wait_a(bar(RDY_X0 + ph), par);
-                    gemm_x3<128, 64, 2, 0, 0>(tm, T_ZA, desc_add(dX, 64u * ph), ACT_SUB, 32u, desc_add(dW1, 64u * ph), W_SUB, 32u, ph > 0);
+                    mstamp(100 + 4 * ph);
+                    gemm_x3<128, 64, 2, 0, 0>(tm, T_ZA, desc_add(dX, 64u * ph), ACT_SUB, 32u, desc_add(dW1, 64u * ph), W_SUB, 32u, ph > 0, [&](int half) { mstamp(100 + 4 * ph + 1 + half); });
+                    mstamp(100 + 4 * ph + 3);
                 }
                 mma_commit_a(bar(DONE_C1));
+                mstamp(108);
                 // db2 of the PREVIOUS tile (dZ2 still sits in the H2 buffer until this tile's E2): runs under E1,
                 // completes before Z2 (in-order pipe), so DONE_C2 covers it
                 if (!first && !(!FUSED && p.forward_only)) gemm_x3<64, 16, 8, 1, 1, true>(tm, T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, tile != (int)blockIdx.x + G);
@@ -251,38 +265,53 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll 1
                 for (int ph = 0; ph < 2; ++ph) {
                     mbar_wait_a(bar(RDY_H1_0 + ph), par);
-                    gemm_x3<128, 64, 2, 0, 0>(tm, T_ZB, desc_add(dH1, 64u * ph), ACT_SUB, 32u, desc_add(dW2, 64u * ph), W_SUB, 32u, ph > 0);
+                    mstamp(120 + 4 * ph);
+                    gemm_x3<128, 64, 2, 0, 0>(tm, T_ZB, desc_add(dH1, 64u * ph), ACT_SUB, 32u, desc_add(dW2, 64u * ph), W_SUB, 32u, ph > 0, [&](int half) { mstamp(120 + 4 * ph + 1 + half); });
+                    mstamp(120 + 4 * ph + 3);
                 }
                 mma_commit_a(bar(DONE_C2));
+                mstamp(128);
                 // OUT = H2 W3^T
 #pragma unroll 1
                 for (int ph = 0; ph < 2; ++ph) {
                     mbar_wait_a(bar(RDY_H2_0 + ph), par);
-                    gemm_x3<128, 16, 2, 0, 0>(tm, T_OUT, desc_add(dH2, 64u * ph), ACT_SUB, 32u, desc_add(dW3, 64u * ph), W3_SUB, 32u, ph > 0);
+                    mstamp(140 + 4 * ph);
+                    gemm_x3<128, 16, 2, 0, 0>(tm, T_OUT, desc_add(dH2, 64u * ph), ACT_SUB, 32u, desc_add(dW3, 64u * ph), W3_SUB, 32u, ph > 0, [&](int half) { mstamp(140 + 4 * ph + 1 + half); });
+                    mstamp(140 + 4 * ph + 3);
                 }
                 mma_commit_a(bar(DONE_C3));
+                mstamp(148);
                 if (!FUSED && p.forward_only) continue;              // statistics pass (FOCOPS mask mean): no backward
                 // dZ2' = dOUT W3 ; dW3^T += H2^T dOUT
                 mbar_wait_a(bar(RDY_D), par);
-                gemm_x3<128, 64, 1, 0, 1>(tm, T_ZA, dD, D_SUB, 32u, dW3, W3_SUB, 2048u, false);
+                mstamp(160);
+                gemm_x3<128, 64, 1, 0, 1>(tm, T_ZA, dD, D_SUB, 32u, dW3, W3_SUB, 2048u, false, [&](int half) { mstamp(161 + half); });
+                mstamp(163);
                 mma_commit_a(bar(DONE_C4A));
+                mstamp(168);
                 gemm_x3<64, 16, 8, 1, 1>(tm, T_DW3, dH2, ACT_SUB, 2048u, dD, D_SUB, 512u, !first);
                 mma_commit_a(bar(DONE_C4B));
+                mstamp(200);
                 // dZ1' = dZ2 W2 ; dW2 += dZ2^T H1
 #pragma unroll 1
                 for (int ph = 0; ph < 2; ++ph) {
                     mbar_wait_a(bar(RDY_DZ2_0 + ph), par);
-                    gemm_x3<128, 64, 2, 0, 1>(tm, T_ZB, desc_add(dH2, 64u * ph), ACT_SUB, 32u, desc_add(dW2, 4096u * ph), W_SUB, 2048u, ph > 0);
+                    mstamp(180 + 4 * ph);
+                    gemm_x3<128, 64, 2, 0, 1>(tm, T_ZB, desc_add(dH2, 64u * ph), ACT_SUB, 32u, desc_add(dW2, 4096u * ph), W_SUB, 2048u, ph > 0, [&](int half) { mstamp(180 + 4 * ph + 1 + half); });
+                    mstamp(180 + 4 * ph + 3);
                 }
                 mma_commit_a(bar(DONE_C5A));
+                mstamp(188);
                 gemm_x3<64, 64, 8, 1, 1>(tm, T_DW2, dH2, ACT_SUB, 2048u, dH1, ACT_SUB, 2048u, !first);
                 mma_commit_a(bar(DONE_C5B));
+                mstamp(201);
                 // dW1 += dZ1^T X (column 63 = db1 with the ones column) ; last tile of the minibatch: its own db2
                 mbar_wait_a(bar(RDY_DZ1), par);
                 gemm_x3<64, 64, 8, 1, 1>(tm, T_DW1, dH1, ACT_SUB, 2048u, dX, ACT_SUB, 2048u, !first);
                 if (!ones_col) gemm_x3<64, 16, 8, 1, 1, true>(tm, T_DB1, dH1, ACT_SUB, 2048u, dOnes, 0u, 0u, !first);
                 if (last) gemm_x3<64, 16, 8, 1, 1, true>(tm, T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, !first);
                 mma_commit_a(bar(DONE_C6));
+                mstamp(202);
             }
         }
     } else {

@@ -83,11 +83,17 @@ __device__ __forceinline__ void x3_block(float (&d)[4 * NJ], uint64_t a0, uint32
 //   representable in bf16 (e.g. the ones tile), only the three A terms are issued and bsplit is not read.
 //   a0 / b0: descriptors of the hi sub-tiles at k-step 0; asplit / bsplit: bytes between sub-tiles;
 //   akstep / bkstep: bytes per k-step (K-major: 32; MN-major: 16 rows * pitch).
-// M = 128 issues both m64 halves before draining the first: half 0 is stored while half 1 runs.  M = 64 reads the
-// image values it adds to before waiting on its MMAs.  Either way the stored value is d, or d + old, as one fp32 add.
-template <int M, int N, int NK, int TA, int TB, bool B_EXACT = false>
+// M = 128 issues both m64 halves before draining the first: half 0 is stored while half 1 runs.  A product that adds
+// to the image reads the old values in batches of independent loads, the first batch before it waits on its MMAs.
+// Either way the stored value is d, or d + old, as one fp32 add.
+// `waited(half)` is called when the MMAs of m64 half `half` have completed (stage-time stamps; nothing by default).
+struct NoStamp {
+    __device__ __forceinline__ void operator()(int) const {}
+};
+template <int M, int N, int NK, int TA, int TB, bool B_EXACT = false, class Stamp = NoStamp>
 __device__ __forceinline__ void gemm_x3(const Acc& acc, uint32_t d_addr, uint64_t a0, uint32_t asplit, uint32_t akstep,
-                                        uint64_t b0, uint32_t bsplit, uint32_t bkstep, bool accumulate) {
+                                        uint64_t b0, uint32_t bsplit, uint32_t bkstep, bool accumulate,
+                                        Stamp waited = Stamp()) {
     static_assert((M == 64 || (M == 128 && TA == 0)) && (N == 16 || N == 64), "unsupported bf16x3 GEMM shape");
     constexpr int NJ = N / 8;
     // Every descriptor of the unrolled k-steps is invariant in the callers' tile loops; computed once there and held
@@ -96,27 +102,56 @@ __device__ __forceinline__ void gemm_x3(const Acc& acc, uint32_t d_addr, uint64_
     b0 = desc_fresh(b0);
     // rows 64..127 of a K-major A: 64 rows further down the tile (row pitch 128 B for SW128, 32 B for SW32)
     const uint32_t a_half_bytes = 64u * (((a0 >> 61) & 7u) == 2u ? 128u : 32u);
-    if constexpr (M == 128) {
+    if constexpr (M == 64) {
+        float d[4 * NJ] = {};
+        float2 old[2][NJ];
+        x3_block<TA, TB, NJ, NK, B_EXACT>(d, a0, asplit, akstep, b0, bsplit, bkstep);
+        if (accumulate) frag_load<NJ>(acc, d_addr, M, 0, old);
+        wg_wait<0>();
+        acc_fence(d);
+        if (accumulate) frag_add_store<NJ>(acc, d_addr, M, 0, d, old);
+        else frag_store<NJ>(acc, d_addr, M, 0, d);
+    } else {
         float d0[4 * NJ] = {}, d1[4 * NJ] = {};
         x3_block<TA, TB, NJ, NK, B_EXACT>(d0, a0, asplit, akstep, b0, bsplit, bkstep);
         x3_block<TA, TB, NJ, NK, B_EXACT>(d1, desc_add(a0, a_half_bytes), asplit, akstep, b0, bsplit, bkstep);
-        wg_wait<1>();
-        acc_fence(d0);
-        frag_store<NJ>(acc, d_addr, M, 0, d0, accumulate);
-        wg_wait<0>();
-        acc_fence(d1);
-        frag_store<NJ>(acc, d_addr, M, 1, d1, accumulate);
-    } else {
-        float d[4 * NJ] = {}, old[4 * NJ];
-        x3_block<TA, TB, NJ, NK, B_EXACT>(d, a0, asplit, akstep, b0, bsplit, bkstep);
-        frag_load<NJ>(acc, d_addr, M, 0, old);
-        wg_wait<0>();
-        acc_fence(d);
         if (accumulate) {
-#pragma unroll
-            for (int i = 0; i < 4 * NJ; ++i) d[i] = d[i] + old[i];
+            // The two fragments leave the 640-thread update kernel (96 registers) room for half a row of old values.
+            // So the four fragment rows go in turn, each batch of old values read as soon as registers are free for it:
+            // half of the first row while the MMAs run, the other half after it, and from then on whole rows into the
+            // registers that the stored rows have given up.
+            constexpr int NH = NJ / 2;
+            float* r00 = frag_row(acc, d_addr, M, 0, 0);
+            float* r01 = r00 + 8 * acc.pitch;                 // M = 128: fragment row m lies in image lane m
+            float* r10 = r00 + 64 * acc.pitch;
+            float* r11 = r00 + 72 * acc.pitch;
+            float2 oa[NH], ob[NH], oc[NJ], od[NJ], oe[NJ];
+            row_load(r00, 0, oa);
+            wg_wait<1>();
+            acc_fence(d0);
+            waited(0);
+            row_add_store(r00, 0, d0, 0, oa);
+            row_load(r00, NH, ob);
+            row_add_store(r00, 0, d0, NH, ob);
+            row_load(r01, 0, oc);
+            row_add_store(r01, 1, d0, 0, oc);
+            row_load(r10, 0, od);
+            row_load(r11, 0, oe);
+            wg_wait<0>();
+            acc_fence(d1);
+            waited(1);
+            row_add_store(r10, 0, d1, 0, od);
+            row_add_store(r11, 1, d1, 0, oe);
+        } else {
+            wg_wait<1>();
+            acc_fence(d0);
+            waited(0);
+            frag_store<NJ>(acc, d_addr, M, 0, d0);
+            wg_wait<0>();
+            acc_fence(d1);
+            waited(1);
+            frag_store<NJ>(acc, d_addr, M, 1, d1);
         }
-        frag_store<NJ>(acc, d_addr, M, 0, d, false);
     }
 }
 

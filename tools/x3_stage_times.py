@@ -1,5 +1,5 @@
 """Where one CTA of the persistent bf16x3 update kernel spends its time: clock64 stamps of CTA (0, 0)
-(thread 0 = loss warp, thread 256 = a non-loss warp)."""
+(thread 0 = loss warp, thread 256 = a non-loss warp, thread 512 = the MMA-issue warpgroup)."""
 import os, sys, tempfile
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -9,7 +9,7 @@ cfg = bench._custom_cfgs(1, tempfile.mkdtemp(), 40)
 cfg['train_cfgs']['matmul_precision'] = 'bf16x3'
 algo = omnisafe_b200.Agent('PPOLag', 'SyntheticBox-v0', custom_cfgs=cfg).agent
 for _ in range(2): algo.train_epoch()
-dbg = torch.zeros(2048, dtype=torch.int64, device='cuda')
+dbg = torch.zeros(3072, dtype=torch.int64, device='cuda')
 torch.cuda.synchronize()
 lib().osb_x3_debug_buffer(ptr(dbg))
 algo._update()
@@ -17,7 +17,14 @@ torch.cuda.synchronize()
 lib().osb_x3_debug_buffer(0)
 NAMES = {0: 'E0 start', 1: 'C6(prev) ok', 2: 'X stored+sync', 3: 'C1 ok', 4: 'E1 done', 5: 'C2 ok', 6: 'E2 done', 7: 'C3 ok', 8: 'dOUT stored', 9: 'E3 done',
          10: 'C4A ok', 11: 'E4 computed', 12: 'C4B ok', 13: 'E4 stored', 14: 'C5A ok', 15: 'E5 computed', 16: 'C5B ok', 17: 'E5 stored', 20: 'tiles done',
-         21: 'C6 ok', 22: 'extracted', 23: 'barrier1', 24: 'reduced', 25: 'barrier2', 26: 'adam done', 27: 'barrier3', 28: 'restaged'}
+         21: 'C6 ok', 22: 'extracted', 23: 'barrier1', 24: 'reduced', 25: 'barrier2', 26: 'adam done', 27: 'barrier3', 28: 'restaged',
+         200: 'dW3 committed', 201: 'dW2 committed', 202: 'dW1 committed'}
+# MMA-issue warpgroup: 100 + 20 k for product k, + 4 ph + event for column-half phase ph, + 8 for the commit
+for k, prod in enumerate(('Z1', 'Z2', 'OUT', "dZ2'", "dZ1'")):
+    for ph in range(2):
+        for ev, what in enumerate(('operands ready', 'rows 0-63 done', 'rows 64-127 done', 'stored')):
+            NAMES[100 + 20 * k + 4 * ph + ev] = f'{prod} ph{ph} {what}'
+    NAMES[100 + 20 * k + 8] = f'{prod} committed'
 for which, off in (('thread 0 (loss warp)', 0), ('thread 256', 1024)):
     d = dbg[off:off + 1024].cpu().tolist()
     n = d[0]
@@ -45,3 +52,11 @@ for (_, c0), (id1, c1) in zip(rows, rows[1:]):
 print('== thread 0: median cycles from the previous stamp, over all stamps of the launch')
 for id_ in sorted(hops):
     print(f'  {NAMES.get(id_, id_):16s} {statistics.median(hops[id_]):8.0f} cyc  (n = {len(hops[id_])})')
+d = dbg[2048:3072].cpu().tolist()
+rows = [(d[1 + 2 * i], d[2 + 2 * i]) for i in range(d[0])]
+hops = {}
+for (_, c0), (id1, c1) in zip(rows, rows[1:]):
+    hops.setdefault(id1, []).append(c1 - c0)
+print('== MMA-issue warpgroup (thread 512): median cycles from its previous stamp')
+for id_ in sorted(hops):
+    print(f'  {NAMES.get(id_, id_):24s} {statistics.median(hops[id_]):8.0f} cyc  (n = {len(hops[id_])})')
