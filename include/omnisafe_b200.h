@@ -386,6 +386,15 @@ int osb_fvp_partials_tc(const float* theta_actor, const float* vec, int O, int A
 int osb_fvp_partials_x3(const float* theta_actor, const float* vec, int O, int A, const float* obs,
                         long long total, int stride, float* dmu, float* gpart, float* stats_scratch,
                         void* stream);
+/* Actor backward with a supplied output gradient (loss kind LOSS_DMU = 6): the backward of actor losses written in
+ * PyTorch.  obs [rows][O] (contiguous, normalised), dmu [rows][A] = dL/dmu; gpart <- per-CTA partials of
+ * J_mu^T dmu over the actor parameters (log_std entries zero: no sigma^-2 factor, no 1/rows scale, no log_std term),
+ * osb_actor_dmu_grid_blocks(rows, O, precision) rows of P_actor floats; stats_scratch: that many * 24 floats.  Reduce
+ * with osb_reduce_partials.  precision as osb_ppo_update_epoch: 2 = bf16x3 tiles (O <= 64), 1 = tf32 tiles
+ * (O <= 512), otherwise the fp32 tiles -- the tiles osb_actor_eval{_x3,_tc,} of the same precision run forward. */
+int osb_actor_dmu_grid_blocks(int rows, int O, int precision);
+int osb_actor_dmu_backward(const float* theta_actor, int O, int A, const float* obs, const float* dmu, int rows,
+                           int precision, float* gpart, float* stats_scratch, void* stream);
 
 /* ---- optimiser side --------------------------------------------------------------------------
  * osb_grad_reduce: grad <- sum of CTA partials (+ 2*critic_norm_coef*theta for critics,

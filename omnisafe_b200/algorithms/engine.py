@@ -7,6 +7,7 @@ from __future__ import annotations
 import torch
 
 from omnisafe_b200._lib import current_stream, lib, ptr
+from omnisafe_b200.algorithms.torch_loss import feistel_order
 from omnisafe_b200.utils import distributed
 from omnisafe_b200.utils.train_state import restore, snapshot
 
@@ -95,6 +96,85 @@ class UpdateEngine:
             self.precision if precision is None else int(precision),
             distributed.nccl_comm(), distributed.world_size(), *distributed.p2p_exchange(self.P)[:2],
             distributed.get_rank(), distributed.p2p_exchange(self.P)[2], current_stream())
+
+    # ---- PolicyGradient._update with the actor objective in PyTorch ------------------------
+    def _optim_step(self, gpart, stats_part, nb, net_mask, critic_norm_coef, max_grad_norm, lr_actor, lr_critic):
+        """Reduce the partials, clip, average over ranks and Adam-step the networks of `net_mask` (the order of
+        osb_ppo_update_epoch)."""
+        a, s, w = self.agent, current_stream(), distributed.world_size()
+        if w == 1:
+            lib().osb_optim_fused(ptr(gpart), ptr(stats_part), nb, self.O, self.A, ptr(a.theta), ptr(a.grad),
+                                  ptr(a.adam_m), ptr(a.adam_v), ptr(a.adam_step), float(critic_norm_coef),
+                                  float(max_grad_norm), float(lr_actor), float(lr_critic), float(lr_critic), net_mask,
+                                  ptr(self.sumsq_part), ptr(self.train_stats), ptr(self.stop_flag), s)
+            return
+        lib().osb_grad_reduce(ptr(gpart), ptr(stats_part), nb, self.O, self.A, ptr(a.theta), ptr(a.grad),
+                              float(critic_norm_coef), net_mask, ptr(self.sumsq_part), ptr(a.adam_step),
+                              ptr(self.train_stats), ptr(self.stop_flag), s)
+        for do_clip, do_adam, scale in ((1, 0, 1.0), (0, 1, 1.0 / w)):
+            if do_adam:
+                distributed.all_reduce_(a.grad)
+            lib().osb_clip_adam(ptr(a.grad), ptr(a.theta), ptr(a.adam_m), ptr(a.adam_v), ptr(a.adam_step),
+                                ptr(self.sumsq_part), self.O, self.A, float(max_grad_norm), float(lr_actor),
+                                float(lr_critic), float(lr_critic), float(scale), float(critic_norm_coef),
+                                ptr(self.train_stats), do_clip, do_adam, net_mask, ptr(self.stop_flag), s)
+
+    def torch_actor_epoch(self, actor_step, *, lagrange, net_mask, batch_size, update_iters, critic_norm_coef=0.0,
+                          max_grad_norm=0.0, lr_actor=0.0, lr_critic=0.0, target_kl=0.0, kl_early_stop=False,
+                          perm=None) -> None:
+        """ppo_epoch with the actor trained through autograd: per minibatch of the same sample order the kernels draw
+        (or `perm`), the critics of `net_mask` take their kernel step, then `actor_step(rows)` returns (loss, gradient
+        of the actor parameters) for the slab rows `rows` [count] (int64), which is clipped, rank-averaged and
+        Adam-stepped by the kernels.  After each pass the full-batch KL check runs as in ppo_epoch."""
+        a, s = self.agent, current_stream()
+        if perm is not None:
+            assert perm.dtype == torch.int32 and perm.shape == (update_iters, self.total)
+        self.stop_flag.zero_()
+        self.kl_state.zero_()
+        self.train_stats.zero_()
+        self.snapshot_old_policy()
+        if not hasattr(self, 'actor_gpart'):
+            self.actor_gpart = torch.zeros(self.P, dtype=torch.float32, device=a.device)
+            self.actor_stats = torch.zeros(3 * 8, dtype=torch.float32, device=a.device)
+        seed = self.next_perm_seed()
+        critics = net_mask & (NET_CRITIC_R | NET_CRITIC_C)
+        opt = dict(critic_norm_coef=critic_norm_coef, max_grad_norm=max_grad_norm, lr_actor=lr_actor,
+                   lr_critic=lr_critic)
+        tiles = self._tc() or self._x3()
+        grad_fn = lib().osb_minibatch_grad_x3 if self._x3() else (lib().osb_minibatch_grad_tc if self._tc()
+                                                                   else lib().osb_minibatch_grad)
+        for it in range(update_iters):
+            if perm is not None:
+                order = perm[it].contiguous()
+            else:
+                it_seed = (seed + 0x9E3779B9 * it) & 0xFFFFFFFF
+                order = feistel_order(self.total, it_seed, a.device).to(torch.int32)
+            rows_all = order.to(torch.int64)
+            for start in range(0, self.total, batch_size):
+                count = min(batch_size, self.total - start)
+                if critics:
+                    grad_fn(ptr(a.theta), self.O, self.A, *self._batch_ptrs(), ptr(self.mu_old),
+                            ptr(self.buf.adv_moments), ptr(order), self.total, 0, start, count, LOSS_RATIO, 0.0, 0.0,
+                            1.0, 0.0, 0, ptr(self.logstd_old), critics, ptr(self.gpart), ptr(self.stats_part),
+                            ptr(self.stop_flag), s)
+                    nb = lib().osb_tc_grid_blocks(count, critics) if tiles else lib().osb_update_grid_blocks(count)
+                    self._optim_step(self.gpart, self.stats_part, nb, critics, **opt)
+                loss, grad = actor_step(rows_all[start:start + count])
+                self.actor_gpart[: self.Pa].copy_(grad)
+                self.actor_stats[0] = loss.detach()
+                self.actor_stats[3] = 1.0
+                self._optim_step(self.actor_gpart, self.actor_stats, 1, NET_ACTOR, **opt)
+            d = self.buf.data
+            self._eval_fn()(ptr(a.theta), self.O, self.A, ptr(d['obs']), ptr(d['act']), ptr(d['logp']),
+                            ptr(d['adv_r']), ptr(d['adv_c']), ptr(self.mu_old), ptr(self.logstd_old),
+                            ptr(self.buf.adv_moments), ptr(lagrange), self.total, 1, 0, ptr(self.eval_ws),
+                            ptr(self.eval_out), s)
+            if distributed.world_size() > 1:
+                distributed.all_reduce_(self.eval_out)
+            lib().osb_kl_check(ptr(self.eval_out), float(target_kl), int(kl_early_stop), ptr(self.stop_flag),
+                               ptr(self.kl_state), s)
+            if kl_early_stop and it + 1 < update_iters and int(self.stop_flag.item()):
+                break
 
     # ---- full-batch pieces for the natural-gradient family ---------------------------------
     def snapshot_old_policy(self) -> None:

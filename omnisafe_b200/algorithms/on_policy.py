@@ -13,6 +13,8 @@ import math
 import time
 
 import torch
+import torch.nn.functional as F
+from torch.distributions import Normal, kl_divergence
 
 from omnisafe_b200.adapter.onpolicy_adapter import OnPolicyAdapter
 from omnisafe_b200.adapter.early_terminated_adapter import EarlyTerminatedAdapter, ExternalEarlyTerminatedAdapter
@@ -23,6 +25,7 @@ from omnisafe_b200.algorithms import registry
 from omnisafe_b200.algorithms.base_algo import BaseAlgo
 from omnisafe_b200.algorithms.engine import (LOSS_COST, LOSS_FOCOPS, LOSS_P3O, LOSS_PPO_CLIP, LOSS_RATIO,
                                              NET_ACTOR, UpdateEngine)
+from omnisafe_b200.algorithms.torch_loss import DeviceStats, overridden_hooks, training_actor
 from omnisafe_b200.common.buffer import VectorOnPolicyBuffer
 from omnisafe_b200.common.lagrange import Lagrange
 from omnisafe_b200.common.logger import Logger
@@ -77,6 +80,10 @@ class PolicyGradient(BaseAlgo):
         self._stats8 = torch.zeros(8, dtype=torch.float64, device=self._device)
         self._epochs_done = 0       # epochs trained so far (a resumed run starts at the saved count)
         self._first_epoch = 0       # where learn() starts
+        # actor hooks overridden outside the library: the actor is then trained through autograd on them
+        self._torch_hooks = overridden_hooks(type(self))
+        self._loss_stats = DeviceStats()
+        self._path_logged = False
 
     def _init_log(self) -> None:
         lc = self._cfgs.logger_cfgs
@@ -113,6 +120,13 @@ class PolicyGradient(BaseAlgo):
         `log` (the logger reads the epoch's metrics back, one synchronisation per epoch).  `eps`
         optionally supplies the [T, N, A] standard-normal stream (parity mode)."""
         epoch_time = time.time()
+        if not self._path_logged:
+            self._path_logged = True
+            if self._torch_hooks:
+                by = ', '.join(f'{h} ({k})' for h, k in self._torch_hooks)
+                self._logger.log(f'INFO: the actor is trained through autograd on the PyTorch loss: {by} overridden')
+            else:
+                self._logger.log('INFO: the actor is trained by the fused update kernels')
         self._env.rollout(self._steps_per_epoch, self._actor_critic, self._buf, self._logger, eps=eps)
         self._buf.finish_paths()
         self._reduce_epoch_statistics()
@@ -168,6 +182,8 @@ class PolicyGradient(BaseAlgo):
             'Time/Epoch': now - epoch_time, 'Time/FPS': gsteps / (now - epoch_time),
         })
         self._log_extra()
+        if self._torch_hooks:     # what the PyTorch losses stored replaces the kernel statistics
+            self._logger.store({k: v for k, v in self._loss_stats.means().items() if k in self._logger._row})
         self._logger.dump_tabular()
         A = self._env.act_dim
         return {'d2h_bytes': 4 * 8 + 24 * 4 + 4 * 4 + 2 * A * 4 + 8, 'fps': gsteps / (now - epoch_time)}
@@ -227,6 +243,9 @@ class PolicyGradient(BaseAlgo):
         a = self._cfgs.algo_cfgs
         if not a.use_cost:
             net_mask &= ~4
+        if self._torch_hooks and net_mask & NET_ACTOR:
+            self._torch_update(net_mask, perm)
+            return
         self._engine.ppo_epoch(
             loss_kind=self._loss_kind, lagrange=self._lagrange_ptr(), net_mask=net_mask,
             batch_size=a.batch_size, update_iters=a.update_iters, clip=getattr(a, 'clip', 0.2),
@@ -237,12 +256,93 @@ class PolicyGradient(BaseAlgo):
             lr_actor=self._actor_critic.actor_lr, lr_critic=self._actor_critic.critic_lr,
             target_kl=a.target_kl, kl_early_stop=a.kl_early_stop, perm=perm)
 
+    # ---- actor objectives in PyTorch (policy_gradient.py:L483-588) ----------------------------------------------
+    # The library's own losses run inside the update kernels (csrc/loss.cuh).  These PyTorch statements of them are
+    # what `super()._loss_pi(...)` reaches from a subclass; they are called only when a hook is overridden.
+    def _compute_adv_surrogate(self, adv_r: torch.Tensor, adv_c: torch.Tensor) -> torch.Tensor:
+        return adv_r
+
+    def _loss_pi(self, obs, act, logp, adv) -> torch.Tensor:
+        distribution = self._actor_critic.actor(obs)
+        ratio = torch.exp(self._actor_critic.actor.log_prob(act) - logp)
+        loss = -(ratio * adv).mean()
+        self._store_pi_stats(distribution, ratio, loss)
+        return loss
+
+    def _loss_pi_cost(self, obs, act, logp, adv_c) -> torch.Tensor:
+        """CPO._loss_pi_cost (second_order/cpo.py:L182-212): mean(ratio * adv_c)."""
+        self._actor_critic.actor(obs)
+        ratio = torch.exp(self._actor_critic.actor.log_prob(act) - logp)
+        loss = (ratio * adv_c).mean()
+        self._loss_stats.store({'Loss/Loss_pi_cost': loss})
+        return loss
+
+    def _store_pi_stats(self, distribution, ratio, loss) -> None:
+        self._loss_stats.store({'Train/Entropy': distribution.entropy().mean(), 'Train/PolicyRatio': ratio,
+                                'Train/PolicyStd': distribution.stddev.mean(), 'Loss/Loss_pi': loss})
+
+    def _actor_loss(self, obs, act, logp, adv_r, adv_c) -> torch.Tensor:
+        """The actor objective of one minibatch (PolicyGradient._update_actor)."""
+        return self._loss_pi(obs, act, logp, self._compute_adv_surrogate(adv_r, adv_c))
+
+    def _torch_batch(self, rows):
+        """(obs, act, logp, adv_r, adv_c) of slab rows `rows` (None: all, in slab order), advantages standardised
+        with the epoch's moments as buffer.get() hands them over."""
+        d, O, A = self._buf.data, self._env.obs_dim, self._env.act_dim
+        m = self._buf.adv_moments
+        obs, act = d['obs'].view(-1, O), d['act'].view(-1, A)
+        logp, adv_r, adv_c = d['logp'].view(-1), d['adv_r'].view(-1), d['adv_c'].view(-1)
+        if rows is not None:
+            obs, act, logp = obs.index_select(0, rows), act.index_select(0, rows), logp.index_select(0, rows)
+            adv_r, adv_c = adv_r.index_select(0, rows), adv_c.index_select(0, rows)
+        return obs, act, logp, (adv_r - m[0]) / m[1], adv_c - m[2]
+
+    def _torch_loss(self, theta, loss_fn, rows=None, grad: bool = True):
+        """loss_fn(obs, act, logp, adv_r, adv_c) with the actor on `theta` (flat actor parameters); with `grad`
+        returns (loss, d loss / d theta), else the loss alone."""
+        e = self._engine
+        if rows is not None:
+            self._p_dist_b = Normal(e.mu_old.view(-1, e.A).index_select(0, rows), torch.exp(e.logstd_old),
+                                    validate_args=False)
+        else:
+            self._p_dist_b = Normal(e.mu_old.view(-1, e.A), torch.exp(e.logstd_old), validate_args=False)
+        theta = theta.detach().clone().requires_grad_(grad)
+        with torch.set_grad_enabled(grad), training_actor(self._actor_critic, e, theta):
+            loss = loss_fn(*self._torch_batch(rows))
+            if not grad:
+                return loss.detach()
+            loss.backward()
+        return loss.detach(), theta.grad
+
+    def _torch_update(self, net_mask: int, perm=None) -> None:
+        """PolicyGradient._update with the actor trained through autograd on `_actor_loss`."""
+        a, ac = self._cfgs.algo_cfgs, self._actor_critic
+        Pa = self._engine.Pa
+        self._loss_stats.clear()
+        self._engine.torch_actor_epoch(
+            lambda rows: self._torch_loss(ac.theta[:Pa], self._actor_loss, rows),
+            lagrange=self._lagrange_ptr(), net_mask=net_mask, batch_size=a.batch_size, update_iters=a.update_iters,
+            critic_norm_coef=a.critic_norm_coef if a.use_critic_norm else 0.0,
+            max_grad_norm=a.max_grad_norm if a.use_max_grad_norm else 0.0,
+            lr_actor=ac.actor_lr, lr_critic=ac.critic_lr, target_kl=a.target_kl, kl_early_stop=a.kl_early_stop,
+            perm=perm)
+
 
 @registry.register
 class PPO(PolicyGradient):
     """base/ppo.py:L28-87 (clipped surrogate)."""
 
     _loss_kind = LOSS_PPO_CLIP
+
+    def _loss_pi(self, obs, act, logp, adv) -> torch.Tensor:
+        a = self._cfgs.algo_cfgs
+        distribution = self._actor_critic.actor(obs)
+        ratio = torch.exp(self._actor_critic.actor.log_prob(act) - logp)
+        ratio_clipped = torch.clamp(ratio, 1 - a.clip, 1 + a.clip)
+        loss = -torch.min(ratio * adv, ratio_clipped * adv).mean()
+        loss = loss - a.entropy_coef * distribution.entropy().mean()
+        self._store_pi_stats(distribution, ratio, loss)
+        return loss
 
 
 class _LagrangeMixin:
@@ -259,6 +359,10 @@ class _LagrangeMixin:
 
     def _lagrange_ptr(self):
         return self._lagrange.state
+
+    def _compute_adv_surrogate(self, adv_r, adv_c):
+        lam = self._lagrange.state[0]
+        return (adv_r - lam * adv_c) / (1 + lam)
 
     def _train_state(self) -> dict:
         return {**super()._train_state(), 'lagrange': self._lagrange.train_state()}
@@ -306,6 +410,9 @@ class IPO(PPO):
     def _lagrange_ptr(self):
         return self._penalty_state
 
+    def _compute_adv_surrogate(self, adv_r, adv_c):
+        return (adv_r - self._penalty * adv_c) / (1 + self._penalty)
+
     def _train_state(self) -> dict:
         return {**super()._train_state(), 'penalty_state': self._penalty_state.cpu().clone(), 'penalty': self._penalty}
 
@@ -340,9 +447,24 @@ class P3O(PPO):
         super()._init_log()
         self._logger.register_key('Loss/Loss_pi_cost', delta=True)
 
+    def _loss_pi_cost(self, obs, act, logp, adv_c) -> torch.Tensor:
+        """kappa * relu(mean(ratio * adv_c) + Jc - cost_limit) (p3o.py:L48-91)."""
+        self._actor_critic.actor(obs)
+        ratio = torch.exp(self._actor_critic.actor.log_prob(act) - logp)
+        loss = self._cfgs.algo_cfgs.kappa * F.relu((ratio * adv_c).mean() + self._jc_minus_limit)
+        self._loss_stats.store({'Loss/Loss_pi_cost': loss})
+        return loss
+
+    def _actor_loss(self, obs, act, logp, adv_r, adv_c) -> torch.Tensor:
+        return self._loss_pi(obs, act, logp, adv_r) + self._loss_pi_cost(obs, act, logp, adv_c)
+
     def _update(self, net_mask: int = 7, perm=None) -> None:
         a = self._cfgs.algo_cfgs
         jc = self._window_means()[1] - a.cost_limit        # the reference reads the logger per minibatch (p3o.py:L88)
+        self._jc_minus_limit = jc
+        if self._torch_hooks:
+            self._torch_update(net_mask if a.use_cost else net_mask & ~4, perm)
+            return
         self._engine.ppo_epoch(
             loss_kind=LOSS_P3O, lagrange=None, net_mask=net_mask if a.use_cost else net_mask & ~4,
             batch_size=a.batch_size, update_iters=a.update_iters, clip=a.clip, entropy_coef=a.entropy_coef,
@@ -363,6 +485,20 @@ class FOCOPS(_LagrangeMixin, PolicyGradient):
     """first_order/focops.py:L31-230."""
 
     _loss_kind = LOSS_FOCOPS
+
+    def _loss_pi(self, obs, act, logp, adv) -> torch.Tensor:
+        """focops.py:L62-108.  The reference's [b, 1] - [b] broadcast makes the mean over a [b, b] matrix, i.e.
+        mean(mask * kl) - mean(mask) * mean(ratio * adv) / lam, which is what is formed here.  `_p_dist_b` is the
+        old policy on the minibatch rows."""
+        a = self._cfgs.algo_cfgs
+        distribution = self._actor_critic.actor(obs)
+        ratio = torch.exp(self._actor_critic.actor.log_prob(act) - logp)
+        kl = kl_divergence(distribution, self._p_dist_b).sum(-1, keepdim=True)
+        mask = (kl.detach() <= a.focops_eta).to(torch.float32)
+        loss = (mask * kl).mean() - mask.mean() * (ratio * adv).mean() / a.focops_lam
+        loss = loss - a.entropy_coef * distribution.entropy().mean()
+        self._store_pi_stats(distribution, ratio, loss)
+        return loss
 
 
 @registry.register
@@ -397,7 +533,7 @@ class NaturalPG(PolicyGradient):
         theta_old = ac.theta[:Pa].clone()
         grads = torch.empty(Pa, dtype=torch.float32, device=self._device)
         self._kind = self._surrogate_kind()
-        loss_before = e.actor_loss_grad(self._kind, self._adv_lagrange(), grads, sign=-1.0)
+        loss_before = self._surrogate_grad('reward', grads, sign=-1.0)
         x = e.conjugate_gradients(grads, a.cg_iters, a.cg_damping, a.fvp_sample_freq)
         assert torch.isfinite(x).all(), 'x is not finite'
         e.fvp(x, e.cg_z, a.cg_damping, a.fvp_sample_freq)
@@ -405,6 +541,45 @@ class NaturalPG(PolicyGradient):
         assert xHx >= 0, 'xHx is negative'
         alpha = math.sqrt(2 * a.target_kl / (xHx + 1e-8))
         return theta_old, grads, x, xHx, alpha, float(loss_before)
+
+    def _reward_loss(self, obs, act, logp, adv_r, adv_c) -> torch.Tensor:
+        return self._loss_pi(obs, act, logp, self._compute_adv_surrogate(adv_r, adv_c))
+
+    def _cost_loss(self, obs, act, logp, adv_r, adv_c) -> torch.Tensor:
+        return self._loss_pi_cost(obs, act, logp, adv_c)
+
+    def _surrogate_grad(self, which: str, out: torch.Tensor, sign: float) -> torch.Tensor:
+        """loss.backward() of the full-batch reward ('reward': the `_surrogate_kind` objective) or cost surrogate +
+        avg_grads: out <- sign * d loss / d theta_actor; returns the device scalar loss (rank-averaged)."""
+        e = self._engine
+        if not self._torch_hooks:
+            kind, lagrange = (self._kind, self._adv_lagrange()) if which == 'reward' else (LOSS_COST, None)
+            return e.actor_loss_grad(kind, lagrange, out, sign=sign)
+        w = distributed.world_size()
+        loss_fn = self._reward_loss if which == 'reward' else self._cost_loss
+        loss, grad = self._torch_loss(self._actor_critic.theta[: e.Pa], loss_fn)
+        out.copy_(grad * (sign / w))
+        loss = loss.reshape(1) / w
+        if w > 1:
+            distributed.all_reduce_(out)
+            distributed.all_reduce_(loss)
+        return loss
+
+    def _trial_loss(self, trial: torch.Tensor, which: str, ev: dict) -> float:
+        """Surrogate of a line-search trial: from the evaluation kernel's statistics `ev`, or the PyTorch loss at
+        `trial` (forward only).  which: 'reward' (the `_surrogate_kind` objective), 'reward_only' (CPO's -mean ratio
+        adv_r) or 'cost'."""
+        if not self._torch_hooks:
+            if which == 'cost':
+                return ev['loss_c']
+            if which == 'reward_only':
+                return ev['loss_r']
+            return ev['loss_c'] if self._kind == LOSS_COST else ev['loss']
+        loss_fn = self._cost_loss if which == 'cost' else self._reward_loss
+        loss = self._torch_loss(trial[: self._engine.Pa], loss_fn, grad=False).reshape(1)
+        if distributed.world_size() > 1:
+            loss = distributed.all_reduce_(loss / distributed.world_size())
+        return float(loss)
 
     def _update_actor(self) -> None:
         theta_old, grads, x, xHx, alpha, _ = self._natural_direction()
@@ -420,6 +595,9 @@ class NaturalPG(PolicyGradient):
         # what the reference logs after the actor step (natural_pg.py:L168-186, trpo.py:L196-222): loss / ratio / KL of
         # the accepted policy on the full batch, StopIter = update_iters
         ev = self._engine.evaluate(self._actor_critic.theta, self._adv_lagrange())
+        if self._torch_hooks:      # Loss/Loss_pi and Train/PolicyRatio: what the loss stores at the accepted policy
+            self._loss_stats.clear()
+            self._trial_loss(self._actor_critic.theta, 'reward', ev)
         ts = self._engine.train_stats.view(3, 8)
         ts[0, 0] = ev['loss_c'] if self._kind == LOSS_COST else ev['loss']
         ts[0, 1] = ev['ratio']
@@ -449,7 +627,7 @@ class TRPO(NaturalPG):
         for step in range(total_steps):
             trial[: e.Pa] = theta_old + step_frac * step_direction
             ev = e.evaluate(trial, self._adv_lagrange())
-            loss = ev['loss_c'] if self._kind == LOSS_COST else ev['loss']
+            loss = self._trial_loss(trial, 'reward', ev)
             loss_improve = loss_before - loss
             if not math.isfinite(loss):
                 self._logger.log('WARNING: loss_pi not finite')
@@ -559,8 +737,8 @@ class CPO(TRPO):
             acceptance_step = step + 1
             ev = e.evaluate(trial, None)
             kl = ev['kl']
-            loss_reward_improve = loss_reward_before - ev['loss_r']
-            loss_cost_diff = ev['loss_c'] - loss_cost_before
+            loss_reward_improve = loss_reward_before - self._trial_loss(trial, 'reward_only', ev)
+            loss_cost_diff = self._trial_loss(trial, 'cost', ev) - loss_cost_before
             if not math.isfinite(kl):
                 self._logger.log('WARNING: KL not finite')
                 continue
@@ -584,7 +762,7 @@ class CPO(TRPO):
         a, e = self._cfgs.algo_cfgs, self._engine
         theta_old, grads, x, xHx, alpha, loss_reward_before = self._natural_direction()
         b_grads = torch.empty(e.Pa, dtype=torch.float32, device=self._device)
-        loss_cost_before = float(e.actor_loss_grad(LOSS_COST, None, b_grads, sign=1.0))
+        loss_cost_before = float(self._surrogate_grad('cost', b_grads, sign=1.0))
         ep_costs = self._window_means()[1] - a.cost_limit
         p = e.conjugate_gradients(b_grads, a.cg_iters, a.cg_damping, a.fvp_sample_freq)
         q, r, s = xHx, e.dot(grads, p), e.dot(b_grads, p)
@@ -611,7 +789,7 @@ class PCPO(CPO):
         theta_old, grads, x, xHx, alpha, loss_reward_before = self._natural_direction()
         h_inv_g = e.cg_z.clone()                     # the reference's `H_inv_g = self._fvp(x)` (pcpo.py:L80)
         b_grads = torch.empty(e.Pa, dtype=torch.float32, device=self._device)
-        loss_cost_before = float(e.actor_loss_grad(LOSS_COST, None, b_grads, sign=1.0))
+        loss_cost_before = float(self._surrogate_grad('cost', b_grads, sign=1.0))
         ep_costs = self._window_means()[1] - a.cost_limit
         p = e.conjugate_gradients(b_grads, a.cg_iters, a.cg_damping, a.fvp_sample_freq)
         q, r, s = xHx, e.dot(grads, p), e.dot(b_grads, p)
@@ -672,6 +850,9 @@ class OnCRPO(TRPO):
     def _load_train_state(self, state: dict) -> None:
         super()._load_train_state(state)
         self._rew_update, self._cost_update = int(state['rew_update']), int(state['cost_update'])
+
+    def _compute_adv_surrogate(self, adv_r, adv_c):
+        return adv_r if self._kind == LOSS_RATIO else -adv_c
 
     def _surrogate_kind(self) -> int:
         a = self._cfgs.algo_cfgs

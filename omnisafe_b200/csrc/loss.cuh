@@ -23,6 +23,8 @@ enum LossKind {
     LOSS_COST = 3,
     LOSS_FVP = 4,      // dOUT supplied: backward half of the tensor-core Fisher-vector products
     LOSS_P3O = 5,      // two passes
+    LOSS_DMU = 6,      // dOUT = dmu supplied per row: J^T dmu of the actor MLP (losses written in PyTorch); compiled
+                       // only into the DMU instantiations of the stepwise kernels
 };
 
 // FOCOPS and P3O need a minibatch mean before any gradient: a forward-only pass 1 feeds pass1_gate().
@@ -243,5 +245,11 @@ __device__ __forceinline__ void eval_sample(const AdvNorm& an, int A, const floa
 int pass1_gate(const float* stats_part, int nblocks, const int* stop_flag, LossParams& lp, cudaStream_t stream);
 // out[8] <- fixed-order sums of the evaluation partials part[nblocks][8] (slots 6 and 7 zero).
 int eval_reduce(const double* part, int nblocks, double* out, cudaStream_t stream);
+// LOSS_DMU launches of the tensor-core kernels (csrc/update_tc.cu, csrc/update_x3.cu) behind osb_actor_dmu_backward:
+// rows obs[rows][O] in order, dmu[rows][A]; gpart: osb_tc_grid_blocks(rows, 1) rows of P_actor floats.
+int dmu_backward_tc(const float* theta_actor, int O, int A, const float* obs, const float* dmu, int rows, float* gpart,
+                    float* stats_scratch, cudaStream_t stream);
+int dmu_backward_x3(const float* theta_actor, int O, int A, const float* obs, const float* dmu, int rows, float* gpart,
+                    float* stats_scratch, cudaStream_t stream);
 
 }  // namespace osb

@@ -65,6 +65,9 @@ __device__ __forceinline__ void block_reduce_store(float (&v)[NV], float* sRed, 
     __syncthreads();
 }
 
+// DMU = true: actor only, LOSS_DMU -- b.act carries the supplied dL/dmu [rows][A] and the backward yields J^T of it
+// (no log_std term, no statistics but the row count).
+template <bool DMU = false>
 __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p) {
     if (p.stop_flag && *p.stop_flag) return;
     const int net = blockIdx.y;
@@ -148,6 +151,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p)
                     st[3] = 1.f;
                     sO[m * LDO] = 2.f * d * inv_b;                       // d mse / d v
                     for (int o = 1; o < OUTP; ++o) sO[m * LDO + o] = 0.f;
+                } else if (DMU) {
+                    for (int a = 0; a < OUTP; ++a) sO[m * LDO + a] = (a < A) ? __ldg(p.b.act + row * A + a) : 0.f;
+                    st[3] = 1.f;
                 } else {
                     float mu[OUTP], act[OUTP];
 #pragma unroll
@@ -707,19 +713,19 @@ int osb_minibatch_grad(const float* theta, int O, int A, const float* obs, const
     const size_t smem = grad_smem_bytes();
     static bool attr = false;
     if (!attr) {
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = true;
     }
     dim3 grid(osb_update_grid_blocks(mb_count), 3);
     if (loss_two_pass(loss_kind) && (net_mask & 1)) {   // pass 1: actor forward only
         GradArgs q = p;
         q.forward_only = 1; q.net_mask = 1;
-        minibatch_grad_kernel<<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(q);
+        minibatch_grad_kernel<false><<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(q);
         OSB_LAUNCH_CHECK();
         const int rc = pass1_gate(stats_part, (int)grid.x, stop_flag, p.lc, (cudaStream_t)stream);
         if (rc) return rc;
     }
-    minibatch_grad_kernel<<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(p);
+    minibatch_grad_kernel<false><<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(p);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
 }
@@ -773,6 +779,43 @@ int osb_fvp_partials(const float* theta_actor, const float* vec, int O, int A, c
         attr = true;
     }
     fvp_kernel<<<osb_fvp_grid_blocks(total, stride), NTHREADS, smem, (cudaStream_t)stream>>>(p);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}
+
+int osb_tc_grid_blocks(long long rows, int net_mask);
+
+// Tiles of the supplied-dmu backward: bf16x3 (precision 2, O <= 64), tf32 (precision 1, O <= 512), else fp32 -- the
+// choice of UpdateEngine._eval_fn, so that the backward differentiates the forward that produced mu.
+static int dmu_tiles(int O, int precision) { return (precision == 2 && O <= 64) ? 2 : (precision == 1 && O <= 512) ? 1 : 0; }
+
+int osb_actor_dmu_grid_blocks(int rows, int O, int precision) {
+    return dmu_tiles(O, precision) ? osb_tc_grid_blocks(rows, 1) : osb_fvp_grid_blocks(rows, 1);
+}
+
+// Actor backward with a supplied output gradient (LOSS_DMU): rows obs[rows][O] (contiguous, normalised), dmu[rows][A]
+// = dL/dmu  ->  gpart[osb_actor_dmu_grid_blocks(rows, O, precision)][P_actor] per-CTA partials of J^T dmu (log_std
+// entries zero), stats_scratch that many * 24 floats.  Reduce with osb_reduce_partials.
+int osb_actor_dmu_backward(const float* theta_actor, int O, int A, const float* obs, const float* dmu, int rows,
+                           int precision, float* gpart, float* stats_scratch, void* stream) {
+    OSB_CHECK_ARG(theta_actor && obs && dmu && gpart && stats_scratch && rows > 0, "bad argument");
+    OSB_CHECK_ARG(O > 0 && A > 0 && A <= OUTP, "bad dims");
+    const int tiles = dmu_tiles(O, precision);
+    if (tiles == 2) return dmu_backward_x3(theta_actor, O, A, obs, dmu, rows, gpart, stats_scratch, (cudaStream_t)stream);
+    if (tiles == 1) return dmu_backward_tc(theta_actor, O, A, obs, dmu, rows, gpart, stats_scratch, (cudaStream_t)stream);
+    GradArgs p;
+    p.b = Batch{obs, dmu, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, rows, 0u, 0, rows, 1};
+    p.lc = LossParams{LOSS_DMU, 0.f, 0.f, 1.f, 0.f, nullptr, nullptr, nullptr, nullptr};
+    p.forward_only = 0;
+    p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch; p.stop_flag = nullptr;
+    p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
+    const size_t smem = grad_smem_bytes();
+    static bool attr = false;
+    if (!attr) {
+        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attr = true;
+    }
+    minibatch_grad_kernel<true><<<dim3(osb_fvp_grid_blocks(rows, 1), 1), NTHREADS, smem, (cudaStream_t)stream>>>(p);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
 }

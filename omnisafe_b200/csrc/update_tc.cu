@@ -73,7 +73,8 @@ __device__ __forceinline__ void load_row16(uint32_t base, int r, int c0, int R, 
 // accumulate over chunks; backward: one dW1 chunk per MMA, flushed from accumulator image into this CTA's partial gradient).
 // EXT = the two-pass / supplied-dOUT loss kinds (FOCOPS, P3O, FVP); the plain instantiation (PPO-clip, ratio,
 // cost surrogate: the headline path) carries none of their registers or branches.
-template <bool CHUNKED, bool EXT>
+// DMU = LOSS_DMU only: the supplied dL/dmu (fvp_dmu, per row) is dOUT as it stands, no loss, no log_std term.
+template <bool CHUNKED, bool EXT, bool DMU = false>
 __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
     if (p.stop_flag && *p.stop_flag) return;
     // one network selected: grid.y == 1 and all of grid.x (up to one CTA per SM) works on that network
@@ -372,11 +373,11 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             for (int a = 0; a < 16; ++a) pf_act[a] = 0.f;
             if (prow >= 0) {
                 if (net == 0) {
-                    const float* src = is_fvp ? p.fvp_dmu : p.b.act;
+                    const float* src = (DMU || is_fvp) ? p.fvp_dmu : p.b.act;
 #pragma unroll
                     for (int a = 0; a < 16; ++a)
                         if (a < A) pf_act[a] = __ldg(src + prow * A + a);
-                    if (!is_fvp) {
+                    if (!DMU && !is_fvp) {
                         pf_logp = __ldg(p.b.logp + prow);
                         pf_advr = __ldg(p.b.adv_r + prow);
                         pf_advc = __ldg(p.b.adv_c + prow);
@@ -401,6 +402,11 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
                     const float d = o16[0] + sB3[0] - pf_tv;
                     st[0] = d * d; st[3] = 1.f;
                     d32[0] = 2.f * d * inv_b;
+                } else if (DMU) {
+#pragma unroll
+                    for (int a = 0; a < 16; ++a)
+                        if (a < A) d32[a] = pf_act[a];
+                    st[3] = 1.f;
                 } else if (is_fvp) {
                     // dOUT = diag(sigma^-2) J v / (rows * A): the backward below then yields J^T of it
 #pragma unroll
@@ -1017,3 +1023,29 @@ int osb_fvp_partials_tc(const float* theta_actor, const float* vec, int O, int A
 }
 
 }  // extern "C"
+
+int osb::dmu_backward_tc(const float* theta_actor, int O, int A, const float* obs, const float* dmu, int rows, float* gpart,
+                         float* stats_scratch, cudaStream_t stream) {
+    OSB_CHECK_ARG(O <= 512 && A <= 16, "tensor-core path needs O <= 512, A <= 16");
+    TcArgs p;
+    p.b = Batch{obs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, rows, 0u, 0, rows, 1};
+    p.lc = LossParams{LOSS_DMU, 0.f, 0.f, 1.f, 0.f, nullptr, nullptr, nullptr, nullptr};
+    p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch; p.stop_flag = nullptr;
+    p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
+    p.fvp_dmu = dmu; p.fvp_vec = nullptr; p.fvp_scale = 1.f;
+    p.forward_only = 0;
+    const size_t smem = tc_smem_bytes();
+    static bool attr = false;
+    if (!attr) {
+        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attr = true;
+    }
+    const int nb = osb_tc_grid_blocks(rows, 1);
+    p.acc = acc_scratch(ACC_UPDATE_TC, (size_t)nb * 128 * TC_COLS * sizeof(float));
+    if (!p.acc) return OSB_ERR_CUDA;
+    if (O > 64) minibatch_grad_tc_kernel<true, false, true><<<dim3(nb, 1), NTC, smem, stream>>>(p);
+    else minibatch_grad_tc_kernel<false, false, true><<<dim3(nb, 1), NTC, smem, stream>>>(p);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}

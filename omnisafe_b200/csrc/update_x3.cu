@@ -173,8 +173,10 @@ constexpr int PSTR = 9472;          // FUSED: row stride of the private partial-
 //   distributed.py:L193-198), apply torch-Adam and re-stage the new weights: no relaunch, no separate
 //   optimiser kernel.
 // AP = padded action width of the loss epilogue (8 or 16).
+// DMU = LOSS_DMU only (FUSED = false): the supplied dL/dmu (fvp_dmu, per row) is dOUT as it stands, no loss, no
+// log_std term.
 // (20 warps = 640 threads: 96 registers each, the register file divided in units of 8 per thread)
-template <bool FUSED, int AP>
+template <bool FUSED, int AP, bool DMU = false>
 __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
     if (p.stop_flag && *p.stop_flag) return;
     const int net = (gridDim.y == 1) ? (__ffs(p.net_mask) - 1) : (int)blockIdx.y;
@@ -452,7 +454,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll
                     for (int a = 0; a < AP; ++a) pf_act[a] = 0.f;
                     if (prow >= 0) {
-                        const float* asrc = (p.lc.kind == LOSS_FVP) ? p.fvp_dmu : p.b.act;
+                        const float* asrc = (DMU || p.lc.kind == LOSS_FVP) ? p.fvp_dmu : p.b.act;
                         if (AP == 8) {
                             const uint32_t dst = sbase + OFF_PF + (uint32_t)(s_row * PF_LD) * 4u;
                             auto cp4 = [&](uint32_t d, const float* src) {
@@ -462,7 +464,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll
                                 for (int a = 0; a < AP; ++a)
                                     if (a < A) cp4(dst + 4u * a, asrc + prow * A + a);
-                                if (p.lc.kind != LOSS_FVP) { cp4(dst + 32u, p.b.logp + prow); cp4(dst + 36u, p.b.adv_r + prow); cp4(dst + 40u, p.b.adv_c + prow); }
+                                if (!DMU && p.lc.kind != LOSS_FVP) { cp4(dst + 32u, p.b.logp + prow); cp4(dst + 36u, p.b.adv_r + prow); cp4(dst + 40u, p.b.adv_c + prow); }
                             } else {
                                 cp4(dst + 32u, (net == 1 ? p.b.tv_r : p.b.tv_c) + prow);
                             }
@@ -470,7 +472,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll
                             for (int a = 0; a < AP; ++a)
                                 if (a < A) pf_act[a] = __ldg(asrc + prow * A + a);
-                            if (p.lc.kind != LOSS_FVP) { pf_logp = __ldg(p.b.logp + prow); pf_advr = __ldg(p.b.adv_r + prow); pf_advc = __ldg(p.b.adv_c + prow); }
+                            if (!DMU && p.lc.kind != LOSS_FVP) { pf_logp = __ldg(p.b.logp + prow); pf_advr = __ldg(p.b.adv_r + prow); pf_advc = __ldg(p.b.adv_c + prow); }
                         } else {
                             pf_tv = __ldg((net == 1 ? p.b.tv_r : p.b.tv_c) + prow);
                         }
@@ -542,6 +544,11 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                             acc_st[0] += d * d; acc_st[3] += 1.f;
                             d16[0] = 2.f * d * inv_b;
                             acc_db[0] += d16[0];
+                        } else if (DMU) {
+                            acc_st[3] += 1.f;
+#pragma unroll
+                            for (int a = 0; a < AP; ++a)
+                                if (a < A) { d16[a] = pf_act[a]; acc_db[a] += pf_act[a]; }
                         } else if (p.lc.kind == LOSS_FVP) {
                             // J^T diag(sigma^-2) dmu / (B A): the supplied tangent is the output gradient
                             acc_st[3] += 1.f;
@@ -942,6 +949,8 @@ static int x3_set_attr() {
         OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<false, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<true, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<true, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<false, 8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<false, 16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = true;
     }
     return OSB_OK;
@@ -1077,3 +1086,23 @@ int osb_ppo_update_iter_x3(float* theta, float* grad, float* adam_m, float* adam
 }
 
 }  // extern "C"
+
+// LOSS_DMU launch behind osb_actor_dmu_backward (csrc/update.cu)
+int osb::dmu_backward_x3(const float* theta_actor, int O, int A, const float* obs, const float* dmu, int rows, float* gpart,
+                         float* stats_scratch, cudaStream_t stream) {
+    OSB_CHECK_ARG(O <= 64 && A <= 16, "bf16x3 path needs O <= 64, A <= 16");
+    X3Args p = {};
+    p.b = Batch{obs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, rows, 0u, 0, rows, 1};
+    p.lc.kind = LOSS_DMU; p.lc.focops_lam = 1.f; p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch;
+    p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
+    p.batch_size = rows; p.world = 1; p.dbg = nullptr;
+    p.fvp_dmu = dmu;
+    const int nb = osb_tc_grid_blocks(rows, 1);
+    int rc = x3_set_attr();
+    if (rc) return rc;
+    if ((rc = x3_bind_acc(p, nb))) return rc;
+    if (A <= 8) minibatch_grad_x3_kernel<false, 8, true><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
+    else minibatch_grad_x3_kernel<false, 16, true><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}
