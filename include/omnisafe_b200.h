@@ -502,6 +502,13 @@ int osb_umma_selftest(const float* A, const float* B, int M, int N, int K, int a
  * kernels issue (csrc/x3_selftest.cu); any other shape is refused. */
 int osb_x3_selftest(const float* A, const float* B, int M, int N, int K, int a_mn, int b_mn, int a_sw,
                     int b_sw, int b_ones, float* out, void* stream);
+/* The row-half products of the bf16x3 update kernel (gemm_x3_rows, csrc/x3.cuh): D = A * B^T with A [128][K] consumed
+ * K-major and B [N][K], issued as one m64 block per row half over the whole K (K = 64: two wgmma chains whose fp32 sum
+ * is stored) into out[128][N], and as the M = 128 product in column-half phases (the second adding to the image) into
+ * out_phases[128][N]; the two must agree bit for bit (tests/test_update_rowhalf_gpu.py).  (N, K, b_mn) must be one of
+ * the shapes the update kernel issues. */
+int osb_x3_rows_selftest(const float* A, const float* B, int N, int K, int b_mn, int a_sw, int b_sw, float* out,
+                         float* out_phases, void* stream);
 int osb_x3_debug_buffer(long long* buf);
 /* development aid: clock64 stamps of CTA 0 of the streaming GAE kernel (tools/gae_stage_times.py); NULL turns it off */
 int osb_gae_debug_buffer(long long* buf);

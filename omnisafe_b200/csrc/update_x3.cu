@@ -16,9 +16,12 @@
 //     dZ2' = dOUT W3            -> dZ2 = dZ2' (1 - H2^2)   (stored over H2)     | dW3^T += H2^T dOUT
 //     dZ1' = dZ2 W2             -> dZ1 = dZ1' (1 - H1^2)   (stored over H1)     | dW2 += dZ2^T H1, db2 += dZ2^T 1
 //                                                                               | dW1 += dZ1^T X,  db1 += dZ1^T 1
-//   Every epilogue writes its activation in two column halves, each announced by its own mbarrier, so the
-//   next layer's MMAs start on k-steps 0-1 while the epilogue still produces k-steps 2-3; weight / bias
-//   gradient MMAs run behind the dependent chain while the epilogue warps work.  The loss warps' per-sample inputs
+//   Rows 0-63 and rows 64-127 of a tile never meet in the forward and backward chain (only the weight-gradient
+//   products contract over samples), so the tile runs as a pipeline of its two row halves: every product of the chain
+//   is one m64 block per half over the whole K, stored once and committed on that half's mbarrier, and every epilogue
+//   warp waits for and announces its own half only -- the epilogue of rows 0-63 runs under the MMAs of rows 64-127 and
+//   the next product of rows 0-63 under the epilogue of rows 64-127.  Weight / bias gradient MMAs run behind the
+//   dependent chain and release their operands as soon as they have read them.  The loss warps' per-sample inputs
 //   are copied asynchronously into shared memory (cp.async) at the start of the tile.
 //
 // FUSED instantiation = the persistent cooperative kernel of one update iteration: after each minibatch the partial
@@ -86,8 +89,25 @@ constexpr int MF_B1 = 0, MF_B2 = 64, MF_B3 = 128, MF_LS = 144 /* logstd[16] sigm
               MF_RED = 200 /* [4*8 + 4*16 + 4*16] */, MF_B3ACC = 360, MF_PART = 376 /* [2][256] */, MF_SCAL = 888 /* [16] */, MF_OLD = 904 /* log sigma_old[16], 1 / sigma_old^2 [16] */, MF_END = 936;
 constexpr uint32_t OFF_ROWS = OFF_MISC + MF_END * 4;                 // long long [2][128]
 constexpr uint32_t OFF_BARS = OFF_ROWS + 2 * XT * 8;                 // uint64 [NBAR]
-enum Bar { RDY_X0 = 0, RDY_X1, RDY_H1_0, RDY_H1_1, RDY_H2_0, RDY_H2_1, RDY_D, RDY_DZ2_0, RDY_DZ2_1, RDY_DZ1,
-           DONE_C1, DONE_C2, DONE_C3, DONE_C4A, DONE_C4B, DONE_C5A, DONE_C5B, DONE_C6, RDY_W, NBAR };
+// mbarriers.  Each completes exactly one phase per tile (waiters use the parity of the CTA's tile counter).  _0 / _1 =
+// rows 0-63 / 64-127 of the tile; an epilogue warp (q = warp % 4 owns rows 32 q .. 32 q + 31) belongs to half q / 2.
+enum Bar {
+    // epilogue warps -> MMA-issue warpgroup, one arrival per warp: the operand's rows of that half are stored
+    RDY_X0 = 0, RDY_X1,            // 8: X is staged by row tid / 4, warps 0-7 rows 0-63, warps 8-15 rows 64-127
+    RDY_H1_0, RDY_H1_1,            // 8
+    RDY_H2_0, RDY_H2_1,            // 8
+    RDY_D0, RDY_D1,                // 2: the loss warps (warp / 4 == 0) of the half
+    RDY_DZ2_0, RDY_DZ2_1,          // 8
+    RDY_DZ1_0, RDY_DZ1_1,          // 8
+    // MMA-issue warpgroup -> epilogue warps, one arrival: the product's rows of that half are in the image
+    DONE_C1_0, DONE_C1_1, DONE_C2_0, DONE_C2_1, DONE_C3_0, DONE_C3_1, DONE_C4A_0, DONE_C4A_1, DONE_C5A_0, DONE_C5A_1,
+    // one arrival, all 16 warps wait: the MMAs of dW3 have read H2, of dW2 H2 and H1, of dW1 X -- dZ2, dZ1 and the
+    // next tile's X may be stored over them
+    DONE_C4B, DONE_C5B, FREE_X,
+    DONE_C6,                       // 1: the tile's last gradient product is in the image
+    RDY_W,                         // 1: the expect_tx arrival of the weight-image bulk copy
+    NBAR };
+__host__ __device__ constexpr uint32_t bar_arrivals(int b) { return b >= DONE_C1_0 ? 1u : (b == RDY_D0 || b == RDY_D1) ? 2u : 8u; }
 constexpr uint32_t OFF_PF = OFF_BARS + NBAR * 8 + 16;                       // float [128][12]: per-sample loss inputs (AP == 8), copied asynchronously
 constexpr int PF_LD = 12;
 constexpr uint32_t X3_SMEM = OFF_PF + XT * PF_LD * 4;
@@ -213,10 +233,8 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
             stage_policy_old(misc + MF_OLD, tid, (tid < A) ? __ldg(p.lc.logstd_old + tid) : 0.f);
     } else {
         if (tid == NEPI) {
-            for (int i = 0; i < NBAR; ++i) {
-                const uint32_t cnt = (i >= DONE_C1) ? 1u : (i == RDY_D ? 4u : 16u);      // (RDY_W: one expect_tx arrival)
-                asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar(i)), "r"(cnt) : "memory");
-            }
+            for (int i = 0; i < NBAR; ++i)
+                asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar(i)), "r"(bar_arrivals(i)) : "memory");
             mbar_init_fence();
         }
     }
@@ -230,8 +248,8 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
         const uint64_t dD = desc32(sbase + OFF_D), dW1 = desc128(sbase + OFF_W1), dW2 = desc128(sbase + OFF_W2);
         const uint64_t dW3 = desc128(sbase + OFF_W3), dOnes = desc32(sbase + OFF_ONES);
         // stage-time stamps of this warpgroup (third region of p.dbg).  Ids: 100 + 20 k for product k of Z1, Z2, OUT, dZ2',
-        // dZ1', plus 4 ph + {0: operands ready, 1 / 2: MMAs of rows 0-63 / 64-127 complete, 3: image stored} for column-half
-        // phase ph, plus 8 once the product is committed; 200 / 201 / 202: dW3, dW2 and the last gradient product committed.
+        // dZ1', plus 4 r + {0: operands ready, 1: MMAs complete, 2: image stored, 3: committed} for row half r;
+        // 200 / 201 / 202: dW3, dW2 and dW1 have read their operands; 203: the last gradient product committed.
         const bool mdbg_on = p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && tid == NEPI;
         int mdbg_n = 0;
         auto mstamp = [&](int id) {
@@ -250,75 +268,78 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 const uint32_t par = (uint32_t)(it & 1);
                 const bool first = tile == (int)blockIdx.x;         // the first tile of a minibatch overwrites the accumulators
                 const bool last = tile + G >= ntiles;
-                // Z1 = X W1^T  (k-steps 0-1 after the first column half of X, 2-3 after the second)
+                // Z1 = X W1^T, one row half after the other: each half is stored and committed on its own, and the epilogue
+                // of rows 0-63 runs under the MMAs of rows 64-127
 #pragma unroll 1
-                for (int ph = 0; ph < 2; ++ph) {
-                    mbar_wait_a(bar(RDY_X0 + ph), par);
-                    mstamp(100 + 4 * ph);
-                    gemm_x3<128, 64, 2, 0, 0>(tm, T_ZA, desc_add(dX, 64u * ph), ACT_SUB, 32u, desc_add(dW1, 64u * ph), W_SUB, 32u, ph > 0, [&](int half) { mstamp(100 + 4 * ph + 1 + half); });
-                    mstamp(100 + 4 * ph + 3);
+                for (int r = 0; r < 2; ++r) {
+                    mbar_wait_a(bar(RDY_X0 + r), par);
+                    mstamp(100 + 4 * r);
+                    gemm_x3_rows<64, 2, 2, 0>(tm, T_ZA, r, dX, ACT_SUB, 32u, dW1, W_SUB, 32u, [&](int) { mstamp(101 + 4 * r); });
+                    mstamp(102 + 4 * r);
+                    mma_commit_a(bar(DONE_C1_0 + r));
+                    mstamp(103 + 4 * r);
                 }
-                mma_commit_a(bar(DONE_C1));
-                mstamp(108);
                 // db2 of the PREVIOUS tile (dZ2 still sits in the H2 buffer until this tile's E2): runs under E1,
-                // completes before Z2 (in-order pipe), so DONE_C2 covers it
+                // completes before Z2 (in-order pipe), so DONE_C2_0 / _1 cover it
                 if (!first && !(!FUSED && p.forward_only)) gemm_x3<64, 16, 8, 1, 1, true>(tm, T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, tile != (int)blockIdx.x + G);
                 // Z2 = H1 W2^T
 #pragma unroll 1
-                for (int ph = 0; ph < 2; ++ph) {
-                    mbar_wait_a(bar(RDY_H1_0 + ph), par);
-                    mstamp(120 + 4 * ph);
-                    gemm_x3<128, 64, 2, 0, 0>(tm, T_ZB, desc_add(dH1, 64u * ph), ACT_SUB, 32u, desc_add(dW2, 64u * ph), W_SUB, 32u, ph > 0, [&](int half) { mstamp(120 + 4 * ph + 1 + half); });
-                    mstamp(120 + 4 * ph + 3);
+                for (int r = 0; r < 2; ++r) {
+                    mbar_wait_a(bar(RDY_H1_0 + r), par);
+                    mstamp(120 + 4 * r);
+                    gemm_x3_rows<64, 2, 2, 0>(tm, T_ZB, r, dH1, ACT_SUB, 32u, dW2, W_SUB, 32u, [&](int) { mstamp(121 + 4 * r); });
+                    mstamp(122 + 4 * r);
+                    mma_commit_a(bar(DONE_C2_0 + r));
+                    mstamp(123 + 4 * r);
                 }
-                mma_commit_a(bar(DONE_C2));
-                mstamp(128);
                 // OUT = H2 W3^T
 #pragma unroll 1
-                for (int ph = 0; ph < 2; ++ph) {
-                    mbar_wait_a(bar(RDY_H2_0 + ph), par);
-                    mstamp(140 + 4 * ph);
-                    gemm_x3<128, 16, 2, 0, 0>(tm, T_OUT, desc_add(dH2, 64u * ph), ACT_SUB, 32u, desc_add(dW3, 64u * ph), W3_SUB, 32u, ph > 0, [&](int half) { mstamp(140 + 4 * ph + 1 + half); });
-                    mstamp(140 + 4 * ph + 3);
+                for (int r = 0; r < 2; ++r) {
+                    mbar_wait_a(bar(RDY_H2_0 + r), par);
+                    mstamp(140 + 4 * r);
+                    gemm_x3_rows<16, 2, 2, 0>(tm, T_OUT, r, dH2, ACT_SUB, 32u, dW3, W3_SUB, 32u, [&](int) { mstamp(141 + 4 * r); });
+                    mstamp(142 + 4 * r);
+                    mma_commit_a(bar(DONE_C3_0 + r));
+                    mstamp(143 + 4 * r);
                 }
-                mma_commit_a(bar(DONE_C3));
-                mstamp(148);
                 if (!FUSED && p.forward_only) continue;              // statistics pass (FOCOPS mask mean): no backward
-                // dZ2' = dOUT W3 ; dW3^T += H2^T dOUT
-                mbar_wait_a(bar(RDY_D), par);
-                mstamp(160);
-                gemm_x3<128, 64, 1, 0, 1>(tm, T_ZA, dD, D_SUB, 32u, dW3, W3_SUB, 2048u, false, [&](int half) { mstamp(161 + half); });
-                mstamp(163);
-                mma_commit_a(bar(DONE_C4A));
-                mstamp(168);
-                gemm_x3<64, 16, 8, 1, 1>(tm, T_DW3, dH2, ACT_SUB, 2048u, dD, D_SUB, 512u, !first);
-                mma_commit_a(bar(DONE_C4B));
-                mstamp(200);
+                // dZ2' = dOUT W3 ; dW3^T += H2^T dOUT (all 128 samples: behind both halves)
+#pragma unroll 1
+                for (int r = 0; r < 2; ++r) {
+                    mbar_wait_a(bar(RDY_D0 + r), par);
+                    mstamp(160 + 4 * r);
+                    gemm_x3_rows<64, 1, 1, 1>(tm, T_ZA, r, dD, D_SUB, 32u, dW3, W3_SUB, 2048u, [&](int) { mstamp(161 + 4 * r); });
+                    mstamp(162 + 4 * r);
+                    mma_commit_a(bar(DONE_C4A_0 + r));
+                    mstamp(163 + 4 * r);
+                }
+                // H2 is free for dZ2 once dW3's MMAs have read it; the gradient images are read only after DONE_C6
+                gemm_x3<64, 16, 8, 1, 1>(tm, T_DW3, dH2, ACT_SUB, 2048u, dD, D_SUB, 512u, !first, [&](int) { mma_release_a(bar(DONE_C4B)); mstamp(200); });
                 // dZ1' = dZ2 W2 ; dW2 += dZ2^T H1
 #pragma unroll 1
-                for (int ph = 0; ph < 2; ++ph) {
-                    mbar_wait_a(bar(RDY_DZ2_0 + ph), par);
-                    mstamp(180 + 4 * ph);
-                    gemm_x3<128, 64, 2, 0, 1>(tm, T_ZB, desc_add(dH2, 64u * ph), ACT_SUB, 32u, desc_add(dW2, 4096u * ph), W_SUB, 2048u, ph > 0, [&](int half) { mstamp(180 + 4 * ph + 1 + half); });
-                    mstamp(180 + 4 * ph + 3);
+                for (int r = 0; r < 2; ++r) {
+                    mbar_wait_a(bar(RDY_DZ2_0 + r), par);
+                    mstamp(180 + 4 * r);
+                    gemm_x3_rows<64, 2, 2, 1>(tm, T_ZB, r, dH2, ACT_SUB, 32u, dW2, W_SUB, 2048u, [&](int) { mstamp(181 + 4 * r); });
+                    mstamp(182 + 4 * r);
+                    mma_commit_a(bar(DONE_C5A_0 + r));
+                    mstamp(183 + 4 * r);
                 }
-                mma_commit_a(bar(DONE_C5A));
-                mstamp(188);
-                gemm_x3<64, 64, 8, 1, 1>(tm, T_DW2, dH2, ACT_SUB, 2048u, dH1, ACT_SUB, 2048u, !first);
-                mma_commit_a(bar(DONE_C5B));
-                mstamp(201);
-                // dW1 += dZ1^T X (column 63 = db1 with the ones column) ; last tile of the minibatch: its own db2
-                mbar_wait_a(bar(RDY_DZ1), par);
-                gemm_x3<64, 64, 8, 1, 1>(tm, T_DW1, dH1, ACT_SUB, 2048u, dX, ACT_SUB, 2048u, !first);
+                gemm_x3<64, 64, 8, 1, 1>(tm, T_DW2, dH2, ACT_SUB, 2048u, dH1, ACT_SUB, 2048u, !first, [&](int) { mma_release_a(bar(DONE_C5B)); mstamp(201); });
+                // dW1 += dZ1^T X (column 63 = db1 with the ones column) ; last tile of the minibatch: its own db2.  Only dW1
+                // reads X, and dZ1 / dZ2 are overwritten no earlier than the next tile's E1 / E2, behind its Z1 / Z2.
+                mbar_wait_a(bar(RDY_DZ1_0), par);
+                mbar_wait_a(bar(RDY_DZ1_1), par);
+                gemm_x3<64, 64, 8, 1, 1>(tm, T_DW1, dH1, ACT_SUB, 2048u, dX, ACT_SUB, 2048u, !first, [&](int) { mma_release_a(bar(FREE_X)); mstamp(202); });
                 if (!ones_col) gemm_x3<64, 16, 8, 1, 1, true>(tm, T_DB1, dH1, ACT_SUB, 2048u, dOnes, 0u, 0u, !first);
                 if (last) gemm_x3<64, 16, 8, 1, 1, true>(tm, T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, !first);
                 mma_commit_a(bar(DONE_C6));
-                mstamp(202);
+                mstamp(203);
             }
         }
     } else {
         // ======================= epilogue warps ===============================================================
-        const int q = warp & 3, h = warp >> 2;
+        const int q = warp & 3, h = warp >> 2, rh = q >> 1;      // rh: the row half of this warp's rows (all but the X staging)
         const uint32_t lane_base = (uint32_t)(q * 32) << 16;
         const int s_row = 32 * q + lane;                 // sample row of this thread in the [s][.] accumulators
         const AdvNorm an = adv_norm(p.b.moments, p.lc.lagrange);
@@ -349,12 +370,12 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
             }
             if (ones_col && xc == 24) xpre[15] = 1.0f;     // column 63: the ones column (every row: padding rows have dZ1 = 0)
         };
-        auto announce = [&](int b) {        // this warp's stores of one column half are visible to the tensor core
+        auto announce = [&](int b) {        // this warp's stores are visible to the tensor core
             fence_async_smem();
             __syncwarp();
             if (lane == 0) mbar_arrive(bar(b));
         };
-        const bool dbg_on = p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && (tid == 0 || tid == 256);
+        const bool dbg_on = p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && (tid == 0 || tid == 320);      // a loss warp of rows 0-63, a non-loss warp of rows 64-127
         int dbg_n = 0;
         auto stamp = [&](int id) {
             if (dbg_on && dbg_n < 400) {
@@ -433,7 +454,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 // ---- E0: X tile (prefetched registers -> bf16x3) ------------------------------------------------
                 stamp(0);
                 if (has_next) tile_rows(mb, tile + G, sRowNext);
-                if (it > 0 && !(!FUSED && p.forward_only)) mbar_wait_a(bar(DONE_C6), par ^ 1u);   // previous tile's dW1 / db1 read X and dZ1
+                if (it > 0 && !(!FUSED && p.forward_only)) mbar_wait_a(bar(FREE_X), par ^ 1u);    // previous tile's dW1 has read X
                 stamp(1);
 #pragma unroll
                 for (int ph = 0; ph < 2; ++ph) {
@@ -441,8 +462,8 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll
                     for (int i = 0; i < 8; ++i) v[i] = xpre[8 * ph + i];
                     store8_x3(sbase + OFF_X, ACT_SUB, xm, 32 * ph + xc, v);
-                    announce(RDY_X0 + ph);
                 }
+                announce(RDY_X0 + (warp >> 3));                            // rows xm = tid / 4: warps 0-7 hold rows 0-63
                 epi_bar_sync();                                            // next tile's row list is complete
                 stamp(2);
                 // loss warps: this tile's per-sample inputs (used in E3) fly under the forward phases -- asynchronously into
@@ -479,7 +500,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     }
                 }
                 // ---- E1: H1 = tanh(Z1 + b1) -------------------------------------------------------------------
-                mbar_wait_a(bar(DONE_C1), par);
+                mbar_wait_a(bar(DONE_C1_0 + rh), par);
                 stamp(3);
 #pragma unroll
                 for (int ph = 0; ph < 2; ++ph) {
@@ -489,11 +510,11 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll
                     for (int i = 0; i < 8; ++i) v[i] = tanh_acc(v[i] + sB1[c0 + i]);
                     store8_x3(sbase + OFF_H1, ACT_SUB, s_row, c0, v);
-                    announce(RDY_H1_0 + ph);
                 }
+                announce(RDY_H1_0 + rh);
                 // ---- E2: H2 = tanh(Z2 + b2) -------------------------------------------------------------------
                 stamp(4);
-                mbar_wait_a(bar(DONE_C2), par);
+                mbar_wait_a(bar(DONE_C2_0 + rh), par);
                 stamp(5);
 #pragma unroll
                 for (int ph = 0; ph < 2; ++ph) {
@@ -503,8 +524,8 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll
                     for (int i = 0; i < 8; ++i) v[i] = tanh_acc(v[i] + sB2[c0 + i]);
                     store8_x3(sbase + OFF_H2, ACT_SUB, s_row, c0, v);
-                    announce(RDY_H2_0 + ph);
                 }
+                announce(RDY_H2_0 + rh);
                 stamp(6);
                 // ---- E3: OUT -> loss -> dOUT (warps with h == 0: one thread per sample) -------------------------
                 if (h == 0) {
@@ -522,7 +543,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                             }
                         }
                     }
-                    mbar_wait_a(bar(DONE_C3), par);
+                    mbar_wait_a(bar(DONE_C3_0 + rh), par);
                     stamp(7);
                     float o[AP], d16[16];
 #pragma unroll
@@ -572,19 +593,19 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                         }
                     }
                     store16_x3_sw32(sbase + OFF_D, D_SUB, s_row, d16);
-                    announce(RDY_D);
+                    announce(RDY_D0 + rh);
                     stamp(8);
                 }
                 stamp(9);
                 if (!FUSED && p.forward_only) {                                      // statistics pass: no backward; H2 is free once OUT is done
                     if (has_next) prefetch_x(sRowNext);
-                    if (h != 0) { mbar_wait_a(bar(DONE_C3), par); }
+                    if (h != 0) { mbar_wait_a(bar(DONE_C3_0 + rh), par); }
                     rpar ^= 1;
                     continue;
                 }
                 // ---- E4: dZ2 = (dOUT W3) (1 - H2^2), stored over H2 once dW3 has read it --------------------------
                 if (has_next) prefetch_x(sRowNext);                        // next tile's rows fly during the backward half
-                mbar_wait_a(bar(DONE_C4A), par);
+                mbar_wait_a(bar(DONE_C4A_0 + rh), par);
                 stamp(10);
                 float dz[16];
 #pragma unroll
@@ -605,11 +626,11 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll
                     for (int i = 0; i < 8; ++i) v[i] = dz[8 * ph + i];
                     store8_x3(sbase + OFF_H2, ACT_SUB, s_row, 32 * ph + 8 * h, v);
-                    announce(RDY_DZ2_0 + ph);
                 }
+                announce(RDY_DZ2_0 + rh);
                 // ---- E5: dZ1 = (dZ2 W2) (1 - H1^2), stored over H1 once dW2 has read it --------------------------
                 stamp(13);
-                mbar_wait_a(bar(DONE_C5A), par);
+                mbar_wait_a(bar(DONE_C5A_0 + rh), par);
                 stamp(14);
 #pragma unroll
                 for (int ph = 0; ph < 2; ++ph) {
@@ -630,7 +651,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     for (int i = 0; i < 8; ++i) v[i] = dz[8 * ph + i];
                     store8_x3(sbase + OFF_H1, ACT_SUB, s_row, 32 * ph + 8 * h, v);
                 }
-                announce(RDY_DZ1);
+                announce(RDY_DZ1_0 + rh);
                 stamp(17);
                 rpar ^= 1;
             }

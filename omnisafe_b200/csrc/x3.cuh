@@ -86,7 +86,8 @@ __device__ __forceinline__ void x3_block(float (&d)[4 * NJ], uint64_t a0, uint32
 // M = 128 issues both m64 halves before draining the first: half 0 is stored while half 1 runs.  A product that adds
 // to the image reads the old values in batches of independent loads, the first batch before it waits on its MMAs.
 // Either way the stored value is d, or d + old, as one fp32 add.
-// `waited(half)` is called when the MMAs of m64 half `half` have completed (stage-time stamps; nothing by default).
+// `waited(half)` is called when the MMAs of m64 half `half` have completed and before the image is written: for
+// stage-time stamps, and for releasing the operands to their next writer (nothing by default).
 struct NoStamp {
     __device__ __forceinline__ void operator()(int) const {}
 };
@@ -109,6 +110,7 @@ __device__ __forceinline__ void gemm_x3(const Acc& acc, uint32_t d_addr, uint64_
         if (accumulate) frag_load<NJ>(acc, d_addr, M, 0, old);
         wg_wait<0>();
         acc_fence(d);
+        waited(0);
         if (accumulate) frag_add_store<NJ>(acc, d_addr, M, 0, d, old);
         else frag_store<NJ>(acc, d_addr, M, 0, d);
     } else {
@@ -153,6 +155,43 @@ __device__ __forceinline__ void gemm_x3(const Acc& acc, uint32_t d_addr, uint64_
             frag_store<NJ>(acc, d_addr, M, 1, d1);
         }
     }
+}
+
+// Rows 64 r .. 64 r + 63 (r = 0 or 1) of a 128-row product with a K-major A, as one m64 block over the whole K, stored
+// once into the image rows of the M = 128 product at d_addr (row m in lane m).  The two row halves of a product share
+// nothing but B, so each can be issued, stored and announced on its own.
+//   NC = 2: K is split into two runs of NK k-steps; each run is its own wgmma chain, started from zero into its own
+//   fragment and both in flight together, and the stored value is the fp32 sum of the two chains, one add per element.
+//   That is the value two column-half phases of gemm_x3<128, ...> leave in the image (the second accumulating), bit for
+//   bit, without the image read.  One chain over all 2 NK k-steps would save the add and a fragment and round differently.
+//   NC = 1: one chain of NK k-steps, stored as it is.
+// a0 / b0 and the strides as for gemm_x3; `waited(r)` is called when the MMAs have completed.
+template <int N, int NK, int NC, int TB, class Stamp = NoStamp>
+__device__ __forceinline__ void gemm_x3_rows(const Acc& acc, uint32_t d_addr, int r, uint64_t a0, uint32_t asplit,
+                                             uint32_t akstep, uint64_t b0, uint32_t bsplit, uint32_t bkstep,
+                                             Stamp waited = Stamp()) {
+    static_assert((N == 16 || N == 64) && (NC == 1 || NC == 2), "unsupported bf16x3 row-half GEMM shape");
+    constexpr int NJ = N / 8;
+    a0 = desc_fresh(a0);
+    b0 = desc_fresh(b0);
+    a0 = desc_add(a0, (uint32_t)r * 64u * (((a0 >> 61) & 7u) == 2u ? 128u : 32u));
+    float d[4 * NJ] = {};
+    x3_block<0, TB, NJ, NK, false>(d, a0, asplit, akstep, b0, bsplit, bkstep);
+    if constexpr (NC == 2) {
+        float d1[4 * NJ] = {};
+        x3_block<0, TB, NJ, NK, false>(d1, desc_add(a0, NK * akstep), asplit, akstep, desc_add(b0, NK * bkstep), bsplit, bkstep);
+        wg_wait<0>();
+        acc_fence(d);
+        acc_fence(d1);
+        waited(r);
+#pragma unroll
+        for (int i = 0; i < 4 * NJ; ++i) d[i] += d1[i];
+    } else {
+        wg_wait<0>();
+        acc_fence(d);
+        waited(r);
+    }
+    frag_store<NJ>(acc, d_addr, 128, r, d);
 }
 
 // ---- fp32 <-> three bf16 ----------------------------------------------------------------------------
@@ -258,6 +297,12 @@ __device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
 // mma_commit on a 32-bit shared address
 __device__ __forceinline__ void mma_commit_a(uint32_t bar) {
     __threadfence_block();
+    asm volatile("bar.sync 3, 128;\n" ::: "memory");
+    if ((threadIdx.x & 127) == 0) mbar_arrive(bar);
+}
+// The warpgroup's MMAs have read their operands: one arrival for the warps that overwrite them.  Called by all 128
+// threads once each is past its wgmma wait; nothing those warps read was written here, so there is no fence.
+__device__ __forceinline__ void mma_release_a(uint32_t bar) {
     asm volatile("bar.sync 3, 128;\n" ::: "memory");
     if ((threadIdx.x & 127) == 0) mbar_arrive(bar);
 }
