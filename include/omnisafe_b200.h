@@ -395,6 +395,17 @@ int osb_fvp_partials_x3(const float* theta_actor, const float* vec, int O, int A
 int osb_actor_dmu_grid_blocks(int rows, int O, int precision);
 int osb_actor_dmu_backward(const float* theta_actor, int O, int A, const float* obs, const float* dmu, int rows,
                            int precision, float* gpart, float* stats_scratch, void* stream);
+/* Critic backward with a supplied output gradient (LOSS_DMU on a critic): the backward of critic losses written in
+ * PyTorch.  theta: the flat [actor | reward critic | cost critic] parameters (P floats); net 1 = reward critic, 2 = cost
+ * critic; obs [rows][O] (contiguous, normalised), dv [rows] = dL/dV.  gpart <- per-CTA partials of J_V^T dv,
+ * osb_critic_dv_grid_blocks(rows, O, precision) rows of P floats of which the critic's segment (at its offset in theta)
+ * is written, as osb_minibatch_grad{,_tc,_x3} write it; stats_scratch: that many * 24 floats.  value [rows] (may be
+ * NULL) <- the forward V of the launch.  Reduce with osb_reduce_partials.  The kernels, tiles and CTAs are those of a
+ * stepwise update launch of that critic alone over `rows` samples (precision chosen as for osb_actor_dmu_backward), so
+ * `value` has the bits of the update kernels' critic forward: with dv = 0 the entry is that forward. */
+int osb_critic_dv_grid_blocks(int rows, int O, int precision);
+int osb_critic_dv_backward(const float* theta, int O, int A, int net, const float* obs, const float* dv, float* value,
+                           int rows, int precision, float* gpart, float* stats_scratch, void* stream);
 
 /* ---- optimiser side --------------------------------------------------------------------------
  * osb_grad_reduce: grad <- sum of CTA partials (+ 2*critic_norm_coef*theta for critics,

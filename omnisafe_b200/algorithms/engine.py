@@ -97,7 +97,7 @@ class UpdateEngine:
             distributed.nccl_comm(), distributed.world_size(), *distributed.p2p_exchange(self.P)[:2],
             distributed.get_rank(), distributed.p2p_exchange(self.P)[2], current_stream())
 
-    # ---- PolicyGradient._update with the actor objective in PyTorch ------------------------
+    # ---- PolicyGradient._update with objectives in PyTorch ---------------------------------
     def _optim_step(self, gpart, stats_part, nb, net_mask, critic_norm_coef, max_grad_norm, lr_actor, lr_critic):
         """Reduce the partials, clip, average over ranks and Adam-step the networks of `net_mask` (the order of
         osb_ppo_update_epoch)."""
@@ -119,30 +119,62 @@ class UpdateEngine:
                                 float(lr_critic), float(lr_critic), float(scale), float(critic_norm_coef),
                                 ptr(self.train_stats), do_clip, do_adam, net_mask, ptr(self.stop_flag), s)
 
-    def torch_actor_epoch(self, actor_step, *, lagrange, net_mask, batch_size, update_iters, critic_norm_coef=0.0,
-                          max_grad_norm=0.0, lr_actor=0.0, lr_critic=0.0, target_kl=0.0, kl_early_stop=False,
-                          perm=None) -> None:
-        """ppo_epoch with the actor trained through autograd: per minibatch of the same sample order the kernels draw
-        (or `perm`), the critics of `net_mask` take their kernel step, then `actor_step(rows)` returns (loss, gradient
-        of the actor parameters) for the slab rows `rows` [count] (int64), which is clipped, rank-averaged and
-        Adam-stepped by the kernels.  After each pass the full-batch KL check runs as in ppo_epoch."""
+    def adam_step(self, net: int, grad: torch.Tensor, lr: float) -> None:
+        """torch.optim.Adam.step() of critic `net` (1 reward, 2 cost) on `grad`, its flat gradient as its optimiser
+        holds it (clipped and rank-averaged by the caller, or not): the kernels' Adam on that network's slice of theta,
+        with its step count and `lr`.  Nothing is clipped, averaged or added here."""
+        a, s = self.agent, current_stream()
+        if not hasattr(self, 'hook_gpart'):
+            self.hook_gpart = torch.zeros(self.P, dtype=torch.float32, device=a.device)
+            self.hook_stats = torch.zeros(3 * 8, dtype=torch.float32, device=a.device)
+        lay = a.layout['reward_critic' if net == 1 else 'cost_critic']
+        self.hook_gpart[lay['start']:lay['start'] + lay['size']].copy_(grad)
+        self.hook_stats.zero_()
+        self.hook_stats[8 * net + 3] = 1.0
+        lib().osb_grad_reduce(ptr(self.hook_gpart), ptr(self.hook_stats), 1, self.O, self.A, ptr(a.theta), ptr(a.grad),
+                              0.0, 1 << net, ptr(self.sumsq_part), ptr(a.adam_step), ptr(self.train_stats), 0, s)
+        lib().osb_clip_adam(ptr(a.grad), ptr(a.theta), ptr(a.adam_m), ptr(a.adam_v), ptr(a.adam_step),
+                            ptr(self.sumsq_part), self.O, self.A, 0.0, 0.0, float(lr), float(lr), 1.0, 0.0,
+                            ptr(self.train_stats), 0, 1, 1 << net, 0, s)
+
+    def stepwise_epoch(self, steps: dict, *, loss_kind, lagrange, net_mask, batch_size, update_iters, clip=0.2,
+                       entropy_coef=0.0, focops_lam=1.0, focops_eta=0.0, critic_norm_coef=0.0, max_grad_norm=0.0,
+                       lr_actor=0.0, lr_critic=0.0, target_kl=0.0, kl_early_stop=False, perm=None) -> None:
+        """ppo_epoch as a host loop of minibatch steps, with networks trained through autograd.  Per minibatch of the
+        sample order the kernels draw (or `perm`), the networks of `net_mask` step in the reference's order: reward
+        critic, cost critic, actor.  A network with a callable in `steps` (net bit -> callable(rows), rows the slab
+        rows [count] int64) runs it; the others take the stepwise kernel step (osb_minibatch_grad* + the optimiser),
+        consecutive ones in one launch.  The actor's callable returns (loss, gradient of the actor parameters), which
+        the kernels clip, rank-average and Adam-step; a critic's callable trains its network itself.  When the actor
+        trains, the old policy is snapshotted first and the full-batch KL check runs after each pass, as in ppo_epoch."""
         a, s = self.agent, current_stream()
         if perm is not None:
             assert perm.dtype == torch.int32 and perm.shape == (update_iters, self.total)
         self.stop_flag.zero_()
         self.kl_state.zero_()
         self.train_stats.zero_()
-        self.snapshot_old_policy()
+        train_actor = bool(net_mask & NET_ACTOR)
+        if train_actor:
+            self.snapshot_old_policy()
         if not hasattr(self, 'actor_gpart'):
             self.actor_gpart = torch.zeros(self.P, dtype=torch.float32, device=a.device)
             self.actor_stats = torch.zeros(3 * 8, dtype=torch.float32, device=a.device)
         seed = self.next_perm_seed()
-        critics = net_mask & (NET_CRITIC_R | NET_CRITIC_C)
         opt = dict(critic_norm_coef=critic_norm_coef, max_grad_norm=max_grad_norm, lr_actor=lr_actor,
                    lr_critic=lr_critic)
         tiles = self._tc() or self._x3()
         grad_fn = lib().osb_minibatch_grad_x3 if self._x3() else (lib().osb_minibatch_grad_tc if self._tc()
                                                                    else lib().osb_minibatch_grad)
+
+        def kernel_step(mask, order, start, count):
+            loss = ((int(loss_kind), float(clip), float(entropy_coef), float(focops_lam), float(focops_eta),
+                     ptr(lagrange)) if mask & NET_ACTOR else (LOSS_RATIO, 0.0, 0.0, 1.0, 0.0, 0))
+            grad_fn(ptr(a.theta), self.O, self.A, *self._batch_ptrs(), ptr(self.mu_old), ptr(self.buf.adv_moments),
+                    ptr(order), self.total, 0, start, count, *loss, ptr(self.logstd_old), mask, ptr(self.gpart),
+                    ptr(self.stats_part), ptr(self.stop_flag), s)
+            nb = lib().osb_tc_grid_blocks(count, mask) if tiles else lib().osb_update_grid_blocks(count)
+            self._optim_step(self.gpart, self.stats_part, nb, mask, **opt)
+
         for it in range(update_iters):
             if perm is not None:
                 order = perm[it].contiguous()
@@ -152,18 +184,29 @@ class UpdateEngine:
             rows_all = order.to(torch.int64)
             for start in range(0, self.total, batch_size):
                 count = min(batch_size, self.total - start)
-                if critics:
-                    grad_fn(ptr(a.theta), self.O, self.A, *self._batch_ptrs(), ptr(self.mu_old),
-                            ptr(self.buf.adv_moments), ptr(order), self.total, 0, start, count, LOSS_RATIO, 0.0, 0.0,
-                            1.0, 0.0, 0, ptr(self.logstd_old), critics, ptr(self.gpart), ptr(self.stats_part),
-                            ptr(self.stop_flag), s)
-                    nb = lib().osb_tc_grid_blocks(count, critics) if tiles else lib().osb_update_grid_blocks(count)
-                    self._optim_step(self.gpart, self.stats_part, nb, critics, **opt)
-                loss, grad = actor_step(rows_all[start:start + count])
-                self.actor_gpart[: self.Pa].copy_(grad)
-                self.actor_stats[0] = loss.detach()
-                self.actor_stats[3] = 1.0
-                self._optim_step(self.actor_gpart, self.actor_stats, 1, NET_ACTOR, **opt)
+                rows = rows_all[start:start + count]
+                pending = 0
+                for bit in (NET_CRITIC_R, NET_CRITIC_C, NET_ACTOR):
+                    if not net_mask & bit:
+                        continue
+                    if bit not in steps:
+                        pending |= bit
+                        continue
+                    if pending:
+                        kernel_step(pending, order, start, count)
+                        pending = 0
+                    if bit != NET_ACTOR:
+                        steps[bit](rows)
+                        continue
+                    loss, grad = steps[bit](rows)
+                    self.actor_gpart[: self.Pa].copy_(grad)
+                    self.actor_stats[0] = loss.detach()
+                    self.actor_stats[3] = 1.0
+                    self._optim_step(self.actor_gpart, self.actor_stats, 1, NET_ACTOR, **opt)
+                if pending:
+                    kernel_step(pending, order, start, count)
+            if not train_actor:
+                continue
             d = self.buf.data
             self._eval_fn()(ptr(a.theta), self.O, self.A, ptr(d['obs']), ptr(d['act']), ptr(d['logp']),
                             ptr(d['adv_r']), ptr(d['adv_c']), ptr(self.mu_old), ptr(self.logstd_old),

@@ -15,6 +15,7 @@ import time
 import torch
 import torch.nn.functional as F
 from torch.distributions import Normal, kl_divergence
+from torch.nn.utils.clip_grad import clip_grad_norm_
 
 from omnisafe_b200.adapter.onpolicy_adapter import OnPolicyAdapter
 from omnisafe_b200.adapter.early_terminated_adapter import EarlyTerminatedAdapter, ExternalEarlyTerminatedAdapter
@@ -24,8 +25,9 @@ from omnisafe_b200.adapter.simmer_adapter import SimmerAdapter
 from omnisafe_b200.algorithms import registry
 from omnisafe_b200.algorithms.base_algo import BaseAlgo
 from omnisafe_b200.algorithms.engine import (LOSS_COST, LOSS_FOCOPS, LOSS_P3O, LOSS_PPO_CLIP, LOSS_RATIO,
-                                             NET_ACTOR, UpdateEngine)
-from omnisafe_b200.algorithms.torch_loss import DeviceStats, overridden_hooks, training_actor
+                                             NET_ACTOR, NET_CRITIC_C, NET_CRITIC_R, UpdateEngine)
+from omnisafe_b200.algorithms.torch_loss import (ACTOR_HOOKS, DeviceStats, overridden_hooks, training_actor,
+                                                 training_critic)
 from omnisafe_b200.common.buffer import VectorOnPolicyBuffer
 from omnisafe_b200.common.lagrange import Lagrange
 from omnisafe_b200.common.logger import Logger
@@ -80,9 +82,12 @@ class PolicyGradient(BaseAlgo):
         self._stats8 = torch.zeros(8, dtype=torch.float64, device=self._device)
         self._epochs_done = 0       # epochs trained so far (a resumed run starts at the saved count)
         self._first_epoch = 0       # where learn() starts
-        # actor hooks overridden outside the library: the actor is then trained through autograd on them
+        # hooks overridden outside the library: the actor is then trained through autograd on the actor hooks, a critic
+        # with its hook
         self._torch_hooks = overridden_hooks(type(self))
-        self._loss_stats = DeviceStats()
+        self._actor_hooks = [h for h, _ in self._torch_hooks if h in ACTOR_HOOKS]
+        self._critic_hooks = {h for h, _ in self._torch_hooks if h not in ACTOR_HOOKS}
+        self._loss_stats = DeviceStats(self._device)
         self._path_logged = False
 
     def _init_log(self) -> None:
@@ -124,7 +129,10 @@ class PolicyGradient(BaseAlgo):
             self._path_logged = True
             if self._torch_hooks:
                 by = ', '.join(f'{h} ({k})' for h, k in self._torch_hooks)
-                self._logger.log(f'INFO: the actor is trained through autograd on the PyTorch loss: {by} overridden')
+                nets = ['the actor'] if self._actor_hooks else []
+                nets += [f'the {w} critic' for w in ('reward', 'cost') if f'_update_{w}_critic' in self._critic_hooks]
+                self._logger.log(f'INFO: {" and ".join(nets)} trained through autograd on the PyTorch hooks: {by} '
+                                 'overridden')
             else:
                 self._logger.log('INFO: the actor is trained by the fused update kernels')
         self._env.rollout(self._steps_per_epoch, self._actor_critic, self._buf, self._logger, eps=eps)
@@ -239,14 +247,10 @@ class PolicyGradient(BaseAlgo):
     def _lagrange_ptr(self):
         return None
 
-    def _update(self, net_mask: int = 7, perm=None) -> None:
+    def _epoch_args(self, net_mask: int) -> dict:
+        """What one epoch of minibatch steps (`ppo_epoch` / `stepwise_epoch`) runs for this class."""
         a = self._cfgs.algo_cfgs
-        if not a.use_cost:
-            net_mask &= ~4
-        if self._torch_hooks and net_mask & NET_ACTOR:
-            self._torch_update(net_mask, perm)
-            return
-        self._engine.ppo_epoch(
+        return dict(
             loss_kind=self._loss_kind, lagrange=self._lagrange_ptr(), net_mask=net_mask,
             batch_size=a.batch_size, update_iters=a.update_iters, clip=getattr(a, 'clip', 0.2),
             entropy_coef=a.entropy_coef, focops_lam=getattr(a, 'focops_lam', 1.0),
@@ -254,7 +258,16 @@ class PolicyGradient(BaseAlgo):
             critic_norm_coef=a.critic_norm_coef if a.use_critic_norm else 0.0,
             max_grad_norm=a.max_grad_norm if a.use_max_grad_norm else 0.0,
             lr_actor=self._actor_critic.actor_lr, lr_critic=self._actor_critic.critic_lr,
-            target_kl=a.target_kl, kl_early_stop=a.kl_early_stop, perm=perm)
+            target_kl=a.target_kl, kl_early_stop=a.kl_early_stop)
+
+    def _update(self, net_mask: int = 7, perm=None) -> None:
+        a = self._cfgs.algo_cfgs
+        if not a.use_cost:
+            net_mask &= ~4
+        if self._hooked_nets(net_mask):
+            self._torch_update(net_mask, perm)
+            return
+        self._engine.ppo_epoch(**self._epoch_args(net_mask), perm=perm)
 
     # ---- actor objectives in PyTorch (policy_gradient.py:L483-588) ----------------------------------------------
     # The library's own losses run inside the update kernels (csrc/loss.cuh).  These PyTorch statements of them are
@@ -314,18 +327,66 @@ class PolicyGradient(BaseAlgo):
             loss.backward()
         return loss.detach(), theta.grad
 
+    def _hooked_nets(self, net_mask: int) -> int:
+        """The networks of `net_mask` that train through a PyTorch hook."""
+        nets = NET_ACTOR if self._actor_hooks else 0
+        nets |= NET_CRITIC_R if '_update_reward_critic' in self._critic_hooks else 0
+        nets |= NET_CRITIC_C if '_update_cost_critic' in self._critic_hooks else 0
+        return nets & net_mask
+
     def _torch_update(self, net_mask: int, perm=None) -> None:
-        """PolicyGradient._update with the actor trained through autograd on `_actor_loss`."""
-        a, ac = self._cfgs.algo_cfgs, self._actor_critic
-        Pa = self._engine.Pa
-        self._loss_stats.clear()
-        self._engine.torch_actor_epoch(
-            lambda rows: self._torch_loss(ac.theta[:Pa], self._actor_loss, rows),
-            lagrange=self._lagrange_ptr(), net_mask=net_mask, batch_size=a.batch_size, update_iters=a.update_iters,
-            critic_norm_coef=a.critic_norm_coef if a.use_critic_norm else 0.0,
-            max_grad_norm=a.max_grad_norm if a.use_max_grad_norm else 0.0,
-            lr_actor=ac.actor_lr, lr_critic=ac.critic_lr, target_kl=a.target_kl, kl_early_stop=a.kl_early_stop,
-            perm=perm)
+        """PolicyGradient._update with the networks that have a hook trained through autograd: the actor on
+        `_actor_loss`, a critic by its `_update_*_critic` (policy_gradient.py:L369-381); the others take their kernel
+        step."""
+        ac, Pa = self._actor_critic, self._engine.Pa
+        hooked = self._hooked_nets(net_mask)
+        if net_mask & NET_ACTOR:
+            self._loss_stats.clear()
+        steps = {}
+        if hooked & NET_ACTOR:
+            steps[NET_ACTOR] = lambda rows: self._torch_loss(ac.theta[:Pa], self._actor_loss, rows)
+        for bit, net in ((NET_CRITIC_R, 1), (NET_CRITIC_C, 2)):
+            if hooked & bit:
+                steps[bit] = lambda rows, net=net: self._critic_step(net, rows)
+        self._engine.stepwise_epoch(steps, **self._epoch_args(net_mask), perm=perm)
+
+    def _critic_step(self, net: int, rows: torch.Tensor) -> None:
+        """One minibatch of `_update_reward_critic` (net 1) or `_update_cost_critic` (net 2) on slab rows `rows`, the
+        model's critic and optimiser and the logger swapped for their training forms while it runs."""
+        d, O = self._buf.data, self._env.obs_dim
+        obs = d['obs'].view(-1, O).index_select(0, rows)
+        target = d['target_value_r' if net == 1 else 'target_value_c'].view(-1).index_select(0, rows)
+        hook = self._update_reward_critic if net == 1 else self._update_cost_critic
+        with training_critic(self, net, self._actor_critic.critic_lr):
+            hook(obs, target)
+
+    # ---- critic objectives in PyTorch (policy_gradient.py:L407-485) ---------------------------------------------
+    # The library's own critic losses run inside the update kernels.  These PyTorch statements of them are what
+    # `super()._update_reward_critic(...)` reaches from a subclass; they are called only when a critic hook is
+    # overridden, with the model's critic and optimiser in their training forms (torch_loss.TrainingCritic).
+    def _update_reward_critic(self, obs: torch.Tensor, target_value_r: torch.Tensor) -> None:
+        ac = self._actor_critic
+        self._critic_loss_step(ac.reward_critic, ac.reward_critic_optimizer, obs, target_value_r,
+                               'Loss/Loss_reward_critic')
+
+    def _update_cost_critic(self, obs: torch.Tensor, target_value_c: torch.Tensor) -> None:
+        ac = self._actor_critic
+        self._critic_loss_step(ac.cost_critic, ac.cost_critic_optimizer, obs, target_value_c, 'Loss/Loss_cost_critic')
+
+    def _critic_loss_step(self, critic, optimizer, obs, target, key: str) -> None:
+        """MSE + critic_norm_coef * sum of squared parameters, backward, clip_grad_norm_, avg_grads, Adam step."""
+        a = self._cfgs.algo_cfgs
+        optimizer.zero_grad()
+        loss = F.mse_loss(critic(obs)[0], target)
+        if a.use_critic_norm:
+            for param in critic.parameters():
+                loss = loss + param.pow(2).sum() * a.critic_norm_coef
+        loss.backward()
+        if a.use_max_grad_norm:
+            clip_grad_norm_(critic.parameters(), a.max_grad_norm)
+        distributed.avg_grads(critic)
+        optimizer.step()
+        self._logger.store({key: loss.detach()})
 
 
 @registry.register
@@ -462,17 +523,16 @@ class P3O(PPO):
         a = self._cfgs.algo_cfgs
         jc = self._window_means()[1] - a.cost_limit        # the reference reads the logger per minibatch (p3o.py:L88)
         self._jc_minus_limit = jc
-        if self._torch_hooks:
-            self._torch_update(net_mask if a.use_cost else net_mask & ~4, perm)
+        net_mask = net_mask if a.use_cost else net_mask & ~4
+        if self._hooked_nets(net_mask):
+            self._torch_update(net_mask, perm)
             return
-        self._engine.ppo_epoch(
-            loss_kind=LOSS_P3O, lagrange=None, net_mask=net_mask if a.use_cost else net_mask & ~4,
-            batch_size=a.batch_size, update_iters=a.update_iters, clip=a.clip, entropy_coef=a.entropy_coef,
-            focops_lam=a.kappa, focops_eta=jc,
-            critic_norm_coef=a.critic_norm_coef if a.use_critic_norm else 0.0,
-            max_grad_norm=a.max_grad_norm if a.use_max_grad_norm else 0.0,
-            lr_actor=self._actor_critic.actor_lr, lr_critic=self._actor_critic.critic_lr,
-            target_kl=a.target_kl, kl_early_stop=a.kl_early_stop, perm=perm)
+        self._engine.ppo_epoch(**self._epoch_args(net_mask), perm=perm)
+
+    def _epoch_args(self, net_mask: int) -> dict:
+        a = self._cfgs.algo_cfgs
+        return {**super()._epoch_args(net_mask), 'lagrange': None, 'clip': a.clip, 'focops_lam': a.kappa,
+                'focops_eta': self._jc_minus_limit}
 
     def _log_extra(self) -> None:
         super()._log_extra()
@@ -552,7 +612,7 @@ class NaturalPG(PolicyGradient):
         """loss.backward() of the full-batch reward ('reward': the `_surrogate_kind` objective) or cost surrogate +
         avg_grads: out <- sign * d loss / d theta_actor; returns the device scalar loss (rank-averaged)."""
         e = self._engine
-        if not self._torch_hooks:
+        if not self._actor_hooks:
             kind, lagrange = (self._kind, self._adv_lagrange()) if which == 'reward' else (LOSS_COST, None)
             return e.actor_loss_grad(kind, lagrange, out, sign=sign)
         w = distributed.world_size()
@@ -569,7 +629,7 @@ class NaturalPG(PolicyGradient):
         """Surrogate of a line-search trial: from the evaluation kernel's statistics `ev`, or the PyTorch loss at
         `trial` (forward only).  which: 'reward' (the `_surrogate_kind` objective), 'reward_only' (CPO's -mean ratio
         adv_r) or 'cost'."""
-        if not self._torch_hooks:
+        if not self._actor_hooks:
             if which == 'cost':
                 return ev['loss_c']
             if which == 'reward_only':
@@ -589,15 +649,16 @@ class NaturalPG(PolicyGradient):
                       'Misc/gradient_norm': float(grads.norm()), 'Misc/H_inv_g': float(x.norm())}
 
     def _update(self, perm=None) -> None:
+        self._loss_stats.clear()
         self._update_actor()
         final_kl = self._engine.kl_state[0].clone()
+        if self._actor_hooks:      # Loss/Loss_pi and Train/PolicyRatio: what the loss stores at the accepted policy
+            self._loss_stats.clear()
+            self._trial_loss(self._actor_critic.theta, 'reward', None)
         super()._update(net_mask=6, perm=perm)   # critics only, update_iters passes (natural_pg.py:L209-223)
         # what the reference logs after the actor step (natural_pg.py:L168-186, trpo.py:L196-222): loss / ratio / KL of
         # the accepted policy on the full batch, StopIter = update_iters
         ev = self._engine.evaluate(self._actor_critic.theta, self._adv_lagrange())
-        if self._torch_hooks:      # Loss/Loss_pi and Train/PolicyRatio: what the loss stores at the accepted policy
-            self._loss_stats.clear()
-            self._trial_loss(self._actor_critic.theta, 'reward', ev)
         ts = self._engine.train_stats.view(3, 8)
         ts[0, 0] = ev['loss_c'] if self._kind == LOSS_COST else ev['loss']
         ts[0, 1] = ev['ratio']

@@ -1,26 +1,35 @@
-"""Actor objectives written in PyTorch on the kernel update path.
+"""Actor and critic objectives written in PyTorch on the kernel update path.
 
 A subclass that overrides `_loss_pi`, `_compute_adv_surrogate` or `_loss_pi_cost` trains its actor through autograd on
-that loss; everything else of the update (critics, clipping, rank averaging, Adam, KL early stop, Fisher-vector
-products, CG) stays on the kernels.  The actor mean mu(obs) is a `torch.autograd.Function`: forward on the actor-
-evaluation kernel of the run's precision, backward on the supplied-dmu kernel (osb_actor_dmu_backward, loss kind
-LOSS_DMU), so the objective sees exactly the network the fused path trains.
+that loss; the clipping, rank averaging, Adam, KL early stop, Fisher-vector products and CG stay on the kernels.  The
+actor mean mu(obs) is a `torch.autograd.Function`: forward on the actor-evaluation kernel of the run's precision,
+backward on the supplied-dmu kernel (osb_actor_dmu_backward, loss kind LOSS_DMU), so the objective sees exactly the
+network the fused path trains.
+
+A subclass that overrides `_update_reward_critic` or `_update_cost_critic` trains that critic with its own minibatch
+step.  While it runs, the critic is a `TrainingCritic`: V(obs) forward and backward on the supplied-dV kernel
+(osb_critic_dv_backward, the update kernels of the run's precision), leaf parameters that are views of the flat
+`theta`, and an optimiser whose step() is the library's Adam on that network.  Networks without a hook keep their
+kernel step.
 """
 from __future__ import annotations
 
 import contextlib
+import math
 
 import torch
 from torch.distributions import Normal
 
 from omnisafe_b200._lib import current_stream, lib, ptr
 
-HOOKS = ('_loss_pi', '_compute_adv_surrogate', '_loss_pi_cost')
+ACTOR_HOOKS = ('_loss_pi', '_compute_adv_surrogate', '_loss_pi_cost')
+CRITIC_HOOKS = ('_update_reward_critic', '_update_cost_critic')
+HOOKS = ACTOR_HOOKS + CRITIC_HOOKS
 _LIBRARY = 'omnisafe_b200'
 
 
 def overridden_hooks(cls: type) -> list[tuple[str, str]]:
-    """[(hook, defining class)] for every actor hook `cls` takes from a class defined outside the library."""
+    """[(hook, defining class)] for every hook `cls` takes from a class defined outside the library."""
     found = []
     for name in HOOKS:
         for klass in cls.__mro__:
@@ -105,15 +114,148 @@ def training_actor(model, engine, theta: torch.Tensor):
         model.actor = saved
 
 
-class DeviceStats:
-    """Logger values stored by PyTorch losses, kept on the device until the epoch is logged (one read per epoch)."""
+class CriticValue(torch.autograd.Function):
+    """V [B] of rows obs [B, O] (contiguous, normalised) for a TrainingCritic; differentiable in its leaf parameters
+    (`params`, views of the flat theta the kernels read).  Forward and backward are osb_critic_dv_backward, the update
+    kernels of the run's precision on that critic: the forward with dV = 0 gives the values with the bits the stepwise
+    update computes; the gradient is J_V^T dV of the critic MLP."""
 
-    def __init__(self) -> None:
+    @staticmethod
+    def forward(ctx, obs: torch.Tensor, critic, *params: torch.Tensor) -> torch.Tensor:
+        B = obs.shape[0]
+        value = torch.empty(B, dtype=torch.float32, device=obs.device)
+        if B > 0:
+            critic._launch(obs, torch.zeros(B, dtype=torch.float32, device=obs.device), value)
+        ctx.save_for_backward(obs)
+        ctx.critic = critic
+        return value
+
+    @staticmethod
+    def backward(ctx, dv: torch.Tensor):
+        (obs,) = ctx.saved_tensors
+        c = ctx.critic
+        e = c._engine
+        grad = torch.zeros(c.size, dtype=torch.float32, device=obs.device)
+        B = obs.shape[0]
+        if B > 0:
+            nb = c._launch(obs, dv.to(torch.float32).contiguous(), None)
+            lib().osb_reduce_partials(ptr(e.gpart[c.start:]), nb, e.P, c.size, 1.0, 0, 0.0, ptr(grad),
+                                      current_stream())
+        return (None, None, *(g.view(p.shape) for g, p in zip(grad.split(c.sizes), c._params)))
+
+
+class TrainingCritic:
+    """What `self._actor_critic.reward_critic` / `.cost_critic` is while a critic hook runs: the reference's VCritic API
+    (`critic(obs)` -> [value]) and nn.Module's `parameters()` / `named_parameters()`: leaf tensors with the reference's
+    names, shapes and order that are views of the network's slice of the flat `theta`, so they always hold what the
+    kernels train."""
+
+    def __init__(self, engine, net: int) -> None:
+        self._engine, self.net = engine, net            # net: 1 reward critic, 2 cost critic
+        lay = engine.agent.layout['reward_critic' if net == 1 else 'cost_critic']
+        self.start, self.size = lay['start'], lay['size']
+        theta = engine.agent.theta
+        self._named = [(name, theta[off:off + math.prod(shape)].view(*shape).requires_grad_(True))
+                       for name, (off, shape) in lay['entries'].items()]
+        self._params = [p for _, p in self._named]
+        self.sizes = [p.numel() for p in self._params]
+
+    def _launch(self, obs: torch.Tensor, dv: torch.Tensor, value: torch.Tensor | None) -> int:
+        """osb_critic_dv_backward on rows obs [B, O] into the engine's partials; returns their row count."""
+        e = self._engine
+        B = obs.shape[0]
+        lib().osb_critic_dv_backward(ptr(e.agent.theta), e.O, e.A, self.net, ptr(obs), ptr(dv), ptr(value), B,
+                                     e.precision, ptr(e.gpart), ptr(e.stats_part), current_stream())
+        return lib().osb_critic_dv_grid_blocks(B, e.O, e.precision)
+
+    def forward(self, obs: torch.Tensor) -> list[torch.Tensor]:
+        e = self._engine
+        assert obs.shape[-1] == e.O, f'obs must be [..., {e.O}], got {tuple(obs.shape)}'
+        lead = obs.shape[:-1]
+        flat = obs.to(torch.float32).reshape(-1, e.O).contiguous()
+        return [CriticValue.apply(flat, self, *self._params).view(lead)]
+
+    __call__ = forward
+
+    def parameters(self):
+        return iter(self._params)
+
+    def named_parameters(self):
+        return iter(self._named)
+
+    def flat_grad(self) -> torch.Tensor:
+        """The leaves' gradients as one flat vector in layout order (zero where a leaf has none)."""
+        return torch.cat([(p.grad if p.grad is not None else torch.zeros_like(p)).reshape(-1) for p in self._params])
+
+
+class TrainingCriticOptimizer:
+    """What `reward_critic_optimizer` / `cost_critic_optimizer` is while a critic hook runs: zero_grad() and step(),
+    the library's Adam on the network's slice of theta with its own step count and the critic learning rate (the Adam
+    state the fused path trains, saves and resumes).  No clipping and no L2 term are added: the hook's are the only
+    ones."""
+
+    def __init__(self, critic: TrainingCritic, lr: float) -> None:
+        self._critic, self.lr = critic, float(lr)
+
+    def zero_grad(self, set_to_none: bool = True) -> None:
+        for p in self._critic.parameters():
+            if set_to_none:
+                p.grad = None
+            elif p.grad is not None:
+                p.grad.zero_()
+
+    def step(self) -> None:
+        c = self._critic
+        c._engine.adam_step(c.net, c.flat_grad(), self.lr)
+
+
+class HookLogger:
+    """What `self._logger` is while a critic hook runs: `store` keeps the values on the device (DeviceStats) until the
+    epoch is logged; everything else is the logger's."""
+
+    def __init__(self, logger, stats: 'DeviceStats') -> None:
+        self._logger, self._stats = logger, stats
+
+    def store(self, data: dict | None = None, **kwargs) -> None:
+        self._stats.store({**(data or {}), **kwargs})
+
+    def __getattr__(self, name: str):
+        return getattr(self._logger, name)
+
+
+@contextlib.contextmanager
+def training_critic(algo, net: int, lr: float):
+    """Swap the model's critic `net` (1 reward, 2 cost) and its optimiser for a TrainingCritic and its optimiser, and
+    `algo._logger` for a HookLogger, for the duration of one critic hook."""
+    model, name = algo._actor_critic, 'reward_critic' if net == 1 else 'cost_critic'
+    saved = getattr(model, name), getattr(model, f'{name}_optimizer', None), algo._logger
+    critic = TrainingCritic(algo._engine, net)
+    setattr(model, name, critic)
+    setattr(model, f'{name}_optimizer', TrainingCriticOptimizer(critic, lr))
+    algo._logger = HookLogger(saved[2], algo._loss_stats)
+    try:
+        yield critic
+    finally:
+        setattr(model, name, saved[0])
+        if saved[1] is None:
+            delattr(model, f'{name}_optimizer')
+        else:
+            setattr(model, f'{name}_optimizer', saved[1])
+        algo._logger = saved[2]
+
+
+class DeviceStats:
+    """Logger values stored by PyTorch losses, kept on the device until the epoch is logged (one read per epoch).
+    Python numbers are stored on `device`."""
+
+    def __init__(self, device=None) -> None:
         self._vals: dict[str, list[torch.Tensor]] = {}
+        self._device = device
 
     def store(self, data: dict) -> None:
         for key, val in data.items():
-            t = torch.as_tensor(val).detach().to(torch.float32).mean().reshape(1)
+            t = torch.as_tensor(val, device=None if torch.is_tensor(val) else self._device)
+            t = t.detach().to(torch.float32).mean().reshape(1)
             self._vals.setdefault(key, []).append(t)
 
     def clear(self) -> None:

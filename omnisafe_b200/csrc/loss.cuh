@@ -23,8 +23,8 @@ enum LossKind {
     LOSS_COST = 3,
     LOSS_FVP = 4,      // dOUT supplied: backward half of the tensor-core Fisher-vector products
     LOSS_P3O = 5,      // two passes
-    LOSS_DMU = 6,      // dOUT = dmu supplied per row: J^T dmu of the actor MLP (losses written in PyTorch); compiled
-                       // only into the DMU instantiations of the stepwise kernels
+    LOSS_DMU = 6,      // dOUT = dmu (actor) or dV (critic) supplied per row: J^T dOUT of the MLP (losses written in
+                       // PyTorch); compiled only into the DMU instantiations of the stepwise kernels
 };
 
 // FOCOPS and P3O need a minibatch mean before any gradient: a forward-only pass 1 feeds pass1_gate().
@@ -251,5 +251,11 @@ int dmu_backward_tc(const float* theta_actor, int O, int A, const float* obs, co
                     float* stats_scratch, cudaStream_t stream);
 int dmu_backward_x3(const float* theta_actor, int O, int A, const float* obs, const float* dmu, int rows, float* gpart,
                     float* stats_scratch, cudaStream_t stream);
+// ... and behind osb_critic_dv_backward: critic `net` (1, 2) of the flat theta, dv[rows] = dL/dV, value[rows] (or
+// null) <- V; gpart: osb_tc_grid_blocks(rows, 1 << net) rows of P floats (the critic's segment written).
+int dv_backward_tc(const float* theta, int O, int A, int net, const float* obs, const float* dv, float* value, int rows,
+                   float* gpart, float* stats_scratch, cudaStream_t stream);
+int dv_backward_x3(const float* theta, int O, int A, int net, const float* obs, const float* dv, float* value, int rows,
+                   float* gpart, float* stats_scratch, cudaStream_t stream);
 
 }  // namespace osb

@@ -33,6 +33,7 @@ struct GradArgs {
     int O, A, P;
     int net_mask;          // bit n set -> process network n
     int forward_only;      // pass 1 of FOCOPS / P3O: actor forward + statistics only (no gradients written)
+    float* value_out;      // LOSS_DMU on a critic (DMU instantiation only), or null: V per row as this launch computes it
 };
 
 // gather chunk kc of the observation rows of a tile into sX (zero padded)
@@ -65,8 +66,8 @@ __device__ __forceinline__ void block_reduce_store(float (&v)[NV], float* sRed, 
     __syncthreads();
 }
 
-// DMU = true: actor only, LOSS_DMU -- b.act carries the supplied dL/dmu [rows][A] and the backward yields J^T of it
-// (no log_std term, no statistics but the row count).
+// DMU = true: LOSS_DMU -- the backward yields J^T of a supplied output gradient (no log_std term, no statistics but the
+// row count): b.act carries dL/dmu [rows][A] for the actor, b.tv_r / b.tv_c carry dL/dV [rows] for a critic.
 template <bool DMU = false>
 __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p) {
     if (p.stop_flag && *p.stop_flag) return;
@@ -143,6 +144,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p)
                 const long long row = sRow[m];
                 if (row < 0) {
                     for (int o = 0; o < OUTP; ++o) sO[m * LDO + o] = 0.f;
+                } else if (DMU && net != 0) {                            // critic: tv_r / tv_c carry dL/dV
+                    if (p.value_out) p.value_out[row] = sO[m * LDO];
+                    sO[m * LDO] = __ldg((net == 1 ? p.b.tv_r : p.b.tv_c) + row);
+                    for (int o = 1; o < OUTP; ++o) sO[m * LDO + o] = 0.f;
+                    st[3] = 1.f;
                 } else if (net != 0) {
                     const float v = sO[m * LDO];
                     const float tgt = __ldg((net == 1 ? p.b.tv_r : p.b.tv_c) + row);
@@ -808,7 +814,7 @@ int osb_actor_dmu_backward(const float* theta_actor, int O, int A, const float* 
     p.lc = LossParams{LOSS_DMU, 0.f, 0.f, 1.f, 0.f, nullptr, nullptr, nullptr, nullptr};
     p.forward_only = 0;
     p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch; p.stop_flag = nullptr;
-    p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
+    p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1; p.value_out = nullptr;
     const size_t smem = grad_smem_bytes();
     static bool attr = false;
     if (!attr) {
@@ -816,6 +822,42 @@ int osb_actor_dmu_backward(const float* theta_actor, int O, int A, const float* 
         attr = true;
     }
     minibatch_grad_kernel<true><<<dim3(osb_fvp_grid_blocks(rows, 1), 1), NTHREADS, smem, (cudaStream_t)stream>>>(p);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}
+
+// The critic's CTAs are those of a stepwise update launch of that critic alone over a minibatch of `rows`
+// (osb_update_grid_blocks / osb_tc_grid_blocks), so each CTA takes the same tiles.
+int osb_critic_dv_grid_blocks(int rows, int O, int precision) {
+    return dmu_tiles(O, precision) ? osb_tc_grid_blocks(rows, 2) : osb_update_grid_blocks(rows);
+}
+
+// Critic backward with a supplied output gradient (LOSS_DMU on network `net`, 1 = reward critic, 2 = cost critic):
+// theta the flat [actor | reward critic | cost critic] parameters, rows obs[rows][O] (contiguous, normalised), dv[rows]
+// = dL/dV  ->  gpart[osb_critic_dv_grid_blocks(rows, O, precision)][P] per-CTA partials of J_V^T dv in the critic's
+// segment (at its offset in theta), stats_scratch that many * 24 floats, value[rows] (if not null) the forward V.
+// Reduce with osb_reduce_partials.
+int osb_critic_dv_backward(const float* theta, int O, int A, int net, const float* obs, const float* dv, float* value,
+                           int rows, int precision, float* gpart, float* stats_scratch, void* stream) {
+    OSB_CHECK_ARG(theta && obs && dv && gpart && stats_scratch && rows > 0, "bad argument");
+    OSB_CHECK_ARG(O > 0 && A > 0 && A <= OUTP && (net == 1 || net == 2), "bad dims");
+    const int P = actor_layout(O, A).size + 2 * critic_layout(O, A).size;
+    const int tiles = dmu_tiles(O, precision);
+    if (tiles == 2) return dv_backward_x3(theta, O, A, net, obs, dv, value, rows, gpart, stats_scratch, (cudaStream_t)stream);
+    if (tiles == 1) return dv_backward_tc(theta, O, A, net, obs, dv, value, rows, gpart, stats_scratch, (cudaStream_t)stream);
+    GradArgs p;
+    p.b = Batch{obs, nullptr, nullptr, nullptr, nullptr, dv, dv, nullptr, nullptr, rows, 0u, 0, rows, 1};
+    p.lc = LossParams{LOSS_DMU, 0.f, 0.f, 1.f, 0.f, nullptr, nullptr, nullptr, nullptr};
+    p.forward_only = 0;
+    p.theta = theta; p.gpart = gpart; p.stats_part = stats_scratch; p.stop_flag = nullptr;
+    p.O = O; p.A = A; p.P = P; p.net_mask = 1 << net; p.value_out = value;
+    const size_t smem = grad_smem_bytes();
+    static bool attr = false;
+    if (!attr) {
+        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attr = true;
+    }
+    minibatch_grad_kernel<true><<<dim3(osb_update_grid_blocks(rows), net + 1), NTHREADS, smem, (cudaStream_t)stream>>>(p);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
 }

@@ -43,6 +43,7 @@ struct TcArgs {
     float fvp_scale;         // LOSS_FVP: 1 / (rows * A)
     int forward_only;        // pass 1 of FOCOPS / P3O: statistics only, no backward
     float* acc;              // accumulator images, one [128][TC_COLS] per CTA
+    float* value_out;        // LOSS_DMU on a critic (DMU instantiation only), or null: V per row as this launch computes it
 };
 
 // accumulator column map (csrc/umma.cuh)
@@ -73,7 +74,8 @@ __device__ __forceinline__ void load_row16(uint32_t base, int r, int c0, int R, 
 // accumulate over chunks; backward: one dW1 chunk per MMA, flushed from accumulator image into this CTA's partial gradient).
 // EXT = the two-pass / supplied-dOUT loss kinds (FOCOPS, P3O, FVP); the plain instantiation (PPO-clip, ratio,
 // cost surrogate: the headline path) carries none of their registers or branches.
-// DMU = LOSS_DMU only: the supplied dL/dmu (fvp_dmu, per row) is dOUT as it stands, no loss, no log_std term.
+// DMU = LOSS_DMU only: the supplied dL/dmu (fvp_dmu, per row) or, for a critic, dL/dV (tv_r / tv_c) is dOUT as it
+// stands, no loss, no log_std term.
 template <bool CHUNKED, bool EXT, bool DMU = false>
 __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
     if (p.stop_flag && *p.stop_flag) return;
@@ -398,7 +400,11 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
 #pragma unroll
             for (int i = 0; i < 32; ++i) d32[i] = 0.f;
             if (prow >= 0) {
-                if (net != 0) {
+                if (DMU && net != 0) {       // critic: the supplied dL/dV (tv_r / tv_c)
+                    if (p.value_out) p.value_out[prow] = o16[0] + sB3[0];
+                    d32[0] = pf_tv;
+                    st[3] = 1.f;
+                } else if (net != 0) {
                     const float d = o16[0] + sB3[0] - pf_tv;
                     st[0] = d * d; st[3] = 1.f;
                     d32[0] = 2.f * d * inv_b;
@@ -1024,15 +1030,10 @@ int osb_fvp_partials_tc(const float* theta_actor, const float* vec, int O, int A
 
 }  // extern "C"
 
-int osb::dmu_backward_tc(const float* theta_actor, int O, int A, const float* obs, const float* dmu, int rows, float* gpart,
-                         float* stats_scratch, cudaStream_t stream) {
-    OSB_CHECK_ARG(O <= 512 && A <= 16, "tensor-core path needs O <= 512, A <= 16");
-    TcArgs p;
-    p.b = Batch{obs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, rows, 0u, 0, rows, 1};
+// LOSS_DMU launch of the DMU instantiations (one network, grid.y == 1) on nb CTAs
+static int launch_dmu_tc(TcArgs& p, int nb, cudaStream_t stream) {
     p.lc = LossParams{LOSS_DMU, 0.f, 0.f, 1.f, 0.f, nullptr, nullptr, nullptr, nullptr};
-    p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch; p.stop_flag = nullptr;
-    p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
-    p.fvp_dmu = dmu; p.fvp_vec = nullptr; p.fvp_scale = 1.f;
+    p.stop_flag = nullptr; p.fvp_vec = nullptr; p.fvp_scale = 1.f;
     p.forward_only = 0;
     const size_t smem = tc_smem_bytes();
     static bool attr = false;
@@ -1041,11 +1042,32 @@ int osb::dmu_backward_tc(const float* theta_actor, int O, int A, const float* ob
         OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = true;
     }
-    const int nb = osb_tc_grid_blocks(rows, 1);
     p.acc = acc_scratch(ACC_UPDATE_TC, (size_t)nb * 128 * TC_COLS * sizeof(float));
     if (!p.acc) return OSB_ERR_CUDA;
-    if (O > 64) minibatch_grad_tc_kernel<true, false, true><<<dim3(nb, 1), NTC, smem, stream>>>(p);
+    if (p.O > 64) minibatch_grad_tc_kernel<true, false, true><<<dim3(nb, 1), NTC, smem, stream>>>(p);
     else minibatch_grad_tc_kernel<false, false, true><<<dim3(nb, 1), NTC, smem, stream>>>(p);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
+}
+
+int osb::dmu_backward_tc(const float* theta_actor, int O, int A, const float* obs, const float* dmu, int rows, float* gpart,
+                         float* stats_scratch, cudaStream_t stream) {
+    OSB_CHECK_ARG(O <= 512 && A <= 16, "tensor-core path needs O <= 512, A <= 16");
+    TcArgs p;
+    p.b = Batch{obs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, rows, 0u, 0, rows, 1};
+    p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch;
+    p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
+    p.fvp_dmu = dmu; p.value_out = nullptr;
+    return launch_dmu_tc(p, osb_tc_grid_blocks(rows, 1), stream);
+}
+
+int osb::dv_backward_tc(const float* theta, int O, int A, int net, const float* obs, const float* dv, float* value, int rows,
+                        float* gpart, float* stats_scratch, cudaStream_t stream) {
+    OSB_CHECK_ARG(O <= 512 && A <= 16, "tensor-core path needs O <= 512, A <= 16");
+    TcArgs p;
+    p.b = Batch{obs, nullptr, nullptr, nullptr, nullptr, dv, dv, nullptr, nullptr, rows, 0u, 0, rows, 1};
+    p.theta = theta; p.gpart = gpart; p.stats_part = stats_scratch;
+    p.O = O; p.A = A; p.P = actor_layout(O, A).size + 2 * critic_layout(O, A).size; p.net_mask = 1 << net;
+    p.fvp_dmu = nullptr; p.value_out = value;
+    return launch_dmu_tc(p, osb_tc_grid_blocks(rows, 1 << net), stream);
 }

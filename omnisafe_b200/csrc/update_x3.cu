@@ -71,6 +71,7 @@ struct X3Args {
     float fvp_scale;             // LOSS_FVP: 1 / (rows * A)
     long long* dbg;              // optional clock64 stamps of CTA (0, 0): [0] = count, then (id, clock) pairs (tools/x3_stage_times.py)
     float* acc;                  // accumulator images, one [128][T_COLS] per CTA
+    float* value_out;            // LOSS_DMU on a critic (DMU instantiation only), or null: V per row as this launch computes it
 };
 
 constexpr int XT = 128;                      // samples per tile
@@ -193,8 +194,8 @@ constexpr int PSTR = 9472;          // FUSED: row stride of the private partial-
 //   distributed.py:L193-198), apply torch-Adam and re-stage the new weights: no relaunch, no separate
 //   optimiser kernel.
 // AP = padded action width of the loss epilogue (8 or 16).
-// DMU = LOSS_DMU only (FUSED = false): the supplied dL/dmu (fvp_dmu, per row) is dOUT as it stands, no loss, no
-// log_std term.
+// DMU = LOSS_DMU only (FUSED = false): the supplied dL/dmu (fvp_dmu, per row) or, for a critic, dL/dV (tv_r / tv_c)
+// is dOUT as it stands, no loss, no log_std term.
 // (20 warps = 640 threads: 96 registers each, the register file divided in units of 8 per thread)
 template <bool FUSED, int AP, bool DMU = false>
 __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
@@ -560,7 +561,12 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                         for (int a = 0; a < AP; ++a) o[a] = t16[a];
                     }
                     if (prow >= 0) {
-                        if (net != 0) {
+                        if (DMU && net != 0) {       // critic: the supplied dL/dV (tv_r / tv_c)
+                            if (p.value_out) p.value_out[prow] = o[0] + sB3[0];
+                            acc_st[3] += 1.f;
+                            d16[0] = pf_tv;
+                            acc_db[0] += pf_tv;
+                        } else if (net != 0) {
                             const float d = o[0] + sB3[0] - pf_tv;
                             acc_st[0] += d * d; acc_st[3] += 1.f;
                             d16[0] = 2.f * d * inv_b;
@@ -1108,22 +1114,38 @@ int osb_ppo_update_iter_x3(float* theta, float* grad, float* adam_m, float* adam
 
 }  // extern "C"
 
-// LOSS_DMU launch behind osb_actor_dmu_backward (csrc/update.cu)
+// LOSS_DMU launch of the DMU instantiations (one network, grid.y == 1) on nb CTAs
+static int launch_dmu_x3(X3Args& p, int nb, cudaStream_t stream) {
+    p.lc.kind = LOSS_DMU; p.lc.focops_lam = 1.f;
+    p.batch_size = p.b.mb_count; p.world = 1; p.dbg = nullptr;
+    int rc = x3_set_attr();
+    if (rc) return rc;
+    if ((rc = x3_bind_acc(p, nb))) return rc;
+    if (p.A <= 8) minibatch_grad_x3_kernel<false, 8, true><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
+    else minibatch_grad_x3_kernel<false, 16, true><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}
+
+// LOSS_DMU launches behind osb_actor_dmu_backward and osb_critic_dv_backward (csrc/update.cu)
 int osb::dmu_backward_x3(const float* theta_actor, int O, int A, const float* obs, const float* dmu, int rows, float* gpart,
                          float* stats_scratch, cudaStream_t stream) {
     OSB_CHECK_ARG(O <= 64 && A <= 16, "bf16x3 path needs O <= 64, A <= 16");
     X3Args p = {};
     p.b = Batch{obs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, rows, 0u, 0, rows, 1};
-    p.lc.kind = LOSS_DMU; p.lc.focops_lam = 1.f; p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch;
+    p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch;
     p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
-    p.batch_size = rows; p.world = 1; p.dbg = nullptr;
     p.fvp_dmu = dmu;
-    const int nb = osb_tc_grid_blocks(rows, 1);
-    int rc = x3_set_attr();
-    if (rc) return rc;
-    if ((rc = x3_bind_acc(p, nb))) return rc;
-    if (A <= 8) minibatch_grad_x3_kernel<false, 8, true><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
-    else minibatch_grad_x3_kernel<false, 16, true><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    return launch_dmu_x3(p, osb_tc_grid_blocks(rows, 1), stream);
+}
+
+int osb::dv_backward_x3(const float* theta, int O, int A, int net, const float* obs, const float* dv, float* value, int rows,
+                        float* gpart, float* stats_scratch, cudaStream_t stream) {
+    OSB_CHECK_ARG(O <= 64 && A <= 16, "bf16x3 path needs O <= 64, A <= 16");
+    X3Args p = {};
+    p.b = Batch{obs, nullptr, nullptr, nullptr, nullptr, dv, dv, nullptr, nullptr, rows, 0u, 0, rows, 1};
+    p.theta = theta; p.gpart = gpart; p.stats_part = stats_scratch;
+    p.O = O; p.A = A; p.P = actor_layout(O, A).size + 2 * critic_layout(O, A).size; p.net_mask = 1 << net;
+    p.value_out = value;
+    return launch_dmu_x3(p, osb_tc_grid_blocks(rows, 1 << net), stream);
 }

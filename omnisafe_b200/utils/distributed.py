@@ -133,6 +133,16 @@ def all_reduce_(t: torch.Tensor) -> torch.Tensor:
     return t
 
 
+def avg_grads(module) -> None:
+    """Average the gradients of `module.parameters()` over ranks (omnisafe/utils/distributed.py:L167-198): the
+    all-reduce SUM and 1/world scale the update kernels apply after clipping."""
+    if world_size() > 1:
+        for param in module.parameters():
+            if param.grad is not None:
+                dist.all_reduce(param.grad, op=dist.ReduceOp.SUM)
+                param.grad.mul_(1.0 / world_size())
+
+
 def barrier() -> None:
     if world_size() > 1:
         dist.barrier()

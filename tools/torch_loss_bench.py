@@ -1,8 +1,10 @@
-"""Cost of an actor objective written in PyTorch: device time of one PPOLag update (the bench.py workload: obs 60 /
-act 8, 4096 envs x T = 128, batch 16384, update_iters 8) on the fused kernels and on the PyTorch-loss path (a subclass
-whose `_loss_pi` returns super()'s), plus whole epochs.  Alternates the two, prints the GPU and its power limit.
+"""Cost of objectives written in PyTorch: device time of one PPOLag update (the bench.py workload: obs 60 / act 8,
+4096 envs x T = 128, batch 16384, update_iters 8) on the fused kernels and on the PyTorch path, plus whole epochs.
+--hook actor: a subclass whose `_loss_pi` returns super()'s; --hook critic: whose `_update_reward_critic` and
+`_update_cost_critic` call super()'s (the actor stays on its kernel step); --hook both.  Alternates the two, prints the
+GPU and its power limit.
 
-    python tools/torch_loss_bench.py [--precision bf16x3] [--reps 5] [--out result.json]
+    python tools/torch_loss_bench.py [--precision bf16x3] [--hook actor|critic|both] [--reps 5] [--out result.json]
 """
 import argparse
 import json
@@ -33,6 +35,7 @@ def timed(fn, k):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--precision', default='bf16x3')
+    ap.add_argument('--hook', default='actor', choices=('actor', 'critic', 'both'))
     ap.add_argument('--reps', type=int, default=5)
     ap.add_argument('--out', default=None)
     args = ap.parse_args()
@@ -40,7 +43,13 @@ def main():
     gpu = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
                          capture_output=True, text=True).stdout.strip()
     base = registry.get('PPOLag')
-    user = type('UserPPOLag', (base,), {'_loss_pi': lambda self, o, a, lp, adv: base._loss_pi(self, o, a, lp, adv)})
+    body = {}
+    if args.hook in ('actor', 'both'):
+        body['_loss_pi'] = lambda self, o, a, lp, adv: base._loss_pi(self, o, a, lp, adv)
+    if args.hook in ('critic', 'both'):
+        body['_update_reward_critic'] = lambda self, o, t: base._update_reward_critic(self, o, t)
+        body['_update_cost_critic'] = lambda self, o, t: base._update_cost_critic(self, o, t)
+    user = type('UserPPOLag', (base,), body)
     algos = {}
     for tag, cls in (('fused', base), ('torch', user)):
         registry._classes['PPOLag'] = cls
@@ -57,7 +66,7 @@ def main():
         for tag, a in algos.items():
             res[tag]['update_ms'].append(timed(a._update, 1))
             res[tag]['epoch_ms'].append(timed(a.train_epoch, 1))
-    out = {'gpu': gpu, 'precision': args.precision, 'workload': 'PPOLag obs60/act8, 4096 envs x T=128, batch 16384, '
+    out = {'gpu': gpu, 'precision': args.precision, 'hook': args.hook, 'workload': 'PPOLag obs60/act8, 4096 envs x T=128, batch 16384, '
            'update_iters 8 (KL early stop may end an update early)'}
     for tag, r in res.items():
         for k, v in r.items():
