@@ -133,12 +133,16 @@ __device__ __forceinline__ void stage_eval_policy(float* pol, int i, float log_s
 //   so fused multiply-adds form as in a hand-inlined loss.
 //   mu, act: the sample's mean (bias included) and action, entries a < A.  mu_old(a): the sample's old mean, called
 //   only by FOCOPS inside its KL loop, so a caller that reads it from global memory keeps no registers for it.
+//   [a_lo, a_hi): the actions whose gradients are formed (default all), and stats: whether st is added to.  Everything
+//   else, logp_new over every action included, is computed in full, so callers that split the actions of a sample among
+//   threads get the same bits in each, and one of them keeps the statistics.
 // EXT = false compiles only PPO-clip, ratio and cost surrogate.
 template <bool EXT, int AP, class MuOld, class Grad>
 __device__ __forceinline__ void actor_sample_loss(const LossParams& lp, const AdvNorm& an, int A, float inv_b,
                                                   const float (&mu)[AP], const float (&act)[AP], MuOld&& mu_old,
                                                   float logp_old, float adv_r_raw, float adv_c_raw, const float* pol,
-                                                  const float* old, float (&st)[5], Grad&& grad) {
+                                                  const float* old, float (&st)[5], Grad&& grad, int a_lo = 0,
+                                                  int a_hi = AP, bool stats = true) {
     float logp_new = 0.f, diff[AP];
 #pragma unroll
     for (int a = 0; a < AP; ++a) {
@@ -165,7 +169,7 @@ __device__ __forceinline__ void actor_sample_loss(const LossParams& lp, const Ad
             const bool pass2 = lp.pass1 != nullptr;
             const float gate = pass2 ? __ldg(lp.pass1) : 0.f;
             dlogp += gate * adv_c * ratio * inv_b;
-            st[2] += pass2 ? gate * (ratio * adv_c + lp.focops_eta) : ratio * adv_c;   // Loss/Loss_pi_cost
+            if (stats) st[2] += pass2 ? gate * (ratio * adv_c + lp.focops_eta) : ratio * adv_c;   // Loss/Loss_pi_cost
         }
     } else if (lp.kind == LOSS_RATIO) {
         loss = -ratio * adv; dlogp = -adv * ratio * inv_b;
@@ -193,12 +197,12 @@ __device__ __forceinline__ void actor_sample_loss(const LossParams& lp, const Ad
         const float mbar = lp.pass1 ? __ldg(lp.pass1) : dmask;
         loss = kl * dmask - mbar * ratio * adv / lp.focops_lam;
         dlogp = -mbar * adv * ratio / lp.focops_lam * inv_b;
-        st[2] += kl; st[4] += dmask;
+        if (stats) { st[2] += kl; st[4] += dmask; }
     }
-    st[0] += loss; st[1] += ratio; st[3] += 1.f;
+    if (stats) { st[0] += loss; st[1] += ratio; st[3] += 1.f; }
 #pragma unroll
     for (int a = 0; a < AP; ++a) {
-        if (a < A) {
+        if (a < A && a >= a_lo && a < a_hi) {
             const float iv = pol[32 + a];
             float dm = dlogp * diff[a] * iv;                    // d logp / d mu
             float dl = dlogp * (diff[a] * diff[a] * iv - 1.f);  // d logp / d log_std

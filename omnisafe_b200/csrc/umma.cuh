@@ -109,6 +109,14 @@ __device__ __forceinline__ void wgmma_bf16_n16(float (&d)[8], uint64_t a, uint64
 // waits on every wgmma before issuing the next (C7520).
 __device__ __forceinline__ int warpgroup_index() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0); }
 
+// Per-warpgroup register budget (all 128 threads of the warpgroup): the calling warpgroup's registers per thread become
+// N (a multiple of 8).  `inc` waits until the CTA's pool, the launch allocation, has N free per thread, so the warpgroups
+// that give registers up must `dec` first or concurrently.
+template <int N>
+__device__ __forceinline__ void wg_regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void wg_regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(N)); }
+
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
 // wait until at most N committed groups of this warpgroup are pending

@@ -21,8 +21,10 @@
 //   is one m64 block per half over the whole K, stored once and committed on that half's mbarrier, and every epilogue
 //   warp waits for and announces its own half only -- the epilogue of rows 0-63 runs under the MMAs of rows 64-127 and
 //   the next product of rows 0-63 under the epilogue of rows 64-127.  Weight / bias gradient MMAs run behind the
-//   dependent chain and release their operands as soon as they have read them.  The loss warps' per-sample inputs
-//   are copied asynchronously into shared memory (cp.async) at the start of the tile.
+//   dependent chain and release their operands as soon as they have read them.  The per-sample loss inputs are copied
+//   asynchronously into shared memory (cp.async) at the start of the tile; all four warps of a sample's rows compute
+//   its loss, each the gradient of a quarter of the actions.  The MMA-issue warpgroup runs on 160 registers per
+//   thread, the epilogue warps on 80 (setmaxnreg).
 //
 // FUSED instantiation = the persistent cooperative kernel of one update iteration: after each minibatch the partial
 // gradients are reduced slice-wise behind a software grid barrier, clipped per network, (multi-rank) exchanged over
@@ -41,6 +43,8 @@ using namespace x3;
 
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 512;\n" ::: "memory"); }      // epilogue warps only
 __device__ __forceinline__ void loss_bar_sync() { asm volatile("bar.sync 2, 128;\n" ::: "memory"); }     // loss warps (h == 0)
+// the four epilogue warps of rows 32 q .. 32 q + 31 (named barriers 4 .. 7)
+__device__ __forceinline__ void rows_bar_sync(int q) { asm volatile("bar.sync %0, 128;\n" ::"r"(4 + q) : "memory"); }
 
 struct X3Args {
     Batch b;
@@ -77,6 +81,11 @@ struct X3Args {
 constexpr int XT = 128;                      // samples per tile
 constexpr int NEPI = 512;                    // 16 epilogue warps: lane quarter q = warp % 4, column group h = warp / 4
 constexpr int NTX3 = NEPI + 128;             // + the MMA-issue warpgroup (warps 16..19)
+// Registers per thread after the one-time setup (setmaxnreg; the launch gives every warp 96).  The MMA-issue warpgroup
+// holds an N = 64 fragment and the 32 image values it adds to in dW2 and dW1 (at 128 it still spills there); the
+// epilogue warps give up 16 each for it.
+constexpr int X3_REGS_MMA = 160, X3_REGS_EPI = 80;
+static_assert(4 * 128 * X3_REGS_EPI + 128 * X3_REGS_MMA <= NTX3 * 96, "register budgets exceed the launch allocation");
 constexpr uint32_t ACT_SUB = XT * 128, ACT_X3 = 3 * ACT_SUB;        // [128][64] bf16 sub-tile, x3 tile
 constexpr uint32_t D_SUB = XT * 32, D_X3 = 3 * D_SUB;               // [128][16] bf16 (SW32)
 constexpr uint32_t W_SUB = 64 * 128, W_X3 = 3 * W_SUB;              // [64][64]
@@ -97,7 +106,7 @@ enum Bar {
     RDY_X0 = 0, RDY_X1,            // 8: X is staged by row tid / 4, warps 0-7 rows 0-63, warps 8-15 rows 64-127
     RDY_H1_0, RDY_H1_1,            // 8
     RDY_H2_0, RDY_H2_1,            // 8
-    RDY_D0, RDY_D1,                // 2: the loss warps (warp / 4 == 0) of the half
+    RDY_D0, RDY_D1,                // 8: each warp stores the dOUT columns of its own actions
     RDY_DZ2_0, RDY_DZ2_1,          // 8
     RDY_DZ1_0, RDY_DZ1_1,          // 8
     // MMA-issue warpgroup -> epilogue warps, one arrival: the product's rows of that half are in the image
@@ -108,10 +117,12 @@ enum Bar {
     DONE_C6,                       // 1: the tile's last gradient product is in the image
     RDY_W,                         // 1: the expect_tx arrival of the weight-image bulk copy
     NBAR };
-__host__ __device__ constexpr uint32_t bar_arrivals(int b) { return b >= DONE_C1_0 ? 1u : (b == RDY_D0 || b == RDY_D1) ? 2u : 8u; }
-constexpr uint32_t OFF_PF = OFF_BARS + NBAR * 8 + 16;                       // float [128][12]: per-sample loss inputs (AP == 8), copied asynchronously
-constexpr int PF_LD = 12;
-constexpr uint32_t X3_SMEM = OFF_PF + XT * PF_LD * 4;
+__host__ __device__ constexpr uint32_t bar_arrivals(int b) { return b >= DONE_C1_0 ? 1u : 8u; }
+// float [128][AP + 3]: per-sample loss inputs (actions or supplied dmu, then logp, adv_r, adv_c; a critic's target at
+// column AP), copied asynchronously by the warps with h == 0 and read by all four warps of the rows
+constexpr uint32_t OFF_PF = OFF_BARS + NBAR * 8 + 16;
+__host__ __device__ constexpr int pf_ld(int AP) { return AP + 3; }
+constexpr uint32_t X3_SMEM = OFF_PF + XT * pf_ld(16) * 4;
 // accumulator columns
 constexpr uint32_t T_ZA = 0, T_ZB = 64, T_OUT = 128, T_DW1 = 144, T_DW2 = 208, T_DW3 = 272, T_DB1 = 288, T_DB2 = 304, T_COLS = 320;
 
@@ -245,6 +256,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 
     if (is_mma_warp) {
         // ======================= MMA-issue warpgroup: uniform control flow ====================================
+        wg_regs_inc<X3_REGS_MMA>();
         const uint64_t dX = desc128(sbase + OFF_X), dH1 = desc128(sbase + OFF_H1), dH2 = desc128(sbase + OFF_H2);
         const uint64_t dD = desc32(sbase + OFF_D), dW1 = desc128(sbase + OFF_W1), dW2 = desc128(sbase + OFF_W2);
         const uint64_t dW3 = desc128(sbase + OFF_W3), dOnes = desc32(sbase + OFF_ONES);
@@ -340,6 +352,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
         }
     } else {
         // ======================= epilogue warps ===============================================================
+        wg_regs_dec<X3_REGS_EPI>();
         const int q = warp & 3, h = warp >> 2, rh = q >> 1;      // rh: the row half of this warp's rows (all but the X staging)
         const uint32_t lane_base = (uint32_t)(q * 32) << 16;
         const int s_row = 32 * q + lane;                 // sample row of this thread in the [s][.] accumulators
@@ -376,7 +389,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
             __syncwarp();
             if (lane == 0) mbar_arrive(bar(b));
         };
-        const bool dbg_on = p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && (tid == 0 || tid == 320);      // a loss warp of rows 0-63, a non-loss warp of rows 64-127
+        const bool dbg_on = p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && (tid == 0 || tid == 320);      // rows 0-63 with h == 0, rows 64-127 with h == 2
         int dbg_n = 0;
         auto stamp = [&](int id) {
             if (dbg_on && dbg_n < 400) {
@@ -422,10 +435,13 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
             }
         }
         uint8_t* wimg = FUSED ? p.wimg + (size_t)net * W_IMG : nullptr;
-        // per-thread partial sums of the loss warps over the tiles of one minibatch (reduced once per minibatch)
-        float acc_st[5] = {0.f, 0.f, 0.f, 0.f, 0.f}, acc_dls[AP], acc_db[AP];      // loss, ratio, kl, count, FOCOPS mask
+        // per-thread partial sums over the tiles of one minibatch (reduced once per minibatch): the statistics of the warps
+        // with h == 0, and every warp's gradients of its own actions a = NA h + j in slot j
+        constexpr int NA = AP / 4;
+        const int a_lo = NA * h;
+        float acc_st[5] = {0.f, 0.f, 0.f, 0.f, 0.f}, acc_dls[NA], acc_db[NA];      // loss, ratio, kl, count, FOCOPS mask
 #pragma unroll
-        for (int a = 0; a < AP; ++a) { acc_dls[a] = 0.f; acc_db[a] = 0.f; }
+        for (int j = 0; j < NA; ++j) { acc_dls[j] = 0.f; acc_db[j] = 0.f; }
 
         int rpar = 0, it = 0;
         if ((int)blockIdx.x < (min(batch, p.b.mb_count) + XT - 1) / XT) {     // rows + X of the first tile
@@ -467,36 +483,23 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 announce(RDY_X0 + (warp >> 3));                            // rows xm = tid / 4: warps 0-7 hold rows 0-63
                 epi_bar_sync();                                            // next tile's row list is complete
                 stamp(2);
-                // loss warps: this tile's per-sample inputs (used in E3) fly under the forward phases -- asynchronously into
-                // shared memory when they fit (AP == 8), so that no register has to wait for them
-                float pf_act[AP], pf_logp = 0.f, pf_advr = 0.f, pf_advc = 0.f, pf_tv = 0.f;
-                long long prow = -1;
+                // this tile's per-sample loss inputs (used in E3) fly under the forward phases, asynchronously into shared
+                // memory (the PF rows), so that no register has to wait for them
                 if (h == 0) {
-                    prow = sRow[s_row];
-#pragma unroll
-                    for (int a = 0; a < AP; ++a) pf_act[a] = 0.f;
+                    const long long prow = sRow[s_row];
                     if (prow >= 0) {
                         const float* asrc = (DMU || p.lc.kind == LOSS_FVP) ? p.fvp_dmu : p.b.act;
-                        if (AP == 8) {
-                            const uint32_t dst = sbase + OFF_PF + (uint32_t)(s_row * PF_LD) * 4u;
-                            auto cp4 = [&](uint32_t d, const float* src) {
-                                asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(d), "l"(src) : "memory");
-                            };
-                            if (net == 0) {
-#pragma unroll
-                                for (int a = 0; a < AP; ++a)
-                                    if (a < A) cp4(dst + 4u * a, asrc + prow * A + a);
-                                if (!DMU && p.lc.kind != LOSS_FVP) { cp4(dst + 32u, p.b.logp + prow); cp4(dst + 36u, p.b.adv_r + prow); cp4(dst + 40u, p.b.adv_c + prow); }
-                            } else {
-                                cp4(dst + 32u, (net == 1 ? p.b.tv_r : p.b.tv_c) + prow);
-                            }
-                        } else if (net == 0) {
+                        const uint32_t dst = sbase + OFF_PF + (uint32_t)(s_row * pf_ld(AP)) * 4u;
+                        auto cp4 = [&](uint32_t d, const float* src) {
+                            asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(d), "l"(src) : "memory");
+                        };
+                        if (net == 0) {
 #pragma unroll
                             for (int a = 0; a < AP; ++a)
-                                if (a < A) pf_act[a] = __ldg(asrc + prow * A + a);
-                            if (!DMU && p.lc.kind != LOSS_FVP) { pf_logp = __ldg(p.b.logp + prow); pf_advr = __ldg(p.b.adv_r + prow); pf_advc = __ldg(p.b.adv_c + prow); }
+                                if (a < A) cp4(dst + 4u * a, asrc + prow * A + a);
+                            if (!DMU && p.lc.kind != LOSS_FVP) { cp4(dst + 4u * AP, p.b.logp + prow); cp4(dst + 4u * AP + 4u, p.b.adv_r + prow); cp4(dst + 4u * AP + 8u, p.b.adv_c + prow); }
                         } else {
-                            pf_tv = __ldg((net == 1 ? p.b.tv_r : p.b.tv_c) + prow);
+                            cp4(dst + 4u * AP, (net == 1 ? p.b.tv_r : p.b.tv_c) + prow);
                         }
                     }
                 }
@@ -528,27 +531,19 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 }
                 announce(RDY_H2_0 + rh);
                 stamp(6);
-                // ---- E3: OUT -> loss -> dOUT (warps with h == 0: one thread per sample) -------------------------
-                if (h == 0) {
-                    if (AP == 8) {
-                        asm volatile("cp.async.wait_all;\n" ::: "memory");
-                        const float* pf = reinterpret_cast<const float*>(gbase + OFF_PF) + s_row * PF_LD;
-                        if (prow >= 0) {
-                            if (net == 0) {
+                // ---- E3: OUT -> loss -> dOUT (one thread per sample in each of the four warps of the rows) -----------
+                // Every warp computes the sample's scalar part of the loss (the same bits in each) and the gradient of
+                // its own actions a_lo .. a_lo + NA - 1; the statistics are those of the warps with h == 0.
+                if (h == 0) asm volatile("cp.async.wait_all;\n" ::: "memory");
+                rows_bar_sync(q);                                          // the PF rows of the four warps' samples
+                mbar_wait_a(bar(DONE_C3_0 + rh), par);
+                stamp(7);
+                {
+                    const long long prow = sRow[s_row];
+                    const float* pf = reinterpret_cast<const float*>(gbase + OFF_PF) + s_row * pf_ld(AP);
+                    float o[AP], dq[NA];
 #pragma unroll
-                                for (int a = 0; a < AP; ++a)
-                                    if (a < A) pf_act[a] = pf[a];
-                                pf_logp = pf[8]; pf_advr = pf[9]; pf_advc = pf[10];
-                            } else {
-                                pf_tv = pf[8];
-                            }
-                        }
-                    }
-                    mbar_wait_a(bar(DONE_C3_0 + rh), par);
-                    stamp(7);
-                    float o[AP], d16[16];
-#pragma unroll
-                    for (int a = 0; a < 16; ++a) d16[a] = 0.f;
+                    for (int j = 0; j < NA; ++j) dq[j] = 0.f;
                     if (AP == 8) {
                         float t8[8];
                         acc_ld8(tm, lane_base + T_OUT, t8);
@@ -560,52 +555,64 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 #pragma unroll
                         for (int a = 0; a < AP; ++a) o[a] = t16[a];
                     }
+                    auto own = [&](int a) { return a < A && a >= a_lo && a < a_lo + NA; };
                     if (prow >= 0) {
-                        if (DMU && net != 0) {       // critic: the supplied dL/dV (tv_r / tv_c)
-                            if (p.value_out) p.value_out[prow] = o[0] + sB3[0];
-                            acc_st[3] += 1.f;
-                            d16[0] = pf_tv;
-                            acc_db[0] += pf_tv;
-                        } else if (net != 0) {
-                            const float d = o[0] + sB3[0] - pf_tv;
-                            acc_st[0] += d * d; acc_st[3] += 1.f;
-                            d16[0] = 2.f * d * inv_b;
-                            acc_db[0] += d16[0];
+                        if (net != 0) {              // critic: one output, action 0 of the warps with h == 0
+                            if (h == 0) {
+                                const float tv = pf[AP];
+                                if (DMU) {           // the supplied dL/dV (tv_r / tv_c)
+                                    if (p.value_out) p.value_out[prow] = o[0] + sB3[0];
+                                    acc_st[3] += 1.f;
+                                    dq[0] = tv;
+                                    acc_db[0] += tv;
+                                } else {
+                                    const float d = o[0] + sB3[0] - tv;
+                                    acc_st[0] += d * d; acc_st[3] += 1.f;
+                                    dq[0] = 2.f * d * inv_b;
+                                    acc_db[0] += dq[0];
+                                }
+                            }
                         } else if (DMU) {
-                            acc_st[3] += 1.f;
+                            if (h == 0) acc_st[3] += 1.f;
 #pragma unroll
                             for (int a = 0; a < AP; ++a)
-                                if (a < A) { d16[a] = pf_act[a]; acc_db[a] += pf_act[a]; }
+                                if (own(a)) { const float dm = pf[a]; dq[a % NA] = dm; acc_db[a % NA] += dm; }
                         } else if (p.lc.kind == LOSS_FVP) {
                             // J^T diag(sigma^-2) dmu / (B A): the supplied tangent is the output gradient
-                            acc_st[3] += 1.f;
+                            if (h == 0) acc_st[3] += 1.f;
 #pragma unroll
                             for (int a = 0; a < AP; ++a)
-                                if (a < A) {
-                                    const float dm = pf_act[a] * sLs[32 + a] * p.fvp_scale;
-                                    d16[a] = dm;
-                                    acc_db[a] += dm;
+                                if (own(a)) {
+                                    const float dm = pf[a] * sLs[32 + a] * p.fvp_scale;
+                                    dq[a % NA] = dm;
+                                    acc_db[a % NA] += dm;
                                 }
                         } else {
-                            float mu[AP];
+                            float mu[AP], act[AP];
 #pragma unroll
-                            for (int a = 0; a < AP; ++a) mu[a] = o[a] + sB3[a];
-                            actor_sample_loss<!FUSED, AP>(p.lc, an, A, inv_b, mu, pf_act,
-                                                                               [&](int a) { return __ldg(p.lc.mu_old + prow * A + a); },
-                                                                               pf_logp, pf_advr, pf_advc, sLs, misc + MF_OLD, acc_st,
-                                                                               [&](int a, float dm, float dl) {
-                                                                                   d16[a] = dm; acc_db[a] += dm; acc_dls[a] += dl;
-                                                                               });
+                            for (int a = 0; a < AP; ++a) { mu[a] = o[a] + sB3[a]; act[a] = (a < A) ? pf[a] : 0.f; }
+                            actor_sample_loss<!FUSED, AP>(p.lc, an, A, inv_b, mu, act,
+                                                          [&](int a) { return __ldg(p.lc.mu_old + prow * A + a); },
+                                                          pf[AP], pf[AP + 1], pf[AP + 2], sLs, misc + MF_OLD, acc_st,
+                                                          [&](int a, float dm, float dl) {
+                                                              dq[a % NA] = dm; acc_db[a % NA] += dm; acc_dls[a % NA] += dl;
+                                                          },
+                                                          a_lo, a_lo + NA, h == 0);
                         }
                     }
-                    store16_x3_sw32(sbase + OFF_D, D_SUB, s_row, d16);
+                    // this warp's columns of the dOUT row: its actions, and (AP == 8) as many of the zero columns 8 .. 15
+#pragma unroll
+                    for (int k = 0; k < 2; ++k) {
+                        const int c = (AP == 8) ? 2 * h + 8 * k : 4 * h + 2 * k;
+                        const bool mine = AP == 16 || k == 0;
+                        store2_x3_sw32(sbase + OFF_D, D_SUB, s_row, c, mine ? dq[(2 * k) % NA] : 0.f, mine ? dq[(2 * k + 1) % NA] : 0.f);
+                    }
                     announce(RDY_D0 + rh);
                     stamp(8);
                 }
                 stamp(9);
                 if (!FUSED && p.forward_only) {                                      // statistics pass: no backward; H2 is free once OUT is done
                     if (has_next) prefetch_x(sRowNext);
-                    if (h != 0) { mbar_wait_a(bar(DONE_C3_0 + rh), par); }
                     rpar ^= 1;
                     continue;
                 }
@@ -674,25 +681,28 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
             }
             // ---- this CTA's partial gradient of the minibatch: accumulator images -> global ------------------------
             if (have_tiles) {
-                // loss-warp sums: lanes -> warp (butterfly) -> the four loss warps (fixed order)
+                // statistics: lanes -> warp (butterfly) -> the four warps with h == 0 (fixed order)
                 if (h == 0) {
 #pragma unroll
                     for (int i = 0; i < 5; ++i) acc_st[i] = warp_sum(acc_st[i]);
-#pragma unroll
-                    for (int a = 0; a < AP; ++a) { acc_dls[a] = warp_sum(acc_dls[a]); acc_db[a] = warp_sum(acc_db[a]); }
                     if (lane == 0) {
 #pragma unroll
                         for (int i = 0; i < 5; ++i) sRed[q * 8 + i] = acc_st[i];
-#pragma unroll
-                        for (int a = 0; a < AP; ++a) { sRed[32 + q * 16 + a] = acc_dls[a]; sRed[96 + q * 16 + a] = acc_db[a]; }
                     }
 #pragma unroll
                     for (int i = 0; i < 5; ++i) acc_st[i] = 0.f;
-#pragma unroll
-                    for (int a = 0; a < AP; ++a) { acc_dls[a] = 0.f; acc_db[a] = 0.f; }
                 }
+                // gradient sums of every warp's own actions: lanes -> warp (butterfly), per action
+#pragma unroll
+                for (int j = 0; j < NA; ++j) { acc_dls[j] = warp_sum(acc_dls[j]); acc_db[j] = warp_sum(acc_db[j]); }
+                if (lane == 0) {
+#pragma unroll
+                    for (int j = 0; j < NA; ++j) { sRed[32 + q * 16 + a_lo + j] = acc_dls[j]; sRed[96 + q * 16 + a_lo + j] = acc_db[j]; }
+                }
+#pragma unroll
+                for (int j = 0; j < NA; ++j) { acc_dls[j] = 0.f; acc_db[j] = 0.f; }
                 if (!FUSED && p.forward_only) {
-                    epi_bar_sync();                    // sRed of the four loss warps
+                    epi_bar_sync();                    // sRed of the sixteen epilogue warps
                     if (tid >= 64 && tid < 72) {
                         const int i = tid - 64;
                         __stcg(p.stats_part + ((size_t)blockIdx.x * 3 + net) * 8 + i, (i < 5) ? (sRed[i] + sRed[8 + i]) + (sRed[16 + i] + sRed[24 + i]) : 0.f);
@@ -744,7 +754,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     acc_ld16(tm, lane_base + T_DB2, v);
                     if (lane < 16) __stcg(gout + L.off_b2 + t_row, v[0]);
                 }
-                epi_bar_sync();                        // sRed of the four loss warps
+                epi_bar_sync();                        // sRed of the sixteen epilogue warps
                 if (tid < L.out) __stcg(gout + L.off_b3 + tid, (sRed[96 + tid] + sRed[112 + tid]) + (sRed[128 + tid] + sRed[144 + tid]));
                 if (net == 0 && tid >= 32 && tid < 32 + A) {
                     const int a = tid - 32;

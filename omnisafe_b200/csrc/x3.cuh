@@ -271,6 +271,16 @@ __device__ __forceinline__ void store16_x3_sw32(uint32_t base, uint32_t split, i
     sts128(o0 + 2 * split, w2[0], w2[1], w2[2], w2[3]); sts128(o1 + 2 * split, w2[4], w2[5], w2[6], w2[7]);
 }
 
+// store the column pair (c, c + 1) (c even) of row r of a SW32 x3 tile: the words store16_x3_sw32 writes there
+__device__ __forceinline__ void store2_x3_sw32(uint32_t base, uint32_t split, int r, int c, float a, float b) {
+    uint32_t w0, w1, w2;
+    split2(a, b, w0, w1, w2);
+    const uint32_t o = base + off32(r, c);
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(o), "r"(w0) : "memory");
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(o + split), "r"(w1) : "memory");
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(o + 2 * split), "r"(w2) : "memory");
+}
+
 // single element stores (weight staging)
 __device__ __forceinline__ void store1_x3(uint32_t base, uint32_t split, uint32_t off, float x) {
     uint32_t w0, w1, w2;

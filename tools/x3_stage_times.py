@@ -1,5 +1,6 @@
 """Where one CTA of the persistent bf16x3 update kernel spends its time: clock64 stamps of CTA (0, 0)
-(thread 0 = a loss warp of rows 0-63, thread 320 = a non-loss warp of rows 64-127, thread 512 = the MMA-issue warpgroup)."""
+(thread 0 = warp 0: rows 0-63, statistics and actions 0 .. AP / 4 - 1 of the loss; thread 320 = warp 10: rows 64-127;
+thread 512 = the MMA-issue warpgroup)."""
 import os, sys, tempfile
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -24,7 +25,7 @@ for k, prod in enumerate(('Z1', 'Z2', 'OUT', "dZ2'", "dZ1'")):
     for r in range(2):
         for ev, what in enumerate(('operands ready', 'MMAs complete', 'stored', 'committed')):
             NAMES[100 + 20 * k + 4 * r + ev] = f'{prod}[{r}] {what}'
-for which, off in (('thread 0 (loss warp, rows 0-63)', 0), ('thread 320 (rows 64-127)', 1024)):
+for which, off in (('thread 0 (rows 0-63)', 0), ('thread 320 (rows 64-127)', 1024)):
     d = dbg[off:off + 1024].cpu().tolist()
     n = d[0]
     print(f'== {which}: {n} stamps (last update iteration kept the buffer)')
