@@ -165,7 +165,7 @@ int osb_eval_synthetic(int O, int A, int max_episode_steps, unsigned seed, unsig
  * Per episode schedule: env.reset() -> osb_eval_ext_observe(is_reset = 1, t = -1); for t = 0, 1, ...:
  * osb_eval_ext_act(t) -> env.step(act_env) -> osb_eval_ext_observe(t); then read ctr: ctr[0] == 0 ends the evaluation,
  * ctr[2] > 0 (N == 1: the episode ended and another follows) asks for env.reset() -> osb_eval_ext_observe(is_reset = 1, t).
- * N > 1 relies on the envs resetting themselves.  osb_eval_ext_act: ObsNormalize, the deterministic forward, act_env[N][A]
+ * N > 1 relies on the envs resetting themselves (an episode the cost rule cuts: osb_eval_ext_observe_rst below).  osb_eval_ext_act: ObsNormalize, the deterministic forward, act_env[N][A]
  * <- ActionScale onto [act_lo, act_hi] (as osb_ext_act), act_out as above; no slabs.  osb_eval_ext_observe: the fp64
  * sums, Saute z, the cost rule and the episode ends of the running envs; next_obs -> s_raw (the buffer step t + 1
  * reads); ObsNormalize pushes the final rows of running envs (final_obs / final_mask may be NULL), then the next rows
@@ -183,6 +183,28 @@ int osb_eval_ext_observe(int O, int N, int t, int obs_normalize, int is_reset, c
                          float safety_budget, float saute_gamma, int early, double cost_limit, double cost_criteria,
                          int* left, int* done_eps, double* ret, double* cost_acc, int* len, int* ctr, double* out_ret,
                          double* out_cost, int* out_len, double* workspace, int* nonfinite, void* stream);
+/* The cost rule at N > 1 on a registered env with the optional reset_envs(mask) hook (envs/core.py).  Per step:
+ * osb_eval_ext_act(t) -> env.step -> osb_eval_ext_observe_rst(t) -> env.reset_envs(rst) -> osb_ext_reset_rows(t) with
+ * mask = rst and the returned rows, with no host synchronisation in between.  osb_eval_ext_observe_rst =
+ * osb_eval_ext_observe of a step (is_reset = 0), plus rst[N] (one byte per env, written on every call): 1 where the cost
+ * rule ended a running env's episode that the env did not end itself (terminated and truncated both 0) and the env has
+ * episodes left, else 0.  osb_ext_reset_rows then writes those envs' reset rows into the state buffer step t + 1 reads
+ * and pushes them into ObsNormalize as the step's third batch, after its final and next rows (no row set: untouched).
+ * t enters osb_eval_ext_act / osb_eval_ext_observe(_rst) / osb_ext_reset_rows only through its parity, so the launches
+ * of a block of steps captured into a CUDA graph at an even t replay as any block at an even offset; once ctr[0] == 0
+ * every launch leaves the results, the statistics and act_out as they are.
+ * osb_eval_ext_prepare performs the one-time host actions of osb_eval_ext_act (kernel attributes, the tensor-core
+ * accumulator image) for a network input of On columns (O, + 1 with safety) and N envs; call it before capturing an
+ * osb_eval_ext_act launch.  The observe and reset-rows launches need no preparation. */
+int osb_eval_ext_observe_rst(int O, int N, int t, int obs_normalize, const float* next_obs, const float* rew,
+                             const float* cost, const unsigned char* terminated, const unsigned char* truncated,
+                             const float* final_obs, const unsigned char* final_mask, float* s_raw, float* norm_mean,
+                             float* norm_sumsq, float* norm_std, long long* norm_count, unsigned* ticket, float* safety,
+                             float safety_budget, float saute_gamma, int early, double cost_limit,
+                             double cost_criteria, int* left, int* done_eps, double* ret, double* cost_acc, int* len,
+                             int* ctr, double* out_ret, double* out_cost, int* out_len, double* workspace,
+                             int* nonfinite, unsigned char* rst, void* stream);
+int osb_eval_ext_prepare(int On, int A, int N, int precision);
 /* ---- rollout on an external env (a user CMDP stepped in PyTorch) ----------------------------
  * The fused step split at the env boundary.  Per epoch: env.reset() -> osb_ext_reset_ingest; for t in [0, T):
  * osb_ext_act(t) -> env.step(act_env) -> osb_ext_observe(t); then osb_ext_act(T) (epoch-end bootstrap, critics only)

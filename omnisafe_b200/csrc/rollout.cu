@@ -1507,10 +1507,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) ext_reset_rows_kernel(const float
 // observations of every running env (reset: the observations of every env with episodes left), as fp64 per-tile
 // moments combined in tile order by the last CTA (ext_observe_kernel's scheme), with per-tile row counts.  The last CTA
 // also advances the done word ctr[0]; ctr[2] counts the envs to reset now (N == 1: every episode end with episodes left),
-// and a reset ingest clears it.
-__global__ void __launch_bounds__(NTHREADS) ext_eval_observe_kernel(ExtObs x, EnvState st, NormState ns, SauteSpec sa,
-                                                                    EvalSpec ev, int O, int N, int t, int obs_normalize,
-                                                                    int is_reset) {
+// and a reset ingest clears it.  RST: rst[env] (one byte per env, written on every launch) is 1 where the cost rule ended
+// a running env's episode that the env itself did not end, and the env has episodes left: the envs the caller resets
+// through reset_envs(mask) before ext_reset_rows_kernel ingests their rows.
+template <bool RST>
+__device__ __forceinline__ void ext_eval_observe_step(ExtObs x, EnvState st, NormState ns, SauteSpec sa, EvalSpec ev,
+                                                      int O, int N, int t, int obs_normalize, int is_reset,
+                                                      uint8_t* rst_out) {
     __shared__ int sRun[XT], sFin[XT];
     __shared__ int s_bad, s_nrun, s_nfin;
     const int tid = threadIdx.x, tile = blockIdx.x, ntiles = gridDim.x;
@@ -1518,7 +1521,7 @@ __global__ void __launch_bounds__(NTHREADS) ext_eval_observe_kernel(ExtObs x, En
     if (tid == 0) s_bad = 0;
     if (tid < XT) {
         const int env = env0 + tid;
-        int run = 0, fin = 0, nxt = 0, rst = 0;
+        int run = 0, fin = 0, nxt = 0, rst = 0, cut = 0;
         if (tid < rows && ev.left[env] > 0) {
             run = 1;
             if (!is_reset) {
@@ -1527,9 +1530,11 @@ __global__ void __launch_bounds__(NTHREADS) ext_eval_observe_kernel(ExtObs x, En
                 const int len = ev.len[env];
                 const double r64 = ev.ret[env] + (double)rew;
                 const double c64 = ev.cost[env] + pow(ev.crit, (double)len) * (double)cst;
-                const bool done = x.term[env] != 0 || x.trunc[env] != 0 || (ev.early && c64 >= ev.cost_limit);
+                const bool env_done = x.term[env] != 0 || x.trunc[env] != 0;
+                const bool done = env_done || (ev.early && c64 >= ev.cost_limit);
                 if (sa.safety) saute_step(sa, t, N, env, rew, cst, done);
                 const int left = ev.left[env];
+                if constexpr (RST) cut = (done && !env_done && left > 1) ? 1 : 0;
                 if (done) {
                     const int k = ev.done_eps[env];
                     const size_t out = (size_t)env + (size_t)k * N;
@@ -1545,6 +1550,9 @@ __global__ void __launch_bounds__(NTHREADS) ext_eval_observe_kernel(ExtObs x, En
             }
         }
         sRun[tid] = run; sFin[tid] = fin;
+        if constexpr (RST) {
+            if (tid < rows) rst_out[env] = (uint8_t)cut;
+        }
         if (!is_reset) {
             if (nxt) atomicAdd(ev.ctr + 1, 1);
             if (rst) atomicAdd(ev.ctr + 2, 1);
@@ -1632,6 +1640,18 @@ __global__ void __launch_bounds__(NTHREADS) ext_eval_observe_kernel(ExtObs x, En
         }
         *ns.ticket = 0u;
     }
+}
+
+__global__ void __launch_bounds__(NTHREADS) ext_eval_observe_kernel(ExtObs x, EnvState st, NormState ns, SauteSpec sa,
+                                                                    EvalSpec ev, int O, int N, int t, int obs_normalize,
+                                                                    int is_reset) {
+    ext_eval_observe_step<false>(x, st, ns, sa, ev, O, N, t, obs_normalize, is_reset, nullptr);
+}
+
+__global__ void __launch_bounds__(NTHREADS) ext_eval_observe_rst_kernel(ExtObs x, EnvState st, NormState ns,
+                                                                        SauteSpec sa, EvalSpec ev, int O, int N, int t,
+                                                                        int obs_normalize, uint8_t* rst) {
+    ext_eval_observe_step<true>(x, st, ns, sa, ev, O, N, t, obs_normalize, 0, rst);
 }
 
 // Window of the last <= W finished episodes in (step, env) append order: Logger deque semantics
@@ -1803,7 +1823,8 @@ static int ext_refuse_if_capturing(cudaStream_t stream, const char* what) {
     OSB_CUDA(cudaStreamIsCapturing(stream, &cs));
     if (cs == cudaStreamCaptureStatusNone) return OSB_OK;
     char msg[256];
-    snprintf(msg, sizeof(msg), "osb_ext_act on a capturing stream needs %s: call osb_ext_prepare before the capture", what);
+    snprintf(msg, sizeof(msg), "osb_ext_act / osb_eval_ext_act on a capturing stream needs %s: call osb_ext_prepare / "
+             "osb_eval_ext_prepare before the capture", what);
     osb_set_error(msg);
     return OSB_ERR_UNSUPPORTED;
 }
@@ -2088,6 +2109,32 @@ int osb_eval_ext_observe(int O, int N, int t, int obs_normalize, int is_reset, c
     return OSB_OK;
 }
 
+// osb_eval_ext_observe of a step (no reset ingest) that also writes rst[N], the envs the cost rule cut with episodes left
+int osb_eval_ext_observe_rst(int O, int N, int t, int obs_normalize, const float* next_obs, const float* rew,
+                             const float* cost, const unsigned char* terminated, const unsigned char* truncated,
+                             const float* final_obs, const unsigned char* final_mask, float* s_raw, float* norm_mean,
+                             float* norm_sumsq, float* norm_std, long long* norm_count, unsigned* ticket, float* safety,
+                             float safety_budget, float saute_gamma, int early, double cost_limit,
+                             double cost_criteria, int* left, int* done_eps, double* ret, double* cost_acc, int* len,
+                             int* ctr, double* out_ret, double* out_cost, int* out_len, double* workspace,
+                             int* nonfinite, unsigned char* rst, void* stream) {
+    OSB_CHECK_ARG(O > 0 && N > 0 && t >= 0, "bad dims / step index");
+    OSB_CHECK_ARG(next_obs && rew && cost && terminated && truncated && s_raw && norm_mean && norm_sumsq && norm_std &&
+                  norm_count && ticket && left && done_eps && ret && cost_acc && len && ctr && out_ret && out_cost &&
+                  out_len && workspace && nonfinite && rst, "bad argument");
+    OSB_CHECK_ARG(safety == nullptr || (safety_budget > 0.f && saute_gamma > 0.f), "safety_budget and saute_gamma must be positive");
+    ExtObs x{next_obs, rew, cost, terminated, truncated, final_obs, final_mask, workspace, nonfinite};
+    EnvState st{s_raw, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    NormState ns{norm_mean, norm_sumsq, norm_std, nullptr, nullptr, norm_count, nullptr, nullptr, nullptr, nullptr, ticket};
+    SauteSpec sa{safety, safety ? safety_budget : 1.f, safety ? saute_gamma : 1.f, 0.f, 1.f};
+    EvalSpec ev{left, done_eps, ret, cost_acc, len, out_ret, out_cost, out_len, nullptr, ctr, cost_criteria, cost_limit,
+                early, N == 1 ? 1 : 0, nullptr};
+    ext_eval_observe_rst_kernel<<<(N + XT - 1) / XT, NTHREADS, 0, (cudaStream_t)stream>>>(x, st, ns, sa, ev, O, N, t,
+                                                                                         obs_normalize, rst);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}
+
 // ---- external envs ---------------------------------------------------------------------------
 int osb_ext_workspace_doubles(int O, int N) { return ((N + XT - 1) / XT) * (4 * O + 1); }
 
@@ -2236,6 +2283,14 @@ int osb_ext_prepare(int O, int A, int N, int precision) {
     OSB_CHECK_ARG(O > 0 && A > 0 && A <= OUTP && N > 0, "bad dims (need 0 < A <= 16)");
     StepArgs p = ext_step_args(O, A, 0, N, precision);
     return launch_rollout<true, false>(p, nullptr, false, true);
+}
+
+// On: the network input width (O, + 1 with the Saute column); the host actions depend on nothing else of the state
+int osb_eval_ext_prepare(int On, int A, int N, int precision) {
+    OSB_CHECK_ARG(On > 0 && A > 0 && A <= OUTP && N > 0, "bad dims (need 0 < A <= 16)");
+    OSB_CHECK_ARG(precision >= 0 && precision <= 2, "precision must be 0, 1 or 2");
+    StepArgs p = ext_step_args(On, A, 0, N, precision);
+    return launch_rollout<true, true>(p, nullptr, false, true);
 }
 
 }  // extern "C"

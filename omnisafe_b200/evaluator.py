@@ -5,7 +5,8 @@ config.json and `torch_save/<model_name>`: the actor from 'pi' and, with `algo_c
 statistics from 'obs_normalizer'.  `evaluate` runs the episodes with the semantics of the reference loop, on the GPU in
 the evaluation mode of the rollout step kernels (csrc/rollout.cu): the synthetic env entirely inside them
 (osb_eval_synthetic), a registered env stepped in PyTorch between an act and an observe launch (osb_eval_ext_act /
-osb_eval_ext_observe, one read of a 3-int counter per step):
+osb_eval_ext_observe, one read of a 3-int counter per step; a graph-safe env at E > 1 replays blocks of 16 steps from
+a CUDA graph and reads the 4-byte done word once per block, OSB_NO_GRAPH=1 keeps it eager):
 
 - the env is built with the config's env_cfgs and its default seed (the evaluator does not call set_seed);
 - every observation the env returns goes through ObsNormalize, which still pushes it into the loaded statistics, so they
@@ -18,9 +19,10 @@ osb_eval_ext_observe, one read of a 3-int counter per step):
 
 One extension: `evaluate(num_envs=E)` runs E envs at once, env e playing episodes e, e + E, ...; results still come
 back in episode order.  E changes the order in which rows reach the normaliser, and so the results: E = 1 (the default)
-is the reference.  With E > 1 the envs reset themselves at their episode ends (an episode cut by the cost rule resets
-its env on the synthetic env; on a registered env, which has no per-env reset, the cost rule needs E = 1), each step
-pushes the rows of the envs still running, in env order.
+is the reference.  With E > 1 the envs reset themselves at their episode ends, and an episode cut by the cost rule
+resets its env: on the synthetic env inside the kernels, on a registered env through its optional `reset_envs(mask)`
+hook (envs/core.py; without it the cost rule needs E = 1).  Each step pushes the rows of the envs still running, in env
+order, then the reset rows of the envs the rule cut that have episodes left.
 
 The evaluator builds its own env state, normaliser and parameters; a live run's are never touched.
 """
@@ -41,6 +43,7 @@ from omnisafe_b200.models.actor_critic import param_layout
 from omnisafe_b200.utils.config import Config
 
 PRECISIONS = {'fp32': 0, 'tf32': 1, 'bf16x3': 2}
+GRAPH_BLOCK = 16    # steps per captured block of a graph-safe registered env (even: t enters only by its parity)
 
 
 class Evaluator:
@@ -78,8 +81,9 @@ class Evaluator:
             probe = SyntheticBoxEnv(cfgs.env_id, num_envs=1, device='cpu', **self._env_cfgs)
             self._obs_dim, self._act_dim = probe.obs_dim, probe.act_dim
         else:
-            self._obs_dim, self._act_dim, _, _ = check_env(make(cfgs.env_id, num_envs=1, device=self._device,
-                                                                **self._env_cfgs))
+            probe = make(cfgs.env_id, num_envs=1, device=self._device, **self._env_cfgs)
+            self._obs_dim, self._act_dim, _, _ = check_env(probe)
+            self._reset_envs = callable(getattr(probe, 'reset_envs', None))
         On, A = self._obs_dim + int(self._saute), self._act_dim
         # the actor's flat parameters in the rollout's layout (the critics are not evaluated)
         layout = param_layout(On, A)
@@ -106,9 +110,10 @@ class Evaluator:
         num_episodes = int(num_episodes)
         assert num_episodes >= 1 and num_envs >= 1, 'num_episodes and num_envs must be positive'
         E, O, dev = min(int(num_envs), num_episodes), self._obs_dim, self._device
-        if not self._synthetic and self._early and E > 1:
-            raise NotImplementedError('the EarlyTerminated rule on a registered env needs num_envs=1: the env cannot be '
-                                      'reset on its own when the cost rule cuts an episode')
+        if not self._synthetic and self._early and E > 1 and not self._reset_envs:
+            raise NotImplementedError(
+                f'evaluating EarlyTerminated on {self._cfgs.env_id} with {E} envs needs the optional reset_envs(mask) '
+                'hook (envs/core.py) to reset the envs the cost limit cuts; without it only num_envs=1 is supported')
         norm = Normalizer((O,), clip=5.0, device=dev)
         if self._norm_sd is not None:
             norm.load_state_dict(self._norm_sd)
@@ -156,8 +161,12 @@ class Evaluator:
             ptr(self._theta), self._precision, int(self._per_step), current_stream())
 
     def _run_registered(self, E, crit, norm, w) -> None:
-        """env.reset() -> ingest; then per step: act launch -> env.step -> observe launch -> read the counters (done
-        word, resets asked for); E = 1 resets the env after every episode that another one follows."""
+        """env.reset() -> ingest; then per step: act launch -> env.step -> observe launch.  Eagerly, the counters (done
+        word, resets asked for) are read after every step, and E = 1 resets the env after every episode that another one
+        follows.  With the cost rule at E > 1 the observe launch also writes the mask of the envs it cut, which
+        env.reset_envs(mask) resets and osb_ext_reset_rows ingests, with no host synchronisation.  A graph-safe env at
+        E > 1 runs one eager block of GRAPH_BLOCK steps, then replays the next block, captured into a CUDA graph, until
+        the done word (read once per block) is 0: steps after the last episode ended change nothing but the env."""
         O, A, dev, L = self._obs_dim, self._act_dim, self._device, lib()
         env = make(self._cfgs.env_id, num_envs=E, device=dev, **self._env_cfgs)   # the env's default seed
         _, _, lo, hi = check_env(env)
@@ -166,21 +175,24 @@ class Evaluator:
         act_env = torch.zeros(E, A, dtype=torch.float32, device=dev)
         ws = torch.zeros(L.osb_eval_ext_workspace_doubles(O, E), dtype=torch.float64, device=dev)
         nonfinite = torch.zeros(1, dtype=torch.int32, device=dev)
+        cut = self._early and E > 1         # envs the cost rule cuts are reset through env.reset_envs(rst)
+        rst = torch.zeros(E, dtype=torch.bool, device=dev) if cut else None
+        graph = E > 1 and bool(getattr(env, 'graph_safe', False)) and not os.getenv('OSB_NO_GRAPH')
         rows = lambda x, width=None, dtype=torch.float32: torch.as_tensor(x).to(            # noqa: E731
             device=dev, dtype=dtype).reshape((E,) if width is None else (E, width)).contiguous()
-        on, s = int(self._obs_normalize), current_stream()
+        on = int(self._obs_normalize)
         tail = (ptr(s_raw), ptr(norm.mean), ptr(norm.sumsq), ptr(norm.std), ptr(norm.count), ptr(norm.ticket),
                 ptr(w['safety']), self._budget, self._saute_gamma, int(self._early), self._cost_limit, crit,
                 ptr(w['left']), ptr(w['done_eps']), ptr(w['ret']), ptr(w['cost']), ptr(w['len']), ptr(w['ctr']),
-                ptr(w['out_ret']), ptr(w['out_cost']), ptr(w['out_len']), ptr(ws), ptr(nonfinite), s)
+                ptr(w['out_ret']), ptr(w['out_cost']), ptr(w['out_len']), ptr(ws), ptr(nonfinite))
 
         def ingest(t):
-            obs = rows(env.reset()[0], O)
-            L.osb_eval_ext_observe(O, E, t, on, 1, ptr(obs), 0, 0, 0, 0, 0, 0, *tail)
+            obs = env.reset()[0]
+            L.osb_eval_ext_observe(O, E, t, on, 1, ptr(rows(obs, O)), 0, 0, 0, 0, 0, 0, *tail, current_stream())
+            return torch.as_tensor(obs).device
 
-        ingest(-1)
-        t = 0
-        while True:
+        def step(t, capture=False):
+            s = current_stream()
             L.osb_eval_ext_act(O, A, on, E, t, ptr(s_raw), ptr(norm.mean), ptr(norm.std), ptr(norm.count),
                                ptr(w['safety']), ptr(self._theta), ptr(act_lo), ptr(act_hi), ptr(act_env), ptr(w['left']),
                                ptr(w['ctr']), ptr(w['act_out']), self._precision, s)
@@ -188,19 +200,58 @@ class Evaluator:
             nobs, rew, cost, term, trunc, info = env.step(action[0] if E == 1 else action)
             nobs, rew, cost = rows(nobs, O), rows(rew), rows(cost)
             term, trunc = rows(term, dtype=torch.uint8), rows(trunc, dtype=torch.uint8)
+            if capture and ('final_observation' not in info or '_final_observation' not in info):
+                raise OsbError(f'{type(env).__name__} is graph_safe but its step info lacks final_observation / '
+                               '_final_observation: a captured step must report them on every step')
             final = mask = None
             if 'final_observation' in info:
                 final = rows(info['final_observation'], O)
                 mask = info.get('_final_observation')
                 mask = (term | trunc) if mask is None else rows(mask, dtype=torch.uint8)
-            L.osb_eval_ext_observe(O, E, t, on, 0, ptr(nobs), ptr(rew), ptr(cost), ptr(term), ptr(trunc), ptr(final),
-                                   ptr(mask), *tail)
-            running, _, resets = (int(x) for x in w['ctr'].cpu())
-            if running == 0:
-                break
-            if resets:
-                ingest(t)
-            t += 1
+            step_ptrs = (ptr(nobs), ptr(rew), ptr(cost), ptr(term), ptr(trunc), ptr(final), ptr(mask))
+            if not cut:
+                L.osb_eval_ext_observe(O, E, t, on, 0, *step_ptrs, *tail, s)
+                return
+            L.osb_eval_ext_observe_rst(O, E, t, on, *step_ptrs, *tail, ptr(rst), s)
+            obs = rows(env.reset_envs(rst.to(env_dev)), O)
+            L.osb_ext_reset_rows(O, E, t, on, ptr(rst), ptr(obs), ptr(s_raw), ptr(norm.mean), ptr(norm.sumsq),
+                                 ptr(norm.std), ptr(norm.count), ptr(norm.ticket), ptr(ws), ptr(nonfinite), s)
+
+        env_dev = ingest(-1)
+        if graph:
+            if env_dev.type != 'cuda':
+                raise ValueError(f'{type(env).__name__} declares graph_safe but reset() returned observations on '
+                                 f'{env_dev}')
+            done_host = torch.zeros(1, dtype=torch.int32).pin_memory()
+
+            def finished():
+                done_host.copy_(w['ctr'][:1], non_blocking=True)
+                torch.cuda.current_stream().synchronize()
+                return int(done_host[0]) == 0
+
+            # t reaches the kernels only through its parity: a block captured at an even t replays at every even t
+            for t in range(GRAPH_BLOCK):
+                step(t)
+            if not finished():
+                L.osb_eval_ext_prepare(O + int(self._saute), A, E, self._precision)
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g):
+                    for t in range(GRAPH_BLOCK, 2 * GRAPH_BLOCK):
+                        step(t, capture=True)
+                while True:
+                    g.replay()
+                    if finished():
+                        break
+        else:
+            t = 0
+            while True:
+                step(t)
+                running, _, resets = (int(x) for x in w['ctr'].cpu())
+                if running == 0:
+                    break
+                if resets:
+                    ingest(t)
+                t += 1
         if int(nonfinite.item()):
             raise OsbError(f'{self._cfgs.env_id} returned a non-finite observation during the evaluation')
 
