@@ -170,7 +170,8 @@ int osb_eval_synthetic(int O, int A, int max_episode_steps, unsigned seed, unsig
  * sums, Saute z, the cost rule and the episode ends of the running envs; next_obs -> s_raw (the buffer step t + 1
  * reads); ObsNormalize pushes the final rows of running envs (final_obs / final_mask may be NULL), then the next rows
  * of running envs (reset: the rows of envs with episodes left) from fp64 per-tile moments combined in tile order.
- * workspace: osb_eval_ext_workspace_doubles(O, N) doubles; nonfinite as for osb_ext_observe. */
+ * workspace: osb_eval_ext_workspace_doubles(O, N) doubles, the same size as osb_ext_workspace_doubles (one layout for
+ * every fp64 push, so this workspace also serves osb_ext_reset_rows); nonfinite as for osb_ext_observe. */
 int osb_eval_ext_workspace_doubles(int O, int N);
 int osb_eval_ext_act(int O, int A, int obs_normalize, int N, int t, const float* s_raw, const float* norm_mean,
                      const float* norm_std, const long long* norm_count, const float* safety, const float* theta,
@@ -211,7 +212,8 @@ int osb_eval_ext_prepare(int On, int A, int N, int precision);
  * and osb_episode_window.  State arrays as for osb_rollout_step: s_raw[2][N][O] and final_raw[2][N][O] by step parity,
  * ep_ret / ep_cost / ep_len [N], the normaliser state (acc_all / acc_fin / fin_count are not used: the observation
  * statistics are combined from fp64 per-tile moments in fixed tile order, so they are exact to fp64 rounding for any
- * observation range and the same on every run).  workspace: osb_ext_workspace_doubles(O, N) doubles.
+ * observation range and the same on every run).  workspace: osb_ext_workspace_doubles(O, N) doubles, the size every
+ * fp64 push of the observe, evaluation-observe and reset-rows calls shares.
  * nonfinite (device int) is set to 1 when an observation (next or final) is not finite; it is never cleared here.
  * osb_ext_act = the network half of osb_rollout_step (same arithmetic in every precision mode, O > 64 under 1 / 2
  * falls back to the fp32 tiles): obs / act / logp / value slabs, bootstrap values of paths truncated at t - 1 (from

@@ -18,7 +18,7 @@ from __future__ import annotations
 import torch
 
 from omnisafe_b200._lib import lib, ptr
-from omnisafe_b200.adapter.external_adapter import ExternalEnvAdapter
+from omnisafe_b200.adapter.external_adapter import ExternalEnvAdapter, device_rows
 from omnisafe_b200.adapter.onpolicy_adapter import OnPolicyAdapter
 from omnisafe_b200.utils.train_state import restore, snapshot
 
@@ -95,7 +95,7 @@ class ExternalEarlyTerminatedAdapter(_CostLimit, ExternalEnvAdapter):
             if not int(self._trig_host[0]):
                 return
             obs, _ = self._env.reset()
-        obs = self._rows(obs, O)
+        obs = device_rows(obs, N, self._device, O)
         self._rst_ptr = obs.untyped_storage().data_ptr()
         nz = self._obs_normalizer
         L.osb_ext_reset_rows(O, N, t, int(self._obs_normalize), ptr(self._trig), ptr(obs), ptr(self.s_raw), ptr(nz.mean),

@@ -33,6 +33,29 @@ from omnisafe_b200.envs.core import check_env, make
 from omnisafe_b200.utils.train_state import restore, snapshot
 
 
+def device_rows(x, n: int, device, width: int | None = None, dtype=torch.float32) -> torch.Tensor:
+    """x as n contiguous rows (of width columns) of dtype on device."""
+    shape = (n,) if width is None else (n, width)
+    return torch.as_tensor(x).to(device=device, dtype=dtype).reshape(shape).contiguous()
+
+
+def step_rows(env, action, n: int, width: int, device, capture: bool = False) -> tuple:
+    """env.step(action) as contiguous device rows for the observe launches: (next obs, reward, cost, terminated,
+    truncated, final obs, final mask), the last two None when the step reports no final observation."""
+    nobs, rew, cost, term, trunc, info = env.step(action)
+    nobs, rew, cost = device_rows(nobs, n, device, width), device_rows(rew, n, device), device_rows(cost, n, device)
+    term, trunc = device_rows(term, n, device, dtype=torch.uint8), device_rows(trunc, n, device, dtype=torch.uint8)
+    if capture and ('final_observation' not in info or '_final_observation' not in info):
+        raise OsbError(f'{type(env).__name__} is graph_safe but its step info lacks final_observation / '
+                       '_final_observation: a captured step must report them on every step')
+    final = mask = None
+    if 'final_observation' in info:
+        final = device_rows(info['final_observation'], n, device, width)
+        mask = info.get('_final_observation')
+        mask = (term | trunc) if mask is None else device_rows(mask, n, device, dtype=torch.uint8)
+    return nobs, rew, cost, term, trunc, final, mask
+
+
 class ExternalEnvAdapter:
     def __init__(self, env_id: str, num_envs: int, seed: int, cfgs, device='cuda',
                  env_id_offset: int = 0) -> None:
@@ -108,12 +131,6 @@ class ExternalEnvAdapter:
             saved['cost_normalizer'] = self._cost_normalizer
         return saved
 
-    # ---- env output -> contiguous device tensors ---------------------------------------------------
-    def _rows(self, x, width: int | None = None, dtype=torch.float32) -> torch.Tensor:
-        x = torch.as_tensor(x)
-        shape = (self._num_envs,) if width is None else (self._num_envs, width)
-        return x.to(device=self._device, dtype=dtype).reshape(shape).contiguous()
-
     def _norm_ptrs(self) -> list:
         n = self._obs_normalizer
         return [ptr(n.mean), ptr(n.sumsq), ptr(n.std), ptr(n.mean1), ptr(n.std1), ptr(n.count), ptr(n.had_fin),
@@ -146,20 +163,8 @@ class ExternalEnvAdapter:
             action = self.act_env.to(env_dev, copy=True)
             if N == 1:
                 action = action[0]                  # a single env takes an unbatched action (reference Unsqueeze)
-            nobs, rew, cost, term, trunc, info = self._env.step(action)
-            nobs = self._rows(nobs, O)
-            rew, cost = self._rows(rew), self._rows(cost)
-            term, trunc = self._rows(term, dtype=torch.uint8), self._rows(trunc, dtype=torch.uint8)
-            final = mask = None
-            if capture and ('final_observation' not in info or '_final_observation' not in info):
-                raise OsbError(f'{type(self._env).__name__} is graph_safe but its step info lacks final_observation / '
-                               '_final_observation: a captured step must report them on every step')
-            if 'final_observation' in info:
-                final = self._rows(info['final_observation'], O)
-                mask = info.get('_final_observation')
-                mask = (term | trunc) if mask is None else self._rows(mask, dtype=torch.uint8)
-            self._observe(T, t, d, (ptr(nobs), ptr(rew), ptr(cost), ptr(term), ptr(trunc), ptr(final), ptr(mask)), s,
-                          env_dev)
+            rows = step_rows(self._env, action, N, O, self._device, capture)
+            self._observe(T, t, d, tuple(ptr(r) for r in rows), s, env_dev)
         self._act(agent, d, T, T, None, s, epoch_dev)
 
     def _observe(self, T: int, t: int, d, step_ptrs: tuple, s: int, env_dev) -> None:
@@ -214,7 +219,7 @@ class ExternalEnvAdapter:
         if replay:
             obs = self._obs0.copy_(torch.as_tensor(reset_obs).reshape(N, O))
         else:
-            obs = self._rows(obs, O)
+            obs = device_rows(obs, N, self._device, O)
         L.osb_ext_reset_ingest(O, N, int(self._obs_normalize), ptr(obs), ptr(self.s_raw), ptr(self.ep_ret),
                                ptr(self.ep_cost), ptr(self.ep_len), *self._norm_ptrs(), ptr(self._ws),
                                ptr(self.nonfinite), s)

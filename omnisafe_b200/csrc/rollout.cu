@@ -1251,8 +1251,9 @@ static size_t rollout_tc_smem_bytes(bool x3) {
 // and ObsNormalize (wrapper.py:L231-241: final rows first -> mean1 / std1, then all rows).
 //
 // The observations of a user env have no bound, so the fixed-point sums of the synthetic path do not apply: each tile
-// writes fp64 (mean, M2) per column for all rows and for the final rows, and the last CTA (ticket) combines them in tile
-// order (Chan et al.) -- no floating-point atomics, the same result on every run.
+// writes fp64 (mean, M2) per column of its rows, and the last CTA (ticket) combines them in tile order (Chan et al.) --
+// no floating-point atomics, the same result on every run.  ext_tile_moments and ext_fold_push below are that push for
+// the training observe, the evaluation observe and the reset rows alike.
 constexpr int XT = 32;
 
 struct ExtObs {
@@ -1263,7 +1264,7 @@ struct ExtObs {
     const uint8_t* trunc;       // [N]
     const float* final_obs;     // [N][O] or null
     const uint8_t* final_mask;  // [N] rows of final_obs that hold a final observation, or null
-    double* part;               // [tiles][4][O] (mean, M2) of all rows and of the final rows, then [tiles] final-row counts
+    double* part;               // the push's workspace (ext_tile_moments)
     int* nonfinite;             // [1] set to 1 when an observation is not finite
 };
 
@@ -1274,6 +1275,102 @@ __device__ __forceinline__ void chan_combine(double& n, double& m, double& q, do
     m += d * nk / nn;
     q += qk + d * d * n * nk / nn;
     n = nn;
+}
+
+// The tile half of the fp64 ObsNormalize push, for the CTA's tile of rows envs from env0.  Per column, two passes over
+// the rows (ascending) give (mean, M2) of set A -- rows r of a with inA[r], every row when ALL -- and of set B -- rows r
+// of b with inB[r], none without FIN; a mean over no rows is 0.  part: [tiles][4][O] (A mean, A M2, B mean, B M2), then
+// [tiles][2] (A rows, B rows).  moments = false writes the row counts only.  Returns whether this CTA is the last on
+// the ticket.
+template <bool ALL, bool FIN>
+__device__ __forceinline__ bool ext_tile_moments(double* part, const float* a, const int* inA, const float* b,
+                                                 const int* inB, int O, int env0, int rows, bool moments,
+                                                 unsigned int* ticket) {
+    const int tid = threadIdx.x, tile = blockIdx.x, ntiles = gridDim.x;
+    int na = ALL ? rows : 0, nb = 0;
+    for (int r = 0; r < rows; ++r) {
+        if constexpr (!ALL) na += inA[r];
+        if constexpr (FIN) nb += inB[r];
+    }
+    double* P = part + (size_t)tile * 4 * O;
+    for (int j = tid; moments && j < O; j += NTHREADS) {
+        double s = 0.0, sf = 0.0;
+        for (int r = 0; r < rows; ++r) {
+            const size_t g = (size_t)(env0 + r) * O + j;
+            if (ALL || inA[r]) s += (double)a[g];
+            if (FIN && inB[r]) sf += (double)b[g];
+        }
+        const double m = na ? s / na : 0.0, mf = nb ? sf / nb : 0.0;
+        double q = 0.0, qf = 0.0;
+        for (int r = 0; r < rows; ++r) {
+            const size_t g = (size_t)(env0 + r) * O + j;
+            if (ALL || inA[r]) { const double d = (double)a[g] - m; q += d * d; }
+            if (FIN && inB[r]) { const double df = (double)b[g] - mf; qf += df * df; }
+        }
+        P[j] = m; P[O + j] = q; P[2 * O + j] = mf; P[3 * O + j] = qf;
+    }
+    double* cnt = part + (size_t)ntiles * 4 * O;
+    if (tid == 0) { cnt[2 * tile] = (double)na; cnt[2 * tile + 1] = (double)nb; }
+    return last_cta(ticket);
+}
+
+// The last CTA's half: combine the tiles in tile order and push set B, then set A, into ns (norm_fold's sequence); a
+// set with no rows is not pushed, and with no row in either the statistics are untouched.  Then count[0] and the
+// ticket.  ALL (the training observe): set A is all N envs, its tile counts follow from N, and the set-B push is also
+// kept as mean1 / std1 with count[1] and had_fin, for the truncation bootstraps of the next act launch.
+template <bool ALL, bool FIN>
+__device__ __forceinline__ void ext_fold_push(const double* part, NormState ns, int O, int N, bool moments) {
+    __shared__ int s_na, s_nb;
+    const int tid = threadIdx.x, ntiles = gridDim.x;
+    __threadfence();
+    const double* cnt = part + (size_t)ntiles * 4 * O;
+    if (tid == 0) {
+        int a = 0, b = 0;
+        for (int k = 0; k < ntiles; ++k) {
+            if constexpr (!ALL) a += (int)__ldcg(cnt + 2 * k);
+            if constexpr (FIN) b += (int)__ldcg(cnt + 2 * k + 1);
+        }
+        s_na = a; s_nb = b;
+    }
+    __syncthreads();
+    const int na = ALL ? N : s_na, nb = FIN ? s_nb : 0;
+    const long long count = __ldcg(ns.count);
+    for (int j = tid; moments && (na > 0 || nb > 0) && j < O; j += NTHREADS) {
+        double n = 0.0, m = 0.0, q = 0.0, nF = 0.0, mF = 0.0, qF = 0.0;
+        for (int k = 0; k < ntiles; ++k) {
+            const double* Pk = part + (size_t)k * 4 * O;
+            chan_combine(n, m, q, ALL ? (double)min(XT, N - k * XT) : __ldcg(cnt + 2 * k), __ldcg(Pk + j),
+                         __ldcg(Pk + O + j));
+            if constexpr (FIN)
+                chan_combine(nF, mF, qF, __ldcg(cnt + 2 * k + 1), __ldcg(Pk + 2 * O + j), __ldcg(Pk + 3 * O + j));
+        }
+        float mean = __ldcg(ns.mean + j), sumsq = __ldcg(ns.sumsq + j);
+        long long c = count;
+        if (nb > 0) {
+            norm_push_moments(mean, sumsq, c, nb, mF, qF);
+            c += nb;
+            if constexpr (ALL) {
+                ns.mean1[j] = mean;
+                ns.std1[j] = norm_std(sumsq, c);
+            }
+        }
+        if (na > 0) {
+            norm_push_moments(mean, sumsq, c, na, m, q);
+            c += na;
+        }
+        ns.mean[j] = mean;
+        ns.sumsq[j] = sumsq;
+        ns.std[j] = norm_std(sumsq, c);
+    }
+    __syncthreads();
+    if (tid == 0) {
+        if constexpr (ALL) {
+            ns.count[1] = count + nb;
+            *ns.had_fin = nb > 0 ? 1 : 0;
+        }
+        ns.count[0] = count + nb + na;
+        *ns.ticket = 0u;
+    }
 }
 
 // EARLY: EarlyTerminatedAdapter.step on top of the step (early_terminated_adapter.py:L77-87), one thread per env.  The
@@ -1288,9 +1385,8 @@ __device__ __forceinline__ void ext_observe_step(ExtObs x, EnvState st, NormStat
                                                  int obs_normalize, int is_reset, EarlySpec et, uint8_t* trig,
                                                  int* trig_total) {
     __shared__ int sFin[XT];
-    __shared__ int s_bad, s_nfin;
-    const int tid = threadIdx.x, tile = blockIdx.x, ntiles = gridDim.x;
-    const int env0 = tile * XT, rows = min(XT, N - env0);
+    __shared__ int s_bad;
+    const int tid = threadIdx.x, env0 = blockIdx.x * XT, rows = min(XT, N - env0);
     if (tid == 0) s_bad = 0;
     if (tid < XT) {
         const int env = env0 + tid;
@@ -1340,72 +1436,11 @@ __device__ __forceinline__ void ext_observe_step(ExtObs x, EnvState st, NormStat
         if (tid == 0 && s_bad) *x.nonfinite = 1;
         return;
     }
-
-    // per-tile moments (two passes over the tile's rows, fp64)
-    int nf = 0;
-    for (int r = 0; r < rows; ++r) nf += sFin[r];
-    double* P = x.part + (size_t)tile * 4 * O;
-    for (int j = tid; j < O; j += NTHREADS) {
-        double s = 0.0, sf = 0.0;
-        for (int r = 0; r < rows; ++r) {
-            const size_t g = (size_t)(env0 + r) * O + j;
-            s += (double)x.next_obs[g];
-            if (sFin[r]) sf += (double)x.final_obs[g];
-        }
-        const double m = s / rows, mf = nf ? sf / nf : 0.0;
-        double q = 0.0, qf = 0.0;
-        for (int r = 0; r < rows; ++r) {
-            const size_t g = (size_t)(env0 + r) * O + j;
-            const double d = (double)x.next_obs[g] - m;
-            q += d * d;
-            if (sFin[r]) { const double df = (double)x.final_obs[g] - mf; qf += df * df; }
-        }
-        P[j] = m; P[O + j] = q; P[2 * O + j] = mf; P[3 * O + j] = qf;
-    }
-    if (tid == 0) x.part[(size_t)ntiles * 4 * O + tile] = (double)nf;
-    const bool last = last_cta(ns.ticket);
+    // set A: every next row; set B: the final rows
+    const bool last = ext_tile_moments<true, true>(x.part, x.next_obs, nullptr, x.final_obs, sFin, O, env0, rows, true,
+                                                   ns.ticket);
     if (tid == 0 && s_bad) *x.nonfinite = 1;
-    if (!last) return;
-
-    // last CTA: combine the tiles in order and push final rows, then all rows (norm_fold's sequence)
-    __threadfence();
-    const double* cnt = x.part + (size_t)ntiles * 4 * O;
-    if (tid == 0) {
-        int total = 0;
-        for (int k = 0; k < ntiles; ++k) total += (int)__ldcg(cnt + k);
-        s_nfin = total;
-    }
-    __syncthreads();
-    const int nfin = s_nfin;
-    const long long count = __ldcg(ns.count);
-    for (int j = tid; j < O; j += NTHREADS) {
-        double n = 0.0, m = 0.0, q = 0.0, nF = 0.0, mF = 0.0, qF = 0.0;
-        for (int k = 0; k < ntiles; ++k) {
-            const double* Pk = x.part + (size_t)k * 4 * O;
-            chan_combine(n, m, q, (double)min(XT, N - k * XT), __ldcg(Pk + j), __ldcg(Pk + O + j));
-            chan_combine(nF, mF, qF, __ldcg(cnt + k), __ldcg(Pk + 2 * O + j), __ldcg(Pk + 3 * O + j));
-        }
-        float mean = __ldcg(ns.mean + j), sumsq = __ldcg(ns.sumsq + j);
-        long long c = count;
-        if (nfin > 0) {
-            norm_push_moments(mean, sumsq, c, nfin, mF, qF);
-            c += nfin;
-            ns.mean1[j] = mean;
-            ns.std1[j] = norm_std(sumsq, c);
-        }
-        norm_push_moments(mean, sumsq, c, N, m, q);
-        c += N;
-        ns.mean[j] = mean;
-        ns.sumsq[j] = sumsq;
-        ns.std[j] = norm_std(sumsq, c);
-    }
-    __syncthreads();
-    if (tid == 0) {
-        ns.count[1] = count + nfin;
-        ns.count[0] = count + nfin + N;
-        *ns.had_fin = nfin > 0 ? 1 : 0;
-        *ns.ticket = 0u;
-    }
+    if (last) ext_fold_push<true, true>(x.part, ns, O, N, true);
 }
 
 __global__ void __launch_bounds__(NTHREADS) ext_observe_kernel(ExtObs x, EnvState st, NormState ns, Slabs sl, int O, int N,
@@ -1421,17 +1456,16 @@ __global__ void __launch_bounds__(NTHREADS) ext_observe_early_kernel(ExtObs x, E
 
 // The reset observations of the envs the cost rule cut at step t (rows of obs where mask is set; the others are ignored)
 // into the state buffer step t + 1 reads, and their ObsNormalize push (ObsNormalize.reset, wrapper.py:L243-261) after the
-// step's own pushes: fp64 per-tile moments of the masked rows combined in tile order by the last CTA, with per-tile row
-// counts, so the row count stays on the device.  No masked row: the statistics are untouched.  mean1 / std1 / had_fin
-// keep the values of the step's final-row push, which the next act launch's truncation bootstraps read.
+// step's own pushes, the masked rows as set A of the fp64 push, so the row count stays on the device.  No masked row:
+// the statistics are untouched.  mean1 / std1 / had_fin keep the values of the step's final-row push, which the next
+// act launch's truncation bootstraps read.
 __global__ void __launch_bounds__(NTHREADS, 1) ext_reset_rows_kernel(const float* __restrict__ obs,
                                                                   const uint8_t* __restrict__ mask, float* s_nxt,
                                                                   NormState ns, double* part, int* nonfinite, int O,
                                                                   int N, int obs_normalize) {
     __shared__ int sM[XT];
-    __shared__ int s_bad, s_n;
-    const int tid = threadIdx.x, tile = blockIdx.x, ntiles = gridDim.x;
-    const int env0 = tile * XT, rows = min(XT, N - env0);
+    __shared__ int s_bad;
+    const int tid = threadIdx.x, env0 = blockIdx.x * XT, rows = min(XT, N - env0);
     if (tid == 0) s_bad = 0;
     if (tid < XT) sM[tid] = (tid < rows && mask[env0 + tid] != 0) ? 1 : 0;
     __syncthreads();
@@ -1450,53 +1484,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) ext_reset_rows_kernel(const float
         if (tid == 0 && s_bad) *nonfinite = 1;
         return;
     }
-    int nr = 0;
-    for (int r = 0; r < rows; ++r) nr += sM[r];
-    double* P = part + (size_t)tile * 2 * O;
-    for (int j = tid; j < O; j += NTHREADS) {
-        double s = 0.0;
-        for (int r = 0; r < rows; ++r)
-            if (sM[r]) s += (double)obs[(size_t)(env0 + r) * O + j];
-        const double m = nr ? s / nr : 0.0;
-        double q = 0.0;
-        for (int r = 0; r < rows; ++r)
-            if (sM[r]) { const double d = (double)obs[(size_t)(env0 + r) * O + j] - m; q += d * d; }
-        P[j] = m; P[O + j] = q;
-    }
-    double* cnt = part + (size_t)ntiles * 2 * O;
-    if (tid == 0) cnt[tile] = (double)nr;
-    const bool last = last_cta(ns.ticket);
+    const bool last = ext_tile_moments<false, false>(part, obs, sM, nullptr, nullptr, O, env0, rows, true, ns.ticket);
     if (tid == 0 && s_bad) *nonfinite = 1;
-    if (!last) return;
-
-    __threadfence();
-    if (tid == 0) {
-        int total = 0;
-        for (int k = 0; k < ntiles; ++k) total += (int)__ldcg(cnt + k);
-        s_n = total;
-    }
-    __syncthreads();
-    const int n = s_n;
-    const long long count = __ldcg(ns.count);
-    if (n > 0) {
-        for (int j = tid; j < O; j += NTHREADS) {
-            double nn = 0.0, m = 0.0, q = 0.0;
-            for (int k = 0; k < ntiles; ++k) {
-                const double* Pk = part + (size_t)k * 2 * O;
-                chan_combine(nn, m, q, __ldcg(cnt + k), __ldcg(Pk + j), __ldcg(Pk + O + j));
-            }
-            float mean = __ldcg(ns.mean + j), sumsq = __ldcg(ns.sumsq + j);
-            norm_push_moments(mean, sumsq, count, n, m, q);
-            ns.mean[j] = mean;
-            ns.sumsq[j] = sumsq;
-            ns.std[j] = norm_std(sumsq, count + n);
-        }
-    }
-    __syncthreads();
-    if (tid == 0) {
-        ns.count[0] = count + n;
-        *ns.ticket = 0u;
-    }
+    if (last) ext_fold_push<false, false>(part, ns, O, N, true);
 }
 
 // Evaluation of a saved policy on a user env (Evaluator.evaluate with a registered env), the observe half of step t after
@@ -1504,8 +1494,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) ext_reset_rows_kernel(const float
 // still running (left > 0), one thread each: the fp64 episode sums, the EarlyTerminated rule, the Saute state, the
 // episode end and the results, as eval_step does for the synthetic env.  The next observations go to the state buffer
 // step t + 1 reads.  ObsNormalize pushes the final observations of the running envs that report one, then the next
-// observations of every running env (reset: the observations of every env with episodes left), as fp64 per-tile
-// moments combined in tile order by the last CTA (ext_observe_kernel's scheme), with per-tile row counts.  The last CTA
+// observations of every running env (reset: the observations of every env with episodes left), through the fp64 push
+// (ext_tile_moments / ext_fold_push).  The last CTA
 // also advances the done word ctr[0]; ctr[2] counts the envs to reset now (N == 1: every episode end with episodes left),
 // and a reset ingest clears it.  RST: rst[env] (one byte per env, written on every launch) is 1 where the cost rule ended
 // a running env's episode that the env itself did not end, and the env has episodes left: the envs the caller resets
@@ -1515,9 +1505,8 @@ __device__ __forceinline__ void ext_eval_observe_step(ExtObs x, EnvState st, Nor
                                                       int O, int N, int t, int obs_normalize, int is_reset,
                                                       uint8_t* rst_out) {
     __shared__ int sRun[XT], sFin[XT];
-    __shared__ int s_bad, s_nrun, s_nfin;
-    const int tid = threadIdx.x, tile = blockIdx.x, ntiles = gridDim.x;
-    const int env0 = tile * XT, rows = min(XT, N - env0);
+    __shared__ int s_bad;
+    const int tid = threadIdx.x, env0 = blockIdx.x * XT, rows = min(XT, N - env0);
     if (tid == 0) s_bad = 0;
     if (tid < XT) {
         const int env = env0 + tid;
@@ -1569,76 +1558,19 @@ __device__ __forceinline__ void ext_eval_observe_step(ExtObs x, EnvState st, Nor
         if (sFin[i / O]) bad |= !isfinite(x.final_obs[g]);
     }
     if (bad) s_bad = 1;
-    int nr = 0, nf = 0;
-    for (int r = 0; r < rows; ++r) { nr += sRun[r]; nf += sFin[r]; }
-    double* P = x.part + (size_t)tile * 4 * O;
-    if (obs_normalize) {
-        for (int j = tid; j < O; j += NTHREADS) {
-            double sm = 0.0, sf = 0.0;
-            for (int r = 0; r < rows; ++r) {
-                const size_t g = (size_t)(env0 + r) * O + j;
-                if (sRun[r]) sm += (double)x.next_obs[g];
-                if (sFin[r]) sf += (double)x.final_obs[g];
-            }
-            const double m = nr ? sm / nr : 0.0, mf = nf ? sf / nf : 0.0;
-            double q = 0.0, qf = 0.0;
-            for (int r = 0; r < rows; ++r) {
-                const size_t g = (size_t)(env0 + r) * O + j;
-                if (sRun[r]) { const double d = (double)x.next_obs[g] - m; q += d * d; }
-                if (sFin[r]) { const double df = (double)x.final_obs[g] - mf; qf += df * df; }
-            }
-            P[j] = m; P[O + j] = q; P[2 * O + j] = mf; P[3 * O + j] = qf;
-        }
-    }
-    double* cnt = x.part + (size_t)ntiles * 4 * O;
-    if (tid == 0) { cnt[2 * tile] = (double)nr; cnt[2 * tile + 1] = (double)nf; }
-    const bool last = last_cta(ns.ticket);
+    // set A: the running rows; set B: their final rows.  Without obs_normalize only the row counts go to count[0].
+    const bool last = ext_tile_moments<false, true>(x.part, x.next_obs, sRun, x.final_obs, sFin, O, env0, rows,
+                                                    obs_normalize, ns.ticket);
     if (tid == 0 && s_bad) *x.nonfinite = 1;
     if (!last) return;
-
-    // last CTA: combine the tiles in order, push the final rows, then the running rows
-    __threadfence();
+    ext_fold_push<false, true>(x.part, ns, O, N, obs_normalize);
     if (tid == 0) {
-        int a = 0, b = 0;
-        for (int k = 0; k < ntiles; ++k) { a += (int)__ldcg(cnt + 2 * k); b += (int)__ldcg(cnt + 2 * k + 1); }
-        s_nrun = a; s_nfin = b;
-    }
-    __syncthreads();
-    const int nrun = s_nrun, nfin = s_nfin;
-    const long long count = __ldcg(ns.count);
-    if (obs_normalize) {
-        for (int j = tid; j < O; j += NTHREADS) {
-            double n = 0.0, m = 0.0, q = 0.0, nF = 0.0, mF = 0.0, qF = 0.0;
-            for (int k = 0; k < ntiles; ++k) {
-                const double* Pk = x.part + (size_t)k * 4 * O;
-                chan_combine(n, m, q, __ldcg(cnt + 2 * k), __ldcg(Pk + j), __ldcg(Pk + O + j));
-                chan_combine(nF, mF, qF, __ldcg(cnt + 2 * k + 1), __ldcg(Pk + 2 * O + j), __ldcg(Pk + 3 * O + j));
-            }
-            float mean = __ldcg(ns.mean + j), sumsq = __ldcg(ns.sumsq + j);
-            long long c = count;
-            if (nfin > 0) {
-                norm_push_moments(mean, sumsq, c, nfin, mF, qF);
-                c += nfin;
-            }
-            if (nrun > 0) {
-                norm_push_moments(mean, sumsq, c, nrun, m, q);
-                c += nrun;
-            }
-            ns.mean[j] = mean;
-            ns.sumsq[j] = sumsq;
-            ns.std[j] = norm_std(sumsq, c);
-        }
-    }
-    __syncthreads();
-    if (tid == 0) {
-        ns.count[0] = count + nfin + nrun;
         if (is_reset) {
             ev.ctr[2] = 0;
         } else {
             ev.ctr[0] = __ldcg(ev.ctr + 1);
             ev.ctr[1] = 0;
         }
-        *ns.ticket = 0u;
     }
 }
 
@@ -2063,7 +1995,10 @@ int osb_eval_synthetic(int O, int A, int max_episode_steps, unsigned seed, unsig
     return OSB_OK;
 }
 
-int osb_eval_ext_workspace_doubles(int O, int N) { return ((N + XT - 1) / XT) * (4 * O + 2); }
+// the workspace of the fp64 ObsNormalize push (ext_tile_moments): the training and evaluation observe launches and the
+// reset rows of either take the same
+int osb_ext_workspace_doubles(int O, int N) { return ((N + XT - 1) / XT) * (4 * O + 2); }
+int osb_eval_ext_workspace_doubles(int O, int N) { return osb_ext_workspace_doubles(O, N); }
 
 int osb_eval_ext_act(int O, int A, int obs_normalize, int N, int t, const float* s_raw, const float* norm_mean,
                      const float* norm_std, const long long* norm_count, const float* safety, const float* theta,
@@ -2084,13 +2019,15 @@ int osb_eval_ext_act(int O, int A, int obs_normalize, int N, int t, const float*
     return launch_rollout<true, true>(p, (cudaStream_t)stream);
 }
 
-int osb_eval_ext_observe(int O, int N, int t, int obs_normalize, int is_reset, const float* next_obs, const float* rew,
-                         const float* cost, const unsigned char* terminated, const unsigned char* truncated,
-                         const float* final_obs, const unsigned char* final_mask, float* s_raw, float* norm_mean,
-                         float* norm_sumsq, float* norm_std, long long* norm_count, unsigned* ticket, float* safety,
-                         float safety_budget, float saute_gamma, int early, double cost_limit, double cost_criteria,
-                         int* left, int* done_eps, double* ret, double* cost_acc, int* len, int* ctr, double* out_ret,
-                         double* out_cost, int* out_len, double* workspace, int* nonfinite, void* stream) {
+// osb_eval_ext_observe, and with rst osb_eval_ext_observe_rst
+static int eval_ext_observe(int O, int N, int t, int obs_normalize, int is_reset, const float* next_obs, const float* rew,
+                            const float* cost, const unsigned char* terminated, const unsigned char* truncated,
+                            const float* final_obs, const unsigned char* final_mask, float* s_raw, float* norm_mean,
+                            float* norm_sumsq, float* norm_std, long long* norm_count, unsigned* ticket, float* safety,
+                            float safety_budget, float saute_gamma, int early, double cost_limit, double cost_criteria,
+                            int* left, int* done_eps, double* ret, double* cost_acc, int* len, int* ctr,
+                            double* out_ret, double* out_cost, int* out_len, double* workspace, int* nonfinite,
+                            unsigned char* rst, void* stream) {
     OSB_CHECK_ARG(O > 0 && N > 0 && t >= -1, "bad dims / step index");
     OSB_CHECK_ARG(next_obs && s_raw && norm_mean && norm_sumsq && norm_std && norm_count && ticket && left && ctr &&
                   workspace && nonfinite, "bad argument");
@@ -2103,10 +2040,28 @@ int osb_eval_ext_observe(int O, int N, int t, int obs_normalize, int is_reset, c
     SauteSpec sa{safety, safety ? safety_budget : 1.f, safety ? saute_gamma : 1.f, 0.f, 1.f};
     EvalSpec ev{left, done_eps, ret, cost_acc, len, out_ret, out_cost, out_len, nullptr, ctr, cost_criteria, cost_limit,
                 early, N == 1 ? 1 : 0, nullptr};
-    ext_eval_observe_kernel<<<(N + XT - 1) / XT, NTHREADS, 0, (cudaStream_t)stream>>>(x, st, ns, sa, ev, O, N, t,
-                                                                                     obs_normalize, is_reset);
+    const int grid = (N + XT - 1) / XT;
+    if (rst)
+        ext_eval_observe_rst_kernel<<<grid, NTHREADS, 0, (cudaStream_t)stream>>>(x, st, ns, sa, ev, O, N, t,
+                                                                                 obs_normalize, rst);
+    else
+        ext_eval_observe_kernel<<<grid, NTHREADS, 0, (cudaStream_t)stream>>>(x, st, ns, sa, ev, O, N, t, obs_normalize,
+                                                                             is_reset);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
+}
+
+int osb_eval_ext_observe(int O, int N, int t, int obs_normalize, int is_reset, const float* next_obs, const float* rew,
+                         const float* cost, const unsigned char* terminated, const unsigned char* truncated,
+                         const float* final_obs, const unsigned char* final_mask, float* s_raw, float* norm_mean,
+                         float* norm_sumsq, float* norm_std, long long* norm_count, unsigned* ticket, float* safety,
+                         float safety_budget, float saute_gamma, int early, double cost_limit, double cost_criteria,
+                         int* left, int* done_eps, double* ret, double* cost_acc, int* len, int* ctr, double* out_ret,
+                         double* out_cost, int* out_len, double* workspace, int* nonfinite, void* stream) {
+    return eval_ext_observe(O, N, t, obs_normalize, is_reset, next_obs, rew, cost, terminated, truncated, final_obs,
+                            final_mask, s_raw, norm_mean, norm_sumsq, norm_std, norm_count, ticket, safety,
+                            safety_budget, saute_gamma, early, cost_limit, cost_criteria, left, done_eps, ret, cost_acc,
+                            len, ctr, out_ret, out_cost, out_len, workspace, nonfinite, nullptr, stream);
 }
 
 // osb_eval_ext_observe of a step (no reset ingest) that also writes rst[N], the envs the cost rule cut with episodes left
@@ -2118,26 +2073,15 @@ int osb_eval_ext_observe_rst(int O, int N, int t, int obs_normalize, const float
                              double cost_criteria, int* left, int* done_eps, double* ret, double* cost_acc, int* len,
                              int* ctr, double* out_ret, double* out_cost, int* out_len, double* workspace,
                              int* nonfinite, unsigned char* rst, void* stream) {
-    OSB_CHECK_ARG(O > 0 && N > 0 && t >= 0, "bad dims / step index");
-    OSB_CHECK_ARG(next_obs && rew && cost && terminated && truncated && s_raw && norm_mean && norm_sumsq && norm_std &&
-                  norm_count && ticket && left && done_eps && ret && cost_acc && len && ctr && out_ret && out_cost &&
-                  out_len && workspace && nonfinite && rst, "bad argument");
-    OSB_CHECK_ARG(safety == nullptr || (safety_budget > 0.f && saute_gamma > 0.f), "safety_budget and saute_gamma must be positive");
-    ExtObs x{next_obs, rew, cost, terminated, truncated, final_obs, final_mask, workspace, nonfinite};
-    EnvState st{s_raw, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    NormState ns{norm_mean, norm_sumsq, norm_std, nullptr, nullptr, norm_count, nullptr, nullptr, nullptr, nullptr, ticket};
-    SauteSpec sa{safety, safety ? safety_budget : 1.f, safety ? saute_gamma : 1.f, 0.f, 1.f};
-    EvalSpec ev{left, done_eps, ret, cost_acc, len, out_ret, out_cost, out_len, nullptr, ctr, cost_criteria, cost_limit,
-                early, N == 1 ? 1 : 0, nullptr};
-    ext_eval_observe_rst_kernel<<<(N + XT - 1) / XT, NTHREADS, 0, (cudaStream_t)stream>>>(x, st, ns, sa, ev, O, N, t,
-                                                                                         obs_normalize, rst);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    OSB_CHECK_ARG(t >= 0, "bad dims / step index");
+    OSB_CHECK_ARG(rst, "bad argument");
+    return eval_ext_observe(O, N, t, obs_normalize, 0, next_obs, rew, cost, terminated, truncated, final_obs,
+                            final_mask, s_raw, norm_mean, norm_sumsq, norm_std, norm_count, ticket, safety,
+                            safety_budget, saute_gamma, early, cost_limit, cost_criteria, left, done_eps, ret, cost_acc,
+                            len, ctr, out_ret, out_cost, out_len, workspace, nonfinite, rst, stream);
 }
 
 // ---- external envs ---------------------------------------------------------------------------
-int osb_ext_workspace_doubles(int O, int N) { return ((N + XT - 1) / XT) * (4 * O + 1); }
-
 static int launch_observe(const ExtObs& x, EnvState st, NormState ns, Slabs sl, int O, int N, int T, int t,
                           int obs_normalize, int is_reset, void* stream) {
     ext_observe_kernel<<<(N + XT - 1) / XT, NTHREADS, 0, (cudaStream_t)stream>>>(x, st, ns, sl, O, N, T, t, obs_normalize,

@@ -35,6 +35,7 @@ import numpy as np
 import torch
 
 from omnisafe_b200._lib import OsbError, current_stream, lib, ptr
+from omnisafe_b200.adapter.external_adapter import device_rows, step_rows
 from omnisafe_b200.adapter.saute_adapter import per_step_budget
 from omnisafe_b200.common.normalizer import Normalizer
 from omnisafe_b200.envs.core import check_env, is_registered, make
@@ -178,8 +179,6 @@ class Evaluator:
         cut = self._early and E > 1         # envs the cost rule cuts are reset through env.reset_envs(rst)
         rst = torch.zeros(E, dtype=torch.bool, device=dev) if cut else None
         graph = E > 1 and bool(getattr(env, 'graph_safe', False)) and not os.getenv('OSB_NO_GRAPH')
-        rows = lambda x, width=None, dtype=torch.float32: torch.as_tensor(x).to(            # noqa: E731
-            device=dev, dtype=dtype).reshape((E,) if width is None else (E, width)).contiguous()
         on = int(self._obs_normalize)
         tail = (ptr(s_raw), ptr(norm.mean), ptr(norm.sumsq), ptr(norm.std), ptr(norm.count), ptr(norm.ticket),
                 ptr(w['safety']), self._budget, self._saute_gamma, int(self._early), self._cost_limit, crit,
@@ -188,7 +187,8 @@ class Evaluator:
 
         def ingest(t):
             obs = env.reset()[0]
-            L.osb_eval_ext_observe(O, E, t, on, 1, ptr(rows(obs, O)), 0, 0, 0, 0, 0, 0, *tail, current_stream())
+            L.osb_eval_ext_observe(O, E, t, on, 1, ptr(device_rows(obs, E, dev, O)), 0, 0, 0, 0, 0, 0, *tail,
+                                   current_stream())
             return torch.as_tensor(obs).device
 
         def step(t, capture=False):
@@ -197,23 +197,13 @@ class Evaluator:
                                ptr(w['safety']), ptr(self._theta), ptr(act_lo), ptr(act_hi), ptr(act_env), ptr(w['left']),
                                ptr(w['ctr']), ptr(w['act_out']), self._precision, s)
             action = act_env.clone()
-            nobs, rew, cost, term, trunc, info = env.step(action[0] if E == 1 else action)
-            nobs, rew, cost = rows(nobs, O), rows(rew), rows(cost)
-            term, trunc = rows(term, dtype=torch.uint8), rows(trunc, dtype=torch.uint8)
-            if capture and ('final_observation' not in info or '_final_observation' not in info):
-                raise OsbError(f'{type(env).__name__} is graph_safe but its step info lacks final_observation / '
-                               '_final_observation: a captured step must report them on every step')
-            final = mask = None
-            if 'final_observation' in info:
-                final = rows(info['final_observation'], O)
-                mask = info.get('_final_observation')
-                mask = (term | trunc) if mask is None else rows(mask, dtype=torch.uint8)
-            step_ptrs = (ptr(nobs), ptr(rew), ptr(cost), ptr(term), ptr(trunc), ptr(final), ptr(mask))
+            rows = step_rows(env, action[0] if E == 1 else action, E, O, dev, capture)
+            step_ptrs = tuple(ptr(r) for r in rows)
             if not cut:
                 L.osb_eval_ext_observe(O, E, t, on, 0, *step_ptrs, *tail, s)
                 return
             L.osb_eval_ext_observe_rst(O, E, t, on, *step_ptrs, *tail, ptr(rst), s)
-            obs = rows(env.reset_envs(rst.to(env_dev)), O)
+            obs = device_rows(env.reset_envs(rst.to(env_dev)), E, dev, O)
             L.osb_ext_reset_rows(O, E, t, on, ptr(rst), ptr(obs), ptr(s_raw), ptr(norm.mean), ptr(norm.sumsq),
                                  ptr(norm.std), ptr(norm.count), ptr(norm.ticket), ptr(ws), ptr(nonfinite), s)
 
