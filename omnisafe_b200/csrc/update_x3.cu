@@ -422,18 +422,32 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
         };
         int step_t0 = 0;
         if (FUSED) step_t0 = p.adam_step[net];
+        const int S = (L.size + G - 1) / G;                        // FUSED: parameters owned by this CTA: [p0, p0 + S)
+        const int p0 = (int)blockIdx.x * S;
+        const bool own = tid < S && p0 + tid < L.size;             // FUSED: this thread owns parameter p0 + tid
         // FUSED: where this thread's parameter (the first of its slice chunk) lives inside the weight-tile image, or -1
         // (log_std, b2, b3, and b1 when it is not folded into W1): byte offset of the hi piece, stride between pieces
         int img_off = -1; uint32_t img_sub = 0;
         if (FUSED) {
-            const int Sx = (L.size + G - 1) / G, px = (int)blockIdx.x * Sx + tid;
-            if (tid < Sx && px < L.size) {
+            const int px = p0 + tid;
+            if (own) {
                 if (px >= L.off_w1 && px < L.off_b1) { const int e = px - L.off_w1; img_off = (int)off128(e / O, e % O); img_sub = W_SUB; }
                 else if (px >= L.off_b1 && px < L.off_w2) { if (ones_col) { img_off = (int)off128(px - L.off_b1, 63); img_sub = W_SUB; } }
                 else if (px >= L.off_w2 && px < L.off_b2) { const int e = px - L.off_w2; img_off = (int)(W_X3 + off128(e >> 6, e & 63)); img_sub = W_SUB; }
                 else if (px >= L.off_w3 && px < L.off_b3) { const int e = px - L.off_w3; img_off = (int)(2 * W_X3 + off128(e >> 6, e & 63)); img_sub = W3_SUB; }
             }
         }
+        // FUSED: where a CTA's partial gradient of parameter px sits in its accumulator image (float offset; row m of an M = 64
+        // product is lane 32 (m / 16) + m % 16), or -1: W1 [n][k] and W2 [n][k] lie along the image's columns, so a warp
+        // reading 32 consecutive parameters touches one or two lines; b1, b2 and W3^T lie along its rows (1280 B apart, a
+        // line per parameter), so their partials, with b3 and log_std, go to the CTA's row of gpart
+        auto grad_src = [&](int px) -> int {
+            int row, col;
+            if (px >= L.off_w1 && px < L.off_b1) { const int e = px - L.off_w1; row = e / O; col = (int)T_DW1 + e % O; }
+            else if (px >= L.off_w2 && px < L.off_b2) { const int e = px - L.off_w2; row = e >> 6; col = (int)T_DW2 + (e & 63); }
+            else return -1;
+            return (32 * (row >> 4) + (row & 15)) * (int)T_COLS + col;
+        };
         uint8_t* wimg = FUSED ? p.wimg + (size_t)net * W_IMG : nullptr;
         // per-thread partial sums over the tiles of one minibatch (reduced once per minibatch): the statistics of the warps
         // with h == 0, and every warp's gradients of its own actions a = NA h + j in slot j
@@ -679,7 +693,12 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     prefetch_x(sRowBuf + rpar * XT);
                 }
             }
-            // ---- this CTA's partial gradient of the minibatch: accumulator images -> global ------------------------
+            // FUSED: the owner's Adam state does not depend on the gradient (only this thread writes it), so its loads fly
+            // under the wait for the last gradient product and the first grid barrier
+            float pre_th = 0.f, pre_m = 0.f, pre_v = 0.f;
+            if (FUSED && own) { pre_th = __ldcg(p.theta_rw + noff + p0 + tid); pre_m = __ldcg(p.adam_m + noff + p0 + tid); pre_v = __ldcg(p.adam_v + noff + p0 + tid); }
+            // ---- this CTA's partial gradient of the minibatch: stepwise, accumulator images -> gpart; FUSED, the slice
+            //      reduction reads dW1 / dW2 in the images themselves and gpart holds b1, b2, W3, b3 and log_std -------
             if (have_tiles) {
                 // statistics: lanes -> warp (butterfly) -> the four warps with h == 0 (fixed order)
                 if (h == 0) {
@@ -709,35 +728,41 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     }
                     break;
                 }
+                epi_bar_sync();                        // sRed of the sixteen epilogue warps
+                if (tid < L.out) __stcg(gout + L.off_b3 + tid, (sRed[96 + tid] + sRed[112 + tid]) + (sRed[128 + tid] + sRed[144 + tid]));
+                if (net == 0 && tid >= 32 && tid < 32 + A) {
+                    const int a = tid - 32;
+                    float g = (sRed[32 + a] + sRed[48 + a]) + (sRed[64 + a] + sRed[80 + a]);
+                    if (blockIdx.x == 0 && loss_has_entropy<!FUSED>(p.lc.kind)) g -= p.lc.entropy_coef / (float)A;
+                    if (p.lc.kind == LOSS_FVP) g = (blockIdx.x == 0) ? 2.f / (float)A * __ldg(p.fvp_vec + L.off_logstd + a) : 0.f;
+                    __stcg(gout + L.off_logstd + a, g);
+                }
+                if (tid >= 64 && tid < 72) {
+                    const int i = tid - 64;
+                    __stcg(p.stats_part + ((size_t)blockIdx.x * 3 + net) * 8 + i, (i < 5) ? (sRed[i] + sRed[8 + i]) + (sRed[16 + i] + sRed[24 + i]) : 0.f);
+                }
                 mbar_wait_a(bar(DONE_C6), (uint32_t)((it - 1) & 1));
                 stamp(21);
                 const int t_row = 16 * q + lane;       // row (lane < 16) of the M = 64 accumulators
                 const int c16 = 16 * h;
                 float v[16];
-                acc_ld16(tm, lane_base + T_DW2 + (uint32_t)c16, v);
-                if (lane < 16) {
-                    float* dst = gout + L.off_w2 + t_row * 64 + c16;
-                    if (FUSED && (L.off_w2 & 3) == 0) {
-#pragma unroll
-                        for (int i = 0; i < 16; i += 4) __stcg(reinterpret_cast<float4*>(dst + i), make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]));
-                    } else {
+                if (FUSED) {                           // db1 = column 63 of dW1 (the slice reduction reads W1, W2 in the images)
+                    if (ones_col && h == 3 && lane < 16) __stcg(gout + L.off_b1 + t_row, __ldcg(tm.p + (size_t)(32 * q + lane) * T_COLS + T_DW1 + 63));
+                } else {
+                    acc_ld16(tm, lane_base + T_DW2 + (uint32_t)c16, v);
+                    if (lane < 16) {
+                        float* dst = gout + L.off_w2 + t_row * 64 + c16;
 #pragma unroll
                         for (int i = 0; i < 16; ++i) __stcg(dst + i, v[i]);
                     }
-                }
-                acc_ld16(tm, lane_base + T_DW1 + (uint32_t)c16, v);
-                if (lane < 16) {
-                    float* dst = gout + L.off_w1 + t_row * O + c16;
-                    if (FUSED && ((L.off_w1 | O) & 3) == 0) {
-#pragma unroll
-                        for (int i = 0; i < 16; i += 4)
-                            if (c16 + i < O) __stcg(reinterpret_cast<float4*>(dst + i), make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]));
-                    } else {
+                    acc_ld16(tm, lane_base + T_DW1 + (uint32_t)c16, v);
+                    if (lane < 16) {
+                        float* dst = gout + L.off_w1 + t_row * O + c16;
 #pragma unroll
                         for (int i = 0; i < 16; ++i)
                             if (c16 + i < O) __stcg(dst + i, v[i]);
+                        if (ones_col && h == 3) __stcg(gout + L.off_b1 + t_row, v[15]);        // column 63 of dW1 = db1
                     }
-                    if (ones_col && h == 3) __stcg(gout + L.off_b1 + t_row, v[15]);        // column 63 of dW1 = db1
                 }
                 if (h == 0) {      // dW3^T [k][o]
                     acc_ld16(tm, lane_base + T_DW3, v);
@@ -754,21 +779,9 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     acc_ld16(tm, lane_base + T_DB2, v);
                     if (lane < 16) __stcg(gout + L.off_b2 + t_row, v[0]);
                 }
-                epi_bar_sync();                        // sRed of the sixteen epilogue warps
-                if (tid < L.out) __stcg(gout + L.off_b3 + tid, (sRed[96 + tid] + sRed[112 + tid]) + (sRed[128 + tid] + sRed[144 + tid]));
-                if (net == 0 && tid >= 32 && tid < 32 + A) {
-                    const int a = tid - 32;
-                    float g = (sRed[32 + a] + sRed[48 + a]) + (sRed[64 + a] + sRed[80 + a]);
-                    if (blockIdx.x == 0 && loss_has_entropy<!FUSED>(p.lc.kind)) g -= p.lc.entropy_coef / (float)A;
-                    if (p.lc.kind == LOSS_FVP) g = (blockIdx.x == 0) ? 2.f / (float)A * __ldg(p.fvp_vec + L.off_logstd + a) : 0.f;
-                    __stcg(gout + L.off_logstd + a, g);
-                }
-                if (tid >= 64 && tid < 72) {
-                    const int i = tid - 64;
-                    __stcg(p.stats_part + ((size_t)blockIdx.x * 3 + net) * 8 + i, (i < 5) ? (sRed[i] + sRed[8 + i]) + (sRed[16 + i] + sRed[24 + i]) : 0.f);
-                }
             } else {
-                for (int i = tid; i < L.size; i += NEPI) __stcg(gout + i, 0.f);      // no tile of this (short) minibatch
+                // no tile of this (short) minibatch; FUSED: the slice reduction adds 0.f for this CTA without reading it
+                if (!FUSED) for (int i = tid; i < L.size; i += NEPI) __stcg(gout + i, 0.f);
                 if (tid < 8) __stcg(p.stats_part + ((size_t)blockIdx.x * 3 + net) * 8 + tid, 0.f);
             }
             stamp(22);
@@ -777,22 +790,33 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
             // ================= in-kernel optimiser step =========================================================
             net_barrier();                                             // every partial gradient of this network is in L2
             stamp(23);
-            const int S = (L.size + G - 1) / G;                        // parameters owned by this CTA: [p0, p0 + S)
-            const int p0 = (int)blockIdx.x * S;
+            // One rank: clip_grad_norm_ almost never clips (max_grad_norm 40), so Adam runs SPECULATIVELY with coefficient 1
+            // before the slice norms are known; the barrier that publishes the norms is then also the one that publishes the
+            // new parameters, and only a step that does clip redoes Adam from the saved state (one more barrier).
+            const bool spec = p.world == 1 && S <= NEPI;
             const int Gh = (G + 1) >> 1;
-            const float* gnet = p.gpart + (size_t)((gridDim.y == 1 ? 0 : net) * G) * PSTR;
-            float ssq = 0.f, st2 = 0.f;
+            // The W1 / W2 partials of CTA b are read straight from its accumulator image: the MMA-issue warpgroup's image stores
+            // precede its DONE_C6 arrival (fence + bar.sync 3 + mbarrier.arrive, release at CTA scope), the epilogue warps
+            // acquire them by their DONE_C6 wait, and epi_bar_sync orders that before thread 0's red.release.gpu in
+            // net_barrier: causality order is transitive across scopes, so the stores happen-before every read behind the
+            // barrier's acquire, and the reads bypass L1 (ld.cg).  No CTA writes its dW / db columns again before the next
+            // minibatch's first tile, which follows the barrier after this reduction.
+            const float* anet = p.acc + (size_t)blockIdx.y * G * 128 * T_COLS;
+            const float* gnet = p.gpart + (size_t)((gridDim.y == 1 ? 0 : net) * G) * PSTR;      // b3 / log_std partials
+            float ssq = 0.f, st2 = 0.f, g_raw = 0.f;       // g_raw: the reduced gradient of the parameter this thread owns
             for (int base = 0; base < S; base += 256) {
                 const int pi = base + (tid & 255), part = tid >> 8;
                 const bool valid = pi < S && p0 + pi < L.size;
                 float sacc = 0.f;
                 if (valid) {
-                    const float* src = gnet + p0 + pi;
+                    const int off = grad_src(p0 + pi);
+                    const float* src = off >= 0 ? anet + off : gnet + p0 + pi;
+                    const size_t stride = off >= 0 ? (size_t)128 * T_COLS : (size_t)PSTR;
                     const int b1 = min(G, (part + 1) * Gh);
                     for (int b = part * Gh; b < b1; b += 32) {       // 32 partial rows in flight per thread
                         float t[32];
 #pragma unroll
-                        for (int u = 0; u < 32; ++u) t[u] = (b + u < b1) ? __ldcg(src + (size_t)(b + u) * PSTR) : 0.f;
+                        for (int u = 0; u < 32; ++u) t[u] = (b + u < b1 && b + u < ntiles) ? __ldcg(src + (size_t)(b + u) * stride) : 0.f;
 #pragma unroll
                         for (int w = 16; w > 0; w >>= 1)
 #pragma unroll
@@ -801,32 +825,35 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     }
                 }
                 sPart[tid] = sacc;
+                stamp(29);
                 epi_bar_sync();
                 if (part == 0 && valid) {
                     const int qg = noff + p0 + pi;
                     float g = sPart[tid] + sPart[256 + tid];
                     if (net != 0 && p.critic_norm_coef > 0.f) {
-                        const float th = __ldcg(p.theta_rw + qg);
+                        const float th = base == 0 ? pre_th : __ldcg(p.theta_rw + qg);      // base 0: this thread owns qg
                         g += 2.f * p.critic_norm_coef * th; st2 += th * th;
                     }
                     __stcg(p.grad + qg, g);
                     ssq += g * g;
+                    if (base == 0) g_raw = g;
+                    else sPart[tid] = g;                   // spec: to its owner, thread pi (only it reads this slot now)
                 }
                 epi_bar_sync();
+                if (spec && base > 0 && own && tid >= 256) g_raw = sPart[tid - 256];      // spec: S <= 512, base 256 is the last chunk
             }
             ssq = warp_sum(ssq); st2 = warp_sum(st2);
-            if (lane == 0) { sPart[warp] = ssq; sPart[16 + warp] = st2; }
+            if (lane == 0) { sPart[256 + warp] = ssq; sPart[272 + warp] = st2; }       // the hand-over slots stay untouched
             epi_bar_sync();
             if (tid == 0) {
                 float a = 0.f, b = 0.f;
-                for (int w = 0; w < 16; ++w) { a += sPart[w]; b += sPart[16 + w]; }
+                for (int w = 0; w < 16; ++w) { a += sPart[256 + w]; b += sPart[272 + w]; }
                 __stcg(p.sumsq_part + (net * 2 + 0) * G + blockIdx.x, a);
                 __stcg(p.sumsq_part + (net * 2 + 1) * G + blockIdx.x, b);
             }
-            // Adam state of this thread's parameter: loaded before the barrier, consumed after it
-            const bool own = tid < S && p0 + tid < L.size;
-            float pre_th = 0.f, pre_m = 0.f, pre_v = 0.f;
-            if (own) { pre_th = __ldcg(p.theta_rw + noff + p0 + tid); pre_m = __ldcg(p.adam_m + noff + p0 + tid); pre_v = __ldcg(p.adam_v + noff + p0 + tid); }
+            stamp(30);
+            if (dbg_on && own) p.dbg[(tid == 0 ? 0 : 1024) + 1023] = __float_as_int(pre_th + pre_m + pre_v);     // waits for the state
+            stamp(31);
             // torch-Adam step of one parameter (+ its three bf16 pieces in the weight-tile image)
             auto adam_store = [&](int qg, float g, float th, float m, float v, bool img) {
                 const float step_size = sScal[8], bc2_sqrt = sScal[9];
@@ -844,12 +871,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     __stcg(reinterpret_cast<unsigned short*>(wimg + img_off + 2 * img_sub), (unsigned short)w2);
                 }
             };
-            // One rank: clip_grad_norm_ almost never clips (max_grad_norm 40), so Adam runs SPECULATIVELY with coefficient 1
-            // before the slice norms are known; the barrier that publishes the norms is then also the one that publishes the
-            // new parameters, and only a step that does clip redoes Adam from the saved state (one more barrier).
-            const bool spec = p.world == 1 && S <= NEPI;
-            float g_raw = 0.f;
-            if (spec && own) { g_raw = __ldcg(p.grad + noff + p0 + tid); adam_store(noff + p0 + tid, g_raw, pre_th, pre_m, pre_v, true); }
+            if (spec && own) adam_store(noff + p0 + tid, g_raw, pre_th, pre_m, pre_v, true);
             stamp(24);
             net_barrier();                                             // every slice norm of this network is in L2
             stamp(25);

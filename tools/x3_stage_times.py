@@ -18,7 +18,8 @@ torch.cuda.synchronize()
 lib().osb_x3_debug_buffer(0)
 NAMES = {0: 'E0 start', 1: 'X free', 2: 'X stored+sync', 3: 'C1 ok', 4: 'E1 done', 5: 'C2 ok', 6: 'E2 done', 7: 'C3 ok', 8: 'dOUT stored', 9: 'E3 done',
          10: 'C4A ok', 11: 'E4 computed', 12: 'C4B ok', 13: 'E4 stored', 14: 'C5A ok', 15: 'E5 computed', 16: 'C5B ok', 17: 'E5 stored', 20: 'tiles done',
-         21: 'C6 ok', 22: 'extracted', 23: 'barrier1', 24: 'reduced', 25: 'barrier2', 26: 'adam done', 27: 'barrier3', 28: 'restaged',
+         21: 'C6 ok', 22: 'partials out', 23: 'barrier1', 29: 'partials loaded', 30: 'norm published', 31: 'Adam state in',
+         24: 'Adam stored', 25: 'barrier2', 26: 'adam done', 27: 'barrier3', 28: 'restaged',
          200: 'dW3 read H2', 201: 'dW2 read H2, H1', 202: 'dW1 read X', 203: 'gradients committed'}
 # MMA-issue warpgroup: 100 + 20 k for product k, + 4 r + event for row half r
 for k, prod in enumerate(('Z1', 'Z2', 'OUT', "dZ2'", "dZ1'")):
