@@ -16,7 +16,7 @@
 namespace osb {
 
 constexpr int TC_ROWS = 128;                                    // rows per tile
-constexpr uint32_t TC_C_Z = 0, TC_C_OUT = 64, TC_COLS = 80;     // accumulator columns: Z [0, 64), OUT [64, 80)
+constexpr uint32_t TC_C_Z = 0, TC_C_OUT = 64, TC_COLS = 80;     // accumulator columns: Z [0, 64) (tf32), OUT [64, 80)
 
 // Operand tiles, byte offsets from the 1024-byte aligned base of the dynamic shared memory.  tf32: X / H2 [128][64],
 // H1 [128][64], W1 [64][64] (one 64-column chunk), W2 [64][64], W3 [16][64]; bf16x3: the activation buffer and the
@@ -201,29 +201,36 @@ __device__ __forceinline__ void tc_forward(uint32_t base, const umma::Acc& tm, u
     if constexpr (X3) {
         const uint64_t dAct = x3::desc128(base + T::X), dW1 = x3::desc128(base + T::W1), dW2 = x3::desc128(base + T::W2),
                        dW3 = x3::desc128(base + T::W3);
+        // The hidden layers' products are staged as fp32 in the activation buffer they are about to overwrite
+        // (x3::Staged): each row quarter's values stay inside its own rows, so the two warps of the rows read theirs,
+        // meet (named barrier 4 + q), and store the pieces over them.
+        static_assert(x3::staged_in_own_rows<64>(T::SUB), "a staged row leaves its own bytes of the activation buffer");
+        const x3::Staged sZ{base + T::X, T::SUB};
         auto hidden = [&](const float* sB) {   // tanh(Z + b) over the activation buffer
+            float v[4][8];
 #pragma unroll
             for (int c8 = 0; c8 < 4; ++c8) {
                 const int c0 = 32 * h + 8 * c8;
-                float v[8];
-                x3::acc_ld8(tm, lane_base + TC_C_Z + (uint32_t)c0, v);
+                x3::staged_load<64>(sZ, 32 * q + lane, c0, v[c8]);
 #pragma unroll
-                for (int i = 0; i < 8; ++i) v[i] = x3::tanh_acc(v[i] + sB[c0 + i]);
-                x3::store8_x3(base + T::X, T::SUB, 32 * q + lane, c0, v);
+                for (int i = 0; i < 8; ++i) v[c8][i] = x3::tanh_acc(v[c8][i] + sB[c0 + i]);
             }
+            asm volatile("bar.sync %0, 64;\n" ::"r"(4 + q) : "memory");
+#pragma unroll
+            for (int c8 = 0; c8 < 4; ++c8) x3::store8_x3(base + T::X, T::SUB, 32 * q + lane, 32 * h + 8 * c8, v[c8]);
             fence_async_smem();
             __syncthreads();
         };
         stage_chunk(0);
         if (mma_wg) {
-            x3::gemm_x3<128, 64, 4, 0, 0>(tm, TC_C_Z, dAct, T::SUB, 32u, dW1, T::WSUB, 32u, false);
+            x3::gemm_x3_staged<64, 4, 0>(sZ, dAct, T::SUB, 32u, dW1, T::WSUB, 32u);
             mma_commit(bar);
         }
         mbar_wait(bar, phase); phase ^= 1;
         after(1);
         hidden(sB1);
         if (mma_wg) {
-            x3::gemm_x3<128, 64, 4, 0, 0>(tm, TC_C_Z, dAct, T::SUB, 32u, dW2, T::WSUB, 32u, false);
+            x3::gemm_x3_staged<64, 4, 0>(sZ, dAct, T::SUB, 32u, dW2, T::WSUB, 32u);
             mma_commit(bar);
         }
         mbar_wait(bar, phase); phase ^= 1;

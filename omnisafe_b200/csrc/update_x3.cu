@@ -123,8 +123,12 @@ __host__ __device__ constexpr uint32_t bar_arrivals(int b) { return b >= DONE_C1
 constexpr uint32_t OFF_PF = OFF_BARS + NBAR * 8 + 16;
 __host__ __device__ constexpr int pf_ld(int AP) { return AP + 3; }
 constexpr uint32_t X3_SMEM = OFF_PF + XT * pf_ld(16) * 4;
-// accumulator columns
-constexpr uint32_t T_ZA = 0, T_ZB = 64, T_OUT = 128, T_DW1 = 144, T_DW2 = 208, T_DW3 = 272, T_DB1 = 288, T_DB2 = 304, T_COLS = 320;
+static_assert(1024 + X3_SMEM <= 232448, "more shared memory than an H100 block can have");
+// The forward products Z1, Z2 and OUT are staged as fp32 in the footprints of H1, H2 and D (x3::Staged), which they
+// become: each row quarter's values stay inside its own rows of the tile, so no other warps' bytes are overwritten.
+static_assert(staged_in_own_rows<64>(ACT_SUB) && staged_in_own_rows<16>(D_SUB), "a staged row leaves its own bytes of the tile");
+// accumulator columns: dZ2' and dZ1' (T_ZA, T_ZB), the weight and bias gradients; [128, 144) is not written
+constexpr uint32_t T_ZA = 0, T_ZB = 64, T_DW1 = 144, T_DW2 = 208, T_DW3 = 272, T_DB1 = 288, T_DB2 = 304, T_COLS = 320;
 
 // fp32 parameters of one network -> bf16x3 weight tiles + fp32 biases in shared memory (all NEPI epilogue threads).
 // All global loads are issued before the first store (one L2 round trip instead of one per loop iteration).
@@ -253,6 +257,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
     fence_async_smem();
     __syncthreads();
     const Acc tm = acc_cta(p.acc, T_COLS);
+    const Staged sZ1{sbase + OFF_H1, ACT_SUB}, sZ2{sbase + OFF_H2, ACT_SUB}, sOut{sbase + OFF_D, D_SUB};
 
     if (is_mma_warp) {
         // ======================= MMA-issue warpgroup: uniform control flow ====================================
@@ -282,25 +287,36 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 const bool first = tile == (int)blockIdx.x;         // the first tile of a minibatch overwrites the accumulators
                 const bool last = tile + G >= ntiles;
                 // Z1 = X W1^T, one row half after the other: each half is stored and committed on its own, and the epilogue
-                // of rows 0-63 runs under the MMAs of rows 64-127
+                // of rows 0-63 runs under the MMAs of rows 64-127.
+                // Z1, Z2 and OUT are staged in shared memory, over the tile each becomes, by generic stores after this
+                // warpgroup's wgmma wait; the commit's fence + bar.sync 3 + mbarrier arrival (release) orders them before
+                // the epilogue's loads (acquire by its DONE wait), and `announce` fences the epilogue's bf16x3 stores
+                // over them for the next MMAs.  Every earlier reader of a destination has completed by then:
+                //   H1 <- Z1(t): the wgmma readers Z2(t-1), dW2(t-1), dW1(t-1) and db1(t-1) were waited on by this
+                //   in-order warpgroup before DONE_C6(t-1); the epilogue's E5(t-1) loads precede its RDY_DZ1 arrivals.
+                //   H2 <- Z2(t): OUT(t-1), dW3(t-1), dZ1'(t-1), dW2(t-1) likewise, and db2 of tile t-1 -- issued after
+                //   Z1(t), or before DONE_C6(t-1) on a minibatch's last tile -- is a gemm_x3 that returns only after its
+                //   wg_wait<0>; E4(t-1)'s loads precede RDY_DZ2.
+                //   D <- OUT(t): dZ2'(t-1) and dW3(t-1) were waited on; every dOUT store of rows of half r precedes the
+                //   RDY_D arrivals (and, in a statistics pass, which skips the backward, the RDY_H2 arrivals) of half r.
 #pragma unroll 1
                 for (int r = 0; r < 2; ++r) {
                     mbar_wait_a(bar(RDY_X0 + r), par);
                     mstamp(100 + 4 * r);
-                    gemm_x3_rows<64, 2, 2, 0>(tm, T_ZA, r, dX, ACT_SUB, 32u, dW1, W_SUB, 32u, [&](int) { mstamp(101 + 4 * r); });
+                    gemm_x3_rows<64, 2, 2, 0>(sZ1, r, dX, ACT_SUB, 32u, dW1, W_SUB, 32u, [&](int) { mstamp(101 + 4 * r); });
                     mstamp(102 + 4 * r);
                     mma_commit_a(bar(DONE_C1_0 + r));
                     mstamp(103 + 4 * r);
                 }
-                // db2 of the PREVIOUS tile (dZ2 still sits in the H2 buffer until this tile's E2): runs under E1,
-                // completes before Z2 (in-order pipe), so DONE_C2_0 / _1 cover it
+                // db2 of the PREVIOUS tile (dZ2 still sits in the H2 buffer until this tile's Z2 is staged there): runs
+                // under E1 and is waited on before Z2 is issued
                 if (!first && !(!FUSED && p.forward_only)) gemm_x3<64, 16, 8, 1, 1, true>(tm, T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, tile != (int)blockIdx.x + G);
                 // Z2 = H1 W2^T
 #pragma unroll 1
                 for (int r = 0; r < 2; ++r) {
                     mbar_wait_a(bar(RDY_H1_0 + r), par);
                     mstamp(120 + 4 * r);
-                    gemm_x3_rows<64, 2, 2, 0>(tm, T_ZB, r, dH1, ACT_SUB, 32u, dW2, W_SUB, 32u, [&](int) { mstamp(121 + 4 * r); });
+                    gemm_x3_rows<64, 2, 2, 0>(sZ2, r, dH1, ACT_SUB, 32u, dW2, W_SUB, 32u, [&](int) { mstamp(121 + 4 * r); });
                     mstamp(122 + 4 * r);
                     mma_commit_a(bar(DONE_C2_0 + r));
                     mstamp(123 + 4 * r);
@@ -310,7 +326,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 for (int r = 0; r < 2; ++r) {
                     mbar_wait_a(bar(RDY_H2_0 + r), par);
                     mstamp(140 + 4 * r);
-                    gemm_x3_rows<16, 2, 2, 0>(tm, T_OUT, r, dH2, ACT_SUB, 32u, dW3, W3_SUB, 32u, [&](int) { mstamp(141 + 4 * r); });
+                    gemm_x3_rows<16, 2, 2, 0>(sOut, r, dH2, ACT_SUB, 32u, dW3, W3_SUB, 32u, [&](int) { mstamp(141 + 4 * r); });
                     mstamp(142 + 4 * r);
                     mma_commit_a(bar(DONE_C3_0 + r));
                     mstamp(143 + 4 * r);
@@ -518,57 +534,55 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     }
                 }
                 // ---- E1: H1 = tanh(Z1 + b1) -------------------------------------------------------------------
+                // Z1 is staged over H1 (see the MMA-issue loop): the four warps of the rows read their values of it, meet,
+                // and only then store the pieces of H1 over them
                 mbar_wait_a(bar(DONE_C1_0 + rh), par);
                 stamp(3);
+                float hv[2][8];
 #pragma unroll
                 for (int ph = 0; ph < 2; ++ph) {
                     const int c0 = 32 * ph + 8 * h;
-                    float v[8];
-                    acc_ld8(tm, lane_base + T_ZA + (uint32_t)c0, v);
+                    staged_load<64>(sZ1, s_row, c0, hv[ph]);
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) v[i] = tanh_acc(v[i] + sB1[c0 + i]);
-                    store8_x3(sbase + OFF_H1, ACT_SUB, s_row, c0, v);
+                    for (int i = 0; i < 8; ++i) hv[ph][i] = tanh_acc(hv[ph][i] + sB1[c0 + i]);
                 }
+                rows_bar_sync(q);
+#pragma unroll
+                for (int ph = 0; ph < 2; ++ph) store8_x3(sbase + OFF_H1, ACT_SUB, s_row, 32 * ph + 8 * h, hv[ph]);
                 announce(RDY_H1_0 + rh);
-                // ---- E2: H2 = tanh(Z2 + b2) -------------------------------------------------------------------
+                // ---- E2: H2 = tanh(Z2 + b2), from Z2 staged over H2 --------------------------------------------
                 stamp(4);
                 mbar_wait_a(bar(DONE_C2_0 + rh), par);
                 stamp(5);
 #pragma unroll
                 for (int ph = 0; ph < 2; ++ph) {
                     const int c0 = 32 * ph + 8 * h;
-                    float v[8];
-                    acc_ld8(tm, lane_base + T_ZB + (uint32_t)c0, v);
+                    staged_load<64>(sZ2, s_row, c0, hv[ph]);
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) v[i] = tanh_acc(v[i] + sB2[c0 + i]);
-                    store8_x3(sbase + OFF_H2, ACT_SUB, s_row, c0, v);
+                    for (int i = 0; i < 8; ++i) hv[ph][i] = tanh_acc(hv[ph][i] + sB2[c0 + i]);
                 }
+                rows_bar_sync(q);
+#pragma unroll
+                for (int ph = 0; ph < 2; ++ph) store8_x3(sbase + OFF_H2, ACT_SUB, s_row, 32 * ph + 8 * h, hv[ph]);
                 announce(RDY_H2_0 + rh);
                 stamp(6);
                 // ---- E3: OUT -> loss -> dOUT (one thread per sample in each of the four warps of the rows) -----------
                 // Every warp computes the sample's scalar part of the loss (the same bits in each) and the gradient of
                 // its own actions a_lo .. a_lo + NA - 1; the statistics are those of the warps with h == 0.
-                if (h == 0) asm volatile("cp.async.wait_all;\n" ::: "memory");
-                rows_bar_sync(q);                                          // the PF rows of the four warps' samples
                 mbar_wait_a(bar(DONE_C3_0 + rh), par);
                 stamp(7);
                 {
+                    // every warp reads the whole OUT row, staged over D, before the four meet: behind the barrier they
+                    // store dOUT over it
+                    float o[AP];
+                    staged_load<16>(sOut, s_row, 0, o);
+                    if (h == 0) asm volatile("cp.async.wait_all;\n" ::: "memory");
+                    rows_bar_sync(q);                                      // and the PF rows of the four warps' samples
                     const long long prow = sRow[s_row];
                     const float* pf = reinterpret_cast<const float*>(gbase + OFF_PF) + s_row * pf_ld(AP);
-                    float o[AP], dq[NA];
+                    float dq[NA];
 #pragma unroll
                     for (int j = 0; j < NA; ++j) dq[j] = 0.f;
-                    if (AP == 8) {
-                        float t8[8];
-                        acc_ld8(tm, lane_base + T_OUT, t8);
-#pragma unroll
-                        for (int a = 0; a < AP; ++a) o[a] = t8[a];
-                    } else {
-                        float t16[16];
-                        acc_ld16(tm, lane_base + T_OUT, t16);
-#pragma unroll
-                        for (int a = 0; a < AP; ++a) o[a] = t16[a];
-                    }
                     auto own = [&](int a) { return a < A && a >= a_lo && a < a_lo + NA; };
                     if (prow >= 0) {
                         if (net != 0) {              // critic: one output, action 0 of the warps with h == 0

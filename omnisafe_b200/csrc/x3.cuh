@@ -157,25 +157,105 @@ __device__ __forceinline__ void gemm_x3(const Acc& acc, uint32_t d_addr, uint64_
     }
 }
 
+// ---- products staged in shared memory ------------------------------------------------------------------
+// A product of N = 64 (16) columns that its epilogue turns into a [128][N] bf16x3 operand tile can be staged as fp32 in
+// that tile's own footprint instead of the image: three SW128 (SW32) sub-tiles `split` bytes apart, of which row r's fp32
+// values take the 128 (32) bytes of row r in sub-tiles 0 and 1 -- columns 0-31 (0-7) in sub-tile 0, 32-63 (8-15) in
+// sub-tile 1 -- with the sub-tile's 16-byte-chunk XOR swizzle.  So the fp32 values of rows 32 q .. 32 q + 31 lie inside
+// those rows' bytes of the tile, and the epilogue warps of those rows alone can read them, meet, and store the bf16x3
+// pieces over them.  The MMA-issue warpgroup writes them only past the wgmma wait that follows the last read of the tile.
+struct Staged {
+    uint32_t base;     // shared address of sub-tile 0 (1024-byte aligned)
+    uint32_t split;    // bytes between the sub-tiles
+};
+template <int N>
+__host__ __device__ constexpr uint32_t staged_off(int r, int c, uint32_t split) {
+    static_assert(N == 16 || N == 64, "staged products are N = 16 (SW32) or N = 64 (SW128)");
+    if constexpr (N == 64) return (uint32_t)(c >> 5) * split + (uint32_t)(r * 128 + ((((c >> 2) & 7) ^ (r & 7)) << 4) + ((c & 3) << 2));
+    else return (uint32_t)(c >> 3) * split + (uint32_t)(r * 32 + ((((c >> 2) & 1) ^ ((r >> 2) & 1)) << 4) + ((c & 3) << 2));
+}
+// every fp32 value of every row r of a [128][N] product staged in sub-tiles `split` bytes apart lies in row r's bytes of
+// sub-tile 0 or 1, 4-byte aligned, and no two values share bytes (for the static_asserts of the kernels that stage)
+template <int N>
+constexpr bool staged_in_own_rows(uint32_t split) {
+    constexpr uint32_t pitch = N == 64 ? 128u : 32u;
+    if (split < 128u * pitch) return false;
+    for (int r = 0; r < 128; ++r) {
+        uint32_t seen[N / 32 + 1] = {};      // bit per float slot of the row in sub-tiles 0 and 1
+        for (int c = 0; c < N; ++c) {
+            const uint32_t off = staged_off<N>(r, c, split), sub = off / split, in = off % split;
+            if (sub > 1u || in / pitch != (uint32_t)r || (in & 3u) != 0u) return false;
+            const uint32_t slot = sub * (pitch / 4u) + (in % pitch) / 4u;
+            if ((seen[slot / 32u] >> (slot % 32u)) & 1u) return false;
+            seen[slot / 32u] |= 1u << (slot % 32u);
+        }
+    }
+    return true;
+}
+// the m64 fragment of rows 64 half .. 64 half + 63 of this warpgroup thread: element (rr, j, e) is row
+// 64 half + 16 w + l / 4 + 8 rr, column 8 j + 2 (l % 4) + e
+template <int N>
+__device__ __forceinline__ void staged_store(const Staged& s, int half, const float (&d)[N / 2]) {
+    const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+        const int m = 64 * half + 16 * w + (l >> 2) + 8 * rr;
+#pragma unroll
+        for (int j = 0; j < N / 8; ++j)
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(s.base + staged_off<N>(m, 8 * j + 2 * (l & 3), s.split)),
+                         "f"(d[4 * j + 2 * rr]), "f"(d[4 * j + 2 * rr + 1]) : "memory");
+    }
+}
+// NV consecutive columns [c0, c0 + NV) (c0 % 4 == 0, NV % 4 == 0) of row r
+template <int N, int NV>
+__device__ __forceinline__ void staged_load(const Staged& s, int r, int c0, float (&v)[NV]) {
+#pragma unroll
+    for (int i = 0; i < NV / 4; ++i)
+        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+                     : "=f"(v[4 * i]), "=f"(v[4 * i + 1]), "=f"(v[4 * i + 2]), "=f"(v[4 * i + 3])
+                     : "r"(s.base + staged_off<N>(r, c0 + 4 * i, s.split)));
+}
+
+// gemm_x3<128, N, NK, 0, TB> without accumulation, stored into the staging footprint s instead of the image: the same
+// wgmmas in the same order, half 0 stored while half 1 runs.  Half 0's rows of the footprint are not rows that half 1's
+// MMAs read, so A may be the tile being staged over.
+template <int N, int NK, int TB>
+__device__ __forceinline__ void gemm_x3_staged(const Staged& s, uint64_t a0, uint32_t asplit, uint32_t akstep, uint64_t b0,
+                                        uint32_t bsplit, uint32_t bkstep) {
+    static_assert(N == 16 || N == 64, "unsupported bf16x3 GEMM shape");
+    constexpr int NJ = N / 8;
+    a0 = desc_fresh(a0);
+    b0 = desc_fresh(b0);
+    float d0[4 * NJ] = {}, d1[4 * NJ] = {};
+    x3_block<0, TB, NJ, NK, false>(d0, a0, asplit, akstep, b0, bsplit, bkstep);
+    x3_block<0, TB, NJ, NK, false>(d1, desc_add(a0, 64u * (((a0 >> 61) & 7u) == 2u ? 128u : 32u)), asplit, akstep, b0, bsplit, bkstep);
+    wg_wait<1>();
+    acc_fence(d0);
+    staged_store<N>(s, 0, d0);
+    wg_wait<0>();
+    acc_fence(d1);
+    staged_store<N>(s, 1, d1);
+}
+
 // Rows 64 r .. 64 r + 63 (r = 0 or 1) of a 128-row product with a K-major A, as one m64 block over the whole K, stored
-// once into the image rows of the M = 128 product at d_addr (row m in lane m).  The two row halves of a product share
-// nothing but B, so each can be issued, stored and announced on its own.
+// once: into the image rows of the M = 128 product at d_addr (row m in lane m), or into the staging footprint s.  The two
+// row halves of a product share nothing but B, so each can be issued, stored and announced on its own.
 //   NC = 2: K is split into two runs of NK k-steps; each run is its own wgmma chain, started from zero into its own
 //   fragment and both in flight together, and the stored value is the fp32 sum of the two chains, one add per element.
 //   That is the value two column-half phases of gemm_x3<128, ...> leave in the image (the second accumulating), bit for
 //   bit, without the image read.  One chain over all 2 NK k-steps would save the add and a fragment and round differently.
 //   NC = 1: one chain of NK k-steps, stored as it is.
 // a0 / b0 and the strides as for gemm_x3; `waited(r)` is called when the MMAs have completed.
-template <int N, int NK, int NC, int TB, class Stamp = NoStamp>
-__device__ __forceinline__ void gemm_x3_rows(const Acc& acc, uint32_t d_addr, int r, uint64_t a0, uint32_t asplit,
-                                             uint32_t akstep, uint64_t b0, uint32_t bsplit, uint32_t bkstep,
-                                             Stamp waited = Stamp()) {
+template <int N, int NK, int NC, int TB, class Stamp>
+__device__ __forceinline__ void rows_x3(float (&d)[N / 2], int r, uint64_t a0, uint32_t asplit, uint32_t akstep,
+                                        uint64_t b0, uint32_t bsplit, uint32_t bkstep, Stamp waited) {
     static_assert((N == 16 || N == 64) && (NC == 1 || NC == 2), "unsupported bf16x3 row-half GEMM shape");
     constexpr int NJ = N / 8;
     a0 = desc_fresh(a0);
     b0 = desc_fresh(b0);
     a0 = desc_add(a0, (uint32_t)r * 64u * (((a0 >> 61) & 7u) == 2u ? 128u : 32u));
-    float d[4 * NJ] = {};
+#pragma unroll
+    for (int i = 0; i < 4 * NJ; ++i) d[i] = 0.f;
     x3_block<0, TB, NJ, NK, false>(d, a0, asplit, akstep, b0, bsplit, bkstep);
     if constexpr (NC == 2) {
         float d1[4 * NJ] = {};
@@ -191,7 +271,21 @@ __device__ __forceinline__ void gemm_x3_rows(const Acc& acc, uint32_t d_addr, in
         acc_fence(d);
         waited(r);
     }
-    frag_store<NJ>(acc, d_addr, 128, r, d);
+}
+template <int N, int NK, int NC, int TB, class Stamp = NoStamp>
+__device__ __forceinline__ void gemm_x3_rows(const Acc& acc, uint32_t d_addr, int r, uint64_t a0, uint32_t asplit,
+                                             uint32_t akstep, uint64_t b0, uint32_t bsplit, uint32_t bkstep,
+                                             Stamp waited = Stamp()) {
+    float d[N / 2];
+    rows_x3<N, NK, NC, TB>(d, r, a0, asplit, akstep, b0, bsplit, bkstep, waited);
+    frag_store<N / 8>(acc, d_addr, 128, r, d);
+}
+template <int N, int NK, int NC, int TB, class Stamp = NoStamp>
+__device__ __forceinline__ void gemm_x3_rows(const Staged& s, int r, uint64_t a0, uint32_t asplit, uint32_t akstep,
+                                             uint64_t b0, uint32_t bsplit, uint32_t bkstep, Stamp waited = Stamp()) {
+    float d[N / 2];
+    rows_x3<N, NK, NC, TB>(d, r, a0, asplit, akstep, b0, bsplit, bkstep, waited);
+    staged_store<N>(s, r, d);
 }
 
 // ---- fp32 <-> three bf16 ----------------------------------------------------------------------------
