@@ -206,6 +206,22 @@ int osb_eval_ext_observe_rst(int O, int N, int t, int obs_normalize, const float
                              int* ctr, double* out_ret, double* out_cost, int* out_len, double* workspace,
                              int* nonfinite, unsigned char* rst, void* stream);
 int osb_eval_ext_prepare(int On, int A, int N, int precision);
+/* Evaluation on a registered env that declares need_time_limit_wrapper / need_auto_reset_wrapper (envs/core.py).  The
+ * evaluation applies TimeLimit only (evaluator.py: TimeLimit(time_limit = 1000), never AutoReset), so such an env does
+ * not reset itself.  osb_eval_ext_observe_wrapped = osb_eval_ext_observe_rst with the wrapper step: tl_steps[N]
+ * (device ints, zero at the first reset) counts the steps of each running env's episode and is cleared at its end; with
+ * time_limit > 0 a step is truncated when the count reaches time_limit, whatever the env's truncated says (time_limit =
+ * 0: the env's flag).  rst[N] is 1 for every episode end with episodes left: N > 1 resets them through
+ * env.reset_envs(rst) -> osb_ext_reset_rows (the reset rows as their own push, as the reference's explicit reset), N == 1
+ * through ctr[2] and env.reset() as above.  No final rows are read: each step's rows are the env's own.  Capturable. */
+int osb_eval_ext_observe_wrapped(int O, int N, int t, int obs_normalize, const float* next_obs, const float* rew,
+                                 const float* cost, const unsigned char* terminated, const unsigned char* truncated,
+                                 float* s_raw, float* norm_mean, float* norm_sumsq, float* norm_std,
+                                 long long* norm_count, unsigned* ticket, float* safety, float safety_budget,
+                                 float saute_gamma, int early, double cost_limit, double cost_criteria, int* left,
+                                 int* done_eps, double* ret, double* cost_acc, int* len, int* ctr, double* out_ret,
+                                 double* out_cost, int* out_len, double* workspace, int* nonfinite, unsigned char* rst,
+                                 int* tl_steps, int time_limit, void* stream);
 /* ---- rollout on an external env (a user CMDP stepped in PyTorch) ----------------------------
  * The fused step split at the env boundary.  Per epoch: env.reset() -> osb_ext_reset_ingest; for t in [0, T):
  * osb_ext_act(t) -> env.step(act_env) -> osb_ext_observe(t); then osb_ext_act(T) (epoch-end bootstrap, critics only)
@@ -263,6 +279,26 @@ int osb_ext_observe_early(int O, int N, int T, int t, int obs_normalize, const f
 int osb_ext_reset_rows(int O, int N, int t, int obs_normalize, const unsigned char* mask, const float* obs, float* s_raw,
                        float* norm_mean, float* norm_sumsq, float* norm_std, long long* norm_count, unsigned* ticket,
                        double* workspace, int* nonfinite, void* stream);
+/* TimeLimit and AutoReset (wrapper.py) for an external env that declares need_time_limit_wrapper /
+ * need_auto_reset_wrapper and does not reset itself.  Per step: osb_ext_act(t) -> env.step -> osb_ext_wrapper_step ->
+ * reset of the envs in done -> osb_ext_observe_wrapped(t).  osb_ext_wrapper_step, one byte per env: steps[N] (device
+ * ints, TimeLimit's _time; zero them at every epoch-start reset) += 1; trunc_out = steps >= time_limit when time_limit
+ * > 0 (the env's own truncated is discarded), else the env's truncated; done = terminated | trunc_out; steps = 0 where
+ * done.  done_total (device int, or NULL) is zeroed on the stream and receives the number of done envs.
+ * osb_ext_observe_wrapped = osb_ext_observe of a step whose final observation is the step's own row: truncated is
+ * trunc_out, the rows of step_obs where done is set are the final rows (final_raw, the first ObsNormalize push), and the
+ * next row of such an env is its row of reset_obs[N][O] (read only where done is set; NULL when no env is done).  The
+ * second push is every env's next row, so the reset rows join the step's batch, as AutoReset inside ObsNormalize does.
+ * Both calls are capturable into a CUDA graph. */
+int osb_ext_wrapper_step(int N, int time_limit, const unsigned char* terminated, const unsigned char* truncated,
+                         int* steps, unsigned char* trunc_out, unsigned char* done, int* done_total, void* stream);
+int osb_ext_observe_wrapped(int O, int N, int T, int t, int obs_normalize, const float* step_obs, const float* rew,
+                            const float* cost, const unsigned char* terminated, const unsigned char* truncated,
+                            const float* reset_obs, const unsigned char* done, float* s_raw, float* final_raw,
+                            float* ep_ret, float* ep_cost, int* ep_len, float* norm_mean, float* norm_sumsq,
+                            float* norm_std, float* norm_mean1, float* norm_std1, long long* norm_count, int* had_fin,
+                            unsigned* ticket, float* rew_slab, float* cost_slab, unsigned char* flags, float* epfin,
+                            double* workspace, int* nonfinite, void* stream);
 /* CUDA-graph capture of the external-env epoch (for envs whose step is itself capturable).
  * osb_ext_prepare performs every one-time host action of osb_ext_act / osb_ext_act_graph for these dimensions
  * (kernel attributes, the tensor-core accumulator image at its final size); call it before capturing.  An act launch on

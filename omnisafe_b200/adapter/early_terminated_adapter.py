@@ -56,6 +56,12 @@ class ExternalEarlyTerminatedAdapter(_CostLimit, ExternalEnvAdapter):
                 "reference's reward statistics take the env's reward where the rule stores 0, which the post-rollout "
                 'normalisation of the reward slab cannot reproduce')
         super().__init__(env_id, num_envs, seed, cfgs, device=device, env_id_offset=env_id_offset)
+        if self._time_limit is not None:
+            name = type(self._env).__name__
+            self._env.close()
+            raise NotImplementedError(
+                f'EarlyTerminated is not supported on {name}, which declares need_time_limit_wrapper / '
+                "need_auto_reset_wrapper: combining the cost limit's reset with AutoReset is not implemented")
         self._hook = callable(getattr(self._env, 'reset_envs', None))
         N = self._num_envs
         if not self._hook and N > 1:
@@ -67,7 +73,6 @@ class ExternalEarlyTerminatedAdapter(_CostLimit, ExternalEnvAdapter):
                 '(early_terminated_adapter.py: num_envs == 1)')
         self._trig = torch.zeros(N, dtype=torch.bool, device=self._device)   # envs the rule cut in the last step
         self._rst_ptr = 0                               # storage of the last reset_envs() output (part of the graph key)
-        self._why_eager = None
         if not self._hook:
             self._trig_total = torch.zeros(1, dtype=torch.int32, device=self._device)
             self._trig_host = torch.zeros(1, dtype=torch.int32).pin_memory()
@@ -76,11 +81,6 @@ class ExternalEarlyTerminatedAdapter(_CostLimit, ExternalEnvAdapter):
                 self._why_eager = (f'{type(self._env).__name__} is graph_safe but has no reset_envs(mask): the cost '
                                    'limit reads a trigger word back after every step and calls env.reset(), so every '
                                    'epoch runs eagerly')
-
-    def rollout(self, steps_per_epoch: int, agent, buffer, logger=None, eps=None) -> None:
-        if logger is not None and self._why_eager and not self._mode_logged:
-            logger.log(self._why_eager)
-        super().rollout(steps_per_epoch, agent, buffer, logger, eps=eps)
 
     def _observe(self, T: int, t: int, d, step_ptrs: tuple, s: int, env_dev) -> None:
         L, N, O = lib(), self._num_envs, self._obs_dim

@@ -13,6 +13,13 @@ statistics and feeds the observation normaliser.  Nothing in the loop synchronis
 (and, for an env on the CPU, the copy of the action to it).  A non-finite observation raises `OsbError` at the end of
 the epoch.
 
+An env that declares need_time_limit_wrapper / need_auto_reset_wrapper (envs/core.py) gets TimeLimit and AutoReset on
+the device (online_adapter.py:L120-131): after env.step, osb_ext_wrapper_step counts each env's steps, replaces the
+truncation at the limit and writes the mask of the done envs; they are reset (env.reset_envs(mask), or at one env
+without the hook env.reset() after a 4-byte read-back) and osb_ext_observe_wrapped takes the step's rows as the final
+observations and the reset rows as the next ones, pushing both in the step's ObsNormalize batches as AutoReset inside
+ObsNormalize does.  The epoch-start env.reset() clears the step counters, as TimeLimit.reset does.
+
 For an env that declares `graph_safe` (envs/core.py) the loop from osb_ext_act(0) to osb_ext_act(T) is captured into
 one CUDA graph in the second epoch and replayed from then on (the first epoch the adapter runs -- also the first one
 after `load_train_state` in a resumed process -- is eager and warms everything up); the
@@ -29,7 +36,7 @@ import torch
 from omnisafe_b200._lib import OsbError, current_stream, lib, ptr
 from omnisafe_b200.adapter.onpolicy_adapter import episode_state, load_episode_state
 from omnisafe_b200.common.normalizer import Normalizer, ScalarNormalizer
-from omnisafe_b200.envs.core import check_env, make
+from omnisafe_b200.envs.core import check_env, make, wrapper_time_limit
 from omnisafe_b200.utils.train_state import restore, snapshot
 
 
@@ -39,12 +46,15 @@ def device_rows(x, n: int, device, width: int | None = None, dtype=torch.float32
     return torch.as_tensor(x).to(device=device, dtype=dtype).reshape(shape).contiguous()
 
 
-def step_rows(env, action, n: int, width: int, device, capture: bool = False) -> tuple:
+def step_rows(env, action, n: int, width: int, device, capture: bool = False, finals: bool = True) -> tuple:
     """env.step(action) as contiguous device rows for the observe launches: (next obs, reward, cost, terminated,
-    truncated, final obs, final mask), the last two None when the step reports no final observation."""
+    truncated, final obs, final mask), the last two None when the step reports no final observation or `finals` is
+    false (an env behind the wrappers, whose step rows are its final rows)."""
     nobs, rew, cost, term, trunc, info = env.step(action)
     nobs, rew, cost = device_rows(nobs, n, device, width), device_rows(rew, n, device), device_rows(cost, n, device)
     term, trunc = device_rows(term, n, device, dtype=torch.uint8), device_rows(trunc, n, device, dtype=torch.uint8)
+    if not finals:
+        return nobs, rew, cost, term, trunc, None, None
     if capture and ('final_observation' not in info or '_final_observation' not in info):
         raise OsbError(f'{type(env).__name__} is graph_safe but its step info lacks final_observation / '
                        '_final_observation: a captured step must report them on every step')
@@ -65,8 +75,21 @@ class ExternalEnvAdapter:
         env_cfgs = dict(env_cfgs.todict() if hasattr(env_cfgs, 'todict') else env_cfgs)
         env_cfgs.pop('env_id_offset', None)
         self._env = make(env_id, num_envs=num_envs, device=self._device, **env_cfgs)
-        self._obs_dim, self._act_dim, lo, hi = check_env(self._env)
+        self._obs_dim, self._act_dim, lo, hi = check_env(self._env, wrappers=True)
         self._num_envs = int(num_envs)
+        try:
+            self._time_limit = wrapper_time_limit(self._env)   # None: the env truncates and resets itself
+        except (NotImplementedError, AssertionError):
+            self._env.close()
+            raise
+        self._reset_hook = callable(getattr(self._env, 'reset_envs', None))
+        if self._time_limit is not None and not self._reset_hook and self._num_envs > 1:
+            name = type(self._env).__name__
+            self._env.close()
+            raise NotImplementedError(
+                f'{name} declares need_auto_reset_wrapper and runs {num_envs} envs: resetting the done envs needs the '
+                'optional reset_envs(mask) hook (envs/core.py); without it only a single env is supported, as upstream '
+                '(AutoReset: num_envs == 1)')
         self._env.set_seed(seed)                      # per-rank seed, as OnlineAdapter does (online_adapter.py:L81)
         self._env_id_offset = int(env_id_offset)
         algo = cfgs.algo_cfgs
@@ -105,6 +128,20 @@ class ExternalEnvAdapter:
         self._epoch_dev = torch.zeros(1, dtype=torch.int32, device=dev)    # u32 Philox epoch counter of the replays
         self._obs0 = torch.zeros(N, O, **f32)           # static copy of env.reset()'s observation (graph mode)
         self._eps_buf = None                            # static [T, N, A] copy of the parity-mode noise (graph mode)
+        self._why_eager = None                          # logged once when a graph-safe env has to run eagerly
+        if self._time_limit is not None:
+            self._tl_steps = torch.zeros(N, dtype=torch.int32, device=dev)     # TimeLimit's _time, per env
+            self._trunc = torch.zeros(N, dtype=torch.uint8, device=dev)        # the wrapped step's truncated
+            self._done = torch.zeros(N, dtype=torch.bool, device=dev)          # the envs AutoReset resets
+            self._rst_ptr = 0                           # storage of the last reset rows (part of the graph key)
+            if not self._reset_hook:
+                self._done_total = torch.zeros(1, dtype=torch.int32, device=dev)
+                self._done_host = None
+                if self._use_graph:
+                    self._use_graph = False
+                    self._why_eager = (f'{type(self._env).__name__} is graph_safe but has no reset_envs(mask): '
+                                       'AutoReset reads a done word back after every step and calls env.reset(), so '
+                                       'every epoch runs eagerly')
 
     @property
     def env(self):
@@ -163,14 +200,38 @@ class ExternalEnvAdapter:
             action = self.act_env.to(env_dev, copy=True)
             if N == 1:
                 action = action[0]                  # a single env takes an unbatched action (reference Unsqueeze)
-            rows = step_rows(self._env, action, N, O, self._device, capture)
+            rows = step_rows(self._env, action, N, O, self._device, capture, finals=self._time_limit is None)
             self._observe(T, t, d, tuple(ptr(r) for r in rows), s, env_dev)
         self._act(agent, d, T, T, None, s, epoch_dev)
 
     def _observe(self, T: int, t: int, d, step_ptrs: tuple, s: int, env_dev) -> None:
         """The observe launch of step t; step_ptrs = (next obs, reward, cost, terminated, truncated, final obs, final
-        mask) as device pointers."""
-        lib().osb_ext_observe(*self._observe_args(T, t, d, step_ptrs), s)
+        mask) as device pointers.  Behind the wrappers: the wrapper step, the reset of the done envs, then the
+        wrapped observe."""
+        L = lib()
+        if self._time_limit is None:
+            L.osb_ext_observe(*self._observe_args(T, t, d, step_ptrs), s)
+            return
+        N, O = self._num_envs, self._obs_dim
+        nobs, rew, cost, term, trunc = step_ptrs[:5]
+        total = 0 if self._reset_hook else ptr(self._done_total)
+        L.osb_ext_wrapper_step(N, self._time_limit, term, trunc, ptr(self._tl_steps), ptr(self._trunc), ptr(self._done),
+                               total, s)
+        if self._reset_hook:
+            obs = self._env.reset_envs(self._done.to(env_dev))
+        else:
+            if self._done_host is None:
+                self._done_host = torch.zeros(1, dtype=torch.int32).pin_memory()
+            self._done_host.copy_(self._done_total, non_blocking=True)
+            torch.cuda.current_stream().synchronize()
+            obs = self._env.reset()[0] if int(self._done_host[0]) else None
+        rst = 0
+        if obs is not None:
+            obs = device_rows(obs, N, self._device, O)
+            self._rst_ptr = obs.untyped_storage().data_ptr()
+            rst = ptr(obs)
+        rows = (nobs, rew, cost, term, ptr(self._trunc), rst, ptr(self._done))
+        L.osb_ext_observe_wrapped(*self._observe_args(T, t, d, rows), s)
 
     def _observe_args(self, T: int, t: int, d, step_ptrs: tuple) -> tuple:
         return (self._obs_dim, self._num_envs, T, t, int(self._obs_normalize), *step_ptrs, ptr(self.s_raw),
@@ -179,8 +240,9 @@ class ExternalEnvAdapter:
 
     def _graph_key(self, T: int, agent, d, eps, reset_obs) -> tuple:
         """The device pointers (and shape) a captured epoch bakes in; a change of any of them forces a recapture."""
-        return (T, ptr(agent.theta), tuple(ptr(v) for v in d.values() if v is not None), ptr(eps),
-                tuple(self._norm_ptrs()), torch.as_tensor(reset_obs).untyped_storage().data_ptr())
+        key = (T, ptr(agent.theta), tuple(ptr(v) for v in d.values() if v is not None), ptr(eps),
+               tuple(self._norm_ptrs()), torch.as_tensor(reset_obs).untyped_storage().data_ptr())
+        return key if self._time_limit is None else (*key, self._rst_ptr)
 
     def _capture(self, T: int, agent, d, eps, env_dev) -> None:
         """Capture the T steps, the epoch-end act and the Philox epoch advance into one CUDA graph."""
@@ -207,10 +269,14 @@ class ExternalEnvAdapter:
         if eps is not None:
             assert eps.shape == (T, N, A) and eps.dtype == torch.float32
         if logger is not None and not self._mode_logged:
+            if self._why_eager:
+                logger.log(self._why_eager)
             logger.log(f'{type(self._env).__name__}: external-env rollout in {self.graph_mode} mode')
             self._mode_logged = True
         L, d, s = lib(), buffer.data, current_stream()
         obs, _ = self._env.reset()
+        if self._time_limit is not None:
+            self._tl_steps.zero_()                  # TimeLimit.reset
         env_dev = torch.as_tensor(obs).device
         if self._use_graph and env_dev.type != 'cuda':
             raise ValueError(f'{type(self._env).__name__} declares graph_safe but reset() returned observations on {env_dev}')

@@ -1380,10 +1380,16 @@ __device__ __forceinline__ void ext_fold_push(const double* part, NormState ns, 
 // leaves the accumulator alone.  trig_total, when not null, receives the number of triggered envs (zeroed by the host
 // before the launch).  The observation rows are those env.step returned, so ObsNormalize pushes the env's own final rows
 // and then every next row, a triggered env that did not end contributing its pre-reset state.
-template <bool EARLY>
+//
+// WRAP: the step of an env behind TimeLimit / AutoReset (wrapper.py), after ext_wrapper_step_kernel and the reset of the
+// done envs.  The launcher passes the step's own rows as both next_obs and final_obs, the done mask as final_mask and
+// the wrapper's truncated as trunc; the next row of a done env comes from reset_obs instead.  So a done env's final row
+// is its step row, and set A of the push is the next rows as they land in the state buffer: AutoReset's reset row sits
+// inside ObsNormalize, in the same batch as every other env's next row.
+template <bool EARLY, bool WRAP = false>
 __device__ __forceinline__ void ext_observe_step(ExtObs x, EnvState st, NormState ns, Slabs sl, int O, int N, int T, int t,
                                                  int obs_normalize, int is_reset, EarlySpec et, uint8_t* trig,
-                                                 int* trig_total) {
+                                                 int* trig_total, const float* reset_obs = nullptr) {
     __shared__ int sFin[XT];
     __shared__ int s_bad;
     const int tid = threadIdx.x, env0 = blockIdx.x * XT, rows = min(XT, N - env0);
@@ -1421,13 +1427,25 @@ __device__ __forceinline__ void ext_observe_step(ExtObs x, EnvState st, NormStat
     for (int i = tid; i < rows * O; i += NTHREADS) {
         const int r = i / O;
         const size_t g = (size_t)env0 * O + i;
-        const float v = x.next_obs[g];
-        bad |= !isfinite(v);
-        s_nxt[g] = v;
-        if (sFin[r]) {
-            const float f = x.final_obs[g];
+        if constexpr (WRAP) {
+            const float f = x.next_obs[g];
             bad |= !isfinite(f);
-            fin_out[g] = f;
+            float v = f;
+            if (sFin[r]) {
+                fin_out[g] = f;
+                v = reset_obs[g];
+                bad |= !isfinite(v);
+            }
+            s_nxt[g] = v;
+        } else {
+            const float v = x.next_obs[g];
+            bad |= !isfinite(v);
+            s_nxt[g] = v;
+            if (sFin[r]) {
+                const float f = x.final_obs[g];
+                bad |= !isfinite(f);
+                fin_out[g] = f;
+            }
         }
     }
     if (bad) s_bad = 1;
@@ -1436,9 +1454,10 @@ __device__ __forceinline__ void ext_observe_step(ExtObs x, EnvState st, NormStat
         if (tid == 0 && s_bad) *x.nonfinite = 1;
         return;
     }
+    if constexpr (WRAP) __syncthreads();       // set A is read back from the state buffer the tile just wrote
     // set A: every next row; set B: the final rows
-    const bool last = ext_tile_moments<true, true>(x.part, x.next_obs, nullptr, x.final_obs, sFin, O, env0, rows, true,
-                                                   ns.ticket);
+    const bool last = ext_tile_moments<true, true>(x.part, WRAP ? s_nxt : x.next_obs, nullptr, x.final_obs, sFin, O, env0,
+                                                   rows, true, ns.ticket);
     if (tid == 0 && s_bad) *x.nonfinite = 1;
     if (last) ext_fold_push<true, true>(x.part, ns, O, N, true);
 }
@@ -1452,6 +1471,33 @@ __global__ void __launch_bounds__(NTHREADS) ext_observe_early_kernel(ExtObs x, E
                                                                      int O, int N, int T, int t, int obs_normalize,
                                                                      EarlySpec et, uint8_t* trig, int* trig_total) {
     ext_observe_step<true>(x, st, ns, sl, O, N, T, t, obs_normalize, 0, et, trig, trig_total);
+}
+
+__global__ void __launch_bounds__(NTHREADS) ext_observe_wrapped_kernel(ExtObs x, EnvState st, NormState ns, Slabs sl,
+                                                                       int O, int N, int T, int t, int obs_normalize,
+                                                                       const float* __restrict__ reset_obs) {
+    ext_observe_step<false, true>(x, st, ns, sl, O, N, T, t, obs_normalize, 0, EarlySpec{nullptr, 0.f}, nullptr, nullptr,
+                                  reset_obs);
+}
+
+// TimeLimit and AutoReset (wrapper.py) around env.step for the envs of a wrapped user env, one thread per env.  steps[env]
+// is TimeLimit's _time: incremented by the step, cleared where the env is done (AutoReset's reset goes through
+// TimeLimit.reset).  With time_limit > 0 the step's truncated is steps >= time_limit, replacing the env's own flag;
+// with 0 (no TimeLimit) it is the env's flag.  done[env] = terminated | truncated: the envs to reset before the observe
+// launch.  done_total, when not null, receives the number of done envs (zeroed by the host before the launch).
+__global__ void __launch_bounds__(256) ext_wrapper_step_kernel(const uint8_t* __restrict__ term,
+                                                               const uint8_t* __restrict__ env_trunc, int* steps,
+                                                               uint8_t* trunc, uint8_t* done, int* done_total, int N,
+                                                               int time_limit) {
+    const int env = blockIdx.x * blockDim.x + threadIdx.x;
+    if (env >= N) return;
+    const int k = steps[env] + 1;
+    const bool tr = time_limit > 0 ? k >= time_limit : env_trunc[env] != 0;
+    const bool d = tr || term[env] != 0;
+    steps[env] = d ? 0 : k;
+    trunc[env] = tr ? 1 : 0;
+    done[env] = d ? 1 : 0;
+    if (d && done_total) atomicAdd(done_total, 1);
 }
 
 // The reset observations of the envs the cost rule cut at step t (rows of obs where mask is set; the others are ignored)
@@ -1500,10 +1546,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) ext_reset_rows_kernel(const float
 // and a reset ingest clears it.  RST: rst[env] (one byte per env, written on every launch) is 1 where the cost rule ended
 // a running env's episode that the env itself did not end, and the env has episodes left: the envs the caller resets
 // through reset_envs(mask) before ext_reset_rows_kernel ingests their rows.
-template <bool RST>
+//
+// WRAP (with RST): an env that declares the TimeLimit / AutoReset wrappers, which the evaluation never auto-resets
+// (evaluator.py: TimeLimit(time_limit) only, the loop resets).  tl_steps[env] is TimeLimit's _time, cleared at each
+// episode end; with tl_limit > 0 a step truncates at tl_steps >= tl_limit instead of by the env's flag.  rst[env] is 1
+// for every episode end with episodes left, and the launcher passes no final rows: a step's rows are the env's own.
+template <bool RST, bool WRAP = false>
 __device__ __forceinline__ void ext_eval_observe_step(ExtObs x, EnvState st, NormState ns, SauteSpec sa, EvalSpec ev,
                                                       int O, int N, int t, int obs_normalize, int is_reset,
-                                                      uint8_t* rst_out) {
+                                                      uint8_t* rst_out, int* tl_steps = nullptr, int tl_limit = 0) {
     __shared__ int sRun[XT], sFin[XT];
     __shared__ int s_bad;
     const int tid = threadIdx.x, env0 = blockIdx.x * XT, rows = min(XT, N - env0);
@@ -1519,11 +1570,23 @@ __device__ __forceinline__ void ext_eval_observe_step(ExtObs x, EnvState st, Nor
                 const int len = ev.len[env];
                 const double r64 = ev.ret[env] + (double)rew;
                 const double c64 = ev.cost[env] + pow(ev.crit, (double)len) * (double)cst;
-                const bool env_done = x.term[env] != 0 || x.trunc[env] != 0;
+                bool env_done;
+                if constexpr (WRAP) {
+                    const int k = tl_steps[env] + 1;
+                    env_done = x.term[env] != 0 || (tl_limit > 0 ? k >= tl_limit : x.trunc[env] != 0);
+                    tl_steps[env] = k;
+                } else {
+                    env_done = x.term[env] != 0 || x.trunc[env] != 0;
+                }
                 const bool done = env_done || (ev.early && c64 >= ev.cost_limit);
                 if (sa.safety) saute_step(sa, t, N, env, rew, cst, done);
                 const int left = ev.left[env];
-                if constexpr (RST) cut = (done && !env_done && left > 1) ? 1 : 0;
+                if constexpr (WRAP) {
+                    cut = (done && left > 1) ? 1 : 0;
+                    if (done) tl_steps[env] = 0;
+                } else if constexpr (RST) {
+                    cut = (done && !env_done && left > 1) ? 1 : 0;
+                }
                 if (done) {
                     const int k = ev.done_eps[env];
                     const size_t out = (size_t)env + (size_t)k * N;
@@ -1584,6 +1647,13 @@ __global__ void __launch_bounds__(NTHREADS) ext_eval_observe_rst_kernel(ExtObs x
                                                                         SauteSpec sa, EvalSpec ev, int O, int N, int t,
                                                                         int obs_normalize, uint8_t* rst) {
     ext_eval_observe_step<true>(x, st, ns, sa, ev, O, N, t, obs_normalize, 0, rst);
+}
+
+__global__ void __launch_bounds__(NTHREADS) ext_eval_observe_wrapped_kernel(ExtObs x, EnvState st, NormState ns,
+                                                                            SauteSpec sa, EvalSpec ev, int O, int N,
+                                                                            int t, int obs_normalize, uint8_t* rst,
+                                                                            int* tl_steps, int tl_limit) {
+    ext_eval_observe_step<true, true>(x, st, ns, sa, ev, O, N, t, obs_normalize, 0, rst, tl_steps, tl_limit);
 }
 
 // Window of the last <= W finished episodes in (step, env) append order: Logger deque semantics
@@ -2027,7 +2097,7 @@ static int eval_ext_observe(int O, int N, int t, int obs_normalize, int is_reset
                             float safety_budget, float saute_gamma, int early, double cost_limit, double cost_criteria,
                             int* left, int* done_eps, double* ret, double* cost_acc, int* len, int* ctr,
                             double* out_ret, double* out_cost, int* out_len, double* workspace, int* nonfinite,
-                            unsigned char* rst, void* stream) {
+                            unsigned char* rst, int* tl_steps, int tl_limit, void* stream) {
     OSB_CHECK_ARG(O > 0 && N > 0 && t >= -1, "bad dims / step index");
     OSB_CHECK_ARG(next_obs && s_raw && norm_mean && norm_sumsq && norm_std && norm_count && ticket && left && ctr &&
                   workspace && nonfinite, "bad argument");
@@ -2041,7 +2111,11 @@ static int eval_ext_observe(int O, int N, int t, int obs_normalize, int is_reset
     EvalSpec ev{left, done_eps, ret, cost_acc, len, out_ret, out_cost, out_len, nullptr, ctr, cost_criteria, cost_limit,
                 early, N == 1 ? 1 : 0, nullptr};
     const int grid = (N + XT - 1) / XT;
-    if (rst)
+    if (tl_steps)
+        ext_eval_observe_wrapped_kernel<<<grid, NTHREADS, 0, (cudaStream_t)stream>>>(x, st, ns, sa, ev, O, N, t,
+                                                                                     obs_normalize, rst, tl_steps,
+                                                                                     tl_limit);
+    else if (rst)
         ext_eval_observe_rst_kernel<<<grid, NTHREADS, 0, (cudaStream_t)stream>>>(x, st, ns, sa, ev, O, N, t,
                                                                                  obs_normalize, rst);
     else
@@ -2061,7 +2135,7 @@ int osb_eval_ext_observe(int O, int N, int t, int obs_normalize, int is_reset, c
     return eval_ext_observe(O, N, t, obs_normalize, is_reset, next_obs, rew, cost, terminated, truncated, final_obs,
                             final_mask, s_raw, norm_mean, norm_sumsq, norm_std, norm_count, ticket, safety,
                             safety_budget, saute_gamma, early, cost_limit, cost_criteria, left, done_eps, ret, cost_acc,
-                            len, ctr, out_ret, out_cost, out_len, workspace, nonfinite, nullptr, stream);
+                            len, ctr, out_ret, out_cost, out_len, workspace, nonfinite, nullptr, nullptr, 0, stream);
 }
 
 // osb_eval_ext_observe of a step (no reset ingest) that also writes rst[N], the envs the cost rule cut with episodes left
@@ -2078,7 +2152,25 @@ int osb_eval_ext_observe_rst(int O, int N, int t, int obs_normalize, const float
     return eval_ext_observe(O, N, t, obs_normalize, 0, next_obs, rew, cost, terminated, truncated, final_obs,
                             final_mask, s_raw, norm_mean, norm_sumsq, norm_std, norm_count, ticket, safety,
                             safety_budget, saute_gamma, early, cost_limit, cost_criteria, left, done_eps, ret, cost_acc,
-                            len, ctr, out_ret, out_cost, out_len, workspace, nonfinite, rst, stream);
+                            len, ctr, out_ret, out_cost, out_len, workspace, nonfinite, rst, nullptr, 0, stream);
+}
+
+// osb_eval_ext_observe_rst of a step on an env behind TimeLimit / AutoReset: tl_steps[N] is the TimeLimit step counter
+// (time_limit > 0) and rst[N] flags every episode end with episodes left; final_obs / final_mask are not read.
+int osb_eval_ext_observe_wrapped(int O, int N, int t, int obs_normalize, const float* next_obs, const float* rew,
+                                 const float* cost, const unsigned char* terminated, const unsigned char* truncated,
+                                 float* s_raw, float* norm_mean, float* norm_sumsq, float* norm_std,
+                                 long long* norm_count, unsigned* ticket, float* safety, float safety_budget,
+                                 float saute_gamma, int early, double cost_limit, double cost_criteria, int* left,
+                                 int* done_eps, double* ret, double* cost_acc, int* len, int* ctr, double* out_ret,
+                                 double* out_cost, int* out_len, double* workspace, int* nonfinite, unsigned char* rst,
+                                 int* tl_steps, int time_limit, void* stream) {
+    OSB_CHECK_ARG(t >= 0 && time_limit >= 0, "bad dims / step index / time limit");
+    OSB_CHECK_ARG(rst && tl_steps, "bad argument");
+    return eval_ext_observe(O, N, t, obs_normalize, 0, next_obs, rew, cost, terminated, truncated, nullptr, nullptr,
+                            s_raw, norm_mean, norm_sumsq, norm_std, norm_count, ticket, safety, safety_budget,
+                            saute_gamma, early, cost_limit, cost_criteria, left, done_eps, ret, cost_acc, len, ctr,
+                            out_ret, out_cost, out_len, workspace, nonfinite, rst, tl_steps, time_limit, stream);
 }
 
 // ---- external envs ---------------------------------------------------------------------------
@@ -2138,6 +2230,39 @@ int osb_ext_observe_early(int O, int N, int T, int t, int obs_normalize, const f
     Slabs sl{nullptr, nullptr, nullptr, rew_slab, cost_slab, nullptr, nullptr, nullptr, nullptr, flags, epfin};
     ext_observe_early_kernel<<<(N + XT - 1) / XT, NTHREADS, 0, s>>>(x, st, ns, sl, O, N, T, t, obs_normalize,
                                                                     EarlySpec{cost_acc, cost_limit}, trig, trig_total);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}
+
+int osb_ext_wrapper_step(int N, int time_limit, const unsigned char* terminated, const unsigned char* truncated,
+                         int* steps, unsigned char* trunc_out, unsigned char* done, int* done_total, void* stream) {
+    OSB_CHECK_ARG(N > 0 && time_limit >= 0, "bad dims / time limit");
+    OSB_CHECK_ARG(terminated && truncated && steps && trunc_out && done, "bad argument");
+    cudaStream_t s = (cudaStream_t)stream;
+    if (done_total) OSB_CUDA(cudaMemsetAsync(done_total, 0, sizeof(int), s));
+    ext_wrapper_step_kernel<<<(N + 255) / 256, 256, 0, s>>>(terminated, truncated, steps, trunc_out, done, done_total, N,
+                                                            time_limit);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}
+
+int osb_ext_observe_wrapped(int O, int N, int T, int t, int obs_normalize, const float* step_obs, const float* rew,
+                            const float* cost, const unsigned char* terminated, const unsigned char* truncated,
+                            const float* reset_obs, const unsigned char* done, float* s_raw, float* final_raw,
+                            float* ep_ret, float* ep_cost, int* ep_len, float* norm_mean, float* norm_sumsq,
+                            float* norm_std, float* norm_mean1, float* norm_std1, long long* norm_count, int* had_fin,
+                            unsigned* ticket, float* rew_slab, float* cost_slab, unsigned char* flags, float* epfin,
+                            double* workspace, int* nonfinite, void* stream) {
+    OSB_CHECK_ARG(O > 0 && N > 0 && T > 0 && t >= 0 && t < T, "bad dims / step index");
+    OSB_CHECK_ARG(step_obs && rew && cost && terminated && truncated && done && s_raw && final_raw && rew_slab &&
+                  cost_slab && flags && epfin && workspace && nonfinite, "bad argument");
+    // the step's rows are the final rows of the done envs: set B of the push, and final_raw for the bootstraps
+    ExtObs x{step_obs, rew, cost, terminated, truncated, step_obs, done, workspace, nonfinite};
+    EnvState st{s_raw, final_raw, nullptr, nullptr, nullptr, ep_ret, ep_cost, ep_len, nullptr};
+    NormState ns{norm_mean, norm_sumsq, norm_std, norm_mean1, norm_std1, norm_count, nullptr, nullptr, nullptr, had_fin, ticket};
+    Slabs sl{nullptr, nullptr, nullptr, rew_slab, cost_slab, nullptr, nullptr, nullptr, nullptr, flags, epfin};
+    ext_observe_wrapped_kernel<<<(N + XT - 1) / XT, NTHREADS, 0, (cudaStream_t)stream>>>(x, st, ns, sl, O, N, T, t,
+                                                                                         obs_normalize, reset_obs);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
 }

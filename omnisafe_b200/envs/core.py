@@ -5,7 +5,8 @@ against the reference `CMDP` also works here.  Such an env is stepped in PyTorch
 (adapter/external_adapter.py); the policy step and everything after it stays on the CUDA kernels.
 
 The env keeps the reference's multi-env contract (online_adapter.py:L52-140): `reset() -> (obs[N, O], info)`,
-`step(action[N, A]) -> (obs, reward[N], cost[N], terminated[N], truncated[N], info)`, it auto-resets finished envs
+`step(action[N, A]) -> (obs, reward[N], cost[N], terminated[N], truncated[N], info)`, unless it declares the wrappers
+(below) it auto-resets finished envs
 itself and reports their last observation in `info['final_observation']` (rows selected by the boolean
 `info['_final_observation']`; when that mask is absent every finished row is taken).  With `num_envs == 1` unbatched
 tensors are accepted, as the reference's `Unsqueeze` wrapper does.  Tensors may live on the CPU or on any CUDA device.
@@ -20,7 +21,7 @@ epoch, which removes the host's per-launch cost.  Such an env promises:
 - `step` does not synchronise with the host, has no data-dependent Python control flow and keeps no host-side state
   (RNG, counters) that must advance from step to step: it runs once per step at capture, never at replay;
 - `info` holds `final_observation` and `_final_observation` on every step (the mask all false when nothing finished),
-  so its structure is the same on every step;
+  so its structure is the same on every step; an env that declares the wrappers (below) need not report them;
 - the tensors `step` returns may be fresh each call: the adapter copies them inside the graph.
 
 An env may define `reset_envs(mask) -> obs` (optional, an omnisafe_b200 extension): a reset of some envs only.  `mask` is
@@ -30,6 +31,19 @@ N = 1, `reset_envs(tensor([True]))` is equivalent to `reset()`.  For a `graph_sa
 `step` is: no host synchronisation, and the same output storage on every call.  The EarlyTerminated algorithms use it to
 reset the envs the cost limit cuts: with it they run any number of envs (a graph-safe env keeps its epoch in the CUDA
 graph); without it they run a single env only, as upstream does, resetting it through `reset()` and eagerly.
+
+An env may declare `need_time_limit_wrapper` / `need_auto_reset_wrapper`, as upstream's custom envs do.  It then does
+not truncate at a time limit or reset itself: the adapter applies TimeLimit and AutoReset (envs/wrapper.py upstream) on
+the device, one step counter per env.  `reset_envs` must not write into the tensors the step just returned (they are read
+after it).  TimeLimit truncates at `max_episode_steps` (which it then requires) and replaces
+the env's own `truncated`; AutoReset resets every env that terminated or truncated, whose step observation becomes the
+final observation (any `final_observation` in `info` is ignored).  The reset goes through `reset_envs(mask)` with the
+device mask of the done envs, after every step and without a host synchronisation, so any number of envs works and a
+`graph_safe` env keeps its epoch in the CUDA graph; such an env need not report `final_observation` in `info`.  Without
+the hook only a single env works, as upstream: the adapter reads back one 4-byte word per step, calls `reset()` when the
+env is done, and runs eagerly.  TimeLimit without AutoReset is refused, as are EarlyTerminated algorithms on such envs.
+`Evaluator` applies TimeLimit(1000) and never AutoReset, resetting finished episodes itself (`reset()` at one env,
+`reset_envs(mask)` at more).
 
 An env may also define `state_dict() -> dict` and `load_state_dict(sd)` (optional, an omnisafe_b200 extension).  When it
 does, a saved training state (`AlgoWrapper.save_state`, `learn(save_state_freq=...)`) holds what `state_dict()` returns and
@@ -197,10 +211,39 @@ def make(env_id: str, num_envs: int = 1, device='cpu', class_name: str | None = 
     return cls(env_id, num_envs=num_envs, device=device, **env_cfgs)
 
 
-def check_env(env) -> tuple[int, int, np.ndarray, np.ndarray]:
-    """Refuse what the external-env rollout cannot run; returns (obs_dim, act_dim, act_low, act_high)."""
+def needs_wrappers(env) -> bool:
+    """Whether the env declares need_time_limit_wrapper or need_auto_reset_wrapper."""
+    return bool(getattr(env, 'need_time_limit_wrapper', False) or getattr(env, 'need_auto_reset_wrapper', False))
+
+
+def wrapper_time_limit(env) -> int | None:
+    """The TimeLimit that training applies to the env (online_adapter.py:L120-131): None when the env declares neither
+    wrapper (it truncates and resets itself), 0 for AutoReset alone (the env's own truncation), else
+    `env.max_episode_steps`.  TimeLimit without AutoReset is refused: the reference's rollout then reads a final
+    observation that nothing provides."""
+    if not needs_wrappers(env):
+        return None
     name = type(env).__name__
-    if getattr(env, 'need_time_limit_wrapper', False) or getattr(env, 'need_auto_reset_wrapper', False):
+    if not getattr(env, 'need_auto_reset_wrapper', False):
+        raise NotImplementedError(
+            f'{name} declares need_time_limit_wrapper without need_auto_reset_wrapper: at the time limit the episode is '
+            'truncated but nothing resets the env or reports its final observation, which the rollout bootstraps from '
+            "(the reference's rollout fails the same way); declare need_auto_reset_wrapper as well")
+    if not getattr(env, 'need_time_limit_wrapper', False):
+        return 0
+    limit = env.max_episode_steps
+    if not limit:
+        raise AssertionError('You must define max_episode_steps as an integer                \nor cancel the use of the '
+                             'time_limit wrapper.')
+    return int(limit)
+
+
+def check_env(env, wrappers: bool = False) -> tuple[int, int, np.ndarray, np.ndarray]:
+    """Refuse what the external-env rollout cannot run; returns (obs_dim, act_dim, act_low, act_high).  An env that
+    declares the TimeLimit / AutoReset wrappers is refused unless `wrappers` (the adapters and `Evaluator`, which
+    apply them on the device)."""
+    name = type(env).__name__
+    if needs_wrappers(env) and not wrappers:
         raise ValueError(f'{name} declares need_time_limit_wrapper / need_auto_reset_wrapper: the env must truncate and '
                          'auto-reset itself (reporting info["final_observation"]); the wrappers are not provided')
     spaces = {}

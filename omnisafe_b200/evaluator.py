@@ -15,14 +15,19 @@ a CUDA graph and reads the 4-byte done word once per block, OSB_NO_GRAPH=1 keeps
 - return and cost are fp64 sums: ep_ret += reward, ep_cost += cost_criteria ** length * cost;
 - Saute / Simmer runs: the network input ends with z, 1 at every episode start, z <- (z - cost / b) / saute_gamma with
   b the per-step budget of algo_cfgs.safety_budget; the reward is not replaced;
-- EarlyTerminated runs: an episode also ends once ep_cost >= cost_limit.
+- EarlyTerminated runs: an episode also ends once ep_cost >= cost_limit;
+- an env that declares need_time_limit_wrapper is truncated after 1000 steps, its own truncation discarded
+  (TimeLimit(time_limit=1000), evaluator.py:L179-180); AutoReset is never applied, so such an env, like one that
+  declares need_auto_reset_wrapper, does not reset itself and every episode end is reset by the evaluation.
 
 One extension: `evaluate(num_envs=E)` runs E envs at once, env e playing episodes e, e + E, ...; results still come
 back in episode order.  E changes the order in which rows reach the normaliser, and so the results: E = 1 (the default)
 is the reference.  With E > 1 the envs reset themselves at their episode ends, and an episode cut by the cost rule
 resets its env: on the synthetic env inside the kernels, on a registered env through its optional `reset_envs(mask)`
 hook (envs/core.py; without it the cost rule needs E = 1).  Each step pushes the rows of the envs still running, in env
-order, then the reset rows of the envs the rule cut that have episodes left.
+order, then the reset rows of the envs the rule cut that have episodes left.  An env that declares either wrapper
+resets every finished env with episodes left through `reset_envs(mask)` (osb_eval_ext_observe_wrapped), so at E > 1 it
+needs the hook.
 
 The evaluator builds its own env state, normaliser and parameters; a live run's are never touched.
 """
@@ -38,12 +43,13 @@ from omnisafe_b200._lib import OsbError, current_stream, lib, ptr
 from omnisafe_b200.adapter.external_adapter import device_rows, step_rows
 from omnisafe_b200.adapter.saute_adapter import per_step_budget
 from omnisafe_b200.common.normalizer import Normalizer
-from omnisafe_b200.envs.core import check_env, is_registered, make
+from omnisafe_b200.envs.core import check_env, is_registered, make, needs_wrappers
 from omnisafe_b200.envs.synthetic import SyntheticBoxEnv, support_envs
 from omnisafe_b200.models.actor_critic import param_layout
 from omnisafe_b200.utils.config import Config
 
 PRECISIONS = {'fp32': 0, 'tf32': 1, 'bf16x3': 2}
+TIME_LIMIT = 1000   # the TimeLimit the reference's evaluator applies (evaluator.py:L179-180)
 GRAPH_BLOCK = 16    # steps per captured block of a graph-safe registered env (even: t enters only by its parity)
 
 
@@ -83,8 +89,10 @@ class Evaluator:
             self._obs_dim, self._act_dim = probe.obs_dim, probe.act_dim
         else:
             probe = make(cfgs.env_id, num_envs=1, device=self._device, **self._env_cfgs)
-            self._obs_dim, self._act_dim, _, _ = check_env(probe)
+            self._obs_dim, self._act_dim, _, _ = check_env(probe, wrappers=True)
             self._reset_envs = callable(getattr(probe, 'reset_envs', None))
+            self._wrapped = needs_wrappers(probe)
+            self._time_limit = TIME_LIMIT if getattr(probe, 'need_time_limit_wrapper', False) else 0
         On, A = self._obs_dim + int(self._saute), self._act_dim
         # the actor's flat parameters in the rollout's layout (the critics are not evaluated)
         layout = param_layout(On, A)
@@ -115,6 +123,11 @@ class Evaluator:
             raise NotImplementedError(
                 f'evaluating EarlyTerminated on {self._cfgs.env_id} with {E} envs needs the optional reset_envs(mask) '
                 'hook (envs/core.py) to reset the envs the cost limit cuts; without it only num_envs=1 is supported')
+        if not self._synthetic and self._wrapped and E > 1 and not self._reset_envs:
+            raise NotImplementedError(
+                f'evaluating {self._cfgs.env_id} with {E} envs needs the optional reset_envs(mask) hook (envs/core.py): '
+                'the env declares need_time_limit_wrapper / need_auto_reset_wrapper, so it does not reset itself and '
+                'the finished envs are reset through the hook; without it only num_envs=1 is supported')
         norm = Normalizer((O,), clip=5.0, device=dev)
         if self._norm_sd is not None:
             norm.load_state_dict(self._norm_sd)
@@ -170,14 +183,17 @@ class Evaluator:
         the done word (read once per block) is 0: steps after the last episode ended change nothing but the env."""
         O, A, dev, L = self._obs_dim, self._act_dim, self._device, lib()
         env = make(self._cfgs.env_id, num_envs=E, device=dev, **self._env_cfgs)   # the env's default seed
-        _, _, lo, hi = check_env(env)
+        _, _, lo, hi = check_env(env, wrappers=True)
         act_lo, act_hi = torch.as_tensor(lo).to(dev), torch.as_tensor(hi).to(dev)
         s_raw = torch.zeros(2, E, O, dtype=torch.float32, device=dev)
         act_env = torch.zeros(E, A, dtype=torch.float32, device=dev)
         ws = torch.zeros(L.osb_eval_ext_workspace_doubles(O, E), dtype=torch.float64, device=dev)
         nonfinite = torch.zeros(1, dtype=torch.int32, device=dev)
-        cut = self._early and E > 1         # envs the cost rule cuts are reset through env.reset_envs(rst)
-        rst = torch.zeros(E, dtype=torch.bool, device=dev) if cut else None
+        wrapped = self._wrapped
+        # envs the cost rule cuts (and behind the wrappers every finished env) are reset through env.reset_envs(rst)
+        cut = (self._early or wrapped) and E > 1
+        rst = torch.zeros(E, dtype=torch.bool, device=dev) if cut or wrapped else None
+        tl_steps = torch.zeros(E, dtype=torch.int32, device=dev) if wrapped else None   # TimeLimit's _time, per env
         graph = E > 1 and bool(getattr(env, 'graph_safe', False)) and not os.getenv('OSB_NO_GRAPH')
         on = int(self._obs_normalize)
         tail = (ptr(s_raw), ptr(norm.mean), ptr(norm.sumsq), ptr(norm.std), ptr(norm.count), ptr(norm.ticket),
@@ -197,12 +213,17 @@ class Evaluator:
                                ptr(w['safety']), ptr(self._theta), ptr(act_lo), ptr(act_hi), ptr(act_env), ptr(w['left']),
                                ptr(w['ctr']), ptr(w['act_out']), self._precision, s)
             action = act_env.clone()
-            rows = step_rows(env, action[0] if E == 1 else action, E, O, dev, capture)
+            rows = step_rows(env, action[0] if E == 1 else action, E, O, dev, capture, finals=not wrapped)
             step_ptrs = tuple(ptr(r) for r in rows)
-            if not cut:
+            if wrapped:
+                L.osb_eval_ext_observe_wrapped(O, E, t, on, *step_ptrs[:5], *tail, ptr(rst), ptr(tl_steps),
+                                               self._time_limit, s)
+            elif cut:
+                L.osb_eval_ext_observe_rst(O, E, t, on, *step_ptrs, *tail, ptr(rst), s)
+            else:
                 L.osb_eval_ext_observe(O, E, t, on, 0, *step_ptrs, *tail, s)
+            if not cut:
                 return
-            L.osb_eval_ext_observe_rst(O, E, t, on, *step_ptrs, *tail, ptr(rst), s)
             obs = device_rows(env.reset_envs(rst.to(env_dev)), E, dev, O)
             L.osb_ext_reset_rows(O, E, t, on, ptr(rst), ptr(obs), ptr(s_raw), ptr(norm.mean), ptr(norm.sumsq),
                                  ptr(norm.std), ptr(norm.count), ptr(norm.ticket), ptr(ws), ptr(nonfinite), s)

@@ -2,6 +2,7 @@
 batch 16384, update_iters 8) on a PyTorch-on-GPU port of the synthetic dynamics registered as a user CMDP.
 
     python tools/external_env_bench.py [--steps K] [--warmup W] [--precision bf16x3|tf32|fp32] [--graph] [--algo NAME]
+                                        [--wrappers]
 
 Every env step is one act launch, the env's own PyTorch kernels and one observe launch.  Prints ONE JSON line:
 env-steps/s over full epochs (rollout + GAE + update, CUDA events), and one rollout split into the device time spent
@@ -9,8 +10,11 @@ inside env.step (CUDA events at its entry and exit) and the rest (act / observe 
 --graph runs the graph-safe TorchBox (same arithmetic, state written in place, no events inside step), whose epoch the
 adapter replays from a CUDA graph; it reports env-steps/s and the rollout time per epoch only.  With OSB_NO_GRAPH=1 the
 same env runs eagerly.  --algo picks the algorithm (default PPOLag); TorchBox has the optional reset_envs(mask) hook, so
-PPOEarlyTerminated runs the cost-limit rule on all 4096 envs (graph-safe TorchBox: inside the replayed graph).  Logs go to
-a temporary directory; nothing is written to the tree.
+PPOEarlyTerminated runs the cost-limit rule on all 4096 envs (graph-safe TorchBox: inside the replayed graph).
+--wrappers runs a TorchBox variant that declares need_time_limit_wrapper and need_auto_reset_wrapper, never truncates or
+resets itself and has reset_envs: the adapter applies TimeLimit(64) and AutoReset on the device, resetting the done envs
+through reset_envs after every step (with --graph inside the replayed graph).  Logs go to a temporary directory; nothing
+is written to the tree.
 """
 from __future__ import annotations
 
@@ -27,6 +31,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 ENV_ID = 'TorchBox-v0'
 GRAPH_ENV_ID = 'TorchBoxGraph-v0'
+WRAPPED_ENV_ID = 'TorchBoxWrapped-v0'
+GRAPH_WRAPPED_ENV_ID = 'TorchBoxWrappedGraph-v0'
 N, T, O, A, TMAX = 4096, 128, 60, 8, 64
 
 
@@ -141,8 +147,57 @@ def register_torch_box() -> None:
             self.s.copy_(torch.where(mask[:, None], self._reset_values(self.episode), self.s))
             return self.s
 
+    class TorchBoxWrapped(TorchBox):
+        """TorchBox behind TimeLimit / AutoReset: the same step without its truncation and reset."""
+        _support_envs = [WRAPPED_ENV_ID]  # noqa: RUF012
+        need_auto_reset_wrapper = need_time_limit_wrapper = True
+
+        @property
+        def max_episode_steps(self):
+            return self.tmax
+
+        def step(self, action):
+            ev = None
+            if self.timing is not None:
+                ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+                ev[0].record()
+            a = action.clamp(-1.0, 1.0)
+            self.s = (0.95 * self.s + 0.1 * a[:, self.idx] + self.bias).clamp(-10.0, 10.0)
+            reward = 1.0 - (self.s * self.s).mean(1)
+            cost = (self.s[:, 0] > 0.0).to(torch.float32)
+            never = torch.zeros(self._num_envs, dtype=torch.bool, device=self.s.device)
+            if ev is not None:
+                ev[1].record()
+                self.timing.append(ev)
+            return self.s, reward, cost, never, never, {}
+
+    class TorchBoxWrappedGraph(TorchBoxGraph):
+        """TorchBoxWrapped for CUDA-graph capture: the state in place, the step's rows in a buffer of their own (the
+        reset of the done envs must not overwrite the rows the step returned)."""
+        _support_envs = [GRAPH_WRAPPED_ENV_ID]  # noqa: RUF012
+        need_auto_reset_wrapper = need_time_limit_wrapper = True
+
+        def __init__(self, env_id, num_envs=1, device='cuda', **kw):
+            super().__init__(env_id, num_envs=num_envs, device=device, **kw)
+            self.out = torch.zeros_like(self.s)
+            self.never = torch.zeros(num_envs, dtype=torch.bool, device=self._device)
+
+        @property
+        def max_episode_steps(self):
+            return self.tmax
+
+        def step(self, action):
+            a = action.clamp(-1.0, 1.0)
+            self.s.copy_((0.95 * self.s + 0.1 * a[:, self.idx] + self.bias).clamp(-10.0, 10.0))
+            self.out.copy_(self.s)
+            reward = 1.0 - (self.s * self.s).mean(1)
+            cost = (self.s[:, 0] > 0.0).to(torch.float32)
+            return self.out, reward, cost, self.never, self.never, {}
+
     env_register(TorchBox)
     env_register(TorchBoxGraph)
+    env_register(TorchBoxWrapped)
+    env_register(TorchBoxWrappedGraph)
 
 
 def timed(fn, k: int) -> float:
@@ -174,11 +229,16 @@ def main() -> None:
     ap.add_argument('--precision', default='bf16x3', choices=['bf16x3', 'tf32', 'fp32'])
     ap.add_argument('--graph', action='store_true', help='graph-safe TorchBox: the epoch is replayed from a CUDA graph')
     ap.add_argument('--algo', default='PPOLag', help='algorithm, e.g. PPOLag or PPOEarlyTerminated')
+    ap.add_argument('--wrappers', action='store_true',
+                    help='TorchBox behind TimeLimit / AutoReset, applied by the adapter on the device')
     args = ap.parse_args()
     import omnisafe_b200
 
     register_torch_box()
-    env_id = GRAPH_ENV_ID if args.graph else ENV_ID
+    if args.wrappers:
+        env_id = GRAPH_WRAPPED_ENV_ID if args.graph else WRAPPED_ENV_ID
+    else:
+        env_id = GRAPH_ENV_ID if args.graph else ENV_ID
     spe = N * T
     cfg = {'seed': 0,
            'train_cfgs': {'device': 'cuda', 'vector_env_nums': N, 'parallel': 1,
