@@ -433,15 +433,15 @@ int osb_actor_eval_x3(const float* theta_actor, int O, int A, const float* obs, 
 int osb_fvp_grid_blocks(long long total, int stride);
 int osb_fvp_partials(const float* theta_actor, const float* vec, int O, int A, const float* obs,
                      long long total, int stride, float* gpart, void* stream);
-/* Tensor-core Fisher-vector product (O <= 512): forward-mode tangent pass with stacked [W;V] weight
- * tiles (dmu scratch [total][A]) + the actor backward of the tensor-core gradient kernel.
+/* Tensor-core Fisher-vector product (O <= 512): forward-mode tangent pass on tf32 tiles (csrc/fvp_tc.cu; dmu
+ * scratch [total][A]) + the actor backward of the tensor-core gradient kernel.
  * gpart: osb_tc_grid_blocks(rows, 1) rows of P_actor floats, rows = ceil(total / stride);
  * stats_scratch: that many * 24 floats.  Reduce with osb_reduce_partials. */
 int osb_fvp_partials_tc(const float* theta_actor, const float* vec, int O, int A, const float* obs,
                         long long total, int stride, float* dmu, float* gpart, float* stats_scratch,
                         void* stream);
 /* Split-bf16 ("bf16x3") variant of osb_fvp_partials_tc (O <= 64): forward-mode tangent kernel on bf16x3 tiles
- * (csrc/fvp_x3.cu) + the bf16x3 actor backward with the tangent as output gradient: fp32-level F v on the tensor
+ * (csrc/fvp_tc.cu) + the bf16x3 actor backward with the tangent as output gradient: fp32-level F v on the tensor
  * cores.  NaturalPG._fvp, natural_pg.py:L74-119. */
 int osb_fvp_partials_x3(const float* theta_actor, const float* vec, int O, int A, const float* obs,
                         long long total, int stride, float* dmu, float* gpart, float* stats_scratch,

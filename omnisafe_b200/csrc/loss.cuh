@@ -255,6 +255,13 @@ int dmu_backward_tc(const float* theta_actor, int O, int A, const float* obs, co
                     float* stats_scratch, cudaStream_t stream);
 int dmu_backward_x3(const float* theta_actor, int O, int A, const float* obs, const float* dmu, int rows, float* gpart,
                     float* stats_scratch, cudaStream_t stream);
+// The backward halves of osb_fvp_partials_tc / osb_fvp_partials_x3 (csrc/fvp_tc.cu): the actor backward of the LOSS_FVP
+// kind with dOUT = dmu / sigma^2 / (rows * A) over rows 0, stride, 2 stride, ... of obs [total][O], dmu [total][A];
+// gpart: osb_tc_grid_blocks(rows, 1) rows of P_actor floats, rows = ceil(total / stride).
+int fvp_backward_tc(const float* theta_actor, const float* vec, int O, int A, const float* obs, long long total, int stride,
+                    const float* dmu, float* gpart, float* stats_scratch, cudaStream_t stream);
+int fvp_backward_x3(const float* theta_actor, const float* vec, int O, int A, const float* obs, long long total, int stride,
+                    const float* dmu, float* gpart, float* stats_scratch, cudaStream_t stream);
 // ... and behind osb_critic_dv_backward: critic `net` (1, 2) of the flat theta, dv[rows] = dL/dV, value[rows] (or
 // null) <- V; gpart: osb_tc_grid_blocks(rows, 1 << net) rows of P floats (the critic's segment written).
 int dv_backward_tc(const float* theta, int O, int A, int net, const float* obs, const float* dv, float* value, int rows,

@@ -1,6 +1,7 @@
 // The tensor-core MLP forward (obs -> 64 -> 64 -> out <= 16, tanh hidden layers) on tiles of 128 rows, shared by
 // rollout_step_tc_kernel (csrc/rollout.cu), policy_tc_kernel (csrc/policy.cu) and actor_eval_tc_kernel
-// (csrc/eval_tc.cu), so that the rollout, the policy step and the evaluation compute one function bit for bit.
+// (csrc/eval_tc.cu), so that the rollout, the policy step and the evaluation compute one function bit for bit; its
+// tiles and staging also carry the Fisher-vector tangent pass (fvp_tangent_kernel, csrc/fvp_tc.cu).
 //   X3 = false: tf32 wgmma tiles (csrc/umma.cuh), layer 1 as a K loop over 64-column chunks for inputs up to 512 wide;
 //   X3 = true : split-bf16 tiles (csrc/x3.cuh), inputs up to 64 wide, one activation buffer (X, H1 and H2 overwrite
 //               each other in place: every epilogue starts after its layer's MMAs completed), accurate tanh.
@@ -115,6 +116,36 @@ __device__ __forceinline__ void tc_stage_weights(uint32_t base, const float* the
     if (tid < 16) sB3[tid] = (tid < L.out) ? __ldg(theta + L.off_b3 + tid) : 0.f;
 }
 
+// Columns [c0, c0 + 8) of obs row `row` (-1: a zero row) of obs [*][O], zero past O; 128-bit loads when vec (O % 4 == 0,
+// obs 16-byte aligned, c0 % 4 == 0).
+__device__ __forceinline__ void tc_gather8(const float* obs, int O, bool vec, long long row, int c0, float (&v)[8]) {
+    if (vec) {
+#pragma unroll
+        for (int v4 = 0; v4 < 2; ++v4) {
+            const int cc = c0 + 4 * v4;
+            const float4 x = (row >= 0 && cc < O) ? __ldg(reinterpret_cast<const float4*>(obs + row * O + cc))
+                                                  : make_float4(0.f, 0.f, 0.f, 0.f);
+            v[4 * v4] = x.x; v[4 * v4 + 1] = x.y; v[4 * v4 + 2] = x.z; v[4 * v4 + 3] = x.w;
+        }
+    } else {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = (row >= 0 && c0 + i < O) ? __ldg(obs + row * O + c0 + i) : 0.f;
+    }
+}
+
+// Chunk c (columns [64 c, 64 c + 64), zero past O) of a [64][O] W1 into the tf32 [64][64] tile sW1, by 256 threads
+// tid = 0 .. 255; thread -> column tid % 64.
+__device__ __forceinline__ void tc_stage_w1_chunk(uint32_t sW1, const float* theta, const NetLayout& L, int O, int c,
+                                                  int tid = threadIdx.x) {
+    using namespace umma;
+    const int k = tid & 63, col = c * 64 + k;
+    float w1c[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) w1c[j] = (col < O) ? __ldg(theta + L.off_w1 + ((tid >> 6) + 4 * j) * O + col) : 0.f;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) sts(tile_addr(sW1, (tid >> 6) + 4 * j, k, 64), tf32r(w1c[j]));
+}
+
 // X tile rows gathered from obs [*][O]: row_of(m) is the obs row of tile row m, or -1 for a zero row.
 //   bf16x3: the whole tile; thread -> row tid / 2, 32-column half; 128-bit loads when vec (O % 4 == 0, obs 16-byte
 //           aligned).  The previous tile's MMAs have completed: the buffer is free.
@@ -129,32 +160,13 @@ __device__ __forceinline__ void tc_stage_rows(uint32_t base, const float* obs, i
         const long long row = row_of(xm);
 #pragma unroll
         for (int c8 = 0; c8 < 4; ++c8) {
-            const int c0 = xh + 8 * c8;
             float v[8];
-            if (vec) {
-#pragma unroll
-                for (int v4 = 0; v4 < 2; ++v4) {
-                    const int cc = c0 + 4 * v4;
-                    const float4 x = (row >= 0 && cc < O) ? __ldg(reinterpret_cast<const float4*>(obs + row * O + cc))
-                                                          : make_float4(0.f, 0.f, 0.f, 0.f);
-                    v[4 * v4] = x.x; v[4 * v4 + 1] = x.y; v[4 * v4 + 2] = x.z; v[4 * v4 + 3] = x.w;
-                }
-            } else {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) v[i] = (row >= 0 && c0 + i < O) ? __ldg(obs + row * O + c0 + i) : 0.f;
-            }
-            x3::store8_x3(base + TcTiles<true>::X, TcTiles<true>::SUB, xm, c0, v);
+            tc_gather8(obs, O, vec, row, xh + 8 * c8, v);
+            x3::store8_x3(base + TcTiles<true>::X, TcTiles<true>::SUB, xm, xh + 8 * c8, v);
         }
     } else {
         const int k = tid & 63, col = c * 64 + k;
-        if (O > 64) {
-            const uint32_t sW1 = base + TcTiles<false>::W1;
-            float w1c[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) w1c[j] = (col < O) ? __ldg(theta + L.off_w1 + ((tid >> 6) + 4 * j) * O + col) : 0.f;
-#pragma unroll
-            for (int j = 0; j < 16; ++j) sts(tile_addr(sW1, (tid >> 6) + 4 * j, k, 64), tf32r(w1c[j]));
-        }
+        if (O > 64) tc_stage_w1_chunk(base + TcTiles<false>::W1, theta, L, O, c);
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
             float xv[16];

@@ -38,7 +38,7 @@ struct TcArgs {
     float* stats_part;
     const int* stop_flag;
     int O, A, P, net_mask;
-    const float* fvp_dmu;    // LOSS_FVP: tangent of mu per row [total][A] (fvp_tangent_tc_kernel)
+    const float* fvp_dmu;    // LOSS_FVP: tangent of mu per row [total][A] (fvp_tangent_kernel, csrc/fvp_tc.cu)
     const float* fvp_vec;    // LOSS_FVP: direction v (log_std block of F v)
     float fvp_scale;         // LOSS_FVP: 1 / (rows * A)
     int forward_only;        // pass 1 of FOCOPS / P3O: statistics only, no backward
@@ -636,286 +636,12 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
     __syncthreads();
 }
 
-// ---------------------------------------------------------------------------------------------
-// Forward-mode tangent pass of the Fisher-vector product (NaturalPG._fvp, base/natural_pg.py:L74-119):
-//   dmu[row][a] = J_mu(row) v      for the rows 0, stride, 2*stride, ...
-// The weight tile of every layer is stored with the direction's block stacked under it
-// ([W ; V], 128 rows), so ONE N = 128 MMA yields the pre-activation and the first tangent term:
-//     [Z1 | X V1^T]            = X   [W1;V1]^T
-//     [Z2 | H1 V2^T + dH1 W2^T] = H1 [W2;V2]^T  (+)  dH1 W2^T   (accumulated into the right half)
-//     dmu                       = H2 V3^T + dH2 W3^T + vb3
-// The backward half (J^T diag(sigma^-2) dmu) is minibatch_grad_tc_kernel with kind LOSS_FVP.
-struct FvpTanArgs {
-    const float* obs; long long total; int stride;
-    const float* theta; const float* vec; float* dmu; int O, A;
-    float* acc;              // accumulator images, one [128][F_COLS] per CTA
-};
-constexpr uint32_t F_Z1 = 0, F_Z2 = 128, F_DMU = 256, F_COLS = 272;
-
-template <bool CHUNKED>     // obs dim > 64: K loop over 64-column chunks of X / [W1;V1]
-__global__ void __launch_bounds__(NTC, 1) fvp_tangent_tc_kernel(FvpTanArgs p) {
-    extern __shared__ __align__(16) uint8_t smem_raw[];
-    const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
-    const uint32_t B0 = smem_u32(smem_raw) + pad;   // X -> H2
-    const uint32_t B1 = B0 + BUF;                   // H1 -> dH2
-    const uint32_t B2 = B1 + BUF;                   // dH1
-    const uint32_t sWV1 = B2 + BUF;                 // [128][64]: rows 0..63 W1, 64..127 V1
-    const uint32_t sWV2 = sWV1 + 32768;             // [128][64]: W2 ; V2
-    const uint32_t sWV3 = sWV2 + 32768;             // [32][64]:  rows 0..15 W3, 16..31 V3
-    float* sB1 = reinterpret_cast<float*>(smem_raw + pad + 3 * BUF + 2 * 32768 + 8192);
-    float* sB2 = sB1 + 64;
-    float* sVB1 = sB2 + 64;
-    float* sVB2 = sVB1 + 64;
-    float* sVB3 = sVB2 + 64;           // [16]
-    long long* sRowBuf = reinterpret_cast<long long*>(sVB3 + 16);   // [2][128]
-    __shared__ uint64_t bar;
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int q = warp & 3, h = warp >> 2;
-    const int O = p.O, A = p.A;
-    const NetLayout L = actor_layout(O, A);
-    const long long nrows = (p.total + p.stride - 1) / p.stride;
-    const int ntiles = (int)((nrows + TT - 1) / TT);
-
-    {   // stacked weight tiles (loads batched so they are all in flight together)
-        float w1v[8], v1v[8], w2v[8], v2v[8], w3v[2], v3v[2];
-        const int k = tid & 63;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int n = (tid >> 6) + 8 * j;
-            w1v[j] = (!CHUNKED && k < O) ? __ldg(p.theta + L.off_w1 + n * O + k) : 0.f;
-            v1v[j] = (!CHUNKED && k < O) ? __ldg(p.vec + L.off_w1 + n * O + k) : 0.f;
-            w2v[j] = __ldg(p.theta + L.off_w2 + n * 64 + k);
-            v2v[j] = __ldg(p.vec + L.off_w2 + n * 64 + k);
-        }
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-            const int o = (tid >> 6) + 8 * j;
-            w3v[j] = (o < A) ? __ldg(p.theta + L.off_w3 + o * 64 + k) : 0.f;
-            v3v[j] = (o < A) ? __ldg(p.vec + L.off_w3 + o * 64 + k) : 0.f;
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int n = (tid >> 6) + 8 * j;
-            sts(tile_addr(sWV1, n, k, 128), tf32r(w1v[j]));
-            sts(tile_addr(sWV1, 64 + n, k, 128), tf32r(v1v[j]));
-            sts(tile_addr(sWV2, n, k, 128), tf32r(w2v[j]));
-            sts(tile_addr(sWV2, 64 + n, k, 128), tf32r(v2v[j]));
-        }
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-            const int o = (tid >> 6) + 8 * j;
-            sts(tile_addr(sWV3, o, k, 32), tf32r(w3v[j]));
-            sts(tile_addr(sWV3, 16 + o, k, 32), tf32r(v3v[j]));
-        }
-    }
-    if (tid < 64) {
-        sB1[tid] = __ldg(p.theta + L.off_b1 + tid); sB2[tid] = __ldg(p.theta + L.off_b2 + tid);
-        sVB1[tid] = __ldg(p.vec + L.off_b1 + tid); sVB2[tid] = __ldg(p.vec + L.off_b2 + tid);
-    }
-    if (tid < 16) sVB3[tid] = (tid < A) ? __ldg(p.vec + L.off_b3 + tid) : 0.f;
-    if (tid == 0) { mbar_init(&bar, 1); mbar_init_fence(); }
-    __syncthreads();
-    const Acc tm = acc_cta(p.acc, F_COLS);
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    uint32_t phase = 0;
-    const int s_row = 32 * q + lane, c16 = 16 * h;
-
-    const bool vec4 = (O & 3) == 0;
-    auto tile_rows = [&](int tile, long long* dst) {
-        if (tid < TT) {
-            const long long k = (long long)tile * TT + tid;
-            dst[tid] = (k < nrows) ? k * p.stride : -1;
-        }
-    };
-    float4 xpre[4];
-    auto prefetch_x = [&](const long long* rows) {
-        const int k4 = (tid & 15) << 2;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const long long row = rows[(tid >> 4) + 32 * j];
-            xpre[j] = (row >= 0 && k4 < O) ? __ldg(reinterpret_cast<const float4*>(p.obs + row * O + k4))
-                                            : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-    };
-    const int nchunks = (O + 63) >> 6;
-    float xr[16];
-    auto load_chunk = [&](const long long* rows, int c) {
-        if (vec4) {
-            const int col = c * 64 + ((tid & 15) << 2);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const long long row = rows[(tid >> 4) + 32 * j];
-                const float4 v = (row >= 0 && col < O) ? __ldg(reinterpret_cast<const float4*>(p.obs + row * O + col))
-                                                        : make_float4(0.f, 0.f, 0.f, 0.f);
-                xr[4 * j] = v.x; xr[4 * j + 1] = v.y; xr[4 * j + 2] = v.z; xr[4 * j + 3] = v.w;
-            }
-        } else {
-            const int col = c * 64 + (tid & 63);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                const long long row = rows[(tid >> 6) + 8 * j];
-                xr[j] = (row >= 0 && col < O) ? __ldg(p.obs + row * O + col) : 0.f;
-            }
-        }
-    };
-    auto store_chunk = [&]() {
-        if (vec4) {
-            const int k4 = (tid & 15) << 2;
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-                asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(tile_addr(B0, (tid >> 4) + 32 * j, k4, TT)),
-                             "f"(tf32r(xr[4 * j])), "f"(tf32r(xr[4 * j + 1])), "f"(tf32r(xr[4 * j + 2])), "f"(tf32r(xr[4 * j + 3]))
-                             : "memory");
-        } else {
-            const int k = tid & 63;
-#pragma unroll
-            for (int j = 0; j < 16; ++j) sts(tile_addr(B0, (tid >> 6) + 8 * j, k, TT), tf32r(xr[j]));
-        }
-    };
-    auto load_wv1_chunk = [&](int c) {                 // [W1 ; V1][:, 64c : 64c+64] -> sWV1 (zero padded)
-        const int k = tid & 63, col = c * 64 + k;
-        float w[8], v[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int n = (tid >> 6) + 8 * j;
-            w[j] = (col < O) ? __ldg(p.theta + L.off_w1 + n * O + col) : 0.f;
-            v[j] = (col < O) ? __ldg(p.vec + L.off_w1 + n * O + col) : 0.f;
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int n = (tid >> 6) + 8 * j;
-            sts(tile_addr(sWV1, n, k, 128), tf32r(w[j]));
-            sts(tile_addr(sWV1, 64 + n, k, 128), tf32r(v[j]));
-        }
-    };
-    int rpar = 0;
-    tile_rows(blockIdx.x, sRowBuf);
-    __syncthreads();
-    if (CHUNKED) load_chunk(sRowBuf, 0);
-    else if (vec4) prefetch_x(sRowBuf);
-
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        long long* sRow = sRowBuf + rpar * TT;
-        long long* sRowNext = sRowBuf + (rpar ^ 1) * TT;
-        const bool has_next = tile + (int)gridDim.x < ntiles;
-        if (has_next) tile_rows(tile + gridDim.x, sRowNext);
-        if (CHUNKED) {
-            // staged chunk by chunk below
-        } else if (vec4) {
-            const int k4 = (tid & 15) << 2;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int m = (tid >> 4) + 32 * j;
-                asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(tile_addr(B0, m, k4, TT)),
-                             "f"(tf32r(xpre[j].x)), "f"(tf32r(xpre[j].y)), "f"(tf32r(xpre[j].z)), "f"(tf32r(xpre[j].w))
-                             : "memory");
-            }
-        } else {
-            const int k = tid & 63;
-            float xv[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                const long long row = sRow[(tid >> 6) + 8 * j];
-                xv[j] = (row >= 0 && k < O) ? __ldg(p.obs + row * O + k) : 0.f;
-            }
-#pragma unroll
-            for (int j = 0; j < 16; ++j) sts(tile_addr(B0, (tid >> 6) + 8 * j, k, TT), tf32r(xv[j]));
-        }
-        fence_async_smem();
-        __syncthreads();
-        // ---- layer 1: [Z1 | X V1^T] ----------------------------------------------------------------
-        if (CHUNKED) {
-            for (int c = 0; c < nchunks; ++c) {
-                load_wv1_chunk(c);
-                store_chunk();
-                fence_async_smem();
-                __syncthreads();
-                if (c + 1 < nchunks) load_chunk(sRow, c + 1);
-                else if (has_next) load_chunk(sRowNext, 0);
-                if (warpgroup_index() == 0) {
-                    tc_gemm(tm, F_Z1, B0, TT, sWV1, 128, 128, 128, 64, c > 0);
-                    mma_commit(&bar);
-                }
-                mbar_wait(&bar, phase); phase ^= 1;
-            }
-        } else {
-            if (vec4 && has_next) prefetch_x(sRowNext);      // next tile's rows fly during the three layers
-            if (warpgroup_index() == 0) {
-                tc_gemm(tm, F_Z1, B0, TT, sWV1, 128, 128, 128, 64, false);
-                mma_commit(&bar);
-            }
-            mbar_wait(&bar, phase); phase ^= 1;
-        }
-        {
-            float z[16], dz[16];
-            acc_ld16(tm, lane_base + F_Z1 + c16, z);
-            acc_ld16(tm, lane_base + F_Z1 + 64 + c16, dz);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                const float hh = tanh_fast(z[i] + sB1[c16 + i]);
-                dz[i] = (1.f - hh * hh) * (dz[i] + sVB1[c16 + i]);
-                z[i] = hh;
-            }
-            store_row16(B1, s_row, c16, TT, z);      // H1
-            store_row16(B2, s_row, c16, TT, dz);     // dH1
-        }
-        fence_async_smem();
-        __syncthreads();
-        // ---- layer 2: [Z2 | H1 V2^T + dH1 W2^T] ------------------------------------------------------
-        if (warpgroup_index() == 0) {
-            tc_gemm(tm, F_Z2, B1, TT, sWV2, 128, 128, 128, 64, false);
-            tc_gemm(tm, F_Z2 + 64, B2, TT, sWV2, 128, 128, 64, 64, true);
-            mma_commit(&bar);
-        }
-        mbar_wait(&bar, phase); phase ^= 1;
-        {
-            float z[16], dz[16];
-            acc_ld16(tm, lane_base + F_Z2 + c16, z);
-            acc_ld16(tm, lane_base + F_Z2 + 64 + c16, dz);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                const float hh = tanh_fast(z[i] + sB2[c16 + i]);
-                dz[i] = (1.f - hh * hh) * (dz[i] + sVB2[c16 + i]);
-                z[i] = hh;
-            }
-            store_row16(B0, s_row, c16, TT, z);      // H2  (X is dead)
-            store_row16(B1, s_row, c16, TT, dz);     // dH2 (H1 is dead: layer-2 MMAs completed)
-        }
-        fence_async_smem();
-        __syncthreads();
-        // ---- output tangent: dmu = H2 V3^T + dH2 W3^T + vb3 -------------------------------------------
-        if (warpgroup_index() == 0) {
-            tc_gemm(tm, F_DMU, B0, TT, sWV3 + 2048u, 32, 128, 16, 64, false);
-            tc_gemm(tm, F_DMU, B1, TT, sWV3, 32, 128, 16, 64, true);
-            mma_commit(&bar);
-        }
-        mbar_wait(&bar, phase); phase ^= 1;
-        if (h == 0) {
-            float o16[16];
-            acc_ld16(tm, lane_base + F_DMU, o16);
-            const long long row = sRow[s_row];
-            if (row >= 0) {
-#pragma unroll
-                for (int a = 0; a < 16; ++a)
-                    if (a < A) p.dmu[row * A + a] = o16[a] + sVB3[a];
-            }
-        }
-        rpar ^= 1;
-        __syncthreads();
-    }
-    __syncthreads();
-}
-
 }  // namespace osb
 
 using namespace osb;
 
 static size_t tc_smem_bytes() {
     return 1024 + 5 * (size_t)BUF + 3 * 16384 + 4096 + 8192 + (64 + 64 + 16 + 48 + 8 + 160 + 16 + 32 + 16) * 4 + 2 * 128 * 8 + 64;
-}
-static size_t fvp_tan_smem_bytes() {
-    return 1024 + 3 * (size_t)BUF + 2 * 32768 + 8192 + (4 * 64 + 16) * 4 + 2 * 128 * 8 + 64;
 }
 
 static int launch_grad_tc(TcArgs& p, int nblocks, cudaStream_t stream) {
@@ -991,43 +717,6 @@ int osb_minibatch_grad_tc(const float* theta, int O, int A, const float* obs, co
     return launch_grad_tc(p, nb, (cudaStream_t)stream);
 }
 
-// Tensor-core Fisher-vector product partials (O <= 512): tangent forward (dmu scratch [total][A]) then
-// the actor backward of minibatch_grad_tc_kernel.  gpart: osb_tc_grid_blocks(rows, 1) rows of
-// P_actor floats; stats_scratch: that many * 24 floats.  Reduce with osb_reduce_partials.
-int osb_fvp_partials_tc(const float* theta_actor, const float* vec, int O, int A, const float* obs,
-                        long long total, int stride, float* dmu, float* gpart, float* stats_scratch,
-                        void* stream) {
-    OSB_CHECK_ARG(theta_actor && vec && obs && dmu && gpart && stats_scratch && total > 0 && stride > 0, "bad argument");
-    OSB_CHECK_ARG(O > 0 && O <= 512 && A > 0 && A <= 16, "tensor-core path needs O <= 512, A <= 16");
-    const long long nrows = (total + stride - 1) / stride;
-    OSB_CHECK_ARG(nrows < (1ll << 31), "too many rows");
-    const int nb = osb_tc_grid_blocks(nrows, 1);
-    cudaStream_t s = (cudaStream_t)stream;
-    {
-        FvpTanArgs t{obs, total, stride, theta_actor, vec, dmu, O, A, nullptr};
-        t.acc = acc_scratch(ACC_FVP_TC, (size_t)nb * 128 * F_COLS * sizeof(float));
-        if (!t.acc) return OSB_ERR_CUDA;
-        const size_t smem = fvp_tan_smem_bytes();
-        static bool attr = false;
-        if (!attr) {
-            OSB_CUDA(cudaFuncSetAttribute(fvp_tangent_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            OSB_CUDA(cudaFuncSetAttribute(fvp_tangent_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            attr = true;
-        }
-        if (O > 64) fvp_tangent_tc_kernel<true><<<nb, NTC, smem, s>>>(t);
-        else fvp_tangent_tc_kernel<false><<<nb, NTC, smem, s>>>(t);
-        OSB_LAUNCH_CHECK();
-    }
-    TcArgs p;
-    p.b = Batch{obs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, total, 0u, 0, (int)nrows, stride};
-    p.lc = LossParams{LOSS_FVP, 0.f, 0.f, 1.f, 0.f, nullptr, nullptr, nullptr, nullptr};
-    p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch; p.stop_flag = nullptr;
-    p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
-    p.fvp_dmu = dmu; p.fvp_vec = vec; p.fvp_scale = 1.0f / ((float)nrows * (float)A);
-    p.forward_only = 0;
-    return launch_grad_tc(p, nb, s);
-}
-
 }  // extern "C"
 
 // LOSS_DMU launch of the DMU instantiations (one network, grid.y == 1) on nb CTAs
@@ -1059,6 +748,19 @@ int osb::dmu_backward_tc(const float* theta_actor, int O, int A, const float* ob
     p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
     p.fvp_dmu = dmu; p.value_out = nullptr;
     return launch_dmu_tc(p, osb_tc_grid_blocks(rows, 1), stream);
+}
+
+int osb::fvp_backward_tc(const float* theta_actor, const float* vec, int O, int A, const float* obs, long long total,
+                         int stride, const float* dmu, float* gpart, float* stats_scratch, cudaStream_t stream) {
+    const long long nrows = (total + stride - 1) / stride;
+    TcArgs p;
+    p.b = Batch{obs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, total, 0u, 0, (int)nrows, stride};
+    p.lc = LossParams{LOSS_FVP, 0.f, 0.f, 1.f, 0.f, nullptr, nullptr, nullptr, nullptr};
+    p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch; p.stop_flag = nullptr;
+    p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
+    p.fvp_dmu = dmu; p.fvp_vec = vec; p.fvp_scale = 1.0f / ((float)nrows * (float)A);
+    p.forward_only = 0;
+    return launch_grad_tc(p, osb_tc_grid_blocks(nrows, 1), stream);
 }
 
 int osb::dv_backward_tc(const float* theta, int O, int A, int net, const float* obs, const float* dv, float* value, int rows,

@@ -70,7 +70,7 @@ struct X3Args {
     uint8_t* wimg;               // FUSED: [3 nets][W_IMG] bf16x3 images of the weight tiles (W1 | W2 | W3), written by the Adam owners,
                                  // pulled into shared memory with one bulk copy (TMA) after every optimiser step
     int forward_only;            // pass 1 of FOCOPS / P3O (stepwise launches only): statistics only
-    const float* fvp_dmu;        // LOSS_FVP: tangent of mu per slab row [total][A] (fvp_tangent_x3_kernel)
+    const float* fvp_dmu;        // LOSS_FVP: tangent of mu per slab row [total][A] (fvp_tangent_kernel, csrc/fvp_tc.cu)
     const float* fvp_vec;        // LOSS_FVP: direction v (its log_std block gives the log_std block of F v)
     float fvp_scale;             // LOSS_FVP: 1 / (rows * A)
     long long* dbg;              // optional clock64 stamps of CTA (0, 0): [0] = count, then (id, clock) pairs (tools/x3_stage_times.py)
@@ -1077,26 +1077,6 @@ int osb_minibatch_grad_x3(const float* theta, int O, int A, const float* obs, co
     return OSB_OK;
 }
 
-// backward half of the bf16x3 Fisher-vector product (called by osb_fvp_partials_x3, csrc/fvp_x3.cu)
-int osb_x3_fvp_backward(const float* theta_actor, const float* vec, int O, int A, const float* obs, long long total, int stride,
-                        const float* dmu, float* gpart, float* stats_scratch, void* stream) {
-    const long long nrows = (total + stride - 1) / stride;
-    X3Args p = {};
-    p.b = Batch{obs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, total, 0u, 0, (int)nrows, stride};
-    p.lc.kind = LOSS_FVP; p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch;
-    p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
-    p.batch_size = (int)nrows; p.world = 1; p.dbg = nullptr;
-    p.fvp_dmu = dmu; p.fvp_vec = vec; p.fvp_scale = 1.0f / ((float)nrows * (float)A);
-    const int nb = osb_tc_grid_blocks(nrows, 1);
-    int rc = x3_set_attr();
-    if (rc) return rc;
-    if ((rc = x3_bind_acc(p, nb))) return rc;
-    if (A <= 8) minibatch_grad_x3_kernel<false, 8><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(p);
-    else minibatch_grad_x3_kernel<false, 16><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(p);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
-}
-
 // One update iteration of PolicyGradient._update (policy_gradient.py:L369-381) as ONE persistent cooperative
 // kernel on bf16x3 tiles: all minibatches of [0, total) in steps of batch_size, each = fused forward + loss +
 // backward, fixed-order partial reduction, per-network clip_grad_norm_, (world > 1: clipped-gradient exchange
@@ -1183,6 +1163,25 @@ int osb::dmu_backward_x3(const float* theta_actor, int O, int A, const float* ob
     p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
     p.fvp_dmu = dmu;
     return launch_dmu_x3(p, osb_tc_grid_blocks(rows, 1), stream);
+}
+
+int osb::fvp_backward_x3(const float* theta_actor, const float* vec, int O, int A, const float* obs, long long total,
+                         int stride, const float* dmu, float* gpart, float* stats_scratch, cudaStream_t stream) {
+    const long long nrows = (total + stride - 1) / stride;
+    X3Args p = {};
+    p.b = Batch{obs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, total, 0u, 0, (int)nrows, stride};
+    p.lc.kind = LOSS_FVP; p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch;
+    p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1;
+    p.batch_size = (int)nrows; p.world = 1; p.dbg = nullptr;
+    p.fvp_dmu = dmu; p.fvp_vec = vec; p.fvp_scale = 1.0f / ((float)nrows * (float)A);
+    const int nb = osb_tc_grid_blocks(nrows, 1);
+    int rc = x3_set_attr();
+    if (rc) return rc;
+    if ((rc = x3_bind_acc(p, nb))) return rc;
+    if (A <= 8) minibatch_grad_x3_kernel<false, 8><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
+    else minibatch_grad_x3_kernel<false, 16><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
 }
 
 int osb::dv_backward_x3(const float* theta, int O, int A, int net, const float* obs, const float* dv, float* value, int rows,

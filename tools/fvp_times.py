@@ -1,5 +1,5 @@
-"""CUDA-event timing of the Fisher-vector product and full-batch actor gradient, fp32 FMA tiles vs
-wgmma tiles (headline batch 4096 x 128, O = 60, A = 8)."""
+"""CUDA-event timing of the Fisher-vector product and full-batch actor gradient, fp32 FMA tiles vs tf32 and
+bf16x3 wgmma tiles (headline batch 4096 x 128, O = 60, A = 8)."""
 import json
 import sys
 
@@ -37,10 +37,11 @@ def timeit(fn, iters=20):
 
 
 res = {}
-for prec, name in ((0, 'fp32'), (1, 'tf32')):
+for prec, name in ((0, 'fp32'), (1, 'tf32'), (2, 'bf16x3')):
     eng.precision = prec
     res[f'fvp_{name}_us'] = round(timeit(lambda: eng.fvp(vec, out, 0.1)), 1)
     res[f'actor_loss_grad_{name}_us'] = round(timeit(lambda: eng.actor_loss_grad(LOSS_RATIO, None, g)), 1)
 flops = 6 * 2 * (60 * 64 + 64 * 64 + 64 * 8) * N * T          # tangent fwd + fwd + bwd, 2 flop per MAC
-res['fvp_tf32_TFLOPs'] = round(flops / (res['fvp_tf32_us'] * 1e-6) / 1e12, 1)
+for name in ('tf32', 'bf16x3'):
+    res[f'fvp_{name}_TFLOPs'] = round(flops / (res[f'fvp_{name}_us'] * 1e-6) / 1e12, 1)
 print(json.dumps(res))
