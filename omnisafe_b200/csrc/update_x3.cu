@@ -73,7 +73,8 @@ struct X3Args {
     const float* fvp_dmu;        // LOSS_FVP: tangent of mu per slab row [total][A] (fvp_tangent_kernel, csrc/fvp_tc.cu)
     const float* fvp_vec;        // LOSS_FVP: direction v (its log_std block gives the log_std block of F v)
     float fvp_scale;             // LOSS_FVP: 1 / (rows * A)
-    long long* dbg;              // optional clock64 stamps of CTA (0, 0): [0] = count, then (id, clock) pairs (tools/x3_stage_times.py)
+    long long* dbg;              // optional clock64 stamps of one CTA (x3_dbg_cta): three regions of X3_DBG_REGION, each [0] = count,
+                                 // then (id, clock) pairs (tools/x3_stage_times.py)
     float* acc;                  // accumulator images, one [128][T_COLS] per CTA
     float* value_out;            // LOSS_DMU on a critic (DMU instantiation only), or null: V per row as this launch computes it
 };
@@ -199,6 +200,15 @@ __device__ __forceinline__ void st_release_sys_u32(unsigned int* p, unsigned int
     asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
+// stage-time stamps (development aid): regions of thread 0, thread 320 and thread 512 (the MMA-issue warpgroup), then the
+// selected CTA as x | y << 16 at X3_DBG_SEL, written by the host before the launch
+constexpr int X3_DBG_REGION = 4096, X3_DBG_MAX = 2000, X3_DBG_SEL = 3 * X3_DBG_REGION;
+__device__ __forceinline__ bool x3_dbg_cta(const long long* dbg) {
+    if (dbg == nullptr) return false;
+    const long long sel = dbg[X3_DBG_SEL];
+    return blockIdx.x == (unsigned)(sel & 0xffff) && blockIdx.y == (unsigned)(sel >> 16);
+}
+
 constexpr int PSTR = 9472;          // FUSED: row stride of the private partial-gradient layout [3][G][PSTR] (16 B aligned rows)
 
 // FUSED = false: one minibatch, per-CTA partial gradients out (the contract of minibatch_grad_tc_kernel).
@@ -267,12 +277,13 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
         const uint64_t dW3 = desc128(sbase + OFF_W3), dOnes = desc32(sbase + OFF_ONES);
         // stage-time stamps of this warpgroup (third region of p.dbg).  Ids: 100 + 20 k for product k of Z1, Z2, OUT, dZ2',
         // dZ1', plus 4 r + {0: operands ready, 1: MMAs complete, 2: image stored, 3: committed} for row half r;
-        // 200 / 201 / 202: dW3, dW2 and dW1 have read their operands; 203: the last gradient product committed.
-        const bool mdbg_on = p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && tid == NEPI;
+        // 200 / 201 / 202: dW3, dW2 and dW1 have read their operands; 203: the last gradient product committed; 204: dW2
+        // stored, 205: dZ1 ready, 206: dW1 stored, 207: the last tile's db2 stored.
+        const bool mdbg_on = tid == NEPI && x3_dbg_cta(p.dbg);
         int mdbg_n = 0;
         auto mstamp = [&](int id) {
-            if (mdbg_on && mdbg_n < 400) {
-                long long* d = p.dbg + 2048;
+            if (mdbg_on && mdbg_n < X3_DBG_MAX) {
+                long long* d = p.dbg + 2 * X3_DBG_REGION;
                 d[1 + 2 * mdbg_n] = id; d[2 + 2 * mdbg_n] = clock64(); ++mdbg_n; d[0] = mdbg_n;
             }
         };
@@ -355,13 +366,18 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     mstamp(183 + 4 * r);
                 }
                 gemm_x3<64, 64, 8, 1, 1>(tm, T_DW2, dH2, ACT_SUB, 2048u, dH1, ACT_SUB, 2048u, !first, [&](int) { mma_release_a(bar(DONE_C5B)); mstamp(201); });
-                // dW1 += dZ1^T X (column 63 = db1 with the ones column) ; last tile of the minibatch: its own db2.  Only dW1
-                // reads X, and dZ1 / dZ2 are overwritten no earlier than the next tile's E1 / E2, behind its Z1 / Z2.
+                mstamp(204);
+                // last tile of the minibatch: its own db2 (dZ2 has been in H2 since RDY_DZ2), issued while the epilogue
+                // stores dZ1, so that the minibatch's last commit follows dW1 directly
+                if (last) { gemm_x3<64, 16, 8, 1, 1, true>(tm, T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, !first); mstamp(207); }
+                // dW1 += dZ1^T X (column 63 = db1 with the ones column).  Only dW1 reads X, and dZ1 / dZ2 are overwritten no
+                // earlier than the next tile's E1 / E2, behind its Z1 / Z2.
                 mbar_wait_a(bar(RDY_DZ1_0), par);
                 mbar_wait_a(bar(RDY_DZ1_1), par);
+                mstamp(205);
                 gemm_x3<64, 64, 8, 1, 1>(tm, T_DW1, dH1, ACT_SUB, 2048u, dX, ACT_SUB, 2048u, !first, [&](int) { mma_release_a(bar(FREE_X)); mstamp(202); });
+                mstamp(206);
                 if (!ones_col) gemm_x3<64, 16, 8, 1, 1, true>(tm, T_DB1, dH1, ACT_SUB, 2048u, dOnes, 0u, 0u, !first);
-                if (last) gemm_x3<64, 16, 8, 1, 1, true>(tm, T_DB2, dH2, ACT_SUB, 2048u, dOnes, 0u, 0u, !first);
                 mma_commit_a(bar(DONE_C6));
                 mstamp(203);
             }
@@ -405,11 +421,11 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
             __syncwarp();
             if (lane == 0) mbar_arrive(bar(b));
         };
-        const bool dbg_on = p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && (tid == 0 || tid == 320);      // rows 0-63 with h == 0, rows 64-127 with h == 2
+        const bool dbg_on = (tid == 0 || tid == 320) && x3_dbg_cta(p.dbg);      // rows 0-63 with h == 0, rows 64-127 with h == 2
         int dbg_n = 0;
         auto stamp = [&](int id) {
-            if (dbg_on && dbg_n < 400) {
-                long long* d = p.dbg + (tid == 0 ? 0 : 1024);
+            if (dbg_on && dbg_n < X3_DBG_MAX) {
+                long long* d = p.dbg + (tid == 0 ? 0 : X3_DBG_REGION);
                 d[1 + 2 * dbg_n] = id; d[2 + 2 * dbg_n] = clock64(); ++dbg_n; d[0] = dbg_n;
             }
         };
@@ -697,16 +713,15 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 rpar ^= 1;
             }
             stamp(20);
-            // ---- rows + X of the first tile of the NEXT minibatch: the gather flies under the optimiser phases ------
+            // ---- rows of the first tile of the NEXT minibatch (its X is gathered behind the slice reduction) ------
+            bool next_x = false;
             if (FUSED && mb + 1 < n_mb) {
                 long long s2; int c2;
                 mb_geom(mb + 1, s2, c2);
-                if ((int)blockIdx.x < (c2 + XT - 1) / XT) {
-                    tile_rows(mb + 1, blockIdx.x, sRowBuf + rpar * XT);
-                    epi_bar_sync();
-                    prefetch_x(sRowBuf + rpar * XT);
-                }
+                next_x = (int)blockIdx.x < (c2 + XT - 1) / XT;
+                if (next_x) tile_rows(mb + 1, blockIdx.x, sRowBuf + rpar * XT);
             }
+            stamp(35);
             // FUSED: the owner's Adam state does not depend on the gradient (only this thread writes it), so its loads fly
             // under the wait for the last gradient product and the first grid barrier
             float pre_th = 0.f, pre_m = 0.f, pre_v = 0.f;
@@ -755,6 +770,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     const int i = tid - 64;
                     __stcg(p.stats_part + ((size_t)blockIdx.x * 3 + net) * 8 + i, (i < 5) ? (sRed[i] + sRed[8 + i]) + (sRed[16 + i] + sRed[24 + i]) : 0.f);
                 }
+                stamp(32);
                 mbar_wait_a(bar(DONE_C6), (uint32_t)((it - 1) & 1));
                 stamp(21);
                 const int t_row = 16 * q + lane;       // row (lane < 16) of the M = 64 accumulators
@@ -831,10 +847,16 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                         float t[32];
 #pragma unroll
                         for (int u = 0; u < 32; ++u) t[u] = (b + u < b1 && b + u < ntiles) ? __ldcg(src + (size_t)(b + u) * stride) : 0.f;
+                        // the pairwise tree, level by level with constant indices: written as a loop over w, it was not
+                        // unrolled and t went to the stack, each loaded value stored there as it arrived
 #pragma unroll
-                        for (int w = 16; w > 0; w >>= 1)
+                        for (int u = 0; u < 16; ++u) t[u] += t[u + 16];
 #pragma unroll
-                            for (int u = 0; u < w; ++u) t[u] += t[u + w];
+                        for (int u = 0; u < 8; ++u) t[u] += t[u + 8];
+#pragma unroll
+                        for (int u = 0; u < 4; ++u) t[u] += t[u + 4];
+                        t[0] += t[2]; t[1] += t[3];
+                        t[0] += t[1];
                         sacc += t[0];
                     }
                 }
@@ -856,6 +878,11 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 epi_bar_sync();
                 if (spec && base > 0 && own && tid >= 256) g_raw = sPart[tid - 256];      // spec: S <= 512, base 256 is the last chunk
             }
+            // X of the next minibatch's first tile flies under the norm, Adam and restaging phases.  Gathered at the start of
+            // the boundary, its 16 registers were live through the statistics and the slice reduction, which then spilled
+            // and waited on the gathered rows.  The row list was written before net_barrier, whose bar.sync orders it
+            // before these reads.
+            if (next_x) prefetch_x(sRowBuf + rpar * XT);
             ssq = warp_sum(ssq); st2 = warp_sum(st2);
             if (lane == 0) { sPart[256 + warp] = ssq; sPart[272 + warp] = st2; }       // the hand-over slots stay untouched
             epi_bar_sync();
@@ -866,7 +893,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 __stcg(p.sumsq_part + (net * 2 + 1) * G + blockIdx.x, b);
             }
             stamp(30);
-            if (dbg_on && own) p.dbg[(tid == 0 ? 0 : 1024) + 1023] = __float_as_int(pre_th + pre_m + pre_v);     // waits for the state
+            if (dbg_on && own) p.dbg[(tid == 0 ? 0 : X3_DBG_REGION) + X3_DBG_REGION - 1] = __float_as_int(pre_th + pre_m + pre_v);     // waits for the state
             stamp(31);
             // torch-Adam step of one parameter (+ its three bf16 pieces in the weight-tile image)
             auto adam_store = [&](int qg, float g, float th, float m, float v, bool img) {
@@ -1011,7 +1038,8 @@ extern "C" {
 int osb_tc_grid_blocks(long long rows, int net_mask);
 
 static long long* g_x3_dbg = nullptr;
-// development aid: clock64 stamps of CTA (0, 0) of the next launches go to buf (2048 long long), NULL turns it off
+// development aid: clock64 stamps of one CTA of the next launches go to buf (3 * 4096 + 1 long long, the last the CTA
+// x | y << 16), NULL turns it off
 int osb_x3_debug_buffer(long long* buf) { g_x3_dbg = buf; return OSB_OK; }
 
 static int x3_set_attr() {
