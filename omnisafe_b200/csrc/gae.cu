@@ -17,11 +17,13 @@
 // (separately rounded fp64 mul/add) from the exact carry-in.  Tiles of 128 steps are walked from
 // the end of the horizon to its start with a per-env carry.
 #include "common.cuh"
+#include "umma.cuh"
 #include <cuda.h>
-#include <stdlib.h>
 #include <string.h>
 
 namespace osb {
+
+using namespace umma;
 
 constexpr int GE = 16;         // envs per block
 constexpr int GC = 32;         // chunks per tile
@@ -80,8 +82,44 @@ __device__ __forceinline__ void gae_load_tile(const GaeArgs& p, int env, bool en
     d.vc[GL] = ok ? __ldg(p.val_c + idx) : 0.f;
 }
 
-// MULTI = more than one 128-step tile: prefetches the next tile (more registers, 1 CTA per SM);
-// the single-tile instantiation fits 64 registers so that two CTAs share an SM.
+// Epilogue of both GAE kernels, called by every thread of a GTHREADS block (tid = linear thread index) with its own
+// sums of adv_r, adv_r^2 and adv_c: the block's partial sums in a fixed order (deterministic) go to partials row
+// blockIdx.x together with its sample count (the block's envs, block_envs of them except in the last block, times T),
+// and the last block to finish folds all partials into sums[4] = {sum adv_r, sum adv_r^2, sum adv_c, count}.
+// red: double [3][GTHREADS / 32] in shared memory.
+__device__ __forceinline__ void gae_stats_epilogue(const GaeArgs& p, int tid, int block_envs, double st_r, double st_r2,
+                                                   double st_c, double* red) {
+    constexpr int W = GTHREADS / 32;
+    __shared__ int s_last;
+    const int warp = tid >> 5, lane = tid & 31;
+    st_r = warp_sum(st_r); st_r2 = warp_sum(st_r2); st_c = warp_sum(st_c);
+    if (lane == 0) { red[warp] = st_r; red[W + warp] = st_r2; red[2 * W + warp] = st_c; }
+    __syncthreads();
+    if (tid == 0) {
+        double a = 0, b = 0, c = 0;
+        for (int w = 0; w < W; ++w) { a += red[w]; b += red[W + w]; c += red[2 * W + w]; }
+        double* o = p.partials + (size_t)blockIdx.x * 4;
+        o[0] = a; o[1] = b; o[2] = c;
+        o[3] = (double)min(block_envs, p.N - (int)blockIdx.x * block_envs) * (double)p.T;
+        __threadfence();
+        s_last = (atomicAdd(p.ticket, 1u) == gridDim.x - 1) ? 1 : 0;
+    }
+    __syncthreads();
+    if (s_last && tid < 32) {
+        __threadfence();
+        double acc[4] = {0, 0, 0, 0};
+        for (int bb = tid; bb < (int)gridDim.x; bb += 32)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) acc[q] += __ldcg(p.partials + (size_t)bb * 4 + q);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc[q] = warp_sum(acc[q]);
+        if (tid == 0) {
+            for (int q = 0; q < 4; ++q) p.sums[q] = acc[q];
+            *p.ticket = 0u;
+        }
+    }
+}
+
 // EST = advantage estimator (onpolicy_buffer.py:L299-331):
 //   0 'gae'      adv = scan(delta, gamma*lam),  target = adv + V                    (L299-303)
 //   1 'gae-rtg'  adv = scan(delta, gamma*lam),  target = discount_cumsum(rewards)   (L305-310)
@@ -93,14 +131,14 @@ __device__ __forceinline__ void gae_load_tile(const GaeArgs& p, int env, bool en
 // where `rewards` is the penalised reward path INCLUDING its bootstrap slot (finish_path subtracts
 // penalty * costs in place, L185) and the cost targets use the same gamma (L192-196).
 // RET = produce discounted_ret (third scan); training keeps no discounted_ret, so the hot instantiation drops it.
-template <bool MULTI, int EST, bool RET>
-__global__ void __launch_bounds__(GTHREADS, (MULTI || EST == 1 || EST == 3) ? 1 : 2) gae_dual_kernel(GaeArgs p) {
+// The 'gae' and 'plain' instantiations fit 64 registers, so that two CTAs share an SM.
+template <int EST, bool RET>
+__global__ void __launch_bounds__(GTHREADS, (EST == 1 || EST == 3) ? 1 : 2) gae_dual_kernel(GaeArgs p) {
     constexpr int NQ = (EST == 0 || EST == 3) ? 3 : 4;    // scanned quantities: adv_r, adv_c, reward-to-go, cost-to-go
     __shared__ double sa[NQ * GC * GPAD];
     __shared__ double sb[NQ * GC * GPAD];
     __shared__ double carry[NQ * GE];
     __shared__ double red[3 * (GTHREADS / 32)];
-    __shared__ int s_last;
 
     const int x = threadIdx.x, y = threadIdx.y;     // env lane (16), time chunk (32)
     const int lin = y * GE + x;
@@ -120,7 +158,7 @@ __global__ void __launch_bounds__(GTHREADS, (MULTI || EST == 1 || EST == 3) ? 1 
 
     for (int k = 0; k < ntiles; ++k) {
         const int t0 = T - (k + 1) * GT + y * GL;  // first step of my chunk (may be < 0)
-        if (!MULTI && k > 0) gae_load_tile(p, env, env_ok, t0, cur);   // no prefetch in the 2-CTA/SM variant
+        if (k > 0) gae_load_tile(p, env, env_ok, t0, cur);
         // fp32 deltas with the reference's three separately rounded ops; bootstrap at path ends.
         float dr[GL], dc[GL], bootr[GL], bootc[GL], r[GL], c[GL], vr[GL], vc[GL];
         bool end[GL], valid[GL];
@@ -148,8 +186,6 @@ __global__ void __launch_bounds__(GTHREADS, (MULTI || EST == 1 || EST == 3) ? 1 
         float nvr[GL], nvc[GL];   // V_{t+1} inside the path (V-trace replay)
 #pragma unroll
         for (int i = 0; i < GL; ++i) { nvr[i] = cur.vr[i + 1]; nvc[i] = cur.vc[i + 1]; }
-        // prefetch the next (earlier) tile while this one is scanned
-        if (MULTI && k + 1 < ntiles) gae_load_tile(p, env, env_ok, t0 - GT, cur);
         // pass 1: fold the chunk into affine maps (a, b) per quantity.
         const double glr = (EST == 3) ? p.g : p.gl_r, glc = (EST == 3) ? p.g : p.gl_c;
         double ar = 1.0, br = 0.0, ac = 1.0, bc = 0.0, ag = 1.0, bg = 0.0, bh = 0.0;   // (ag, bh): cost-to-go
@@ -254,35 +290,7 @@ __global__ void __launch_bounds__(GTHREADS, (MULTI || EST == 1 || EST == 3) ? 1 
         }
         __syncthreads();
     }
-    // epilogue: block partial sums for the advantage statistics (fixed order -> deterministic);
-    // the last block to finish folds all partials into sums[4].
-    st_r = warp_sum(st_r); st_r2 = warp_sum(st_r2); st_c = warp_sum(st_c);
-    if (tl == 0) { red[0 * 16 + tw] = st_r; red[1 * 16 + tw] = st_r2; red[2 * 16 + tw] = st_c; }
-    __syncthreads();
-    if (lin == 0) {
-        double a = 0, b = 0, c = 0;
-        for (int w = 0; w < GTHREADS / 32; ++w) { a += red[w]; b += red[16 + w]; c += red[32 + w]; }
-        double* o = p.partials + (size_t)blockIdx.x * 4;
-        o[0] = a; o[1] = b; o[2] = c;
-        const int nenv = min(GE, N - (int)blockIdx.x * GE);
-        o[3] = (double)nenv * (double)T;
-        __threadfence();
-        s_last = (atomicAdd(p.ticket, 1u) == gridDim.x - 1) ? 1 : 0;
-    }
-    __syncthreads();
-    if (s_last && lin < 32) {
-        __threadfence();
-        double acc[4] = {0, 0, 0, 0};
-        for (int bb = lin; bb < (int)gridDim.x; bb += 32)
-#pragma unroll
-            for (int q = 0; q < 4; ++q) acc[q] += __ldcg(p.partials + (size_t)bb * 4 + q);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) acc[q] = warp_sum(acc[q]);
-        if (lin == 0) {
-            for (int q = 0; q < 4; ++q) p.sums[q] = acc[q];
-            *p.ticket = 0u;
-        }
-    }
+    gae_stats_epilogue(p, lin, GE, st_r, st_r2, st_c, red);
 }
 
 
@@ -307,6 +315,7 @@ constexpr int SL = 8;                                   // steps per chunk
 constexpr int ST = SW * SL;                             // 128 steps per tile
 constexpr int SE = 32;                                  // envs per CTA
 constexpr int STHREADS = SW * 32;
+static_assert(STHREADS == GTHREADS, "gae_stats_epilogue reduces over GTHREADS / 32 warps");
 constexpr uint32_t S_PLANE = ST * SE * 4;               // reward / cost plane of a tile
 constexpr uint32_t S_PLANE_V = (ST + 1) * SE * 4;       // value planes carry one more row: V_{t+1} of the tile's last step
 constexpr uint32_t S_FLAGS = ST * SE;
@@ -321,60 +330,28 @@ constexpr uint32_t S_SMEM = S_OFF_BARS + 2 * NSTG * 8 + 16;
 
 struct GaeMaps { CUtensorMap rew, cost, val_r, val_c, flags; };
 
-__device__ __forceinline__ uint32_t s_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void s_mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void s_mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void s_mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ bool s_mbar_test(uint32_t bar, uint32_t parity) {
+__device__ __forceinline__ bool mbar_test_a(uint32_t bar, uint32_t parity) {
     uint32_t ok;
     asm volatile("{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
                  : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
     return ok != 0u;
 }
-__device__ __forceinline__ void s_mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t ok;
-    do {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                     : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-    } while (!ok);
-}
 // one box of a [T][N] plane -> shared memory; coordinates (env, step) may lie outside the tensor (zero fill)
-__device__ __forceinline__ void s_tma_load(uint32_t dst, const CUtensorMap* tm, int env0, int t0, uint32_t bar) {
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm, int env0, int t0, uint32_t bar) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];\n"
                  ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(env0), "r"(t0), "r"(bar) : "memory");
 }
 
-// 16 bytes global -> shared, asynchronously (LDGSTS); src_bytes == 0 zero-fills (rows / envs outside the slab)
-__device__ __forceinline__ void s_cp16(uint32_t dst, const void* src, uint32_t src_bytes) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-// this thread's earlier cp.async copies arrive on the mbarrier when they have landed (counted in the barrier's expected arrivals)
-__device__ __forceinline__ void s_cp_arrive(uint32_t bar) {
-    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];\n" ::"r"(bar) : "memory");
-}
-
-// TMA = false (OSB_GAE_LDGSTS=1): every thread copies 16-byte pieces of the tile with cp.async (LDGSTS) -- ~9 copies per thread
-//   and tile, each thread's batch arriving on the stage's mbarrier.
-// TMA = true (default): one elected thread issues cp.async.bulk.tensor.2d boxes {32 envs x 128 (129) steps}.
-//   A box of 128-byte rows 4N bytes apart costs one row request per row: the per-SM request rate, not DRAM, bounds it.
-// MODE 0: both halves by cp.async; MODE 1: both by TMA; MODE 2: the A half (reward, cost, flags) by TMA and the B half
-// (values) by cp.async -- two independent load paths working side by side.
-template <int MODE>
+// One elected thread issues the cp.async.bulk.tensor.2d boxes {32 envs x 128 (129) steps} of a tile.  A box of 128-byte
+// rows 4N bytes apart costs one row request per row: the per-SM request rate, not DRAM, bounds it.
 __global__ void __launch_bounds__(STHREADS, 1) gae_stream_kernel(const __grid_constant__ GaeMaps tm, GaeArgs p, double gl8_r, double gl8_c) {
     extern __shared__ __align__(128) uint8_t s_raw[];
-    const uint32_t pad = (128u - (s_u32(s_raw) & 127u)) & 127u;
+    const uint32_t pad = (128u - (smem_u32(s_raw) & 127u)) & 127u;
     uint8_t* sm = s_raw + pad;
-    const uint32_t sb = s_u32(sm);
+    const uint32_t sb = smem_u32(sm);
     double* sMaps = reinterpret_cast<double*>(sm + S_OFF_MAPS);
     double* sCarry = reinterpret_cast<double*>(sm + S_OFF_CARRY);
     double* sRed = reinterpret_cast<double*>(sm + S_OFF_RED);
-    __shared__ int s_last;
     const uint32_t bars = sb + S_OFF_BARS;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int N = p.N, T = p.T;
@@ -386,56 +363,28 @@ __global__ void __launch_bounds__(STHREADS, 1) gae_stream_kernel(const __grid_co
     auto fullB = [&](int s) { return bars + (uint32_t)(NSTG + s) * 8u; };
     // the two halves of a tile's load (one elected thread).  A = reward, cost, flags: dead after pass 1 of the tile that
     // used the stage; B = the two value planes: read until the end of pass 2.
-    // one 16-byte piece c of a [rows][32 envs] float plane of tile k (8 pieces per row)
-    auto cp_f32 = [&](const float* plane, uint32_t dst, int t0, int c) {
-        const int row = c >> 3, part = c & 7, t = t0 + row, e = env0 + 4 * part;
-        const bool ok = t >= 0 && t < T && e < N;
-        s_cp16(dst + (uint32_t)c * 16u, plane + (ok ? (size_t)t * N + e : 0), ok ? 16u : 0u);
-    };
     auto load_A = [&](int k) {
         const int s = k % NSTG, t0 = T - (k + 1) * ST;
         const uint32_t dst = sb + (uint32_t)s * S_STAGE;
-        if constexpr (MODE != 0) {
-            if (tid == 0) {
-                s_mbar_expect_tx(fullA(s), 2 * S_PLANE + S_FLAGS);
-                s_tma_load(dst + S_OFF_REW, &tm.rew, env0, t0, fullA(s));
-                s_tma_load(dst + S_OFF_COST, &tm.cost, env0, t0, fullA(s));
-                s_tma_load(dst + S_OFF_FL, &tm.flags, env0, t0, fullA(s));
-            }
-        } else {
-#pragma unroll
-            for (int j = 0; j < ST * 8 / STHREADS; ++j) {
-                cp_f32(p.rew, dst + S_OFF_REW, t0, tid + j * STHREADS);
-                cp_f32(p.cost, dst + S_OFF_COST, t0, tid + j * STHREADS);
-            }
-            if (tid < ST * 2) {                                          // flags: 2 pieces of 16 envs per row
-                const int row = tid >> 1, part = tid & 1, t = t0 + row, e = env0 + 16 * part;
-                const bool ok = t >= 0 && e < N;
-                s_cp16(dst + S_OFF_FL + (uint32_t)tid * 16u, p.flags + (ok ? (size_t)t * N + e : 0), ok ? 16u : 0u);
-            }
-            s_cp_arrive(fullA(s));
+        if (tid == 0) {
+            mbar_expect_tx(fullA(s), 2 * S_PLANE + S_FLAGS);
+            tma_load_2d(dst + S_OFF_REW, &tm.rew, env0, t0, fullA(s));
+            tma_load_2d(dst + S_OFF_COST, &tm.cost, env0, t0, fullA(s));
+            tma_load_2d(dst + S_OFF_FL, &tm.flags, env0, t0, fullA(s));
         }
     };
     auto load_B = [&](int k) {
         const int s = k % NSTG, t0 = T - (k + 1) * ST;
         const uint32_t dst = sb + (uint32_t)s * S_STAGE;
-        if constexpr (MODE == 1) {
-            if (tid == 0) {
-                s_mbar_expect_tx(fullB(s), 2 * S_PLANE_V);
-                s_tma_load(dst + S_OFF_VR, &tm.val_r, env0, t0, fullB(s));
-                s_tma_load(dst + S_OFF_VC, &tm.val_c, env0, t0, fullB(s));
-            }
-        } else {
-            for (int c = tid; c < (ST + 1) * 8; c += STHREADS) {
-                cp_f32(p.val_r, dst + S_OFF_VR, t0, c);
-                cp_f32(p.val_c, dst + S_OFF_VC, t0, c);
-            }
-            s_cp_arrive(fullB(s));
+        if (tid == 0) {
+            mbar_expect_tx(fullB(s), 2 * S_PLANE_V);
+            tma_load_2d(dst + S_OFF_VR, &tm.val_r, env0, t0, fullB(s));
+            tma_load_2d(dst + S_OFF_VC, &tm.val_c, env0, t0, fullB(s));
         }
     };
     if (tid == 0) {
-        for (int i = 0; i < NSTG; ++i) { s_mbar_init(fullA(i), MODE != 0 ? 1u : (uint32_t)STHREADS); s_mbar_init(fullB(i), MODE == 1 ? 1u : (uint32_t)STHREADS); }
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+        for (int i = 0; i < NSTG; ++i) { mbar_init_a(fullA(i), 1u); mbar_init_a(fullB(i), 1u); }
+        mbar_init_fence();
     }
     if (tid < 2 * 2 * 32) sCarry[tid] = 0.0;
     __syncthreads();
@@ -484,7 +433,7 @@ __global__ void __launch_bounds__(STHREADS, 1) gae_stream_kernel(const __grid_co
             }
         };
         stamp(0);
-        s_mbar_wait(fullA(0), 0u);
+        mbar_wait_a(fullA(0), 0u);
         stamp(1);
         fetch_boot(0);
 #pragma unroll 1
@@ -500,7 +449,7 @@ __global__ void __launch_bounds__(STHREADS, 1) gae_stream_kernel(const __grid_co
             const float* sVr = reinterpret_cast<const float*>(stg + S_OFF_VR) + row0 * SE + lane;
             const float* sVc = reinterpret_cast<const float*>(stg + S_OFF_VC) + row0 * SE + lane;
             const unsigned em = endmask;
-            s_mbar_wait(fullB(sg), (uint32_t)((k / NSTG) & 1));
+            mbar_wait_a(fullB(sg), (uint32_t)((k / NSTG) & 1));
             stamp(8);
             // ---- pass 1: fp32 deltas (three separately rounded ops, onpolicy_buffer.py:L301) + chunk map ----
             // (rows with t < 0 of the last tile and lanes past N see TMA zero fill: they are computed and discarded)
@@ -544,7 +493,7 @@ __global__ void __launch_bounds__(STHREADS, 1) gae_stream_kernel(const __grid_co
             // ---- path ends / bootstrap values of the next tile (its A half was requested a whole tile ago) ----------
             const bool more = k + 1 < ntiles;
             bool fetched = false;
-            if (more && s_mbar_test(fullA(sgn), phn)) { fetch_boot(k + 1); fetched = true; }
+            if (more && mbar_test_a(fullA(sgn), phn)) { fetch_boot(k + 1); fetched = true; }
             // ---- carry-in: compose the maps of the later chunks of this tile onto the tile carry -------------
             double Ar = sCarry[((s ^ 1) * 2 + 0) * 32 + lane], Ac = sCarry[((s ^ 1) * 2 + 1) * 32 + lane];
 #pragma unroll
@@ -580,48 +529,10 @@ __global__ void __launch_bounds__(STHREADS, 1) gae_stream_kernel(const __grid_co
             }
             if (warp == 0) { sCarry[(s * 2 + 0) * 32 + lane] = Ar; sCarry[(s * 2 + 1) * 32 + lane] = Ac; }
             stamp(fetched ? 6 : 7);
-            if (more && !fetched) { s_mbar_wait(fullA(sgn), phn); fetch_boot(k + 1); }
-        }
-        st_r = warp_sum(st_r); st_r2 = warp_sum(st_r2); st_c = warp_sum(st_c);
-        if (lane == 0) { sRed[warp] = st_r; sRed[SW + warp] = st_r2; sRed[2 * SW + warp] = st_c; }
-    }
-    __syncthreads();
-    if (tid == 0) {
-        double a = 0, b = 0, c = 0;
-        for (int w = 0; w < SW; ++w) { a += sRed[w]; b += sRed[SW + w]; c += sRed[2 * SW + w]; }
-        double* o = p.partials + (size_t)blockIdx.x * 4;
-        o[0] = a; o[1] = b; o[2] = c;
-        o[3] = (double)min(SE, N - env0) * (double)T;
-        __threadfence();
-        s_last = (atomicAdd(p.ticket, 1u) == gridDim.x - 1) ? 1 : 0;
-    }
-    __syncthreads();
-    if (s_last && tid < 32) {
-        __threadfence();
-        double acc[4] = {0, 0, 0, 0};
-        for (int bb = tid; bb < (int)gridDim.x; bb += 32)
-#pragma unroll
-            for (int q = 0; q < 4; ++q) acc[q] += __ldcg(p.partials + (size_t)bb * 4 + q);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) acc[q] = warp_sum(acc[q]);
-        if (tid == 0) {
-            for (int q = 0; q < 4; ++q) p.sums[q] = acc[q];
-            *p.ticket = 0u;
+            if (more && !fetched) { mbar_wait_a(fullA(sgn), phn); fetch_boot(k + 1); }
         }
     }
-}
-
-// sums[4] = {sum adv_r, sum adv_r^2, sum adv_c, count}; one warp, fixed order.
-__global__ void gae_stats_reduce_kernel(const double* __restrict__ partials, int nblocks,
-                                        double* __restrict__ sums) {
-    double acc[4] = {0, 0, 0, 0};
-    for (int b = threadIdx.x; b < nblocks; b += 32)
-#pragma unroll
-        for (int q = 0; q < 4; ++q) acc[q] += partials[(size_t)b * 4 + q];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) acc[q] = warp_sum(acc[q]);
-    if (threadIdx.x == 0)
-        for (int q = 0; q < 4; ++q) sums[q] = acc[q];
+    gae_stats_epilogue(p, tid, SE, st_r, st_r2, st_c, sRed);
 }
 
 // moments[4] = {mean_r, std_r + 1e-8, mean_c, 1}  (vector_onpolicy_buffer.py:L131-136)
@@ -720,38 +631,32 @@ static bool osb_plane_map(CUtensorMap* m, const void* base, int T, int N, int el
 }
 // returns 0 when launched, 1 when the shape / alignment / driver does not allow the TMA path (caller falls back)
 static int osb_gae_stream_launch(const GaeArgs& a, cudaStream_t s) {
-    static const bool legacy = getenv("OSB_GAE_LEGACY") != nullptr;
-    if (legacy || (a.N & 15) != 0) return 1;                      // row strides of the u8 plane must be 16 B multiples
+    if ((a.N & 15) != 0) return 1;                                // row strides of the u8 plane must be 16 B multiples
     const uintptr_t al = (uintptr_t)a.rew | (uintptr_t)a.cost | (uintptr_t)a.val_r | (uintptr_t)a.val_c | (uintptr_t)a.flags;
     if (al & 15u) return 1;
-    static const int mode = getenv("OSB_GAE_LDGSTS") ? 0 : getenv("OSB_GAE_TMA") ? 1 : getenv("OSB_GAE_MIXED") ? 2 : 1;
-    const bool use_tma = mode != 0;
     static GaeMaps maps = {};
-    if (use_tma) {
-        struct Key { const void* p[5]; int T, N; };
-        static Key key = {};
-        static bool have = false;
-        const Key now = {{a.rew, a.cost, a.val_r, a.val_c, a.flags}, a.T, a.N};
-        if (!have || memcmp(&key, &now, sizeof(Key)) != 0) {
-            if (!osb_plane_map(&maps.rew, a.rew, a.T, a.N, 4, ST) || !osb_plane_map(&maps.cost, a.cost, a.T, a.N, 4, ST) ||
-                !osb_plane_map(&maps.val_r, a.val_r, a.T, a.N, 4, ST + 1) || !osb_plane_map(&maps.val_c, a.val_c, a.T, a.N, 4, ST + 1) ||
-                !osb_plane_map(&maps.flags, a.flags, a.T, a.N, 1, ST)) { have = false; return 1; }
-            key = now; have = true;
-        }
+    struct Key { const void* p[5]; int T, N; };
+    static Key key = {};
+    static bool have = false;
+    const Key now = {{a.rew, a.cost, a.val_r, a.val_c, a.flags}, a.T, a.N};
+    if (!have || memcmp(&key, &now, sizeof(Key)) != 0) {
+        if (!osb_plane_map(&maps.rew, a.rew, a.T, a.N, 4, ST) || !osb_plane_map(&maps.cost, a.cost, a.T, a.N, 4, ST) ||
+            !osb_plane_map(&maps.val_r, a.val_r, a.T, a.N, 4, ST + 1) || !osb_plane_map(&maps.val_c, a.val_c, a.T, a.N, 4, ST + 1) ||
+            !osb_plane_map(&maps.flags, a.flags, a.T, a.N, 1, ST)) { have = false; return 1; }
+        key = now; have = true;
     }
     static bool attr = false;
     if (!attr) {
-        if (cudaFuncSetAttribute(gae_stream_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S_SMEM + 128)) != cudaSuccess ||
-            cudaFuncSetAttribute(gae_stream_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S_SMEM + 128)) != cudaSuccess ||
-            cudaFuncSetAttribute(gae_stream_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S_SMEM + 128)) != cudaSuccess) { (void)cudaGetLastError(); return 1; }
+        if (cudaFuncSetAttribute(gae_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S_SMEM + 128)) != cudaSuccess) {
+            (void)cudaGetLastError();
+            return 1;
+        }
         attr = true;
     }
     double g8r = 1.0, g8c = 1.0;
     for (int i = 0; i < SL; ++i) { g8r *= a.gl_r; g8c *= a.gl_c; }
     const int nblk = (a.N + SE - 1) / SE;
-    if (mode == 1) gae_stream_kernel<1><<<nblk, STHREADS, S_SMEM + 128, s>>>(maps, a, g8r, g8c);
-    else if (mode == 2) gae_stream_kernel<2><<<nblk, STHREADS, S_SMEM + 128, s>>>(maps, a, g8r, g8c);
-    else gae_stream_kernel<0><<<nblk, STHREADS, S_SMEM + 128, s>>>(maps, a, g8r, g8c);
+    gae_stream_kernel<<<nblk, STHREADS, S_SMEM + 128, s>>>(maps, a, g8r, g8c);
     return 0;
 }
 
@@ -788,28 +693,25 @@ int osb_adv_estimate(const float* rew, const float* cost, const float* val_r, co
     a.sums = sums;
     a.ticket = reinterpret_cast<unsigned int*>(workspace + (size_t)nblocks * 4 + 1);
     cudaStream_t s = (cudaStream_t)stream;
-    // the 64-register instantiation (two CTAs per SM) is the default: it keeps two CTAs per SM resident, which the
-    // register-hungry prefetching variant does not; that one is kept for experiments (OSB_GAE_PREFETCH=1)
-    static const bool prefetch = getenv("OSB_GAE_PREFETCH") != nullptr;
+    // the training path ('gae', no discounted_ret slab) runs the streaming kernel; every other estimator, a
+    // discounted_ret slab, and a shape the streaming kernel cannot take run the generic kernel
     const bool ret = disc_ret != nullptr;
     const dim3 blk(GE, GC);
     if (estimator == 1) {
-        if (ret) gae_dual_kernel<false, 1, true><<<nblocks, blk, 0, s>>>(a);
-        else gae_dual_kernel<false, 1, false><<<nblocks, blk, 0, s>>>(a);
+        if (ret) gae_dual_kernel<1, true><<<nblocks, blk, 0, s>>>(a);
+        else gae_dual_kernel<1, false><<<nblocks, blk, 0, s>>>(a);
     } else if (estimator == 2) {
-        if (ret) gae_dual_kernel<false, 2, true><<<nblocks, blk, 0, s>>>(a);
-        else gae_dual_kernel<false, 2, false><<<nblocks, blk, 0, s>>>(a);
+        if (ret) gae_dual_kernel<2, true><<<nblocks, blk, 0, s>>>(a);
+        else gae_dual_kernel<2, false><<<nblocks, blk, 0, s>>>(a);
     } else if (estimator == 3) {
-        if (ret) gae_dual_kernel<false, 3, true><<<nblocks, blk, 0, s>>>(a);
-        else gae_dual_kernel<false, 3, false><<<nblocks, blk, 0, s>>>(a);
-    } else if (prefetch && T > GT) {
-        gae_dual_kernel<true, 0, true><<<nblocks, blk, 0, s>>>(a);
+        if (ret) gae_dual_kernel<3, true><<<nblocks, blk, 0, s>>>(a);
+        else gae_dual_kernel<3, false><<<nblocks, blk, 0, s>>>(a);
     } else if (ret) {
-        gae_dual_kernel<false, 0, true><<<nblocks, blk, 0, s>>>(a);
+        gae_dual_kernel<0, true><<<nblocks, blk, 0, s>>>(a);
     } else if (osb_gae_stream_launch(a, s) != 0) {
-        // training path (no discounted_ret slab) when the TMA streaming kernel cannot take the shape (N % 16 != 0,
-        // unaligned slabs) or OSB_GAE_LEGACY is set: the two-scan instantiation of the generic kernel
-        gae_dual_kernel<false, 0, false><<<nblocks, blk, 0, s>>>(a);
+        // the streaming kernel cannot take the shape (N % 16 != 0, unaligned slabs), or its tensor maps or shared-memory
+        // size cannot be set up
+        gae_dual_kernel<0, false><<<nblocks, blk, 0, s>>>(a);
     }
     OSB_LAUNCH_CHECK();
     return OSB_OK;

@@ -59,6 +59,29 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity)) {
     }
 }
+// the same on 32-bit shared addresses, for barriers placed in dynamic shared memory by offset
+__device__ __forceinline__ void mbar_init_a(uint32_t bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(bar) : "memory");
+}
+// one arrival that also makes the current phase wait for `bytes` of asynchronous (TMA) copies to land
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
+    uint32_t ok;
+    do {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+            "selp.u32 %0, 1, 0, p;\n\t}\n"
+            : "=r"(ok)
+            : "r"(bar), "r"(parity)
+            : "memory");
+    } while (!ok);
+}
 
 // generic-proxy smem writes -> visible to the async proxy (tensor core operand reads)
 __device__ __forceinline__ void fence_async_smem() {

@@ -259,8 +259,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
             stage_policy_old(misc + MF_OLD, tid, (tid < A) ? __ldg(p.lc.logstd_old + tid) : 0.f);
     } else {
         if (tid == NEPI) {
-            for (int i = 0; i < NBAR; ++i)
-                asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar(i)), "r"(bar_arrivals(i)) : "memory");
+            for (int i = 0; i < NBAR; ++i) mbar_init_a(bar(i), bar_arrivals(i));
             mbar_init_fence();
         }
     }
@@ -1007,7 +1006,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 // weights: ONE bulk copy (TMA) of the image the Adam owners just wrote; biases / log_std: a few scalar loads
                 if (tid == 0) {
                     asm volatile("fence.proxy.async.global;\n" ::: "memory");       // generic-proxy writes (other SMs, acquired above) -> async-proxy read
-                    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(bar(RDY_W)), "r"(W_IMG) : "memory");
+                    mbar_expect_tx(bar(RDY_W), W_IMG);
                     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
                                  ::"r"(sbase + OFF_W1), "l"(wimg), "r"(W_IMG), "r"(bar(RDY_W)) : "memory");
                 }

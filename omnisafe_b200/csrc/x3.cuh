@@ -382,22 +382,7 @@ __device__ __forceinline__ void store1_x3(uint32_t base, uint32_t split, uint32_
     sts16(base + off, (uint16_t)w0); sts16(base + split + off, (uint16_t)w1); sts16(base + 2 * split + off, (uint16_t)w2);
 }
 
-// ---- mbarrier / issue helpers on 32-bit shared addresses ----------------------------------------------
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
-    uint32_t ok;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}\n"
-            : "=r"(ok)
-            : "r"(bar), "r"(parity)
-            : "memory");
-    } while (!ok);
-}
+// ---- issue helpers on 32-bit shared addresses ---------------------------------------------------------
 // mma_commit on a 32-bit shared address
 __device__ __forceinline__ void mma_commit_a(uint32_t bar) {
     __threadfence_block();

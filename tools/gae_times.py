@@ -1,10 +1,10 @@
 """CUDA-event timing of the dual-GAE launch (training configuration: no discounted_ret slab) at several horizons."""
-import json, os, sys
+import json, sys
 import torch
 sys.path.insert(0, '.')
 from omnisafe_b200.common.buffer import VectorOnPolicyBuffer
 
-out = {'kernel': 'gae_dual_kernel<false, 0, false> (OSB_GAE_LEGACY)' if os.environ.get('OSB_GAE_LEGACY') else ('gae_stream_kernel<cp.async> (OSB_GAE_LDGSTS)' if os.environ.get('OSB_GAE_LDGSTS') else 'gae_stream_kernel<TMA>')}
+out = {'kernel': 'gae_stream_kernel<TMA>'}
 for T, N in ((128, 4096), (512, 4096), (2048, 4096), (4096, 4096), (128, 32768)):
     buf = VectorOnPolicyBuffer(4, 2, T, 0.99, 0.95, 0.95, 'gae', 0.0, True, True, num_envs=N, device='cuda', keep_discounted_ret=False)
     for k in ('reward', 'cost', 'value_r', 'value_c', 'boot_r', 'boot_c'):
