@@ -15,7 +15,6 @@ kernel step.
 from __future__ import annotations
 
 import contextlib
-import math
 
 import torch
 from torch.distributions import Normal
@@ -135,30 +134,30 @@ class CriticValue(torch.autograd.Function):
         (obs,) = ctx.saved_tensors
         c = ctx.critic
         e = c._engine
-        grad = torch.zeros(c.size, dtype=torch.float32, device=obs.device)
+        grad = torch.zeros(e.P, dtype=torch.float32, device=obs.device)   # kernel layout, so the pads are in place
         B = obs.shape[0]
         if B > 0:
             nb = c._launch(obs, dv.to(torch.float32).contiguous(), None)
-            lib().osb_reduce_partials(ptr(e.gpart[c.start:]), nb, e.P, c.size, 1.0, 0, 0.0, ptr(grad),
+            lib().osb_reduce_partials(ptr(e.gpart[c.start:]), nb, e.P, c.size, 1.0, 0, 0.0, ptr(grad[c.start:]),
                                       current_stream())
-        return (None, None, *(g.view(p.shape) for g, p in zip(grad.split(c.sizes), c._params)))
+        return (None, None, *c._pmap.views(grad, c.name).values())
 
 
 class TrainingCritic:
     """What `self._actor_critic.reward_critic` / `.cost_critic` is while a critic hook runs: the reference's VCritic API
     (`critic(obs)` -> [value]) and nn.Module's `parameters()` / `named_parameters()`: leaf tensors with the reference's
-    names, shapes and order that are views of the network's slice of the flat `theta`, so they always hold what the
-    kernels train."""
+    names, shapes and order that are views of the network's blocks of the flat `theta` (ParamMap.views; strided for
+    hidden widths below 64), so they always hold what the kernels train."""
 
     def __init__(self, engine, net: int) -> None:
         self._engine, self.net = engine, net            # net: 1 reward critic, 2 cost critic
-        lay = engine.agent.layout['reward_critic' if net == 1 else 'cost_critic']
+        self.name = 'reward_critic' if net == 1 else 'cost_critic'
+        agent = engine.agent
+        self._pmap = agent.param_map
+        lay = agent.layout[self.name]
         self.start, self.size = lay['start'], lay['size']
-        theta = engine.agent.theta
-        self._named = [(name, theta[off:off + math.prod(shape)].view(*shape).requires_grad_(True))
-                       for name, (off, shape) in lay['entries'].items()]
+        self._named = [(name, v.requires_grad_(True)) for name, v in self._pmap.views(agent.theta, self.name).items()]
         self._params = [p for _, p in self._named]
-        self.sizes = [p.numel() for p in self._params]
 
     def _launch(self, obs: torch.Tensor, dv: torch.Tensor, value: torch.Tensor | None) -> int:
         """osb_critic_dv_backward on rows obs [B, O] into the engine's partials; returns their row count."""
@@ -184,8 +183,13 @@ class TrainingCritic:
         return iter(self._named)
 
     def flat_grad(self) -> torch.Tensor:
-        """The leaves' gradients as one flat vector in layout order (zero where a leaf has none)."""
-        return torch.cat([(p.grad if p.grad is not None else torch.zeros_like(p)).reshape(-1) for p in self._params])
+        """The leaves' gradients as the network's slice of the kernel layout: zero where a leaf has none and at the
+        pads."""
+        grad = torch.zeros(self._engine.P, dtype=torch.float32, device=self._params[0].device)
+        for g, p in zip(self._pmap.views(grad, self.name).values(), self._params):
+            if p.grad is not None:
+                g.copy_(p.grad)
+        return grad[self.start:self.start + self.size]
 
 
 class TrainingCriticOptimizer:

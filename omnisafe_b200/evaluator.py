@@ -45,7 +45,7 @@ from omnisafe_b200.adapter.saute_adapter import per_step_budget
 from omnisafe_b200.common.normalizer import Normalizer
 from omnisafe_b200.envs.core import check_env, is_registered, make, needs_wrappers
 from omnisafe_b200.envs.synthetic import SyntheticBoxEnv, support_envs
-from omnisafe_b200.models.actor_critic import param_layout
+from omnisafe_b200.models.actor_critic import HID, ParamMap
 from omnisafe_b200.utils.config import Config
 
 PRECISIONS = {'fp32': 0, 'tf32': 1, 'bf16x3': 2}
@@ -94,13 +94,11 @@ class Evaluator:
             self._wrapped = needs_wrappers(probe)
             self._time_limit = TIME_LIMIT if getattr(probe, 'need_time_limit_wrapper', False) else 0
         On, A = self._obs_dim + int(self._saute), self._act_dim
-        # the actor's flat parameters in the rollout's layout (the critics are not evaluated)
-        layout = param_layout(On, A)
-        theta = torch.zeros(layout['total'], dtype=torch.float32)
-        for name, (off, shape) in layout['actor']['entries'].items():
-            w = params['pi'][name]
-            assert tuple(w.shape) == shape, f"'pi'.{name} has shape {tuple(w.shape)}, expected {shape}"
-            theta[off:off + w.numel()] = w.reshape(-1).float()
+        # the actor's flat parameters in the kernel layout, zero-padded to width 64 (the critics are not evaluated)
+        actor_cfgs = getattr(getattr(cfgs, 'model_cfgs', None), 'actor', None)
+        pmap = ParamMap(On, A, actor_hidden=getattr(actor_cfgs, 'hidden_sizes', [HID, HID]))
+        theta = torch.zeros(pmap.kernel['total'], dtype=torch.float32)
+        pmap.load_state_dict(theta, 'actor', params['pi'], what="'pi'")
         self._theta = theta.to(self._device)
         self._obs_normalize = bool(getattr(a, 'obs_normalize', True))
         self._norm_sd = params['obs_normalizer'] if self._obs_normalize else None

@@ -1,1 +1,1 @@
-from omnisafe_b200.models.actor_critic import ConstraintActorCritic, param_layout  # noqa: F401
+from omnisafe_b200.models.actor_critic import ConstraintActorCritic, ParamMap, param_layout  # noqa: F401

@@ -11,6 +11,11 @@ kernels share it.  `actor_state_dict()` re-exports the actor under the reference
 `{'pi': ..., 'obs_normalizer': ...}` checkpoints stay loadable by the reference Evaluator
 (omnisafe/evaluator.py:L153-178, algorithms/on_policy/base/policy_gradient.py:L183-189).
 
+`model_cfgs.actor.hidden_sizes` and `model_cfgs.critic.hidden_sizes` may be any two widths from 1 to 64.  `theta`, the
+gradient and the Adam moments keep the 64-wide kernel layout; a narrower network sits in it zero-padded (ParamMap), which
+owns the one mapping between the reference's shapes and that layout: `named_views`, `actor_state_dict()`, the
+initialisation, the critic hooks, the evaluator and the golden fixtures all go through it.
+
 The reference's model API on a trained policy -- `step` / `forward`, `actor.predict / forward / log_prob / std` and
 `reward_critic(obs)` / `cost_critic(obs)` -- runs on one batched launch of the policy-step kernel (csrc/policy.cu,
 osb_policy_step) in the model's `precision` (0 fp32, 1 tf32, 2 bf16x3; the algorithms set it from
@@ -30,18 +35,25 @@ from torch.distributions.utils import _standard_normal
 from omnisafe_b200._lib import lib, ptr
 from omnisafe_b200.utils.train_state import restore, snapshot
 
-HID = 64
+HID = 64     # the hidden width every kernel computes
 NET_ACTOR, NET_REWARD, NET_COST = 1, 2, 4   # net_mask bits of osb_policy_step
+NETS = ('actor', 'reward_critic', 'cost_critic')
 
 
-def param_layout(obs_dim: int, act_dim: int, hid: int = HID) -> dict:
+def param_layout(obs_dim: int, act_dim: int, hid: int = HID, *, actor_hidden=None, critic_hidden=None) -> dict:
+    """Offsets and shapes of the flat vector [actor | reward_critic | cost_critic] in the reference's named_parameters()
+    order, for two-hidden-layer networks: both layers `hid` wide, or of widths `actor_hidden` / `critic_hidden` where
+    given.  The default is the kernel layout, the one `theta`, its gradient and the Adam moments always have; other
+    widths give the reference layout of a narrower model."""
     O, A = obs_dim, act_dim
-    actor = [('log_std', (A,)), ('mean.0.weight', (hid, O)), ('mean.0.bias', (hid,)),
-             ('mean.2.weight', (hid, hid)), ('mean.2.bias', (hid,)), ('mean.4.weight', (A, hid)),
+    a1, a2 = (hid, hid) if actor_hidden is None else actor_hidden
+    c1, c2 = (hid, hid) if critic_hidden is None else critic_hidden
+    actor = [('log_std', (A,)), ('mean.0.weight', (a1, O)), ('mean.0.bias', (a1,)),
+             ('mean.2.weight', (a2, a1)), ('mean.2.bias', (a2,)), ('mean.4.weight', (A, a2)),
              ('mean.4.bias', (A,))]
-    critic = [('critic_0.0.weight', (hid, O)), ('critic_0.0.bias', (hid,)),
-              ('critic_0.2.weight', (hid, hid)), ('critic_0.2.bias', (hid,)),
-              ('critic_0.4.weight', (1, hid)), ('critic_0.4.bias', (1,))]
+    critic = [('critic_0.0.weight', (c1, O)), ('critic_0.0.bias', (c1,)),
+              ('critic_0.2.weight', (c2, c1)), ('critic_0.2.bias', (c2,)),
+              ('critic_0.4.weight', (1, c2)), ('critic_0.4.bias', (1,))]
     out, off = {}, 0
     for net, spec in (('actor', actor), ('reward_critic', critic), ('cost_critic', critic)):
         start, entries = off, {}
@@ -53,22 +65,77 @@ def param_layout(obs_dim: int, act_dim: int, hid: int = HID) -> dict:
     return out
 
 
+class ParamMap:
+    """Where the reference's parameters of networks with hidden widths `actor_hidden` [a1, a2] and `critic_hidden`
+    [c1, c2] (both critics) live in the kernel layout.
+
+    Every kernel computes 64-wide hidden layers.  A narrower network is the 64-wide one with its real weights in the
+    leading rows / columns of each padded matrix and zeros everywhere else: a padded unit has z = 0 and tanh(0) = 0, every
+    product touching a pad is +-0 in every precision, and every gradient at a pad is +-0, so Adam, clipping, the Fisher
+    products and CG leave the pads at +0 and the padded network computes exactly the narrow one."""
+
+    def __init__(self, obs_dim: int, act_dim: int, actor_hidden=(HID, HID), critic_hidden=(HID, HID)) -> None:
+        for which, hs in (('actor', actor_hidden), ('critic', critic_hidden)):
+            assert isinstance(hs, (list, tuple)) and len(hs) == 2 and all(
+                isinstance(h, (int, np.integer)) and not isinstance(h, bool) and 1 <= h <= HID for h in hs), (
+                f'model_cfgs.{which}.hidden_sizes must be exactly two hidden layers of widths 1..{HID}, got {hs!r}')
+        self.actor_hidden = tuple(int(h) for h in actor_hidden)
+        self.critic_hidden = tuple(int(h) for h in critic_hidden)
+        self.kernel = param_layout(obs_dim, act_dim)
+        self.ref = param_layout(obs_dim, act_dim, actor_hidden=self.actor_hidden, critic_hidden=self.critic_hidden)
+
+    def views(self, theta: torch.Tensor, net: str) -> dict[str, torch.Tensor]:
+        """The reference's parameters of `net` as views of a kernel-layout vector: each is the leading block of its
+        padded tensor (the whole tensor at width 64, a strided view below)."""
+        out = {}
+        for name, (off, shape) in self.kernel[net]['entries'].items():
+            block = tuple(slice(0, n) for n in self.ref[net]['entries'][name][1])
+            out[name] = theta[off:off + int(np.prod(shape))].view(*shape)[block]
+        return out
+
+    def to_kernel(self, flat) -> torch.Tensor:
+        """A reference-order flat vector (`ref` layout) as a kernel-layout vector with zero pads."""
+        flat = torch.as_tensor(flat)
+        assert flat.shape == (self.ref['total'],), f'expected a flat vector of {self.ref["total"]}, got {tuple(flat.shape)}'
+        theta = torch.zeros(self.kernel['total'], dtype=flat.dtype, device=flat.device)
+        for net in NETS:
+            for name, view in self.views(theta, net).items():
+                off, shape = self.ref[net]['entries'][name]
+                view.copy_(flat[off:off + view.numel()].view(shape))
+        return theta
+
+    def to_ref(self, theta) -> torch.Tensor:
+        """A kernel-layout vector as the reference-order flat vector (pads dropped)."""
+        theta = torch.as_tensor(theta)
+        return torch.cat([v.reshape(-1) for net in NETS for v in self.views(theta, net).values()])
+
+    def state_dict(self, theta: torch.Tensor, net: str) -> dict[str, torch.Tensor]:
+        """`net`'s parameters under the reference's names and shapes: contiguous CPU copies."""
+        return {k: v.detach().cpu().contiguous().clone() for k, v in self.views(theta, net).items()}
+
+    def load_state_dict(self, theta: torch.Tensor, net: str, state: dict, what: str = '') -> None:
+        """Copy a reference-shaped state dict of `net` into its blocks of the kernel-layout `theta` (pads untouched)."""
+        for name, view in self.views(theta, net).items():
+            assert name in state, f'{what or net} has no {name!r}'
+            w = torch.as_tensor(state[name])
+            assert tuple(w.shape) == tuple(view.shape), (
+                f'{what or net}.{name} has shape {tuple(w.shape)}, expected {tuple(view.shape)}')
+            view.copy_(w)
+
+
 class ConstraintActorCritic:
-    NETS = ('actor', 'reward_critic', 'cost_critic')
+    NETS = NETS
 
     def __init__(self, obs_dim: int, act_dim: int, model_cfgs, epochs: int, device='cuda',
                  generator: torch.Generator | None = None) -> None:
-        hs_a = list(model_cfgs.actor.hidden_sizes)
-        hs_c = list(model_cfgs.critic.hidden_sizes)
-        assert hs_a == [HID, HID] and hs_c == [HID, HID], (
-            'the fused sm_90a kernels are specialised for hidden_sizes [64, 64]')
+        self.param_map = ParamMap(obs_dim, act_dim, model_cfgs.actor.hidden_sizes, model_cfgs.critic.hidden_sizes)
         assert model_cfgs.actor.activation == 'tanh' and model_cfgs.critic.activation == 'tanh', (
             'the fused kernels implement tanh activations')
         assert model_cfgs.actor_type == 'gaussian_learning'
         assert model_cfgs.weight_initialization_mode == 'kaiming_uniform'
         self.obs_dim, self.act_dim = int(obs_dim), int(act_dim)
         self.device = torch.device(device)
-        self.layout = param_layout(obs_dim, act_dim)
+        self.layout = self.param_map.kernel
         P = self.layout['total']
         self.theta = torch.zeros(P, dtype=torch.float32, device=self.device)
         self.grad = torch.zeros(P, dtype=torch.float32, device=self.device)
@@ -86,20 +153,20 @@ class ConstraintActorCritic:
         self.reward_critic = VCritic(self, NET_REWARD)
         self.cost_critic = VCritic(self, NET_COST)
 
-    # -- initialisation (utils/model.py:L25-44: kaiming_uniform_(a=sqrt(5)); torch default bias)
+    # -- initialisation (utils/model.py:L25-44: kaiming_uniform_(a=sqrt(5)); torch default bias) --------------------
     def _init_parameters(self, generator) -> None:
+        """Each layer's real block drawn with its real fan-in, weight then bias, layer by layer; the pads stay 0."""
         theta = torch.zeros(self.layout['total'], dtype=torch.float32)
         for net in self.NETS:
-            ent = self.layout[net]['entries']
-            names = list(ent)
+            views = self.param_map.views(theta, net)
+            names = list(views)
             for wname, bname in zip(names[-6::2], names[-5::2]):
-                off, shape = ent[wname]
-                fan_in = shape[1]
+                w, b = views[wname], views[bname]
+                fan_in = w.shape[1]
                 bw = math.sqrt(6.0 / ((1.0 + 5.0) * fan_in))
-                theta[off:off + shape[0] * shape[1]].uniform_(-bw, bw, generator=generator)
-                boff, bshape = ent[bname]
+                w.copy_(torch.empty(w.shape).uniform_(-bw, bw, generator=generator))
                 bb = 1.0 / math.sqrt(fan_in)
-                theta[boff:boff + bshape[0]].uniform_(-bb, bb, generator=generator)
+                b.copy_(torch.empty(b.shape).uniform_(-bb, bb, generator=generator))
         self.theta.copy_(theta)
 
     # -- views ------------------------------------------------------------------------------
@@ -108,13 +175,14 @@ class ConstraintActorCritic:
         return slice(e['start'], e['start'] + e['size'])
 
     def named_views(self, net: str) -> dict[str, torch.Tensor]:
-        return {name: self.theta[off:off + int(np.prod(shape))].view(*shape)
-                for name, (off, shape) in self.layout[net]['entries'].items()}
+        """`net`'s parameters under the reference's names and shapes, as views of `theta`."""
+        return self.param_map.views(self.theta, net)
 
     def actor_state_dict(self) -> dict[str, torch.Tensor]:
-        return {k: v.detach().cpu().clone() for k, v in self.named_views('actor').items()}
+        return self.param_map.state_dict(self.theta, 'actor')
 
     def load_flat(self, theta) -> None:
+        """Load a kernel-layout vector (ParamMap.to_kernel makes one from the reference's flat order)."""
         self.theta.copy_(torch.as_tensor(theta, dtype=torch.float32))
 
     # -- learning-rate schedule (actor_critic.py:L99-113: LinearLR 1 -> 0 over `epochs`) ------
