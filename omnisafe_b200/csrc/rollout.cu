@@ -115,45 +115,69 @@ __device__ void norm_push(float& mean, float& sumsq, long long count_old, long l
     norm_push_moments(mean, sumsq, count_old, n, mraw, m2);
 }
 
-// Executed by the last-arriving CTA of a launch: folds the launch's fixed-point sums into the running statistics in
-// ObsNormalize's push order -- the final-observation rows (acc_fin, *fin_count rows; none: skipped), the next
-// observations (acc_all, n_all > 0 rows), then the reset rows (acc_rst, n_rst rows; none or null: skipped) -- and clears
-// the sums and fin_count.  stats1: mean1 / std1 / count[1] / had_fin take the state after the final rows, which the
-// bootstrap values of the next step's truncated paths are computed from.  push = false: only count[0] advances.
-__device__ void norm_fold(const NormState& ns, int O, long long n_all, bool stats1, bool push = true,
-                          long long* acc_rst = nullptr, long long n_rst = 0) {
-    __threadfence();
-    const int nfin = *((volatile int*)ns.fin_count);
-    long long count = __ldcg(ns.count);          // (.cg: in the persistent kernel another SM may have written these last step)
+// The running statistics a fold updates: NormState's own, or a CTA's shared-memory copy of them (the persistent kernel).
+struct NormStats {
+    float *mean, *sumsq, *std, *mean1, *std1;
+    long long* count;   // [2]
+    int* had_fin;
+};
+
+// A fold's arithmetic, by every thread of one CTA: the fixed-point sums of a step pushed into s in ObsNormalize's push
+// order -- the final-observation rows (acc_fin, nfin rows; none: skipped), the next observations (acc_all, n_all > 0
+// rows), then the reset rows (acc_rst, n_rst rows; none or null: skipped).  count is s.count[0] before the fold; ld reads
+// s's arrays; per_col(j) runs after column j.  stats1: mean1 / std1 / count[1] / had_fin take the state after the final
+// rows, which the bootstrap values of the next step's truncated paths are computed from.  push = false: only count[0]
+// advances.
+template <class Ld, class PerCol>
+__device__ __forceinline__ void norm_fold_stats(const NormStats& s, Ld&& ld, int O, long long count, int nfin,
+                                                const long long* acc_all, const long long* acc_fin, long long n_all,
+                                                bool stats1, bool push, const long long* acc_rst, long long n_rst,
+                                                PerCol&& per_col) {
     for (int j = threadIdx.x; push && j < O; j += blockDim.x) {
-        float mean = __ldcg(ns.mean + j), sumsq = __ldcg(ns.sumsq + j);
+        float mean = ld(s.mean + j), sumsq = ld(s.sumsq + j);
         long long c = count;
         if (nfin > 0) {
-            norm_push(mean, sumsq, c, nfin, __ldcg(ns.acc_fin + j), __ldcg(ns.acc_fin + O + j));
+            norm_push(mean, sumsq, c, nfin, __ldcg(acc_fin + j), __ldcg(acc_fin + O + j));
             c += nfin;
             if (stats1) {
-                ns.mean1[j] = mean;
-                ns.std1[j] = norm_std(sumsq, c);
+                s.mean1[j] = mean;
+                s.std1[j] = norm_std(sumsq, c);
             }
         }
-        norm_push(mean, sumsq, c, n_all, __ldcg(ns.acc_all + j), __ldcg(ns.acc_all + O + j));
+        norm_push(mean, sumsq, c, n_all, __ldcg(acc_all + j), __ldcg(acc_all + O + j));
         c += n_all;
         if (n_rst > 0) {
             norm_push(mean, sumsq, c, n_rst, __ldcg(acc_rst + j), __ldcg(acc_rst + O + j));
             c += n_rst;
         }
-        ns.mean[j] = mean;
-        ns.sumsq[j] = sumsq;
-        ns.std[j] = norm_std(sumsq, c);
-        ns.acc_all[j] = 0; ns.acc_all[O + j] = 0;
-        ns.acc_fin[j] = 0; ns.acc_fin[O + j] = 0;
-        if (acc_rst) { acc_rst[j] = 0; acc_rst[O + j] = 0; }
+        s.mean[j] = mean;
+        s.sumsq[j] = sumsq;
+        s.std[j] = norm_std(sumsq, c);
+        per_col(j);
     }
     __syncthreads();
     if (threadIdx.x == 0) {
-        if (stats1) ns.count[1] = count + nfin;
-        ns.count[0] = count + nfin + n_all + n_rst;
-        if (stats1) *ns.had_fin = nfin > 0 ? 1 : 0;
+        if (stats1) s.count[1] = count + nfin;
+        s.count[0] = count + nfin + n_all + n_rst;
+        if (stats1) *s.had_fin = nfin > 0 ? 1 : 0;
+    }
+}
+
+// Executed by the last-arriving CTA of a launch: folds the launch's fixed-point sums into the running statistics
+// (norm_fold_stats) and clears the sums, fin_count and the ticket.
+__device__ void norm_fold(const NormState& ns, int O, long long n_all, bool stats1, bool push = true,
+                          long long* acc_rst = nullptr, long long n_rst = 0) {
+    __threadfence();
+    const int nfin = *((volatile int*)ns.fin_count);
+    const long long count = __ldcg(ns.count);    // (.cg: written by another CTA in an earlier launch)
+    norm_fold_stats(NormStats{ns.mean, ns.sumsq, ns.std, ns.mean1, ns.std1, ns.count, ns.had_fin},
+                    [](const float* a) { return __ldcg(a); }, O, count, nfin, ns.acc_all, ns.acc_fin, n_all, stats1,
+                    push, acc_rst, n_rst, [&](int j) {
+                        ns.acc_all[j] = 0; ns.acc_all[O + j] = 0;
+                        ns.acc_fin[j] = 0; ns.acc_fin[O + j] = 0;
+                        if (acc_rst) { acc_rst[j] = 0; acc_rst[O + j] = 0; }
+                    });
+    if (threadIdx.x == 0) {
         *ns.fin_count = 0;
         *ns.ticket = 0u;
     }
@@ -310,6 +334,7 @@ struct StepArgs {
     int precision;        // 0 = fp32 FMA tiles of 32 envs, 1 = wgmma TF32 tiles of 128 envs, 2 = split-bf16 wgmma tiles (O <= 64)
     unsigned int* bar_ctr;    // persistent epoch kernel: grid-barrier arrival counter and release flag (zero at launch)
     unsigned int* bar_flag;
+    long long* ring;          // persistent training kernel: 3 RING_SLOTs of normaliser sums (zero at launch)
     long long* dbg;           // optional clock64 stamps (persistent kernel), normally null
     float* acc;               // tensor-core tiles: accumulator images, one [128][TC_COLS] per CTA
     // external-env act step (EXT instantiations only): the sampled action after ActionScale onto [act_lo, act_hi]
@@ -629,6 +654,20 @@ __device__ __forceinline__ void grid_step_barrier(const StepArgs& p, int t, int&
     __syncthreads();
 }
 
+// The same barrier without a last arriver's work: every CTA arrives and waits for the others.
+__device__ __forceinline__ void grid_step_arrive_wait(const StepArgs& p, int t) {
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const unsigned all = gridDim.x * gridDim.y * (unsigned)(t + 1);
+        unsigned v;
+        asm volatile("atom.release.gpu.global.add.u32 %0, [%1], 1;" : "=r"(v) : "l"(p.bar_ctr) : "memory");
+        ++v;
+        while (v < all) asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p.bar_ctr) : "memory");
+    }
+    __syncthreads();
+}
+
 // EXT = true: the act half of a step on a user env (csrc: osb_ext_act).  The network part is the same; the actor CTAs
 // hand the scaled action to the env through p.act_env instead of running the synthetic transition, and the normaliser is
 // fed by the observe kernel after env.step.
@@ -843,6 +882,7 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
 // split-bf16, fp32-level values / log-probs).  Everything around the forward (ObsNormalize, sampling, env transition,
 // slab append, normaliser sums, ticket) is the arithmetic of rollout_step_kernel.
 constexpr int RTC = TC_ROWS;
+constexpr int RTA = 64;       // envs per actor tile of the persistent training kernel
 constexpr int SNW = KC + 1;   // row stride of the next-state staging tiles
 
 // the 4-byte-word region after the operand tiles (all offsets in words)
@@ -862,13 +902,22 @@ constexpr int TF_GSTEP = TF_STEP + RTC;           // [128] total steps of the en
 constexpr int TF_SD = TF_GSTEP + RTC;             // [3][16] sigma, 2 sigma^2, log sigma per action
 constexpr int TF_EARLY = TF_SD + 48;              // [128] accumulated cost incl. this step (EarlyTerminated)
 constexpr int TF_WORDS = TF_EARLY + RTC;
-static_assert(TF_ACC % 2 == 0, "the fixed-point sums need 8-byte alignment");
+// persistent training kernel only: its own copy of the running statistics (NormStats)
+constexpr int TF_NS = TF_WORDS;                   // [5][64] mean, sumsq, std, mean1, std1
+constexpr int TF_NCNT = TF_NS + 5 * 64;           // long long [2] count, then int had_fin
+constexpr int TF_WORDS_PERSIST = TF_NCNT + 6;
+static_assert(TF_ACC % 2 == 0 && TF_NCNT % 2 == 0, "the fixed-point sums and counts need 8-byte alignment");
+
+// The persistent training kernel's normaliser sums: a ring of three slots, step t adding into slot t % 3.  Slot layout
+// in long longs: acc_all [2][O] at 0, acc_fin [2][O] at 128, fin_count (an int) at 256.
+constexpr int RING_SLOT = 258;
+__device__ __forceinline__ long long* ring_slot(long long* ring, int t) { return ring + (t % 3) * RING_SLOT; }
 
 // PERSIST = true: ONE cooperative launch runs the whole epoch (steps 0 .. T, the last one being the critics' epoch-end
-// bootstrap): the weight tiles, biases and the accumulator image allocation stay resident, every step ends in a grid barrier whose
-// last arriver folds the step's normaliser sums into the running statistics before it releases the others
+// bootstrap): the weight tiles, biases and the accumulator image allocation stay resident, every step ends in a grid barrier
+// after which every CTA folds the step's normaliser sums into its own copy of the running statistics (RING below)
 // (adapter/onpolicy_adapter.py:L58-136 is the loop this replaces).  Data written by other CTAs in earlier steps
-// (raw states, flags, normaliser statistics) is read with ld.global.cg.
+// (raw states, flags, normaliser sums) is read with ld.global.cg.
 // EXT = true: the act half of a step on a user env, as in rollout_step_kernel<true> (never persistent: Python runs
 // env.step between the launches).
 // EVAL = true: the evaluation of a saved policy, as in rollout_step_kernel<EXT, true>; PERSIST (synthetic env only): ONE
@@ -900,20 +949,32 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
     uint32_t* sGstep = reinterpret_cast<uint32_t*>(fbase + TF_GSTEP);
     float* sSd = fbase + TF_SD;
     float* sEarlyAcc = fbase + TF_EARLY;
+    // RING: the persistent training kernel.  Every CTA holds the running statistics in shared memory (sNs, loaded at
+    // launch) and folds each step's sums from the ring into them after the step's barrier, so that the barrier is a
+    // plain arrive / wait; the designated CTA clears the ring slot of step t - 2 in step t and writes sNs back to
+    // NormState at the end.
+    constexpr bool RING = PERSIST && !EVAL;
+    const NormStats sNs{fbase + TF_NS, fbase + TF_NS + 64, fbase + TF_NS + 128, fbase + TF_NS + 192, fbase + TF_NS + 256,
+                        reinterpret_cast<long long*>(fbase + TF_NCNT), reinterpret_cast<int*>(fbase + TF_NCNT + 4)};
     __shared__ uint64_t bar;
     __shared__ int s_last, s_anyfin;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int q = warp & 3, h = warp >> 2;
-    const int net = PERSIST ? (int)blockIdx.y : (p.is_tail ? (int)blockIdx.y + 1 : (int)blockIdx.y);
-    const int env0 = blockIdx.x * RTC;
     const int O = p.es.O, A = p.es.A, N = p.N, T = p.T;
+    // RING: a 1-D grid of ceil(N / RTA) actor CTAs on tiles of R = RTA envs, then ceil(N / RTC) CTAs per critic on tiles
+    // of R = RTC envs (ring_grid).  Otherwise grid = (env tiles of RTC) x networks.
+    const int n_act = (N + RTA - 1) / RTA, n_crit = (N + RTC - 1) / RTC, cb = (int)blockIdx.x - n_act;
+    const int net = RING ? (cb < 0 ? 0 : 1 + cb / n_crit)
+                         : PERSIST ? (int)blockIdx.y : (p.is_tail ? (int)blockIdx.y + 1 : (int)blockIdx.y);
+    const int R = (RING && net == 0) ? RTA : RTC;
+    const int env0 = RING ? (cb < 0 ? (int)blockIdx.x * RTA : (cb % n_crit) * RTC) : (int)blockIdx.x * RTC;
     const int On = O + (p.sa.safety ? 1 : 0);            // network input width (Saute: [obs | z]), <= 64 here
     const NetLayout L = net_layout(net, On, A);
     const float* theta = p.theta + net_offset(net, On, A);
     const int e_env = tid >> 1, e_half = tid & 1;       // actor CTAs: 2 threads per env in the transition
     const int my_env = env0 + e_env;
-    const bool my_ok = (net == 0) && my_env < N;
+    const bool my_ok = (net == 0) && (!RING || e_env < R) && my_env < N;
 
     tc_stage_weights<X3>(B0, theta, L, On, sB1, sB2, sB3);
     if (net == 0 && tid < 16) {          // Normal(mu, sigma): sigma = exp(log_std) is state independent
@@ -921,15 +982,25 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
         sSd[tid] = sd; sSd[16 + tid] = __fmul_rn(2.f, __fmul_rn(sd, sd)); sSd[32 + tid] = logf(sd);
     }
     if (tid == 0) { mbar_init(&bar, 1); mbar_init_fence(); s_anyfin = 0; }
+    const bool designated = RING && blockIdx.x == gridDim.x - 1;   // a cost-critic CTA: off the actors' chain
+    if constexpr (RING) {
+        if (tid < O) {
+            sNs.mean[tid] = __ldcg(p.ns.mean + tid); sNs.sumsq[tid] = __ldcg(p.ns.sumsq + tid);
+            sNs.std[tid] = __ldcg(p.ns.std + tid);
+            sNs.mean1[tid] = __ldcg(p.ns.mean1 + tid); sNs.std1[tid] = __ldcg(p.ns.std1 + tid);
+        }
+        if (tid == 0) { sNs.count[0] = __ldcg(p.ns.count); sNs.count[1] = __ldcg(p.ns.count + 1); *sNs.had_fin = __ldcg(p.ns.had_fin); }
+    }
     __syncthreads();
     const Acc tm = acc_cta(p.acc, TC_COLS);
     const uint32_t lane_base = (uint32_t)(q * 32) << 16;
     uint32_t phase = 0;
 
     // development aid (tools/rollout_stage_times.py): clock64 stamps of thread 0 of the first actor and reward-critic CTA
-    const bool dbg_on = PERSIST && p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y < 2 && tid == 0;
+    const bool dbg_on = PERSIST && p.dbg != nullptr && tid == 0 &&
+                        (RING ? (blockIdx.x == 0 || cb == 0) : (blockIdx.x == 0 && blockIdx.y < 2));
     int dbg_n = 0;
-#define RSTAMP(id) do { if (dbg_on && dbg_n < 250) { long long* d_ = p.dbg + (blockIdx.y ? 512 : 0); d_[1 + 2 * dbg_n] = (id); d_[2 + 2 * dbg_n] = clock64(); ++dbg_n; d_[0] = dbg_n; } } while (0)
+#define RSTAMP(id) do { if (dbg_on && dbg_n < 250) { long long* d_ = p.dbg + (net ? 512 : 0); d_[1 + 2 * dbg_n] = (id); d_[2 + 2 * dbg_n] = clock64(); ++dbg_n; d_[0] = dbg_n; } } while (0)
     const int t_first = PERSIST ? 0 : p.t, t_last = PERSIST ? T : p.t;
 #pragma unroll 1
     for (int t = t_first; t <= t_last; ++t) {
@@ -938,12 +1009,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
     if (EVAL && PERSIST && t > 0 && __ldcg(p.ev.ctr) == 0) break;   // every env has finished (uniform after the barrier)
     const float* eps_t = PERSIST ? (p.eps ? p.eps + (size_t)t * N * A : nullptr) : p.eps;
     const uint32_t gstep_t = PERSIST ? p.global_step + (uint32_t)t : p.global_step;
-    const bool normalize = p.es.obs_normalize && __ldcg(p.ns.count) > 1;
+    const bool normalize = p.es.obs_normalize && (RING ? sNs.count[0] : __ldcg(p.ns.count)) > 1;
     const float* s_cur = p.st.s_raw + (size_t)(t & 1) * N * O;
     float* s_nxt = p.st.s_raw + (size_t)((t + 1) & 1) * N * O;
     if (PERSIST) { if (tid == 0) s_anyfin = 0; __syncthreads(); }
     // which envs of this tile finish in this step (time limit / hash-driven termination): known before the forward
-    if (!EXT && !EVAL && net == 0 && tid < RTC) {
+    if (!EXT && !EVAL && net == 0 && tid < R) {
         const int env = env0 + tid;
         int fl = 0, ep_step = 0; uint32_t epi = 0, gstep = 0;
         if (env < N) {
@@ -964,19 +1035,22 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
 #pragma unroll 1
     for (int pass = first_pass; pass < 2; ++pass) {
         const float* raw = pass ? s_cur : p.st.final_raw + (size_t)((t - 1) & 1) * N * O;
-        const float* gmean = pass ? p.ns.mean : p.ns.mean1;
-        const float* gstd = pass ? p.ns.std : p.ns.std1;
-        const bool norm_on = pass ? normalize : (p.es.obs_normalize && __ldcg(p.ns.count + 1) > 1);
+        const float* gmean = RING ? (pass ? sNs.mean : sNs.mean1) : (pass ? p.ns.mean : p.ns.mean1);
+        const float* gstd = RING ? (pass ? sNs.std : sNs.std1) : (pass ? p.ns.std : p.ns.std1);
+        const bool norm_on = pass ? normalize : (p.es.obs_normalize && (RING ? sNs.count[1] : __ldcg(p.ns.count + 1)) > 1);
         float* obs_out = (!EVAL && pass && net == 0) ? p.sl.obs + (size_t)t * N * On : nullptr;
         const bool own_state = !EVAL && PERSIST && pass && net == 0 && t > t_first;
-        if (tid < 64) { sMean[tid] = (tid < O) ? __ldcg(gmean + tid) : 0.f; sStd[tid] = (tid < O) ? __ldcg(gstd + tid) : 1.f; }
+        if (tid < 64) {
+            sMean[tid] = (tid < O) ? (RING ? gmean[tid] : __ldcg(gmean + tid)) : 0.f;
+            sStd[tid] = (tid < O) ? (RING ? gstd[tid] : __ldcg(gstd + tid)) : 1.f;
+        }
         __syncthreads();
         if ((O & 3) == 0 && On == O) {   // 128-bit row loads, all 8 in flight per thread
             const int kq = tid & 15, k4 = kq << 2;
             float4 xv[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                const int env = env0 + (tid >> 4) + 16 * j;
+                const int env = (!RING || 16 * j < R) ? env0 + (tid >> 4) + 16 * j : N;   // rows past the tile: not loaded
                 if (own_state) {          // persistent kernel, actor CTA: the state this CTA wrote in the previous step is still in smem
                     const float* r = sRaw + ((tid >> 4) + 16 * j) * SNW + k4;
                     xv[j] = (env < N && k4 < O) ? make_float4(r[0], r[1], r[2], r[3]) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -988,6 +1062,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
             const float s0 = sStd[k4], s1 = sStd[k4 + 1], s2 = sStd[k4 + 2], s3 = sStd[k4 + 3];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
+                if constexpr (RING) {
+                    if (16 * j >= R) break;
+                }
                 const int e = (tid >> 4) + 16 * j;
                 const int env = env0 + e;
                 float4 v = xv[j];
@@ -1018,24 +1095,34 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
         } else {
             const int k = tid & 63;
             const float mk = sMean[k], sk = sStd[k];
-#pragma unroll 8
-            for (int j = 0; j < 32; ++j) {
-                const int e = (tid >> 6) + 4 * j;
-                const int env = env0 + e;
-                float v = 0.f;
-                if (env < N && k < O) {
-                    v = own_state ? sRaw[e * SNW + k] : __ldcg(raw + (size_t)env * O + k);
-                    if (pass && net == 0) sRaw[e * SNW + k] = v;
-                    if (norm_on) v = norm_clip(v, mk, sk);
-                    if (obs_out) obs_out[(size_t)env * On + k] = v;
+#pragma unroll 1
+            for (int j0 = 0; j0 < 32; j0 += 8) {   // 8 rows at a time, their loads all in flight
+                if constexpr (RING) {
+                    if (4 * j0 >= R) break;                       // rows past the actor tile
                 }
-                if constexpr (X3) x3::store1_x3(B0, TcTiles<true>::SUB, x3::off128(e, k), v);
-                else sts(tile_addr(B0, e, k, RTC), tf32r(v));
+                float xv[8];
+#pragma unroll
+                for (int u = 0; u < 8; ++u) {
+                    const int e = (tid >> 6) + 4 * (j0 + u), env = env0 + e;
+                    xv[u] = (env < N && k < O) ? (own_state ? sRaw[e * SNW + k] : __ldcg(raw + (size_t)env * O + k)) : 0.f;
+                }
+#pragma unroll
+                for (int u = 0; u < 8; ++u) {
+                    const int e = (tid >> 6) + 4 * (j0 + u), env = env0 + e;
+                    float v = xv[u];
+                    if (env < N && k < O) {
+                        if (pass && net == 0) sRaw[e * SNW + k] = v;
+                        if (norm_on) v = norm_clip(v, mk, sk);
+                        if (obs_out) obs_out[(size_t)env * On + k] = v;
+                    }
+                    if constexpr (X3) x3::store1_x3(B0, TcTiles<true>::SUB, x3::off128(e, k), v);
+                    else sts(tile_addr(B0, e, k, RTC), tf32r(v));
+                }
             }
         }
         if (On != O) {          // Saute: column O of the tile = the safety state (1 on final observations)
             __syncthreads();    // the staging loop above zero-filled that column
-            if (tid < RTC) {
+            if (tid < R) {
                 const int env = env0 + tid;
                 float z = 0.f;
                 if (env < N) {
@@ -1049,9 +1136,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
         fence_async_smem();
         __syncthreads();
         RSTAMP(2);
-        tc_forward<X3>(B0, tm, &bar, phase, sB1, sB2, 1, TcNop{}, [&](int l) {   // bf16x3: stamps 3-5, one per layer
+        auto stamp = [&](int l) {   // bf16x3: stamps 3-5, one per layer
             if (X3) RSTAMP(2 + l);
-        });
+        };
+        // bf16x3 actor tiles of RTA = 64 envs: one m64 block per layer.  tf32 runs its 128-row forward on them too, rows
+        // past the tile computing values nobody reads.
+        if constexpr (X3 && RING) {
+            if (net == 0) tc_forward<X3, RTA>(B0, tm, &bar, phase, sB1, sB2, 1, TcNop{}, stamp);
+            else tc_forward<X3>(B0, tm, &bar, phase, sB1, sB2, 1, TcNop{}, stamp);
+        } else {
+            tc_forward<X3>(B0, tm, &bar, phase, sB1, sB2, 1, TcNop{}, stamp);
+        }
         if (h == 0) {
             float o16[16];
             acc_ld16(tm, lane_base + TC_C_OUT, o16);
@@ -1090,7 +1185,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
         if (A <= 8) {
             const int pr = tid & 3, a0 = 2 * pr, a1 = a0 + 1;
 #pragma unroll 1
-            for (int g = 0; g < 2; ++g) {
+            for (int g = 0; 64 * g < R; ++g) {
                 const int e = 64 * g + (tid >> 2);
                 const int env = env0 + e;
                 const bool ok = env < N;
@@ -1118,7 +1213,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
         } else {
             const int qq = tid & 7;
 #pragma unroll 1
-            for (int g = 0; g < RTC / 32; ++g) {
+            for (int g = 0; 32 * g < R; ++g) {
                 const int e = 32 * g + (tid >> 3);
                 const int env = env0 + e;
                 const bool ok = env < N;
@@ -1143,7 +1238,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
         if constexpr (EXT) return;
         __syncthreads();
         if (p.et.cost_acc) {      // EarlyTerminated: the step's cost is known from state dim 0 -> finish flags before the transition
-            if (tid < RTC && env0 + tid < N) {
+            if (tid < R && env0 + tid < N) {
                 const int env = env0 + tid;
                 const float acc = __fadd_rn(p.et.cost_acc[env], env_step_cost(p.es, sRaw[tid * SNW], sAct[tid * OUTP], __ldg(p.st.bias)));
                 if (acc > p.et.cost_limit) sFlag[tid] = early_end(sFlag[tid]);
@@ -1152,17 +1247,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
             __syncthreads();
         }
         RSTAMP(7);
-        // ---- env transition + normaliser sums, elementwise: thread -> (dim j = tid % 64, env quarter g = tid / 64).
+        // ---- env transition + normaliser sums, elementwise: thread -> (dim j = tid % 64, env quarter g = tid / 64 of the
+        //      tile's R envs).
         //      The raw state comes from shared memory (kept by the obs staging), the next state goes out in whole
         //      rows (coalesced), the fixed-point column sums accumulate in registers. ---------------------------------------
         {
-            const int j = tid & 63, g = tid >> 6;
+            const int j = tid & 63, g = tid >> 6, eq = R >> 2;
             long long sx = 0, sxx = 0, fx = 0, fxx = 0;
             if (j < O) {
                 const int ja = j % A;
                 const float bj = __ldg(p.st.bias + j);
 #pragma unroll 4
-                for (int e = 32 * g; e < 32 * g + 32; ++e) {
+                for (int e = eq * g; e < eq * g + eq; ++e) {
                     const int env = env0 + e;
                     if (env < N) {
                         const float a = env_action(sAct[e * OUTP + ja]);
@@ -1210,26 +1306,42 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
                                    sEarlyAcc[e_env]);
         }
         if (p.es.obs_normalize) {
+            NormState ns = p.ns;
+            if constexpr (RING) {
+                long long* slot = ring_slot(p.ring, t);
+                ns.acc_all = slot; ns.acc_fin = slot + 128; ns.fin_count = reinterpret_cast<int*>(slot + 256);
+            }
             if (tid < O) {
                 long long a0 = 0, a1 = 0, a2 = 0, a3 = 0;
                 for (int gg = 0; gg < 4; ++gg) {
                     a0 += sAcc[(gg * 4 + 0) * 64 + tid]; a1 += sAcc[(gg * 4 + 1) * 64 + tid];
                     a2 += sAcc[(gg * 4 + 2) * 64 + tid]; a3 += sAcc[(gg * 4 + 3) * 64 + tid];
                 }
-                push_fix_sums(p.ns, O, tid, a0, a1, a2, a3);
+                push_fix_sums(ns, O, tid, a0, a1, a2, a3);
             }
             if (tid == 64) {
                 int nfin = 0;
-                for (int r = 0; r < RTC; ++r) nfin += (env0 + r < N) ? (sFlag[r] & EP_FIN) : 0;
-                if (nfin) atomicAdd(p.ns.fin_count, nfin);
+                for (int r = 0; r < R; ++r) nfin += (env0 + r < N) ? (sFlag[r] & EP_FIN) : 0;
+                if (nfin) atomicAdd(ns.fin_count, nfin);
             }
         }
     }
     RSTAMP(9);
-    if (PERSIST) {
+    if constexpr (RING) {
         if (!is_tail) {
-            grid_step_barrier(p, t, s_last, [&] { if (p.es.obs_normalize) norm_fold(p.ns, O, N, true); });
+            if (designated) {   // slot (t + 1) % 3 held step t - 2's sums, which every CTA folded before barrier t - 1
+                long long* slot = ring_slot(p.ring, t + 1);
+                for (int i = tid; i < RING_SLOT; i += NTHREADS) slot[i] = 0;
+            }
+            grid_step_arrive_wait(p, t);
             RSTAMP(10);
+            if (p.es.obs_normalize) {
+                const long long* slot = ring_slot(p.ring, t);
+                norm_fold_stats(sNs, [](const float* a) { return *a; }, O, sNs.count[0], __ldcg(reinterpret_cast<const int*>(slot + 256)),
+                                slot, slot + 128, N, true, true, nullptr, 0, [](int) {});
+                __syncthreads();
+                RSTAMP(11);
+            }
         }
     } else if (!EXT && p.es.obs_normalize && !is_tail && last_cta(p.ns.ticket)) {
         norm_fold(p.ns, O, N, true);
@@ -1237,11 +1349,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
     }   // step loop
 #undef RSTAMP
     __syncthreads();
+    if (designated) {   // the host, checkpoints and the next epoch read the running statistics from NormState
+        if (tid < O) {
+            p.ns.mean[tid] = sNs.mean[tid]; p.ns.sumsq[tid] = sNs.sumsq[tid]; p.ns.std[tid] = sNs.std[tid];
+            p.ns.mean1[tid] = sNs.mean1[tid]; p.ns.std1[tid] = sNs.std1[tid];
+        }
+        if (tid == 0) { p.ns.count[0] = sNs.count[0]; p.ns.count[1] = sNs.count[1]; *p.ns.had_fin = *sNs.had_fin; }
+    }
 }
 
-// 1024: the alignment pad in front of the operand tiles
-static size_t rollout_tc_smem_bytes(bool x3) {
-    return 1024 + (x3 ? TcTiles<true>::FLOATS : TcTiles<false>::FLOATS) + TF_WORDS * sizeof(float) + 64;
+// 1024: the alignment pad in front of the operand tiles.  ring: the persistent training kernel (its NormStats copy).
+static size_t rollout_tc_smem_bytes(bool x3, bool ring) {
+    return 1024 + (x3 ? TcTiles<true>::FLOATS : TcTiles<false>::FLOATS) + (ring ? TF_WORDS_PERSIST : TF_WORDS) * sizeof(float) + 64;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1831,7 +1950,10 @@ static int ext_refuse_if_capturing(cudaStream_t stream, const char* what) {
     return OSB_ERR_UNSUPPORTED;
 }
 
-static size_t rollout_tc_acc_bytes(int N) { return (size_t)((N + RTC - 1) / RTC) * 3 * 128 * TC_COLS * sizeof(float); }
+// CTAs of the persistent training kernel: ceil(N / RTA) actor tiles, then ceil(N / RTC) tiles per critic
+static int ring_grid(int N) { return (N + RTA - 1) / RTA + 2 * ((N + RTC - 1) / RTC); }
+// one [128][TC_COLS] image per CTA, enough for every grid (ring_grid(N) >= 3 ceil(N / RTC))
+static size_t rollout_tc_acc_bytes(int N) { return (size_t)ring_grid(N) * 128 * TC_COLS * sizeof(float); }
 
 static int sm_count() {
     static int n_sm = 0;
@@ -1843,10 +1965,15 @@ static int sm_count() {
 static bool tc_tiles(const StepArgs& p) {
     return (p.precision == 1 || p.precision == 2) && p.es.O + (p.sa.safety ? 1 : 0) <= 64;
 }
-// the persistent kernel needs every CTA (env tiles x networks) resident
-static bool persistent_fits(const StepArgs& p, int nets) { return tc_tiles(p) && (p.N + RTC - 1) / RTC * nets <= sm_count(); }
+// the persistent kernels need every CTA resident: training ring_grid(N), evaluation one actor CTA per RTC envs
+static bool persistent_fits(const StepArgs& p, bool eval) {
+    return tc_tiles(p) && (eval ? (p.N + RTC - 1) / RTC : ring_grid(p.N)) <= sm_count();
+}
 
-static unsigned int* g_grid_bar = nullptr;   // grid-barrier arrival counter and release flag of the persistent kernels
+// the persistent kernels' grid-barrier arrival counter and release flag (64 bytes), then the training kernel's ring of
+// normaliser sums (3 RING_SLOTs)
+static unsigned int* g_grid_bar = nullptr;
+constexpr size_t GRID_BAR_BYTES = 64 + 3 * RING_SLOT * sizeof(long long);
 
 // One launch of the step kernels: a training step (EVAL = false: grid = env tiles x the actor and both critics, the
 // epoch-end tail only the critics) or an evaluation step (grid = env tiles x the actor); on the synthetic env or, EXT,
@@ -1857,7 +1984,7 @@ static int launch_rollout(StepArgs& p, cudaStream_t stream, bool persistent = fa
     const int nets = EVAL ? 1 : (p.is_tail ? 2 : 3);
     if (tc_tiles(p)) {
         const bool x3 = p.precision == 2;
-        const size_t smem_tc = rollout_tc_smem_bytes(x3);
+        const size_t smem_tc = rollout_tc_smem_bytes(x3, persistent && !EVAL);
         static bool attr_tc = false;
         if (!attr_tc) {
             if constexpr (EXT) {
@@ -1870,7 +1997,7 @@ static int launch_rollout(StepArgs& p, cudaStream_t stream, bool persistent = fa
                                      (const void*)rollout_step_tc_kernel<true, true, false, EVAL>};
             for (int i = 0; i < (EXT ? 2 : 4); ++i)
                 OSB_CUDA(cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (int)rollout_tc_smem_bytes(i & 1)));
+                                              (int)rollout_tc_smem_bytes(i & 1, i >= 2 && !EVAL)));
             attr_tc = true;
         }
         if constexpr (EXT) {
@@ -1880,12 +2007,13 @@ static int launch_rollout(StepArgs& p, cudaStream_t stream, bool persistent = fa
         p.acc = acc_scratch(ACC_ROLLOUT, rollout_tc_acc_bytes(p.N));
         if (!p.acc) return OSB_ERR_CUDA;
         if (prepare_only) return OSB_OK;
-        const dim3 grid_tc((p.N + RTC - 1) / RTC, nets);
+        const dim3 grid_tc = (persistent && !EVAL) ? dim3(ring_grid(p.N)) : dim3((p.N + RTC - 1) / RTC, nets);
         if (persistent) {
             // every CTA resident: the step barrier is a software grid barrier
-            if (!g_grid_bar) OSB_CUDA(cudaMalloc(&g_grid_bar, 64));
+            if (!g_grid_bar) OSB_CUDA(cudaMalloc(&g_grid_bar, GRID_BAR_BYTES));
             p.bar_ctr = g_grid_bar; p.bar_flag = g_grid_bar + 1;
-            OSB_CUDA(cudaMemsetAsync(p.bar_ctr, 0, 2 * sizeof(unsigned int), stream));
+            p.ring = reinterpret_cast<long long*>(g_grid_bar + 16);
+            OSB_CUDA(cudaMemsetAsync(p.bar_ctr, 0, EVAL ? 2 * sizeof(unsigned int) : GRID_BAR_BYTES, stream));
             void* args[] = {&p};
             osb_count_launch();
             OSB_CUDA(cudaLaunchCooperativeKernel(x3 ? (void*)rollout_step_tc_kernel<true, true, false, EVAL>
@@ -1980,8 +2108,9 @@ int osb_rollout_epoch(int O, int A, int max_episode_steps, unsigned seed, unsign
     int rc = launch_env_reset(p.es, p.st, p.ns, N, s);
     if (rc) return rc;
     p.dbg = g_rollout_dbg;
-    // tensor-core modes with every CTA resident: one persistent launch per epoch
-    if (persistent_fits(p, 3)) {
+    // tensor-core modes with every CTA resident: one persistent launch per epoch.  OSB_ROLLOUT_PER_STEP=1 keeps one
+    // launch per step, the persistent kernel's reference.
+    if (persistent_fits(p, false) && !getenv("OSB_ROLLOUT_PER_STEP")) {
         p.t = 0; p.is_tail = 0; p.eps = eps_all; p.global_step = epoch_index * (unsigned)T;
         rc = launch_rollout<false, false>(p, s, true);
         if (rc) return rc;
@@ -2046,7 +2175,7 @@ int osb_eval_synthetic(int O, int A, int max_episode_steps, unsigned seed, unsig
     // every env's first episode starts from a reset, its observations pushed as one batch (a vector env's reset)
     env_reset_kernel<<<(N + RT - 1) / RT, NTHREADS, 0, s>>>(p.es, p.st, p.ns, p.sa, N);
     OSB_LAUNCH_CHECK();
-    if (!per_step && persistent_fits(p, 1)) {   // p.T bounds the persistent kernel's steps
+    if (!per_step && persistent_fits(p, true)) {   // p.T bounds the persistent kernel's steps
         p.t = 0;
         return launch_rollout<false, true>(p, s, true);
     }

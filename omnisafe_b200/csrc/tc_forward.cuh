@@ -192,12 +192,17 @@ struct TcNop {
 // stage(c) stages chunk c of X (bf16x3: the whole tile, c = 0) right before layer 1 consumes it; tf32 runs layer 1 as a
 // K loop over nchunks chunks.  stage = TcNop: the caller has staged, fenced and synchronised the whole X tile.
 // after(l) runs in every thread once layer l's MMAs completed (l = 1, 2, 3).
-template <bool X3, class Stage, class After = TcNop>
+// ROWS = 64 (bf16x3 only): rows 0 .. 63 of the tile, one m64 block per layer (rows 64 .. 127 are neither read nor
+// written).  A row of an m64 block depends only on that row and the k-step order, so each row has the bits of the
+// 128-row forward.  The epilogues then give each row 4 threads: warp w owns rows 32 (w % 2) + lane, columns 16 (w / 2) ..
+// 16 (w / 2) + 15.
+template <bool X3, int ROWS = 128, class Stage, class After = TcNop>
 __device__ __forceinline__ void tc_forward(uint32_t base, const umma::Acc& tm, uint64_t* bar, uint32_t& phase,
                                            const float* sB1, const float* sB2, int nchunks, Stage&& stage,
                                            After&& after = After{}) {
     using namespace umma;
     using T = TcTiles<X3>;
+    static_assert(ROWS == 128 || (X3 && ROWS == 64), "the tf32 forward runs 128-row tiles");
     constexpr bool staged = std::is_same<typename std::decay<Stage>::type, TcNop>::value;
     auto stage_chunk = [&](int c) {
         if constexpr (!staged) {
@@ -218,38 +223,45 @@ __device__ __forceinline__ void tc_forward(uint32_t base, const umma::Acc& tm, u
         // meet (named barrier 4 + q), and store the pieces over them.
         static_assert(x3::staged_in_own_rows<64>(T::SUB), "a staged row leaves its own bytes of the activation buffer");
         const x3::Staged sZ{base + T::X, T::SUB};
+        // ROWS = 64: the 4 warps of row block w % 2 read their rows, meet (named barrier 4 + w % 2), and store
+        constexpr int CW = ROWS == 128 ? 32 : 16;                          // columns per thread
+        const int er = ROWS == 128 ? 32 * q + lane : 32 * (warp & 1) + lane, ec = ROWS == 128 ? 32 * h : 16 * (warp >> 1);
+        const int eb = ROWS == 128 ? 4 + q : 4 + (warp & 1), en = ROWS == 128 ? 64 : 128;
         auto hidden = [&](const float* sB) {   // tanh(Z + b) over the activation buffer
-            float v[4][8];
+            float v[CW / 8][8];
 #pragma unroll
-            for (int c8 = 0; c8 < 4; ++c8) {
-                const int c0 = 32 * h + 8 * c8;
-                x3::staged_load<64>(sZ, 32 * q + lane, c0, v[c8]);
+            for (int c8 = 0; c8 < CW / 8; ++c8) {
+                const int c0 = ec + 8 * c8;
+                x3::staged_load<64>(sZ, er, c0, v[c8]);
 #pragma unroll
                 for (int i = 0; i < 8; ++i) v[c8][i] = x3::tanh_acc(v[c8][i] + sB[c0 + i]);
             }
-            asm volatile("bar.sync %0, 64;\n" ::"r"(4 + q) : "memory");
+            asm volatile("bar.sync %0, %1;\n" ::"r"(eb), "r"(en) : "memory");
 #pragma unroll
-            for (int c8 = 0; c8 < 4; ++c8) x3::store8_x3(base + T::X, T::SUB, 32 * q + lane, 32 * h + 8 * c8, v[c8]);
+            for (int c8 = 0; c8 < CW / 8; ++c8) x3::store8_x3(base + T::X, T::SUB, er, ec + 8 * c8, v[c8]);
             fence_async_smem();
             __syncthreads();
         };
         stage_chunk(0);
         if (mma_wg) {
-            x3::gemm_x3_staged<64, 4, 0>(sZ, dAct, T::SUB, 32u, dW1, T::WSUB, 32u);
+            if constexpr (ROWS == 128) x3::gemm_x3_staged<64, 4, 0>(sZ, dAct, T::SUB, 32u, dW1, T::WSUB, 32u);
+            else x3::gemm_x3_rows<64, 4, 1, 0>(sZ, 0, dAct, T::SUB, 32u, dW1, T::WSUB, 32u);
             mma_commit(bar);
         }
         mbar_wait(bar, phase); phase ^= 1;
         after(1);
         hidden(sB1);
         if (mma_wg) {
-            x3::gemm_x3_staged<64, 4, 0>(sZ, dAct, T::SUB, 32u, dW2, T::WSUB, 32u);
+            if constexpr (ROWS == 128) x3::gemm_x3_staged<64, 4, 0>(sZ, dAct, T::SUB, 32u, dW2, T::WSUB, 32u);
+            else x3::gemm_x3_rows<64, 4, 1, 0>(sZ, 0, dAct, T::SUB, 32u, dW2, T::WSUB, 32u);
             mma_commit(bar);
         }
         mbar_wait(bar, phase); phase ^= 1;
         after(2);
         hidden(sB2);
         if (mma_wg) {
-            x3::gemm_x3<128, 16, 4, 0, 0>(tm, TC_C_OUT, dAct, T::SUB, 32u, dW3, T::W3SUB, 32u, false);
+            if constexpr (ROWS == 128) x3::gemm_x3<128, 16, 4, 0, 0>(tm, TC_C_OUT, dAct, T::SUB, 32u, dW3, T::W3SUB, 32u, false);
+            else x3::gemm_x3_rows<16, 4, 1, 0>(tm, TC_C_OUT, 0, dAct, T::SUB, 32u, dW3, T::W3SUB, 32u);   // row m in lane m
             mma_commit(bar);
         }
         mbar_wait(bar, phase); phase ^= 1;

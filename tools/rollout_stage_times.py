@@ -15,7 +15,7 @@ algo._env.rollout(algo._steps_per_epoch, algo._actor_critic, algo._buf, algo._lo
 torch.cuda.synchronize()
 lib().osb_rollout_debug_buffer(0)
 NAMES = {1: 'step start', 2: 'obs tile staged', 3: 'layer 1 MMAs done', 4: 'E1 + layer 2 MMAs done', 5: 'E2 + layer 3 MMAs done', 6: 'outputs written',
-         7: 'sampled + log-prob', 8: 'env transition', 9: 'normaliser sums', 10: 'grid barrier (+finalize)'}
+         7: 'sampled + log-prob', 8: 'env transition', 9: 'normaliser sums', 10: 'grid barrier', 11: 'normaliser fold'}
 for which, off in (('actor CTA', 0), ('reward-critic CTA', 512)):
     d = dbg[off:off + 512].cpu().tolist()
     n = d[0]
