@@ -509,6 +509,32 @@ int osb_optim_fused_p2p(const float* gpart, const float* stats_part, int nblocks
  * episode has finished yet (the reference asserts, naive_lagrange/ppo_lag.py:L74). */
 int osb_lagrange_update(const double* window_sums, float cost_limit, float lambda_lr,
                         float upper_bound, float* state, int* nan_flag, void* stream);
+/* Lagrange.update_lagrange_multiplier with lambda_optimizer = any other optimiser torch steps on a 0-d
+ * fp32 parameter given only lr (common/lagrange.py:L86-97): torch.optim.<kind> with its defaults, as
+ * its single-tensor CPU path computes it, then the clamp to [0, upper_bound] (upper_bound < 0 = none).
+ * Jc = window_sums[1] / window_sums[3]; an empty window or a NaN Jc sets *nan_flag and leaves state alone.
+ * state[OSB_LAMBDA_STATE] (fp32), initialised by the host; s[0] = lambda, s[4] = torch's step count
+ * (counted for every kind), unused slots 0:
+ *   SGD        -                                 Adagrad    s[1] sum (0)
+ *   AdamW      s[1] exp_avg (0), s[2] exp_avg_sq (0)    Adadelta   s[1] square_avg (0), s[2] acc_delta (0)
+ *   Adamax     s[1] exp_avg (0), s[2] exp_inf (0)       RMSprop    s[1] square_avg (0)
+ *   NAdam      s[1] exp_avg, s[2] exp_avg_sq, s[3] mu_product (1)
+ *   RAdam      s[1] exp_avg (0), s[2] exp_avg_sq (0)    Rprop      s[1] prev (0), s[2] step_size (lr)
+ *   ASGD       s[1] eta (lr), s[2] mu (1), s[3] ax (0)  Adafactor  s[1] variance (0) */
+#define OSB_LAMBDA_STATE 8
+#define OSB_LAMBDA_SGD 0
+#define OSB_LAMBDA_ADAMW 1
+#define OSB_LAMBDA_ADAMAX 2
+#define OSB_LAMBDA_NADAM 3
+#define OSB_LAMBDA_RADAM 4
+#define OSB_LAMBDA_RMSPROP 5
+#define OSB_LAMBDA_RPROP 6
+#define OSB_LAMBDA_ADAGRAD 7
+#define OSB_LAMBDA_ADADELTA 8
+#define OSB_LAMBDA_ASGD 9
+#define OSB_LAMBDA_ADAFACTOR 10
+int osb_lagrange_update_opt(int kind, const double* window_sums, double cost_limit, double lambda_lr,
+                            double upper_bound, float* state, int* nan_flag, void* stream);
 /* PID-Lagrangian controller step (PIDLagrangian.pid_update, common/pid_lagrange.py:L95-125) in the
  * reference's Python-float (fp64) arithmetic.  pid_state: 64 doubles {integral, EMA(delta), EMA(Jc),
  * penalty, deque length, deque head, -, -, ring[pid_d_delay]}, initialised by the host to

@@ -31,6 +31,7 @@ def parse_header(path: str = HEADER) -> dict[str, tuple[object, list[object]]]:
         text = fh.read()
     text = re.sub(r'/\*.*?\*/', '', text, flags=re.S)
     text = re.sub(r'//[^\n]*', '', text)
+    text = re.sub(r'^\s*#[^\n]*', '', text, flags=re.M)   # preprocessor lines (include guard, constants)
     protos = {}
     for m in re.finditer(r'([A-Za-z_][\w\s\*]*?)\b(osb_\w+)\s*\(([^)]*)\)\s*;', text):
         ret, name, args = m.group(1).strip(), m.group(2), m.group(3).strip()

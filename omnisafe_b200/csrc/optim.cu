@@ -11,6 +11,7 @@
 //   conjugate_gradients                  utils/math.py:L86-132
 #include "common.cuh"
 #include "mlp.cuh"
+#include "../../include/omnisafe_b200.h"
 #include <cooperative_groups.h>
 #include <string.h>
 
@@ -354,6 +355,147 @@ __global__ void lagrange_update_kernel(const double* __restrict__ window_sums, f
     state[0] = lam; state[1] = m; state[2] = v; state[3] = (float)t;
 }
 
+// lambda <- clamp(torch.optim.<kind>(lambda, grad = -(Jc - limit)), 0, upper) for every optimiser other than
+// Adam that torch steps on a 0-d fp32 parameter given only `lr` (common/lagrange.py:L86-97), each as torch's
+// single-tensor CPU path computes it: fp32 tensor ops with torch's defaults, Python-float (fp64) scalars.
+// The fp32 roundings follow torch's CPU kernels on a 0-d tensor: `add_(t, alpha)`, `addcmul_` and `lerp_`
+// fuse their multiply-add (fmaf), `addcdiv_(t1, t2, value)` is self + (value * t1) / t2, and a Python-float
+// operand is first rounded to fp32.  The fp64 scalars are formed with separately rounded operations.
+// State layout: see osb_lagrange_update_opt in include/omnisafe_b200.h.
+__device__ __forceinline__ float t_lerp(float self, float end, float w) {      // Tensor.lerp_(end, w)
+    const float d = __fsub_rn(end, self);
+    return fabsf(w) < 0.5f ? __fmaf_rn(w, d, self) : __fmaf_rn(-d, __fsub_rn(1.f, w), end);
+}
+__device__ __forceinline__ float t_addcmul(float self, float a, float b, float v) {
+    return __fmaf_rn(__fmul_rn(v, a), b, self);
+}
+__device__ __forceinline__ float t_addcdiv(float self, float a, float b, float v) {
+    return __fadd_rn(self, __fdiv_rn(__fmul_rn(v, a), b));
+}
+__device__ __forceinline__ double one_minus_pow(double b, double t) { return __dsub_rn(1.0, pow(b, t)); }
+
+__global__ void lagrange_update_opt_kernel(int kind, const double* __restrict__ window_sums, double cost_limit,
+                                           double lr, double upper_bound, float* __restrict__ s,
+                                           int* __restrict__ nan_flag) {
+    if (threadIdx.x != 0) return;
+    const double cnt = window_sums[3];
+    const double jc = window_sums[1] / cnt;
+    if (!(cnt > 0.0) || isnan(jc)) { *nan_flag = 1; return; }   // the reference asserts (ppo_lag.py:L74)
+    // grad of -lambda * (Jc - limit): the Python-float difference rounded to fp32, negated
+    const float g = -(float)__dsub_rn(jc, cost_limit);
+    float lam = s[0];
+    const double t = (double)__fadd_rn(s[4], 1.f);
+    s[4] = (float)t;
+    switch (kind) {
+    case OSB_LAMBDA_SGD:
+        lam = __fmaf_rn((float)-lr, g, lam);
+        break;
+    case OSB_LAMBDA_ADAMW:
+    case OSB_LAMBDA_ADAMAX:
+    case OSB_LAMBDA_NADAM:
+    case OSB_LAMBDA_RADAM: {
+        float m = t_lerp(s[1], g, (float)(1.0 - 0.9)), v = s[2];
+        const double bc1 = one_minus_pow(0.9, t), bc2 = one_minus_pow(0.999, t);
+        if (kind == OSB_LAMBDA_ADAMAX) {
+            v = fmaxf(__fmul_rn(v, 0.999f), __fadd_rn(fabsf(g), 1e-8f));
+            lam = t_addcdiv(lam, m, v, (float)-__ddiv_rn(lr, bc1));
+            s[1] = m; s[2] = v;
+            break;
+        }
+        v = t_addcmul(__fmul_rn(v, 0.999f), g, g, (float)(1.0 - 0.999));
+        if (kind == OSB_LAMBDA_ADAMW) {
+            // decoupled weight decay 1e-2 (AdamW's default)
+            lam = __fmul_rn(s[0], (float)__dsub_rn(1.0, __dmul_rn(lr, 1e-2)));
+            const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), (float)sqrt(bc2)), 1e-8f);
+            lam = t_addcdiv(lam, m, denom, (float)-__ddiv_rn(lr, bc1));
+        } else if (kind == OSB_LAMBDA_NADAM) {
+            const double mu = __dmul_rn(0.9, __dsub_rn(1.0, __dmul_rn(0.5, pow(0.96, __dmul_rn(t, 4e-3)))));
+            const double mu_next =
+                __dmul_rn(0.9, __dsub_rn(1.0, __dmul_rn(0.5, pow(0.96, __dmul_rn(__dadd_rn(t, 1.0), 4e-3)))));
+            const float mu_product = __fmul_rn(s[3], (float)mu);
+            const double mu_product_next = __dmul_rn((double)mu_product, mu_next);
+            const float denom = __fadd_rn(__fsqrt_rn(__fdiv_rn(v, (float)bc2)), 1e-8f);
+            lam = t_addcdiv(lam, g, denom,
+                            (float)__ddiv_rn(__dmul_rn(-lr, __dsub_rn(1.0, mu)), __dsub_rn(1.0, (double)mu_product)));
+            lam = t_addcdiv(lam, m, denom, (float)__ddiv_rn(__dmul_rn(-lr, mu_next), __dsub_rn(1.0, mu_product_next)));
+            s[3] = mu_product;
+        } else {   // RAdam
+            const float bce = __fdiv_rn(m, (float)bc1);
+            const double rho_inf = __dsub_rn(__ddiv_rn(2.0, __dsub_rn(1.0, 0.999)), 1.0);
+            const double rho_t = __dsub_rn(rho_inf, __ddiv_rn(__dmul_rn(__dmul_rn(2.0, t), pow(0.999, t)), bc2));
+            float upd = __fmul_rn(bce, (float)lr);
+            if (rho_t > 5.0) {
+                const double rect = sqrt(__ddiv_rn(__dmul_rn(__dmul_rn(__dsub_rn(rho_t, 4.0), __dsub_rn(rho_t, 2.0)), rho_inf),
+                                                   __dmul_rn(__dmul_rn(__dsub_rn(rho_inf, 4.0), __dsub_rn(rho_inf, 2.0)), rho_t)));
+                // (bc2 ** 0.5) / tensor is Tensor.__rtruediv__: reciprocal, then the scalar product
+                const float adaptive = __fmul_rn(__frcp_rn(__fadd_rn(__fsqrt_rn(v), 1e-8f)), (float)sqrt(bc2));
+                upd = __fmul_rn(__fmul_rn(upd, adaptive), (float)rect);
+            }
+            lam = __fmaf_rn(-1.f, upd, lam);
+        }
+        s[1] = m; s[2] = v;
+        break;
+    }
+    case OSB_LAMBDA_RMSPROP: {
+        const float sq = t_addcmul(__fmul_rn(s[1], 0.99f), g, g, (float)(1.0 - 0.99));
+        lam = t_addcdiv(lam, g, __fadd_rn(__fsqrt_rn(sq), 1e-8f), (float)-lr);
+        s[1] = sq;
+        break;
+    }
+    case OSB_LAMBDA_RPROP: {
+        const float prod = __fmul_rn(g, s[1]);
+        const float sign = prod > 0.f ? 1.2f : prod < 0.f ? 0.5f : 1.f;
+        const float step = fminf(fmaxf(__fmul_rn(s[2], sign), 1e-6f), 50.f);
+        const float gm = sign == 0.5f ? 0.f : g;
+        const float sg = gm > 0.f ? 1.f : gm < 0.f ? -1.f : 0.f;
+        lam = __fmaf_rn(-sg, step, lam);
+        s[1] = gm; s[2] = step;
+        break;
+    }
+    case OSB_LAMBDA_ADAGRAD: {
+        const float sum = t_addcmul(s[1], g, g, 1.f);
+        lam = t_addcdiv(lam, g, __fadd_rn(__fsqrt_rn(sum), 1e-10f), (float)-lr);   // lr_decay 0: clr = lr
+        s[1] = sum;
+        break;
+    }
+    case OSB_LAMBDA_ADADELTA: {
+        const float w = (float)(1.0 - 0.9);
+        const float sq = t_addcmul(__fmul_rn(s[1], 0.9f), g, g, w);
+        const float std_ = __fsqrt_rn(__fadd_rn(sq, 1e-6f));
+        const float delta = __fmul_rn(__fdiv_rn(__fsqrt_rn(__fadd_rn(s[2], 1e-6f)), std_), g);
+        s[2] = t_addcmul(__fmul_rn(s[2], 0.9f), delta, delta, w);
+        lam = __fmaf_rn((float)-lr, delta, lam);
+        s[1] = sq;
+        break;
+    }
+    case OSB_LAMBDA_ASGD: {   // lambd 1e-4, alpha 0.75, t0 1e6
+        const double eta = (double)s[1];
+        lam = __fmul_rn(lam, (float)__dsub_rn(1.0, __dmul_rn(1e-4, eta)));
+        lam = __fmaf_rn((float)-eta, g, lam);
+        s[3] = s[2] != 1.f ? __fadd_rn(s[3], __fmul_rn(__fsub_rn(lam, s[3]), s[2])) : lam;
+        s[1] = (float)__ddiv_rn(lr, pow(__dadd_rn(1.0, __dmul_rn(__dmul_rn(1e-4, lr), t)), 0.75));
+        s[2] = (float)__drcp_rn(fmax(1.0, __dsub_rn(t, 1e6)));
+        break;
+    }
+    case OSB_LAMBDA_ADAFACTOR: {   // beta2_decay -0.8, eps (finfo(fp32).eps, 1e-3), d 1, relative step
+        const double rho = fmin(lr, __drcp_rn(sqrt(t)));
+        const double alpha = __dmul_rn(fmax(1e-3, (double)fabsf(lam)), rho);
+        const float var = t_lerp(s[1], __fmul_rn(g, g), (float)pow(t, -0.8));
+        const float eps1 = 1.1920928955078125e-07f;
+        const float upd = __fmul_rn(__frcp_rn(__fsqrt_rn(fmaxf(var, __fmul_rn(eps1, eps1)))), g);
+        const double denom = fmax(1.0, (double)fabsf(upd));
+        lam = __fmaf_rn((float)-__ddiv_rn(alpha, denom), upd, lam);
+        s[1] = var;
+        break;
+    }
+    default:
+        return;
+    }
+    lam = fmaxf(lam, 0.f);
+    if (upper_bound >= 0.0) lam = fminf(lam, (float)upper_bound);
+    s[0] = lam;
+}
+
 // PID-Lagrangian controller (common/pid_lagrange.py:L95-125), Python-float (fp64) arithmetic.
 // pid_state: [0] integral term, [1] EMA of delta, [2] EMA of Jc, [3] cost penalty, [4] deque length,
 // [5] deque head (oldest entry), [8 + i] ring buffer of the delayed cost EMAs (capacity d_delay <= 56).
@@ -602,6 +744,16 @@ int osb_lagrange_update(const double* window_sums, float cost_limit, float lambd
                         float upper_bound, float* state, int* nan_flag, void* stream) {
     OSB_CHECK_ARG(window_sums && state && nan_flag, "null pointer");
     lagrange_update_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(window_sums, cost_limit, lambda_lr, upper_bound, state, nan_flag);
+    OSB_LAUNCH_CHECK();
+    return OSB_OK;
+}
+
+int osb_lagrange_update_opt(int kind, const double* window_sums, double cost_limit, double lambda_lr,
+                            double upper_bound, float* state, int* nan_flag, void* stream) {
+    OSB_CHECK_ARG(window_sums && state && nan_flag, "null pointer");
+    OSB_CHECK_ARG(kind >= OSB_LAMBDA_SGD && kind <= OSB_LAMBDA_ADAFACTOR, "unknown lambda optimiser kind");
+    lagrange_update_opt_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(kind, window_sums, cost_limit, lambda_lr,
+                                                                  upper_bound, state, nan_flag);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
 }

@@ -38,6 +38,14 @@ from omnisafe_b200.utils.train_state import restore, snapshot
 HID = 64     # the hidden width every kernel computes
 NET_ACTOR, NET_REWARD, NET_COST = 1, 2, 4   # net_mask bits of osb_policy_step
 NETS = ('actor', 'reward_critic', 'cost_critic')
+# model_cfgs.weight_initialization_mode -> the weight draw of utils/model.py:L25-44 (kaiming_uniform is drawn directly)
+INIT_MODES = {
+    'kaiming_uniform': None,
+    'xavier_normal': torch.nn.init.xavier_normal_,
+    'glorot': torch.nn.init.xavier_uniform_,
+    'xavier_uniform': torch.nn.init.xavier_uniform_,
+    'orthogonal': lambda w, generator: torch.nn.init.orthogonal_(w, gain=np.sqrt(2), generator=generator),
+}
 
 
 def param_layout(obs_dim: int, act_dim: int, hid: int = HID, *, actor_hidden=None, critic_hidden=None) -> dict:
@@ -132,7 +140,9 @@ class ConstraintActorCritic:
         assert model_cfgs.actor.activation == 'tanh' and model_cfgs.critic.activation == 'tanh', (
             'the fused kernels implement tanh activations')
         assert model_cfgs.actor_type == 'gaussian_learning'
-        assert model_cfgs.weight_initialization_mode == 'kaiming_uniform'
+        self.init_mode = model_cfgs.weight_initialization_mode
+        if self.init_mode not in INIT_MODES:
+            raise TypeError(f'Invalid initialization function: {self.init_mode}')   # utils/model.py:L44
         self.obs_dim, self.act_dim = int(obs_dim), int(act_dim)
         self.device = torch.device(device)
         self.layout = self.param_map.kernel
@@ -153,9 +163,10 @@ class ConstraintActorCritic:
         self.reward_critic = VCritic(self, NET_REWARD)
         self.cost_critic = VCritic(self, NET_COST)
 
-    # -- initialisation (utils/model.py:L25-44: kaiming_uniform_(a=sqrt(5)); torch default bias) --------------------
+    # -- initialisation (utils/model.py:L25-44: initialize_layer on each weight; torch default bias) ----------------------
     def _init_parameters(self, generator) -> None:
-        """Each layer's real block drawn with its real fan-in, weight then bias, layer by layer; the pads stay 0."""
+        """Each layer's real block drawn with its real fans, weight then bias, layer by layer; the pads stay 0.
+        kaiming_uniform_(a=sqrt(5)) is U(+-1/sqrt(fan_in)); the other modes are torch.nn.init's on the real block."""
         theta = torch.zeros(self.layout['total'], dtype=torch.float32)
         for net in self.NETS:
             views = self.param_map.views(theta, net)
@@ -163,8 +174,11 @@ class ConstraintActorCritic:
             for wname, bname in zip(names[-6::2], names[-5::2]):
                 w, b = views[wname], views[bname]
                 fan_in = w.shape[1]
-                bw = math.sqrt(6.0 / ((1.0 + 5.0) * fan_in))
-                w.copy_(torch.empty(w.shape).uniform_(-bw, bw, generator=generator))
+                if self.init_mode == 'kaiming_uniform':
+                    bw = math.sqrt(6.0 / ((1.0 + 5.0) * fan_in))
+                    w.copy_(torch.empty(w.shape).uniform_(-bw, bw, generator=generator))
+                else:
+                    w.copy_(INIT_MODES[self.init_mode](torch.empty(w.shape), generator=generator))
                 bb = 1.0 / math.sqrt(fan_in)
                 b.copy_(torch.empty(b.shape).uniform_(-bb, bb, generator=generator))
         self.theta.copy_(theta)
