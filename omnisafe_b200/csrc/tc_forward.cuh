@@ -1,5 +1,5 @@
 // The tensor-core MLP forward (obs -> 64 -> 64 -> out <= 16, tanh hidden layers) on tiles of 128 rows, shared by
-// rollout_step_tc_kernel (csrc/rollout.cu), policy_tc_kernel (csrc/policy.cu) and actor_eval_tc_kernel
+// rollout_step_tc_kernel (csrc/rollout.cu), policy_tc_kernel (csrc/policy.cu) and the actor evaluations
 // (csrc/eval_tc.cu), so that the rollout, the policy step and the evaluation compute one function bit for bit; its
 // tiles and staging also carry the Fisher-vector tangent pass (fvp_tangent_kernel, csrc/fvp_tc.cu).
 //   X3 = false: tf32 wgmma tiles (csrc/umma.cuh), layer 1 as a K loop over 64-column chunks for inputs up to 512 wide;
@@ -293,6 +293,50 @@ __device__ __forceinline__ void tc_forward(uint32_t base, const umma::Acc& tm, u
         mbar_wait(bar, phase); phase ^= 1;
         after(3);
     }
+}
+
+// The bf16x3 forward of rows 64 h .. 64 h + 63 of a tile, h = the calling warpgroup, issued, waited on and finished by
+// that warpgroup alone: the warpgroups of a CTA run their 64-row blocks without meeting, and one's epilogues run
+// under the others' MMAs.  The m64 blocks are those of tc_forward (a row depends only on that row and the k-step
+// order; the same products in the same order), so every row has the bits of the 128-row forward.  Every layer's A
+// operand is in registers: the m64k16 fragments of the bf16x3 pieces, a[piece][ks] for columns 16 ks .. 16 ks + 15
+// (x3_block_ra).  The caller splits X into a; the hidden epilogues split tanh(Z + b) into it, the accumulator fragment
+// of one layer being the A fragment of the next, so the MMAs read only the weights from shared memory.
+// The weights are at the TcTiles<true> offsets from base.  Returns the OUT product without its bias as the m64n16
+// fragment: element (rr, j, e) of thread (warp w, lane l) of the warpgroup is row 16 w + l / 4 + 8 rr of its 64 rows,
+// column 8 j + 2 (l % 4) + e.
+__device__ __forceinline__ void tc_forward_x3_half(uint32_t base, uint32_t (&a)[3][4][4], const float* sB1,
+                                                   const float* sB2, float (&out)[8]) {
+    using namespace umma;
+    using T = TcTiles<true>;
+    const uint64_t dW1 = x3::desc128(base + T::W1), dW2 = x3::desc128(base + T::W2), dW3 = x3::desc128(base + T::W3);
+    const int l = threadIdx.x & 31;
+    auto hidden = [&](const float (&d)[32], const float* sB) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+                const int c = 8 * j + 2 * (l & 3), q = 2 * (j & 1) + rr;
+                x3::split2(x3::tanh_acc(d[4 * j + 2 * rr] + sB[c]), x3::tanh_acc(d[4 * j + 2 * rr + 1] + sB[c + 1]),
+                           a[0][j >> 1][q], a[1][j >> 1][q], a[2][j >> 1][q]);
+            }
+    };
+    float d[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) d[i] = 0.f;
+    x3::x3_block_ra<0, 8, 4>(d, a, x3::desc_fresh(dW1), T::WSUB, 32u);
+    wg_wait<0>();
+    acc_fence(d);
+    hidden(d, sB1);
+    x3::x3_block_ra<0, 8, 4>(d, a, x3::desc_fresh(dW2), T::WSUB, 32u);
+    wg_wait<0>();
+    acc_fence(d);
+    hidden(d, sB2);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) out[i] = 0.f;
+    x3::x3_block_ra<0, 2, 4>(out, a, x3::desc_fresh(dW3), T::W3SUB, 32u);
+    wg_wait<0>();
+    acc_fence(out);
 }
 
 }  // namespace osb

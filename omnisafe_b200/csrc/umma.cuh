@@ -127,6 +127,29 @@ __device__ __forceinline__ void wgmma_bf16_n16(float (&d)[8], uint64_t a, uint64
         : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB) : "memory");
 }
 
+// The same with A from registers: the m64k16 fragment of the thread, a[0] / a[1] = rows l / 4 and l / 4 + 8 of the
+// warp's 16 rows at k = 2 (l % 4) + {0, 1}, a[2] / a[3] the same at k + 8 (bf16x2 words, lower k in the low half).
+template <int TB>
+__device__ __forceinline__ void wgmma_bf16_n64_ra(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %38, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1, %37;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "n"(TB), "r"(scale_d) : "memory");
+}
+template <int TB>
+__device__ __forceinline__ void wgmma_bf16_n16_ra(float (&d)[8], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %14, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+        "{%8, %9, %10, %11}, %12, p, 1, 1, %13;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "n"(TB), "r"(scale_d) : "memory");
+}
+
 // Warpgroup of the calling thread, taken from lane 0 so that ptxas can prove a branch on it uniform over the warp.
 // A wgmma-issuing branch must test this value: on a test of threadIdx.x itself ptxas assumes a divergent path and
 // waits on every wgmma before issuing the next (C7520).

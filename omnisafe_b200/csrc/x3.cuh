@@ -77,6 +77,31 @@ __device__ __forceinline__ void x3_block(float (&d)[4 * NJ], uint64_t a0, uint32
     wg_commit();
 }
 
+// x3_block<0, TB, NJ, NK, false> with A from registers: a[p][ks] is the m64k16 fragment (wgmma_bf16_n64_ra) of piece p
+// (0 hi, 1 mid, 2 lo) at k-step ks.  The same products in the same order as with A read from a shared-memory tile.
+template <int TB, int NJ, int NK>
+__device__ __forceinline__ void x3_block_ra(float (&d)[4 * NJ], const uint32_t (&a)[3][NK][4], uint64_t b0, uint32_t bsplit,
+                                            uint32_t bkstep) {
+    auto mma = [&](const uint32_t (&ap)[4], uint64_t b, uint32_t s) {
+        if constexpr (NJ == 8) wgmma_bf16_n64_ra<TB>(d, ap, b, s);
+        else wgmma_bf16_n16_ra<TB>(d, ap, b, s);
+    };
+    wg_fence();
+    acc_fence(d);
+#pragma unroll
+    for (int ks = 0; ks < NK; ++ks) {
+        const uint64_t b = desc_add(b0, (uint32_t)ks * bkstep), b1 = desc_add(b, bsplit), b2 = desc_add(b, 2 * bsplit);
+        const uint32_t s = ks > 0 ? 1u : 0u;
+        mma(a[2][ks], b, s);
+        mma(a[0][ks], b2, 1u);
+        mma(a[1][ks], b1, 1u);
+        mma(a[1][ks], b, 1u);
+        mma(a[0][ks], b1, 1u);
+        mma(a[0][ks], b, 1u);
+    }
+    wg_commit();
+}
+
 // D[acc] (+)= A * B over NK k-steps of 16, with the six split products (small terms first); called by all 128 threads
 // of one warpgroup.
 //   M = 64 or 128, N = 16 or 64; TA / TB: A / B read MN-major (an MN-major A has M = 64); B_EXACT: B is exactly
