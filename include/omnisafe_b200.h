@@ -28,6 +28,18 @@ extern "C" {
 /* ---- plumbing ---------------------------------------------------------------------------- */
 const char* osb_last_error(void);
 int osb_abi_version(void);
+
+/* Hidden-layer activations (model_cfgs.actor / critic.activation) and real hidden widths (1..64, the networks being
+ * zero-padded 64-wide tiles) of the networks the following launches compute, process-wide until changed.  Default:
+ * tanh, [64, 64].  Every launch of a network's kernels reads the spec when it is enqueued, so a model sets its own
+ * before its launches; a captured graph keeps the spec it was captured with.  Sigmoid and softplus units past a layer's
+ * width output +0, so the pads of a narrower network stay exact. */
+#define OSB_ACT_TANH 0
+#define OSB_ACT_IDENTITY 1
+#define OSB_ACT_RELU 2
+#define OSB_ACT_SIGMOID 3
+#define OSB_ACT_SOFTPLUS 4
+int osb_set_net_spec(int actor_act, int critic_act, int a1, int a2, int c1, int c2);
 /* kernels launched by this library in this process so far (bench.py counts its timed region with it) */
 long long osb_launch_count(void);
 int osb_device_info(int device, int* sm_count, int* cc_major, int* cc_minor);

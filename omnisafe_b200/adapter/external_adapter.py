@@ -239,8 +239,9 @@ class ExternalEnvAdapter:
                 ptr(d['reward']), ptr(d['cost']), ptr(d['flags']), ptr(d['epfin']), ptr(self._ws), ptr(self.nonfinite))
 
     def _graph_key(self, T: int, agent, d, eps, reset_obs) -> tuple:
-        """The device pointers (and shape) a captured epoch bakes in; a change of any of them forces a recapture."""
-        key = (T, ptr(agent.theta), tuple(ptr(v) for v in d.values() if v is not None), ptr(eps),
+        """The device pointers, the shape and the network spec (activations, widths) a captured epoch bakes in; a change
+        of any of them forces a recapture."""
+        key = (T, agent.net_spec, ptr(agent.theta), tuple(ptr(v) for v in d.values() if v is not None), ptr(eps),
                tuple(self._norm_ptrs()), torch.as_tensor(reset_obs).untyped_storage().data_ptr())
         return key if self._time_limit is None else (*key, self._rst_ptr)
 
@@ -274,6 +275,7 @@ class ExternalEnvAdapter:
             logger.log(f'{type(self._env).__name__}: external-env rollout in {self.graph_mode} mode')
             self._mode_logged = True
         L, d, s = lib(), buffer.data, current_stream()
+        agent.apply_net_spec()
         obs, _ = self._env.reset()
         if self._time_limit is not None:
             self._tl_steps.zero_()                  # TimeLimit.reset

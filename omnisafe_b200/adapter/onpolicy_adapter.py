@@ -81,6 +81,7 @@ class OnPolicyAdapter:
                 + [ptr(agent.theta), ptr(eps), self.noise_seed, self._epoch_index & 0xFFFFFFFF,
                    self.window_lens, ptr(self.ep_ring), ptr(self.ep_meta), ptr(self.window_sums),
                    int(self.precision), current_stream()])
+        agent.apply_net_spec()
         lib().osb_rollout_epoch(*args)
         # the policy never sees rewards inside a rollout: the per-step reward / cost normalisation of the
         # reference commutes with the rollout and runs on the finished slab (episode statistics stay raw,

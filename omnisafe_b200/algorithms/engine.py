@@ -82,6 +82,7 @@ class UpdateEngine:
                   max_grad_norm=0.0, lr_actor=0.0, lr_critic=0.0, target_kl=0.0, kl_early_stop=False,
                   perm=None, precision: int | None = None) -> None:
         a = self.agent
+        a.apply_net_spec()
         if perm is not None:
             assert perm.dtype == torch.int32 and perm.shape == (update_iters, self.total)
         lib().osb_ppo_update_epoch(
@@ -148,6 +149,7 @@ class UpdateEngine:
         the kernels clip, rank-average and Adam-step; a critic's callable trains its network itself.  When the actor
         trains, the old policy is snapshotted first and the full-batch KL check runs after each pass, as in ppo_epoch."""
         a, s = self.agent, current_stream()
+        a.apply_net_spec()
         if perm is not None:
             assert perm.dtype == torch.int32 and perm.shape == (update_iters, self.total)
         self.stop_flag.zero_()
@@ -223,6 +225,7 @@ class UpdateEngine:
     def snapshot_old_policy(self) -> None:
         """p_dist = actor(obs) at the current parameters (trpo.py:L177, cpo.py:L366)."""
         a = self.agent
+        a.apply_net_spec()
         self._eval_fn()(ptr(a.theta), self.O, self.A, ptr(self.buf.data['obs']), 0, 0, 0, 0, 0, 0,
                         0, 0, self.total, 1, ptr(self.mu_old), 0, 0, current_stream())
         self.logstd_old.copy_(a.theta[:self.A])
@@ -231,6 +234,7 @@ class UpdateEngine:
         """loss.backward() of the full-batch surrogate + avg_grads (natural_pg.py:L150-157):
         out_grad <- sign * d loss / d theta_actor; returns the device scalar `loss` (rank-averaged)."""
         a = self.agent
+        a.apply_net_spec()
         if (self._tc() or self._x3()) and loss_kind in (LOSS_RATIO, LOSS_COST):
             nb = lib().osb_tc_grid_blocks(self.total, NET_ACTOR)
             (lib().osb_minibatch_grad_x3 if self._x3() else lib().osb_minibatch_grad_tc)(
@@ -258,6 +262,7 @@ class UpdateEngine:
     def fvp(self, vec: torch.Tensor, out: torch.Tensor, damping: float, stride: int = 1) -> None:
         """NaturalPG._fvp (natural_pg.py:L74-119): out <- avg_ranks(F vec) + damping * vec."""
         a = self.agent
+        a.apply_net_spec()
         if self._x3():
             nb = lib().osb_tc_grid_blocks((self.total + stride - 1) // stride, NET_ACTOR)
             lib().osb_fvp_partials_x3(ptr(a.theta), ptr(vec), self.O, self.A, ptr(self.buf.data['obs']),
@@ -303,6 +308,7 @@ class UpdateEngine:
         Returns python floats averaged over ranks: loss (= -mean ratio*adv), loss_r (= -mean
         ratio*adv_r), loss_c (= mean ratio*adv_c), kl (= mean over samples AND action dims)."""
         d = self.buf.data
+        self.agent.apply_net_spec()
         self._eval_fn()(ptr(theta_actor), self.O, self.A, ptr(d['obs']), ptr(d['act']), ptr(d['logp']),
                         ptr(d['adv_r']), ptr(d['adv_c']), ptr(self.mu_old), ptr(self.logstd_old),
                         ptr(self.buf.adv_moments), ptr(lagrange), self.total, 1, 0, ptr(self.eval_ws),

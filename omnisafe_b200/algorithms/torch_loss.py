@@ -49,6 +49,7 @@ class ActorMean(torch.autograd.Function):
         B, A = obs.shape[0], engine.A
         mu = torch.empty(B, A, dtype=torch.float32, device=obs.device)
         if B > 0:
+            engine.agent.apply_net_spec()
             engine._eval_fn()(ptr(theta_actor), engine.O, A, ptr(obs), 0, 0, 0, 0, 0, 0, 0, 0, B, 1, ptr(mu), 0, 0,
                               current_stream())
         ctx.save_for_backward(obs, theta_actor)
@@ -65,6 +66,7 @@ class ActorMean(torch.autograd.Function):
             dmu = dmu.to(torch.float32).contiguous()
             nb = lib().osb_actor_dmu_grid_blocks(B, e.O, e.precision)
             s = current_stream()
+            e.agent.apply_net_spec()
             lib().osb_actor_dmu_backward(ptr(theta_actor), e.O, e.A, ptr(obs), ptr(dmu), B, e.precision,
                                          ptr(e.fvp_part), ptr(e.stats_part), s)
             lib().osb_reduce_partials(ptr(e.fvp_part), nb, e.Pa, e.Pa, 1.0, 0, 0.0, ptr(grad), s)
@@ -163,6 +165,7 @@ class TrainingCritic:
         """osb_critic_dv_backward on rows obs [B, O] into the engine's partials; returns their row count."""
         e = self._engine
         B = obs.shape[0]
+        e.agent.apply_net_spec()
         lib().osb_critic_dv_backward(ptr(e.agent.theta), e.O, e.A, self.net, ptr(obs), ptr(dv), ptr(value), B,
                                      e.precision, ptr(e.gpart), ptr(e.stats_part), current_stream())
         return lib().osb_critic_dv_grid_blocks(B, e.O, e.precision)

@@ -1,4 +1,5 @@
 // C-ABI plumbing shared by all entry points: error string, version, device query.
+#include "activation.cuh"
 #include "common.cuh"
 #include <mutex>
 #include <string.h>
@@ -31,9 +32,24 @@ int osb_device_info(int device, int* sm_count, int* cc_major, int* cc_minor) {
     return OSB_OK;
 }
 
+static osb::NetSpec g_net_spec = {{osb::ACT_TANH, osb::ACT_TANH}, {{64, 64}, {64, 64}}};
+
+// Hidden activations and real hidden widths of the networks the following launches compute (process-wide until
+// changed): actor_act / critic_act are OSB_ACT_* codes, a1, a2 the actor's widths and c1, c2 the critics'.
+int osb_set_net_spec(int actor_act, int critic_act, int a1, int a2, int c1, int c2) {
+    OSB_CHECK_ARG(actor_act >= osb::ACT_TANH && actor_act <= osb::ACT_SOFTPLUS && critic_act >= osb::ACT_TANH &&
+                      critic_act <= osb::ACT_SOFTPLUS, "activation code out of range");
+    OSB_CHECK_ARG(a1 >= 1 && a1 <= 64 && a2 >= 1 && a2 <= 64 && c1 >= 1 && c1 <= 64 && c2 >= 1 && c2 <= 64,
+                  "hidden widths must be 1..64");
+    g_net_spec = osb::NetSpec{{actor_act, critic_act}, {{a1, a2}, {c1, c2}}};
+    return OSB_OK;
+}
+
 }  // extern "C"
 
 namespace osb {
+
+const NetSpec& net_spec() { return g_net_spec; }
 
 // Device scratch for the tensor-core accumulator images (csrc/umma.cuh): one buffer per (device, slot), grown on
 // demand.  A buffer that has been handed out is never freed (growth allocates a new one and keeps the old one for the

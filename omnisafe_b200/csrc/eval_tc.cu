@@ -25,7 +25,8 @@ struct EvalTcArgs {
     double* out;        // bf16x3: the folded sums
 };
 
-__global__ void __launch_bounds__(NTHREADS, 2) actor_eval_tc_kernel(EvalTcArgs p) {
+template <int ACT>
+__global__ void __launch_bounds__(NTHREADS, 2) actor_eval_tc_kernel(EvalTcArgs p, NetSpec spec) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
     const uint32_t B0 = smem_u32(smem_raw) + pad;
@@ -82,7 +83,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) actor_eval_tc_kernel(EvalTcArgs p
             }
         };
         tc_forward<false>(
-            B0, tm, &bar, phase, sB1, sB2, nchunks,
+            B0, tm, &bar, phase, sB1, sB2, nchunks, Hidden<ACT, umma::TanhFast>(spec, 0),
             [&](int c) { tc_stage_rows<false>(B0, p.obs, O, vec, c, theta, L, [&](int m) { return sRow[m]; }); },
             [&](int l) {
                 if (l == 2) load_sample();
@@ -141,7 +142,8 @@ __host__ __device__ __forceinline__ uint32_t x3_slot_bytes(int O, int A, bool kl
 // one fp64 partial row per CTA, folded by the last CTA to finish (self-resetting; zero when the module loads)
 __device__ unsigned int g_eval_x3_ticket;
 
-__global__ void __launch_bounds__(XW_THREADS, 1) actor_eval_x3_kernel(EvalTcArgs p) {
+template <int ACT>
+__global__ void __launch_bounds__(XW_THREADS, 1) actor_eval_x3_kernel(EvalTcArgs p, NetSpec spec) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
     const uint32_t B0 = smem_u32(smem_raw) + pad;
@@ -279,7 +281,7 @@ __global__ void __launch_bounds__(XW_THREADS, 1) actor_eval_x3_kernel(EvalTcArgs
         wg_sync();                                   // every thread has read its obs
         if (t == 0 && bulk_next) issue(u + G, 0);    // the obs run is free: the next tile's flies under this forward
         float o[8];
-        tc_forward_x3_half(W, xa, sB1, sB2, o);
+        tc_forward_x3_half(W, xa, sB1, sB2, Hidden<ACT, x3::TanhAcc>(spec, 0), o);
         {
             const int w = t >> 5;
 #pragma unroll
@@ -341,11 +343,6 @@ static int actor_eval_tc(const float* theta_actor, int O, int A, const float* ob
                          double* workspace, double* out, void* stream) {
     EvalTcArgs p{obs, act, logp, adv_r, adv_c, mu_old, logstd_old, moments, lagrange, theta_actor, mu_store, workspace, nullptr, total, stride, O, A, out};
     const size_t smem = 1024 + TcTiles<false>::FLOATS + EW_WORDS * sizeof(float);
-    static bool attr = false;
-    if (!attr) {
-        OSB_CUDA(cudaFuncSetAttribute(actor_eval_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = true;
-    }
     const long long nrows = (total + stride - 1) / stride;
     const long long tiles = (nrows + TC_ROWS - 1) / TC_ROWS;
     const int cap = 2 * grid_sms();
@@ -353,8 +350,18 @@ static int actor_eval_tc(const float* theta_actor, int O, int A, const float* ob
     p.acc = acc_scratch(ACC_EVAL_TC, (size_t)blocks * 128 * TC_COLS * sizeof(float));
     if (!p.acc) return OSB_ERR_CUDA;
     cudaStream_t s = (cudaStream_t)stream;
-    actor_eval_tc_kernel<<<blocks, NTHREADS, smem, s>>>(p);
-    OSB_LAUNCH_CHECK();
+    const NetSpec spec = net_spec();
+    const int rc = with_act<false>(spec.act[0], [&](auto a) {
+        static bool attr = false;
+        if (!attr) {
+            OSB_CUDA(cudaFuncSetAttribute(actor_eval_tc_kernel<a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            attr = true;
+        }
+        actor_eval_tc_kernel<a.value><<<blocks, NTHREADS, smem, s>>>(p, spec);
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    });
+    if (rc) return rc;
     return mu_store ? OSB_OK : eval_reduce(workspace, blocks, out, s);
 }
 
@@ -363,19 +370,22 @@ static int actor_eval_x3(const float* theta_actor, int O, int A, const float* ob
                          const float* moments, const float* lagrange, long long total, int stride, float* mu_store,
                          double* workspace, double* out, void* stream) {
     EvalTcArgs p{obs, act, logp, adv_r, adv_c, mu_old, logstd_old, moments, lagrange, theta_actor, mu_store, workspace, nullptr, total, stride, O, A, out};
-    static bool attr = false;
-    if (!attr) {
-        const size_t most = 1024 + XW_RING + XW_WG * x3_slot_bytes(64, 16, true);
-        OSB_CUDA(cudaFuncSetAttribute(actor_eval_x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)most));
-        attr = true;
-    }
     const size_t smem = 1024 + XW_RING + XW_WG * x3_slot_bytes(O, A, mu_store == nullptr);
     const long long nrows = (total + stride - 1) / stride;
     const long long groups = (nrows + 64 * XW_WG - 1) / (64 * XW_WG);     // 64-row tiles, XW_WG per CTA at a time
     const int blocks = (int)(groups < grid_sms() ? groups : grid_sms());
-    actor_eval_x3_kernel<<<blocks, XW_THREADS, smem, (cudaStream_t)stream>>>(p);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    const NetSpec spec = net_spec();
+    return with_act<false>(spec.act[0], [&](auto a) {
+        static bool attr = false;
+        if (!attr) {
+            const size_t most = 1024 + XW_RING + XW_WG * x3_slot_bytes(64, 16, true);
+            OSB_CUDA(cudaFuncSetAttribute(actor_eval_x3_kernel<a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)most));
+            attr = true;
+        }
+        actor_eval_x3_kernel<a.value><<<blocks, XW_THREADS, smem, (cudaStream_t)stream>>>(p, spec);
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    });
 }
 
 }  // namespace osb

@@ -4,10 +4,11 @@
 //   NaturalPG._fvp (algorithms/on_policy/base/natural_pg.py:L74-119):  F v = grad( (grad KL)^T v ), which for the
 //   Gaussian actor at theta = theta_old is  [ (2 / A) v_logsigma ;  (1 / (B A)) sum_s J(s)^T diag(sigma^-2) J(s) v_mu ]
 //   (SURVEY §8a row 13).  This kernel computes d mu(s) = J(s) v_mu by forward-mode differentiation of the MLP:
-//       T1 = X V1^T + bv1,              dH1 = (1 - H1^2) T1
-//       T2 = dH1 W2^T + H1 V2^T + bv2,  dH2 = (1 - H2^2) T2
+//       T1 = X V1^T + bv1,              dH1 = f'(H1) T1
+//       T2 = dH1 W2^T + H1 V2^T + bv2,  dH2 = f'(H2) T2
 //       dmu = dH2 W3^T + H2 V3^T + bv3
-//   next to the ordinary forward (Z1 = X W1^T + b1, H1 = tanh Z1, ...), on the tiles of csrc/tc_forward.cuh:
+//   next to the ordinary forward (Z1 = X W1^T + b1, H1 = f(Z1), ...; f the hidden activation of csrc/activation.cuh),
+//   on the tiles of csrc/tc_forward.cuh:
 //     X3 = false: tf32 wgmma (O <= 512; CHUNKED: layer 1 as a K loop over 64-column chunks of X, W1 and V1), tanh_fast;
 //     X3 = true : split-bf16, six bf16 wgmma products per product (O <= 64), tanh_acc.
 //   The backward half J^T diag(sigma^-2) dmu / (B A) is the precision's update kernel with loss kind LOSS_FVP
@@ -75,8 +76,8 @@ __device__ __forceinline__ void fvp_store8(uint32_t tile, int r, int c0, const f
     }
 }
 
-template <bool X3, bool CHUNKED>
-__global__ void __launch_bounds__(FVP_NT<X3>, 1) fvp_tangent_kernel(FvpTanArgs p) {
+template <bool X3, bool CHUNKED, int ACT>
+__global__ void __launch_bounds__(FVP_NT<X3>, 1) fvp_tangent_kernel(FvpTanArgs p, NetSpec spec) {
     using T = TcTiles<X3>;
     using F = FvpTiles<X3>;
     constexpr int EC = 64 * 128 / FVP_NT<X3>;      // epilogue columns per thread
@@ -162,8 +163,9 @@ __global__ void __launch_bounds__(FVP_NT<X3>, 1) fvp_tangent_kernel(FvpTanArgs p
             for (int j = 0; j < 16; ++j) sts(tile_addr(sX, (tid >> 6) + 8 * j, tid & 63, TC_ROWS), tf32r(xpre[j >> 3][j & 7]));
         }
     };
-    // H = tanh(Z + b) into `dst`, dH = (1 - H^2) (T + bv) into the tangent buffer; the layer's MMAs have completed
-    auto epilogue = [&](const float* sBz, const float* sBt, uint32_t dst) {
+    // H = f(Z + b) into `dst`, dH = f'(H) (T + bv) into the tangent buffer; the layer's MMAs have completed
+    const Hidden<ACT, TcTanh<X3>> af(spec, 0);
+    auto epilogue = [&](const float* sBz, const float* sBt, int width, uint32_t dst) {
 #pragma unroll
         for (int c8 = 0; c8 < EC / 8; ++c8) {
             const int c0 = EC * h + 8 * c8;
@@ -172,9 +174,9 @@ __global__ void __launch_bounds__(FVP_NT<X3>, 1) fvp_tangent_kernel(FvpTanArgs p
             acc_ld<8>(tm, lane_base + FVP_C_T + (uint32_t)c0, t);
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
-                const float hh = X3 ? x3::tanh_acc(z[i] + sBz[c0 + i]) : tanh_fast(z[i] + sBz[c0 + i]);
+                const float hh = af(z[i] + sBz[c0 + i], c0 + i, width);
                 z[i] = hh;
-                t[i] = (1.f - hh * hh) * (t[i] + sBt[c0 + i]);
+                t[i] = af.d(hh) * (t[i] + sBt[c0 + i]);
             }
             fvp_store8<X3>(dst, s_row, c0, z);
             fvp_store8<X3>(sD, s_row, c0, t);
@@ -210,7 +212,7 @@ __global__ void __launch_bounds__(FVP_NT<X3>, 1) fvp_tangent_kernel(FvpTanArgs p
             if constexpr (!CHUNKED) gather_next();
             mbar_wait(&bar, phase); phase ^= 1;
         }
-        epilogue(sB, sBv, sH1);                                 // H1, dH1
+        epilogue(sB, sBv, af.w1, sH1);                                // H1, dH1
         // ---- layer 2: Z2 = H1 W2^T, T2 = dH1 W2^T + H1 V2^T ---------------------------------------------------------
         if (mma_wg) {
             fvp_gemm<X3, 64>(tm, FVP_C_Z, sH1, sW2, false);
@@ -220,7 +222,7 @@ __global__ void __launch_bounds__(FVP_NT<X3>, 1) fvp_tangent_kernel(FvpTanArgs p
         }
         if constexpr (X3) gather(tile + gridDim.x, 0);
         mbar_wait(&bar, phase); phase ^= 1;
-        epilogue(sB + 64, sBv + 64, sX);                        // H2 over X, dH2 over dH1
+        epilogue(sB + 64, sBv + 64, af.w2, sX);                       // H2 over X, dH2 over dH1
         // ---- layer 3: dmu = dH2 W3^T + H2 V3^T + bv3 ----------------------------------------------------------------
         if (mma_wg) {
             fvp_gemm<X3, 16>(tm, FVP_C_OUT, sD, sW3, false);
@@ -255,18 +257,23 @@ static int fvp_partials(const float* theta_actor, const float* vec, int O, int A
     t.acc = acc_scratch(ACC_FVP, (size_t)nb * 128 * FVP_COLS * sizeof(float));
     if (!t.acc) return OSB_ERR_CUDA;
     const size_t smem = 1024 + FvpTiles<X3>::FLOATS + FVP_WORDS * sizeof(float);
-    static bool attr = false;
-    if (!attr) {
-        OSB_CUDA(cudaFuncSetAttribute(fvp_tangent_kernel<X3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const NetSpec spec = net_spec();
+    const int rc = with_act<false>(spec.act[0], [&](auto a) {
+        static bool attr = false;
+        if (!attr) {
+            OSB_CUDA(cudaFuncSetAttribute(fvp_tangent_kernel<X3, false, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            if constexpr (!X3)
+                OSB_CUDA(cudaFuncSetAttribute(fvp_tangent_kernel<false, true, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            attr = true;
+        }
+        void (*kernel)(FvpTanArgs, NetSpec) = fvp_tangent_kernel<X3, false, a.value>;
         if constexpr (!X3)
-            OSB_CUDA(cudaFuncSetAttribute(fvp_tangent_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = true;
-    }
-    void (*kernel)(FvpTanArgs) = fvp_tangent_kernel<X3, false>;
-    if constexpr (!X3)
-        if (O > 64) kernel = fvp_tangent_kernel<false, true>;
-    kernel<<<nb, FVP_NT<X3>, smem, stream>>>(t);
-    OSB_LAUNCH_CHECK();
+            if (O > 64) kernel = fvp_tangent_kernel<false, true, a.value>;
+        kernel<<<nb, FVP_NT<X3>, smem, stream>>>(t, spec);
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    });
+    if (rc) return rc;
     return X3 ? fvp_backward_x3(theta_actor, vec, O, A, obs, total, stride, dmu, gpart, stats_scratch, stream)
               : fvp_backward_tc(theta_actor, vec, O, A, obs, total, stride, dmu, gpart, stats_scratch, stream);
 }

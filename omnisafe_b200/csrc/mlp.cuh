@@ -1,6 +1,6 @@
 // Tile-level MLP building blocks (fp32 FMA path, exact-fp32 "parity" arithmetic).
 //
-// The actor / reward-critic / cost-critic are three independent Linear-Tanh-Linear-Tanh-Linear
+// The actor / reward-critic / cost-critic are three independent Linear-Act-Linear-Act-Linear
 // trunks (omnisafe/utils/model.py:L73-111, models/actor/gaussian_learning_actor.py:L29-62,
 // models/critic/v_critic.py:L27-73).  A CTA of 256 threads owns a tile of MT samples; activations
 // and one network's weights live in shared memory and every layer is a register-tiled GEMM.
@@ -10,6 +10,7 @@
 //   actor : log_std[A], W1[H][O], b1[H], W2[H][H], b2[H], W3[A][H], b3[A]
 //   critic:             W1[H][O], b1[H], W2[H][H], b2[H], W3[1][H], b3[1]
 #pragma once
+#include "activation.cuh"
 #include "common.cuh"
 
 namespace osb {
@@ -184,11 +185,11 @@ __device__ __forceinline__ void gemm_tn(const float* __restrict__ P, const float
     }
 }
 
-// Hidden layers of one network on a tile: X[MT][LD] (chunk 0 resident) -> H1, H2.
+// Hidden layers of one network on a tile: X[MT][LD] (chunk 0 resident) -> H1 = f(Z1), H2 = f(Z2), f = act.
 // For O > KC the caller supplies a functor that (re)loads X chunk kc and W1 chunk kc.
-template <int MT, typename LoadChunk>
+template <int MT, class Act, typename LoadChunk>
 __device__ __forceinline__ void mlp_hidden(const float* __restrict__ sX, float* __restrict__ sH1,
-                                           float* __restrict__ sH2, NetSmem& W, int nchunks,
+                                           float* __restrict__ sH2, NetSmem& W, int nchunks, const Act& act,
                                            LoadChunk load_chunk) {
     constexpr int MI = MT / 16;
     const int tm = threadIdx.x >> 4, tn = threadIdx.x & 15;
@@ -210,7 +211,7 @@ __device__ __forceinline__ void mlp_hidden(const float* __restrict__ sX, float* 
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int n = tn + 16 * j;
-            sH1[(tm + 16 * i) * LD + n] = tanhf(z[i][j] + W.b1[n]);
+            sH1[(tm + 16 * i) * LD + n] = act(z[i][j] + W.b1[n], n, act.w1);
         }
     __syncthreads();
     gemm_nt<MT, LD, LD>(sH1, W.w2, HID, acc);
@@ -219,7 +220,7 @@ __device__ __forceinline__ void mlp_hidden(const float* __restrict__ sX, float* 
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int n = tn + 16 * j;
-            sH2[(tm + 16 * i) * LD + n] = tanhf(acc[i][j] + W.b2[n]);
+            sH2[(tm + 16 * i) * LD + n] = act(acc[i][j] + W.b2[n], n, act.w2);
         }
     __syncthreads();
 }

@@ -94,7 +94,8 @@ __device__ __forceinline__ void policy_head(const PolicyArgs& p, const float* sM
 
 // ---------------------------------------------------------------------------------------------
 // fp32 FMA tiles: one CTA per (32 rows, network), the GEMMs of rollout_step_kernel.
-__global__ void __launch_bounds__(NTHREADS) policy_fma_kernel(PolicyArgs p) {
+template <int ACT>
+__global__ void __launch_bounds__(NTHREADS) policy_fma_kernel(PolicyArgs p, NetSpec spec) {
     extern __shared__ __align__(16) float smem[];
     NetSmem W;
     float* base = carve_net_smem<false>(smem, W);
@@ -122,7 +123,7 @@ __global__ void __launch_bounds__(NTHREADS) policy_fma_kernel(PolicyArgs p) {
     load_chunk(0);
     if (net == 0) stage_sigma(p, sSd);
     __syncthreads();
-    mlp_hidden<PT>(sX, sH1, sH2, W, nchunks, load_chunk);
+    mlp_hidden<PT>(sX, sH1, sH2, W, nchunks, Hidden<ACT>(spec, net), load_chunk);
     mlp_out<PT>(sH2, sO, W, L.out);
     if (net == 0) {
         policy_head(p, sO, LDO, sSd, r0, PT);
@@ -134,8 +135,8 @@ __global__ void __launch_bounds__(NTHREADS) policy_fma_kernel(PolicyArgs p) {
 // ---------------------------------------------------------------------------------------------
 // Tensor-core tiles: grid (CTAs per network, networks), each CTA loops over tiles of 128 rows through the forward of
 // rollout_step_tc_kernel (csrc/tc_forward.cuh; X3 = true: bf16x3, X3 = false: tf32).
-template <bool X3>
-__global__ void __launch_bounds__(NTHREADS, 2) policy_tc_kernel(PolicyArgs p) {
+template <bool X3, int ACT>
+__global__ void __launch_bounds__(NTHREADS, 2) policy_tc_kernel(PolicyArgs p, NetSpec spec) {
     using namespace umma;
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
@@ -171,6 +172,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) policy_tc_kernel(PolicyArgs p) {
         const long long r0 = tile * TC_ROWS;
         auto row_of = [&](int m) -> long long { return r0 + m < p.B ? r0 + m : -1; };
         tc_forward<X3>(B0, tm, &bar, phase, sB1, sB2, nchunks,
+                       Hidden<ACT, TcTanh<X3>>(spec, net),
                        [&](int c) { tc_stage_rows<X3>(B0, p.obs, O, p.vec, c, theta, L, row_of); });
         if (h == 0) {
             float o16[16];
@@ -209,11 +211,18 @@ static bool g_policy_attr = false;
 
 static int policy_prepare() {
     if (!g_policy_attr) {
-        OSB_CUDA(cudaFuncSetAttribute(policy_fma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)policy_fma_smem_bytes()));
-        OSB_CUDA(cudaFuncSetAttribute(policy_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)policy_tc_smem_bytes(false)));
-        OSB_CUDA(cudaFuncSetAttribute(policy_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)policy_tc_smem_bytes(true)));
+        for (int act = ACT_TANH; act <= ACT_MIXED; ++act) {
+            const int rc = with_act<true>(act, [](auto a) {
+                OSB_CUDA(cudaFuncSetAttribute(policy_fma_kernel<a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (int)policy_fma_smem_bytes()));
+                OSB_CUDA(cudaFuncSetAttribute(policy_tc_kernel<false, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (int)policy_tc_smem_bytes(false)));
+                OSB_CUDA(cudaFuncSetAttribute(policy_tc_kernel<true, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (int)policy_tc_smem_bytes(true)));
+                return OSB_OK;
+            });
+            if (rc) return rc;
+        }
         g_policy_attr = true;
     }
     if (!acc_scratch(ACC_POLICY, policy_acc_bytes())) return OSB_ERR_CUDA;
@@ -257,18 +266,22 @@ int osb_policy_step(const float* theta, int O, int A, long long B, const float* 
         if (net_mask & (1 << net)) p.nets |= net << (2 * nnets++);
     p.vec = (O & 3) == 0 && ((uintptr_t)obs & 15) == 0;
     if (tc) {
-        const bool x3 = use_x3(precision, O);
         p.acc = acc_scratch(ACC_POLICY, policy_acc_bytes());
         if (!p.acc) return OSB_ERR_CUDA;
-        const dim3 grid(policy_tc_blocks(B, nnets), nnets);
-        if (x3) policy_tc_kernel<true><<<grid, NTHREADS, policy_tc_smem_bytes(true), s>>>(p);
-        else policy_tc_kernel<false><<<grid, NTHREADS, policy_tc_smem_bytes(false), s>>>(p);
-    } else {
-        const dim3 grid((unsigned)((B + PT - 1) / PT), nnets);
-        policy_fma_kernel<<<grid, NTHREADS, policy_fma_smem_bytes(), s>>>(p);
     }
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    const NetSpec spec = net_spec();
+    return with_act<true>(launch_act(spec, net_mask), [&](auto a) {
+        if (tc) {
+            const dim3 grid(policy_tc_blocks(B, nnets), nnets);
+            if (use_x3(precision, O)) policy_tc_kernel<true, a.value><<<grid, NTHREADS, policy_tc_smem_bytes(true), s>>>(p, spec);
+            else policy_tc_kernel<false, a.value><<<grid, NTHREADS, policy_tc_smem_bytes(false), s>>>(p, spec);
+        } else {
+            const dim3 grid((unsigned)((B + PT - 1) / PT), nnets);
+            policy_fma_kernel<a.value><<<grid, NTHREADS, policy_fma_smem_bytes(), s>>>(p, spec);
+        }
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    });
 }
 
 }  // extern "C"

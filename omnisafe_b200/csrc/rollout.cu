@@ -674,8 +674,8 @@ __device__ __forceinline__ void grid_step_arrive_wait(const StepArgs& p, int t) 
 // EVAL = true: a step of the evaluation of a saved policy (actor CTAs only, no slabs): eval_step on the synthetic env;
 // EXT, the deterministic action into act_env for env.step (the observe half is ext_eval_observe_kernel).  A launch after
 // every env has finished its episodes returns at once.
-template <bool EXT, bool EVAL = false>
-__global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
+template <bool EXT, bool EVAL, int ACT>
+__global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p, NetSpec spec) {
     if constexpr (EVAL) {
         if (__ldcg(p.ev.ctr) == 0) return;
     }
@@ -697,6 +697,7 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
     __shared__ int s_anyfin;
 
     const int net = p.is_tail ? (int)blockIdx.y + 1 : (int)blockIdx.y;
+    const Hidden<ACT> af(spec, net);
     const int env0 = blockIdx.x * RT;
     const int O = p.es.O, A = p.es.A, N = p.N, t = p.t;
     const int On = O + (p.sa.safety ? 1 : 0);            // network input width (Saute: [obs | z])
@@ -735,7 +736,7 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
             __syncthreads();
             load_obs_tile(fin, env0, N, O, 0, sMean, sStd, norm1, sX, nullptr, z_cur, true);
             __syncthreads();
-            mlp_hidden<RT>(sX, sH1, sH2, W, nchunks, load_chunk_fin);
+            mlp_hidden<RT>(sX, sH1, sH2, W, nchunks, af, load_chunk_fin);
             mlp_out<RT>(sH2, sO, W, 1);
             if (threadIdx.x < RT && env0 + threadIdx.x < N)
                 store_critic(p.sl, net, N, t, env0 + threadIdx.x, true, false, sO[threadIdx.x * LDO]);
@@ -757,7 +758,7 @@ __global__ void __launch_bounds__(NTHREADS) rollout_step_kernel(StepArgs p) {
     load_obs_tile(s_cur, env0, N, O, 0, sMean, sStd, normalize, sX,
                   (!EVAL && net == 0) ? p.sl.obs + (size_t)t * N * On : nullptr, z_cur);
     __syncthreads();
-    mlp_hidden<RT>(sX, sH1, sH2, W, nchunks, load_chunk_cur);
+    mlp_hidden<RT>(sX, sH1, sH2, W, nchunks, af, load_chunk_cur);
     mlp_out<RT>(sH2, sO, W, L.out);
     if constexpr (EVAL) {
         __syncthreads();
@@ -923,8 +924,8 @@ __device__ __forceinline__ long long* ring_slot(long long* ring, int t) { return
 // EVAL = true: the evaluation of a saved policy, as in rollout_step_kernel<EXT, true>; PERSIST (synthetic env only): ONE
 // cooperative launch runs every step until all envs have finished, the last CTA at each step's grid barrier running
 // eval_fold.
-template <bool X3, bool PERSIST, bool EXT = false, bool EVAL = false>
-__global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p) {
+template <bool X3, bool PERSIST, bool EXT, bool EVAL, int ACT>
+__global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p, NetSpec spec) {
     static_assert(!(EXT && PERSIST), "the external-env steps are one launch per step");
     if constexpr (EVAL) {
         if (__ldcg(p.ev.ctr) == 0) return;
@@ -1141,11 +1142,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) rollout_step_tc_kernel(StepArgs p
         };
         // bf16x3 actor tiles of RTA = 64 envs: one m64 block per layer.  tf32 runs its 128-row forward on them too, rows
         // past the tile computing values nobody reads.
+        const Hidden<ACT, TcTanh<X3>> af(spec, net);
         if constexpr (X3 && RING) {
-            if (net == 0) tc_forward<X3, RTA>(B0, tm, &bar, phase, sB1, sB2, 1, TcNop{}, stamp);
-            else tc_forward<X3>(B0, tm, &bar, phase, sB1, sB2, 1, TcNop{}, stamp);
+            if (net == 0) tc_forward<X3, RTA>(B0, tm, &bar, phase, sB1, sB2, 1, af, TcNop{}, stamp);
+            else tc_forward<X3>(B0, tm, &bar, phase, sB1, sB2, 1, af, TcNop{}, stamp);
         } else {
-            tc_forward<X3>(B0, tm, &bar, phase, sB1, sB2, 1, TcNop{}, stamp);
+            tc_forward<X3>(B0, tm, &bar, phase, sB1, sB2, 1, af, TcNop{}, stamp);
         }
         if (h == 0) {
             float o16[16];
@@ -1982,64 +1984,70 @@ constexpr size_t GRID_BAR_BYTES = 64 + 3 * RING_SLOT * sizeof(long long);
 template <bool EXT, bool EVAL>
 static int launch_rollout(StepArgs& p, cudaStream_t stream, bool persistent = false, bool prepare_only = false) {
     const int nets = EVAL ? 1 : (p.is_tail ? 2 : 3);
-    if (tc_tiles(p)) {
-        const bool x3 = p.precision == 2;
-        const size_t smem_tc = rollout_tc_smem_bytes(x3, persistent && !EVAL);
-        static bool attr_tc = false;
-        if (!attr_tc) {
-            if constexpr (EXT) {
-                if (int rc = ext_refuse_if_capturing(stream, "the tensor-core kernel attributes")) return rc;
+    const NetSpec spec = net_spec();
+    // the evaluation steps run the actor alone; the tail step only the critics
+    const int act = EVAL ? spec.act[0] : launch_act(spec, p.is_tail ? 6 : 7);
+    return with_act<!EVAL>(act, [&](auto a) {
+        if (tc_tiles(p)) {
+            const bool x3 = p.precision == 2;
+            const size_t smem_tc = rollout_tc_smem_bytes(x3, persistent && !EVAL);
+            static bool attr_tc = false;
+            if (!attr_tc) {
+                if constexpr (EXT) {
+                    if (int rc = ext_refuse_if_capturing(stream, "the tensor-core kernel attributes")) return rc;
+                }
+                // {tf32, bf16x3} x {one step, persistent}; EXT launches only the one-step pair
+                const void* kernels[] = {(const void*)rollout_step_tc_kernel<false, false, EXT, EVAL, a.value>,
+                                         (const void*)rollout_step_tc_kernel<true, false, EXT, EVAL, a.value>,
+                                         (const void*)rollout_step_tc_kernel<false, true, false, EVAL, a.value>,
+                                         (const void*)rollout_step_tc_kernel<true, true, false, EVAL, a.value>};
+                for (int i = 0; i < (EXT ? 2 : 4); ++i)
+                    OSB_CUDA(cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                  (int)rollout_tc_smem_bytes(i & 1, i >= 2 && !EVAL)));
+                attr_tc = true;
             }
-            // {tf32, bf16x3} x {one step, persistent}; EXT launches only the one-step pair
-            const void* kernels[] = {(const void*)rollout_step_tc_kernel<false, false, EXT, EVAL>,
-                                     (const void*)rollout_step_tc_kernel<true, false, EXT, EVAL>,
-                                     (const void*)rollout_step_tc_kernel<false, true, false, EVAL>,
-                                     (const void*)rollout_step_tc_kernel<true, true, false, EVAL>};
-            for (int i = 0; i < (EXT ? 2 : 4); ++i)
-                OSB_CUDA(cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (int)rollout_tc_smem_bytes(i & 1, i >= 2 && !EVAL)));
-            attr_tc = true;
-        }
-        if constexpr (EXT) {
-            if (acc_scratch_capacity(ACC_ROLLOUT) < rollout_tc_acc_bytes(p.N))
-                if (int rc = ext_refuse_if_capturing(stream, "a larger accumulator image")) return rc;
-        }
-        p.acc = acc_scratch(ACC_ROLLOUT, rollout_tc_acc_bytes(p.N));
-        if (!p.acc) return OSB_ERR_CUDA;
-        if (prepare_only) return OSB_OK;
-        const dim3 grid_tc = (persistent && !EVAL) ? dim3(ring_grid(p.N)) : dim3((p.N + RTC - 1) / RTC, nets);
-        if (persistent) {
-            // every CTA resident: the step barrier is a software grid barrier
-            if (!g_grid_bar) OSB_CUDA(cudaMalloc(&g_grid_bar, GRID_BAR_BYTES));
-            p.bar_ctr = g_grid_bar; p.bar_flag = g_grid_bar + 1;
-            p.ring = reinterpret_cast<long long*>(g_grid_bar + 16);
-            OSB_CUDA(cudaMemsetAsync(p.bar_ctr, 0, EVAL ? 2 * sizeof(unsigned int) : GRID_BAR_BYTES, stream));
-            void* args[] = {&p};
-            osb_count_launch();
-            OSB_CUDA(cudaLaunchCooperativeKernel(x3 ? (void*)rollout_step_tc_kernel<true, true, false, EVAL>
-                                                    : (void*)rollout_step_tc_kernel<false, true, false, EVAL>,
-                                                 grid_tc, dim3(NTHREADS), args, smem_tc, stream));
+            if constexpr (EXT) {
+                if (acc_scratch_capacity(ACC_ROLLOUT) < rollout_tc_acc_bytes(p.N))
+                    if (int rc = ext_refuse_if_capturing(stream, "a larger accumulator image")) return rc;
+            }
+            p.acc = acc_scratch(ACC_ROLLOUT, rollout_tc_acc_bytes(p.N));
+            if (!p.acc) return OSB_ERR_CUDA;
+            if (prepare_only) return OSB_OK;
+            const dim3 grid_tc = (persistent && !EVAL) ? dim3(ring_grid(p.N)) : dim3((p.N + RTC - 1) / RTC, nets);
+            if (persistent) {
+                // every CTA resident: the step barrier is a software grid barrier
+                if (!g_grid_bar) OSB_CUDA(cudaMalloc(&g_grid_bar, GRID_BAR_BYTES));
+                p.bar_ctr = g_grid_bar; p.bar_flag = g_grid_bar + 1;
+                p.ring = reinterpret_cast<long long*>(g_grid_bar + 16);
+                OSB_CUDA(cudaMemsetAsync(p.bar_ctr, 0, EVAL ? 2 * sizeof(unsigned int) : GRID_BAR_BYTES, stream));
+                NetSpec sp = spec;
+                void* args[] = {&p, &sp};
+                osb_count_launch();
+                OSB_CUDA(cudaLaunchCooperativeKernel(x3 ? (void*)rollout_step_tc_kernel<true, true, false, EVAL, a.value>
+                                                        : (void*)rollout_step_tc_kernel<false, true, false, EVAL, a.value>,
+                                                     grid_tc, dim3(NTHREADS), args, smem_tc, stream));
+                return OSB_OK;
+            }
+            if (x3) rollout_step_tc_kernel<true, false, EXT, EVAL, a.value><<<grid_tc, NTHREADS, smem_tc, stream>>>(p, spec);
+            else rollout_step_tc_kernel<false, false, EXT, EVAL, a.value><<<grid_tc, NTHREADS, smem_tc, stream>>>(p, spec);
+            OSB_LAUNCH_CHECK();
             return OSB_OK;
         }
-        if (x3) rollout_step_tc_kernel<true, false, EXT, EVAL><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
-        else rollout_step_tc_kernel<false, false, EXT, EVAL><<<grid_tc, NTHREADS, smem_tc, stream>>>(p);
+        const int On = p.es.O + (p.sa.safety ? 1 : 0);
+        const size_t smem = rollout_smem_bytes(On);
+        static size_t attr = 0;
+        if (smem > attr) {
+            if constexpr (EXT) {
+                if (int rc = ext_refuse_if_capturing(stream, "a larger shared-memory attribute")) return rc;
+            }
+            OSB_CUDA(cudaFuncSetAttribute(rollout_step_kernel<EXT, EVAL, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            attr = smem;
+        }
+        if (prepare_only) return OSB_OK;
+        rollout_step_kernel<EXT, EVAL, a.value><<<dim3((p.N + RT - 1) / RT, nets), NTHREADS, smem, stream>>>(p, spec);
         OSB_LAUNCH_CHECK();
         return OSB_OK;
-    }
-    const int On = p.es.O + (p.sa.safety ? 1 : 0);
-    const size_t smem = rollout_smem_bytes(On);
-    static size_t attr = 0;
-    if (smem > attr) {
-        if constexpr (EXT) {
-            if (int rc = ext_refuse_if_capturing(stream, "a larger shared-memory attribute")) return rc;
-        }
-        OSB_CUDA(cudaFuncSetAttribute(rollout_step_kernel<EXT, EVAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = smem;
-    }
-    if (prepare_only) return OSB_OK;
-    rollout_step_kernel<EXT, EVAL><<<dim3((p.N + RT - 1) / RT, nets), NTHREADS, smem, stream>>>(p);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    });
 }
 
 extern "C" {

@@ -1,10 +1,10 @@
-// The tensor-core MLP forward (obs -> 64 -> 64 -> out <= 16, tanh hidden layers) on tiles of 128 rows, shared by
+// The tensor-core MLP forward (obs -> 64 -> 64 -> out <= 16, hidden activation of csrc/activation.cuh) on tiles of 128 rows, shared by
 // rollout_step_tc_kernel (csrc/rollout.cu), policy_tc_kernel (csrc/policy.cu) and the actor evaluations
 // (csrc/eval_tc.cu), so that the rollout, the policy step and the evaluation compute one function bit for bit; its
 // tiles and staging also carry the Fisher-vector tangent pass (fvp_tangent_kernel, csrc/fvp_tc.cu).
 //   X3 = false: tf32 wgmma tiles (csrc/umma.cuh), layer 1 as a K loop over 64-column chunks for inputs up to 512 wide;
 //   X3 = true : split-bf16 tiles (csrc/x3.cuh), inputs up to 64 wide, one activation buffer (X, H1 and H2 overwrite
-//               each other in place: every epilogue starts after its layer's MMAs completed), accurate tanh.
+//               each other in place: every epilogue starts after its layer's MMAs completed), accurate tanh (x3::TanhAcc).
 // 256 threads: warpgroup 0 issues the MMAs; in the epilogues thread (warp w, lane l) owns tile row 32 (w % 4) + l and
 // the 32-column half w / 4.  The OUT product lands in accumulator columns [TC_C_OUT, TC_C_OUT + 16) without its bias.
 #pragma once
@@ -182,12 +182,17 @@ __device__ __forceinline__ void tc_stage_rows(uint32_t base, const float* obs, i
     }
 }
 
+// the tanh of a precision's tiles: MUFU tanh.approx for tf32, x3::tanh_acc for bf16x3 (the Tanh of Hidden<ACT, Tanh>)
+template <bool X3>
+using TcTanh = typename std::conditional<X3, x3::TanhAcc, umma::TanhFast>::type;
+
 struct TcNop {
     template <class... Ts>
     __device__ __forceinline__ void operator()(Ts...) const {}
 };
 
-// The forward of one tile: layer 1, tanh(. + b1), layer 2, tanh(. + b2), then the OUT GEMM.  Returns after the OUT
+// The forward of one tile: layer 1, f(. + b1), layer 2, f(. + b2), then the OUT GEMM; f = act, a Hidden<ACT, Tanh> with
+// the precision's tanh (umma::TanhFast for tf32, x3::TanhAcc for bf16x3).  Returns after the OUT
 // MMAs completed; `phase` is the mbarrier parity, carried across calls.
 // stage(c) stages chunk c of X (bf16x3: the whole tile, c = 0) right before layer 1 consumes it; tf32 runs layer 1 as a
 // K loop over nchunks chunks.  stage = TcNop: the caller has staged, fenced and synchronised the whole X tile.
@@ -196,9 +201,9 @@ struct TcNop {
 // written).  A row of an m64 block depends only on that row and the k-step order, so each row has the bits of the
 // 128-row forward.  The epilogues then give each row 4 threads: warp w owns rows 32 (w % 2) + lane, columns 16 (w / 2) ..
 // 16 (w / 2) + 15.
-template <bool X3, int ROWS = 128, class Stage, class After = TcNop>
+template <bool X3, int ROWS = 128, class Act, class Stage, class After = TcNop>
 __device__ __forceinline__ void tc_forward(uint32_t base, const umma::Acc& tm, uint64_t* bar, uint32_t& phase,
-                                           const float* sB1, const float* sB2, int nchunks, Stage&& stage,
+                                           const float* sB1, const float* sB2, int nchunks, const Act& act, Stage&& stage,
                                            After&& after = After{}) {
     using namespace umma;
     using T = TcTiles<X3>;
@@ -227,14 +232,14 @@ __device__ __forceinline__ void tc_forward(uint32_t base, const umma::Acc& tm, u
         constexpr int CW = ROWS == 128 ? 32 : 16;                          // columns per thread
         const int er = ROWS == 128 ? 32 * q + lane : 32 * (warp & 1) + lane, ec = ROWS == 128 ? 32 * h : 16 * (warp >> 1);
         const int eb = ROWS == 128 ? 4 + q : 4 + (warp & 1), en = ROWS == 128 ? 64 : 128;
-        auto hidden = [&](const float* sB) {   // tanh(Z + b) over the activation buffer
+        auto hidden = [&](const float* sB, int width) {   // f(Z + b) over the activation buffer
             float v[CW / 8][8];
 #pragma unroll
             for (int c8 = 0; c8 < CW / 8; ++c8) {
                 const int c0 = ec + 8 * c8;
                 x3::staged_load<64>(sZ, er, c0, v[c8]);
 #pragma unroll
-                for (int i = 0; i < 8; ++i) v[c8][i] = x3::tanh_acc(v[c8][i] + sB[c0 + i]);
+                for (int i = 0; i < 8; ++i) v[c8][i] = act(v[c8][i] + sB[c0 + i], c0 + i, width);
             }
             asm volatile("bar.sync %0, %1;\n" ::"r"(eb), "r"(en) : "memory");
 #pragma unroll
@@ -250,7 +255,7 @@ __device__ __forceinline__ void tc_forward(uint32_t base, const umma::Acc& tm, u
         }
         mbar_wait(bar, phase); phase ^= 1;
         after(1);
-        hidden(sB1);
+        hidden(sB1, act.w1);
         if (mma_wg) {
             if constexpr (ROWS == 128) x3::gemm_x3_staged<64, 4, 0>(sZ, dAct, T::SUB, 32u, dW2, T::WSUB, 32u);
             else x3::gemm_x3_rows<64, 4, 1, 0>(sZ, 0, dAct, T::SUB, 32u, dW2, T::WSUB, 32u);
@@ -258,7 +263,7 @@ __device__ __forceinline__ void tc_forward(uint32_t base, const umma::Acc& tm, u
         }
         mbar_wait(bar, phase); phase ^= 1;
         after(2);
-        hidden(sB2);
+        hidden(sB2, act.w2);
         if (mma_wg) {
             if constexpr (ROWS == 128) x3::gemm_x3<128, 16, 4, 0, 0>(tm, TC_C_OUT, dAct, T::SUB, 32u, dW3, T::W3SUB, 32u, false);
             else x3::gemm_x3_rows<16, 4, 1, 0>(tm, TC_C_OUT, 0, dAct, T::SUB, 32u, dW3, T::W3SUB, 32u);   // row m in lane m
@@ -268,11 +273,11 @@ __device__ __forceinline__ void tc_forward(uint32_t base, const umma::Acc& tm, u
         after(3);
     } else {
         const uint32_t sX = base + T::X, sH1 = base + T::H1;
-        auto hidden = [&](const float* sB, uint32_t dst) {   // tanh(Z + b) into the next layer's operand tile
+        auto hidden = [&](const float* sB, int width, uint32_t dst) {   // f(Z + b) into the next layer's operand tile
             float v[32];
             acc_ld32(tm, lane_base + TC_C_Z + 32 * h, v);
 #pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = tanh_fast(v[i] + sB[32 * h + i]);
+            for (int i = 0; i < 32; ++i) v[i] = act(v[i] + sB[32 * h + i], 32 * h + i, width);
             store_row32(dst, 32 * q + lane, 32 * h, TC_ROWS, v);
             fence_async_smem();
             __syncthreads();
@@ -284,11 +289,11 @@ __device__ __forceinline__ void tc_forward(uint32_t base, const umma::Acc& tm, u
             mbar_wait(bar, phase); phase ^= 1;
         }
         after(1);
-        hidden(sB1, sH1);
+        hidden(sB1, act.w1, sH1);
         if (mma_wg) { tc_gemm(tm, TC_C_Z, sH1, TC_ROWS, base + T::W2, 64, 128, 64, 64, false); mma_commit(bar); }
         mbar_wait(bar, phase); phase ^= 1;
         after(2);
-        hidden(sB2, sX);
+        hidden(sB2, act.w2, sX);
         if (mma_wg) { tc_gemm(tm, TC_C_OUT, sX, TC_ROWS, base + T::W3, 16, 128, 16, 64, false); mma_commit(bar); }
         mbar_wait(bar, phase); phase ^= 1;
         after(3);
@@ -300,24 +305,25 @@ __device__ __forceinline__ void tc_forward(uint32_t base, const umma::Acc& tm, u
 // under the others' MMAs.  The m64 blocks are those of tc_forward (a row depends only on that row and the k-step
 // order; the same products in the same order), so every row has the bits of the 128-row forward.  Every layer's A
 // operand is in registers: the m64k16 fragments of the bf16x3 pieces, a[piece][ks] for columns 16 ks .. 16 ks + 15
-// (x3_block_ra).  The caller splits X into a; the hidden epilogues split tanh(Z + b) into it, the accumulator fragment
+// (x3_block_ra).  The caller splits X into a; the hidden epilogues split f(Z + b) (f = act) into it, the accumulator fragment
 // of one layer being the A fragment of the next, so the MMAs read only the weights from shared memory.
 // The weights are at the TcTiles<true> offsets from base.  Returns the OUT product without its bias as the m64n16
 // fragment: element (rr, j, e) of thread (warp w, lane l) of the warpgroup is row 16 w + l / 4 + 8 rr of its 64 rows,
 // column 8 j + 2 (l % 4) + e.
+template <class Act>
 __device__ __forceinline__ void tc_forward_x3_half(uint32_t base, uint32_t (&a)[3][4][4], const float* sB1,
-                                                   const float* sB2, float (&out)[8]) {
+                                                   const float* sB2, const Act& act, float (&out)[8]) {
     using namespace umma;
     using T = TcTiles<true>;
     const uint64_t dW1 = x3::desc128(base + T::W1), dW2 = x3::desc128(base + T::W2), dW3 = x3::desc128(base + T::W3);
     const int l = threadIdx.x & 31;
-    auto hidden = [&](const float (&d)[32], const float* sB) {
+    auto hidden = [&](const float (&d)[32], const float* sB, int width) {
 #pragma unroll
         for (int j = 0; j < 8; ++j)
 #pragma unroll
             for (int rr = 0; rr < 2; ++rr) {
                 const int c = 8 * j + 2 * (l & 3), q = 2 * (j & 1) + rr;
-                x3::split2(x3::tanh_acc(d[4 * j + 2 * rr] + sB[c]), x3::tanh_acc(d[4 * j + 2 * rr + 1] + sB[c + 1]),
+                x3::split2(act(d[4 * j + 2 * rr] + sB[c], c, width), act(d[4 * j + 2 * rr + 1] + sB[c + 1], c + 1, width),
                            a[0][j >> 1][q], a[1][j >> 1][q], a[2][j >> 1][q]);
             }
     };
@@ -327,11 +333,11 @@ __device__ __forceinline__ void tc_forward_x3_half(uint32_t base, uint32_t (&a)[
     x3::x3_block_ra<0, 8, 4>(d, a, x3::desc_fresh(dW1), T::WSUB, 32u);
     wg_wait<0>();
     acc_fence(d);
-    hidden(d, sB1);
+    hidden(d, sB1, act.w1);
     x3::x3_block_ra<0, 8, 4>(d, a, x3::desc_fresh(dW2), T::WSUB, 32u);
     wg_wait<0>();
     acc_fence(d);
-    hidden(d, sB2);
+    hidden(d, sB2, act.w2);
 #pragma unroll
     for (int i = 0; i < 8; ++i) out[i] = 0.f;
     x3::x3_block_ra<0, 2, 4>(out, a, x3::desc_fresh(dW3), T::W3SUB, 32u);

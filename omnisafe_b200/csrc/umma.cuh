@@ -320,6 +320,9 @@ __device__ __forceinline__ float tanh_fast(float x) {
     asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
+struct TanhFast {
+    __device__ __forceinline__ float operator()(float x) const { return tanh_fast(x); }
+};
 // explicit shared-window (32-bit address) accessors: keeps every tile access an LDS/STS
 __device__ __forceinline__ float lds(uint32_t a) {
     float v;

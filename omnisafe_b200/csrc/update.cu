@@ -68,11 +68,12 @@ __device__ __forceinline__ void block_reduce_store(float (&v)[NV], float* sRed, 
 
 // DMU = true: LOSS_DMU -- the backward yields J^T of a supplied output gradient (no log_std term, no statistics but the
 // row count): b.act carries dL/dmu [rows][A] for the actor, b.tv_r / b.tv_c carry dL/dV [rows] for a critic.
-template <bool DMU = false>
-__global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p) {
+template <bool DMU, int ACT>
+__global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p, NetSpec spec) {
     if (p.stop_flag && *p.stop_flag) return;
     const int net = blockIdx.y;
     if (!((p.net_mask >> net) & 1)) return;
+    const Hidden<ACT> af(spec, net);
 
     extern __shared__ __align__(16) float smem[];
     NetSmem W;
@@ -130,7 +131,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p)
         if (nchunks > 1) load_w1_chunk(theta, L, 0, W);
         __syncthreads();
         auto load_chunk = [&](int kc) { load_w1_chunk(theta, L, kc, W); gather_obs(p.b.obs, sRow, O, kc, sX); };
-        mlp_hidden<UT>(sX, sH1, sH2, W, nchunks, load_chunk);
+        mlp_hidden<UT>(sX, sH1, sH2, W, nchunks, af, load_chunk);
         mlp_out<UT>(sH2, sO, W, L.out);
 
         // ---- per-sample loss and dL/dOUT (threads < UT), dOUT overwrites sO ---------------------
@@ -202,7 +203,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p)
                 ab3 += c;
             }
         }
-        {   // dZ2 = (dOUT . W3) * (1 - H2^2) -> sD
+        {   // dZ2 = (dOUT . W3) * f'(H2) -> sD
             float acc[UT / 16][4];
             gemm_nt<UT, LDO, LDO>(sO, W.w3t, OUTP, acc);
             const int tm = threadIdx.x >> 4, tn = threadIdx.x & 15;
@@ -212,7 +213,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p)
                 for (int j = 0; j < 4; ++j) {
                     const int mm = tm + 16 * i, n = tn + 16 * j;
                     const float h = sH2[mm * LD + n];
-                    sD[mm * LD + n] = acc[i][j] * (1.f - h * h);
+                    sD[mm * LD + n] = acc[i][j] * af.d(h);
                 }
         }
         __syncthreads();
@@ -229,7 +230,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p)
                 ab2 += c;
             }
         }
-        {   // dZ1 = (dZ2 . W2) * (1 - H1^2) -> sH2 (H2 is dead now)
+        {   // dZ1 = (dZ2 . W2) * f'(H1) -> sH2 (H2 is dead now)
             float acc[UT / 16][4];
             gemm_nt<UT, LD, LD>(sD, W.w2t, HID, acc);
             __syncthreads();   // all reads of sH2 (dW3 above) and sD are done before overwriting sH2
@@ -240,7 +241,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p)
                 for (int j = 0; j < 4; ++j) {
                     const int mm = tm + 16 * i, n = tn + 16 * j;
                     const float h = sH1[mm * LD + n];
-                    sH2[mm * LD + n] = acc[i][j] * (1.f - h * h);
+                    sH2[mm * LD + n] = acc[i][j] * af.d(h);
                 }
         }
         __syncthreads();
@@ -334,7 +335,9 @@ struct EvalArgs {
     int stride;              // evaluate rows 0, stride, 2*stride, ... (fvp_sample_freq)
 };
 
-__global__ void __launch_bounds__(NTHREADS, 1) actor_eval_kernel(EvalArgs p) {
+template <int ACT>
+__global__ void __launch_bounds__(NTHREADS, 1) actor_eval_kernel(EvalArgs p, NetSpec spec) {
+    const Hidden<ACT> af(spec, 0);
     extern __shared__ __align__(16) float smem[];
     NetSmem W;
     float* base = carve_net_smem<false>(smem, W);
@@ -372,7 +375,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) actor_eval_kernel(EvalArgs p) {
         if (nchunks > 1) load_w1_chunk(p.theta, L, 0, W);
         __syncthreads();
         auto load_chunk = [&](int kc) { load_w1_chunk(p.theta, L, kc, W); gather_obs(p.b.obs, sRow, O, kc, sX); };
-        mlp_hidden<UT>(sX, sH1, sH2, W, nchunks, load_chunk);
+        mlp_hidden<UT>(sX, sH1, sH2, W, nchunks, af, load_chunk);
         mlp_out<UT>(sH2, sO, W, A);
         if (threadIdx.x < UT) {
             const long long row = sRow[threadIdx.x];
@@ -435,7 +438,9 @@ __device__ __forceinline__ void load_mat64(const float* __restrict__ src, int ld
     }
 }
 
-__global__ void __launch_bounds__(NTHREADS, 1) fvp_kernel(FvpArgs p) {
+template <int ACT>
+__global__ void __launch_bounds__(NTHREADS, 1) fvp_kernel(FvpArgs p, NetSpec spec) {
+    const Hidden<ACT> af(spec, 0);
     extern __shared__ __align__(16) float smem[];
     NetSmem W;
     float* base = carve_net_smem<true>(smem, W);
@@ -521,9 +526,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) fvp_kernel(FvpArgs p) {
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const int mm = tm + 16 * i, n = tn + 16 * j;
-                const float h = tanhf(z[i][j] + W.b1[n]);
+                const float h = af(z[i][j] + W.b1[n], n, af.w1);
                 sH1[mm * LD + n] = h;
-                sT[mm * LD + n] = (1.f - h * h) * (dz[i][j] + vb1[n]);   // dH1
+                sT[mm * LD + n] = af.d(h) * (dz[i][j] + vb1[n]);   // dH1
             }
         __syncthreads();
         // layer 2: Z2 = H1 W2^T + b2 ; dZ2 = H1 V2^T + dH1 W2^T + vb2
@@ -536,9 +541,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) fvp_kernel(FvpArgs p) {
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const int mm = tm + 16 * i, n = tn + 16 * j;
-                const float h = tanhf(z[i][j] + W.b2[n]);
+                const float h = af(z[i][j] + W.b2[n], n, af.w2);
                 sH2[mm * LD + n] = h;
-                sT[mm * LD + n] = (1.f - h * h) * (dz[i][j] + acc[i][j] + vb2[n]);   // dH2
+                sT[mm * LD + n] = af.d(h) * (dz[i][j] + acc[i][j] + vb2[n]);   // dH2
             }
         __syncthreads();
         // output tangent: dMu = H2 V3^T + dH2 W3^T + vb3 ; dOUT = dMu / sigma^2 * scale
@@ -582,7 +587,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fvp_kernel(FvpArgs p) {
             for (int j = 0; j < 4; ++j) {
                 const int mm = tm + 16 * i, n = tn + 16 * j;
                 const float h = sH2[mm * LD + n];
-                sT[mm * LD + n] = acc[i][j] * (1.f - h * h);   // dZ2
+                sT[mm * LD + n] = acc[i][j] * af.d(h);   // dZ2
             }
         __syncthreads();
         {
@@ -606,7 +611,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fvp_kernel(FvpArgs p) {
             for (int j = 0; j < 4; ++j) {
                 const int mm = tm + 16 * i, n = tn + 16 * j;
                 const float h = sH1[mm * LD + n];
-                sH2[mm * LD + n] = acc[i][j] * (1.f - h * h);   // dZ1
+                sH2[mm * LD + n] = acc[i][j] * af.d(h);   // dZ1
             }
         {
             const int j0 = (threadIdx.x >> 4) * 4, k0 = (threadIdx.x & 15) * 4;
@@ -717,23 +722,35 @@ int osb_minibatch_grad(const float* theta, int O, int A, const float* obs, const
     p.P = actor_layout(O, A).size + 2 * critic_layout(O, A).size;
     p.net_mask = net_mask;
     const size_t smem = grad_smem_bytes();
-    static bool attr = false;
-    if (!attr) {
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = true;
-    }
+    const NetSpec spec = net_spec();
     dim3 grid(osb_update_grid_blocks(mb_count), 3);
     if (loss_two_pass(loss_kind) && (net_mask & 1)) {   // pass 1: actor forward only
         GradArgs q = p;
         q.forward_only = 1; q.net_mask = 1;
-        minibatch_grad_kernel<false><<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(q);
-        OSB_LAUNCH_CHECK();
-        const int rc = pass1_gate(stats_part, (int)grid.x, stop_flag, p.lc, (cudaStream_t)stream);
+        const int rc = with_act<false>(spec.act[0], [&](auto a) {
+            static bool attr = false;
+            if (!attr) {
+                OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_kernel<false, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                attr = true;
+            }
+            minibatch_grad_kernel<false, a.value><<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(q, spec);
+            OSB_LAUNCH_CHECK();
+            return OSB_OK;
+        });
         if (rc) return rc;
+        const int rg = pass1_gate(stats_part, (int)grid.x, stop_flag, p.lc, (cudaStream_t)stream);
+        if (rg) return rg;
     }
-    minibatch_grad_kernel<false><<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(p);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    return with_act<true>(launch_act(spec, net_mask), [&](auto a) {
+        static bool attr = false;
+        if (!attr) {
+            OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_kernel<false, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            attr = true;
+        }
+        minibatch_grad_kernel<false, a.value><<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(p, spec);
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    });
 }
 
 // Full-batch actor pass.  mu_store != NULL: write mu(theta) for every row (old-policy snapshot).
@@ -751,18 +768,23 @@ int osb_actor_eval(const float* theta_actor, int O, int A, const float* obs, con
     p.mu_old = mu_old; p.theta = theta_actor; p.logstd_old = logstd_old; p.lagrange = lagrange; p.mu_store = mu_store;
     p.part = workspace; p.O = O; p.A = A; p.stride = stride;
     const size_t smem = eval_smem_bytes();
-    static bool attr = false;
-    if (!attr) {
-        OSB_CUDA(cudaFuncSetAttribute(actor_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = true;
-    }
     const long long nrows = (total + stride - 1) / stride;
     long long tiles = (nrows + UT - 1) / UT;
     const int cap = 2 * grid_sms();
     const int blocks = (int)(tiles < cap ? tiles : cap);
     cudaStream_t s = (cudaStream_t)stream;
-    actor_eval_kernel<<<blocks, NTHREADS, smem, s>>>(p);
-    OSB_LAUNCH_CHECK();
+    const NetSpec spec = net_spec();
+    const int rc = with_act<false>(spec.act[0], [&](auto a) {
+        static bool attr = false;
+        if (!attr) {
+            OSB_CUDA(cudaFuncSetAttribute(actor_eval_kernel<a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            attr = true;
+        }
+        actor_eval_kernel<a.value><<<blocks, NTHREADS, smem, s>>>(p, spec);
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    });
+    if (rc) return rc;
     return mu_store ? OSB_OK : eval_reduce(workspace, blocks, out, s);
 }
 
@@ -779,14 +801,17 @@ int osb_fvp_partials(const float* theta_actor, const float* vec, int O, int A, c
     OSB_CHECK_ARG(theta_actor && vec && obs && gpart && total > 0 && stride > 0, "bad argument");
     FvpArgs p{obs, total, stride, theta_actor, vec, gpart, O, A};
     const size_t smem = fvp_smem_bytes();
-    static bool attr = false;
-    if (!attr) {
-        OSB_CUDA(cudaFuncSetAttribute(fvp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = true;
-    }
-    fvp_kernel<<<osb_fvp_grid_blocks(total, stride), NTHREADS, smem, (cudaStream_t)stream>>>(p);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    const NetSpec spec = net_spec();
+    return with_act<false>(spec.act[0], [&](auto a) {
+        static bool attr = false;
+        if (!attr) {
+            OSB_CUDA(cudaFuncSetAttribute(fvp_kernel<a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            attr = true;
+        }
+        fvp_kernel<a.value><<<osb_fvp_grid_blocks(total, stride), NTHREADS, smem, (cudaStream_t)stream>>>(p, spec);
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    });
 }
 
 int osb_tc_grid_blocks(long long rows, int net_mask);
@@ -816,14 +841,17 @@ int osb_actor_dmu_backward(const float* theta_actor, int O, int A, const float* 
     p.theta = theta_actor; p.gpart = gpart; p.stats_part = stats_scratch; p.stop_flag = nullptr;
     p.O = O; p.A = A; p.P = actor_layout(O, A).size; p.net_mask = 1; p.value_out = nullptr;
     const size_t smem = grad_smem_bytes();
-    static bool attr = false;
-    if (!attr) {
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = true;
-    }
-    minibatch_grad_kernel<true><<<dim3(osb_fvp_grid_blocks(rows, 1), 1), NTHREADS, smem, (cudaStream_t)stream>>>(p);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    const NetSpec spec = net_spec();
+    return with_act<false>(spec.act[0], [&](auto a) {
+        static bool attr = false;
+        if (!attr) {
+            OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_kernel<true, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            attr = true;
+        }
+        minibatch_grad_kernel<true, a.value><<<dim3(osb_fvp_grid_blocks(rows, 1), 1), NTHREADS, smem, (cudaStream_t)stream>>>(p, spec);
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    });
 }
 
 // The critic's CTAs are those of a stepwise update launch of that critic alone over a minibatch of `rows`
@@ -852,14 +880,17 @@ int osb_critic_dv_backward(const float* theta, int O, int A, int net, const floa
     p.theta = theta; p.gpart = gpart; p.stats_part = stats_scratch; p.stop_flag = nullptr;
     p.O = O; p.A = A; p.P = P; p.net_mask = 1 << net; p.value_out = value;
     const size_t smem = grad_smem_bytes();
-    static bool attr = false;
-    if (!attr) {
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = true;
-    }
-    minibatch_grad_kernel<true><<<dim3(osb_update_grid_blocks(rows), net + 1), NTHREADS, smem, (cudaStream_t)stream>>>(p);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    const NetSpec spec = net_spec();
+    return with_act<false>(spec.act[1], [&](auto a) {
+        static bool attr = false;
+        if (!attr) {
+            OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_kernel<true, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            attr = true;
+        }
+        minibatch_grad_kernel<true, a.value><<<dim3(osb_update_grid_blocks(rows), net + 1), NTHREADS, smem, (cudaStream_t)stream>>>(p, spec);
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    });
 }
 
 }  // extern "C"

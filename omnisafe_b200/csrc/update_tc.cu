@@ -8,14 +8,14 @@
 // time in transposed form by a role-swapped MMA (D^T = W * X^T) instead of a transposed copy:
 //
 //   per 128-sample tile and network (O <= 64; for 64 < O <= 512, MMA1 / MMA2 and MMA9 loop over 64-column chunks of X):
-//     MMA1  Z1    [s][n] = X  * W1^T      -> H1    = tanh(.+b1)            (A operand of layer 2)
+//     MMA1  Z1    [s][n] = X  * W1^T      -> H1    = f(.+b1)               (A operand of layer 2)
 //     MMA2  Z1^T  [n][s] = W1 * X^T       -> H1^T                          (B operand of dW2)
 //     MMA3  Z2    [s][n] = H1 * W2^T      -> H2
 //     MMA4  OUT   [s][o] = H2 * W3^T      -> per-sample loss, dOUT
-//     MMA5  dZ2   [s][k] = dOUT * W3      -> * (1 - H2^2)                  (B operand of dZ1^T)
-//     MMA6  dZ2^T [k][s] = W3^T * dOUT^T  -> * (1 - H2^2)                  (A operand of dW2)
+//     MMA5  dZ2   [s][k] = dOUT * W3      -> * f'(H2)                      (B operand of dZ1^T)
+//     MMA6  dZ2^T [k][s] = W3^T * dOUT^T  -> * f'(H2)                      (A operand of dW2)
 //     MMA7  dW2   [j][k] += dZ2^T * H1    (accumulator images kept across tiles)
-//     MMA8  dZ1^T [k][s] = W2^T * dZ2^T   -> * (1 - H1^2)                  (A operand of dW1)
+//     MMA8  dZ1^T [k][s] = W2^T * dZ2^T   -> * f'(H1)                      (A operand of dW1)
 //     MMA9  dW1   [j][o] += dZ1^T * X     (accumulator images kept across tiles)
 //   dW3, the bias gradients and d log_std stay on the CUDA cores (tiny).
 #include "common.cuh"
@@ -76,12 +76,13 @@ __device__ __forceinline__ void load_row16(uint32_t base, int r, int c0, int R, 
 // cost surrogate: the headline path) carries none of their registers or branches.
 // DMU = LOSS_DMU only: the supplied dL/dmu (fvp_dmu, per row) or, for a critic, dL/dV (tv_r / tv_c) is dOUT as it
 // stands, no loss, no log_std term.
-template <bool CHUNKED, bool EXT, bool DMU = false>
-__global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
+template <bool CHUNKED, bool EXT, bool DMU, int ACT>
+__global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p, NetSpec spec) {
     if (p.stop_flag && *p.stop_flag) return;
     // one network selected: grid.y == 1 and all of grid.x (up to one CTA per SM) works on that network
     const int net = (gridDim.y == 1) ? (__ffs(p.net_mask) - 1) : (int)blockIdx.y;
     if (!((p.net_mask >> net) & 1)) return;
+    const Hidden<ACT, umma::TanhFast> af(spec, net);
 
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;   // tiles need 1024 B alignment
@@ -321,7 +322,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             float v[16];
             acc_ld16(tm, lane_base + C_Z + c16, v);
 #pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] = tanh_fast(v[i] + sB1[c16 + i]);
+            for (int i = 0; i < 16; ++i) v[i] = af(v[i] + sB1[c16 + i], c16 + i, af.w1);
             store_row16(B2, s_row, c16, TT, v);
         }
         fence_async_smem();
@@ -332,13 +333,13 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             tc_gemm(tm, C_ZT2, sW2, 64, B2, TT, 64, 128, 64, false);
             mma_commit(&bar);
         }
-        {   // deferred: H1^T = tanh(Z1^T + b1) -> B3 (B operand of dW2, needed only in P5)
+        {   // deferred: H1^T = f(Z1^T + b1) -> B3 (B operand of dW2, needed only in P5)
             float w[32];
             acc_ld32(tm, lane_base + C_ZT + c32, w);
             if (lane < 16) {
                 const float bb = sB1[t_row];
 #pragma unroll
-                for (int i = 0; i < 32; ++i) w[i] = tanh_fast(w[i] + bb);
+                for (int i = 0; i < 32; ++i) w[i] = af(w[i] + bb, t_row, af.w1);
                 store_row32(B3, t_row, c32, 64, w);
             }
         }
@@ -347,7 +348,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             float v[16];
             acc_ld16(tm, lane_base + C_Z + c16, v);
 #pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] = tanh_fast(v[i] + sB2[c16 + i]);
+            for (int i = 0; i < 16; ++i) v[i] = af(v[i] + sB2[c16 + i], c16 + i, af.w2);
             store_row16(B0, s_row, c16, TT, v);                  // H2 (X is dead)
         }
         fence_async_smem();
@@ -357,13 +358,13 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             tc_gemm(tm, C_OUT, B0, TT, sW3, 16, 128, 16, 64, false);
             mma_commit(&bar);
         }
-        {   // deferred: H2^T = tanh(Z2^T + b2) -> B2 (H1 is dead: MMA3 / MMA3T completed)
+        {   // deferred: H2^T = f(Z2^T + b2) -> B2 (H1 is dead: MMA3 / MMA3T completed)
             float w[32];
             acc_ld32(tm, lane_base + C_ZT2 + c32, w);
             if (lane < 16) {
                 const float bb = sB2[t_row];
 #pragma unroll
-                for (int i = 0; i < 32; ++i) w[i] = tanh_fast(w[i] + bb);
+                for (int i = 0; i < 32; ++i) w[i] = af(w[i] + bb, t_row, af.w2);
                 store_row32(B2, t_row, c32, 64, w);
             }
         }
@@ -485,7 +486,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             if (lane < 16) {
                 load_row32(B2, t_row, c32, 64, hh);              // H2^T
 #pragma unroll
-                for (int i = 0; i < 32; ++i) w[i] *= (1.f - hh[i] * hh[i]);
+                for (int i = 0; i < 32; ++i) w[i] *= af.d(hh[i]);
                 store_row32(B4, t_row, c32, 64, w);              // dZ2^T [k][s]
             }
         }
@@ -495,7 +496,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             acc_ld16(tm, lane_base + C_Z + c16, v);
             load_row16(B0, s_row, c16, TT, hh);
 #pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] *= (1.f - hh[i] * hh[i]);
+            for (int i = 0; i < 16; ++i) v[i] *= af.d(hh[i]);
             store_row16(B2, s_row, c16, TT, v);                  // dZ2 [s][k]
         }
         fence_async_smem();
@@ -525,7 +526,7 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p) {
             if (lane < 16) {
                 load_row32(B3, t_row, c32, 64, hh);
 #pragma unroll
-                for (int i = 0; i < 32; ++i) w[i] *= (1.f - hh[i] * hh[i]);
+                for (int i = 0; i < 32; ++i) w[i] *= af.d(hh[i]);
                 store_row32(B0, t_row, c32, 64, w);              // dZ1^T [k][s] (H2 is dead)
             }
         }
@@ -646,28 +647,31 @@ static size_t tc_smem_bytes() {
 
 static int launch_grad_tc(TcArgs& p, int nblocks, cudaStream_t stream) {
     const size_t smem = tc_smem_bytes();
-    static bool attr = false;
-    if (!attr) {
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = true;
-    }
     const bool single = (p.net_mask & (p.net_mask - 1)) == 0;     // one network: it gets every CTA
     dim3 grid(nblocks, single ? 1 : 3);
     p.acc = acc_scratch(ACC_UPDATE_TC, (size_t)grid.x * grid.y * 128 * TC_COLS * sizeof(float));
     if (!p.acc) return OSB_ERR_CUDA;
     const bool ext = loss_two_pass(p.lc.kind) || p.lc.kind == LOSS_FVP;
-    if (p.O > 64) {
-        if (ext) minibatch_grad_tc_kernel<true, true><<<grid, NTC, smem, stream>>>(p);
-        else minibatch_grad_tc_kernel<true, false><<<grid, NTC, smem, stream>>>(p);
-    } else {
-        if (ext) minibatch_grad_tc_kernel<false, true><<<grid, NTC, smem, stream>>>(p);
-        else minibatch_grad_tc_kernel<false, false><<<grid, NTC, smem, stream>>>(p);
-    }
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    const NetSpec spec = net_spec();
+    return with_act<true>(launch_act(spec, p.net_mask), [&](auto a) {
+        static bool attr = false;
+        if (!attr) {
+            OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<false, false, false, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<false, true, false, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<true, false, false, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<true, true, false, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            attr = true;
+        }
+        if (p.O > 64) {
+            if (ext) minibatch_grad_tc_kernel<true, true, false, a.value><<<grid, NTC, smem, stream>>>(p, spec);
+            else minibatch_grad_tc_kernel<true, false, false, a.value><<<grid, NTC, smem, stream>>>(p, spec);
+        } else {
+            if (ext) minibatch_grad_tc_kernel<false, true, false, a.value><<<grid, NTC, smem, stream>>>(p, spec);
+            else minibatch_grad_tc_kernel<false, false, false, a.value><<<grid, NTC, smem, stream>>>(p, spec);
+        }
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    });
 }
 
 extern "C" {
@@ -725,18 +729,21 @@ static int launch_dmu_tc(TcArgs& p, int nb, cudaStream_t stream) {
     p.stop_flag = nullptr; p.fvp_vec = nullptr; p.fvp_scale = 1.f;
     p.forward_only = 0;
     const size_t smem = tc_smem_bytes();
-    static bool attr = false;
-    if (!attr) {
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = true;
-    }
     p.acc = acc_scratch(ACC_UPDATE_TC, (size_t)nb * 128 * TC_COLS * sizeof(float));
     if (!p.acc) return OSB_ERR_CUDA;
-    if (p.O > 64) minibatch_grad_tc_kernel<true, false, true><<<dim3(nb, 1), NTC, smem, stream>>>(p);
-    else minibatch_grad_tc_kernel<false, false, true><<<dim3(nb, 1), NTC, smem, stream>>>(p);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    const NetSpec spec = net_spec();
+    return with_act<false>(launch_act(spec, p.net_mask), [&](auto a) {
+        static bool attr = false;
+        if (!attr) {
+            OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<false, false, true, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_tc_kernel<true, false, true, a.value>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            attr = true;
+        }
+        if (p.O > 64) minibatch_grad_tc_kernel<true, false, true, a.value><<<dim3(nb, 1), NTC, smem, stream>>>(p, spec);
+        else minibatch_grad_tc_kernel<false, false, true, a.value><<<dim3(nb, 1), NTC, smem, stream>>>(p, spec);
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    });
 }
 
 int osb::dmu_backward_tc(const float* theta_actor, int O, int A, const float* obs, const float* dmu, int rows, float* gpart,

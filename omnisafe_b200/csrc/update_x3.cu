@@ -10,11 +10,11 @@
 //
 //   per tile (activations stored ONCE as [sample][feature] bf16x3 tiles; the weight-gradient GEMMs read the
 //   same tiles MN-major, so there are no transposed copies):
-//     Z1   = X  W1^T            -> H1 = tanh(. + b1)
-//     Z2   = H1 W2^T            -> H2 = tanh(. + b2)
+//     Z1   = X  W1^T            -> H1 = f(. + b1)          (f: csrc/activation.cuh)
+//     Z2   = H1 W2^T            -> H2 = f(. + b2)
 //     OUT  = H2 W3^T            -> per-sample loss, dOUT
-//     dZ2' = dOUT W3            -> dZ2 = dZ2' (1 - H2^2)   (stored over H2)     | dW3^T += H2^T dOUT
-//     dZ1' = dZ2 W2             -> dZ1 = dZ1' (1 - H1^2)   (stored over H1)     | dW2 += dZ2^T H1, db2 += dZ2^T 1
+//     dZ2' = dOUT W3            -> dZ2 = dZ2' f'(H2)       (stored over H2)     | dW3^T += H2^T dOUT
+//     dZ1' = dZ2 W2             -> dZ1 = dZ1' f'(H1)       (stored over H1)     | dW2 += dZ2^T H1, db2 += dZ2^T 1
 //                                                                               | dW1 += dZ1^T X,  db1 += dZ1^T 1
 //   Rows 0-63 and rows 64-127 of a tile never meet in the forward and backward chain (only the weight-gradient
 //   products contract over samples), so the tile runs as a pipeline of its two row halves: every product of the chain
@@ -77,6 +77,7 @@ struct X3Args {
                                  // then (id, clock) pairs (tools/x3_stage_times.py)
     float* acc;                  // accumulator images, one [128][T_COLS] per CTA
     float* value_out;            // LOSS_DMU on a critic (DMU instantiation only), or null: V per row as this launch computes it
+    NetSpec spec;          // hidden activations and widths (csrc/activation.cuh)
 };
 
 constexpr int XT = 128;                      // samples per tile
@@ -219,14 +220,21 @@ constexpr int PSTR = 9472;          // FUSED: row stride of the private partial-
 //   distributed.py:L193-198), apply torch-Adam and re-stage the new weights: no relaunch, no separate
 //   optimiser kernel.
 // AP = padded action width of the loss epilogue (8 or 16).
+constexpr int X3_ACT_STRIDE = 32;
+constexpr int x3_apv(int AP, int ACT) { return AP + X3_ACT_STRIDE * ACT; }
 // DMU = LOSS_DMU only (FUSED = false): the supplied dL/dmu (fvp_dmu, per row) or, for a critic, dL/dV (tv_r / tv_c)
 // is dOUT as it stands, no loss, no log_std term.
 // (20 warps = 640 threads: 96 registers each, the register file divided in units of 8 per thread)
-template <bool FUSED, int AP, bool DMU = false>
+// APV = x3_apv(AP, ACT): the action width and the hidden activation in one template argument, so that the tanh
+// instantiations (APV = AP) keep the symbols minibatch_grad_x3_kernel<FUSED, AP, DMU> that profiles and the SASS tests
+// name; the activations' widths come in p.spec.
+template <bool FUSED, int APV, bool DMU = false>
 __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
+    constexpr int AP = APV % X3_ACT_STRIDE, ACT = APV / X3_ACT_STRIDE;
     if (p.stop_flag && *p.stop_flag) return;
     const int net = (gridDim.y == 1) ? (__ffs(p.net_mask) - 1) : (int)blockIdx.y;
     if (!((p.net_mask >> net) & 1)) return;
+    const Hidden<ACT, TanhAcc> af(p.spec, net);
 
     extern __shared__ __align__(16) uint8_t smem_raw[];
     const uint32_t pad = (1024u - (smem_u32(smem_raw) & 1023u)) & 1023u;
@@ -548,7 +556,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                         }
                     }
                 }
-                // ---- E1: H1 = tanh(Z1 + b1) -------------------------------------------------------------------
+                // ---- E1: H1 = f(Z1 + b1) ----------------------------------------------------------------------
                 // Z1 is staged over H1 (see the MMA-issue loop): the four warps of the rows read their values of it, meet,
                 // and only then store the pieces of H1 over them
                 mbar_wait_a(bar(DONE_C1_0 + rh), par);
@@ -559,13 +567,13 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     const int c0 = 32 * ph + 8 * h;
                     staged_load<64>(sZ1, s_row, c0, hv[ph]);
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) hv[ph][i] = tanh_acc(hv[ph][i] + sB1[c0 + i]);
+                    for (int i = 0; i < 8; ++i) hv[ph][i] = af(hv[ph][i] + sB1[c0 + i], c0 + i, af.w1);
                 }
                 rows_bar_sync(q);
 #pragma unroll
                 for (int ph = 0; ph < 2; ++ph) store8_x3(sbase + OFF_H1, ACT_SUB, s_row, 32 * ph + 8 * h, hv[ph]);
                 announce(RDY_H1_0 + rh);
-                // ---- E2: H2 = tanh(Z2 + b2), from Z2 staged over H2 --------------------------------------------
+                // ---- E2: H2 = f(Z2 + b2), from Z2 staged over H2 -----------------------------------------------
                 stamp(4);
                 mbar_wait_a(bar(DONE_C2_0 + rh), par);
                 stamp(5);
@@ -574,7 +582,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     const int c0 = 32 * ph + 8 * h;
                     staged_load<64>(sZ2, s_row, c0, hv[ph]);
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) hv[ph][i] = tanh_acc(hv[ph][i] + sB2[c0 + i]);
+                    for (int i = 0; i < 8; ++i) hv[ph][i] = af(hv[ph][i] + sB2[c0 + i], c0 + i, af.w2);
                 }
                 rows_bar_sync(q);
 #pragma unroll
@@ -659,7 +667,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     rpar ^= 1;
                     continue;
                 }
-                // ---- E4: dZ2 = (dOUT W3) (1 - H2^2), stored over H2 once dW3 has read it --------------------------
+                // ---- E4: dZ2 = (dOUT W3) f'(H2), stored over H2 once dW3 has read it -----------------------------
                 if (has_next) prefetch_x(sRowNext);                        // next tile's rows fly during the backward half
                 mbar_wait_a(bar(DONE_C4A_0 + rh), par);
                 stamp(10);
@@ -671,7 +679,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     acc_ld8(tm, lane_base + T_ZA + (uint32_t)c0, v);
                     load8_x3(sbase + OFF_H2, ACT_SUB, s_row, c0, hh);
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) dz[8 * ph + i] = v[i] * (1.f - hh[i] * hh[i]);
+                    for (int i = 0; i < 8; ++i) dz[8 * ph + i] = v[i] * af.d(hh[i]);
                 }
                 stamp(11);
                 mbar_wait_a(bar(DONE_C4B), par);
@@ -684,7 +692,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     store8_x3(sbase + OFF_H2, ACT_SUB, s_row, 32 * ph + 8 * h, v);
                 }
                 announce(RDY_DZ2_0 + rh);
-                // ---- E5: dZ1 = (dZ2 W2) (1 - H1^2), stored over H1 once dW2 has read it --------------------------
+                // ---- E5: dZ1 = (dZ2 W2) f'(H1), stored over H1 once dW2 has read it -----------------------------
                 stamp(13);
                 mbar_wait_a(bar(DONE_C5A_0 + rh), par);
                 stamp(14);
@@ -695,7 +703,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     acc_ld8(tm, lane_base + T_ZB + (uint32_t)c0, v);
                     load8_x3(sbase + OFF_H1, ACT_SUB, s_row, c0, hh);
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) dz[8 * ph + i] = v[i] * (1.f - hh[i] * hh[i]);
+                    for (int i = 0; i < 8; ++i) dz[8 * ph + i] = v[i] * af.d(hh[i]);
                 }
                 stamp(15);
                 mbar_wait_a(bar(DONE_C5B), par);
@@ -1032,6 +1040,25 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
 
 using namespace osb;
 
+// the instantiations of one activation (the DMU ones run one network: never ACT_MIXED)
+template <int ACT>
+static int x3_set_attr() {
+    static bool attr = false;
+    if (!attr) {
+        const size_t smem = 1024 + X3_SMEM;
+        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<false, x3_apv(8, ACT), false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<false, x3_apv(16, ACT), false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<true, x3_apv(8, ACT), false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<true, x3_apv(16, ACT), false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        if constexpr (ACT != ACT_MIXED) {
+            OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<false, x3_apv(8, ACT), true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<false, x3_apv(16, ACT), true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        }
+        attr = true;
+    }
+    return OSB_OK;
+}
+
 extern "C" {
 
 int osb_tc_grid_blocks(long long rows, int net_mask);
@@ -1040,21 +1067,6 @@ static long long* g_x3_dbg = nullptr;
 // development aid: clock64 stamps of one CTA of the next launches go to buf (3 * 4096 + 1 long long, the last the CTA
 // x | y << 16), NULL turns it off
 int osb_x3_debug_buffer(long long* buf) { g_x3_dbg = buf; return OSB_OK; }
-
-static int x3_set_attr() {
-    static bool attr = false;
-    if (!attr) {
-        const size_t smem = 1024 + X3_SMEM;
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<false, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<false, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<true, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<true, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<false, 8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        OSB_CUDA(cudaFuncSetAttribute(minibatch_grad_x3_kernel<false, 16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = true;
-    }
-    return OSB_OK;
-}
 
 // accumulator images for a grid of nb x (up to) 3 CTAs
 static int x3_bind_acc(X3Args& p, int nb) {
@@ -1085,23 +1097,32 @@ int osb_minibatch_grad_x3(const float* theta, int O, int A, const float* obs, co
     p.O = O; p.A = A; p.P = actor_layout(O, A).size + 2 * critic_layout(O, A).size; p.net_mask = net_mask;
     p.batch_size = mb_count; p.world = 1; p.dbg = g_x3_dbg;
     const int nb = osb_tc_grid_blocks(mb_count, net_mask);
-    int rc = x3_set_attr();
+    int rc = x3_bind_acc(p, nb);
     if (rc) return rc;
-    if ((rc = x3_bind_acc(p, nb))) return rc;
     const bool single = (net_mask & (net_mask - 1)) == 0;
+    p.spec = net_spec();
+    const NetSpec& spec = p.spec;
     if (loss_two_pass(loss_kind) && (net_mask & 1)) {   // pass 1: actor forward only
         X3Args q = p;
         q.forward_only = 1; q.net_mask = 1;
         const int nb1 = osb_tc_grid_blocks(mb_count, 1);
-        if (A <= 8) minibatch_grad_x3_kernel<false, 8><<<dim3(nb1, 1), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(q);
-        else minibatch_grad_x3_kernel<false, 16><<<dim3(nb1, 1), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(q);
-        OSB_LAUNCH_CHECK();
+        rc = with_act<false>(spec.act[0], [&](auto a) {
+            if (int r = x3_set_attr<a.value>()) return r;
+            if (A <= 8) minibatch_grad_x3_kernel<false, x3_apv(8, a.value), false><<<dim3(nb1, 1), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(q);
+            else minibatch_grad_x3_kernel<false, x3_apv(16, a.value), false><<<dim3(nb1, 1), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(q);
+            OSB_LAUNCH_CHECK();
+            return OSB_OK;
+        });
+        if (rc) return rc;
         if ((rc = pass1_gate(stats_part, nb1, stop_flag, p.lc, (cudaStream_t)stream))) return rc;
     }
-    if (A <= 8) minibatch_grad_x3_kernel<false, 8><<<dim3(nb, single ? 1 : 3), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(p);
-    else minibatch_grad_x3_kernel<false, 16><<<dim3(nb, single ? 1 : 3), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(p);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    return with_act<true>(launch_act(spec, net_mask), [&](auto a) {
+        if (int r = x3_set_attr<a.value>()) return r;
+        if (A <= 8) minibatch_grad_x3_kernel<false, x3_apv(8, a.value), false><<<dim3(nb, single ? 1 : 3), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(p);
+        else minibatch_grad_x3_kernel<false, x3_apv(16, a.value), false><<<dim3(nb, single ? 1 : 3), NTX3, 1024 + X3_SMEM, (cudaStream_t)stream>>>(p);
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    });
 }
 
 // One update iteration of PolicyGradient._update (policy_gradient.py:L369-381) as ONE persistent cooperative
@@ -1154,15 +1175,19 @@ int osb_ppo_update_iter_x3(float* theta, float* grad, float* adam_m, float* adam
     step_base += (unsigned int)n_mb;
     const int first = (int)(total < batch_size ? total : batch_size);
     const int nb = osb_tc_grid_blocks(first, net_mask);
-    int rc = x3_set_attr();
+    int rc = x3_bind_acc(p, nb);
     if (rc) return rc;
-    if ((rc = x3_bind_acc(p, nb))) return rc;
     const bool single = (net_mask & (net_mask - 1)) == 0;
+    p.spec = net_spec();
     void* args[] = {&p};
-    osb_count_launch();
-    OSB_CUDA(cudaLaunchCooperativeKernel(A <= 8 ? (void*)minibatch_grad_x3_kernel<true, 8> : (void*)minibatch_grad_x3_kernel<true, 16>,
-                                         dim3(nb, single ? 1 : 3), dim3(NTX3), args, 1024 + X3_SMEM, s));
-    return OSB_OK;
+    return with_act<true>(launch_act(p.spec, net_mask), [&](auto a) {
+        if (int r = x3_set_attr<a.value>()) return r;
+        osb_count_launch();
+        OSB_CUDA(cudaLaunchCooperativeKernel(A <= 8 ? (void*)minibatch_grad_x3_kernel<true, x3_apv(8, a.value), false>
+                                                    : (void*)minibatch_grad_x3_kernel<true, x3_apv(16, a.value), false>,
+                                             dim3(nb, single ? 1 : 3), dim3(NTX3), args, 1024 + X3_SMEM, s));
+        return OSB_OK;
+    });
 }
 
 }  // extern "C"
@@ -1171,13 +1196,17 @@ int osb_ppo_update_iter_x3(float* theta, float* grad, float* adam_m, float* adam
 static int launch_dmu_x3(X3Args& p, int nb, cudaStream_t stream) {
     p.lc.kind = LOSS_DMU; p.lc.focops_lam = 1.f;
     p.batch_size = p.b.mb_count; p.world = 1; p.dbg = nullptr;
-    int rc = x3_set_attr();
+    int rc = x3_bind_acc(p, nb);
     if (rc) return rc;
-    if ((rc = x3_bind_acc(p, nb))) return rc;
-    if (p.A <= 8) minibatch_grad_x3_kernel<false, 8, true><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
-    else minibatch_grad_x3_kernel<false, 16, true><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    p.spec = net_spec();
+    const NetSpec& spec = p.spec;
+    return with_act<false>(launch_act(spec, p.net_mask), [&](auto a) {
+        if (int r = x3_set_attr<a.value>()) return r;
+        if (p.A <= 8) minibatch_grad_x3_kernel<false, x3_apv(8, a.value), true><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
+        else minibatch_grad_x3_kernel<false, x3_apv(16, a.value), true><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    });
 }
 
 // LOSS_DMU launches behind osb_actor_dmu_backward and osb_critic_dv_backward (csrc/update.cu)
@@ -1202,13 +1231,17 @@ int osb::fvp_backward_x3(const float* theta_actor, const float* vec, int O, int 
     p.batch_size = (int)nrows; p.world = 1; p.dbg = nullptr;
     p.fvp_dmu = dmu; p.fvp_vec = vec; p.fvp_scale = 1.0f / ((float)nrows * (float)A);
     const int nb = osb_tc_grid_blocks(nrows, 1);
-    int rc = x3_set_attr();
+    int rc = x3_bind_acc(p, nb);
     if (rc) return rc;
-    if ((rc = x3_bind_acc(p, nb))) return rc;
-    if (A <= 8) minibatch_grad_x3_kernel<false, 8><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
-    else minibatch_grad_x3_kernel<false, 16><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
+    p.spec = net_spec();
+    const NetSpec& spec = p.spec;
+    return with_act<false>(spec.act[0], [&](auto a) {
+        if (int r = x3_set_attr<a.value>()) return r;
+        if (A <= 8) minibatch_grad_x3_kernel<false, x3_apv(8, a.value), false><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
+        else minibatch_grad_x3_kernel<false, x3_apv(16, a.value), false><<<dim3(nb, 1), NTX3, 1024 + X3_SMEM, stream>>>(p);
+        OSB_LAUNCH_CHECK();
+        return OSB_OK;
+    });
 }
 
 int osb::dv_backward_x3(const float* theta, int O, int A, int net, const float* obs, const float* dv, float* value, int rows,

@@ -465,6 +465,9 @@ __device__ __forceinline__ float tanh_acc(float x) {
     const float big = copysignf(fmaf(-2.0f, r, 1.0f), x);
     return ax < 1.0f ? small : big;
 }
+struct TanhAcc {
+    __device__ __forceinline__ float operator()(float x) const { return tanh_acc(x); }
+};
 
 }  // namespace x3
 }  // namespace osb

@@ -45,7 +45,7 @@ from omnisafe_b200.adapter.saute_adapter import per_step_budget
 from omnisafe_b200.common.normalizer import Normalizer
 from omnisafe_b200.envs.core import check_env, is_registered, make, needs_wrappers
 from omnisafe_b200.envs.synthetic import SyntheticBoxEnv, support_envs
-from omnisafe_b200.models.actor_critic import HID, ParamMap
+from omnisafe_b200.models.actor_critic import HID, ParamMap, activation_code, set_net_spec
 from omnisafe_b200.utils.config import Config
 
 PRECISIONS = {'fp32': 0, 'tf32': 1, 'bf16x3': 2}
@@ -97,6 +97,9 @@ class Evaluator:
         # the actor's flat parameters in the kernel layout, zero-padded to width 64 (the critics are not evaluated)
         actor_cfgs = getattr(getattr(cfgs, 'model_cfgs', None), 'actor', None)
         pmap = ParamMap(On, A, actor_hidden=getattr(actor_cfgs, 'hidden_sizes', [HID, HID]))
+        # the actor's hidden activation, as upstream's evaluator builds its actor from config.json (evaluator.py:L292-299)
+        self._actor_act = activation_code(getattr(actor_cfgs, 'activation', 'tanh'), 'actor')
+        self._actor_hidden = pmap.actor_hidden
         theta = torch.zeros(pmap.kernel['total'], dtype=torch.float32)
         pmap.load_state_dict(theta, 'actor', params['pi'], what="'pi'")
         self._theta = theta.to(self._device)
@@ -137,6 +140,7 @@ class Evaluator:
              'out_ret': f64(num_episodes), 'out_cost': f64(num_episodes), 'out_len': i32(num_episodes),
              'act_out': torch.zeros(E, self._act_dim, dtype=torch.float32, device=dev),
              'safety': torch.ones(2, E, dtype=torch.float32, device=dev) if self._saute else None}
+        set_net_spec(self._actor_act, 0, self._actor_hidden, (HID, HID))
         with torch.cuda.device(dev):
             if self._synthetic:
                 self._run_synthetic(E, num_episodes, float(cost_criteria), norm, w)

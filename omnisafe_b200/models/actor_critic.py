@@ -1,8 +1,9 @@
 """Flat-parameter ConstraintActorCritic (actor + reward critic + cost critic).
 
 Mirrors omnisafe/models/actor_critic/constraint_actor_critic.py:L31-109 and
-actor_critic.py:L60-113: three independent Linear-Tanh-Linear-Tanh-Linear trunks
-(utils/model.py:L73-111), GaussianLearningActor with a state-independent `log_std`
+actor_critic.py:L60-113: three independent Linear-Act-Linear-Act-Linear trunks
+(utils/model.py:L73-111; Act = model_cfgs.actor.activation for the actor, model_cfgs.critic.activation for both
+critics: identity, relu, sigmoid, softplus or tanh), GaussianLearningActor with a state-independent `log_std`
 (models/actor/gaussian_learning_actor.py:L29-62), one Adam optimiser per network and a LinearLR
 decay of the actor learning rate.  All parameters live in ONE flat fp32 device vector
 `theta = [actor | reward_critic | cost_critic]` in the reference's named_parameters() order
@@ -15,6 +16,10 @@ kernels share it.  `actor_state_dict()` re-exports the actor under the reference
 gradient and the Adam moments keep the 64-wide kernel layout; a narrower network sits in it zero-padded (ParamMap), which
 owns the one mapping between the reference's shapes and that layout: `named_views`, `actor_state_dict()`, the
 initialisation, the critic hooks, the evaluator and the golden fixtures all go through it.
+
+The kernels read the activations and the real widths from one process-wide spec (osb_set_net_spec).  Every launch for
+this model -- `step`, the actor and critic calls, the rollout, the update, the Fisher products and the critic hooks --
+is preceded by `apply_net_spec()`, so models with different specs can alternate in one process.
 
 The reference's model API on a trained policy -- `step` / `forward`, `actor.predict / forward / log_prob / std` and
 `reward_critic(obs)` / `cost_critic(obs)` -- runs on one batched launch of the policy-step kernel (csrc/policy.cu,
@@ -36,6 +41,8 @@ from omnisafe_b200._lib import lib, ptr
 from omnisafe_b200.utils.train_state import restore, snapshot
 
 HID = 64     # the hidden width every kernel computes
+# model_cfgs.*.activation (omnisafe/utils/model.py:L62-70); the index is the kernels' code (OSB_ACT_*)
+ACTIVATIONS = ('tanh', 'identity', 'relu', 'sigmoid', 'softplus')
 NET_ACTOR, NET_REWARD, NET_COST = 1, 2, 4   # net_mask bits of osb_policy_step
 NETS = ('actor', 'reward_critic', 'cost_critic')
 # model_cfgs.weight_initialization_mode -> the weight draw of utils/model.py:L25-44 (kaiming_uniform is drawn directly)
@@ -78,7 +85,8 @@ class ParamMap:
     [c1, c2] (both critics) live in the kernel layout.
 
     Every kernel computes 64-wide hidden layers.  A narrower network is the 64-wide one with its real weights in the
-    leading rows / columns of each padded matrix and zeros everywhere else: a padded unit has z = 0 and tanh(0) = 0, every
+    leading rows / columns of each padded matrix and zeros everywhere else: a padded unit has z = 0 and outputs +0 (tanh,
+    identity and relu map 0 to 0; for sigmoid and softplus the kernels output +0 past the layer's real width), every
     product touching a pad is +-0 in every precision, and every gradient at a pad is +-0, so Adam, clipping, the Fisher
     products and CG leave the pads at +0 and the padded network computes exactly the narrow one."""
 
@@ -131,14 +139,28 @@ class ParamMap:
             view.copy_(w)
 
 
+def activation_code(name, which: str) -> int:
+    """The kernel code of `model_cfgs.<which>.activation`; any other name fails as utils/model.py:L69 does."""
+    assert name in ACTIVATIONS, f'model_cfgs.{which}.activation must be one of {ACTIVATIONS}, got {name!r}'
+    return ACTIVATIONS.index(name)
+
+
+def set_net_spec(actor_act: int, critic_act: int, actor_hidden, critic_hidden) -> None:
+    """The activations and real hidden widths the following kernel launches compute with (osb_set_net_spec)."""
+    lib().osb_set_net_spec(int(actor_act), int(critic_act), *(int(h) for h in actor_hidden),
+                           *(int(h) for h in critic_hidden))
+
+
 class ConstraintActorCritic:
     NETS = NETS
 
     def __init__(self, obs_dim: int, act_dim: int, model_cfgs, epochs: int, device='cuda',
                  generator: torch.Generator | None = None) -> None:
         self.param_map = ParamMap(obs_dim, act_dim, model_cfgs.actor.hidden_sizes, model_cfgs.critic.hidden_sizes)
-        assert model_cfgs.actor.activation == 'tanh' and model_cfgs.critic.activation == 'tanh', (
-            'the fused kernels implement tanh activations')
+        self.activation = (model_cfgs.actor.activation, model_cfgs.critic.activation)
+        self.net_spec = (activation_code(model_cfgs.actor.activation, 'actor'),
+                         activation_code(model_cfgs.critic.activation, 'critic'),
+                         self.param_map.actor_hidden, self.param_map.critic_hidden)
         assert model_cfgs.actor_type == 'gaussian_learning'
         self.init_mode = model_cfgs.weight_initialization_mode
         if self.init_mode not in INIT_MODES:
@@ -182,6 +204,10 @@ class ConstraintActorCritic:
                 bb = 1.0 / math.sqrt(fan_in)
                 b.copy_(torch.empty(b.shape).uniform_(-bb, bb, generator=generator))
         self.theta.copy_(theta)
+
+    def apply_net_spec(self) -> None:
+        """Make this model's activations and widths the ones the next kernel launches use."""
+        set_net_spec(*self.net_spec)
 
     # -- views ------------------------------------------------------------------------------
     def net_slice(self, net: str) -> slice:
@@ -268,6 +294,7 @@ class ConstraintActorCritic:
             out['value_c'] = new(B)
         if B == 0:
             return out
+        self.apply_net_spec()
         with torch.cuda.device(self.device):
             lib().osb_policy_step(
                 ptr(self.theta), self.obs_dim, A, B, ptr(obs), ptr(eps), ptr(act_in), net_mask, int(self.precision),
