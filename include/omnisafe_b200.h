@@ -482,7 +482,8 @@ int osb_critic_dv_backward(const float* theta, int O, int A, int net, const floa
 /* ---- optimiser side --------------------------------------------------------------------------
  * osb_grad_reduce: grad <- sum of CTA partials (+ 2*critic_norm_coef*theta for critics,
  * policy_gradient.py:L431-433); advances adam_step[net]; accumulates train_stats[3][8]
- * ({sum of minibatch mean loss, mean ratio, mean kl, #minibatches}).  sumsq_part: 6*osb_optim_blocks.
+ * ({sum of minibatch mean loss, mean ratio, mean kl, #minibatches, actor: mean entropy bonus -entropy_coef * mean
+ * entropy (stats_part slot 5)}).  sumsq_part: 6*osb_optim_blocks.
  * osb_clip_adam: clip_grad_norm_ per network (do_clip) and torch.optim.Adam step (do_adam);
  * multi-rank order = clip -> all-reduce SUM -> grad_scale = 1/world -> Adam (policy_gradient.py:L437-443). */
 int osb_optim_blocks(int O, int A);

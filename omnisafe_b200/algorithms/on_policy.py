@@ -184,7 +184,8 @@ class PolicyGradient(BaseAlgo):
             'Train/Epoch': epoch, 'Train/Entropy': 0.5 + 0.5 * math.log(2 * math.pi) + logstd,
             'Train/KL': kl[0], 'Train/StopIter': kl[1], 'Train/PolicyRatio': ts[0][1] / n_mb[0],
             'Train/LR': self._actor_critic.actor_lr, 'Train/PolicyStd': std,
-            'TotalEnvSteps': (epoch + 1) * gsteps, 'Loss/Loss_pi': ts[0][0] / n_mb[0],
+            # Loss/Loss_pi after loss -= entropy_coef * entropy.mean() (base/ppo.py:L76-84): slot 4 holds the bonus
+            'TotalEnvSteps': (epoch + 1) * gsteps, 'Loss/Loss_pi': (ts[0][0] + ts[0][4]) / n_mb[0],
             'Loss/Loss_reward_critic': ts[1][0] / n_mb[1], 'Loss/Loss_cost_critic': ts[2][0] / n_mb[2],
             'Time/Total': now - start, 'Time/Rollout': roll - epoch_time, 'Time/Update': now - roll,
             'Time/Epoch': now - epoch_time, 'Time/FPS': gsteps / (now - epoch_time),

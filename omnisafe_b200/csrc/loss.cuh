@@ -126,7 +126,8 @@ __device__ __forceinline__ void stage_eval_policy(float* pol, int i, float log_s
 }
 
 // Actor loss of one sample.
-//   st = {loss, ratio, slot 2, count, slot 4}: the sample's statistics are added to it (slot 2: FOCOPS KL, P3O
+//   st = {loss, ratio, slot 2, count, slot 4}: the sample's statistics are added to it (slot 0: the loss without the
+//   entropy bonus, which entropy_bonus_sum adds to slot 5, and without the P3O penalty; slot 2: FOCOPS KL, P3O
 //   ratio * adv_c in pass 1 and the penalty term in pass 2; slot 4: FOCOPS mask 1{KL <= eta}).
 //   grad(a, dL/dmu_a, dL/dlog_std_a) receives the gradients of every action a < A, already divided by the minibatch
 //   size (inv_b).  The caller stores or accumulates them right there, in the same straight-line code as the products,
@@ -214,6 +215,19 @@ __device__ __forceinline__ void actor_sample_loss(const LossParams& lp, const Ad
             grad(a, dm, dl);
         }
     }
+}
+
+// Slot 5 of the actor's statistics: the entropy bonus -entropy_coef * mean entropy summed over the CTA's `count` samples
+// (Loss/Loss_pi is logged after loss -= entropy_coef * entropy.mean(), base/ppo.py:L76-84, first_order/focops.py:
+// L108-116).  Every sample's entropy is 0.5 + 0.5 log 2 pi + mean_a log sigma_a, so a CTA forms it once, where it adds
+// the bonus's gradient -entropy_coef / A to every log_std.  pol: the update layout of stage_policy's comment, still
+// holding the sigma of the minibatch.  Logging only.
+template <bool EXT = true>
+__device__ __forceinline__ float entropy_bonus_sum(const LossParams& lp, int A, const float* pol, float count) {
+    if (!loss_has_entropy<EXT>(lp.kind)) return 0.f;
+    float ls = 0.f;
+    for (int a = 0; a < A; ++a) ls += pol[a];
+    return -lp.entropy_coef * (1.4189385332046727f + ls / (float)A) * count;
 }
 
 // Full-batch evaluation of one sample, added to acc = {sum_a KL(old || new), ratio * adv, ratio * adv_c, ratio,

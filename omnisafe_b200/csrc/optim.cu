@@ -29,7 +29,7 @@ struct ReduceArgs {
     int net_mask;
     float* sumsq_part;        // [3][NB]
     int* adam_step;           // [3]
-    float* train_stats;       // [3][8] running sums over minibatch steps
+    float* train_stats;       // [3][8] running sums over minibatch steps: loss, ratio, kl, steps, entropy bonus (actor)
     const int* stop_flag;
 };
 
@@ -61,15 +61,16 @@ __global__ void __launch_bounds__(OT) grad_reduce_kernel(ReduceArgs p) {
         if (blockIdx.x == 0) {
             p.adam_step[net] += 1;
             // per-minibatch means of the loss statistics; the regulariser is added in clip_adam
-            float acc[4] = {0.f, 0.f, 0.f, 0.f};
+            float acc[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
             for (int b = 0; b < p.nblocks; ++b)
-                for (int i = 0; i < 4; ++i) acc[i] += p.stats_part[((size_t)b * 3 + net) * 8 + i];
+                for (int i = 0; i < 5; ++i) acc[i] += p.stats_part[((size_t)b * 3 + net) * 8 + (i < 4 ? i : 5)];
             const float inv = acc[3] > 0.f ? 1.f / acc[3] : 0.f;
             float* ts = p.train_stats + net * 8;
             ts[0] += acc[0] * inv;   // mean loss of this minibatch
             ts[1] += acc[1] * inv;   // mean ratio
             ts[2] += acc[2] * inv;   // mean kl (FOCOPS)
             ts[3] += 1.f;            // number of minibatch steps
+            ts[4] += acc[4] * inv;   // actor: mean entropy bonus (csrc/loss.cuh entropy_bonus_sum)
         }
     }
 }
@@ -171,12 +172,12 @@ __device__ __forceinline__ void clip_scale_and_stats(const FusedOptArgs& p, int 
                 *s_bc2 = (float)sqrt(bc2);
             }
         } else {
-            float acc[4] = {0.f, 0.f, 0.f, 0.f};
+            float acc[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
             for (int b = lane; b < p.r.nblocks; b += 32)
 #pragma unroll
-                for (int i = 0; i < 4; ++i) acc[i] += __ldcg(p.r.stats_part + ((size_t)b * 3 + net) * 8 + i);
+                for (int i = 0; i < 5; ++i) acc[i] += __ldcg(p.r.stats_part + ((size_t)b * 3 + net) * 8 + (i < 4 ? i : 5));
 #pragma unroll
-            for (int i = 0; i < 4; ++i) acc[i] = warp_sum(acc[i]);
+            for (int i = 0; i < 5; ++i) acc[i] = warp_sum(acc[i]);
             if (lane == 0) {
                 p.r.adam_step[net] = step_t;                   // every CTA read it before the grid barrier
                 const float inv = acc[3] > 0.f ? 1.f / acc[3] : 0.f;
@@ -185,6 +186,7 @@ __device__ __forceinline__ void clip_scale_and_stats(const FusedOptArgs& p, int 
                 ts[1] += acc[1] * inv;
                 ts[2] += acc[2] * inv;
                 ts[3] += 1.f;
+                ts[4] += acc[4] * inv;
             }
         }
     }

@@ -316,7 +316,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) minibatch_grad_kernel(GradArgs p,
             gout[L.off_logstd + threadIdx.x] = g;
         }
         if (threadIdx.x < ST_N)
-            p.stats_part[((size_t)blockIdx.x * 3 + net) * ST_N + threadIdx.x] = sStat[threadIdx.x];
+            p.stats_part[((size_t)blockIdx.x * 3 + net) * ST_N + threadIdx.x] =
+                (threadIdx.x == 5 && net == 0) ? entropy_bonus_sum(p.lc, A, sPol, sStat[3]) : sStat[threadIdx.x];
     }
 }
 

@@ -632,7 +632,9 @@ __global__ void __launch_bounds__(NTC, 1) minibatch_grad_tc_kernel(TcArgs p, Net
             if (is_fvp) g = (blockIdx.x == 0) ? 2.f / (float)A * __ldg(p.fvp_vec + L.off_logstd + tid) : 0.f;
             gout[L.off_logstd + tid] = g;
         }
-        if (tid < 8) p.stats_part[((size_t)blockIdx.x * 3 + net) * 8 + tid] = sStat[tid];
+        if (tid < 8)
+            p.stats_part[((size_t)blockIdx.x * 3 + net) * 8 + tid] =
+                (tid == 5 && net == 0) ? entropy_bonus_sum<EXT>(p.lc, A, sPol, sStat[3]) : sStat[tid];
     }
     __syncthreads();
 }

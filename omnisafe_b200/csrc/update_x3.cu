@@ -775,7 +775,9 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 }
                 if (tid >= 64 && tid < 72) {
                     const int i = tid - 64;
-                    __stcg(p.stats_part + ((size_t)blockIdx.x * 3 + net) * 8 + i, (i < 5) ? (sRed[i] + sRed[8 + i]) + (sRed[16 + i] + sRed[24 + i]) : 0.f);
+                    float s = (i < 5) ? (sRed[i] + sRed[8 + i]) + (sRed[16 + i] + sRed[24 + i]) : 0.f;
+                    if (i == 5 && net == 0) s = entropy_bonus_sum<!FUSED>(p.lc, A, sLs, (sRed[3] + sRed[11]) + (sRed[19] + sRed[27]));
+                    __stcg(p.stats_part + ((size_t)blockIdx.x * 3 + net) * 8 + i, s);
                 }
                 stamp(32);
                 mbar_wait_a(bar(DONE_C6), (uint32_t)((it - 1) & 1));
@@ -932,13 +934,13 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                     sScal[3] = t2;
                 }
             } else if (warp == 1 && blockIdx.x == 0) {               // loss statistics of this minibatch (logger means)
-                float acc[4] = {0.f, 0.f, 0.f, 0.f};
+                float acc[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
                 for (int b = lane; b < G; b += 32)
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) acc[i] += __ldcg(p.stats_part + ((size_t)b * 3 + net) * 8 + i);
+                    for (int i = 0; i < 5; ++i) acc[i] += __ldcg(p.stats_part + ((size_t)b * 3 + net) * 8 + (i < 4 ? i : 5));
 #pragma unroll
-                for (int i = 0; i < 4; ++i) acc[i] = warp_sum(acc[i]);
-                if (lane == 0) { sScal[4] = acc[0]; sScal[5] = acc[1]; sScal[6] = acc[2]; sScal[7] = acc[3]; }
+                for (int i = 0; i < 5; ++i) acc[i] = warp_sum(acc[i]);
+                if (lane == 0) { sScal[4] = acc[0]; sScal[5] = acc[1]; sScal[6] = acc[2]; sScal[7] = acc[3]; sScal[10] = acc[4]; }
             }
             epi_bar_sync();
             if (blockIdx.x == 0 && tid == 0) {
@@ -948,6 +950,7 @@ __global__ void __launch_bounds__(NTX3, 1) minibatch_grad_x3_kernel(X3Args p) {
                 ts[1] += sScal[5] * inv;
                 ts[2] += sScal[6] * inv;
                 ts[3] += 1.f;
+                ts[4] += sScal[10] * inv;
             }
             const float clipc = sScal[0];
             const unsigned int xstep = p.step_base + (unsigned int)mb;

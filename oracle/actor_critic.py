@@ -44,9 +44,10 @@ def unflatten(theta, O: int, A: int):
             for net in ('actor', 'reward_critic', 'cost_critic')}
 
 
-def init_theta(O: int, A: int, seed: int = 0) -> np.ndarray:
+def init_theta(O: int, A: int, seed: int = 0, log_std=None) -> np.ndarray:
     """Random init with the reference's scheme: kaiming_uniform_(a=sqrt(5)) weights and torch's
-    default Linear bias init (utils/model.py:L25-44), log_std = 0."""
+    default Linear bias init (utils/model.py:L25-44), log_std = 0 (the reference's initial value) or the
+    given [A] values (a policy whose std has been trained, e.g. trained_log_std(A))."""
     g = torch.Generator().manual_seed(seed)
     lay = layout(O, A)
     theta = torch.zeros(lay['total'])
@@ -59,7 +60,31 @@ def init_theta(O: int, A: int, seed: int = 0) -> np.ndarray:
             W.uniform_(-bound_w, bound_w, generator=g)
             bound_b = 1.0 / math.sqrt(fan_in)
             views[net][b].uniform_(-bound_b, bound_b, generator=g)
+    if log_std is not None:
+        views['actor']['log_std'].copy_(torch.as_tensor(np.asarray(log_std, np.float32)).reshape(A))
     return theta.numpy().copy()
+
+
+def trained_log_std(A: int, seed: int = 0) -> np.ndarray:
+    """log_std of a policy after training: distinct per action, spread evenly over [-1.6, 0.4] (sigma 0.20 to 1.49)
+    in a seeded order that is neither increasing nor decreasing; A = 1: -0.7.  At log_std = 0 sigma, sigma^2 and
+    1 / sigma^2 are all 1 and log sigma is 0, so a loss or Fisher product that confuses them looks right there."""
+    if A == 1:
+        return np.array([-0.7], np.float32)
+    vals = np.linspace(-1.6, 0.4, A)
+    rng = np.random.default_rng(seed)
+    while True:
+        order = rng.permutation(A)
+        steps = np.diff(order)
+        if A < 3 or ((steps > 0).any() and (steps < 0).any()):
+            return vals[order].astype(np.float32)
+
+
+def log_std_shift(A: int, seed: int = 0) -> np.ndarray:
+    """Per-action change of log_std between an old policy and the current one: magnitudes in [0.05, 0.3], seeded
+    signs, so the KL terms see sigma_old != sigma in every action."""
+    rng = np.random.default_rng(seed + 1)
+    return (rng.uniform(0.05, 0.3, A) * rng.choice([-1.0, 1.0], A)).astype(np.float32)
 
 
 def mlp(p, x):

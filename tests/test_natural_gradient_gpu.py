@@ -21,7 +21,7 @@ import torch
 from oracle import actor_critic as oac
 from oracle import fisher64 as f64
 from oracle import learner as ol
-from test_update_gpu import _rand_data, _rows, _setup
+from test_update_gpu import _rand_data, _rows, _setup, sigma_cases
 from test_update_x3_gpu import _oracle_grad
 
 pytestmark = pytest.mark.gpu
@@ -41,6 +41,10 @@ SHAPES = [
     (111, 8, 40, 30),      # obs dims > 64: K-chunked layer 1 (tf32); bf16x3 takes the fp32 tiles
     (376, 8, 64, 40),
 ]
+# at a trained log_std (oracle.actor_critic.trained_log_std): ragged last tile, A = 1, A > 8 with more tiles than CTAs,
+# obs dims > 64
+SHAPES_TRAINED = [(17, 6, 9, 31), (33, 1, 50, 11), (45, 9, 300, 70), (111, 8, 40, 30)]
+SHAPE_CASES = sigma_cases(SHAPES, SHAPES_TRAINED)
 PRECISIONS = [0, 1, 2]     # engine.precision: fp32 FMA tiles, tf32 wgmma tiles, split-bf16 wgmma tiles
 
 # fp32 and bf16x3: the bars test_update_gpu / test_update_x3_gpu apply to the same arithmetic; tf32: the bars of
@@ -67,29 +71,30 @@ def _standardised(data):
 
 
 @functools.lru_cache(maxsize=None)
-def _case(O, A, N, T):
-    """Env-major batch with raw advantages, the actor block of theta and a direction vector (float32)."""
+def _case(O, A, N, T, trained=False):
+    """Env-major batch with raw advantages, the actor block of theta and a direction vector (float32).  trained: the
+    actor's log_std is oracle.actor_critic.trained_log_std (sigma 0.2 to 1.5) instead of the initial 0."""
     rng = np.random.default_rng(1000 + 7 * O + N)
-    theta = oac.init_theta(O, A, seed=O + A)
+    theta = oac.init_theta(O, A, seed=O + A, log_std=oac.trained_log_std(A, O) if trained else None)
     data = _raw(_rand_data(rng, N, T, O, A, theta))
     Pa = oac.layout(O, A)['actor']['size']
     return theta, theta[:Pa].copy(), data, rng.standard_normal(Pa).astype(np.float32)
 
 
 @functools.lru_cache(maxsize=None)
-def _ref_fvp(O, A, N, T):
-    _, th, data, vec = _case(O, A, N, T)
+def _ref_fvp(O, A, N, T, trained=False):
+    _, th, data, vec = _case(O, A, N, T, trained)
     return f64.fvp64(th, vec, data['obs'], DAMPING)
 
 
 @functools.lru_cache(maxsize=None)
-def _ref_grad(O, A, N, T, kind):
-    _, th, data, _ = _case(O, A, N, T)
+def _ref_grad(O, A, N, T, kind, trained=False):
+    _, th, data, _ = _case(O, A, N, T, trained)
     return f64.surrogate_grad64(th, data, MOMENTS, LAM, kind)
 
 
-def _engine(cuda, O, A, N, T, precision):
-    theta, _, data, _ = _case(O, A, N, T)
+def _engine(cuda, O, A, N, T, precision, trained=False):
+    theta, _, data, _ = _case(O, A, N, T, trained)
     agent, buf, eng = _setup(cuda, data, N, T, O, A, theta)
     buf.adv_moments.copy_(torch.tensor(MOMENTS))
     eng.precision = precision
@@ -127,25 +132,25 @@ def _check_blocks(what, got, want, O, A, bar, per_block=True):
 
 @pytest.mark.timeout(300)
 @pytest.mark.parametrize('precision', PRECISIONS)
-@pytest.mark.parametrize('O,A,N,T', SHAPES)
-def test_fvp_vs_fp64(cuda, O, A, N, T, precision):
+@pytest.mark.parametrize('O,A,N,T,trained', SHAPE_CASES)
+def test_fvp_vs_fp64(cuda, O, A, N, T, trained, precision):
     """UpdateEngine.fvp (F v + damping v) vs the double-backward Hessian of the mean KL."""
-    agent, buf, eng, path = _engine(cuda, O, A, N, T, precision)
-    vec = torch.as_tensor(_case(O, A, N, T)[3]).to(cuda)
+    agent, buf, eng, path = _engine(cuda, O, A, N, T, precision, trained)
+    vec = torch.as_tensor(_case(O, A, N, T, trained)[3]).to(cuda)
     out = torch.zeros_like(vec)
     eng.fvp(vec, out, DAMPING)
     torch.cuda.synchronize()
     print(f'[{path}]')
-    _check_blocks('fvp', out.cpu().numpy(), _ref_fvp(O, A, N, T), O, A, BARS[path])
+    _check_blocks('fvp', out.cpu().numpy(), _ref_fvp(O, A, N, T, trained), O, A, BARS[path])
 
 
 @pytest.mark.timeout(300)
-@pytest.mark.parametrize('precision', PRECISIONS)
-def test_fvp_strided_vs_fp64(cuda, precision):
+@pytest.mark.parametrize('precision,trained', sigma_cases([(p,) for p in PRECISIONS], [(p,) for p in PRECISIONS]))
+def test_fvp_strided_vs_fp64(cuda, precision, trained):
     """fvp_sample_freq = 3: the FVP over slab rows 0, 3, 6, ..."""
     O, A, N, T = 64, 16, 100, 50
-    agent, buf, eng, path = _engine(cuda, O, A, N, T, precision)
-    _, th, _, vec = _case(O, A, N, T)
+    agent, buf, eng, path = _engine(cuda, O, A, N, T, precision, trained)
+    _, th, _, vec = _case(O, A, N, T, trained)
     out = torch.zeros(eng.Pa, device=cuda)
     eng.fvp(torch.as_tensor(vec).to(cuda), out, DAMPING, stride=3)
     torch.cuda.synchronize()
@@ -156,17 +161,17 @@ def test_fvp_strided_vs_fp64(cuda, precision):
 
 @pytest.mark.timeout(300)
 @pytest.mark.parametrize('precision', PRECISIONS)
-@pytest.mark.parametrize('O,A,N,T', SHAPES)
-def test_actor_loss_grad_vs_fp64(cuda, O, A, N, T, precision):
+@pytest.mark.parametrize('O,A,N,T,trained', SHAPE_CASES)
+def test_actor_loss_grad_vs_fp64(cuda, O, A, N, T, trained, precision):
     """UpdateEngine.actor_loss_grad: the full-batch ratio surrogate (Lagrangian mix) and cost surrogate, both signs,
     gradient and loss value, vs float64 autograd on the standardised advantages."""
-    agent, buf, eng, path = _engine(cuda, O, A, N, T, precision)
+    agent, buf, eng, path = _engine(cuda, O, A, N, T, precision, trained)
     bar = BARS[path]
     lag = torch.tensor([LAM], dtype=torch.float32, device=cuda)
     eng.snapshot_old_policy()
     print(f'[{path}]')
     for kind, name in ((LOSS_RATIO, 'ratio'), (LOSS_COST, 'cost')):
-        want, want_loss = _ref_grad(O, A, N, T, name)
+        want, want_loss = _ref_grad(O, A, N, T, name, trained)
         for sign in (-1.0, 1.0):
             g = torch.zeros(eng.Pa, device=cuda)
             loss = float(eng.actor_loss_grad(kind, lag, g, sign))
@@ -178,13 +183,14 @@ def test_actor_loss_grad_vs_fp64(cuda, O, A, N, T, precision):
 
 @pytest.mark.timeout(300)
 @pytest.mark.parametrize('precision', PRECISIONS)
-@pytest.mark.parametrize('O,A,N,T', SHAPES)
-def test_old_policy_and_evaluate_vs_fp64(cuda, O, A, N, T, precision):
+@pytest.mark.parametrize('O,A,N,T,trained', SHAPE_CASES)
+def test_old_policy_and_evaluate_vs_fp64(cuda, O, A, N, T, trained, precision):
     """snapshot_old_policy vs the float64 mean; evaluate of the unchanged actor (KL 0) and of theta + 0.02 v (KL,
-    surrogates, mean ratio); at the policy's own log-probs the unchanged actor has ratio 1."""
-    agent, buf, eng, path = _engine(cuda, O, A, N, T, precision)
+    surrogates, mean ratio); at the policy's own log-probs the unchanged actor has ratio 1.  At a trained log_std the
+    evaluated actor's log_std also moves by 0.05 to 0.3 per action (oracle.actor_critic.log_std_shift)."""
+    agent, buf, eng, path = _engine(cuda, O, A, N, T, precision, trained)
     bar = BARS[path]
-    _, th, data, vec = _case(O, A, N, T)
+    _, th, data, vec = _case(O, A, N, T, trained)
     lag = torch.tensor([LAM], dtype=torch.float32, device=cuda)
     eng.snapshot_old_policy()
     obs, act = _slab(buf, 'obs'), _slab(buf, 'act')
@@ -196,6 +202,8 @@ def test_old_policy_and_evaluate_vs_fp64(cuda, O, A, N, T, precision):
     ev0 = eng.evaluate(agent.theta, lag)
     assert abs(ev0['kl']) < 1e-9, ev0['kl']
     th2 = (th + np.float32(0.02) * vec).astype(np.float32)
+    if trained:
+        th2[:A] = th[:A] + oac.log_std_shift(A, O)
     theta2 = agent.theta.clone()
     theta2[: eng.Pa] = torch.as_tensor(th2).to(cuda)
     got = eng.evaluate(theta2, lag)
@@ -216,12 +224,12 @@ def _fvp_ref(th, obs):
 
 @pytest.mark.timeout(300)
 @pytest.mark.parametrize('precision', [0, 2])
-@pytest.mark.parametrize('O,A,N,T', [(12, 3, 8, 24), (60, 8, 512, 80)])
-def test_conjugate_gradients_vs_fp64(cuda, O, A, N, T, precision):
+@pytest.mark.parametrize('O,A,N,T,trained', sigma_cases([(12, 3, 8, 24), (60, 8, 512, 80)], [(12, 3, 8, 24), (60, 8, 512, 80)]))
+def test_conjugate_gradients_vs_fp64(cuda, O, A, N, T, trained, precision):
     """conjugate_gradients(b, 15, damping 0.1) on b = -grad of the reward surrogate vs the float64 CG on fvp64."""
-    agent, buf, eng, path = _engine(cuda, O, A, N, T, precision)
-    _, th, data, _ = _case(O, A, N, T)
-    b = (-_ref_grad(O, A, N, T, 'ratio')[0]).astype(np.float32)
+    agent, buf, eng, path = _engine(cuda, O, A, N, T, precision, trained)
+    _, th, data, _ = _case(O, A, N, T, trained)
+    b = (-_ref_grad(O, A, N, T, 'ratio', trained)[0]).astype(np.float32)
     x = eng.conjugate_gradients(torch.as_tensor(b).to(cuda), 15, DAMPING)
     torch.cuda.synchronize()
     want, steps, _ = f64.cg64(_fvp_ref(th, data['obs']), b, 15)
@@ -379,8 +387,10 @@ def test_minibatch_grad_moments_vs_autograd(cuda, fn, loss_kind):
             scale = np.abs(want[s:s + n]).max()
             np.testing.assert_allclose(got[s:s + n], want[s:s + n], rtol=2e-4, atol=2e-5 * max(scale, 1e-3), err_msg=net)
     print(f'{fn} kind {loss_kind}: worst block l2-rel {worst:.2e}, loss {ts[0, 0]:.6f}')
+    # slot 0 without the entropy bonus, slot 4 the bonus (at log_std = 0)
     ent = 0.01 * (0.5 + 0.5 * np.log(2 * np.pi)) if loss_kind == 0 else 0.0
     np.testing.assert_allclose(ts[0, 0], loss + ent, rtol=5e-3 if tc else 1e-3, atol=1e-4)
+    np.testing.assert_allclose(ts[0, 4], -ent, rtol=1e-5, atol=1e-7)
 
 
 @pytest.mark.timeout(300)

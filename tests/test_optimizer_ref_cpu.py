@@ -10,7 +10,7 @@ import pytest
 from oracle import actor_critic as oac
 from oracle import learner as ol
 from oracle import optim64 as o64
-from test_update_gpu import _rand_data
+from test_update_gpu import _rand_data, _theta, sigma_cases
 
 MOMENTS = [0.37, 2.3, -0.41, 1.0]
 LAM = 0.37
@@ -30,13 +30,14 @@ def _standardised(data):
     return out
 
 
-@pytest.mark.parametrize('regime', ['critics', 'all'])
-def test_ppo_epoch64_vs_learner(monkeypatch, regime):
+@pytest.mark.parametrize('regime,trained', sigma_cases([('critics',), ('all',)], [('critics',), ('all',)]))
+def test_ppo_epoch64_vs_learner(monkeypatch, regime, trained):
     """Learner.update_ppo (float32) on standardised advantages vs ppo_epoch64 on the raw ones: the same clip
-    decision for every network on every step, and parameters within fp32 rounding of the update."""
+    decision for every network on every step, parameters within fp32 rounding of the update, and the logged actor
+    loss (entropy bonus included) on every step."""
     rng = np.random.default_rng(5)
     N, T, O, A = 16, 24, 12, 3
-    theta = oac.init_theta(O, A, seed=3)
+    theta = _theta(O, A, 3, trained)
     data = _raw(_rand_data(rng, N, T, O, A, theta))
     if regime == 'critics':
         data['target_value_r'] = data['target_value_r'] * np.float32(50)
@@ -54,7 +55,7 @@ def test_ppo_epoch64_vs_learner(monkeypatch, regime):
 
     monkeypatch.setattr(ol, 'clip_grad_norm_', recording_clip)
     L = ol.Learner(theta, O, A, lr_actor=3e-3, lr_critic=1e-3)
-    L.update_ppo(_standardised(data), perms, LAM, **kw)
+    st = L.update_ppo(_standardised(data), perms, LAM, **kw)
     state, rec, passes = o64.ppo_epoch64(theta, data, MOMENTS, perms, LAM, net_mask=7, loss_kind=0,
                                          update_iters=2, lrs=(3e-3, 1e-3, 1e-3), **kw)
     assert passes == 2 and len(rec['steps']) == 2 * 4
@@ -75,6 +76,9 @@ def test_ppo_epoch64_vs_learner(monkeypatch, regime):
     assert np.linalg.norm(diff) < 1e-4 * np.linalg.norm(upd)
     np.testing.assert_allclose(state['theta'], L.flat(), rtol=1e-4, atol=1e-6)
     np.testing.assert_array_equal(state['step'], [8, 8, 8])
+    # the logged actor loss: slot 0 (without the bonus) - entropy_coef x the mean entropy
+    np.testing.assert_allclose([r['loss'][0] - kw['entropy_coef'] * r['entropy'] for r in rec['steps']], st['loss_pi'],
+                               rtol=1e-4, atol=1e-6)
 
 
 def test_ppo_epoch64_golden(golden_dir):

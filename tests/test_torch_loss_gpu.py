@@ -165,6 +165,34 @@ class _NpzView(dict):
 
 
 @pytest.mark.parametrize('prec', list(PREC))
+def test_logged_loss_pi_kernel_equals_torch_loss(cuda, tmp_path, golden_dir, monkeypatch, prec):
+    """Loss/Loss_pi of one PPOLag update at entropy_coef 0.01 and a trained log_std is the same on the kernel path and
+    through super()._loss_pi: the per-minibatch loss after loss -= entropy_coef * entropy.mean() (base/ppo.py:L76-84)."""
+    g = _NpzView(np.load(os.path.join(golden_dir, 'update_ppolag.npz')))
+    g.update(N=np.array(8), T=np.array(24), O=np.array(12), A=np.array(3))
+    theta0 = np.array(g['theta0'], np.float32)
+    theta0[:3] = oac.trained_log_std(3)
+    g['theta0'] = theta0
+    lag = {'cost_limit': float(g['cost_limit']), 'lagrangian_multiplier_init': float(g['lam0']),
+           'lambda_lr': float(g['lambda_lr'])}
+    logged = []
+    for tag, cls in (('kernel', None), ('torch', _subclass('PPOLag', '_loss_pi'))):
+        cfg = _golden_cfg(tmp_path / tag, g, prec, {'entropy_coef': 0.01}, lag)
+        algo = _agent(monkeypatch, tmp_path, 'PPOLag', cls, cfg).agent
+        assert bool(algo._torch_hooks) == (cls is not None)
+        perms = _load_golden_batch(algo, g, float(g['Jc']))
+        algo._update(perm=perms)
+        torch.cuda.synchronize()
+        if cls is None:
+            ts = algo._engine.train_stats.view(3, 8).tolist()
+            logged.append((ts[0][0] + ts[0][4]) / ts[0][3])      # as the epoch log forms Loss/Loss_pi
+        else:
+            logged.append(float(algo._loss_stats.means()['Loss/Loss_pi']))
+    print(f'[{prec}] Loss/Loss_pi kernel {logged[0]:.7f}, super()._loss_pi {logged[1]:.7f}')
+    np.testing.assert_allclose(logged[0], logged[1], rtol=5e-2 if prec == 'tf32' else 2e-3, atol=1e-5)
+
+
+@pytest.mark.parametrize('prec', list(PREC))
 @pytest.mark.parametrize('fname', ['update_trpolag.npz', 'update_cpo.npz', 'update_pcpo.npz'])
 def test_natural_golden_through_torch_loss(cuda, tmp_path, golden_dir, monkeypatch, fname, prec):
     g = np.load(os.path.join(golden_dir, fname))

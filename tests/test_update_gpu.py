@@ -47,6 +47,22 @@ def _rows(perm_env_major, N, T):
     return ((k % T) * N + (k // T)).astype(np.int32)
 
 
+def sigma_cases(unit, trained):
+    """Parameter sets of a test at the reference's initial log_std = 0 (`unit`, under their usual ids) and at a trained
+    log_std (`trained`, oracle.actor_critic.trained_log_std; ids end in '-trained'): the last argument is the flag."""
+    return ([pytest.param(*c, False, id='-'.join(map(str, c))) for c in unit]
+            + [pytest.param(*c, True, id='-'.join(map(str, c)) + '-trained') for c in trained])
+
+
+def entropy_mean(log_std):
+    """Mean entropy of the Gaussian policy over samples and action dims: 0.5 + 0.5 log 2 pi + mean_a log sigma_a."""
+    return 0.5 + 0.5 * np.log(2 * np.pi) + float(np.mean(np.asarray(log_std, np.float64)))
+
+
+def _theta(O, A, seed, trained):
+    return oac.init_theta(O, A, seed=seed, log_std=oac.trained_log_std(A, seed) if trained else None)
+
+
 def _rand_data(rng, N, T, O, A, theta):
     B = N * T
     obs = rng.standard_normal((B, O)).astype(np.float32)
@@ -59,13 +75,15 @@ def _rand_data(rng, N, T, O, A, theta):
             'target_value_c': rng.standard_normal(B).astype(np.float32)}
 
 
-@pytest.mark.parametrize('O,A,N,T,loss_kind', [(60, 8, 20, 13, 0), (60, 8, 32, 8, 1), (17, 6, 9, 31, 3),
-                                               (111, 8, 16, 10, 0), (376, 8, 7, 20, 0)])
-def test_minibatch_grad_vs_autograd(cuda, O, A, N, T, loss_kind):
+@pytest.mark.parametrize('O,A,N,T,loss_kind,trained', sigma_cases(
+    [(60, 8, 20, 13, 0), (60, 8, 32, 8, 1), (17, 6, 9, 31, 3), (111, 8, 16, 10, 0), (376, 8, 7, 20, 0)],
+    # ragged last tile, A = 1, A = 16 with more tiles than CTAs, obs dims > 64; every single-pass kind
+    [(60, 8, 20, 13, 0), (17, 6, 9, 31, 3), (33, 1, 50, 11, 0), (64, 16, 300, 70, 1), (111, 8, 16, 10, 1)]))
+def test_minibatch_grad_vs_autograd(cuda, O, A, N, T, loss_kind, trained):
     from omnisafe_b200._lib import current_stream, lib, ptr
 
     rng = np.random.default_rng(O + N)
-    theta = oac.init_theta(O, A, seed=5)
+    theta = _theta(O, A, 5, trained)
     data = _rand_data(rng, N, T, O, A, theta)
     agent, buf, eng = _setup(cuda, data, N, T, O, A, theta)
     B = N * T
@@ -109,9 +127,18 @@ def test_minibatch_grad_vs_autograd(cuda, O, A, N, T, loss_kind):
         s, n = lay[net]['start'], lay[net]['size']
         scale = np.abs(want[s:s + n]).max()
         np.testing.assert_allclose(got[s:s + n], want[s:s + n], rtol=2e-4, atol=2e-5 * max(scale, 1e-3), err_msg=net)
+    # the log_std block on its own (A entries next to ~10^4 weights in the actor's bar)
+    rel = float(np.linalg.norm(got[:A] - want[:A]) / np.linalg.norm(want[:A]))
+    print(f'actor.log_std: l2-rel {rel:.2e}')
+    assert rel < 1e-4, rel
+    np.testing.assert_allclose(got[:A], want[:A], rtol=2e-4, atol=2e-5 * np.abs(want[:A]).max(), err_msg='log_std')
+    # slot 0: the loss without the entropy bonus; slot 4: the bonus; Loss/Loss_pi = slot 0 + slot 4 is the oracle loss,
+    # bonus included (base/ppo.py:L76-84)
     ts = eng.train_stats.cpu().numpy().reshape(3, 8)
-    np.testing.assert_allclose(ts[0, 0], float(loss) + (0.01 * (0.5 + 0.5 * np.log(2 * np.pi)) if loss_kind == 0 else 0.0),
-                               rtol=1e-3, atol=1e-4)
+    bonus = -0.01 * entropy_mean(theta[:A]) if loss_kind == 0 else 0.0
+    np.testing.assert_allclose(ts[0, 0], float(loss) - bonus, rtol=1e-3, atol=1e-4)
+    np.testing.assert_allclose(ts[0, 4], bonus, rtol=1e-5, atol=1e-7)
+    np.testing.assert_allclose(ts[0, 0] + ts[0, 4], float(loss), rtol=1e-3, atol=1e-4)
 
 
 def test_ppolag_update_epoch_golden(cuda, golden_dir):

@@ -7,19 +7,22 @@ import torch
 
 from oracle import actor_critic as oac
 from oracle import learner as ol
-from test_update_gpu import _rand_data, _rows, _setup
+from test_update_gpu import _rand_data, _rows, _setup, _theta, sigma_cases
 
 pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.timeout(120)
-@pytest.mark.parametrize('O,A,N,T,loss_kind', [(60, 8, 20, 13, 0), (60, 8, 64, 40, 0), (17, 6, 9, 31, 3), (64, 16, 16, 24, 1), (60, 8, 512, 80, 0),
-                                                (111, 8, 40, 30, 1), (376, 8, 33, 12, 3), (128, 4, 300, 9, 1), (65, 8, 20, 7, 0)])   # obs dims > 64: K-chunked layer 1
-def test_tc_grad_vs_autograd(cuda, O, A, N, T, loss_kind):
+@pytest.mark.parametrize('O,A,N,T,loss_kind,trained', sigma_cases(
+    [(60, 8, 20, 13, 0), (60, 8, 64, 40, 0), (17, 6, 9, 31, 3), (64, 16, 16, 24, 1), (60, 8, 512, 80, 0),
+     (111, 8, 40, 30, 1), (376, 8, 33, 12, 3), (128, 4, 300, 9, 1), (65, 8, 20, 7, 0)],   # obs dims > 64: K-chunked layer 1
+    [(60, 8, 20, 13, 0), (17, 6, 9, 31, 3), (33, 1, 50, 11, 0), (64, 16, 16, 24, 1), (60, 8, 512, 80, 0),
+     (111, 8, 40, 30, 1), (376, 8, 33, 12, 3)]))
+def test_tc_grad_vs_autograd(cuda, O, A, N, T, loss_kind, trained):
     from omnisafe_b200._lib import current_stream, lib, ptr
 
     rng = np.random.default_rng(O + N)
-    theta = oac.init_theta(O, A, seed=5)
+    theta = _theta(O, A, 5, trained)
     data = _rand_data(rng, N, T, O, A, theta)
     agent, buf, eng = _setup(cuda, data, N, T, O, A, theta)
     B = N * T
@@ -69,7 +72,10 @@ def test_tc_grad_vs_autograd(cuda, O, A, N, T, loss_kind):
             rel = float(np.linalg.norm(g - w) / (np.linalg.norm(w) + 1e-30))
             print(f'{net}.{name}: max-err/scale {err:.2e}  l2-rel {rel:.2e}  cos {cos:.6f}')
             tol = 2e-2 if (net == 'actor' and loss_kind == 0) else 5e-3   # PPO clip flips near the boundary
-            bad += (rel > tol) or (cos < 0.9999)
+            # at a trained log_std (sigma down to 0.2) the tf32 mean's error is amplified in (act - mu) / sigma^2: the
+            # PPO actor blocks measured l2-rel up to 1.7e-2 and cos down to 0.99986 on an H100, so cos > 0.9998 there
+            min_cos = 0.9998 if (trained and net == 'actor' and loss_kind == 0) else 0.9999
+            bad += (rel > tol) or (cos < min_cos)
     assert bad == 0
 
 

@@ -10,7 +10,7 @@ import torch
 
 from oracle import actor_critic as oac
 from oracle import learner as ol
-from test_update_gpu import _rand_data, _rows, _setup
+from test_update_gpu import _rand_data, _rows, _setup, _theta, entropy_mean, sigma_cases
 
 pytestmark = pytest.mark.gpu
 
@@ -35,16 +35,19 @@ def _oracle_grad(theta, O, A, data, idx, lam, loss_kind, coef):
 
 
 @pytest.mark.timeout(300)
-@pytest.mark.parametrize('O,A,N,T,loss_kind,count', [
+@pytest.mark.parametrize('O,A,N,T,loss_kind,count,trained', sigma_cases([
     (60, 8, 20, 13, 0, None), (60, 8, 64, 40, 0, None), (17, 6, 9, 31, 3, None), (64, 16, 16, 24, 1, None),
     (60, 8, 256, 80, 0, 16384),      # the bench minibatch: 16 384 rows, obs 60 / act 8
     (60, 8, 256, 80, 1, 16384), (33, 1, 50, 11, 3, None),
-])
-def test_x3_grad_vs_autograd(cuda, O, A, N, T, loss_kind, count):
+], [  # ragged last tile, A = 1, A = 16, more tiles than CTAs (165 tiles of 128 rows); every single-pass kind
+    (60, 8, 20, 13, 0, None), (17, 6, 9, 31, 3, None), (33, 1, 50, 11, 0, None), (64, 16, 16, 24, 1, None),
+    (60, 8, 300, 70, 1, None),
+]))
+def test_x3_grad_vs_autograd(cuda, O, A, N, T, loss_kind, count, trained):
     from omnisafe_b200._lib import current_stream, lib, ptr
 
     rng = np.random.default_rng(O + N)
-    theta = oac.init_theta(O, A, seed=5)
+    theta = _theta(O, A, 5, trained)
     data = _rand_data(rng, N, T, O, A, theta)
     agent, buf, eng = _setup(cuda, data, N, T, O, A, theta)
     B = N * T
@@ -79,8 +82,12 @@ def test_x3_grad_vs_autograd(cuda, O, A, N, T, loss_kind, count):
             print(f'{net}.{name}: l2-rel {rel:.2e}')
             assert rel < 1e-4, (net, name, rel)
         np.testing.assert_allclose(got[s:s + n], want[s:s + n], rtol=2e-4, atol=2e-5 * max(scale, 1e-3), err_msg=net)
-    np.testing.assert_allclose(ts[0, 0], loss + (0.01 * (0.5 + 0.5 * np.log(2 * np.pi)) if loss_kind == 0 else 0.0),
-                               rtol=1e-3, atol=1e-4)
+    # slot 0: the loss without the entropy bonus; slot 4: the bonus; Loss/Loss_pi = slot 0 + slot 4 is the oracle loss,
+    # bonus included (base/ppo.py:L76-84)
+    bonus = -0.01 * entropy_mean(theta[:A]) if loss_kind == 0 else 0.0
+    np.testing.assert_allclose(ts[0, 0], loss - bonus, rtol=1e-3, atol=1e-4)
+    np.testing.assert_allclose(ts[0, 4], bonus, rtol=1e-5, atol=1e-7)
+    np.testing.assert_allclose(ts[0, 0] + ts[0, 4], loss, rtol=1e-3, atol=1e-4)
 
 
 @pytest.mark.timeout(300)
@@ -137,14 +144,19 @@ def test_x3_epoch_matches_fp32_epoch(cuda):
 
 
 @pytest.mark.timeout(300)
-@pytest.mark.parametrize('N,T,batch,iters', [(64, 32, 512, 3), (50, 26, 512, 2), (13, 100, 640, 2), (256, 80, 16384, 1)])
-def test_x3_fused_iteration_equals_stepwise(cuda, N, T, batch, iters):
+@pytest.mark.parametrize('N,T,batch,iters,trained', sigma_cases(
+    [(64, 32, 512, 3), (50, 26, 512, 2), (13, 100, 640, 2), (256, 80, 16384, 1)],
+    [(50, 26, 512, 2), (100, 80, 4096, 2)]))   # slices > 512 parameters (staged with the weights) and <= 512
+def test_x3_fused_iteration_equals_stepwise(cuda, N, T, batch, iters, trained):
     """The persistent kernel (optimiser inside, software grid barriers, short last minibatch, CTAs without a tile)
     and the launch-per-minibatch path (bf16x3 gradient kernel + optim_fused) produce the same parameters.  Both
-    paths share the clip formula, so this does not check the clip itself: test_optimizer_gpu does, against float64."""
+    paths share the clip formula, so this does not check the clip itself: test_optimizer_gpu does, against float64.
+    At a trained log_std the actor steps at lr 1e-2 with the entropy bonus on, so log_std moves ~1e-2 per minibatch
+    and the persistent kernel must stage the new sigma after every Adam step as the stepwise launches do."""
     rng = np.random.default_rng(N + T)
     O, A = 60, 8
-    theta = oac.init_theta(O, A, seed=2)
+    theta = _theta(O, A, 2, trained)
+    lr_actor, ent = (1e-2, 0.01) if trained else (3e-4, 0.0)
     data = _rand_data(rng, N, T, O, A, theta)
     B = N * T
     perms = torch.as_tensor(np.stack([_rows(rng.permutation(B), N, T) for _ in range(iters)])).to(cuda)
@@ -158,8 +170,8 @@ def test_x3_fused_iteration_equals_stepwise(cuda, N, T, batch, iters):
             agent, buf, eng = _setup(cuda, data, N, T, O, A, theta)
             lag = torch.tensor([0.2, 0, 0, 0], dtype=torch.float32, device=cuda)
             eng.ppo_epoch(loss_kind=0, lagrange=lag, net_mask=7, batch_size=batch, update_iters=iters, clip=0.2,
-                          critic_norm_coef=0.001, max_grad_norm=0.5, lr_actor=3e-4, lr_critic=3e-4,
-                          target_kl=10.0, kl_early_stop=False, perm=perms, precision=2)
+                          entropy_coef=ent, critic_norm_coef=0.001, max_grad_norm=0.5, lr_actor=lr_actor,
+                          lr_critic=3e-4, target_kl=10.0, kl_early_stop=False, perm=perms, precision=2)
             torch.cuda.synchronize()
         finally:
             os.environ.pop('OSB_X3_NO_FUSE', None)
