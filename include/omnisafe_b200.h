@@ -569,7 +569,6 @@ int osb_cg_init(const float* b, int n, float* x, float* r, float* p, float* cg_s
 int osb_cg_step(const float* z, int n, float* x, float* r, float* p, float* cg_scalars,
                 float residual_tol, float eps, void* stream);
 int osb_dot(const float* a, const float* b, int n, float* out, void* stream);
-int osb_axpy(const float* x, const float* y, float alpha, int n, float* out, void* stream);
 
 /* ---- epoch driver + NCCL -------------------------------------------------------------------
  * One epoch of PolicyGradient._update (policy_gradient.py:L345-405) issued from C: old-policy

@@ -33,7 +33,7 @@ def _digest() -> str:
             with open(os.path.join(CSRC, f), 'rb') as fh:
                 h.update(f.encode())
                 h.update(fh.read())
-    with open(os.path.join(HERE, '..', 'include', 'omnisafe_b200.h'), 'rb') as fh:   # optim.cu includes it
+    with open(os.path.join(HERE, '..', 'include', 'omnisafe_b200.h'), 'rb') as fh:   # every source includes it (csrc/common.cuh)
         h.update(fh.read())
     h.update(' '.join(FLAGS).encode())
     return h.hexdigest()

@@ -3,6 +3,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+// The C ABI: every extern "C" definition of the library is compiled against its declaration here, so a definition
+// whose parameters drift from the header (which the ctypes binding parses) fails to build.
+#include "../../include/omnisafe_b200.h"
 
 #define OSB_OK 0
 #define OSB_ERR_ARG 1

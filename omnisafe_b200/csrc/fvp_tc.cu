@@ -23,8 +23,6 @@
 #include "loss.cuh"
 #include "tc_forward.cuh"
 
-extern "C" int osb_tc_grid_blocks(long long rows, int net_mask);
-
 namespace osb {
 
 using namespace umma;

@@ -11,7 +11,7 @@
 //   conjugate_gradients                  utils/math.py:L86-132
 #include "common.cuh"
 #include "mlp.cuh"
-#include "../../include/omnisafe_b200.h"
+#include "optim.cuh"
 #include <cooperative_groups.h>
 #include <string.h>
 
@@ -110,23 +110,14 @@ __global__ void __launch_bounds__(OT) clip_adam_kernel(AdamArgs p) {
     if (p.do_clip && p.max_grad_norm > 0.f) {
         float tot = 0.f;
         for (int b = 0; b < p.NB; ++b) tot += p.sumsq_part[net * p.NB + b];
-        const float coef = fminf(p.max_grad_norm / (sqrtf(tot) + 1e-6f), 1.0f);
-        g *= coef;
+        g *= clip_coef(tot, p.max_grad_norm);
         p.grad[q] = g;
     }
     if (!p.do_adam) return;
     g *= p.grad_scale;
-    // torch.optim.Adam, single-tensor path (betas 0.9/0.999, eps 1e-8, no weight decay)
-    const int t = p.adam_step[net];
-    const double bc1 = 1.0 - pow(0.9, (double)t);
-    const double bc2 = 1.0 - pow(0.999, (double)t);
-    const float step_size = (float)((double)p.lr[net] / bc1);
-    const float bc2_sqrt = (float)sqrt(bc2);
+    const AdamScalars s = adam_scalars(p.lr[net], p.adam_step[net]);
     float m = p.m[q], v = p.v[q];
-    m = __fadd_rn(m, __fmul_rn(0.1f, __fadd_rn(g, -m)));                       // exp_avg.lerp_(grad, 1-b1)
-    v = __fadd_rn(__fmul_rn(v, 0.999f), __fmul_rn(__fmul_rn(0.001f, g), g));   // mul_(b2).addcmul_(g, g, 1-b2)
-    const float denom = __fadd_rn(__fdiv_rn(sqrtf(v), bc2_sqrt), 1e-8f);
-    p.theta[q] = __fadd_rn(p.theta[q], __fmul_rn(-step_size, __fdiv_rn(m, denom)));
+    p.theta[q] = adam_update(g, p.theta[q], m, v, s);
     p.m[q] = m; p.v[q] = v;
 }
 
@@ -166,10 +157,10 @@ __device__ __forceinline__ void clip_scale_and_stats(const FusedOptArgs& p, int 
         tot = warp_sum(tot); t2 = warp_sum(t2);
         if (warp == 0) {
             if (lane == 0) {
-                *s_scale = (p.max_grad_norm > 0.f) ? fminf(p.max_grad_norm / (sqrtf(tot) + 1e-6f), 1.0f) : 1.0f;
-                const double bc1 = 1.0 - pow(0.9, (double)step_t), bc2 = 1.0 - pow(0.999, (double)step_t);
-                *s_step = (float)((double)p.lr[net] / bc1);
-                *s_bc2 = (float)sqrt(bc2);
+                *s_scale = (p.max_grad_norm > 0.f) ? clip_coef(tot, p.max_grad_norm) : 1.0f;
+                const AdamScalars s = adam_scalars(p.lr[net], step_t);
+                *s_step = s.step_size;
+                *s_bc2 = s.bc2_sqrt;
             }
         } else {
             float acc[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
@@ -180,60 +171,67 @@ __device__ __forceinline__ void clip_scale_and_stats(const FusedOptArgs& p, int 
             for (int i = 0; i < 5; ++i) acc[i] = warp_sum(acc[i]);
             if (lane == 0) {
                 p.r.adam_step[net] = step_t;                   // every CTA read it before the grid barrier
-                const float inv = acc[3] > 0.f ? 1.f / acc[3] : 0.f;
-                float* ts = p.r.train_stats + net * 8;
-                ts[0] += acc[0] * inv + ((net != 0) ? p.r.critic_norm_coef * t2 : 0.f);
-                ts[1] += acc[1] * inv;
-                ts[2] += acc[2] * inv;
-                ts[3] += 1.f;
-                ts[4] += acc[4] * inv;
+                fold_minibatch_stats(p.r.train_stats, net, acc[0], acc[1], acc[2], acc[3], acc[4], p.r.critic_norm_coef, t2);
             }
         }
     }
 }
 
-__global__ void __launch_bounds__(OT) optim_fused_kernel(FusedOptArgs p) {
-    namespace cg = cooperative_groups;
-    if (p.r.stop_flag && *p.r.stop_flag) return;          // uniform across the grid
-    const int net = blockIdx.y;
-    const bool active = ((p.r.net_mask >> net) & 1) != 0;
+// What a thread of the fused optimiser kernels carries past the clip: parameter q (inside its network when in_net)
+// with the reduced gradient g (before clipping) and its value th before the step.
+struct FusedOptThread {
+    int q;
+    bool active, in_net;
+    float g, th;
+};
+
+// The phase the fused optimiser kernels share: the fixed-order partial reduction of one parameter per thread plus the
+// critic L2 gradient, the per-CTA squared norms of the gradient and of the critic parameters into sumsq_part, the grid
+// barrier, then the clip scale, the Adam step sizes and the loss statistics (clip_scale_and_stats) in shared memory.
+__device__ __forceinline__ FusedOptThread reduce_and_clip(const FusedOptArgs& p, float* s_scale, float* s_step,
+                                                          float* s_bc2) {
     __shared__ float red[OT / 32], red2[OT / 32];
-    __shared__ float s_scale, s_step, s_bc2;
-    const NetLayout L = net_layout(net, p.r.O, p.r.A);
-    const int noff = net_offset(net, p.r.O, p.r.A);
+    const int net = blockIdx.y;
     const int pl = blockIdx.x * OT + threadIdx.x;
-    const int q = noff + pl;
-    float g = 0.f, th = 0.f;
+    FusedOptThread t;
+    t.q = net_offset(net, p.r.O, p.r.A) + pl;
+    t.active = ((p.r.net_mask >> net) & 1) != 0;
+    t.in_net = pl < net_layout(net, p.r.O, p.r.A).size;
+    t.g = 0.f; t.th = 0.f;
     int step_t = 0;
-    if (active) {
+    if (t.active) {
         step_t = p.r.adam_step[net] + 1;                   // read before the grid barrier, bumped after it
-        if (pl < L.size) {
-            g = reduce_partials16(p.r.gpart, p.r.nblocks, p.r.P, q);
-            th = p.r.theta[q];
-            if (net != 0 && p.r.critic_norm_coef > 0.f) g += 2.f * p.r.critic_norm_coef * th;
+        if (t.in_net) {
+            t.g = reduce_partials16(p.r.gpart, p.r.nblocks, p.r.P, t.q);
+            t.th = p.r.theta[t.q];
+            if (net != 0 && p.r.critic_norm_coef > 0.f) t.g += 2.f * p.r.critic_norm_coef * t.th;
         }
-        float s = warp_sum(g * g), s2 = warp_sum(net != 0 ? th * th : 0.f);
+        float s = warp_sum(t.g * t.g), s2 = warp_sum(net != 0 ? t.th * t.th : 0.f);
         if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = s; red2[threadIdx.x >> 5] = s2; }
         __syncthreads();
         if (threadIdx.x == 0) {
-            float t = 0.f, t2 = 0.f;
-            for (int w = 0; w < OT / 32; ++w) { t += red[w]; t2 += red2[w]; }
-            p.r.sumsq_part[net * gridDim.x + blockIdx.x] = t;
-            p.r.sumsq_part[(3 + net) * gridDim.x + blockIdx.x] = t2;
+            float a = 0.f, a2 = 0.f;
+            for (int w = 0; w < OT / 32; ++w) { a += red[w]; a2 += red2[w]; }
+            p.r.sumsq_part[net * gridDim.x + blockIdx.x] = a;
+            p.r.sumsq_part[(3 + net) * gridDim.x + blockIdx.x] = a2;
         }
     }
-    cg::this_grid().sync();
-    if (active) clip_scale_and_stats(p, net, step_t, &s_scale, &s_step, &s_bc2);
+    cooperative_groups::this_grid().sync();
+    if (t.active) clip_scale_and_stats(p, net, step_t, s_scale, s_step, s_bc2);
     __syncthreads();
-    if (active && pl < L.size) {
-        g *= s_scale;
-        p.r.grad[q] = g;
-        float m = p.m[q], v = p.v[q];
-        m = __fadd_rn(m, __fmul_rn(0.1f, __fadd_rn(g, -m)));
-        v = __fadd_rn(__fmul_rn(v, 0.999f), __fmul_rn(__fmul_rn(0.001f, g), g));
-        const float denom = __fadd_rn(__fdiv_rn(sqrtf(v), s_bc2), 1e-8f);
-        p.r.theta[q] = __fadd_rn(th, __fmul_rn(-s_step, __fdiv_rn(m, denom)));
-        p.m[q] = m; p.v[q] = v;
+    return t;
+}
+
+__global__ void __launch_bounds__(OT) optim_fused_kernel(FusedOptArgs p) {
+    if (p.r.stop_flag && *p.r.stop_flag) return;          // uniform across the grid
+    __shared__ float s_scale, s_step, s_bc2;
+    const FusedOptThread t = reduce_and_clip(p, &s_scale, &s_step, &s_bc2);
+    if (t.active && t.in_net) {
+        const float g = t.g * s_scale;
+        p.r.grad[t.q] = g;
+        float m = p.m[t.q], v = p.v[t.q];
+        p.r.theta[t.q] = adam_update(g, t.th, m, v, {s_step, s_bc2});
+        p.m[t.q] = m; p.v[t.q] = v;
     }
 }
 
@@ -265,40 +263,12 @@ __global__ void __launch_bounds__(OT) optim_fused_p2p_kernel(P2POptArgs a) {
     namespace cg = cooperative_groups;
     const FusedOptArgs& p = a.f;
     if (p.r.stop_flag && *p.r.stop_flag) return;          // uniform across the grid and across ranks
-    const int net = blockIdx.y;
-    const bool active = ((p.r.net_mask >> net) & 1) != 0;
-    __shared__ float red[OT / 32], red2[OT / 32];
     __shared__ float s_scale, s_step, s_bc2;
-    const NetLayout L = net_layout(net, p.r.O, p.r.A);
-    const int noff = net_offset(net, p.r.O, p.r.A);
-    const int pl = blockIdx.x * OT + threadIdx.x;
-    const int q = noff + pl;
-    const int par = (int)(a.step_id & 1u);
-    float g = 0.f, th = 0.f;
-    int step_t = 0;
-    if (active) {
-        step_t = p.r.adam_step[net] + 1;
-        if (pl < L.size) {
-            g = reduce_partials16(p.r.gpart, p.r.nblocks, p.r.P, q);
-            th = p.r.theta[q];
-            if (net != 0 && p.r.critic_norm_coef > 0.f) g += 2.f * p.r.critic_norm_coef * th;
-        }
-        float s = warp_sum(g * g), s2 = warp_sum(net != 0 ? th * th : 0.f);
-        if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5] = s; red2[threadIdx.x >> 5] = s2; }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            float t = 0.f, t2 = 0.f;
-            for (int w = 0; w < OT / 32; ++w) { t += red[w]; t2 += red2[w]; }
-            p.r.sumsq_part[net * gridDim.x + blockIdx.x] = t;
-            p.r.sumsq_part[(3 + net) * gridDim.x + blockIdx.x] = t2;
-        }
-    }
-    cg::this_grid().sync();
-    if (active) clip_scale_and_stats(p, net, step_t, &s_scale, &s_step, &s_bc2);
-    __syncthreads();
+    const FusedOptThread t = reduce_and_clip(p, &s_scale, &s_step, &s_bc2);
     // ---- publish the clipped gradient, exchange flags over NVLink, sum the peers ---------------------
+    const int par = (int)(a.step_id & 1u);
     float* mine = a.peer_buf[a.rank] + (size_t)par * p.r.P;
-    if (pl < L.size) mine[q] = active ? g * s_scale : 0.f;
+    if (t.in_net) mine[t.q] = t.active ? t.g * s_scale : 0.f;
     __threadfence_system();
     cg::this_grid().sync();
     if (blockIdx.x == 0 && blockIdx.y == 0) {
@@ -316,22 +286,19 @@ __global__ void __launch_bounds__(OT) optim_fused_p2p_kernel(P2POptArgs a) {
     // a peer that never published (time-out above) leaves its buffer stale: skip the step instead of applying garbage --
     // the sticky error flag is raised by the host (distributed.p2p_check), the parameters stay those of the last good step
     const bool exchange_ok = *((volatile int*)a.error_flag) == 0;
-    if (active && pl < L.size && exchange_ok) {
+    if (t.active && t.in_net && exchange_ok) {
         float sum = 0.f;
         for (int r = 0; r < a.world; ++r) {
             const float* pb = a.peer_buf[r] + (size_t)par * p.r.P;
             float v;
-            asm volatile("ld.relaxed.sys.global.f32 %0, [%1];" : "=f"(v) : "l"(pb + q) : "memory");
+            asm volatile("ld.relaxed.sys.global.f32 %0, [%1];" : "=f"(v) : "l"(pb + t.q) : "memory");
             sum += v;
         }
         const float gavg = sum / (float)a.world;
-        p.r.grad[q] = gavg;
-        float m = p.m[q], v = p.v[q];
-        m = __fadd_rn(m, __fmul_rn(0.1f, __fadd_rn(gavg, -m)));
-        v = __fadd_rn(__fmul_rn(v, 0.999f), __fmul_rn(__fmul_rn(0.001f, gavg), gavg));
-        const float denom = __fadd_rn(__fdiv_rn(sqrtf(v), s_bc2), 1e-8f);
-        p.r.theta[q] = __fadd_rn(th, __fmul_rn(-s_step, __fdiv_rn(m, denom)));
-        p.m[q] = m; p.v[q] = v;
+        p.r.grad[t.q] = gavg;
+        float m = p.m[t.q], v = p.v[t.q];
+        p.r.theta[t.q] = adam_update(gavg, t.th, m, v, {s_step, s_bc2});
+        p.m[t.q] = m; p.v[t.q] = v;
     }
 }
 
@@ -347,11 +314,7 @@ __global__ void lagrange_update_kernel(const double* __restrict__ window_sums, f
     const float g = (float)(-(jc - (double)cost_limit));
     float lam = state[0], m = state[1], v = state[2];
     const int t = (int)state[3] + 1;
-    const double bc1 = 1.0 - pow(0.9, (double)t), bc2 = 1.0 - pow(0.999, (double)t);
-    m = __fadd_rn(m, __fmul_rn(0.1f, __fadd_rn(g, -m)));
-    v = __fadd_rn(__fmul_rn(v, 0.999f), __fmul_rn(__fmul_rn(0.001f, g), g));
-    const float denom = __fadd_rn(__fdiv_rn(sqrtf(v), (float)sqrt(bc2)), 1e-8f);
-    lam = __fadd_rn(lam, __fmul_rn(-(float)((double)lambda_lr / bc1), __fdiv_rn(m, denom)));
+    lam = adam_update(g, lam, m, v, adam_scalars(lambda_lr, t));
     lam = fmaxf(lam, 0.f);
     if (upper_bound >= 0.f) lam = fminf(lam, upper_bound);
     state[0] = lam; state[1] = m; state[2] = v; state[3] = (float)t;
@@ -613,13 +576,6 @@ __global__ void __launch_bounds__(1024) dot_kernel(const float* __restrict__ a, 
     if (threadIdx.x == 0) out[0] = (float)d;
 }
 
-// out = y + alpha * x
-__global__ void axpy_kernel(const float* __restrict__ x, const float* __restrict__ y, float alpha, int n,
-                            float* __restrict__ out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = y[i] + alpha * x[i];
-}
-
 }  // namespace osb
 
 using namespace osb;
@@ -808,13 +764,6 @@ int osb_cg_step(const float* z, int n, float* x, float* r, float* p, float* cg_s
 int osb_dot(const float* a, const float* b, int n, float* out, void* stream) {
     OSB_CHECK_ARG(a && b && out && n > 0, "bad argument");
     dot_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(a, b, n, out);
-    OSB_LAUNCH_CHECK();
-    return OSB_OK;
-}
-
-int osb_axpy(const float* x, const float* y, float alpha, int n, float* out, void* stream) {
-    OSB_CHECK_ARG(x && y && out && n > 0, "bad argument");
-    axpy_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(x, y, alpha, n, out);
     OSB_LAUNCH_CHECK();
     return OSB_OK;
 }

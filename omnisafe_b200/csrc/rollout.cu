@@ -1893,9 +1893,6 @@ static int launch_env_reset(const EnvSpec& es, const EnvState& st, const NormSta
 
 extern "C" {
 
-int osb_episode_window(const unsigned char* flags, const float* epfin, int T, int N, int W,
-                       float* ring, int* meta, double* window_sums, void* stream);
-
 // Opaque-struct-free C ABI: the caller passes plain device pointers.
 int osb_env_reset(int O, int A, int max_episode_steps, unsigned seed, unsigned term_threshold,
                   unsigned env_id_offset, float cost_threshold, int obs_normalize, int N,

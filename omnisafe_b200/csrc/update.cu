@@ -815,8 +815,6 @@ int osb_fvp_partials(const float* theta_actor, const float* vec, int O, int A, c
     });
 }
 
-int osb_tc_grid_blocks(long long rows, int net_mask);
-
 // Tiles of the supplied-dmu backward: bf16x3 (precision 2, O <= 64), tf32 (precision 1, O <= 512), else fp32 -- the
 // choice of UpdateEngine._eval_fn, so that the backward differentiates the forward that produced mu.
 static int dmu_tiles(int O, int precision) { return (precision == 2 && O <= 64) ? 2 : (precision == 1 && O <= 512) ? 1 : 0; }

@@ -678,8 +678,6 @@ static int launch_grad_tc(TcArgs& p, int nblocks, cudaStream_t stream) {
 
 extern "C" {
 
-int osb_update_grid_blocks(int mb_count);
-
 // CTAs along x of the tensor-core kernel: three networks share the SMs (a third each); a single
 // network (full-batch actor passes of the natural-gradient family) spreads over all of them.
 int osb_tc_grid_blocks(long long rows, int net_mask) {
