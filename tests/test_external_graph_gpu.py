@@ -12,6 +12,7 @@ import torch
 import external_envs as xe
 from oracle import actor_critic as oac
 from test_external_env_gpu import _cfgs, _check_golden, _custom, _model_cfgs
+from test_update_gpu import _theta, sigma_cases
 
 pytestmark = pytest.mark.gpu
 
@@ -197,12 +198,14 @@ def test_graph_wide_box_golden(cuda, monkeypatch, golden_dir, precision, tol):
     _check_golden(ad, buf, sl, g, tol)
 
 
-@pytest.mark.parametrize('parity', [False, True])
-@pytest.mark.parametrize('precision', [0, 2])
-def test_graph_equals_eager_bitwise(cuda, monkeypatch, precision, parity):
+BITWISE_CASES = [(p, parity) for p in (0, 2) for parity in (False, True)]
+
+
+@pytest.mark.parametrize('precision,parity,trained', sigma_cases(BITWISE_CASES, BITWISE_CASES))
+def test_graph_equals_eager_bitwise(cuda, monkeypatch, precision, parity, trained):
     """N = 256, O = 45, four epochs: every slab, epfin, the normaliser and the episode ring are the same bits."""
     N, T, O, A, E = 256, 16, 45, 3, 4
-    theta = oac.init_theta(O, A, seed=6)
+    theta = _theta(O, A, 6, trained)
     eps = np.random.default_rng(3).standard_normal((E, T, N, A)).astype(np.float32) if parity else None
     kw = dict(max_episode_steps=7)
     ad, _, graph = _run(monkeypatch, cuda, GRAPH_WIDE_ID, N, T, O, A, 5, theta, eps, precision, E, True, **kw)

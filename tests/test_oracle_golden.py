@@ -3,7 +3,9 @@ produced by the unmodified reference (tests/golden/make_golden.py)."""
 import os
 
 import numpy as np
+import pytest
 
+from oracle import actor_critic as oac
 from oracle import gae as ogae
 from oracle import rollout as orollout
 from oracle.normalizer import Normalizer
@@ -97,6 +99,68 @@ def test_rollout_golden(golden_dir):
     np.testing.assert_allclose(w[:, 0], g['win_ret'], rtol=1e-5, atol=1e-5)
     np.testing.assert_allclose(w[:, 1], g['win_cost'])
     np.testing.assert_allclose(w[:, 2], g['win_len'])
+
+
+def trained_golden(golden_dir, A):
+    """One action dimension of rollout_ppolag_trained.npz (tests/golden/make_golden_trained_std.py) as a dict."""
+    g = np.load(os.path.join(golden_dir, 'rollout_ppolag_trained.npz'))
+    return {k[len(f'A{A}_'):]: g[k] for k in g.files if k.startswith(f'A{A}_')}
+
+
+def _check_slabs(sl, g, tol):
+    t = dict(rtol=tol, atol=tol)
+    np.testing.assert_allclose(sl['obs'], g['slab_obs'], **t)
+    np.testing.assert_allclose(sl['act'], g['slab_act'], **t)
+    np.testing.assert_allclose(sl['rew'], g['slab_reward'], **t)
+    assert np.array_equal(sl['cost'], g['slab_cost'])
+    np.testing.assert_allclose(sl['val_r'], g['slab_value_r'], **t)
+    np.testing.assert_allclose(sl['val_c'], g['slab_value_c'], **t)
+    np.testing.assert_allclose(sl['logp'], g['slab_logp'], rtol=tol, atol=max(tol, 2e-5))
+
+
+@pytest.mark.parametrize('A', [3, 9])
+def test_rollout_golden_trained_std(golden_dir, A):
+    """Oracle rollout == the unmodified reference with the actor's log_std at trained_log_std(A): sigma differs per
+    action, so each action's sigma, 2 sigma^2 and log sigma reach the slabs."""
+    g = trained_golden(golden_dir, A)
+    N, T, O = int(g['N']), int(g['T']), int(g['O'])
+    assert int(g['A']) == A
+    theta = g['theta']
+    np.testing.assert_array_equal(theta[:A], oac.trained_log_std(A))
+    env = SyntheticBoxEnv(N, O, A, max_episode_steps=int(g['tmax']), seed=int(g['seed']), term_prob=float(g['term_prob']))
+    norm, window = Normalizer((O,)), []
+    sl = orollout.rollout_epoch(env, norm, theta, T, g['eps'], window=window)
+    _check_slabs(sl, g, 1e-5)
+    np.testing.assert_allclose(norm.mean, g['norm_mean'], rtol=1e-5, atol=1e-5)
+    assert norm.count == int(g['norm_count'])
+    w = np.array(window[-10:], np.float32)
+    np.testing.assert_allclose(w[:, 0], g['win_ret'], rtol=1e-5, atol=1e-5)
+    np.testing.assert_array_equal(w[:, 2], g['win_len'])
+    # the fixture's log-probabilities are those of the trained sigma, not of sigma = 1
+    eps = g['eps'].astype(np.float64)
+    logp = (-0.5 * eps * eps - theta[:A].astype(np.float64) - 0.5 * np.log(2 * np.pi)).sum(-1)
+    np.testing.assert_allclose(g['slab_logp'], logp, rtol=1e-5, atol=2e-5)
+
+
+def test_external_golden_trained_std(golden_dir, monkeypatch):
+    """Two epochs of the unmodified reference on the WideBox CMDP (asymmetric action box) at a trained log_std."""
+    import external_envs as xe
+
+    g = np.load(os.path.join(golden_dir, 'rollout_external_trained.npz'))
+    N, T, O, A, E = int(g['N']), int(g['T']), int(g['O']), int(g['A']), int(g['epochs_rolled'])
+    np.testing.assert_array_equal(g['theta'][:A], oac.trained_log_std(A))
+    scale = orollout.action_scale
+    monkeypatch.setattr(orollout, 'action_scale', lambda act: scale(act, g['act_lo'], g['act_hi']))
+    env, norm, window = xe.WideBoxOracle(N, O, A, int(g['tmax']), seed=int(g['seed'])), Normalizer((O,)), []
+    eps = g['eps'].reshape(E, T, N, A)
+    for e in range(E):
+        sl = orollout.rollout_epoch(env, norm, g['theta'], T, eps[e], window=window)
+    _check_slabs(sl, g, 2e-5)
+    np.testing.assert_allclose(norm.mean, g['norm_mean'], rtol=2e-5, atol=2e-5)
+    assert norm.count == int(g['norm_count'])
+    w = np.array(window[-10:], np.float32)
+    np.testing.assert_allclose(w[:, 0], g['win_ret'], rtol=2e-5, atol=2e-5)
+    np.testing.assert_array_equal(w[:, 2], g['win_len'])
 
 
 def test_rollout_reward_cost_normalize_golden(golden_dir):

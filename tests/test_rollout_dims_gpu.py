@@ -12,21 +12,27 @@ Fast mode (no `eps`) draws the noise in the kernels.  Each fast-mode case is run
 oracle/philox.py at the adapter's noise seed, env gid and global step epoch_index * T + t: both runs must give the same
 slabs within a few fp32 ulp (the accuracy of the kernels' logf / sincosf), so the kernels draw exactly the reference's
 normal for each (env, step, component), and a second epoch draws new ones.  On an H100 (700 W) the largest action
-deviation seen in fp32 and bf16x3 was 7.2e-7 (log_std = 0, so that is the normal's own deviation), 0.18 of FAST_TOL."""
+deviation seen in fp32 and bf16x3 was 7.2e-7 (log_std = 0, so that is the normal's own deviation), 0.18 of FAST_TOL.
+
+Cases whose id ends in '-trained' run the same checks with the actor's log_std at oracle.actor_critic.trained_log_std(A)
+(sigma 0.20 to 1.49, distinct per action), where a sigma taken from the wrong action or staged for some actions only no
+longer looks right."""
 from types import SimpleNamespace as NS
 
 import numpy as np
 import pytest
 import torch
 
+from itertools import product
+
 import external_envs as xe
-from oracle import actor_critic as oac
 from oracle import evaluator as eval_oracle
 from oracle import philox
 from oracle import rollout as orollout
 from oracle.normalizer import Normalizer as ONormalizer
 from oracle.synthetic_env import SyntheticBoxEnv as OEnv
 from test_rollout_gpu import _compare, _gpu_rollout, _model_cfgs
+from test_update_gpu import _theta, sigma_cases
 
 pytestmark = pytest.mark.gpu
 
@@ -106,14 +112,14 @@ def _oracle_epochs(N, T, O, A, theta, eps, tmax, term_prob, epochs=2, **kw):
 
 # ---- a. action-dimension sweep against the oracle --------------------------------------------------------------------
 
-@pytest.mark.parametrize('precision', [0, 1, 2])
-@pytest.mark.parametrize('A', A_SWEEP)
-def test_action_dims_vs_oracle(cuda, A, precision):
+@pytest.mark.parametrize('A,precision,trained', sigma_cases(list(product(A_SWEEP, [0, 1, 2])),
+                                                          list(product([1, 2, 3, 8, 9, 16], [0, 1, 2]))))
+def test_action_dims_vs_oracle(cuda, A, precision, trained):
     """Every A from 1 to 16 that takes a different lane layout, two epochs (normaliser, episode counters and window
     carry over), ragged env tiles, terminations and truncations; fp32 tiles and the persistent tensor-core kernel."""
     N = 129 if A % 2 else 50
     T, O, tmax, tp, W = 10, 60, 4, 0.05, 16
-    theta = oac.init_theta(O, A, seed=A)
+    theta = _theta(O, A, A, trained)
     eps = np.random.default_rng(100 + A).standard_normal((2, T, N, A)).astype(np.float32)
     ad, _, outs = _rollout(cuda, N, T, O, A, theta, eps, tmax, tp, precision, window=W)
     refs, window = _oracle_epochs(N, T, O, A, theta, eps, tmax, tp)
@@ -124,14 +130,14 @@ def test_action_dims_vs_oracle(cuda, A, precision):
 
 
 @pytest.mark.timeout(300)
-@pytest.mark.parametrize('precision', [1, 2])
-@pytest.mark.parametrize('A', [1, 9, 16])
-def test_action_dims_per_step_launch(cuda, A, precision):
+@pytest.mark.parametrize('A,precision,trained', sigma_cases(list(product([1, 9, 16], [1, 2])),
+                                                          [(1, 2), (9, 1), (9, 2), (16, 2)]))
+def test_action_dims_per_step_launch(cuda, A, precision, trained):
     """N = 6000 is more CTAs (47 tiles x 3 networks) than the H100 has SMs: the tensor-core tiles run one launch per
     step, where the step index and the noise pointer come from the host instead of the persistent loop."""
     N, T, O, tmax, tp, W = 6000, 5, 60, 3, 0.02, 64
     assert -(-N // RTC) * 3 > _sm_count(cuda)
-    theta = oac.init_theta(O, A, seed=20 + A)
+    theta = _theta(O, A, 20 + A, trained)
     eps = np.random.default_rng(200 + A).standard_normal((2, T, N, A)).astype(np.float32)
     ad, _, outs = _rollout(cuda, N, T, O, A, theta, eps, tmax, tp, precision, window=W)
     refs, window = _oracle_epochs(N, T, O, A, theta, eps, tmax, tp)
@@ -142,14 +148,14 @@ def test_action_dims_per_step_launch(cuda, A, precision):
 
 # ---- b. obs-dim boundaries ---------------------------------------------------------------------------------------------
 
-@pytest.mark.parametrize('precision', [0, 1, 2])
-@pytest.mark.parametrize('A', [2, 16])
-@pytest.mark.parametrize('O', [2, 63, 64, 65])
-def test_obs_dim_boundaries(cuda, O, A, precision):
+@pytest.mark.parametrize('O,A,precision,trained', sigma_cases(list(product([2, 63, 64, 65], [2, 16], [0, 1, 2])),
+                                                            list(product([63, 64, 65], [2, 16], [0, 2]))
+                                                            + [(64, 16, 1), (65, 16, 1)]))
+def test_obs_dim_boundaries(cuda, O, A, precision, trained):
     """O = 64 is the widest input of the tensor-core tiles (one K chunk), O = 65 the narrowest that falls back to the
     fp32 tiles; O = 2 leaves most of the chunk as padding."""
     N, T, tmax, tp, W = 50, 8, 5, 0.05, 16
-    theta = oac.init_theta(O, A, seed=O + A)
+    theta = _theta(O, A, O + A, trained)
     eps = np.random.default_rng(O * 31 + A).standard_normal((2, T, N, A)).astype(np.float32)
     ad, _, outs = _rollout(cuda, N, T, O, A, theta, eps, tmax, tp, precision, window=W)
     refs, window = _oracle_epochs(N, T, O, A, theta, eps, tmax, tp)
@@ -174,10 +180,11 @@ def _safety_adapter(dev, kind, N, O, A, tmax, tp):
     return cls('SyntheticBox-v0', N, SEED, cfgs, device=dev)
 
 
-@pytest.mark.parametrize('precision', [0, 2])
-@pytest.mark.parametrize('O', [63, 64])
-@pytest.mark.parametrize('kind', ['PPOSaute', 'PPOSimmerPID'])
-def test_safety_column_at_tile_boundary(cuda, kind, O, precision):
+SAFETY_CASES = list(product(['PPOSaute', 'PPOSimmerPID'], [63, 64], [0, 2]))
+
+
+@pytest.mark.parametrize('kind,O,precision,trained', sigma_cases(SAFETY_CASES, SAFETY_CASES))
+def test_safety_column_at_tile_boundary(cuda, kind, O, precision, trained):
     """The safety state z is the network's column O: with O = 63 the input is 64 wide and stays on the tensor-core
     tiles, with O = 64 it is 65 wide and takes the fp32 tiles.  Against the oracle's Saute / Simmer semantics."""
     from omnisafe_b200._lib import lib
@@ -187,7 +194,7 @@ def test_safety_column_at_tile_boundary(cuda, kind, O, precision):
     N, T, A, tmax, tp = 129, 12, 2, 6, 0.03
     ad = _safety_adapter(cuda, kind, N, O, A, tmax, tp)
     ad.precision = precision
-    theta = oac.init_theta(O + 1, A, seed=O)
+    theta = _theta(O + 1, A, O, trained)
     eps = np.random.default_rng(O).standard_normal((2, T, N, A)).astype(np.float32)
     agent = ConstraintActorCritic(O + 1, A, _model_cfgs(), epochs=1, device=cuda)
     agent.load_flat(theta)
@@ -210,15 +217,14 @@ def test_safety_column_at_tile_boundary(cuda, kind, O, precision):
     _check_window(ad, window, 16, precision)
 
 
-@pytest.mark.parametrize('precision', [0, 2])
-@pytest.mark.parametrize('A', [1, 16])
-def test_early_terminated_action_dims(cuda, A, precision):
+@pytest.mark.parametrize('A,precision,trained', sigma_cases(list(product([1, 16], [0, 2])), list(product([1, 16], [0, 2]))))
+def test_early_terminated_action_dims(cuda, A, precision, trained):
     """The EarlyTerminated cost rule reads action 0 of the sampled action in the kernel: A = 1 (a single component)
     and A = 16 (two components per lane)."""
     from test_saute_gpu import _early_rollout
 
     N, T, O, tmax, tp, limit = 256, 30, 17, 6, 0.03, 1.0
-    theta = oac.init_theta(O, A, seed=40 + A)
+    theta = _theta(O, A, 40 + A, trained)
     eps = np.random.default_rng(A).standard_normal((T, N, A)).astype(np.float32)
     ad, buf = _early_rollout(cuda, N, T, O, A, 3, theta, eps, tmax, tp, limit, precision)
     env = OEnv(N, O, A, max_episode_steps=tmax, seed=3, term_prob=tp)
@@ -261,14 +267,18 @@ def _assert_same_slabs(fast, parity, what, tf32=False):
             np.testing.assert_allclose(fast[0][k][0], parity[0][k][0], **FAST_TOL, err_msg=f'{what} step 0: {k}')
 
 
+FAST_SHAPES = [(0, 129), (1, 129), (2, 129), (1, 6000), (2, 6000)]
+
+
 @pytest.mark.timeout(300)
-@pytest.mark.parametrize('precision,N', [(0, 129), (1, 129), (2, 129), (1, 6000), (2, 6000)])
-@pytest.mark.parametrize('A', [1, 2, 3, 8, 9, 16])
-def test_fast_mode_noise_matches_oracle(cuda, A, precision, N):
+@pytest.mark.parametrize('A,precision,N,trained', sigma_cases(
+    [(A, *s) for A, s in product([1, 2, 3, 8, 9, 16], FAST_SHAPES)],
+    [(A, *s) for A, s in product([1, 3, 9, 16], [(0, 129), (1, 129), (2, 129), (2, 6000)])]))
+def test_fast_mode_noise_matches_oracle(cuda, A, precision, N, trained):
     """Fast mode against the same rollout fed oracle/philox.py's noise, two epochs, the fp32 tiles, the persistent
     tensor-core kernel (N = 129) and its per-step launch (N = 6000)."""
     T, O, tmax, tp = (8, 60, 5, 0.05) if N < 1000 else (5, 60, 3, 0.02)
-    theta = oac.init_theta(O, A, seed=60 + A)
+    theta = _theta(O, A, 60 + A, trained)
     ad, _, fast = _rollout(cuda, N, T, O, A, theta, None, tmax, tp, precision)
     eps = np.stack([philox.rollout_eps(ad.noise_seed, N, T, e, A) for e in range(2)])
     _, _, parity = _rollout(cuda, N, T, O, A, theta, eps, tmax, tp, precision)
@@ -290,16 +300,17 @@ def graph_envs():
     return GRAPH_WIDE_ID
 
 
-@pytest.mark.parametrize('precision', [0, 2])
-@pytest.mark.parametrize('graph', [False, True])
-@pytest.mark.parametrize('A', [3, 9])
-def test_fast_mode_noise_registered_env(cuda, monkeypatch, graph_envs, A, graph, precision):
+REGISTERED_CASES = list(product([3, 9], [False, True], [0, 2]))
+
+
+@pytest.mark.parametrize('A,graph,precision,trained', sigma_cases(REGISTERED_CASES, REGISTERED_CASES))
+def test_fast_mode_noise_registered_env(cuda, monkeypatch, graph_envs, A, graph, precision, trained):
     """The act kernel of the external-env path draws at act_global_step: the host's epoch_index * T + t when eager,
     the device epoch counter under graph replay (epoch 1 captures and replays, epoch 2 replays)."""
     from test_external_graph_gpu import _run
 
     N, T, O, E = 100, 8, 45, 3
-    theta = oac.init_theta(O, A, seed=80 + A)
+    theta = _theta(O, A, 80 + A, trained)
     ad, _, fast = _run(monkeypatch, cuda, graph_envs, N, T, O, A, 5, theta, None, precision, E, graph)
     eps = np.stack([philox.rollout_eps(ad.noise_seed, N, T, e, A) for e in range(E)])
     ad2, _, parity = _run(monkeypatch, cuda, graph_envs, N, T, O, A, 5, theta, eps, precision, E, graph)

@@ -13,8 +13,8 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import actor_critic as oac
 from test_rollout_gpu import _model_cfgs
+from test_update_gpu import _theta, sigma_cases
 
 pytestmark = pytest.mark.gpu
 
@@ -47,7 +47,7 @@ def _adapter(dev, kind, N, O, A):
                device=dev)
 
 
-def _epochs(dev, kind, N, O, A, precision, per_step, monkeypatch):
+def _epochs(dev, kind, N, O, A, precision, per_step, monkeypatch, trained=False):
     """Two rollout epochs; the state after each, and the number of launches they took."""
     from omnisafe_b200._lib import lib
     from omnisafe_b200.common.buffer import VectorOnPolicyBuffer
@@ -61,7 +61,7 @@ def _epochs(dev, kind, N, O, A, precision, per_step, monkeypatch):
     ad = _adapter(dev, kind, N, O, A)
     ad.precision = precision
     agent = ConstraintActorCritic(On, A, _model_cfgs(), epochs=1, device=dev)
-    agent.load_flat(oac.init_theta(On, A, seed=O + A))
+    agent.load_flat(_theta(On, A, O + A, trained))
     buf = VectorOnPolicyBuffer(On, A, T, 0.99, 0.95, 0.95, 'gae', 0.0, True, True, num_envs=N, device=dev)
     nz, env = ad._obs_normalizer, ad._env
     before = lib().osb_launch_count()
@@ -92,13 +92,16 @@ CASES = [   # kind, N, O, A
 ]
 
 
-@pytest.mark.parametrize('precision', [1, 2])
-@pytest.mark.parametrize('kind,N,O,A', CASES)
-def test_persistent_epoch_matches_per_step(cuda, monkeypatch, kind, N, O, A, precision):
+TRAINED = [c for c in CASES if c[1] in (4096, 100) or c[0] == 'PPOSaute']     # sigma per action pair, per lane, z
+
+
+@pytest.mark.parametrize('kind,N,O,A,precision,trained', sigma_cases([(*c, p) for c in CASES for p in (1, 2)],
+                                                                     [(*c, p) for c in TRAINED for p in (1, 2)]))
+def test_persistent_epoch_matches_per_step(cuda, monkeypatch, kind, N, O, A, precision, trained):
     if N == 'largest':
         N = _largest_n(cuda)
-    ref, launches_ref = _epochs(cuda, kind, N, O, A, precision, True, monkeypatch)
-    got, launches = _epochs(cuda, kind, N, O, A, precision, False, monkeypatch)
+    ref, launches_ref = _epochs(cuda, kind, N, O, A, precision, True, monkeypatch, trained)
+    got, launches = _epochs(cuda, kind, N, O, A, precision, False, monkeypatch, trained)
     assert launches_ref > 2 * (T + 1) and launches < 2 * (T + 1), (launches_ref, launches)
     for e in range(2):
         assert got[e].keys() == ref[e].keys()
