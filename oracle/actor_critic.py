@@ -7,13 +7,45 @@ and the flat parameter order of utils/tools.py:L35-129 (named_parameters order, 
 """
 from __future__ import annotations
 
+import contextlib
 import math
 
 import numpy as np
 import torch
+import torch.nn.functional as F
 from torch.distributions import Normal
 
 HID = 64
+# model_cfgs.*.activation (utils/model.py:L62-70); softplus with nn.Softplus's defaults (beta 1, threshold 20)
+ACT = {'tanh': torch.tanh, 'identity': lambda z: z, 'relu': torch.relu, 'sigmoid': torch.sigmoid, 'softplus': F.softplus}
+_DEFAULT = {'actor': ('tanh', (HID, HID)), 'critic': ('tanh', (HID, HID))}
+_spec = dict(_DEFAULT)
+
+
+@contextlib.contextmanager
+def nets(actor: str = 'tanh', critic: str = 'tanh', actor_hidden=(HID, HID), critic_hidden=(HID, HID)):
+    """Inside the block, `mlp` is the network of these activations and real hidden widths: the actor's when its
+    parameters hold 'log_std', both critics' otherwise.  Parameters keep the 64-wide layout; each layer computes its real
+    units only (the leading rows / columns of the padded tensors), so a sigmoid or softplus network is the narrow one and
+    not one whose pad units output sigmoid(0) or log 2, and autograd leaves exact zeros at the pads.  Leaving the block
+    restores the enclosing spec (tanh, 64 wide outside every block)."""
+    global _spec
+    for which, act, hs in (('actor', actor, actor_hidden), ('critic', critic, critic_hidden)):
+        assert act in ACT, (which, act)
+        assert len(hs) == 2 and all(1 <= int(h) <= HID for h in hs), (which, hs)
+    saved = _spec
+    _spec = {'actor': (actor, tuple(int(h) for h in actor_hidden)),
+             'critic': (critic, tuple(int(h) for h in critic_hidden))}
+    try:
+        yield
+    finally:
+        _spec = saved
+
+
+def net_spec(which: str):
+    """(activation function, (width 1, width 2)) of 'actor' or 'critic' under the current `nets` block."""
+    act, widths = _spec[which]
+    return ACT[act], widths
 
 
 def layout(O: int, A: int, hid: int = HID):
@@ -44,22 +76,24 @@ def unflatten(theta, O: int, A: int):
             for net in ('actor', 'reward_critic', 'cost_critic')}
 
 
-def init_theta(O: int, A: int, seed: int = 0, log_std=None) -> np.ndarray:
+def init_theta(O: int, A: int, seed: int = 0, log_std=None, actor_hidden=(HID, HID),
+               critic_hidden=(HID, HID)) -> np.ndarray:
     """Random init with the reference's scheme: kaiming_uniform_(a=sqrt(5)) weights and torch's
     default Linear bias init (utils/model.py:L25-44), log_std = 0 (the reference's initial value) or the
-    given [A] values (a policy whose std has been trained, e.g. trained_log_std(A))."""
+    given [A] values (a policy whose std has been trained, e.g. trained_log_std(A)).  Hidden widths below 64: only the
+    real block of each layer is drawn, with its real fan-in, and every pad stays +0."""
     g = torch.Generator().manual_seed(seed)
     lay = layout(O, A)
     theta = torch.zeros(lay['total'])
     views = unflatten(theta, O, A)
-    for net in ('actor', 'reward_critic', 'cost_critic'):
-        for w, b in (('w1', 'b1'), ('w2', 'b2'), ('w3', 'b3')):
-            W = views[net][w]
+    for net, (h1, h2) in (('actor', actor_hidden), ('reward_critic', critic_hidden), ('cost_critic', critic_hidden)):
+        for w, b, rows, cols in (('w1', 'b1', h1, O), ('w2', 'b2', h2, h1), ('w3', 'b3', None, h2)):
+            W, B = views[net][w][:rows, :cols], views[net][b][:rows]
             fan_in = W.shape[1]
             bound_w = math.sqrt(6.0 / ((1 + 5.0) * fan_in))
-            W.uniform_(-bound_w, bound_w, generator=g)
+            W.copy_(torch.empty(W.shape).uniform_(-bound_w, bound_w, generator=g))
             bound_b = 1.0 / math.sqrt(fan_in)
-            views[net][b].uniform_(-bound_b, bound_b, generator=g)
+            B.copy_(torch.empty(B.shape).uniform_(-bound_b, bound_b, generator=g))
     if log_std is not None:
         views['actor']['log_std'].copy_(torch.as_tensor(np.asarray(log_std, np.float32)).reshape(A))
     return theta.numpy().copy()
@@ -88,9 +122,12 @@ def log_std_shift(A: int, seed: int = 0) -> np.ndarray:
 
 
 def mlp(p, x):
-    h = torch.tanh(torch.nn.functional.linear(x, p['w1'], p['b1']))
-    h = torch.tanh(torch.nn.functional.linear(h, p['w2'], p['b2']))
-    return torch.nn.functional.linear(h, p['w3'], p['b3'])
+    """Linear-Act-Linear-Act-Linear of the actor ('log_std' in p) or a critic, with the activation and the real widths
+    of the current `nets` block (tanh, 64 wide outside one)."""
+    f, (a1, a2) = net_spec('actor' if 'log_std' in p else 'critic')
+    h = f(F.linear(x, p['w1'][:a1], p['b1'][:a1]))
+    h = f(F.linear(h, p['w2'][:a2, :a1], p['b2'][:a2]))
+    return F.linear(h, p['w3'][:, :a2], p['b3'])
 
 
 def actor_dist(p, obs) -> Normal:

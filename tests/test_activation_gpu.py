@@ -3,7 +3,6 @@
 - goldens of the unmodified reference (make_golden_activation.py; actor [24, 40], critic [8, 64], the 'softplus' case
   with relu critics): a rollout epoch, PPOLag._update, CPO's Fisher-vector product and CG, and CPO._update, at the bars
   of the tanh tests of the same widths (test_hidden_sizes_gpu.py); the rollout also in tf32 at its 5e-3;
-- one FOCOPS and one P3O minibatch gradient of every network against float64 autograd, per precision;
 - the full-batch actor evaluation (mu) of every precision against the reference actor's mean;
 - the policy step fed the rollout's rows gives the rollout's actions, values and log-probabilities bit for bit;
 - Evaluator on the synthetic env and on a registered env against the evaluation oracles, with the actor activation
@@ -58,8 +57,8 @@ def _golden(golden_dir, name, tag):
     return g, pmap, O, A, str(g['actor_activation']), str(g['critic_activation'])
 
 
-def _mlp(p, x, act, dtype=torch.float64):
-    """Linear-act-Linear-act-Linear of reference-named (or oracle-named) parameters."""
+def _mlp(p, x, act, dtype):
+    """Linear-act-Linear-act-Linear of reference-named parameters."""
     names = list(p)[-6:]
     h = torch.as_tensor(x, dtype=dtype)
     for layer in range(2):
@@ -238,81 +237,6 @@ def test_cpo_update_golden(cuda, tmp_path, golden_dir, tag, prec):
     bad = ~np.isclose(got, want, rtol=2e-3, atol=2e-5)
     assert bad.mean() < 1e-3 and np.abs(got - want).max() < 5e-3, (bad.sum(), np.abs(got - want).max())
     _assert_pads_zero(pmap, theta=ac.theta, adam_m=ac.adam_m, adam_v=ac.adam_v)
-
-
-# ---- FOCOPS and P3O against float64 autograd --------------------------------------------------------------------------
-@pytest.mark.parametrize('path', ['fp32', 'tf32', 'bf16x3'])
-@pytest.mark.parametrize('kind', ['focops', 'p3o'])
-@pytest.mark.parametrize('aa,ca', [('sigmoid', 'softplus'), ('relu', 'identity'), ('softplus', 'softplus')])
-def test_two_pass_minibatch_grad_vs_fp64(cuda, monkeypatch, aa, ca, kind, path):
-    """One FOCOPS (every sample inside the KL mask) or P3O (gate on) minibatch of every network against
-    oracle/optim64.py's float64 autograd with the activations substituted into oracle.actor_critic.mlp."""
-    from test_update_gpu import _rand_data, _rows
-
-    from oracle import actor_critic as oac
-    from oracle import optim64 as o64
-    from omnisafe_b200._lib import current_stream, lib, ptr
-    from omnisafe_b200.algorithms.engine import UpdateEngine
-    from omnisafe_b200.common.buffer import VectorOnPolicyBuffer
-    from omnisafe_b200.models import ConstraintActorCritic
-
-    monkeypatch.setattr(oac, 'mlp', lambda p, x: _mlp(p, x, aa if 'log_std' in p else ca, x.dtype))
-    O, A, N, T, start, count = 60, 8, 40, 25, 37, 900
-    rng = np.random.default_rng(17)
-    theta_old = oac.init_theta(O, A, seed=9)
-    data = _rand_data(rng, N, T, O, A, theta_old)
-    data['adv_r'] = (data['adv_r'] * np.float32(2.3) + np.float32(0.37)).astype(np.float32)
-    data['adv_c'] = (data['adv_c'] - np.float32(0.41)).astype(np.float32)
-    moments = [0.37, 2.3, -0.41, 1.0]
-    Pa = oac.layout(O, A)['actor']['size']
-    theta = theta_old.copy()
-    theta[:Pa] += (0.2 * np.abs(theta_old[:Pa]).mean() * rng.standard_normal(Pa)).astype(np.float32)
-    mu_old = _mlp(oac.unflatten(theta_old, O, A)['actor'], data['obs'], aa).numpy().astype(np.float32)
-    perm = rng.permutation(N * T)
-    idx = perm[start:start + count]
-    if kind == 'focops':
-        loss_kind, lam, lam_f, eta = 2, 0.37, 1.5, 1e6       # every sample inside the mask
-    else:
-        loss_kind, lam, lam_f, eta = 5, 0.0, 0.7, 1e6        # gate on: -surr + eta > 0
-    want, info = o64.minibatch64(theta, data, moments, idx, lam, loss_kind=loss_kind, old_mu=mu_old,
-                                 old_logstd=theta_old[:A], critic_norm_coef=0.01, clip=0.2, entropy_coef=0.01,
-                                 focops_lam=lam_f, focops_eta=eta)
-    agent = ConstraintActorCritic(O, A, _model_cfgs(aa, ca, (64, 64), (64, 64)), epochs=1, device=cuda)
-    agent.load_flat(theta)
-    buf = VectorOnPolicyBuffer(O, A, T, 0.99, 0.95, 0.95, 'gae', 0.0, True, True, num_envs=N, device=cuda)
-    for k in ('obs', 'act', 'logp', 'adv_r', 'adv_c', 'target_value_r', 'target_value_c'):
-        x = np.asarray(data[k], np.float32)
-        buf.data[k].copy_(torch.as_tensor(x.reshape(N, T, *x.shape[1:]).swapaxes(0, 1).copy()).to(cuda))
-    buf.adv_moments.copy_(torch.tensor(moments))
-    eng = UpdateEngine(agent, buf)
-    eng.mu_old.copy_(torch.as_tensor(mu_old.reshape(N, T, A).swapaxes(0, 1).copy()))
-    eng.logstd_old.copy_(torch.as_tensor(theta_old[:A]))
-    eng.train_stats.zero_()
-    fn = {'fp32': lib().osb_minibatch_grad, 'tf32': lib().osb_minibatch_grad_tc, 'bf16x3': lib().osb_minibatch_grad_x3}[path]
-    lag = torch.tensor([lam], dtype=torch.float32, device=cuda)
-    rows = torch.as_tensor(_rows(perm, N, T)).to(cuda)
-    d, s = buf.data, current_stream()
-    agent.apply_net_spec()
-    fn(ptr(agent.theta), O, A, ptr(d['obs']), ptr(d['act']), ptr(d['logp']), ptr(d['adv_r']), ptr(d['adv_c']),
-       ptr(d['target_value_r']), ptr(d['target_value_c']), ptr(eng.mu_old), ptr(buf.adv_moments), ptr(rows), N * T, 0,
-       start, count, loss_kind, 0.2, 0.01, lam_f, eta, ptr(lag), ptr(eng.logstd_old), 7, ptr(eng.gpart),
-       ptr(eng.stats_part), 0, s)
-    nb = lib().osb_update_grid_blocks(count) if path == 'fp32' else lib().osb_tc_grid_blocks(count, 7)
-    lib().osb_grad_reduce(ptr(eng.gpart), ptr(eng.stats_part), nb, O, A, ptr(agent.theta), ptr(agent.grad), 0.01, 7,
-                          ptr(eng.sumsq_part), ptr(agent.adam_step), ptr(eng.train_stats), 0, s)
-    torch.cuda.synchronize()
-    got = agent.grad.cpu().numpy().astype(np.float64)
-    lay = oac.layout(O, A)
-    for net in o64.NETS:
-        for name, (off, shape) in lay[net]['entries'].items():
-            n = int(np.prod(shape))
-            gg, w = got[off:off + n], want[off:off + n]
-            rel = float(np.linalg.norm(gg - w) / max(np.linalg.norm(w), 1e-30))
-            if path == 'tf32':       # PPO-clip decisions of a tf32 forward may differ from float64 near the boundary
-                cos = float((gg * w).sum() / (np.linalg.norm(gg) * np.linalg.norm(w)))
-                assert rel < 2e-2 and cos > 0.999, (net, name, rel, cos)
-            else:
-                assert rel < 1e-4, (net, name, rel)
 
 
 # ---- acting and evaluation --------------------------------------------------------------------------------------------

@@ -20,7 +20,7 @@ import torch
 
 from oracle import actor_critic as oac
 from oracle import optim64 as o64
-from test_update_gpu import _rand_data, _rows, _setup, _theta, sigma_cases
+from test_update_gpu import _default_spec_after, _rand_data, _rows, _setup, _theta, net_cases, oracle_nets, sigma_cases  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -254,10 +254,10 @@ REGIMES = {   # critic-target scale, max_grad_norm, critic_norm_coef; the norms 
 # 'small' regime has no L2 term, advantages of 1e-2 standard deviations and critic targets within ~0.1 of the values.
 
 
-def _regime_data(O, A, N, T, regime, seed, trained=False):
+def _regime_data(O, A, N, T, regime, seed, trained=False, nets=None):
     rng = np.random.default_rng(seed)
-    theta = _theta(O, A, seed % 7, trained)
-    data = _rand_data(rng, N, T, O, A, theta)
+    theta = _theta(O, A, seed % 7, trained, nets)
+    data = _rand_data(rng, N, T, O, A, theta, nets)
     data['adv_r'] = (data['adv_r'] * np.float32(MOMENTS[1]) + np.float32(MOMENTS[0])).astype(np.float32)
     data['adv_c'] = (data['adv_c'] + np.float32(MOMENTS[2])).astype(np.float32)
     scale = REGIMES[regime][0]
@@ -265,7 +265,8 @@ def _regime_data(O, A, N, T, regime, seed, trained=False):
         adv_r = (data['adv_r'] - np.float32(MOMENTS[0])) / np.float32(MOMENTS[1])
         data['adv_r'] = (np.float32(MOMENTS[0]) + np.float32(MOMENTS[1] * 1e-2) * adv_r).astype(np.float32)
         data['adv_c'] = (np.float32(MOMENTS[2]) + np.float32(1e-2) * (data['adv_c'] - np.float32(MOMENTS[2]))).astype(np.float32)
-        v_r, v_c = oac.values(theta, data['obs'], O, A)
+        with oracle_nets(nets):
+            v_r, v_c = oac.values(theta, data['obs'], O, A)
         data['target_value_r'] = (v_r + np.float32(0.1) * data['target_value_r']).astype(np.float32)
         data['target_value_c'] = (v_c + np.float32(0.1) * data['target_value_c']).astype(np.float32)
     else:
@@ -288,8 +289,8 @@ def _check_regime(rec, regime, mask):
             assert norms[0, j] < 0.03, (j, norms[0, j])
 
 
-def _engine_case(cuda, O, A, N, T, theta, data):
-    agent, buf, eng = _setup(cuda, data, N, T, O, A, theta)
+def _engine_case(cuda, O, A, N, T, theta, data, nets=None):
+    agent, buf, eng = _setup(cuda, data, N, T, O, A, theta, nets=nets)
     buf.adv_moments.copy_(torch.tensor(MOMENTS))
     eng.train_stats.zero_()
     return agent, buf, eng
@@ -389,29 +390,31 @@ def _compare_stats(path, eng, rec, mask, ent=None):
         np.testing.assert_allclose(ts[0, 4] / n, want, rtol=rtol, atol=1e-7, err_msg='entropy bonus')
 
 
-def _epoch_case(cuda, path, O, A, mask, loss_kind, regime, batch, seed, trained=False):
+def _epoch_case(cuda, path, O, A, mask, loss_kind, regime, batch, seed, trained=False, nets=None):
     """One minibatch step, then two passes over 3.5 minibatches (short last one), each from the same initial state,
-    on the device and in float64.  trained: a trained log_std, the actor at LRS_TRAINED and the entropy bonus on."""
+    on the device and in float64.  trained: a trained log_std, the actor at LRS_TRAINED and the entropy bonus on.
+    nets: a network spec of test_update_gpu.NETS (tanh 64 wide if None)."""
     rows = batch * 7 // 2
     T = 64 if rows % 64 == 0 else 32
     N = rows // T
-    theta, data, perms = _regime_data(O, A, N, T, regime, seed, trained)
+    theta, data, perms = _regime_data(O, A, N, T, regime, seed, trained, nets)
     _, max_norm, coef = REGIMES[regime]
     lrs, ent = (LRS_TRAINED, ENT_TRAINED) if trained else (LRS, 0.0)
     kw = dict(net_mask=mask, loss_kind=loss_kind, batch_size=batch, critic_norm_coef=coef, max_grad_norm=max_norm,
               lrs=lrs, clip=0.2, entropy_coef=ent)
-    one, rec1, _ = o64.ppo_epoch64(theta, data, MOMENTS, perms[:1, :batch], LAM, update_iters=1, **kw)
-    want, rec, passes = o64.ppo_epoch64(theta, data, MOMENTS, perms, LAM, update_iters=2, **kw)
+    with oracle_nets(nets):
+        one, rec1, _ = o64.ppo_epoch64(theta, data, MOMENTS, perms[:1, :batch], LAM, update_iters=1, **kw)
+        want, rec, passes = o64.ppo_epoch64(theta, data, MOMENTS, perms, LAM, update_iters=2, **kw)
     assert passes == 2 and len(rec['steps']) == 8
     _check_regime(rec, regime, mask)
     rows_dev = torch.as_tensor(np.stack([_rows(p, N, T) for p in perms])).to(cuda)
     run = dict(mask=mask, loss_kind=loss_kind, batch=batch, max_norm=max_norm, coef=coef, lrs=lrs, ent=ent)
-    agent, buf, eng = _engine_case(cuda, O, A, N, T, theta, data)
+    agent, buf, eng = _engine_case(cuda, O, A, N, T, theta, data, nets)
     _run_passes(path, agent, buf, eng, rows_dev[:1, :batch].contiguous(), **run)
     got1 = _host(agent)
     assert (got1['step'] == [(mask >> j) & 1 for j in range(3)]).all(), got1['step']
     w1 = _compare_step(path, got1, one, rec1['steps'][0], O, A, mask, max_norm)
-    agent, buf, eng = _engine_case(cuda, O, A, N, T, theta, data)
+    agent, buf, eng = _engine_case(cuda, O, A, N, T, theta, data, nets)
     _run_passes(path, agent, buf, eng, rows_dev, **run)
     got = _host(agent)
     np.testing.assert_array_equal(got['step'], want['step'])
@@ -449,11 +452,20 @@ X3_CASES += [
 # again after each Adam step drifts from ppo_epoch64's (every single-pass kind; A = 1 and A = 16; spec / nonspec / full)
 X3_TRAINED = [(60, 8, 7, 'spec', 'none', 0), (17, 6, 3, 'nonspec', 'all', 1), (33, 1, 7, 'spec', 'all', 3),
               (64, 16, 3, 'full', 'none', 0)]
+# test_update_gpu.NETS with every network clipping: A = 1 and A = 16 (the A > 8 kernel, whose template argument packs
+# the activation), all three networks (ACT_MIXED unless the activations agree), the actor alone and the critics alone,
+# speculative and non-speculative Adam
+X3_NETS = [(33, 1, 7, 'spec', 'all', 0, False, 'tanh-relu'), (64, 16, 7, 'nonspec', 'all', 1, False, 'sp-id'),
+           (60, 8, 7, 'spec', 'all', 1, False, 'sig-sp'),
+           (64, 16, 1, 'spec', 'all', 3, False, 'sig-sp'), (60, 8, 6, 'nonspec', 'all', 0, False, 'sig-1'),
+           (17, 6, 6, 'spec', 'all', 1, False, 'sp-id'), (64, 16, 7, 'spec', 'all', 0, True, 'tanh-relu'),
+           (33, 1, 1, 'nonspec', 'all', 3, False, 'sig-1'), (64, 16, 6, 'nonspec', 'all', 0, False, 'tanh-relu')]
 
 
 @pytest.mark.timeout(600)
-@pytest.mark.parametrize('O,A,mask,mode,regime,loss_kind,trained', sigma_cases(X3_CASES, X3_TRAINED))
-def test_persistent_x3_passes_vs_fp64(cuda, O, A, mask, mode, regime, loss_kind, trained):
+@pytest.mark.parametrize('O,A,mask,mode,regime,loss_kind,trained,nets', net_cases(sigma_cases(X3_CASES, X3_TRAINED),
+                                                                                  X3_NETS))
+def test_persistent_x3_passes_vs_fp64(cuda, O, A, mask, mode, regime, loss_kind, trained, nets):
     """The persistent bf16x3 kernel (optimiser inside): speculative Adam (slice <= 512 parameters), its redo when a
     network clips, and the non-speculative slices; W1 / b1 (ones column when O < 64) / W3 (A up to 16) written into
     the weight-tile image and read back by the next three minibatches; log_std and its sigma staged again after every
@@ -464,23 +476,31 @@ def test_persistent_x3_passes_vs_fp64(cuda, O, A, mask, mode, regime, loss_kind,
     G, S = _spec_slices(mask, batch, O, A)
     assert all((s <= NEPI) == (mode != 'nonspec') for s in S), (mode, G, S)
     assert mode != 'full' or G == cap, (G, cap)
-    w1, we = _epoch_case(cuda, 'x3_fused', O, A, mask, loss_kind, regime, batch, seed=O + 10 * A + mask, trained=trained)
+    w1, we = _epoch_case(cuda, 'x3_fused', O, A, mask, loss_kind, regime, batch, seed=O + 10 * A + mask, trained=trained,
+                         nets=nets)
     kind = f'{mode} redo' if mode != 'nonspec' and regime != 'none' else mode
-    print(f'[x3_fused {kind} O={O} A={A} mask={mask} {regime} kind {loss_kind} G={G} S={S}] one step worst block '
+    print(f'[x3_fused {kind} O={O} A={A} mask={mask} {regime} kind {loss_kind} G={G} S={S}{" " + nets if nets else ""}] '
+          f'one step worst block '
           f'l2 {w1:.2e}; epoch ' + ', '.join(f'{k} {v:.2e}' for k, v in we.items()))
 
 
 @pytest.mark.timeout(600)
-@pytest.mark.parametrize('path,O,A,regime,trained', sigma_cases(
+@pytest.mark.parametrize('path,O,A,regime,trained,nets', net_cases(sigma_cases(
     [(path, O, A, regime) for path in ('fp32', 'tf32', 'bf16x3') for O, A in ((60, 8), (17, 6))
      for regime in ('critics', 'all', 'none')],
     # tf32 only with every network clipped: unclipped at lr 1e-2 its trajectory leaves float64's within the two passes
     # (last-step actor gradient norm 1.82 vs 1.53 on an H100)
-    [('fp32', 60, 8, 'none'), ('bf16x3', 60, 8, 'none')] + [(path, 17, 6, 'all') for path in ('fp32', 'tf32', 'bf16x3')]))
-def test_stepwise_passes_vs_fp64(cuda, path, O, A, regime, trained):
+    [('fp32', 60, 8, 'none'), ('bf16x3', 60, 8, 'none')] + [(path, 17, 6, 'all') for path in ('fp32', 'tf32', 'bf16x3')]),
+    # test_update_gpu.NETS, every network clipping, A = 1 and A = 16.  tf32 at 17 x 6: at 60 x 8 the first minibatch
+    # of sp-id and sig-sp has PPO-clip decisions that tf32 rounding flips (the one-step actor gradient measured 6e-2
+    # l2-rel on an H100, 5e-4 with the ratio loss on the same data), a jump of whole samples no rounding bar covers
+    [('fp32', 33, 1, 'all', False, 'sig-sp'), ('tf32', 17, 6, 'all', False, 'sp-id'),
+     ('bf16x3', 64, 16, 'all', False, 'sig-1'), ('fp32', 64, 16, 'all', False, 'tanh-relu'),
+     ('bf16x3', 33, 1, 'all', True, 'sp-id'), ('tf32', 17, 6, 'all', False, 'sig-1')]))
+def test_stepwise_passes_vs_fp64(cuda, path, O, A, regime, trained, nets):
     """The minibatch gradient kernels + osb_optim_fused (launch per minibatch), PPO clip loss, every network."""
-    w1, we = _epoch_case(cuda, path, O, A, 7, 0, regime, 1024, seed=O + A, trained=trained)
-    print(f'[{path} O={O} A={A} {regime}] one step worst block l2 {w1:.2e}; epoch ' +
+    w1, we = _epoch_case(cuda, path, O, A, 7, 0, regime, 1024, seed=O + A, trained=trained, nets=nets)
+    print(f'[{path} O={O} A={A} {regime}{" " + nets if nets else ""}] one step worst block l2 {w1:.2e}; epoch ' +
           ', '.join(f'{k} {v:.2e}' for k, v in we.items()))
 
 

@@ -1,5 +1,11 @@
 """GPU parity: fused minibatch forward/backward, optimiser, KL evaluation, Lagrange multiplier,
-Fisher-vector product and CG vs the oracle and vs golden fixtures of the unmodified reference."""
+Fisher-vector product and CG vs the oracle and vs golden fixtures of the unmodified reference.
+
+NETS is the table of non-tanh network specs the float64 suites (this file, test_update_tc_gpu, test_update_x3_gpu,
+test_natural_gradient_gpu, test_optimizer_gpu, test_two_pass_loss_gpu) add to their tanh cases; a case's `nets` is a key
+of NETS, optionally with an edge regime of the data: '+sat' (layer-1 pre-activations spread over about +-100) or '+zero'
+(relu units at z = +-0 exactly), see _rand_data."""
+import contextlib
 import os
 from types import SimpleNamespace as NS
 
@@ -12,21 +18,65 @@ from oracle import learner as ol
 
 pytestmark = pytest.mark.gpu
 
+# (actor activation, critic activation, actor widths, critic widths)
+NETS = {
+    'relu': ('relu', 'relu', (64, 64), (64, 64)),                  # a single non-tanh instantiation
+    'sig-sp': ('sigmoid', 'softplus', (24, 40), (8, 64)),          # ACT_MIXED; masks differ by layer and by network
+    'sp-id': ('softplus', 'identity', (40, 24), (64, 8)),          # ACT_MIXED with the widths reversed
+    'id-sig': ('identity', 'sigmoid', (64, 64), (33, 17)),         # a masked critic behind an unmasked actor
+    'tanh-relu': ('tanh', 'relu', (64, 64), (64, 64)),             # the precision's tanh inside the mixed variant
+    'sig-1': ('sigmoid', 'sigmoid', (1, 63), (63, 1)),             # extreme widths
+}
+SAT_RANGE = 100.0      # '+sat': the largest |layer-1 pre-activation| of every network
 
-def _model_cfgs(lr_actor=3e-4, lr_critic=3e-4):
-    return NS(actor=NS(hidden_sizes=[64, 64], activation='tanh', lr=lr_actor),
-              critic=NS(hidden_sizes=[64, 64], activation='tanh', lr=lr_critic),
+
+@pytest.fixture(autouse=True)
+def _default_spec_after():
+    """Launches made directly through the C ABI read the process-wide spec: leave the default (tanh, 64 wide) behind."""
+    yield
+    from omnisafe_b200.models.actor_critic import set_net_spec
+
+    set_net_spec(0, 0, (64, 64), (64, 64))
+
+
+def _spec(nets):
+    """(NETS entry or None, edge regime or '') of a case's `nets`."""
+    if nets is None:
+        return None, ''
+    key, _, edge = nets.partition('+')
+    return NETS[key], edge
+
+
+def oracle_nets(nets):
+    """The oracle's network spec (oracle.actor_critic.nets) of a case; tanh 64 wide for nets=None."""
+    spec, _ = _spec(nets)
+    return oac.nets(*spec) if spec else contextlib.nullcontext()
+
+
+def net_cases(cases, new):
+    """Parameter sets of a test that gains a trailing `nets` argument: `cases` (pytest.params, e.g. sigma_cases) keep
+    their ids with nets=None; each tuple of `new` ends in (..., nets) and gets the id of its values joined by '-'."""
+    return ([pytest.param(*c.values, None, id=c.id) for c in cases]
+            + [pytest.param(*c, id='-'.join(map(str, c))) for c in new])
+
+
+def _model_cfgs(lr_actor=3e-4, lr_critic=3e-4, nets=None):
+    aa, ca, ah, ch = _spec(nets)[0] or ('tanh', 'tanh', (64, 64), (64, 64))
+    return NS(actor=NS(hidden_sizes=list(ah), activation=aa, lr=lr_actor),
+              critic=NS(hidden_sizes=list(ch), activation=ca, lr=lr_critic),
               actor_type='gaussian_learning', linear_lr_decay=False, weight_initialization_mode='kaiming_uniform')
 
 
-def _setup(dev, data, N, T, O, A, theta, lr_actor=3e-4, lr_critic=3e-4):
-    """Build agent + slab buffer from env-major `data` (as VectorOnPolicyBuffer.get() returns it)."""
+def _setup(dev, data, N, T, O, A, theta, lr_actor=3e-4, lr_critic=3e-4, nets=None):
+    """Build agent + slab buffer from env-major `data` (as VectorOnPolicyBuffer.get() returns it); the agent's network
+    spec is the one the following direct C-ABI launches use."""
     from omnisafe_b200.algorithms.engine import UpdateEngine
     from omnisafe_b200.common.buffer import VectorOnPolicyBuffer
     from omnisafe_b200.models import ConstraintActorCritic
 
-    agent = ConstraintActorCritic(O, A, _model_cfgs(lr_actor, lr_critic), epochs=1, device=dev)
+    agent = ConstraintActorCritic(O, A, _model_cfgs(lr_actor, lr_critic, nets), epochs=1, device=dev)
     agent.load_flat(theta)
+    agent.apply_net_spec()
     buf = VectorOnPolicyBuffer(O, A, T, 0.99, 0.95, 0.95, 'gae', 0.0, True, True, num_envs=N, device=dev)
 
     def tm(x):  # env-major [N*T, ...] -> time-major [T, N, ...]
@@ -59,15 +109,89 @@ def entropy_mean(log_std):
     return 0.5 + 0.5 * np.log(2 * np.pi) + float(np.mean(np.asarray(log_std, np.float64)))
 
 
-def _theta(O, A, seed, trained):
-    return oac.init_theta(O, A, seed=seed, log_std=oac.trained_log_std(A, seed) if trained else None)
+def _theta(O, A, seed, trained, nets=None):
+    spec, _ = _spec(nets)
+    widths = dict(actor_hidden=spec[2], critic_hidden=spec[3]) if spec else {}
+    return oac.init_theta(O, A, seed=seed, log_std=oac.trained_log_std(A, seed) if trained else None, **widths)
 
 
-def _rand_data(rng, N, T, O, A, theta):
+def _edge(theta, obs, O, A, nets):
+    """The edge regime of `nets`, applied to theta's layer 1 (in place) and to obs (in place):
+      sat:  every network's W1 and b1 scaled so that its float64 pre-activations over `obs` reach +-SAT_RANGE: past
+            softplus's threshold 20, past z = -87 where sigmoid's 1 / (1 + e^-z) underflows, and sigmoid outputs
+            within float32 rounding of 1, whose derivative h (1 - h) comes from the stored h;
+      zero: every 5th row of obs all zeros and 8 entries of every network's b1 exactly 0, so those units see z = +-0:
+            relu'(0) is 0 in torch and [h > 0] in the kernels."""
+    spec, edge = _spec(nets)
+    if not edge:
+        return
+    views = oac.unflatten(theta, O, A)
+    if edge == 'zero':
+        obs[::5] = 0.0
+        for net in views.values():
+            net['b1'][3:64:8] = 0.0
+        return
+    assert edge == 'sat', edge
+    x = torch.as_tensor(obs, dtype=torch.float64)
+    for net, width in zip(views.values(), (spec[2][0], spec[3][0], spec[3][0])):
+        z = torch.nn.functional.linear(x, net['w1'][:width].double(), net['b1'][:width].double())
+        s = SAT_RANGE / -float(z.min())
+        net['w1'].mul_(s)
+        net['b1'].mul_(s)
+        z = torch.nn.functional.linear(x, net['w1'][:width].double(), net['b1'][:width].double())
+        assert float(z.min()) < -0.99 * SAT_RANGE and float(z.max()) > 0.5 * SAT_RANGE, (float(z.min()), float(z.max()))
+        assert (z.abs() < 5).float().mean() > 0.02, 'no units left in the unsaturated range'
+
+
+def relu_kinks(theta, obs, O, A, nets, net):
+    """Fraction of the relu units of `net` ('actor', 'reward_critic', 'cost_critic'), over the rows of `obs` and both
+    hidden layers, whose float64 pre-activation z lies within tf32 rounding of 0: |z| < 2^-10 (sum_k |w_k x_k| + |b|)
+    (both operands of every product rounded to 10 mantissa bits).  The tf32 tiles may put such a unit on the other side
+    of relu's kink, which moves the sample's whole contribution through that unit: a flip, not a rounding error."""
+    spec, _ = _spec(nets)
+    p = {k: v.double() for k, v in oac.unflatten(np.asarray(theta, np.float32), O, A)[net].items()}
+    act, (a1, a2) = (spec[0], spec[2]) if net == 'actor' else (spec[1], spec[3])
+    if act != 'relu':
+        return 0.0
+    h, near, total = torch.as_tensor(np.asarray(obs, np.float64)), 0, 0
+    for w, b, rows, cols in ((p['w1'], p['b1'], a1, O), (p['w2'], p['b2'], a2, a1)):
+        w, b = w[:rows, :cols], b[:rows]
+        z = h @ w.T + b
+        near += int((z.abs() < 2.0 ** -10 * (h.abs() @ w.abs().T) + b.abs() * 2.0 ** -10).sum())
+        total += z.numel()
+        h = torch.relu(z)
+    return near / total
+
+
+# tf32 tiles at '+sat': a layer's inputs reach |h| ~ 100 (softplus, identity), and a tf32 operand carries 2^-11 of its
+# own magnitude, not of the result's; the fp32 and bf16x3 tiles meet their 1e-4 bars on the same data, so the
+# activations are right.  Measured on an H100 (700 W): worst block l2-rel 9.6e-3 (test_update_tc_gpu, sp-id, the
+# identity critic's b2) and whole-vector 5.5e-3 (test_natural_gradient_gpu, the sp-id actor's ratio surrogate).
+TF32_SAT_L2 = 2e-2
+
+
+def tf32_bar(l2, min_cos, theta, obs, O, A, nets, net):
+    """The tf32 bars (l2-relative, cosine) of `net`'s gradient for a case of `nets`: the tanh bars, raised for relu
+    units near the kink to l2 sqrt(f) and cosine 1 - f with f = relu_kinks (one flipped unit-row is one term of a sum
+    of f^-1 such terms; measured on an H100 (700 W) at f = 2.5e-3 to 6.7e-3: l2 0.1 to 0.53 sqrt(f)), and to
+    TF32_SAT_L2 at '+sat'."""
+    f = relu_kinks(theta, obs, O, A, nets, net) if nets else 0.0
+    if f:
+        l2, min_cos = max(l2, float(np.sqrt(f))), min(min_cos, 1.0 - f)
+    if nets and _spec(nets)[1] == 'sat':
+        l2 = max(l2, TF32_SAT_L2)
+    return l2, min_cos
+
+
+def _rand_data(rng, N, T, O, A, theta, nets=None):
+    """Random batch at the policy `theta` (under the network spec of `nets`); an edge regime of `nets` edits theta's
+    layer 1 in place first (_edge)."""
     B = N * T
     obs = rng.standard_normal((B, O)).astype(np.float32)
     eps = rng.standard_normal((B, A)).astype(np.float32)
-    act, v_r, v_c, logp = oac.step(theta, obs, eps, O, A)
+    _edge(theta, obs, O, A, nets)
+    with oracle_nets(nets):
+        act, v_r, v_c, logp = oac.step(theta, obs, eps, O, A)
     logp = (logp + 0.3 * rng.standard_normal(B)).astype(np.float32)   # push ratios across the clip range
     return {'obs': obs, 'act': act, 'logp': logp,
             'adv_r': rng.standard_normal(B).astype(np.float32), 'adv_c': rng.standard_normal(B).astype(np.float32),
@@ -75,17 +199,21 @@ def _rand_data(rng, N, T, O, A, theta):
             'target_value_c': rng.standard_normal(B).astype(np.float32)}
 
 
-@pytest.mark.parametrize('O,A,N,T,loss_kind,trained', sigma_cases(
+@pytest.mark.parametrize('O,A,N,T,loss_kind,trained,nets', net_cases(sigma_cases(
     [(60, 8, 20, 13, 0), (60, 8, 32, 8, 1), (17, 6, 9, 31, 3), (111, 8, 16, 10, 0), (376, 8, 7, 20, 0)],
     # ragged last tile, A = 1, A = 16 with more tiles than CTAs, obs dims > 64; every single-pass kind
-    [(60, 8, 20, 13, 0), (17, 6, 9, 31, 3), (33, 1, 50, 11, 0), (64, 16, 300, 70, 1), (111, 8, 16, 10, 1)]))
-def test_minibatch_grad_vs_autograd(cuda, O, A, N, T, loss_kind, trained):
+    [(60, 8, 20, 13, 0), (17, 6, 9, 31, 3), (33, 1, 50, 11, 0), (64, 16, 300, 70, 1), (111, 8, 16, 10, 1)]), [
+    # NETS: ragged last tile, A = 1 (trained), A = 16 with more tiles than CTAs, obs dims > 64, the edge regimes
+    (60, 8, 20, 13, 0, False, 'sig-sp'), (33, 1, 50, 11, 0, True, 'sp-id'), (64, 16, 300, 70, 1, False, 'id-sig'),
+    (111, 8, 16, 10, 3, False, 'sig-1'), (17, 6, 9, 31, 3, True, 'tanh-relu'), (60, 8, 20, 13, 1, False, 'relu+zero'),
+    (60, 8, 20, 13, 0, False, 'sig-sp+sat'), (60, 8, 20, 13, 1, False, 'sp-id+sat')]))
+def test_minibatch_grad_vs_autograd(cuda, O, A, N, T, loss_kind, trained, nets):
     from omnisafe_b200._lib import current_stream, lib, ptr
 
     rng = np.random.default_rng(O + N)
-    theta = _theta(O, A, 5, trained)
-    data = _rand_data(rng, N, T, O, A, theta)
-    agent, buf, eng = _setup(cuda, data, N, T, O, A, theta)
+    theta = _theta(O, A, 5, trained, nets)
+    data = _rand_data(rng, N, T, O, A, theta, nets)
+    agent, buf, eng = _setup(cuda, data, N, T, O, A, theta, nets=nets)
     B = N * T
     lam = 0.37
     lag = torch.tensor([lam], dtype=torch.float32, device=cuda)
@@ -109,24 +237,34 @@ def test_minibatch_grad_vs_autograd(cuda, O, A, N, T, loss_kind, trained):
     idx = torch.as_tensor(perm_em[start:start + count])
     t = {k: torch.as_tensor(v)[idx] for k, v in data.items()}
     adv = (t['adv_r'] - lam * t['adv_c']) / (1 + lam)
-    if loss_kind == 0:
-        loss, _ = L.loss_pi_ppo(t['obs'], t['act'], t['logp'], adv, 0.2, 0.01)
-    elif loss_kind == 1:
-        loss = L.loss_pi_plain(t['obs'], t['act'], t['logp'], adv)
-    else:
-        loss = L.loss_pi_cost(t['obs'], t['act'], t['logp'], t['adv_c'])
-    loss.backward()
-    for net, tgt in (('reward_critic', 'target_value_r'), ('cost_critic', 'target_value_c')):
-        lv = torch.nn.functional.mse_loss(oac.critic_value(L.params[net], t['obs']), t[tgt])
-        for p_ in L.params[net].values():
-            lv = lv + p_.pow(2).sum() * coef
-        lv.backward()
+    with oracle_nets(nets):
+        if loss_kind == 0:
+            loss, _ = L.loss_pi_ppo(t['obs'], t['act'], t['logp'], adv, 0.2, 0.01)
+        elif loss_kind == 1:
+            loss = L.loss_pi_plain(t['obs'], t['act'], t['logp'], adv)
+        else:
+            loss = L.loss_pi_cost(t['obs'], t['act'], t['logp'], t['adv_c'])
+        loss.backward()
+        for net, tgt in (('reward_critic', 'target_value_r'), ('cost_critic', 'target_value_c')):
+            lv = torch.nn.functional.mse_loss(oac.critic_value(L.params[net], t['obs']), t[tgt])
+            for p_ in L.params[net].values():
+                lv = lv + p_.pow(2).sum() * coef
+            lv.backward()
     want = torch.cat([L.flat_grad(n) for n in ol.NETS]).numpy()
     lay = oac.layout(O, A)
+    worst = 0.0
     for net in ol.NETS:
         s, n = lay[net]['start'], lay[net]['size']
         scale = np.abs(want[s:s + n]).max()
         np.testing.assert_allclose(got[s:s + n], want[s:s + n], rtol=2e-4, atol=2e-5 * max(scale, 1e-3), err_msg=net)
+        if nets:      # the suite's 1e-4 l2 bar per parameter block
+            for name, (off, shape) in lay[net]['entries'].items():
+                w, g = want[off:off + int(np.prod(shape))], got[off:off + int(np.prod(shape))]
+                rel = float(np.linalg.norm(g - w) / (np.linalg.norm(w) + 1e-30))
+                worst = max(worst, rel)
+                assert rel < 1e-4 or not w.any() and not g.any(), (net, name, rel)
+    if nets:
+        print(f'[fp32 {nets} O={O} A={A} kind {loss_kind}] worst block l2-rel {worst:.2e}')
     # the log_std block on its own (A entries next to ~10^4 weights in the actor's bar)
     rel = float(np.linalg.norm(got[:A] - want[:A]) / np.linalg.norm(want[:A]))
     print(f'actor.log_std: l2-rel {rel:.2e}')

@@ -7,24 +7,29 @@ import torch
 
 from oracle import actor_critic as oac
 from oracle import learner as ol
-from test_update_gpu import _rand_data, _rows, _setup, _theta, sigma_cases
+from test_update_gpu import (_default_spec_after, _rand_data, _rows, _setup, _theta, net_cases, oracle_nets,  # noqa: F401
+                             sigma_cases, tf32_bar)
 
 pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.timeout(120)
-@pytest.mark.parametrize('O,A,N,T,loss_kind,trained', sigma_cases(
+@pytest.mark.parametrize('O,A,N,T,loss_kind,trained,nets', net_cases(sigma_cases(
     [(60, 8, 20, 13, 0), (60, 8, 64, 40, 0), (17, 6, 9, 31, 3), (64, 16, 16, 24, 1), (60, 8, 512, 80, 0),
      (111, 8, 40, 30, 1), (376, 8, 33, 12, 3), (128, 4, 300, 9, 1), (65, 8, 20, 7, 0)],   # obs dims > 64: K-chunked layer 1
     [(60, 8, 20, 13, 0), (17, 6, 9, 31, 3), (33, 1, 50, 11, 0), (64, 16, 16, 24, 1), (60, 8, 512, 80, 0),
-     (111, 8, 40, 30, 1), (376, 8, 33, 12, 3)]))
-def test_tc_grad_vs_autograd(cuda, O, A, N, T, loss_kind, trained):
+     (111, 8, 40, 30, 1), (376, 8, 33, 12, 3)]), [
+    # test_update_gpu.NETS: ragged last tile, A = 1 (trained), A = 16 with more tiles than CTAs, obs dims > 64, sat
+    (60, 8, 20, 13, 0, False, 'relu'), (33, 1, 50, 11, 0, True, 'sig-sp'), (64, 16, 300, 70, 1, False, 'sp-id'),
+    (111, 8, 40, 30, 3, False, 'id-sig'), (376, 8, 33, 12, 1, False, 'tanh-relu'), (17, 6, 9, 31, 3, False, 'sig-1'),
+    (60, 8, 20, 13, 0, False, 'sig-sp+sat'), (60, 8, 20, 13, 1, False, 'sp-id+sat')]))
+def test_tc_grad_vs_autograd(cuda, O, A, N, T, loss_kind, trained, nets):
     from omnisafe_b200._lib import current_stream, lib, ptr
 
     rng = np.random.default_rng(O + N)
-    theta = _theta(O, A, 5, trained)
-    data = _rand_data(rng, N, T, O, A, theta)
-    agent, buf, eng = _setup(cuda, data, N, T, O, A, theta)
+    theta = _theta(O, A, 5, trained, nets)
+    data = _rand_data(rng, N, T, O, A, theta, nets)
+    agent, buf, eng = _setup(cuda, data, N, T, O, A, theta, nets=nets)
     B = N * T
     lam = 0.37
     lag = torch.tensor([lam], dtype=torch.float32, device=cuda)
@@ -47,21 +52,22 @@ def test_tc_grad_vs_autograd(cuda, O, A, N, T, loss_kind, trained):
     idx = torch.as_tensor(perm_em[start:start + count])
     t = {k: torch.as_tensor(v)[idx] for k, v in data.items()}
     adv = (t['adv_r'] - lam * t['adv_c']) / (1 + lam)
-    if loss_kind == 0:
-        loss, _ = L.loss_pi_ppo(t['obs'], t['act'], t['logp'], adv, 0.2, 0.01)
-    elif loss_kind == 1:
-        loss = L.loss_pi_plain(t['obs'], t['act'], t['logp'], adv)
-    else:
-        loss = L.loss_pi_cost(t['obs'], t['act'], t['logp'], t['adv_c'])
-    loss.backward()
-    for net, tgt in (('reward_critic', 'target_value_r'), ('cost_critic', 'target_value_c')):
-        lv = torch.nn.functional.mse_loss(oac.critic_value(L.params[net], t['obs']), t[tgt])
-        for p_ in L.params[net].values():
-            lv = lv + p_.pow(2).sum() * coef
-        lv.backward()
+    with oracle_nets(nets):
+        if loss_kind == 0:
+            loss, _ = L.loss_pi_ppo(t['obs'], t['act'], t['logp'], adv, 0.2, 0.01)
+        elif loss_kind == 1:
+            loss = L.loss_pi_plain(t['obs'], t['act'], t['logp'], adv)
+        else:
+            loss = L.loss_pi_cost(t['obs'], t['act'], t['logp'], t['adv_c'])
+        loss.backward()
+        for net, tgt in (('reward_critic', 'target_value_r'), ('cost_critic', 'target_value_c')):
+            lv = torch.nn.functional.mse_loss(oac.critic_value(L.params[net], t['obs']), t[tgt])
+            for p_ in L.params[net].values():
+                lv = lv + p_.pow(2).sum() * coef
+            lv.backward()
     want = torch.cat([L.flat_grad(n) for n in ol.NETS]).numpy()
     lay = oac.layout(O, A)
-    bad = 0
+    bad, worst = 0, 0.0
     for net in ol.NETS:
         for name, (off, shape) in lay[net]['entries'].items():
             n = int(np.prod(shape))
@@ -75,7 +81,11 @@ def test_tc_grad_vs_autograd(cuda, O, A, N, T, loss_kind, trained):
             # at a trained log_std (sigma down to 0.2) the tf32 mean's error is amplified in (act - mu) / sigma^2: the
             # PPO actor blocks measured l2-rel up to 1.7e-2 and cos down to 0.99986 on an H100, so cos > 0.9998 there
             min_cos = 0.9998 if (trained and net == 'actor' and loss_kind == 0) else 0.9999
+            tol, min_cos = tf32_bar(tol, min_cos, theta, data['obs'][idx], O, A, nets, net)
             bad += (rel > tol) or (cos < min_cos)
+            worst = max(worst, rel)
+    if nets:
+        print(f'[tf32 {nets} O={O} A={A} kind {loss_kind}] worst block l2-rel {worst:.2e}')
     assert bad == 0
 
 

@@ -10,46 +10,53 @@ import torch
 
 from oracle import actor_critic as oac
 from oracle import learner as ol
-from test_update_gpu import _rand_data, _rows, _setup, _theta, entropy_mean, sigma_cases
+from test_update_gpu import (_default_spec_after, _rand_data, _rows, _setup, _theta, entropy_mean, net_cases,  # noqa: F401
+                             oracle_nets, sigma_cases)
 
 pytestmark = pytest.mark.gpu
 
 
-def _oracle_grad(theta, O, A, data, idx, lam, loss_kind, coef):
+def _oracle_grad(theta, O, A, data, idx, lam, loss_kind, coef, nets=None):
     L = ol.Learner(theta, O, A)
     t = {k: torch.as_tensor(v)[idx] for k, v in data.items()}
     adv = (t['adv_r'] - lam * t['adv_c']) / (1 + lam)
-    if loss_kind == 0:
-        loss, _ = L.loss_pi_ppo(t['obs'], t['act'], t['logp'], adv, 0.2, 0.01)
-    elif loss_kind == 1:
-        loss = L.loss_pi_plain(t['obs'], t['act'], t['logp'], adv)
-    else:
-        loss = L.loss_pi_cost(t['obs'], t['act'], t['logp'], t['adv_c'])
-    loss.backward()
-    for net, tgt in (('reward_critic', 'target_value_r'), ('cost_critic', 'target_value_c')):
-        lv = torch.nn.functional.mse_loss(oac.critic_value(L.params[net], t['obs']), t[tgt])
-        for p_ in L.params[net].values():
-            lv = lv + p_.pow(2).sum() * coef
-        lv.backward()
+    with oracle_nets(nets):
+        if loss_kind == 0:
+            loss, _ = L.loss_pi_ppo(t['obs'], t['act'], t['logp'], adv, 0.2, 0.01)
+        elif loss_kind == 1:
+            loss = L.loss_pi_plain(t['obs'], t['act'], t['logp'], adv)
+        else:
+            loss = L.loss_pi_cost(t['obs'], t['act'], t['logp'], t['adv_c'])
+        loss.backward()
+        for net, tgt in (('reward_critic', 'target_value_r'), ('cost_critic', 'target_value_c')):
+            lv = torch.nn.functional.mse_loss(oac.critic_value(L.params[net], t['obs']), t[tgt])
+            for p_ in L.params[net].values():
+                lv = lv + p_.pow(2).sum() * coef
+            lv.backward()
     return torch.cat([L.flat_grad(n) for n in ol.NETS]).numpy(), float(loss)
 
 
 @pytest.mark.timeout(300)
-@pytest.mark.parametrize('O,A,N,T,loss_kind,count,trained', sigma_cases([
+@pytest.mark.parametrize('O,A,N,T,loss_kind,count,trained,nets', net_cases(sigma_cases([
     (60, 8, 20, 13, 0, None), (60, 8, 64, 40, 0, None), (17, 6, 9, 31, 3, None), (64, 16, 16, 24, 1, None),
     (60, 8, 256, 80, 0, 16384),      # the bench minibatch: 16 384 rows, obs 60 / act 8
     (60, 8, 256, 80, 1, 16384), (33, 1, 50, 11, 3, None),
 ], [  # ragged last tile, A = 1, A = 16, more tiles than CTAs (165 tiles of 128 rows); every single-pass kind
     (60, 8, 20, 13, 0, None), (17, 6, 9, 31, 3, None), (33, 1, 50, 11, 0, None), (64, 16, 16, 24, 1, None),
     (60, 8, 300, 70, 1, None),
+]), [  # test_update_gpu.NETS: ragged last tile, A = 1 (trained), A = 16 with more tiles than CTAs, the edge regimes
+    (60, 8, 20, 13, 0, None, False, 'relu+zero'), (33, 1, 50, 11, 3, None, True, 'sig-sp'),
+    (64, 16, 300, 70, 1, None, False, 'sp-id'), (17, 6, 9, 31, 3, None, False, 'id-sig'),
+    (60, 8, 64, 40, 0, None, False, 'tanh-relu'), (60, 8, 20, 13, 1, None, False, 'sig-1'),
+    (60, 8, 20, 13, 0, None, False, 'sig-sp+sat'), (60, 8, 20, 13, 1, None, False, 'sp-id+sat'),
 ]))
-def test_x3_grad_vs_autograd(cuda, O, A, N, T, loss_kind, count, trained):
+def test_x3_grad_vs_autograd(cuda, O, A, N, T, loss_kind, count, trained, nets):
     from omnisafe_b200._lib import current_stream, lib, ptr
 
     rng = np.random.default_rng(O + N)
-    theta = _theta(O, A, 5, trained)
-    data = _rand_data(rng, N, T, O, A, theta)
-    agent, buf, eng = _setup(cuda, data, N, T, O, A, theta)
+    theta = _theta(O, A, 5, trained, nets)
+    data = _rand_data(rng, N, T, O, A, theta, nets)
+    agent, buf, eng = _setup(cuda, data, N, T, O, A, theta, nets=nets)
     B = N * T
     lam = 0.37
     lag = torch.tensor([lam], dtype=torch.float32, device=cuda)
@@ -70,8 +77,10 @@ def test_x3_grad_vs_autograd(cuda, O, A, N, T, loss_kind, count, trained):
     torch.cuda.synchronize()
     got = agent.grad.cpu().numpy()
     ts = eng.train_stats.cpu().numpy().reshape(3, 8).copy()
-    want, loss = _oracle_grad(theta, O, A, data, torch.as_tensor(perm_em[start:start + count]), lam, loss_kind, coef)
+    want, loss = _oracle_grad(theta, O, A, data, torch.as_tensor(perm_em[start:start + count]), lam, loss_kind, coef,
+                              nets)
     lay = oac.layout(O, A)
+    worst = 0.0
     for net in ol.NETS:
         s, n = lay[net]['start'], lay[net]['size']
         scale = np.abs(want[s:s + n]).max()
@@ -79,9 +88,12 @@ def test_x3_grad_vs_autograd(cuda, O, A, N, T, loss_kind, count, trained):
             m = int(np.prod(shape))
             w, g = want[off:off + m], got[off:off + m]
             rel = float(np.linalg.norm(g - w) / (np.linalg.norm(w) + 1e-30))
+            worst = max(worst, rel)
             print(f'{net}.{name}: l2-rel {rel:.2e}')
             assert rel < 1e-4, (net, name, rel)
         np.testing.assert_allclose(got[s:s + n], want[s:s + n], rtol=2e-4, atol=2e-5 * max(scale, 1e-3), err_msg=net)
+    if nets:
+        print(f'[bf16x3 {nets} O={O} A={A} kind {loss_kind}] worst block l2-rel {worst:.2e}')
     # slot 0: the loss without the entropy bonus; slot 4: the bonus; Loss/Loss_pi = slot 0 + slot 4 is the oracle loss,
     # bonus included (base/ppo.py:L76-84)
     bonus = -0.01 * entropy_mean(theta[:A]) if loss_kind == 0 else 0.0
